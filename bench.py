@@ -46,12 +46,9 @@ BATCH_PER_GPU = 16
 
 
 def _peaks():
-    p = ROOT / "MEASURED_PEAKS.json"
-    if p.exists():
-        d = json.loads(p.read_text())
-        return {"tensor_tflops": float(d.get("bf16_tflops_sustained", d.get("bf16_tflops", 1590.0))),
-                "hbm_gbs": float(d.get("hbm_gbs", 6650.0)), "source": "MEASURED_PEAKS.json (sustained bf16 cuBLAS)"}
-    return {"tensor_tflops": 1400.0, "hbm_gbs": 6650.0, "source": "fallback (B200_PROFILING.md: ~1.4 PF sustained)"}
+    # NVIDIA's data sheet for the H100 SXM (700 W): dense fp16 tensor rate and HBM3 bandwidth; the clocks sampled during
+    # the timed region show whether the card ran below them
+    return {"tensor_tflops": 989.0, "hbm_gbs": 3350.0, "source": "H100 SXM data sheet (dense fp16, HBM3), not measured"}
 
 
 class ClockSampler(threading.Thread):
@@ -407,6 +404,13 @@ def run_gpu(args):
     ms_total = t_ms.item()
     ms_per_step = ms_total / args.steps
     value = world * B / (ms_per_step * 1e-3)
+    if args.dump_outputs and rank == 0:
+        # what the timed loop returned in its last step: the final latents [world * B, 3, 64, 64] (all ranks' shards as
+        # gathered inside the step when world > 1; seeded inputs, so two builds can be compared output for output)
+        import numpy as np
+        dump = Path(args.dump_outputs)
+        dump.mkdir(parents=True, exist_ok=True)
+        np.save(dump / "latent.npy", (gathered["all"] if world > 1 else out).float().cpu().numpy())
 
     if args.quick:       # A/B and ablation runs: only the device-resident figure
         if rank == 0:
@@ -482,7 +486,7 @@ def run_gpu(args):
             dist.destroy_process_group()
         return
 
-    # ---- roofline of the dominant kernel family (implicit-GEMM conv / linear / fused MLP on tcgen05), measured live ----
+    # ---- roofline of the dominant kernel family (implicit-GEMM conv / linear on wgmma), measured live ----
     ms_kind = (C.c_double * 4)()
     flops = C.c_double()
     nconv = C.c_int32()
@@ -498,9 +502,8 @@ def run_gpu(args):
     conv_tflops = flops.value / (pk[0] * 1e-3) / 1e12 if pk[0] > 0 else 0.0
     traffic, tensor_pct, ncu_file = newest_ncu_summary()
     roofline = {
-        "kernel": "tcgen05 GEMM kernels: conv_gemm_sm100_kernel<1|2>, conv_gemm_persist_sm100_kernel<1|2> (all conv3x3 / "
-                  "conv1x1 / linear layers) + mlp_fused_sm100_kernel (Swin MLPs) + swin_attn_tc_kernel (norm1 + qkv + window "
-                  "attention + proj of every Swin block)", "bound": "tensor",
+        "kernel": "wgmma GEMM kernels: conv_gemm_sm90_kernel<BN, MS> (all conv3x3 / conv1x1 / linear layers, Swin MLPs as "
+                  "fc1 + fc2) + swin_attn_fused_kernel (norm1 + qkv + window attention + proj of the Swin blocks it covers)", "bound": "tensor",
         "achieved": conv_tflops, "peak": peaks["tensor_tflops"], "unit": "TFLOP/s",
         "frac": conv_tflops / peaks["tensor_tflops"],
         # dram__bytes_read.sum + dram__bytes_write.sum per launch, averaged over the GEMM launches of the newest committed
@@ -590,7 +593,7 @@ def run_gpu(args):
                                "realsr_swinunet_realesrgan256_journal.yaml with steps=15, random-init weights"
                                % ("2" if world == 1 else "3", B),
                    "global_batch": world * B, "parallelism": f"dp{world} (independent image shards, NCCL weight broadcast + final all_gather)",
-                   "l2": "no explicit flush: per-step working set (237 MB fp16 weights + >1 GB activations) exceeds the 126 MB L2"},
+                   "l2": "no explicit flush: per-step working set (237 MB fp16 weights + >1 GB activations) exceeds the 50 MB L2"},
         "e2e": {"value": e2e_value, "unit": "images/s", "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": d2h},
         "gpu_launches": int(launches_per_loop * args.steps * 2),
         "launches_per_denoise_step": int(launches_per_forward - 6 + 1),
@@ -616,6 +619,8 @@ def main():
     ap.add_argument("--no-other-configs", action="store_true")
     ap.add_argument("--no-bookends", action="store_true")
     ap.add_argument("--quick", action="store_true", help="device-resident timing only (A/B and ablation runs)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the last step's output latents as DIR/latent.npy (float32)")
     args = ap.parse_args()
     if args.impl == "reference":
         run_reference(args)

@@ -1,4 +1,4 @@
-/* resshift_b200 — C ABI of the B200-native ResShift denoising hot path.
+/* resshift_b200 — C ABI of the H100-native (sm_90a) ResShift denoising hot path.
  *
  * The reference (zsyOAOA/ResShift) is pure Python/PyTorch and has no FFI; its plugin mechanism is
  * `instantiate_from_config` on yaml `target:` strings (reference utils/util_common.py:19-29, used at
@@ -210,26 +210,22 @@ int rs_op_window_attention(const void* qkv, int N, int H, int W, int heads, int 
 /* fused attention half of a Swin block: y = x + proj(window_attention(qkv(norm1(x)))) (reference
  * models/swin_transformer.py:246-275 with WindowAttention.forward :114-145); x NHWC fp16 [N,H,W,E] (in place when
  * y == x), norm1 statistics as the producers' (mean, M2) pairs gn_part[N][gn_slots][E][2], weights packed fp16;
- * part_out (optional): pairs of y per 8x8 window, [N][(H/8)*(W/8)][E][2]; gstat_out (optional, tcgen05 kernel only, with
- * counters [N] zeroed by the caller): the 32 group (mean, rstd) of y per image, finalised by the last CTA to deliver
- * an image's pairs.  relbias_dense must be the output of
- * rs_op_expand_relpos (relative_position_bias_table gathered by relative_position_index, :82-97,130-133): the tcgen05
- * kernel keeps only its 225 distinct values per head (bias(i, j) depends on (yi - yj, xi - xj) alone).
- * RS_SWIN_IMPL=mma selects the mma.sync kernel (same arithmetic, reads the dense table as given). */
+ * part_out (optional): pairs of y per 8x8 window, [N][(H/8)*(W/8)][E][2]; gstat_out (optional, needs part_out; counters
+ * [N] are accepted for compatibility and not used): the 32 group (mean, rstd) of y per image, reduced from the window
+ * pairs by a finalisation kernel after the attention kernel.  relbias_dense must be the output of rs_op_expand_relpos
+ * (relative_position_bias_table gathered by relative_position_index, :82-97,130-133). */
 int rs_op_swin_attn(const void* x, int N, int H, int W, int E, int heads, int shift, const float* gn_part, int gn_slots,
                     const float* gamma, const float* beta, const void* wqkv_packed, const float* bqkv, const float* relbias_dense,
                     const void* wproj_packed, const float* bproj, void* y, float* part_out, float* gstat_out_or_null,
                     uint32_t* counters_or_null, void* stream);
-/* fused Swin MLP (reference models/swin_transformer.py:17-33,279): out = residual + fc2(GELU(fc1(x))) */
+/* fused Swin MLP (reference models/swin_transformer.py:17-33,279): out = residual + fc2(GELU(fc1(x))) in one kernel,
+ * E in {64, 128, 192, 256}, Hd % 64 == 0; dbg_timeline_or_null must be NULL */
 int rs_op_mlp(const void* x, int N, int H, int W, int E, int Hd, const void* w1_packed, const float* b1,
               const void* w2_packed, const float* b2, const void* residual, void* out, void* dbg_timeline_or_null,
               void* stream);
 /* host-only: tile configuration the conv launcher picks: out[9] = BN, msub, stages, CTAs/SM, estimated cycles,
    CTAs per tile group (1 or 2), split-K factor, persistent kernel (0 / 1), cluster split-K (0 / 1) */
 int rs_debug_tile_config(int m_tiles, int cout, int num_kblocks, int32_t* out);
-/* profiling aid: later rs_op_swin_attn launches (tcgen05 kernel) write a clock64 timeline of CTA 0's first tile into
- * dev_buf[128 x int64] (two tiles x 64 stamps); NULL switches it off */
-int rs_debug_swin_timeline(void* dev_buf_or_null);
 /* nearest x2 (reference models/unet.py:71-81) */
 int rs_op_upsample2x(const void* x, int N, int H, int W, int C, void* y, void* stream);
 

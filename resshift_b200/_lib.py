@@ -94,7 +94,6 @@ _SIGNATURES = {
                                   _P, _P, _P, _P, _P]),
     "rs_op_mlp": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P, _P, _P, _P, _P, _P, _P]),
     "rs_debug_tile_config": (C.c_int, [C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int32)]),
-    "rs_debug_swin_timeline": (C.c_int, [_P]),
     "rs_op_upsample2x": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P]),
     "rs_vq_create": (C.c_int, [C.POINTER(VQConfigC), C.POINTER(_P)]),
     "rs_vq_plan_create": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(_P)]),
@@ -112,7 +111,7 @@ def _load():
     if not LIB_PATH.exists():
         raise ImportError(
             f"resshift_b200: CUDA library {LIB_PATH} not found. Build it with "
-            f"`python -c 'import __graft_entry__ as g; g.build()'` (nvcc, sm_100a). There is no CPU fallback.")
+            f"`python -c 'import __graft_entry__ as g; g.build()'` (nvcc, sm_90a). There is no CPU fallback.")
     lib = C.CDLL(str(LIB_PATH))
     for name, (res, args) in _SIGNATURES.items():
         fn = getattr(lib, name)            # AttributeError if the .so does not export a declared symbol

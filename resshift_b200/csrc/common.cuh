@@ -1,5 +1,5 @@
-// Common device/host helpers for the ResShift B200 (sm_100a) kernels.
-// Raw PTX wrappers for mbarrier / TMA / tcgen05 (no CUTLASS dependency).
+// Common device/host helpers for the ResShift H100 (sm_90a) kernels.
+// Raw PTX wrappers for mbarrier / TMA / clusters / wgmma (no CUTLASS dependency).
 #pragma once
 
 #include <cuda.h>
@@ -86,26 +86,6 @@ __device__ __forceinline__ float gelu_erf_f(float v) {
   return h + fmaf(-fabsf(h), ex, fabsf(h));
 }
 
-// Two GELUs at once on the packed fp32 pipe (fma.rn.f32x2, sm_100): same polynomial, half the FMA-pipe issue slots.
-__device__ __forceinline__ float2 gelu_erf_f2(float2 v) {
-  float2 z = __fmul2_rn(make_float2(fabsf(v.x), fabsf(v.y)), make_float2(0.70710678118654752f, 0.70710678118654752f));
-  z.x = fminf(z.x, 4.0f); z.y = fminf(z.y, 4.0f);
-  float2 pz = __ffma2_rn(z, make_float2(-2.177763781e-05f, -2.177763781e-05f), make_float2(5.068330793e-04f, 5.068330793e-04f));
-  pz = __ffma2_rn(z, pz, make_float2(-5.339398049e-03f, -5.339398049e-03f));
-  pz = __ffma2_rn(z, pz, make_float2(3.423144668e-02f, 3.423144668e-02f));
-  pz = __ffma2_rn(z, pz, make_float2(-1.528908461e-01f, -1.528908461e-01f));
-  pz = __ffma2_rn(z, pz, make_float2(-9.167589545e-01f, -9.167589545e-01f));
-  pz = __ffma2_rn(z, pz, make_float2(-1.628154397e+00f, -1.628154397e+00f));
-  pz = __ffma2_rn(z, pz, make_float2(6.178960575e-06f, 6.178960575e-06f));
-  float2 ex;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(ex.x) : "f"(pz.x));
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(ex.y) : "f"(pz.y));
-  // 1 + sign(v) (1 - ex)  =  1 + s - s ex   with s = +-1
-  const float2 s = make_float2(copysignf(1.0f, v.x), copysignf(1.0f, v.y));
-  const float2 t = __ffma2_rn(make_float2(-s.x, -s.y), ex, make_float2(1.0f + s.x, 1.0f + s.y));
-  return __fmul2_rn(__fmul2_rn(v, make_float2(0.5f, 0.5f)), t);
-}
-
 // ----------------------------------------------------------------------------------------
 // mbarrier
 // ----------------------------------------------------------------------------------------
@@ -136,15 +116,14 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
   return ok != 0;
 }
 // Arrive on a barrier that lives in another CTA of the cluster (address from mapa_u32) with the default CTA-scope
-// release.  The cluster-scope form (mbarrier.arrive.release.cluster) costs ~2000 cycles per arrival (it fences at
-// cluster scope; profiles/r1_s21 vs r1_s22 timelines) and is not needed when the data the arrival publishes is consumed
-// inside the ARRIVING thread's own CTA (its tensor core reading its own shared memory, made visible by
-// fence.proxy.async) and the remote waiter only needs the count.
+// release.  The cluster-scope form (mbarrier.arrive.release.cluster) fences at cluster scope and is not needed when the
+// remote waiter only needs the count: the consumer warps arrive after wgmma.wait_group shows their reads of the slot
+// retired, so the peer's next TMA write into it cannot overtake them.
 __device__ __forceinline__ void mbar_arrive_remote(uint32_t bar_cluster_addr) {
   asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(bar_cluster_addr) : "memory");
 }
-// Bounded spin: a pipeline bug must not hang the GPU box (that is a strike); after ~2 s of
-// polling the kernel traps instead, which surfaces as a launch failure on the host.
+// Bounded spin: a pipeline bug must not hang the GPU; after ~2 s of polling the kernel traps instead, which surfaces
+// as a launch failure on the host.
 __device__ __forceinline__ uint64_t global_timer_ns() {
   uint64_t t;
   asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
@@ -155,10 +134,8 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   const uint64_t t0 = global_timer_ns();
   uint32_t spins = 0;
   while (!mbar_try_wait(bar, parity)) {
-    if ((++spins & 0xFFu) == 0 && global_timer_ns() - t0 > 2000000000ull) {
-      printf("rs: mbarrier wait timeout (block %d thread %d parity %u)\n", blockIdx.x, threadIdx.x, parity);
-      __trap();
-    }
+    if ((++spins & 0xFFu) == 0 && global_timer_ns() - t0 > 2000000000ull) __trap();   // (no printf: a call here
+                                                                                        // would serialise the wgmma pipeline)
   }
 }
 
@@ -183,7 +160,7 @@ __device__ __forceinline__ void tma_load_4d(void* dst, const CUtensorMap* m, uin
       : "memory");
 }
 
-// ---- CTA-pair (cta_group::2) variants: the pair's barrier lives in the leader CTA (cluster rank 0) ----
+// ---- clusters: rank, cluster-wide barrier, distributed shared memory, TMA multicast ----
 __device__ __forceinline__ uint32_t cluster_ctarank() {
   uint32_t r;
   asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
@@ -206,18 +183,12 @@ __device__ __forceinline__ float4 ld_shared_cluster_f4(uint32_t cluster_addr) {
                : "memory");
   return v;
 }
-__device__ __forceinline__ void tma_load_2d_cg2(void* dst, const CUtensorMap* m, uint32_t bar_cluster_addr, int c0, int c1) {
+// 2-D tile load written to the same shared-memory offset of every CTA in `cta_mask`; each destination CTA's barrier at
+// the offset of `bar` receives the bytes that landed there
+__device__ __forceinline__ void tma_load_2d_mc(void* dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1, uint16_t cta_mask) {
   asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(bar_cluster_addr), "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_4d_cg2(void* dst, const CUtensorMap* m, uint32_t bar_cluster_addr, int c0, int c1,
-                                                int c2, int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], "
-      "[%2];" ::"r"(smem_u32(dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(bar_cluster_addr), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
+      "cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4}], [%2], %5;"
+      ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(cta_mask)
       : "memory");
 }
 
@@ -244,119 +215,31 @@ __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
 }
 
 // ----------------------------------------------------------------------------------------
-// tcgen05 (5th-gen tensor cores, accumulators in TMEM)
+// wgmma (Hopper warpgroup MMA, accumulators in registers; the instruction wrappers are in wgmma.cuh)
 // ----------------------------------------------------------------------------------------
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-template <int kCols>
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst) {  // whole warp
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)),
-               "n"(kCols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_alloc_dyn(uint32_t* smem_dst, uint32_t cols) {  // whole warp
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)),
-               "r"(cols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_dyn(uint32_t taddr, uint32_t cols) {  // whole warp
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(cols) : "memory");
+// registers and shared memory written before this point are ordered before the warpgroup's next wgmma
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+// at most kPending committed groups of this warpgroup are still in flight (their operands may still be read)
+template <int kPending>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(kPending) : "memory"); }
+// keeps the accumulator registers live across the wait: no use of them is scheduled before it
+template <int kRegs>
+__device__ __forceinline__ void wgmma_fence_regs(float (&d)[kRegs]) {
+#pragma unroll
+  for (int i = 0; i < kRegs; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// cta_group::2 flavours (issued by the leader CTA of a pair; TMEM allocation by one warp of EACH CTA)
-__device__ __forceinline__ void tmem_alloc_dyn_cg2(uint32_t* smem_dst, uint32_t cols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)), "r"(cols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish_cg2() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_dyn_cg2(uint32_t taddr, uint32_t cols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(cols) : "memory");
-}
-// D[tmem of both CTAs: 256 rows] (+)= A[128 rows from each CTA's smem] * B[N/2 rows from each CTA's smem]
-__device__ __forceinline__ void umma_f16_cg2(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                             uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// arrive (once the issued MMAs retire) on the barrier at this smem offset in every CTA of `cta_mask`
-__device__ __forceinline__ void umma_commit_cg2(uint64_t* bar, uint16_t cta_mask) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-                   smem_u32(bar)),
-               "h"(cta_mask)
-               : "memory");
-}
-
-// D[tmem] (+)= A[smem desc] * B[smem desc]; issued by ONE thread.
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                         uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Arrive on an mbarrier when all previously issued tcgen05.mma of this thread have completed.
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-
-// TMEM -> registers: 32 lanes x 32-bit, N consecutive columns per thread (thread i <-> lane base+i).
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
-      "[%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-// same, with the destination registers of the load as in/out operands: every use of v is ordered after the wait
-__device__ __forceinline__ void tmem_ld_wait16(uint32_t (&v)[16]) {
-  asm volatile("tcgen05.wait::ld.sync.aligned;"
-               : "+r"(v[0]), "+r"(v[1]), "+r"(v[2]), "+r"(v[3]), "+r"(v[4]), "+r"(v[5]), "+r"(v[6]), "+r"(v[7]), "+r"(v[8]),
-                 "+r"(v[9]), "+r"(v[10]), "+r"(v[11]), "+r"(v[12]), "+r"(v[13]), "+r"(v[14]), "+r"(v[15])
-               :
-               : "memory");
-}
-
-// Shared-memory matrix descriptor, K-major operand, 128-byte swizzle:
-//   rows are 128 B (64 fp16) apart, 8-row groups 1024 B apart (SBO), descriptor version 1 (sm_100).
-// Bit layout follows the PTX ISA "tcgen05 shared memory descriptor" (start addr [0,14), LBO [16,30),
-// SBO [32,46), version [46,48), layout type [61,64) with SWIZZLE_128B = 2).
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t smem_addr) {
+// Shared-memory matrix descriptor, K-major operand, 128-byte swizzle (sm_90 layout):
+//   rows are 128 B (64 fp16) apart, 8-row groups 1024 B apart (SBO).  Bit layout follows the PTX ISA "matrix
+//   descriptor" of wgmma (start addr [0,14), LBO [16,30), SBO [32,46), base offset [49,52), swizzle [62,64) with
+//   SWIZZLE_128B = 1).  Advancing 16 fp16 (32 B) along K inside the swizzled row is +2 on the address field.
+__device__ __forceinline__ uint64_t wgmma_desc_sw128(uint32_t smem_addr) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4);
   d |= static_cast<uint64_t>(1) << 16;            // LBO (ignored for swizzled K-major); 16 B
   d |= static_cast<uint64_t>(1024 >> 4) << 32;    // SBO = 1024 B
-  d |= static_cast<uint64_t>(1) << 46;            // version
-  d |= static_cast<uint64_t>(2) << 61;            // SWIZZLE_128B
-  return d;
-}
-// Instruction descriptor for kind::f16: fp16 A/B (K-major both), fp32 accumulate, M x N.
-__host__ __device__ __forceinline__ uint32_t umma_idesc_f16(int M, int N) {
-  uint32_t d = 0;
-  d |= 1u << 4;                                  // D format: F32
-  d |= 0u << 7;                                  // A format: F16
-  d |= 0u << 10;                                 // B format: F16
-  d |= static_cast<uint32_t>(N >> 3) << 17;      // N / 8
-  d |= static_cast<uint32_t>(M >> 4) << 24;      // M / 16
+  d |= static_cast<uint64_t>(1) << 62;            // SWIZZLE_128B
   return d;
 }
 

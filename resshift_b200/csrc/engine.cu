@@ -1,4 +1,4 @@
-// Engine: the Swin-UNet denoiser of ResShift as a static program of sm_100a kernel launches, plus the
+// Engine: the Swin-UNet denoiser of ResShift as a static program of sm_90a kernel launches, plus the
 // residual-shift sampling loop, behind the C ABI declared in include/resshift_b200.h.
 //
 // Topology restates UNetModelSwin.__init__/forward (reference models/unet.py:659-895), ResBlock
@@ -401,19 +401,16 @@ struct Builder {
     return prod;
   }
   const bool fuse_mlp = env_int("RS_MLP_FUSE", 1) && !env_is("RS_CONV_IMPL", "simt");
-  // norm2 applied inside the fused MLP kernel (bit-identical to the separate pass): implemented, measured twice — with
-  // every MLP CTA combining the statistics itself (round 1) and with producer-finalised statistics (profiles/r2_s2:
-  // 4.73 vs 4.69 ms per step) — and not faster either way, so it stays OFF (RS_MLP_NORM_FUSE=1 enables it)
+  // norm2 applied inside the fused MLP kernel (bit-identical to the separate pass; RS_MLP_NORM_FUSE=1, off by default:
+  // not measured faster)
   const bool fuse_mlp_norm = env_int("RS_MLP_NORM_FUSE", 0) != 0;
-  // norm1 + qkv + window attention + proj + residual as one tcgen05 kernel per Swin block (swin_attn_tc.cuh; RS_SWIN_FUSE=0:
-  // four launches; RS_SWIN_IMPL=mma: the mma.sync version of the fused kernel)
+  // norm1 + qkv + window attention + proj + residual as one kernel per Swin block (swin_attn_fused.cuh; RS_SWIN_FUSE=0:
+  // four launches)
   const bool fuse_swin_attn = env_int("RS_SWIN_FUSE", 1) != 0 && !env_is("RS_CONV_IMPL", "simt") && !env_is("RS_ATTN_IMPL", "simt");
-  // measured in the graph (profiles/r2_s33_min_pairs.log; ms per denoise step, fused from N pairs up):
-  //   batch 16: all levels 3.876, >= 9: 3.834, >= 33 (64x64 + 32x32): 3.809, >= 129 (64x64 only): 3.846, none: 3.902
-  //   batch  8: all 2.920, >= 33 (64x64 + 32x32 with 64 pairs): 2.826, >= 129 (64x64 only): 2.812, none: 2.877
-  //   batch  1: all 2.252, none 2.097 (64x64 = 32 pairs)
-  // i.e. the fused kernel wins where its persistent CTAs cover most of the machine (>= ~100 window pairs) and loses where a
-  // level is one 29-us tile on a few SMs against four small launches whose prologues overlap.
+  // a level with few window pairs is one long serial tile per CTA on a handful of SMs; below this many pairs the four
+  // small launches, whose prologues overlap through PDL, are used instead.  At the benchmark shape (batch 16, the 64x64 and
+  // 32x32 levels fused) the default measured 127.7 ms per 15-step loop against 134.8 ms with every level on four launches
+  // (H100 80GB HBM3 SXM, 700 W)
   const int fuse_swin_min_pairs = env_int("RS_SWIN_FUSE_MIN_PAIRS", 96);
   const bool fuse_stats = env_int("RS_GN_FUSE", 1) && !env_is("RS_CONV_EPI", "direct") && !env_is("RS_CONV_IMPL", "simt");
   Builder(rs_plan& p) : P(p), E(*p.e), cur(&p.ops) {}
@@ -743,9 +740,8 @@ int build_plan(rs_plan& P) {
     cat[j] = P.make_view(B, in_h[k], in_w[k], ctot);
   }
   // ---- concurrent batch slices for the few-tile levels (see rs_plan::branches) --------------------------------
-  // (measured, profiles/r2_s3: 2 slices 4.34 ms / step, 4 slices 4.76 ms against 3.90 ms for the plain sequence — the
-  // tile planner re-splits every half-batch layer until it fills the machine again, so the slices do not actually share
-  // it and only the launch count doubles.  Kept selectable, OFF by default.)
+  // (the tile planner re-splits every half-batch layer until it fills the machine again, so the slices do not actually
+  // share it and only the launch count doubles; selectable, OFF by default)
   {
     int nb = env_int("RS_LOWRES_STREAMS", 1);
     if (nb < 1) nb = 1;
@@ -834,23 +830,19 @@ void resolve(rs_plan& P, View& v) {
 // (img_off: a producer that covers only images [img_off, ...) of the consumer — a batch slice on a side stream)
 // Who reduces the (mean, M2) pairs to the image's 32 (mean, rstd)?
 //   * few tile slots (the denoiser's maps, <= 32 slots): every consumer CTA combines them itself — a finalisation step on
-//     the producer's tail costs more than it saves (profiles/r2_s1, r2_s2);
+//     the producer's tail sits on every producer CTA;
 //   * many slots (the VQ-GAN's 128x128 / 256x256 maps, RS_GN_FINALIZE_SLOTS moves the threshold): gn_finalize_kernel, a
 //     small launch in front of the consumer (default), or — RS_GN_PRODUCER_FINALIZE=1 — the last producer CTA of each
-//     image (arrival counters; measured +100 us per layer on one-tile CTAs and +800 us on the persistent kernel, whose
-//     CTAs all finish together so that ONE of them ends up reducing all 16 images: profiles/r2_s9_*).
+//     image (arrival counters; on a persistent conv the CTAs all finish together, so ONE of them ends up reducing every
+//     image).
 bool gn_finalizes(const Op& g) {
   static const int thr = env_int("RS_GN_FINALIZE_SLOTS", 64);
   return g.gn.slots > thr && !g.gn.win_slots;      // (the fused Swin attention kernel delivers pairs only)
 }
 bool gn_producer_finalizes(const Op& g) {
   static const int on = env_int("RS_GN_PRODUCER_FINALIZE", 0);
-  // the tcgen05 Swin attention kernel finalises its own output statistics: its CTAs own runs of consecutive windows, so
-  // every image ends on a different CTA and each CTA arrives once per image (swin_attn_tc.cuh).  Implemented, tested, and
-  // measured slower in the graph (3.98 vs 3.85 ms per step, profiles/r2_s28: the arrival sits on every CTA's tail), so it is
-  // OFF by default (RS_SWIN_FINALIZE=1 enables it); the consumers combine the window pairs
-  static const int swin_fin = env_int("RS_SWIN_FINALIZE", 0);
-  if (g.gn.win_slots) return swin_fin != 0 && swin_attn_uses_tc();
+  // (the fused Swin attention kernel delivers window pairs only: its consumers combine them)
+  if (g.gn.win_slots) return false;
   // (a GroupNorm without a fusable producer runs gn_stats_kernel, whose few CTAs per image arrive themselves)
   return gn_finalizes(g) && (on != 0 || !g.gn.fused);
 }
@@ -988,7 +980,7 @@ struct Prof {
 
 // RS_SKIP_KINDS (timing ablation only — results are garbage): bit 0 conv3x3, 1 conv1x1 / linear, 2 GroupNorm, 3 window
 // attention, 4 upsample, 5 fused MLP.  The time a kernel family really costs inside the graph-replayed step is the
-// difference between the full step and the step without it (per-launch events and ncu both over-state small kernels).
+// difference between the full step and the step without it (per-launch events over-state small kernels).
 inline bool op_skipped(const Op& op) {
   static const int skip = env_int("RS_SKIP_KINDS", 0);
   if (!skip) return false;
@@ -1049,7 +1041,7 @@ int run_ops(rs_plan& P, const std::vector<Op>& ops, const float* film_base, long
       case OP_UPSAMPLE: {
         UpsampleParams u{op.u_in.ptr, op.u_in.sN(), op.u_in.ld, op.u_out.ptr, op.u_in.N, op.u_in.H, op.u_in.W, op.u_in.C};
         const long long total = (long long)u.N * 4 * u.H * u.W * (u.C / 8);
-        (void)launch_k(upsample2x_kernel, dim3((unsigned)std::min<long long>((total + 255) / 256, 148 * 16)), dim3(256), (size_t)(0), st, u);
+        (void)launch_k(upsample2x_kernel, dim3((unsigned)std::min<long long>((total + 255) / 256, num_sms() * 16)), dim3(256), (size_t)(0), st, u);
         if (cudaGetLastError() != cudaSuccess) rc = fail(-2, "upsample launch failed");
         break;
       }
@@ -1263,7 +1255,7 @@ int rs_plan_profile(rs_plan* p, const float* x, const float* timesteps, const fl
     float ms = 0.f;
     cudaEventElapsedTime(&ms, prof.ev[2 * i], prof.ev[2 * i + 1]);
     const int kd = prof.kind[i];
-    // (the fused Swin attention kernel is a tcgen05 GEMM kernel: qkv + QK^T + PV + proj; it counts with the GEMM family)
+    // (the fused Swin attention kernel is a GEMM kernel: qkv + QK^T + PV + proj; it counts with the GEMM family)
     ms_by_kind[(kd == (int)OP_MLP || kd == (int)OP_SWIN_ATTN) ? 0 : kd] += ms;
   }
   double fl = 0.0; int nc = 0;

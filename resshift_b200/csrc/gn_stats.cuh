@@ -44,8 +44,7 @@ __device__ __forceinline__ float2 ldcg_f2(const float* p) {
 // counter += v with acquire-release semantics at GPU scope, by ONE thread after a CTA barrier: the barrier orders the
 // other threads' pair stores before it (causality is cumulative over bar.sync), the release half publishes them, and —
 // if this turns out to be the last arrival — the acquire half orders the finaliser's reads after every earlier arrival.
-// (Each thread issuing __threadfence() instead costs MEMBAR.SC.GPU + CCTL.IVALL x 256 threads per tile: measured
-// +50 % on the stats-bearing 3x3 layers, profiles/r2_s1_*.)
+// (Each thread issuing __threadfence() instead would cost a GPU-scope fence per thread and tile.)
 __device__ __forceinline__ unsigned int atom_add_acq_rel_gpu(unsigned int* p, unsigned int v) {
   unsigned int old;
   asm volatile("atom.add.acq_rel.gpu.global.u32 %0, [%1], %2;" : "=r"(old) : "l"(p), "r"(v) : "memory");
@@ -149,7 +148,7 @@ __device__ __forceinline__ void gn_arrive(const GnSink* const (&sink)[kMax], con
 }
 
 // Deferred arrivals of a persistent producer: instead of one arrival (barrier + GPU-scope atomic round trip + barrier,
-// ~2 us during which the eight epilogue warps idle) per output tile, thread 0 records (sink, image, channels) in a small
+// during which the epilogue warps idle) per output tile, thread 0 records (sink, image, channels) in a small
 // shared list — merging repeats — and the CTA arrives ONCE for every entry after its last tile.
 constexpr int kGnListCap = 64;
 struct GnArriveList {

@@ -10,13 +10,11 @@
 
 #include "common.cuh"
 #include "conv_gemm.cuh"
-#include "conv_persist.cuh"
 #include "elementwise.cuh"
 #include "mlp_fused.cuh"
 #include "norm_act.cuh"
 #include "window_attn.cuh"
 #include "swin_attn_fused.cuh"
-#include "swin_attn_tc.cuh"
 
 namespace rs {
 
@@ -124,6 +122,27 @@ inline cudaError_t launch_k(void (*kernel)(KArgs...), dim3 grid, dim3 block, siz
   return launch_kc(kernel, grid, block, smem, st, 1, std::forward<Args>(args)...);
 }
 
+// streaming multiprocessors of the current device (grid sizes of persistent kernels, the wave model of the cost
+// estimates), read once per device; host-only previews without a device assume an H100 SXM (132)
+inline int num_sms() {
+  static int cache[64] = {};
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) { (void)cudaGetLastError(); return 132; }
+  if (cache[dev] == 0) {
+    int n = 0;
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) { (void)cudaGetLastError(); n = 132; }
+    cache[dev] = n;
+  }
+  return cache[dev];
+}
+
+// shared memory of the conv epilogue's staging area: msub output tiles + per-warp GroupNorm partials + arrival flag
+inline size_t conv_epi_bytes(int BN, int msub) {
+  return (size_t)msub * ((size_t)BN * kConvBM * 2 + (size_t)4 * BN * 2 * sizeof(float)) + 16;
+}
+// what a persistent conv CTA needs beyond its operand ring: staging area, barriers, bias tile, alignment slack
+inline size_t conv_persist_extra_bytes(int BN) { return (conv_epi_bytes(BN, 1) + 1023) / 1024 * 1024 + 256 + 1024 + 1024; }
+
 inline int pow2_floor_div(int x, int cap) {   // largest power of two dividing x, capped
   int p = 1;
   while (p * 2 <= cap && x % (p * 2) == 0) p *= 2;
@@ -162,11 +181,12 @@ struct ConvDesc {
 
 struct TileConfig { int BN = 0, msub = 1, stages = 2, occ = 1, cg = 1, splitk = 1, persist = 0, cluster_split = 0; double est_cycles = 1e30; };
 
-// Cost model calibrated on B200 timelines (profiles/r1_s5_*, r1_s6_*).  Per 64-channel k-block and 128-pixel tile the
-// tensor pipe needs 2*BN cycles; every operand byte crosses shared memory twice (TMA write + UMMA read, 128 B/clk
-// per SM), which is what actually bounds a single-CTA tile (A 16 KB + B BN*128 B);  a CTA pair (cg = 2,
-// tcgen05 cta_group::2) stages only half of B per SM.  Shallow rings are additionally latency-bound (~3000 cycles
-// per load).  The epilogue (~18 cycles per column + set-up) hides under a co-resident CTA; whole waves are counted.
+// Cost model that ranks tile configurations (its constants come from the throughput figures of the H100 SXM and have not
+// been calibrated against timelines).  Per 64-channel k-block and 128-pixel tile the tensor pipe needs 4*BN cycles
+// (dense fp16 wgmma: 4096 flop/clk/SM); every operand byte crosses shared memory (TMA write, 128 B/clk per SM) and is
+// read by wgmma (A once, B once per warpgroup); a CTA pair (cg = 2) fetches only half of B from L2 per CTA (TMA
+// multicast).  Shallow rings are additionally latency-bound (~3000 cycles per load).  The epilogue (~18 cycles per
+// column + set-up) hides under a co-resident CTA; whole waves are counted.
 inline TileConfig pick_tile_config(int m_tiles, int cout16, int num_kb, int f_bn, bool allow_split = false, bool allow_persist = false,
                                    bool allow_cluster_split = false) {
   const int f_msub = env_int("RS_CONV_MSUB", 0), f_occ = env_int("RS_CONV_OCC", 0), f_stages = env_int("RS_CONV_STAGES", 0);
@@ -175,23 +195,24 @@ inline TileConfig pick_tile_config(int m_tiles, int cout16, int num_kb, int f_bn
   double best_real = 1e30;     // realistic estimate of `best` (see the end of the function)
   for (int cand = std::min(cout16, 256); cand >= 16; cand -= 16) {
     if (f_bn ? (cand != std::min(f_bn, std::min(cout16, 256))) : (cout16 % cand != 0)) continue;
+    if (!conv_bn_supported(cand)) continue;
     const int n_tiles = (cout16 + cand - 1) / cand;
     for (int cg = 1; cg <= 2; ++cg) {
       if (f_cg && cg != f_cg && !(f_cg == 2 && m_tiles < 2)) continue;   // a single tile cannot form a pair
       if (cg == 2 && (cand % 16 != 0 || m_tiles < 2)) continue;
-      // persistent kernel (conv_persist.cuh): one CTA (pair) per SM walks ceil(units / workers) tiles; the epilogue
-      // (~5000 + 3 cycles per column with double-buffered staging, profiles/r1_s38_persist_sweep.log) hides under the next tile's main loop, so
-      // a tile costs max(main loop, epilogue) and set-up / first round trip / last epilogue are paid once
-      if (allow_persist && 2 * cand <= 512) {
+      // persistent mode: one CTA (pair) per SM walks ceil(units / workers) tiles; the producer fetches the next tile's
+      // operands while the consumers run the epilogue, so a tile costs about max(main loop, epilogue) and set-up / first
+      // round trip are paid once
+      if (allow_persist) {
         const long long units_p = (long long)((m_tiles + cg - 1) / cg) * n_tiles;
-        const int workers = cg == 2 ? 74 : 148;
-        const int sbytes_p = kConvBM * kConvBK * 2 + (cand / cg) * kConvBK * 2;
-        const size_t extra = (size_t)2 * cand * kConvBM * 2 + (size_t)cand * 40 + 1280 + sizeof(GnArriveList);   // two staging buffers, wsum, two bias slots, arrival list
+        const int workers = cg == 2 ? num_sms() / 2 : num_sms();
+        const int sbytes_p = kConvBM * kConvBK * 2 + cand * kConvBK * 2;
+        const size_t extra = conv_persist_extra_bytes(cand);
         const int st_p = (int)std::min<size_t>(8, ((size_t)227 * 1024 - extra) / (size_t)sbytes_p);
-        // (only layers with at least two PIXEL tiles per worker: that is where the model below was calibrated; getting
-        // there through many narrow channel tiles would re-read the A operand once per channel tile)
+        // (only layers with at least two PIXEL tiles per worker; getting there through many narrow channel tiles would
+        // re-read the A operand once per channel tile)
         if ((m_tiles + cg - 1) / cg >= 2 * workers && st_p >= 2) {
-          const double kb_p = std::max(std::max(2.0 * cand, 2.0 * sbytes_p / 128.0), 2600.0 / st_p);
+          const double kb_p = std::max(std::max(4.0 * cand, 2.0 * sbytes_p / 128.0), 2600.0 / st_p);
           const double epi_p = 5000.0 + 3.0 * cand;
           const double rounds = std::ceil((double)units_p / workers);
           const double total = rounds * std::max(num_kb * kb_p, epi_p) + epi_p + 3000.0;
@@ -202,11 +223,11 @@ inline TileConfig pick_tile_config(int m_tiles, int cout16, int num_kb, int f_bn
         }
       }
       for (int ms = 1; ms <= 2; ++ms) {
-        if (ms == 2 && (f_msub != 2 || cg == 2 || m_tiles % 2 || 2 * cand > 512)) continue;   // msub = 2 only on request
-        const int sbytes = ms * kConvBM * kConvBK * 2 + (cand / cg) * kConvBK * 2;
+        if (ms == 2 && (f_msub != 2 || cg == 2 || m_tiles % 2 || !conv_kernel_for(cand, 2))) continue;   // msub = 2 only on request
+        const int sbytes = ms * kConvBM * kConvBK * 2 + cand * kConvBK * 2;
         for (int occ = 1; occ <= 2; ++occ) {
           if (f_occ && occ != f_occ) continue;
-          if (occ == 2 && ms * cand > 256) continue;                       // TMEM: 512 columns per SM
+          if (occ == 2 && ms * cand > 128) continue;                       // registers: accumulators of two CTAs per SM
           const int budget = (occ == 2 ? 111 : 222) * 1024 - 2048;
           int st = std::min(std::min(8, std::max(2, num_kb)), budget / sbytes);
           // the staged epilogue (output tile + statistics scratch) reuses the ring: it must be at least that large
@@ -218,16 +239,16 @@ inline TileConfig pick_tile_config(int m_tiles, int cout16, int num_kb, int f_bn
           }
           if (f_stages) st = f_stages;
           if (st < 2 || (size_t)st * sbytes + 2304 > (size_t)(occ == 2 ? 113 : 227) * 1024) continue;
-          const double smem_cycles = (sbytes + ms * (kConvBM * kConvBK * 2.0 + (cand / cg) * kConvBK * 2.0)) / 128.0;
+          const double smem_cycles = (sbytes + ms * kConvBM * kConvBK * 2.0 + 2.0 * cand * kConvBK * 2.0) / 128.0;
           // SM time for every resident CTA to advance one k-block: tensor / smem work of each, or the load latency
           // amortised over the ring depth
-          // load latency: ~3000 cycles when many tiles share each weight tile (L2 hits), ~7500 when the layer has so few
-          // pixel tiles that every weight tile is a fresh HBM read for a handful of CTAs (profiles/r1_s12_smallm_sweep.log)
+          // load latency: assumed ~3000 cycles when many tiles share each weight tile (L2 hits), ~7500 when the layer has so
+          // few pixel tiles that every weight tile is a fresh HBM read for a handful of CTAs
           const double load_lat = m_tiles >= 64 ? 3000.0 : 7500.0;
-          const double kb_cycles = std::max(occ * std::max(ms * 2.0 * cand, smem_cycles), load_lat / st);
+          const double kb_cycles = std::max(occ * std::max(ms * 4.0 * cand, smem_cycles), load_lat / st);
           const double epi = 18.0 * cand * ms + 3000.0 + (cg == 2 ? 2500.0 : 0.0);  // + pipeline fill / set-up (+ cluster syncs)
           const long long units = (long long)((m_tiles + cg * ms - 1) / (cg * ms)) * n_tiles;   // CTAs or CTA pairs
-          const double slots = (cg == 2 ? 74.0 : 148.0) * occ;
+          const double slots = (cg == 2 ? num_sms() / 2 : num_sms()) * (double)occ;
           // split-K: S CTAs (pairs) share one output tile's K loop; costs an fp32 round trip + a small reduce kernel
           const int f_split = env_int("RS_CONV_SPLITK", 0);
           const int kSplits[6] = {1, 2, 3, 4, 6, 8};
@@ -237,8 +258,7 @@ inline TileConfig pick_tile_config(int m_tiles, int cout16, int num_kb, int f_bn
           for (int mode = 0; mode < 2; ++mode)
           for (int si = 0; si < 6; ++si) {
             const int S = kSplits[si];
-            // (S = 2 only: clusters of 8 CTAs with ~200 KB of shared memory each schedule poorly — 30 us vs 21 us for the
-            //  8x8 640->640 layer, profiles/r1_s35_cluster_split_sweep.log)
+            // (S = 2 only: clusters of 4 CTAs; larger clusters of CTAs with ~200 KB of shared memory each schedule poorly)
             if (mode == 1 && (S != 2 || !allow_cluster_split || cg != 2 || occ != 1 || (cand / S) % 8 != 0)) continue;
             if (mode == 1 && f_mode && std::strcmp(f_mode, "global") == 0) continue;
             if (mode == 0 && S > 1 && f_mode && std::strcmp(f_mode, "cluster") == 0) continue;
@@ -248,8 +268,8 @@ inline TileConfig pick_tile_config(int m_tiles, int cout16, int num_kb, int f_bn
             const double waves = std::ceil((double)units * S / slots);
             const double kbs = std::ceil((double)num_kb / S);
             const double round = kbs * kb_cycles + (occ == 2 ? 0.5 * epi : epi);
-            // global: fp32 partials written once by the conv epilogue and read once by the reduce kernel (~2 KB/clk
-            // chip-wide each way in practice), plus a second kernel launch / drain (~10 us of fixed cost for the pair);
+            // global: fp32 partials written once by the conv epilogue and read once by the reduce kernel (assumed ~2 KB/clk
+            // chip-wide each way), plus a second kernel launch / drain (a fixed cost for the pair);
             // cluster: a cluster barrier and one pass over the tile through distributed shared memory
             const double part_bytes = 4.0 * m_tiles * 128.0 * cout16 * S;
             const double total = waves * round + (S == 1 ? 0.0 : mode == 1 ? 6000.0 : 19000.0 + 2.0 * part_bytes / 2048.0);
@@ -266,9 +286,8 @@ inline TileConfig pick_tile_config(int m_tiles, int cout16, int num_kb, int f_bn
       }
     }
   }
-  // the ranking model above orders one-tile-per-CTA configurations well (scripts/conv_sweep.py) but is optimistic in
-  // absolute terms; the persistent estimate is calibrated in absolute cycles, so compare it with the realistic figure
-  // (ties go to the persistent kernel: it measured faster on every >= 2-tiles-per-SM layer of the model)
+  // the ranking model above is optimistic in absolute terms (set-up, first round trip and epilogue are exposed once per
+  // wave); compare the persistent estimate with that realistic figure, ties going to the persistent mode
   if (bestp.BN && 0.85 * bestp.est_cycles < best_real) return bestp;
   return best;
 }
@@ -296,10 +315,6 @@ inline int conv_finalize(ConvDesc& d) {
   p.Hout = Hout; p.Wout = Wout; p.Nimg = N; p.Cout = d.Cout;
   p.num_taps = d.ksize * d.ksize;
   p.kchunks = (d.in.C + kConvBK - 1) / kConvBK;
-  {
-    const int tail = d.in.C - (p.kchunks - 1) * kConvBK;                 // real channels of the last 64-channel chunk
-    p.tail_k16 = env_int("RS_CONV_TAILSKIP", 1) ? (tail + 15) / 16 : kConvBK / 16;
-  }
   p.w_tap_stride = d.ipad;
   RS_CHECK(d.ipad % 8 == 0 && d.ipad >= d.in.C, "weight channel padding");
   // pixel box
@@ -309,10 +324,9 @@ inline int conv_finalize(ConvDesc& d) {
   p.tiles_w = Wout / p.bw; p.tiles_h = Hout / p.bh; p.tiles_n = (N + p.bn - 1) / p.bn;
   const int m_tiles = p.tiles_w * p.tiles_h * p.tiles_n;
   // ---- tile configuration: channel tile BN, sub-tiles per CTA (msub), CTAs per SM (occ), ring depth (stages) ----
-  // Chosen by a small cost model calibrated on B200 timelines (profiles/r1_s5_*): the main loop is bound by the bytes
-  // of TMA loads in flight per SM (ring capacity / ~3000-cycle load latency, at most ~75 B/clk) unless the tensor
-  // pipe is slower (2*BN cycles per 64-channel k-block per 128-pixel sub-tile); the epilogue (~18 cycles per output
-  // column per sub-tile) hides under the other resident CTA when two fit; whole waves of CTAs are counted.
+  // Chosen by the cost model of pick_tile_config: the main loop is bound by the bytes of TMA loads in flight per SM
+  // (ring capacity / ~3000-cycle load latency) unless the tensor pipe is slower (4*BN cycles per 64-channel k-block per
+  // 128-pixel sub-tile); the epilogue hides under the other resident CTA when two fit; whole waves of CTAs are counted.
   const int cout16 = (d.Cout + 15) / 16 * 16;
   const int num_kb = p.num_taps * p.kchunks;
   const bool contiguous_tiles = (p.bw == Wout) || (p.bh == 1);
@@ -320,21 +334,20 @@ inline int conv_finalize(ConvDesc& d) {
   const int want_persist = env_int("RS_CONV_PERSIST", -1);           // 0 / 1 disables / forces the persistent kernel
   // (the persistent kernel batches its GroupNorm arrivals in a shared list of kGnListCap (sink, image) entries)
   const bool persist_ok = d.has_out && !d.out_f32 && want_persist != 0 && !env_is("RS_CONV_EPI", "direct") &&
-                          !env_is("RS_CONV_IMPL", "simt") && env_int("RS_CONV_MSUB", 0) != 2 &&
-                          (!(d.sink[0].part || d.sink[1].part) || 2 * N <= kGnListCap);
+                          !env_is("RS_CONV_IMPL", "simt") && env_int("RS_CONV_MSUB", 0) != 2;
   const bool can_cluster_split = d.allow_split && contiguous_tiles && p.bn <= 2 && d.has_out && !d.out_f32 && d.Cout % 8 == 0;
   const TileConfig tc = pick_tile_config(m_tiles, cout16, num_kb, d.bn_override ? d.bn_override : env_int("RS_CONV_BN", 0), can_split,
                                          persist_ok && want_persist != 1, can_cluster_split);
   const int BN = tc.BN, msub = tc.msub, stages = tc.stages, cg = tc.cg;
   p.cg = cg;
   p.splitk = tc.splitk; p.partial = d.partial; p.splitk_cluster = tc.cluster_split;
-  RS_CHECK(BN >= 16 && BN <= 256 && BN % 16 == 0, "no valid tile configuration");
+  RS_CHECK(conv_kernel_for(BN, msub) != nullptr, "no valid tile configuration");
   p.BN = BN; p.n_tiles = (cout16 + BN - 1) / BN;
   p.msub = msub;
-  int cols = 32; while (cols < msub * BN) cols *= 2;
-  p.tmem_cols = cols;
-  const int stage_bytes = msub * kConvBM * kConvBK * 2 + (BN / cg) * kConvBK * 2;
+  const int stage_bytes = msub * kConvBM * kConvBK * 2 + BN * kConvBK * 2;
   p.stages = stages;
+  p.epi_off = 0;
+  p.bar_off = stages * stage_bytes;
   d.smem = (size_t)stages * stage_bytes + 1024 + 256 + 1024;   // ring + alignment slack + barriers + bias tile
   RS_CHECK(d.smem <= 227 * 1024, "shared memory budget exceeded");
   d.grid = (cg == 2 ? ((m_tiles + 1) / 2) * p.n_tiles * 2 : (m_tiles / msub) * p.n_tiles) * p.splitk;
@@ -391,19 +404,22 @@ inline int conv_finalize(ConvDesc& d) {
   // when RS_CONV_PERSIST = 1 forces it for any eligible layer
   {
     const int units = (cg == 2 ? (m_tiles + 1) / 2 : m_tiles) * p.n_tiles;
-    const int workers = cg == 2 ? 74 : 148;
-    const bool eligible = persist_ok && p.tma_out && p.splitk == 1 && msub == 1 && 2 * BN <= 512;
+    const int workers = cg == 2 ? num_sms() / 2 : num_sms();
+    const bool eligible = persist_ok && p.tma_out && p.splitk == 1 && msub == 1;
     p.persist = (eligible && (tc.persist || want_persist == 1)) ? 1 : 0;
     RS_CHECK(!tc.persist || p.persist, "persistent configuration chosen for an ineligible layer");
     p.num_units = units;
     if (p.persist) {
-      const size_t extra = (size_t)2 * BN * kConvBM * 2 + (size_t)4 * BN * 2 * sizeof(float) + (size_t)2 * BN * sizeof(float) + 256 + 1024 + sizeof(GnArriveList);
+      // the staging area (output tile + statistics scratch) follows the ring: the producer refills the ring while the
+      // consumers drain the previous tile
+      const size_t extra = conv_persist_extra_bytes(BN);
       const int st = (int)std::min<size_t>(8, ((size_t)227 * 1024 - extra) / (size_t)stage_bytes);
       RS_CHECK(st >= 2, "persistent conv: shared memory budget");
       p.stages = std::min(st, std::max(2, num_kb));
-      d.smem = (size_t)p.stages * stage_bytes + extra;
-      int cols2 = 32; while (cols2 < 2 * BN) cols2 *= 2;
-      p.tmem_cols = cols2;
+      p.epi_off = p.stages * stage_bytes;
+      p.bar_off = p.epi_off + (int)conv_epi_bytes(BN, 1);
+      d.smem = (size_t)p.bar_off + 256 + 1024 + 1024;
+      RS_CHECK(d.smem <= 227 * 1024, "persistent conv: shared memory budget");
       d.grid = cg * std::min(units, workers);
     }
   }
@@ -444,7 +460,7 @@ inline int conv_finalize(ConvDesc& d) {
     d.red_grid_x = r.slots;
     // column blocks so that the reduce kernel fills the machine even with one slot per image
     int cpc = d.Cout;
-    while (cpc > 64 && cpc % 16 == 0 && (long long)r.slots * N * (d.Cout / cpc) < 2 * 148) cpc /= 2;
+    while (cpc > 64 && cpc % 16 == 0 && (long long)r.slots * N * (d.Cout / cpc) < 2 * num_sms()) cpc /= 2;
     r.cols_per_cta = cpc;
     d.red_grid_z = (d.Cout + cpc - 1) / cpc;
     const int lanes = 256 / std::max(1, cpc / 8);
@@ -467,7 +483,7 @@ inline int conv_finalize(ConvDesc& d) {
     }
   }
   if (!env_is("RS_CONV_IMPL", "simt")) {
-    int rc = encode_weight_map(&p.tmB, d.wt, p.num_taps * d.ipad, d.Cout, BN / cg);
+    int rc = encode_weight_map(&p.tmB, d.wt, p.num_taps * d.ipad, d.Cout, BN / cg);   // pair mode: each CTA loads half
     if (rc) return rc;
   }
   return 0;
@@ -476,16 +492,17 @@ inline int conv_finalize(ConvDesc& d) {
 inline int conv_init() {   // once per process, outside any stream capture
   static bool attr_set = false;
   if (!attr_set) {
-    RS_CUDA_OK(cudaFuncSetAttribute(conv_gemm_sm100_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    RS_CUDA_OK(cudaFuncSetAttribute(conv_gemm_sm100_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    RS_CUDA_OK(cudaFuncSetAttribute(conv_gemm_persist_sm100_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    RS_CUDA_OK(cudaFuncSetAttribute(conv_gemm_persist_sm100_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    for (int bn : kConvBNs)
+      for (int ms = 1; ms <= 2; ++ms)
+        if (ConvKernelFn k = conv_kernel_for(bn, ms))
+          RS_CUDA_OK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     RS_CUDA_OK(cudaFuncSetAttribute(window_attn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));
-    RS_CUDA_OK(cudaFuncSetAttribute(mlp_fused_sm100_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    RS_CUDA_OK(cudaFuncSetAttribute(mlp_fused_sm90_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    RS_CUDA_OK(cudaFuncSetAttribute(mlp_fused_sm90_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    RS_CUDA_OK(cudaFuncSetAttribute(mlp_fused_sm90_kernel<192>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    RS_CUDA_OK(cudaFuncSetAttribute(mlp_fused_sm90_kernel<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     RS_CUDA_OK(cudaFuncSetAttribute(swin_attn_fused_kernel<192>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SwinSmem<192>::total));
     RS_CUDA_OK(cudaFuncSetAttribute(swin_attn_fused_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SwinSmem<64>::total));
-    RS_CUDA_OK(cudaFuncSetAttribute(swin_attn_tc_kernel<192>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SwinTcSmem<192>::total));
-    RS_CUDA_OK(cudaFuncSetAttribute(swin_attn_tc_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SwinTcSmem<64>::total));
     attr_set = true;
   }
   return 0;
@@ -497,15 +514,10 @@ inline int conv_launch(const ConvDesc& d, cudaStream_t st) {
     const int warps = 8;
     (void)launch_k(conv_simt_kernel, dim3((unsigned)((npix + warps - 1) / warps)), dim3(warps * 32), (size_t)(0), st, d.prm, d.simt);
   } else {
-    if (d.prm.persist && d.prm.cg == 2)
-      (void)launch_kc(conv_gemm_persist_sm100_kernel<2>, dim3(d.grid), dim3(kConvThreads), (size_t)(d.smem), st, 2, d.prm);
-    else if (d.prm.persist)
-      (void)launch_kc(conv_gemm_persist_sm100_kernel<1>, dim3(d.grid), dim3(kConvThreads), (size_t)(d.smem), st, 1, d.prm);
-    else if (d.prm.cg == 2)
-      (void)launch_kc(conv_gemm_sm100_kernel<2>, dim3(d.grid), dim3(kConvThreads), (size_t)(d.smem), st,
-                      d.prm.splitk_cluster ? 2 * d.prm.splitk : 2, d.prm);
-    else
-      (void)launch_kc(conv_gemm_sm100_kernel<1>, dim3(d.grid), dim3(kConvThreads), (size_t)(d.smem), st, 1, d.prm);
+    const ConvKernelFn k = conv_kernel_for(d.prm.BN, d.prm.msub);
+    RS_CHECK(k != nullptr, "no conv kernel for this channel tile");
+    const int cluster = d.prm.cg == 2 ? (d.prm.splitk_cluster ? 2 * d.prm.splitk : 2) : 1;
+    (void)launch_kc(k, dim3(d.grid), dim3(kConvThreads), (size_t)(d.smem), st, cluster, d.prm);
     if (d.prm.splitk > 1 && !d.prm.splitk_cluster)
       (void)launch_k(splitk_reduce_kernel, dim3(d.red_grid_x, d.prm.Nimg, d.red_grid_z), dim3(256), d.red_smem, st, d.red);
   }
@@ -543,7 +555,7 @@ struct GnDesc {
 inline void gn_chunks(int HW, int N, int* chunks, int* rows) {
   // enough CTAs to fill the machine, at least 32 rows each, and every chunk with the SAME number of rows (the
   // statistics combine assumes equal counts per slot): the largest divisor of HW not above the target
-  int c = std::max(1, std::min((HW + 31) / 32, (148 * 4 + N - 1) / N));
+  int c = std::max(1, std::min((HW + 31) / 32, (num_sms() * 4 + N - 1) / N));
   while (c > 1 && HW % c != 0) --c;
   *chunks = c; *rows = HW / c;
 }
@@ -576,7 +588,7 @@ inline int gn_launch(const GnDesc& g, cudaStream_t st) {
   }
   // apply: ~4 CTAs per SM in total, all resident at once (each CTA re-derives the per-channel affine from the
   // partials — a latency, not a bandwidth cost), at least 16 rows each
-  int actas = std::max(1, std::min((HW + 15) / 16, (148 * 4 + N - 1) / N));
+  int actas = std::max(1, std::min((HW + 15) / 16, (num_sms() * 4 + N - 1) / N));
   const int arows = (HW + actas - 1) / actas;
   actas = (HW + arows - 1) / arows;
   // small tensors: split the channels too (slices aligned to GroupNorm groups and to 8-channel vectors) until there
@@ -585,7 +597,7 @@ inline int gn_launch(const GnDesc& g, cudaStream_t st) {
   {
     const int cpg = C / 32;
     int unit = cpg; while (unit % 8) unit += cpg;                   // lcm(8, channels per group)
-    for (int cs = 2; actas * N * csplit < 222 && cs <= C / unit; ++cs)
+    for (int cs = 2; actas * N * csplit < num_sms() * 3 / 2 && cs <= C / unit; ++cs)
       if (C % cs == 0 && (C / cs) % unit == 0) csplit = cs;
   }
   GnApplyParams ap{g.in.ptr, g.in.sN(), g.in.ld, g.out.ptr, g.out.sN(), g.out.ld, C, HW, N, g.gstat, g.part, slots, g.eps,
@@ -595,7 +607,7 @@ inline int gn_launch(const GnDesc& g, cudaStream_t st) {
   return 0;
 }
 
-// ---- fused Swin MLP ---------------------------------------------------------------------------
+// ---- fused Swin MLP (mlp_fused.cuh) ---------------------------------------------------------------
 struct MlpDesc {
   View in, out, res;
   bool has_res = true;
@@ -603,7 +615,6 @@ struct MlpDesc {
   const __half* w2 = nullptr; const float* b2 = nullptr;    // fc2: [E][Hd] fp16
   int E = 0, Hd = 0;
   GnSink sink[2] = {};
-  long long* dbg = nullptr;
   // optional fused input GroupNorm (plain affine): `in` is then the un-normalised tensor
   const float* gn_in_gstat = nullptr;      // finalised group statistics, or
   const float* gn_in_part = nullptr; int gn_in_slots = 0;   // the producers' (mean, M2) pairs to combine in the kernel
@@ -613,18 +624,17 @@ struct MlpDesc {
 };
 
 inline bool mlp_supported(int E, int Hd, int H, int W, int N) {
+  (void)N;
   bool fus = false;
-  const int slots = conv_tile_slots(H, W, &fus);
-  const int bw = pow2_floor_div(W, kConvBM), bh = pow2_floor_div(H, kConvBM / bw), bn = kConvBM / (bw * bh);
-  const int tiles = slots * ((N + bn - 1) / bn);
-  return E % 64 == 0 && E <= 256 && Hd % kMlpHc == 0 && fus && tiles % 2 == 0;   // the kernel runs as CTA pairs
+  conv_tile_slots(H, W, &fus);
+  return (E == 64 || E == 128 || E == 192 || E == 256) && Hd % kMlpHc == 0 && fus;
 }
 
 inline int mlp_finalize(MlpDesc& d) {
   MlpParams& p = d.prm;
   std::memset(&p, 0, sizeof(p));
   const int H = d.in.H, W = d.in.W, N = d.in.N;
-  RS_CHECK(mlp_supported(d.E, d.Hd, H, W, N), "fused MLP: unsupported shape (E % 64, E <= 256, hidden % 128, even tile count)");
+  RS_CHECK(mlp_supported(d.E, d.Hd, H, W, N), "fused MLP: unsupported shape (E in {64, 128, 192, 256}, hidden % 64)");
   RS_CHECK(d.in.C == d.E && d.out.C == d.E, "fused MLP: channel mismatch");
   p.E = d.E; p.Hd = d.Hd; p.bias1 = d.b1; p.bias2 = d.b2;
   p.bw = pow2_floor_div(W, kConvBM);
@@ -633,44 +643,25 @@ inline int mlp_finalize(MlpDesc& d) {
   p.tiles_w = W / p.bw; p.tiles_h = H / p.bh;
   const int tiles_n = (N + p.bn - 1) / p.bn;
   p.Wout = W; p.Hout = H; p.Nimg = N;
-  // shared memory per CTA: X (E/64 tiles) + two H buffers + barriers + both bias vectors; the rest is ring slots for
-  // this CTA's HALF of the weight tiles: two hidden chunks of the fc2 stream, everything else to the fc1 stream
-  const size_t kW1 = (size_t)(kMlpHc / 2) * 128;
-  const size_t slot2 = (size_t)(d.E / 2) * 128;
-  const int kHT = kMlpHc / 64, kx = d.E / 64;
-  const size_t fixed = (size_t)kx * 16384 + (size_t)2 * kHT * 16384 + 1024 + 512 + (size_t)(d.Hd + d.E) * sizeof(float) +
-                       (size_t)(2 * d.E * 2 + 2 * 32 * 2) * sizeof(float);   // + input-GN affine / group statistics
-  RS_CHECK(fixed + kHT * slot2 + (size_t)kx * kW1 <= 227 * 1024, "fused MLP: not enough shared memory for the weight rings");
-  const size_t budget = 227 * 1024 - fixed;
-  p.ring2 = (int)std::min<size_t>(2 * kHT, (budget - (size_t)kx * kW1) / slot2);
-  p.ring1 = (int)std::min<size_t>(12, (budget - (size_t)p.ring2 * slot2) / kW1);
-  p.has_res = d.has_res ? 1 : 0;
-  const int tiles = p.tiles_w * p.tiles_h * tiles_n;      // even (mlp_supported): CTA pairs
-  // few-tile layers (8x8 / 16x16 levels): split the hidden dimension over two pairs of one cluster; partial outputs
-  // meet in distributed shared memory (RS_MLP_HSPLIT = 1 disables, = 2 forces)
-  {
-    const int want = env_int("RS_MLP_HSPLIT", 0);
-    const bool can = (d.Hd / kMlpHc) >= 2 && (d.E / 2) % 8 == 0 &&
-                     (size_t)kConvBM * (d.E * 4 + 16) + (size_t)kConvBM * (d.E / 2) * 2 + (size_t)2 * d.E * 4 <= (size_t)200 * 1024;
-    p.hsplit = (can && want != 1 && (want == 2 || tiles <= 64)) ? 2 : 1;
-  }
-  d.grid = tiles * p.hsplit;
-  p.out_ptr = d.out.ptr; p.out_sN = d.out.sN(); p.out_sH = d.out.sH(); p.out_sW = d.out.sW();
-  p.res_ptr = d.has_res ? d.res.ptr : nullptr;
-  if (d.has_res) { p.res_sN = d.res.sN(); p.res_sH = d.res.sH(); p.res_sW = d.res.sW(); }
-  d.smem = fixed + (size_t)p.ring1 * kW1 + (size_t)p.ring2 * slot2;
+  // ring slots for the weight tiles: as many as fit next to X, one hidden chunk and the bias / affine tables
+  const int slot = std::max(kMlpHc, d.E) * kConvBK * 2;
+  const int fixed = MlpSmem(d.E, d.Hd, 0).total + 1024;     // + alignment slack
+  p.ring = std::min(8, (227 * 1024 - fixed) / slot);
+  RS_CHECK(p.ring >= 2, "fused MLP: not enough shared memory for the weight ring");
+  d.smem = (size_t)MlpSmem(d.E, d.Hd, p.ring).total + 1024;
   RS_CHECK(d.smem <= 227 * 1024, "fused MLP: shared memory budget exceeded");
+  p.has_res = d.has_res ? 1 : 0;
+  d.grid = p.tiles_w * p.tiles_h * tiles_n;
   int rc = encode_act_map(&p.tmX, d.in.ptr, d.E, W, H, N, d.in.sW(), d.in.sH(), d.in.sN(), p.bw, p.bh, p.bn, 64);
   if (rc) return rc;
-  rc = encode_weight_map(&p.tmW1, d.w1, d.E, d.Hd, kMlpHc / 2); if (rc) return rc;   // each CTA of a pair fetches half a tile
-  rc = encode_weight_map(&p.tmW2, d.w2, d.Hd, d.E, d.E / 2); if (rc) return rc;
+  rc = encode_weight_map(&p.tmW1, d.w1, d.E, d.Hd, kMlpHc); if (rc) return rc;
+  rc = encode_weight_map(&p.tmW2, d.w2, d.Hd, d.E, d.E); if (rc) return rc;
   rc = encode_act_map(&p.tmOut, d.out.ptr, d.E, W, H, N, d.out.sW(), d.out.sH(), d.out.sN(), p.bw, p.bh, p.bn, 64);
   if (rc) return rc;
   if (d.has_res) {
     rc = encode_act_map(&p.tmRes, d.res.ptr, d.E, W, H, N, d.res.sW(), d.res.sH(), d.res.sN(), p.bw, p.bh, p.bn, 64);
     if (rc) return rc;
   }
-  p.dbg = d.dbg;
   p.gn_in_gstat = d.gn_in_gstat; p.gn_in_part = d.gn_in_part; p.gn_in_slots = d.gn_in_slots;
   p.gn_in_gamma = d.gn_in_gamma; p.gn_in_beta = d.gn_in_beta; p.gn_in_eps = 1e-5f;
   RS_CHECK(!(d.gn_in_gstat || d.gn_in_part) || (d.gn_in_gamma && d.gn_in_beta && d.Hd >= 4 * d.E && d.E % 32 == 0),
@@ -691,13 +682,18 @@ inline int mlp_finalize(MlpDesc& d) {
 }
 
 inline int mlp_launch(const MlpDesc& d, cudaStream_t st) {
-  (void)launch_kc(mlp_fused_sm100_kernel, dim3(d.grid), dim3(kMlpThreads), d.smem, st, 2 * d.prm.hsplit, d.prm);
+  switch (d.E) {
+    case 64: (void)launch_k(mlp_fused_sm90_kernel<64>, dim3(d.grid), dim3(kMlpThreads), d.smem, st, d.prm); break;
+    case 128: (void)launch_k(mlp_fused_sm90_kernel<128>, dim3(d.grid), dim3(kMlpThreads), d.smem, st, d.prm); break;
+    case 192: (void)launch_k(mlp_fused_sm90_kernel<192>, dim3(d.grid), dim3(kMlpThreads), d.smem, st, d.prm); break;
+    case 256: (void)launch_k(mlp_fused_sm90_kernel<256>, dim3(d.grid), dim3(kMlpThreads), d.smem, st, d.prm); break;
+    default: RS_CHECK(false, "fused MLP: embedding width");
+  }
   RS_CUDA_OK(cudaGetLastError());
   return 0;
 }
 
-// ---- fused attention half of a Swin block (swin_attn_fused.cuh, swin_attn_tc.cuh) -----------------
-static long long* g_swin_timeline = nullptr;   // rs_debug_swin_timeline
+// ---- fused attention half of a Swin block (swin_attn_fused.cuh) -----------------
 struct SwinAttnDesc {
   View x, y;                               // input / output token tensors [N, H, W, E] (y may alias x)
   int heads = 0, shift = 0;
@@ -708,12 +704,10 @@ struct SwinAttnDesc {
   const __half* wproj = nullptr; int wproj_ld = 0; const float* bproj = nullptr;
   GnSink sink[2] = {};
   SwinAttnParams prm;
-  SwinTcParams tc;                         // tcgen05 version (swin_attn_tc.cuh): tensor maps of the two weight matrices
-  bool use_tc = false;
-  long long* dbg = nullptr;
+  // the kernel delivers window pairs; a sink with group statistics gets them from gn_finalize_kernel right after it
+  GnFinalizeParams fin[2] = {};
   int grid = 0;
 };
-inline bool swin_attn_uses_tc() { return !env_is("RS_SWIN_IMPL", "mma"); }
 inline bool swin_attn_supported(int E, int heads, int H, int W) {
   return (E == 192 || E == 64) && heads * 32 == E && H % 8 == 0 && W % 8 == 0;
 }
@@ -742,29 +736,27 @@ inline int swin_attn_finalize(SwinAttnDesc& d) {
     }
   }
   const int pairs = (p.total_windows + 1) / 2;
-  d.grid = std::min(pairs, 148);
-  // tcgen05 version unless RS_SWIN_IMPL=mma (the mma.sync kernel stays as the tested restatement of the same arithmetic)
-  d.use_tc = swin_attn_uses_tc() && d.wqkv_ld == E && d.wproj_ld == E;
-  if (!d.use_tc)                                            // the mma.sync kernel delivers pairs only: consumers combine them
-    for (int k = 0; k < 2; ++k) { p.sink[k].gstat = nullptr; p.sink[k].counter = nullptr; }
-  if (d.use_tc) {
-    std::memset(&d.tc, 0, sizeof(d.tc));
-    d.tc.a = p; d.tc.dbg = d.dbg;
-    int rc = encode_weight_map(&d.tc.tmWqkv, d.wqkv, E, 3 * E, 64); if (rc) return rc;
-    rc = encode_weight_map(&d.tc.tmWproj, d.wproj, E, E, E); if (rc) return rc;
+  d.grid = std::min(pairs, num_sms());
+  const int nW = (d.x.H / 8) * (d.x.W / 8);
+  for (int k = 0; k < 2; ++k) {
+    d.fin[k] = GnFinalizeParams{};
+    if (p.sink[k].gstat) {
+      RS_CHECK(p.sink[k].coff == 0 && p.sink[k].cstride == E, "fused Swin attention: group statistics of a channel slice");
+      d.fin[k] = GnFinalizeParams{p.sink[k].part, p.sink[k].gstat, nW, E, 64.0f, p.sink[k].eps};
+    }
+    p.sink[k].gstat = nullptr; p.sink[k].counter = nullptr;
   }
   return 0;
 }
 inline int swin_attn_launch(const SwinAttnDesc& d, cudaStream_t st) {
-  if (d.use_tc) {
-    if (d.x.C == 192) (void)launch_k(swin_attn_tc_kernel<192>, dim3(d.grid), dim3(kTcThreads), (size_t)SwinTcSmem<192>::total, st, d.tc);
-    else (void)launch_k(swin_attn_tc_kernel<64>, dim3(d.grid), dim3(kTcThreads), (size_t)SwinTcSmem<64>::total, st, d.tc);
-    RS_CUDA_OK(cudaGetLastError());
-    return 0;
-  }
   if (d.x.C == 192) (void)launch_k(swin_attn_fused_kernel<192>, dim3(d.grid), dim3(kSwinThreads), SwinSmem<192>::total, st, d.prm);
   else (void)launch_k(swin_attn_fused_kernel<64>, dim3(d.grid), dim3(kSwinThreads), SwinSmem<64>::total, st, d.prm);
   RS_CUDA_OK(cudaGetLastError());
+  for (int k = 0; k < 2; ++k)
+    if (d.fin[k].gstat) {
+      (void)launch_k(gn_finalize_kernel, dim3(32, d.x.N), dim3(256), (size_t)0, st, d.fin[k]);
+      RS_CUDA_OK(cudaGetLastError());
+    }
   return 0;
 }
 
@@ -779,8 +771,8 @@ inline int attn_launch(const View& qkv, const View& out, const float* bias, int 
   const int windows = qkv.N * (qkv.H / 8) * (qkv.W / 8);
   // heads per CTA: all of them when there are plenty of windows, fewer (more CTAs) otherwise
   int hpc = heads;
-  while (hpc > 1 && (long long)windows * (heads / hpc) < 4 * 148 && hpc % 2 == 0) hpc /= 2;
-  if (hpc > 1 && (long long)windows * (heads / hpc) < 4 * 148 && heads % hpc == 0) hpc = 1;
+  while (hpc > 1 && (long long)windows * (heads / hpc) < 4 * num_sms() && hpc % 2 == 0) hpc /= 2;
+  if (hpc > 1 && (long long)windows * (heads / hpc) < 4 * num_sms() && heads % hpc == 0) hpc = 1;
   WinAttnParams p{qkv.ptr, qkv.ld, out.ptr, out.ld, bias, qkv.N, qkv.H, qkv.W, heads, E, shift, 0.17677669529663687f, hpc};
   if (env_is("RS_ATTN_IMPL", "simt")) {
     (void)launch_k(window_attn_simt_kernel, dim3(windows, heads), dim3(64), (size_t)0, st, p);

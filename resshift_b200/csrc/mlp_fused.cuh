@@ -1,21 +1,20 @@
-// Fused Swin MLP:  out = residual + fc2( GELU( fc1(x) ) )  in ONE kernel, hidden activations never leave the SM.
+// Fused Swin MLP:  out = residual + fc2( GELU( fc1(x) ) )  in ONE kernel on wgmma, hidden activations never leave the SM.
 //
 // reference: Mlp.forward (models/swin_transformer.py:27-33: 1x1 conv E -> 4E, exact-erf GELU, 1x1 conv 4E -> E) and the
 // residual add around it in SwinTransformerBlock.forward (:279).  Unfused this is two GEMMs with a [pixels, 4E] fp16
-// intermediate (100 MB at batch 16, 64x64) written to and re-read from HBM; here a CTA owns a 128-pixel tile and walks
-// the hidden dimension in chunks of 128:
+// intermediate written to and re-read from HBM; here a CTA owns a 128-pixel tile and walks the hidden dimension in
+// chunks of 64 (with the accumulators of both GEMMs in registers, a wider chunk would spill).  Each of the two consumer
+// warpgroups owns 64 rows of the tile:
 //
-//     acc1[128 x 128]  = X[128 x E] . W1_j^T            (tcgen05, TMEM, double buffered over chunks j)
-//     H_j              = GELU(acc1 + b1_j)  -> fp16, written to shared memory AS THE NEXT MMA's A OPERAND
-//                                              (K-major, 128-byte swizzle: exactly what a TMA load would have produced)
-//     acc2[128 x E]   += H_j . W2_j^T                    (tcgen05, TMEM, accumulates over all chunks)
+//     acc1[64 x 64]   = X[64 x E] . W1_j^T            (wgmma, registers)
+//     H_j             = GELU(acc1 + b1_j) -> fp16, written to shared memory as the next wgmma's A operand
+//                                           (K-major, 128-byte swizzle: what a TMA load would have produced)
+//     acc2[64 x E]   += H_j . W2_j^T                   (wgmma, registers, accumulates over all chunks)
 //
-// then the usual staged epilogue (+ b2, + residual through a TMA load, fp16, TMA store, fused GroupNorm partials).
-// Warp roles: warps 0..15 = GELU stage + final epilogue, warps 16 / 17 = TMA producers (X once + the W1_j tiles; the
-// W2_j tiles; one ring each), warp 18 = MMA issuer (each GELU warp owns a 32-row x 16-column slice of every
-// chunk and signals the MMA warp on its own: no CTA-wide barrier in the loop).  MMA1 of chunk j+1 overlaps the GELU
-// stage of chunk j.  The kernel runs as CTA pairs (cluster of 2, tcgen05 cta_group::2): 256 pixels per pair, each CTA
-// stages its own 128 pixels of X / H and half of every weight tile; the leader CTA issues the MMAs of both.
+// then the staged epilogue of conv_gemm.cuh (+ b2, + residual through a TMA load, fp16, TMA store, GroupNorm partials).
+// Warp 8 is the TMA producer: X once, then per chunk the fc1 weight tiles followed by the fc2 weight tiles, through one
+// ring of slots in the order the consumers use them.  Optionally the Swin block's norm2 is applied to the X tile in shared
+// memory first (same arithmetic as gn_apply_kernel, so the operand is bit-identical to the separate pass).
 #pragma once
 
 #include "common.cuh"
@@ -23,35 +22,22 @@
 
 namespace rs {
 
-constexpr int kMlpHc = 128;          // hidden columns per chunk (64-column chunks make the MMA issue rate the bottleneck)
-constexpr int kMlpEpiWarps = 16;     // four warps per TMEM lane quadrant: the GELU stage is instruction-bound
-constexpr int kMlpThreads = 96 + 32 * kMlpEpiWarps;
-// warps 0..15: GELU + epilogue; warps 16 / 17: TMA producers; warp 18: MMA issuer.  The scheduler picks the highest
-// eligible warp id first, so the single-thread control warps must sit above the instruction-bound GELU warps or every
-// MMA issue waits behind them (profiles/r1_s20_mlp_timeline.log: ~400 cycles per tcgen05.mma with the old order).
-constexpr int kMlpTma1Warp = kMlpEpiWarps, kMlpTma2Warp = kMlpEpiWarps + 1, kMlpMmaWarp = kMlpEpiWarps + 2;
+constexpr int kMlpHc = 64;                  // hidden columns per chunk (one 128-byte swizzled K tile of GEMM 2)
+constexpr int kMlpThreads = kConvThreads;   // two consumer warpgroups + the TMA producer warp
+constexpr int kMlpTmaWarp = kConvTmaWarp;
 
 struct MlpParams {
   CUtensorMap tmX, tmW1, tmW2, tmOut, tmRes;
   const float* bias1;                // [Hd]
   const float* bias2;                // [E]
-  int E, Hd;                         // E % 64 == 0, E <= 256;  Hd % 64 == 0
-  int ring1, ring2;                  // ring depths: fc1 weight half-tiles (kMlpHc/2 x 64), fc2 weight half-tiles (E/2 x 64)
+  int E, Hd;                         // E in {64, 128, 192, 256};  Hd % 64 == 0
+  int ring;                          // weight ring depth (slots of max(64, E) rows x 64 fp16)
   int bw, bh, bn, tiles_w, tiles_h;
   int Wout, Hout, Nimg;
   int has_res;
-  const __half* res_ptr; long long res_sN, res_sH, res_sW;   // raw NHWC views for the hsplit epilogue
-  __half* out_ptr; long long out_sN, out_sH, out_sW;
-  int hsplit;                        // 1, or 2: the hidden dimension is split over two CTA pairs of one cluster (few-tile
-                                     // layers); each pair walks half of the chunks and the partial outputs are summed
-                                     // through distributed shared memory, each pair finishing half of the E columns
   GnSink sink[2]; int gn_slots;      // fused GroupNorm statistics of the output (gn_stats.cuh)
-  long long* dbg;                    // optional: CTA 0 writes a clock64 timeline [64 chunks][8] (profiling aid)
   // optional fused input GroupNorm (the Swin block's norm2, models/swin_transformer.py:279): X is then the UN-normalised
-  // tensor and the CTA applies  a*x + b  (per image, per channel; plain affine, no FiLM / SiLU) to its X tile in
-  // shared memory before the first GEMM — one gn_apply launch and one activation round trip less per Swin block.
-  // Statistics arrive as the per-(image, group) pairs (mean, rstd) finalised by the producer (gn_stats.cuh), exactly
-  // as gn_apply_kernel reads them: the operand equals what the separate pass would have stored, bit for bit.
+  // tensor and the CTA applies  a*x + b  (per image, per channel) to its X tile in shared memory before the first GEMM
   const float* gn_in_gstat;          // [N][32][2] finalised by the producer, or nullptr
   const float* gn_in_part;           // [N][gn_in_slots][E][2] (mean, M2) pairs, combined here when gn_in_gstat == nullptr
   int gn_in_slots;
@@ -60,480 +46,291 @@ struct MlpParams {
   const float* gn_in_beta;           // [E]
 };
 
+// shared-memory layout (offsets from the 1024-aligned base)
+struct MlpSmem {
+  int x, h, ring, bars, b1, b2, ab, total;
+  __host__ __device__ MlpSmem(int E, int Hd, int ring_depth) {
+    const int slot = (E > kMlpHc ? E : kMlpHc) * kConvBK * 2;
+    x = 0;                                          // E/64 tiles of [128 rows x 64] (the staging area at the end)
+    h = x + (E / 64) * kConvBM * kConvBK * 2;       // [128 rows x 64]: one hidden chunk
+    ring = h + (kMlpHc / 64) * kConvBM * kConvBK * 2;
+    bars = ring + ring_depth * slot;
+    b1 = bars + 1024;
+    b2 = b1 + Hd * 4;
+    ab = b2 + E * 4;                                // [2][E][2] input-GN affine, then [2][32][2] group (mean, rstd)
+    total = ab + (4 * E + 128) * 4;
+  }
+};
+
 #ifdef __CUDACC__
 
-__global__ void __launch_bounds__(kMlpThreads, 1) mlp_fused_sm100_kernel(const __grid_constant__ MlpParams p) {
+template <int E>
+__global__ void __launch_bounds__(kMlpThreads, 1) mlp_fused_sm90_kernel(const __grid_constant__ MlpParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  const int kx = p.E >> 6;                         // k-blocks of the first GEMM
-  const int chunks_total = p.Hd / kMlpHc;
+  constexpr int kx = E / 64;                       // k-blocks of the first GEMM
   constexpr int kTile = kConvBM * kConvBK * 2;     // 16 KB: 128 rows x 64 fp16
-  constexpr int kW1 = (kMlpHc / 2) * kConvBK * 2;  // this CTA's half of an fc1 weight tile: kMlpHc/2 rows x 64 fp16
-  constexpr int kHT = kMlpHc / kConvBK;            // 64-column tiles per hidden chunk (= k-blocks of the second GEMM)
-  uint8_t* sX = smem;                              // kx tiles (this CTA's 128 pixels)
-  const int slot2 = (p.E / 2) * 128;               // this CTA's half of an fc2 weight tile: E/2 rows x 64 fp16
-  uint8_t* sW1 = sX + (size_t)kx * kTile;          // ring1 x kW1     (two rings, a producer warp each: neither weight
-  uint8_t* sW2 = sW1 + (size_t)p.ring1 * kW1;      // ring2 x slot2    stream ever waits behind the other one's slots)
-  uint8_t* sH = sW2 + (size_t)p.ring2 * slot2;     // 2 buffers x kHT tiles
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sH + 2 * kHT * kTile);
-  uint64_t* w1_full = bars;                        // leader's: bytes of BOTH CTAs' halves
-  uint64_t* w1_empty = w1_full + p.ring1;          // per CTA: released by the leader's multicast tcgen05.commit
-  uint64_t* w2_full = w1_empty + p.ring1;
-  uint64_t* w2_empty = w2_full + p.ring2;
-  uint64_t* x_full = w2_empty + p.ring2;           // leader's
-  uint64_t* acc1_full = x_full + 1;                // [2] per CTA (multicast commit)
-  uint64_t* acc1_empty = acc1_full + 2;            // [2] leader's: one arrival per GELU warp of both CTAs
-  uint64_t* h_full = acc1_empty + 2;               // [2] leader's: same
-  uint64_t* h_empty = h_full + 2;                  // [2] per CTA (multicast commit)
-  uint64_t* acc2_full = h_empty + 2;               // per CTA (multicast commit)
-  uint64_t* res_bar = acc2_full + 1;
-  uint64_t* x_ready = res_bar + 1;                 // leader's: X tiles of both CTAs normalised in place (fused input GN)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(x_ready + 1);
-  float* s_b1 = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(bars) + 512);   // [Hd] fc1 bias
-  float* s_b2 = s_b1 + p.Hd;                                                          // [E]  fc2 bias
-  float* s_ab = s_b2 + p.E;                                                           // [2 images][E][2] input-GN affine, [2][32][2] mean / rstd
+  constexpr int kW1 = kMlpHc * kConvBK * 2;        // fc1 weight tile: 64 hidden rows x 64 fp16
+  constexpr int kW2 = E * kConvBK * 2;             // fc2 weight tile: E rows x 64 fp16
+  constexpr int kSlot = kW1 > kW2 ? kW1 : kW2;
+  const MlpSmem L(E, p.Hd, p.ring);
+  uint8_t* sX = smem + L.x;
+  uint8_t* sH = smem + L.h;
+  uint8_t* sRing = smem + L.ring;
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + L.bars);
+  uint64_t* empty_bar = full_bar + p.ring;
+  uint64_t* x_full = empty_bar + p.ring;
+  uint64_t* res_bar = x_full + 1;
+  float* s_b1 = reinterpret_cast<float*>(smem + L.b1);
+  float* s_b2 = reinterpret_cast<float*>(smem + L.b2);
+  float* s_ab = reinterpret_cast<float*>(smem + L.ab);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  long long* dbg = (p.dbg && blockIdx.x == 0) ? p.dbg : nullptr;
-  const long long t_start = clock64();
-  // CTA pair (cluster of 2, tcgen05 cta_group::2): a 256-pixel tile, 128 pixels per CTA.  Each CTA stages only HALF of
-  // every weight tile, so the same shared memory holds two hidden chunks of both weight streams in flight (one chunk
-  // deep the loop is a chain of exposed load latencies: profiles/r1_s18_*), and the L2 -> SM weight traffic halves.
-  // cluster rank = 2 * (hidden-dimension split) + (rank inside the pair); the pair's leader is the even rank
-  const uint32_t crank = cluster_ctarank();
-  const uint32_t rank = crank & 1;                 // leader = rank 0: arms the operand barriers, issues every MMA
-  const uint32_t lead = crank & ~1u;
-  const uint16_t pmask = (uint16_t)(3u << lead);   // multicast mask of this pair
-  const int hs = (int)(crank >> 1);
-  const int jc0 = hs * chunks_total / p.hsplit;                    // this pair's chunk range [jc0, jc0 + chunks)
-  const int chunks = (hs + 1) * chunks_total / p.hsplit - jc0;
-  int mt = (int)(blockIdx.x / (2 * p.hsplit)) * 2 + (int)rank;
+  const int chunks = p.Hd / kMlpHc;
+  int mt = (int)blockIdx.x;
   const int tw = mt % p.tiles_w; mt /= p.tiles_w;
   const int th = mt % p.tiles_h; mt /= p.tiles_h;
   const int w0 = tw * p.bw, h0 = th * p.bh, n0 = mt * p.bn;
+  const bool gn_in = p.gn_in_gstat || p.gn_in_part;
 
-  if (warp == kMlpTma1Warp && lane == 0) {
+  if (warp == kMlpTmaWarp && lane == 0) {
     tma_prefetch_desc(&p.tmX); tma_prefetch_desc(&p.tmW1); tma_prefetch_desc(&p.tmW2);
     tma_prefetch_desc(&p.tmOut); if (p.has_res) tma_prefetch_desc(&p.tmRes);
-    for (int s = 0; s < p.ring1; ++s) { mbar_init(&w1_full[s], 1); mbar_init(&w1_empty[s], 1); }
-    for (int s = 0; s < p.ring2; ++s) { mbar_init(&w2_full[s], 1); mbar_init(&w2_empty[s], 1); }
-    mbar_init(x_full, 1);
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(&acc1_full[b], 1); mbar_init(&h_empty[b], 1);                                 // tcgen05.commit
-      mbar_init(&acc1_empty[b], 2 * kMlpEpiWarps); mbar_init(&h_full[b], 2 * kMlpEpiWarps);   // GELU warps of both CTAs
-    }
-    mbar_init(acc2_full, 1); mbar_init(res_bar, 1); mbar_init(x_ready, 2 * kMlpEpiWarps);
+    for (int s = 0; s < p.ring; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], kConvEpiWarps); }
+    mbar_init(x_full, 1); mbar_init(res_bar, 1);
     mbar_fence_init();
   }
-  if (warp == kMlpMmaWarp) { tmem_alloc_dyn_cg2(tmem_slot, 512u); tmem_relinquish_cg2(); }
-  tc_fence_before();
-  cluster_sync_all();                              // peer barriers exist before any remote arrival / peer TMA completion
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t tm_acc2 = tmem_base + 2 * kMlpHc;
+  __syncthreads();
   pdl_trigger();
   pdl_wait();
 
-  // Control warps run warp-uniformly with only the asynchronous instructions predicated on one elected lane (see
-  // conv_gemm.cuh: keeps addresses / descriptors in uniform registers and the issue loops short).
-  if (warp == kMlpTma1Warp) {
-    // ===================== TMA producer 1: X once, then the fc1 weight stream =====================
-    // (the two weight streams have a warp each: a lane blocked in mbarrier.try_wait stalls its whole warp)
+  if (warp == kMlpTmaWarp) {
+    // ===================== TMA producer: X once, then per chunk kx fc1 tiles and one fc2 tile =====================
     const bool el = elect_one();
-    const uint32_t lead_x = mapa_u32(smem_u32(x_full), lead);
     if (el) {
-      if (p.gn_in_gstat || p.gn_in_part) {
-        // fused input GroupNorm: each CTA's GELU warps wait for their OWN tile, normalise it, then signal the leader
-        mbar_arrive_expect_tx(x_full, (uint32_t)(kx * kTile));
-        for (int kb = 0; kb < kx; ++kb) tma_load_4d(sX + (size_t)kb * kTile, &p.tmX, x_full, kb * kConvBK, w0, h0, n0);
-      } else {
-        if (rank == 0) mbar_arrive_expect_tx(x_full, (uint32_t)(2 * kx * kTile));
-        for (int kb = 0; kb < kx; ++kb) tma_load_4d_cg2(sX + (size_t)kb * kTile, &p.tmX, lead_x, kb * kConvBK, w0, h0, n0);
-      }
+      mbar_arrive_expect_tx(x_full, (uint32_t)(kx * kTile));
+      for (int kb = 0; kb < kx; ++kb) tma_load_4d(sX + (size_t)kb * kTile, &p.tmX, x_full, kb * kConvBK, w0, h0, n0);
     }
-    int st1 = 0; uint32_t ph1 = 0;
-    const int row0 = (int)rank * (kMlpHc / 2);
-    for (int j = 0; j < chunks; ++j)
-      for (int kb = 0; kb < kx; ++kb) {
-        mbar_wait(&w1_empty[st1], ph1 ^ 1);
-        // both CTAs' halves complete on the LEADER's barrier; only the leader arms it (with the bytes of both)
-        const uint32_t lead_bar = mapa_u32(smem_u32(&w1_full[st1]), lead);
-        if (el) {
-          if (rank == 0) mbar_arrive_expect_tx(&w1_full[st1], (uint32_t)(2 * kW1));
-          tma_load_2d_cg2(sW1 + (size_t)st1 * kW1, &p.tmW1, lead_bar, kb * kConvBK, (jc0 + j) * kMlpHc + row0);
-        }
-        if (++st1 == p.ring1) { st1 = 0; ph1 ^= 1; }
-      }
-  } else if (warp == kMlpTma2Warp) {
-    // ===================== TMA producer 2: the fc2 weight stream =====================
-    const bool el = elect_one();
-    int st2 = 0; uint32_t ph2 = 0;
-    const int row0 = (int)rank * (p.E / 2);
-    for (int j = 0; j < chunks; ++j)
-      for (int t = 0; t < kHT; ++t) {
-        mbar_wait(&w2_empty[st2], ph2 ^ 1);
-        const uint32_t lead_bar = mapa_u32(smem_u32(&w2_full[st2]), lead);
-        if (el) {
-          if (rank == 0) mbar_arrive_expect_tx(&w2_full[st2], (uint32_t)(2 * slot2));
-          tma_load_2d_cg2(sW2 + (size_t)st2 * slot2, &p.tmW2, lead_bar, (jc0 + j) * kMlpHc + t * kConvBK, row0);
-        }
-        if (++st2 == p.ring2) { st2 = 0; ph2 ^= 1; }
-      }
-  } else if (warp == kMlpMmaWarp) {
-    if (rank == 0) {
-      // ===================== MMA issuer (leader CTA) =====================
-      // order: GEMM1(0), GEMM1(1), then per chunk j: GEMM2(j) as soon as H_j is written, then GEMM1(j + 2) into the
-      // accumulator buffer GELU(j) has just released — the GELU warps always find the next chunk's acc1 ready.
-      const bool el = elect_one();
-      const uint32_t idesc1 = umma_idesc_f16(2 * kConvBM, kMlpHc);
-      const uint32_t idesc2 = umma_idesc_f16(2 * kConvBM, p.E);
-      const uint32_t sX0 = smem_u32(sX), sW10 = smem_u32(sW1), sW20 = smem_u32(sW2), sH0 = smem_u32(sH);
-      int st1 = 0, st2 = 0; uint32_t ph1 = 0, ph2 = 0;
-      auto gemm1 = [&](int c) {
-        const int b = c & 1;
-        mbar_wait(&acc1_empty[b], ((c >> 1) & 1) ^ 1);
-        tc_fence_after();
-        if (dbg && el) dbg[c * 8 + 0] = clock64() - t_start;
-        const uint32_t d = tmem_base + b * kMlpHc;
-        for (int kb = 0; kb < kx; ++kb) {
-          mbar_wait(&w1_full[st1], ph1);
-          tc_fence_after();
-          const uint64_t adesc = umma_desc_sw128(sX0 + (uint32_t)kb * kTile);
-          const uint64_t bdesc = umma_desc_sw128(sW10 + (uint32_t)st1 * kW1);
-          if (el) {
-            umma_f16_cg2(d, adesc, bdesc, idesc1, kb != 0 ? 1u : 0u);
-#pragma unroll
-            for (int k = 1; k < 4; ++k) umma_f16_cg2(d, adesc + 2 * k, bdesc + 2 * k, idesc1, 1u);
-            umma_commit_cg2(&w1_empty[st1], pmask);                       // frees the slot in BOTH CTAs
-            if (kb == kx - 1) umma_commit_cg2(&acc1_full[b], pmask);
-          }
-          if (++st1 == p.ring1) { st1 = 0; ph1 ^= 1; }
-        }
-        if (dbg && el) dbg[c * 8 + 1] = clock64() - t_start;
-      };
-      mbar_wait((p.gn_in_gstat || p.gn_in_part) ? x_ready : x_full, 0);
-      tc_fence_after();
-      gemm1(0);
-      if (chunks > 1) gemm1(1);
-      for (int j = 0; j < chunks; ++j) {
-        const int b = j & 1;
-        mbar_wait(&h_full[b], (j >> 1) & 1);
-        tc_fence_after();
-        if (dbg && el) dbg[j * 8 + 2] = clock64() - t_start;
-        for (int t = 0; t < kHT; ++t) {
-          mbar_wait(&w2_full[st2], ph2);
-          tc_fence_after();
-          const uint64_t adesc = umma_desc_sw128(sH0 + (uint32_t)(b * kHT + t) * kTile);
-          const uint64_t bdesc = umma_desc_sw128(sW20 + (uint32_t)st2 * (uint32_t)slot2);
-          if (el) {
-            umma_f16_cg2(tm_acc2, adesc, bdesc, idesc2, (j | t) != 0 ? 1u : 0u);
-#pragma unroll
-            for (int k = 1; k < 4; ++k) umma_f16_cg2(tm_acc2, adesc + 2 * k, bdesc + 2 * k, idesc2, 1u);
-            umma_commit_cg2(&w2_empty[st2], pmask);
-            if (t == kHT - 1) {
-              umma_commit_cg2(&h_empty[b], pmask);
-              if (j == chunks - 1) umma_commit_cg2(acc2_full, pmask);
-            }
-          }
-          if (++st2 == p.ring2) { st2 = 0; ph2 ^= 1; }
-        }
-        if (dbg && el) dbg[j * 8 + 3] = clock64() - t_start;
-        if (j + 2 < chunks) gemm1(j + 2);
-      }
-    }
-  } else {
-    // ===================== GELU stage + final epilogue (16 warps per CTA, this CTA's 128 pixels) =====================
-    // warp -> TMEM lane quadrant (warp % 4) and one 16-column slice of every 64 hidden columns; warps run
-    // independently (per-warp arrivals on the LEADER's barriers, no CTA-wide barrier inside the chunk loop)
-    const int quad = warp & 3;                     // TMEM lane quadrant this warp may read (warp id % 4)
-    const int cpar = warp >> 2;                    // 0..3
-    const int r = quad * 32 + lane;
-    const int etid = threadIdx.x;
-    const uint32_t lane_base = static_cast<uint32_t>(quad * 32) << 16;
-    if ((p.gn_in_gstat || p.gn_in_part)) {
-      // ---- fused input GroupNorm: statistics -> per-(image, channel) affine -> X tile normalised in place ----
-      // (same arithmetic and summation order as gn_apply_kernel, so the operand equals what the separate pass stored)
-      const int E = p.E, cpg = E / 32;
-      const int nimg = p.bn;                                       // images this tile touches (1 or 2)
-      float* s_mr = s_ab + 2 * E * 2;                              // [2][32][2] group (mean, rstd)
-      if (p.gn_in_gstat) {
-        if (etid < 32 * nimg) {
-          const int img = etid >> 5, g = etid & 31;
-          float2 mr = make_float2(0.f, 0.f);
-          if (n0 + img < p.Nimg) mr = ldcg_f2(p.gn_in_gstat + ((size_t)(n0 + img) * 32 + g) * 2);
-          s_mr[(img * 32 + g) * 2] = mr.x; s_mr[(img * 32 + g) * 2 + 1] = mr.y;
-        }
-      } else {
-        // combine the producers' pairs: same arithmetic and order as gn_apply_kernel (the operand must equal what the
-        // separate pass would have stored)
-        float* s_ch = s_b1;                                        // scratch [2][E][2] (bias1 is loaded afterwards)
-        const float ns = (float)(p.Hout * p.Wout) / (float)p.gn_in_slots;
-        for (int idx = etid; idx < nimg * E; idx += 32 * kMlpEpiWarps) {
-          const int img = idx / E, c = idx - img * E;
-          float2 mq = make_float2(0.f, 0.f);
-          if (n0 + img < p.Nimg)
-            mq = gn_channel_from_pairs(p.gn_in_part + (size_t)(n0 + img) * p.gn_in_slots * E * 2 + (size_t)c * 2, p.gn_in_slots, E, ns);
-          s_ch[(img * E + c) * 2] = mq.x; s_ch[(img * E + c) * 2 + 1] = mq.y;
-        }
-        named_bar_sync(1, 32 * kMlpEpiWarps);
-        if (etid < 32 * nimg) {
-          const int img = etid >> 5, g = etid & 31;
-          float chp[2 * 8];                                        // cpg <= 8 (E <= 256)
-          for (int j = 0; j < cpg; ++j) { chp[2 * j] = s_ch[(img * E + g * cpg + j) * 2]; chp[2 * j + 1] = s_ch[(img * E + g * cpg + j) * 2 + 1]; }
-          const float2 mr = gn_group_from_channels(chp, cpg, (float)(p.Hout * p.Wout), p.gn_in_eps);
-          s_mr[(img * 32 + g) * 2] = mr.x; s_mr[(img * 32 + g) * 2 + 1] = mr.y;
-        }
-      }
-      named_bar_sync(1, 32 * kMlpEpiWarps);
-      for (int idx = etid; idx < nimg * E; idx += 32 * kMlpEpiWarps) {
-        const int img = idx / E, c = idx - img * E, g = c / cpg;
-        const float a = s_mr[(img * 32 + g) * 2 + 1] * __ldg(p.gn_in_gamma + c);
-        const float b = __ldg(p.gn_in_beta + c) - s_mr[(img * 32 + g) * 2] * a;
-        s_ab[(img * E + c) * 2] = a; s_ab[(img * E + c) * 2 + 1] = b;
-      }
-      named_bar_sync(1, 32 * kMlpEpiWarps);
-      mbar_wait(x_full, 0);                                         // this CTA's X tile has landed
-      // in place: 128 rows x kx x eight 16-byte units (8 channels each); unit u of row rr sits at (u ^ (rr & 7))
-      const int rows_per_img = p.bw * p.bh;                         // bn == 2: rows 0..63 -> image n0, 64..127 -> n0 + 1
-      for (int idx = etid; idx < kx * kConvBM * 8; idx += 32 * kMlpEpiWarps) {
-        const int kb = idx / (kConvBM * 8), rem = idx - kb * (kConvBM * 8);
-        const int rr = rem >> 3, us = rem & 7;
-        const int ch = kb * 64 + ((us ^ (rr & 7)) << 3);
-        const float* ab = s_ab + ((size_t)(nimg == 2 && rr >= rows_per_img ? E : 0) + ch) * 2;
-        uint4* ptr = reinterpret_cast<uint4*>(sX + (size_t)kb * kTile + rr * 128 + us * 16);
-        uint4 raw = *ptr;
-        __half2* hh = reinterpret_cast<__half2*>(&raw);
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          float2 f = __half22float2(hh[j]);
-          f.x = fmaf(f.x, ab[(2 * j) * 2], ab[(2 * j) * 2 + 1]);
-          f.y = fmaf(f.y, ab[(2 * j + 1) * 2], ab[(2 * j + 1) * 2 + 1]);
-          hh[j] = __floats2half2_rn(f.x, f.y);
-        }
-        *ptr = raw;
-      }
-      fence_proxy_async_smem();                                     // the tensor core reads X through the async proxy
-      __syncwarp();
-      if (lane == 0) mbar_arrive_remote(mapa_u32(smem_u32(x_ready), lead));
-      named_bar_sync(1, 32 * kMlpEpiWarps);                         // the scratch aliasing the bias area is free again
-    }
-    for (int i = etid; i < p.Hd; i += 32 * kMlpEpiWarps) s_b1[i] = __ldg(p.bias1 + i);
-    for (int i = etid; i < p.E; i += 32 * kMlpEpiWarps) s_b2[i] = __ldg(p.bias2 + i);
-    named_bar_sync(1, 32 * kMlpEpiWarps);
-    const int c16 = cpar * 16;
-    const int u0 = c16 >> 3;                       // 16-byte unit of this warp's first 8 columns inside a 128-byte row
-    const uint32_t lead_acc1_empty = mapa_u32(smem_u32(acc1_empty), lead);
-    const uint32_t lead_h_full = mapa_u32(smem_u32(h_full), lead);
+    int stage = 0; uint32_t phase = 0;
+    auto next = [&]() { if (++stage == p.ring) { stage = 0; phase ^= 1; } };
     for (int j = 0; j < chunks; ++j) {
-      const int b = j & 1;
-      mbar_wait(&acc1_full[b], (j >> 1) & 1);
-      if (dbg && etid == 0) dbg[j * 8 + 4] = clock64() - t_start;
-      mbar_wait(&h_empty[b], ((j >> 1) & 1) ^ 1);
-      tc_fence_after();
-      if (dbg && etid == 0) dbg[j * 8 + 5] = clock64() - t_start;
-      uint32_t v[kHT][16];
-#pragma unroll
-      for (int t = 0; t < kHT; ++t) tmem_ld16(tmem_base + lane_base + b * kMlpHc + t * kConvBK + c16, v[t]);   // all in flight
-#pragma unroll
-      for (int t = 0; t < kHT; ++t) tmem_ld_wait16(v[t]);
-#pragma unroll
-      for (int t = 0; t < kHT; ++t) {
-        const float4* bp = reinterpret_cast<const float4*>(s_b1 + (jc0 + j) * kMlpHc + t * kConvBK + c16);
-        uint32_t q[8];
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          const float4 b4 = bp[i];
-          // (scalar FFMA: the packed fma.rn.f32x2 form issues at half rate — scripts/ubench/gelu_rate.cu — and buys nothing)
-          const __half2 h0 = __floats2half2_rn(gelu_erf_f(__uint_as_float(v[t][4 * i]) + b4.x), gelu_erf_f(__uint_as_float(v[t][4 * i + 1]) + b4.y));
-          const __half2 h1 = __floats2half2_rn(gelu_erf_f(__uint_as_float(v[t][4 * i + 2]) + b4.z), gelu_erf_f(__uint_as_float(v[t][4 * i + 3]) + b4.w));
-          q[2 * i] = *reinterpret_cast<const uint32_t*>(&h0);
-          q[2 * i + 1] = *reinterpret_cast<const uint32_t*>(&h1);
+      for (int kb = 0; kb < kx; ++kb) {
+        mbar_wait(&empty_bar[stage], phase ^ 1);
+        if (el) {
+          mbar_arrive_expect_tx(&full_bar[stage], (uint32_t)kW1);
+          tma_load_2d(sRing + (size_t)stage * kSlot, &p.tmW1, &full_bar[stage], kb * kConvBK, j * kMlpHc);
         }
-        const uint32_t row = smem_u32(sH + (size_t)(b * kHT + t) * kTile + r * 128);
-        st_shared_v4(row + (((u0) ^ (r & 7)) << 4), q[0], q[1], q[2], q[3]);
-        st_shared_v4(row + (((u0 + 1) ^ (r & 7)) << 4), q[4], q[5], q[6], q[7]);
+        next();
       }
-      if (dbg && etid == 0) dbg[j * 8 + 6] = clock64() - t_start;
-      fence_proxy_async_smem();          // H_j will be read by the tensor core through the async proxy
-      tc_fence_before();                 // this warp's tcgen05.ld of acc1[b] is complete (wait::ld above)
-      __syncwarp();
-      if (lane == 0) { mbar_arrive_remote(lead_acc1_empty + b * 8); mbar_arrive_remote(lead_h_full + b * 8); }
-      if (dbg && etid == 0) dbg[j * 8 + 7] = clock64() - t_start;
+      for (int t = 0; t < kMlpHc / kConvBK; ++t) {
+        mbar_wait(&empty_bar[stage], phase ^ 1);
+        if (el) {
+          mbar_arrive_expect_tx(&full_bar[stage], (uint32_t)kW2);
+          tma_load_2d(sRing + (size_t)stage * kSlot, &p.tmW2, &full_bar[stage], j * kMlpHc + t * kConvBK, 0);
+        }
+        next();
+      }
     }
+    return;
+  }
 
-    // ---- final epilogue: acc2 + bias2 (+ residual) -> fp16 -> TMA store, GroupNorm partials ----
-    mbar_wait(acc2_full, 0);
-    tc_fence_after();
-    if (dbg && etid == 0) dbg[63 * 8 + 0] = clock64() - t_start;
-    if (p.hsplit > 1) {
-      // hidden-dimension split, step 1: this pair's partial output tile (fp32) -> own shared memory (everything the
-      // MMAs read is dead now); the cluster-wide reduction follows after the role branches
-      const int pitch = p.E * 4 + 16;
-      const uint32_t drow = smem_u32(smem) + (uint32_t)(r * pitch);
-      for (int c = cpar * 16; c < p.E; c += 64) {
-        uint32_t v[16];
-        tmem_ld16(tm_acc2 + lane_base + c, v);
-        tmem_ld_wait16(v);
-#pragma unroll
-        for (int jv = 0; jv < 4; ++jv) st_shared_v4(drow + (uint32_t)(c * 4 + jv * 16), v[4 * jv], v[4 * jv + 1], v[4 * jv + 2], v[4 * jv + 3]);
+  // ===================== consumers (8 warps, warpgroup wg owns rows 64 wg .. 64 wg + 63) =====================
+  const int wg = warp >> 2;
+  const int rA = 64 * wg + 16 * (warp & 3) + (lane >> 2), rB = rA + 8;
+  const int etid = threadIdx.x;
+  constexpr int kCons = 32 * kConvEpiWarps;
+  if (gn_in) {
+    // ---- fused input GroupNorm: statistics -> per-(image, channel) affine (same arithmetic and order as gn_apply_kernel) ----
+    const int cpg = E / 32;
+    const int nimg = p.bn;                                       // images this tile touches (1 or 2)
+    float* s_mr = s_ab + 2 * E * 2;                              // [2][32][2] group (mean, rstd)
+    if (p.gn_in_gstat) {
+      if (etid < 32 * nimg) {
+        const int img = etid >> 5, g = etid & 31;
+        float2 mr = make_float2(0.f, 0.f);
+        if (n0 + img < p.Nimg) mr = ldcg_f2(p.gn_in_gstat + ((size_t)(n0 + img) * 32 + g) * 2);
+        s_mr[(img * 32 + g) * 2] = mr.x; s_mr[(img * 32 + g) * 2 + 1] = mr.y;
       }
     } else {
-    const int lw = r % p.bw, lh = (r / p.bw) % p.bh, ln = r / (p.bw * p.bh);
-    const int nblk = p.E >> 6;
-    uint8_t* sblk = sX;                                  // X is dead: every MMA has retired
-    float* wsum = reinterpret_cast<float*>(sH);          // [4 quads][E][2]
-    if (p.has_res) {
-      if (etid == 0) {
-        mbar_arrive_expect_tx(res_bar, (uint32_t)(nblk * kTile));
-        for (int bq = 0; bq < nblk; ++bq) tma_load_4d(sblk + (size_t)bq * kTile, &p.tmRes, res_bar, bq * 64, w0, h0, n0);
+      float* s_ch = s_b1;                                        // scratch [2][E][2] (bias1 is loaded afterwards; Hd >= 4E)
+      const float ns = (float)(p.Hout * p.Wout) / (float)p.gn_in_slots;
+      for (int idx = etid; idx < nimg * E; idx += kCons) {
+        const int img = idx / E, c = idx - img * E;
+        float2 mq = make_float2(0.f, 0.f);
+        if (n0 + img < p.Nimg)
+          mq = gn_channel_from_pairs(p.gn_in_part + (size_t)(n0 + img) * p.gn_in_slots * E * 2 + (size_t)c * 2, p.gn_in_slots, E, ns);
+        s_ch[(img * E + c) * 2] = mq.x; s_ch[(img * E + c) * 2 + 1] = mq.y;
       }
-      mbar_wait(res_bar, 0);
+      named_bar_sync(1, kCons);
+      if (etid < 32 * nimg) {
+        const int img = etid >> 5, g = etid & 31;
+        float chp[2 * 8];                                        // cpg <= 8 (E <= 256)
+        for (int j = 0; j < cpg; ++j) { chp[2 * j] = s_ch[(img * E + g * cpg + j) * 2]; chp[2 * j + 1] = s_ch[(img * E + g * cpg + j) * 2 + 1]; }
+        const float2 mr = gn_group_from_channels(chp, cpg, (float)(p.Hout * p.Wout), p.gn_in_eps);
+        s_mr[(img * 32 + g) * 2] = mr.x; s_mr[(img * 32 + g) * 2 + 1] = mr.y;
+      }
     }
-    const bool want_stats = p.sink[0].part != nullptr;
-    const uint32_t trow2 = tm_acc2 + lane_base;
-    for (int c = cpar * 16; c < p.E; c += 64) {
-      uint32_t v[16];
-      tmem_ld16(trow2 + c, v);
-      tmem_ld_wait();
-      float f[16];
-      {
-        const float4* bp = reinterpret_cast<const float4*>(s_b2 + c);
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          const float4 b4 = bp[i];
-          f[4 * i] = __uint_as_float(v[4 * i]) + b4.x; f[4 * i + 1] = __uint_as_float(v[4 * i + 1]) + b4.y;
-          f[4 * i + 2] = __uint_as_float(v[4 * i + 2]) + b4.z; f[4 * i + 3] = __uint_as_float(v[4 * i + 3]) + b4.w;
-        }
-      }
-      uint8_t* brow = sblk + (size_t)(c >> 6) * kTile + r * 128;
-      const int u0 = (c & 63) >> 3;
-      uint4* a0 = reinterpret_cast<uint4*>(brow + (((u0) ^ (r & 7)) << 4));
-      uint4* a1 = reinterpret_cast<uint4*>(brow + (((u0 + 1) ^ (r & 7)) << 4));
-      if (p.has_res) {
-        const uint4 r0 = *a0, r1 = *a1;
-        const __half2* h0p = reinterpret_cast<const __half2*>(&r0);
-        const __half2* h1p = reinterpret_cast<const __half2*>(&r1);
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          const float2 x0 = __half22float2(h0p[i]);
-          const float2 x1 = __half22float2(h1p[i]);
-          f[2 * i] += x0.x; f[2 * i + 1] += x0.y;
-          f[8 + 2 * i] += x1.x; f[8 + 2 * i + 1] += x1.y;
-        }
-      }
-      uint4 o0, o1;
-      __half2* q0 = reinterpret_cast<__half2*>(&o0);
-      __half2* q1 = reinterpret_cast<__half2*>(&o1);
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        q0[i] = __floats2half2_rn(f[2 * i], f[2 * i + 1]);
-        q1[i] = __floats2half2_rn(f[8 + 2 * i], f[8 + 2 * i + 1]);
-      }
-      *a0 = o0; *a1 = o1;
-      if (want_stats) warp_chunk_stats(o0, o1, lane, wsum + ((size_t)quad * p.E + c) * 2);
+    named_bar_sync(1, kCons);
+    for (int idx = etid; idx < nimg * E; idx += kCons) {
+      const int img = idx / E, c = idx - img * E, g = c / cpg;
+      const float a = s_mr[(img * 32 + g) * 2 + 1] * __ldg(p.gn_in_gamma + c);
+      const float b = __ldg(p.gn_in_beta + c) - s_mr[(img * 32 + g) * 2] * a;
+      s_ab[(img * E + c) * 2] = a; s_ab[(img * E + c) * 2 + 1] = b;
     }
-    fence_proxy_async_smem();
-    named_bar_sync(1, 32 * kMlpEpiWarps);
+    named_bar_sync(1, kCons);                                    // the scratch aliasing the bias area is free again
+  }
+  for (int i = etid; i < p.Hd; i += kCons) s_b1[i] = __ldg(p.bias1 + i);
+  for (int i = etid; i < E; i += kCons) s_b2[i] = __ldg(p.bias2 + i);
+  mbar_wait(x_full, 0);
+  if (gn_in) {
+    // in place: 128 rows x kx x eight 16-byte units (8 channels each); unit u of row rr sits at (u ^ (rr & 7))
+    const int rows_per_img = p.bw * p.bh;                         // bn == 2: rows 0..63 -> image n0, 64..127 -> n0 + 1
+    for (int idx = etid; idx < kx * kConvBM * 8; idx += kCons) {
+      const int kb = idx / (kConvBM * 8), rem = idx - kb * (kConvBM * 8);
+      const int rr = rem >> 3, us = rem & 7;
+      const int ch = kb * 64 + ((us ^ (rr & 7)) << 3);
+      const float* ab = s_ab + ((size_t)(p.bn == 2 && rr >= rows_per_img ? E : 0) + ch) * 2;
+      uint4* ptr = reinterpret_cast<uint4*>(sX + (size_t)kb * kTile + rr * 128 + us * 16);
+      uint4 raw = *ptr;
+      __half2* hh = reinterpret_cast<__half2*>(&raw);
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        float2 f = __half22float2(hh[j]);
+        f.x = fmaf(f.x, ab[(2 * j) * 2], ab[(2 * j) * 2 + 1]);
+        f.y = fmaf(f.y, ab[(2 * j + 1) * 2], ab[(2 * j + 1) * 2 + 1]);
+        hh[j] = __floats2half2_rn(f.x, f.y);
+      }
+      *ptr = raw;
+    }
+    fence_proxy_async_smem();                                     // the tensor core reads X through the async proxy
+  }
+  named_bar_sync(1, kCons);                                       // biases (and the normalised X tile) visible
+
+  const uint32_t sX0 = smem_u32(sX), sH0 = smem_u32(sH), sR0 = smem_u32(sRing);
+  int stage = 0; uint32_t phase = 0;
+  auto release = [&](int s) { if (s >= 0 && lane == 0) mbar_arrive(&empty_bar[s]); };
+  float acc2[E / 2];
+#pragma unroll
+  for (int i = 0; i < E / 2; ++i) acc2[i] = 0.f;
+  for (int j = 0; j < chunks; ++j) {
+    // ---- GEMM 1: acc1 = X . W1_j^T ----
+    float acc1[kMlpHc / 2];
+#pragma unroll
+    for (int i = 0; i < kMlpHc / 2; ++i) acc1[i] = 0.f;
+    int prev = -1;
+    for (int kb = 0; kb < kx; ++kb) {
+      mbar_wait(&full_bar[stage], phase);
+      const uint64_t adesc = wgmma_desc_sw128(sX0 + (uint32_t)(kb * kTile + wg * (64 * 128)));
+      const uint64_t bdesc = wgmma_desc_sw128(sR0 + (uint32_t)(stage * kSlot));
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < kConvBK / 16; ++k) Wgmma<kMlpHc>::mma(acc1, adesc + 2 * k, bdesc + 2 * k);
+      wgmma_commit();
+      wgmma_wait<1>();
+      release(prev);
+      prev = stage;
+      if (++stage == p.ring) { stage = 0; phase ^= 1; }
+    }
+    wgmma_wait<0>();
+    wgmma_fence_regs(acc1);
+    release(prev);
+    // ---- H_j = GELU(acc1 + b1) -> fp16 rows of this warpgroup (GEMM 2 of chunk j - 1 has retired: H is free) ----
+    const float* b1 = s_b1 + j * kMlpHc;
+#pragma unroll
+    for (int i = 0; i < kMlpHc / 8; ++i) {
+      const int c = 8 * i + 2 * (lane & 3);
+      const float2 bb = *reinterpret_cast<const float2*>(b1 + c);
+      uint8_t* tile = sH + (size_t)(c >> 6) * kTile + 4 * (lane & 3);
+      const int u = (c & 63) >> 3;
+#pragma unroll
+      for (int hr = 0; hr < 2; ++hr) {
+        const int r = hr ? rB : rA;
+        *reinterpret_cast<__half2*>(tile + r * 128 + ((u ^ (r & 7)) << 4)) =
+            __floats2half2_rn(gelu_erf_f(acc1[4 * i + 2 * hr] + bb.x), gelu_erf_f(acc1[4 * i + 2 * hr + 1] + bb.y));
+      }
+    }
+    fence_proxy_async_smem();                                     // H_j is read by the tensor core through the async proxy
+    named_bar_sync(2 + wg, 128);                                  // the warpgroup's 64 rows of H_j are complete
+    // ---- GEMM 2: acc2 += H_j . W2_j^T ----
+    prev = -1;
+    for (int t = 0; t < kMlpHc / kConvBK; ++t) {
+      mbar_wait(&full_bar[stage], phase);
+      const uint64_t adesc = wgmma_desc_sw128(sH0 + (uint32_t)(t * kTile + wg * (64 * 128)));
+      const uint64_t bdesc = wgmma_desc_sw128(sR0 + (uint32_t)(stage * kSlot));
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < kConvBK / 16; ++k) Wgmma<E>::mma(acc2, adesc + 2 * k, bdesc + 2 * k);
+      wgmma_commit();
+      wgmma_wait<1>();
+      release(prev);
+      prev = stage;
+      if (++stage == p.ring) { stage = 0; phase ^= 1; }
+    }
+    wgmma_wait<0>();
+    wgmma_fence_regs(acc2);
+    release(prev);
+  }
+
+  // ---- epilogue: acc2 + b2 (+ residual) -> fp16 -> TMA store, GroupNorm partials ----
+  named_bar_sync(1, kCons);                                       // X and H are dead: every MMA of both warpgroups retired
+  uint8_t* sblk = sX;                                             // kx staging blocks of [128 rows x 64 columns]
+  float* wsum = reinterpret_cast<float*>(sH);                     // [4 quads][E][2]
+  if (p.has_res) {
     if (etid == 0) {
-      for (int bq = 0; bq < nblk; ++bq) tma_store_4d(&p.tmOut, sblk + (size_t)bq * kTile, bq * 64, w0, h0, n0);
-      tma_store_commit();
+      mbar_arrive_expect_tx(res_bar, (uint32_t)(kx * kTile));
+      for (int bq = 0; bq < kx; ++bq) tma_load_4d(sblk + (size_t)bq * kTile, &p.tmRes, res_bar, bq * 64, w0, h0, n0);
     }
-    if (want_stats) {
-      const int slot = th * p.tiles_w + tw;
-      if (n0 < p.Nimg)
-        write_quad_pairs(wsum, p.E, p.E, 0, p.bn, n0, p.Nimg, slot, p.gn_slots, p.sink[0], p.sink[1], etid, 32 * kMlpEpiWarps);
-      if (p.sink[0].gstat || p.sink[1].gstat) {
-        int* s_flag = reinterpret_cast<int*>(wsum + 8 * p.E);
-        const GnSink* const sk[4] = {&p.sink[0], &p.sink[0], p.sink[1].part ? &p.sink[1] : nullptr, p.sink[1].part ? &p.sink[1] : nullptr};
-        const int n1 = (p.bn == 2 && n0 + 1 < p.Nimg) ? n0 + 1 : -1;
-        const int im[4] = {n0 < p.Nimg ? n0 : -1, n0 < p.Nimg ? n1 : -1, n0 < p.Nimg ? n0 : -1, n0 < p.Nimg ? n1 : -1};
-        const unsigned int ad[4] = {(unsigned)p.E, (unsigned)p.E, (unsigned)p.E, (unsigned)p.E};
-        gn_arrive<4>(sk, im, ad, p.gn_slots, 128.0f / (float)p.bn, etid, 32 * kMlpEpiWarps, 1, s_flag);
-      }
-    }
-    if (etid == 0) tma_store_wait_read();
-    }
-    if (dbg && etid == 0) dbg[63 * 8 + 1] = clock64() - t_start;
+    mbar_wait(res_bar, 0);
   }
-
-  if (p.hsplit > 1) {
-    // ---- hidden-dimension split, step 2: sum the pairs' partial tiles through distributed shared memory ----
-    // pair `hs` finishes columns [hs * E / hsplit, (hs + 1) * E / hsplit) for its CTAs' 128 pixels each: fixed order
-    // (split 0, 1), + bias2, + residual, fp16 store, GroupNorm partials of the stored values.
-    cluster_sync_all();
-    if (warp < kMlpEpiWarps) {
-      const int etid = threadIdx.x;
-      const int S = p.hsplit, cw = p.E / S, upr = cw >> 3;
-      const int pitch = p.E * 4 + 16;
-      const int cbase = hs * cw;
-      __half* s_out = reinterpret_cast<__half*>(smem + (size_t)kConvBM * pitch);        // [128][cw] stored values
-      float* s_col = reinterpret_cast<float*>(s_out + (size_t)kConvBM * cw);            // [2 halves][cw][2]
-      const uint32_t dump0 = smem_u32(smem);
-      for (int u = etid; u < kConvBM * upr; u += 32 * kMlpEpiWarps) {
-        const int rr = u / upr, cu = u - rr * upr;
-        const int col = cbase + cu * 8;
-        float acc[8];
 #pragma unroll
-        for (int jv = 0; jv < 8; ++jv) acc[jv] = 0.f;
-        for (int sp = 0; sp < S; ++sp) {
-          const uint32_t a = mapa_u32(dump0 + (uint32_t)(rr * pitch + col * 4), (uint32_t)(sp * 2) + rank);
-          const float4 x0 = ld_shared_cluster_f4(a), x1 = ld_shared_cluster_f4(a + 16);
-          acc[0] += x0.x; acc[1] += x0.y; acc[2] += x0.z; acc[3] += x0.w;
-          acc[4] += x1.x; acc[5] += x1.y; acc[6] += x1.z; acc[7] += x1.w;
-        }
-        const int lw = rr % p.bw, lh = (rr / p.bw) % p.bh, ln = rr / (p.bw * p.bh);
-        const int w = w0 + lw, h = h0 + lh, n = n0 + ln;
-        const bool ok = (w < p.Wout) && (h < p.Hout) && (n < p.Nimg);
-        uint4 o = make_uint4(0, 0, 0, 0);
-        if (ok) {
+  for (int i = 0; i < E / 8; ++i) {
+    const int c = 8 * i + 2 * (lane & 3);
+    const float2 bb = *reinterpret_cast<const float2*>(s_b2 + c);
+    uint8_t* tile = sblk + (size_t)(c >> 6) * kTile + 4 * (lane & 3);
+    const int u = (c & 63) >> 3;
 #pragma unroll
-          for (int jv = 0; jv < 8; ++jv) acc[jv] += __ldg(p.bias2 + col + jv);
-          if (p.has_res) {
-            const uint4 rv = *reinterpret_cast<const uint4*>(p.res_ptr + n * p.res_sN + h * p.res_sH + w * p.res_sW + col);
-            const __half2* rh = reinterpret_cast<const __half2*>(&rv);
-#pragma unroll
-            for (int jv = 0; jv < 4; ++jv) { const float2 f = __half22float2(rh[jv]); acc[2 * jv] += f.x; acc[2 * jv + 1] += f.y; }
-          }
-          __half2* oh = reinterpret_cast<__half2*>(&o);
-#pragma unroll
-          for (int jv = 0; jv < 4; ++jv) oh[jv] = __floats2half2_rn(acc[2 * jv], acc[2 * jv + 1]);
-          *reinterpret_cast<uint4*>(p.out_ptr + n * p.out_sN + h * p.out_sH + w * p.out_sW + col) = o;
-        }
-        *reinterpret_cast<uint4*>(s_out + (size_t)rr * cw + cu * 8) = o;                  // zeros outside the tensor
-      }
-      if (p.sink[0].part != nullptr) {
-        named_bar_sync(1, 32 * kMlpEpiWarps);
-        for (int t = etid; t < 2 * cw; t += 32 * kMlpEpiWarps) {
-          const int half = t / cw, c = t - half * cw;
-          const __half* colp = s_out + (size_t)(half * 64) * cw + c;
-          const float pv = __half2float(colp[0]);
-          float s1 = 0.f, s2 = 0.f;
-          for (int rr = 1; rr < 64; ++rr) {
-            const float d = __half2float(colp[(size_t)rr * cw]) - pv;
-            s1 += d; s2 = fmaf(d, d, s2);
-          }
-          s_col[(half * cw + c) * 2] = pv + s1 * (1.0f / 64.0f);
-          s_col[(half * cw + c) * 2 + 1] = fmaxf(s2 - s1 * s1 * (1.0f / 64.0f), 0.f);
-        }
-        named_bar_sync(1, 32 * kMlpEpiWarps);
-        const int slot = th * p.tiles_w + tw;
-        if (n0 < p.Nimg)
-          write_tile_pairs(s_col, cw, cw, cbase, p.bn, n0, p.Nimg, slot, p.gn_slots, p.sink[0], p.sink[1], etid, 32 * kMlpEpiWarps);
-        if (p.sink[0].gstat || p.sink[1].gstat) {
-          int* s_flag = reinterpret_cast<int*>(s_col + 4 * cw);
-          const GnSink* const sk[4] = {&p.sink[0], &p.sink[0], p.sink[1].part ? &p.sink[1] : nullptr, p.sink[1].part ? &p.sink[1] : nullptr};
-          const int n1 = (p.bn == 2 && n0 + 1 < p.Nimg) ? n0 + 1 : -1;
-          const int im[4] = {n0 < p.Nimg ? n0 : -1, n0 < p.Nimg ? n1 : -1, n0 < p.Nimg ? n0 : -1, n0 < p.Nimg ? n1 : -1};
-          const unsigned int ad[4] = {(unsigned)cw, (unsigned)cw, (unsigned)cw, (unsigned)cw};
-          gn_arrive<4>(sk, im, ad, p.gn_slots, 128.0f / (float)p.bn, etid, 32 * kMlpEpiWarps, 1, s_flag);
-        }
-      }
+    for (int hr = 0; hr < 2; ++hr) {
+      const int r = hr ? rB : rA;
+      __half2* dst = reinterpret_cast<__half2*>(tile + r * 128 + ((u ^ (r & 7)) << 4));
+      float f0 = acc2[4 * i + 2 * hr] + bb.x, f1 = acc2[4 * i + 2 * hr + 1] + bb.y;
+      if (p.has_res) { const float2 x = __half22float2(*dst); f0 += x.x; f1 += x.y; }
+      *dst = __floats2half2_rn(f0, f1);
     }
   }
-
-  tc_fence_before();
-  cluster_sync_all();                              // neither CTA retires while the other can still touch its smem / barriers / TMEM
-  if (warp == kMlpMmaWarp) { tc_fence_after(); tmem_dealloc_dyn_cg2(tmem_base, 512u); }
+  named_bar_sync(1, kCons);                                       // the staged tile is complete
+  const bool want_stats = p.sink[0].part != nullptr;
+  if (want_stats) {
+    // statistics of the values as stored: warp (quad, column parity) reads back 32 rows x 16 columns (gn_stats.cuh)
+    const int quad = warp & 3, cpar = warp >> 2;
+    const int r = quad * 32 + lane;
+    for (int c = cpar * 16; c < E; c += 32) {
+      const uint8_t* brow = sblk + (size_t)(c >> 6) * kTile + r * 128;
+      const int u0 = (c & 63) >> 3;
+      const uint4 o0 = *reinterpret_cast<const uint4*>(brow + (((u0) ^ (r & 7)) << 4));
+      const uint4 o1 = *reinterpret_cast<const uint4*>(brow + (((u0 + 1) ^ (r & 7)) << 4));
+      warp_chunk_stats(o0, o1, lane, wsum + ((size_t)quad * E + c) * 2);
+    }
+  }
+  fence_proxy_async_smem();
+  named_bar_sync(1, kCons);
+  if (etid == 0) {
+    for (int bq = 0; bq < kx; ++bq) tma_store_4d(&p.tmOut, sblk + (size_t)bq * kTile, bq * 64, w0, h0, n0);
+    tma_store_commit();
+  }
+  if (want_stats) {
+    const int slot = th * p.tiles_w + tw;
+    if (n0 < p.Nimg)
+      write_quad_pairs(wsum, E, E, 0, p.bn, n0, p.Nimg, slot, p.gn_slots, p.sink[0], p.sink[1], etid, kCons);
+    if (p.sink[0].gstat || p.sink[1].gstat) {
+      int* s_flag = reinterpret_cast<int*>(wsum + 8 * E);
+      const GnSink* const sk[4] = {&p.sink[0], &p.sink[0], p.sink[1].part ? &p.sink[1] : nullptr, p.sink[1].part ? &p.sink[1] : nullptr};
+      const int n1 = (p.bn == 2 && n0 + 1 < p.Nimg) ? n0 + 1 : -1;
+      const int im[4] = {n0 < p.Nimg ? n0 : -1, n0 < p.Nimg ? n1 : -1, n0 < p.Nimg ? n0 : -1, n0 < p.Nimg ? n1 : -1};
+      const unsigned int ad[4] = {(unsigned)E, (unsigned)E, (unsigned)E, (unsigned)E};
+      gn_arrive<4>(sk, im, ad, p.gn_slots, 128.0f / (float)p.bn, etid, kCons, 1, s_flag);
+    }
+  }
+  if (etid == 0) tma_store_wait_read();
 }
 
 #endif

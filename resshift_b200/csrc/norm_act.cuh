@@ -122,9 +122,9 @@ __global__ void __launch_bounds__(256) gn_stats_kernel(const __grid_constant__ G
 
 // Group statistics from the producers' pairs as a small kernel of its own: one CTA per (group, image), the K = slots * cpg
 // items of the group strided over 256 threads (4 loads in flight each), common pivot = item 0, fixed reduction order.
-// For tensors with hundreds of tile slots per image (the VQ-GAN's 128x128 / 256x256 maps) this beats both alternatives
-// measured in profiles/r2_s9_*: every consumer CTA re-reading slots x C pairs, and the last producer CTA reducing them on
-// the tail of a persistent conv kernel (one CTA ends up last for all 16 images: +800 us per layer).
+// For tensors with hundreds of tile slots per image (the VQ-GAN's 128x128 / 256x256 maps) it avoids both alternatives:
+// every consumer CTA re-reading slots x C pairs, and the last producer CTA reducing them on the tail of a persistent conv
+// kernel (one CTA ends up last for every image).
 struct GnFinalizeParams {
   const float* part;        // [N][slots][C][2]
   float* gstat;             // [N][32][2] = (mean, rstd)

@@ -17,10 +17,10 @@
 //     operand rows while the last head computes, results staged in shared memory and written as full token rows;
 //   * (mean, M2) of y per (image, window, channel) for the norm2 that follows (slots = windows per image, 64 tokens each).
 //
-// 8 warps: warp w owns token rows [16w, 16w + 16) = rows [(w & 3) * 16, ...) of window (w >> 2).  mma.sync rather than
-// tcgen05: the shifted-window gather does not map onto TMA boxes (wrapped windows split into partial boxes), per-window
-// M = 64 tiles would idle half a UMMA, and the whole attention half is 25 % of the model's FLOPs — what matters here is
-// that qkv / P / O never leave the SM and that three launches disappear from the dependency chain of every Swin block.
+// 8 warps: warp w owns token rows [16w, 16w + 16) = rows [(w & 3) * 16, ...) of window (w >> 2).  mma.sync: the
+// shifted-window gather does not map onto TMA boxes (wrapped windows split into partial boxes), and the whole attention
+// half is 25 % of the model's FLOPs — what matters here is that qkv / P / O never leave the SM and that three launches
+// disappear from the dependency chain of every Swin block.
 #pragma once
 
 #include "common.cuh"

@@ -1,4 +1,4 @@
-"""Run an UNMODIFIED reference entry script (inference_resshift.py, app.py, ...) on the B200-native hot path:
+"""Run an UNMODIFIED reference entry script (inference_resshift.py, app.py, ...) on the H100-native hot path:
 
     python -m resshift_b200.launch /path/to/ResShift/inference_resshift.py -i in -o out --task realsr --scale 4
 

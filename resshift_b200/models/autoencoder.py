@@ -1,6 +1,6 @@
 """``VQModelTorch`` — same constructor, ``state_dict`` and call surface as the reference's
 ``ldm.models.autoencoder.VQModelTorch`` (reference ldm/models/autoencoder.py:12-47), the VQ-GAN first stage around the
-denoising loop (SURVEY.md §8f rank 1), executed by the sm_100a kernels of ``librs_b200.so``: the same tcgen05
+denoising loop (SURVEY.md §8f rank 1), executed by the sm_90a kernels of ``librs_b200.so``: the same wgmma
 implicit-GEMM conv / GroupNorm kernels as the denoiser, the 4096-token single-head attention as tensor-core GEMMs +
 a row softmax, nearest-codebook quantisation as one small kernel (csrc/vq.inc).
 

@@ -1,6 +1,6 @@
 """``UNetModelSwin`` — same constructor, ``state_dict`` and call surface as the reference's
 ``models.unet.UNetModelSwin`` (reference models/unet.py:603-912), with the forward pass executed by
-the sm_100a kernels of ``librs_b200.so`` through the C ABI (include/resshift_b200.h).
+the sm_90a kernels of ``librs_b200.so`` through the C ABI (include/resshift_b200.h).
 
 PyTorch owns every allocation (parameters, packed-weight arena, workspace, outputs); the library only
 enqueues kernels on the current CUDA stream.  There is no eager / CPU fallback: calling the module

@@ -1,2 +1,2 @@
-"""Overlay of the reference's top-level ``sampler`` module: same names, B200-native hot path."""
+"""Overlay of the reference's top-level ``sampler`` module: same names, H100-native hot path."""
 from resshift_b200.sampler import BaseSampler, ResShiftSampler  # noqa: F401

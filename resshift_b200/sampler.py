@@ -1,5 +1,5 @@
 """``ResShiftSampler`` — the orchestration surface of the reference's ``sampler.py`` (reference
-sampler.py:26-308) over the B200-native hot path.
+sampler.py:26-308) over the H100-native hot path.
 
 Same constructor and methods (``sample_func``, ``inference``); models are still built from the yaml
 ``target:`` strings (reference utils/util_common.py:19-29), so pointing ``model.target`` /

@@ -62,7 +62,7 @@ def _worker(rank, world, port, q):
             dist.destroy_process_group()
 
 
-@pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs two GPUs (gpurun --gpus 2)")
+@pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs two GPUs")
 def test_two_gpu_sampler_shards_equal_single_gpu_run():
     import torch.multiprocessing as mp
     ctx = mp.get_context("spawn")

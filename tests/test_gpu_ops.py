@@ -36,6 +36,7 @@ CONV_CASES = [
 ]
 
 
+# (parameter ids kept from the first GPU generation: "tcgen05_*" names the tensor-core kernel, today the wgmma one)
 @pytest.mark.parametrize("impl", ["tcgen05_cg1", "tcgen05_cg2", "tcgen05_msub2", "tcgen05_persist_cg1", "tcgen05_persist_cg2", "simt"])
 @pytest.mark.parametrize("case", CONV_CASES)
 def test_conv2d(case, impl):
@@ -45,10 +46,10 @@ def test_conv2d(case, impl):
         os.environ["RS_CONV_MSUB"] = "2"       # two 128-pixel sub-tiles per CTA (falls back to 1 for odd tile counts)
         os.environ["RS_CONV_CG"] = "1"
     elif impl.endswith("cg1"):
-        os.environ["RS_CONV_CG"] = "1"         # one CTA per 128-pixel tile (tcgen05 cta_group::1)
+        os.environ["RS_CONV_CG"] = "1"         # one CTA per 128-pixel tile
     elif impl.endswith("cg2"):
-        os.environ["RS_CONV_CG"] = "2"         # CTA pairs: 256-pixel tiles, tcgen05 cta_group::2, half of B per CTA
-    # persistent kernel (one CTA / pair per SM walking several tiles, double-buffered accumulators) forced on; off
+        os.environ["RS_CONV_CG"] = "2"         # CTA pairs: two 128-pixel tiles, each CTA loads half of B and multicasts it
+    # persistent mode (one CTA / pair per SM walking several tiles) forced on; off
     # otherwise so that both kernels are covered whatever the cost model would pick
     os.environ["RS_CONV_PERSIST"] = "1" if "persist" in impl else "0"
     try:
@@ -322,8 +323,8 @@ def test_conv2d_split_k(case, force, mode):
 @pytest.mark.parametrize("case", [(2, 16, 16, 192, 768), (1, 64, 64, 64, 256), (3, 8, 8, 192, 768), (4, 32, 32, 192, 768)])
 def test_fused_mlp(case, hsplit, monkeypatch):
     """out = residual + fc2(GELU(fc1(x))) in one kernel (hidden activations stay on chip, rounded to fp16 like the
-    unfused path rounds its stored intermediate).  hsplit = 2: the hidden dimension is split over two CTA pairs of one
-    cluster and the partial outputs are summed through distributed shared memory (few-tile layers)."""
+    unfused path rounds its stored intermediate).  RS_MLP_HSPLIT is set both ways: the kernel has no hidden-dimension
+    split, so the results must not depend on it."""
     monkeypatch.setenv("RS_MLP_HSPLIT", str(hsplit))
     N, H, W, E, Hd = case
     g = torch.Generator(device="cuda").manual_seed(sum(case))
@@ -442,19 +443,20 @@ def test_window_attention(hw, shift, impl):
     assert st["nan"] == 0 and st["max_abs"] <= 4e-3 * ref.abs().max().item() + 2e-3, st
 
 
+# impl "tc": the kernel also delivers the group statistics of y; "mma": window pairs only (ids kept from the first GPU
+# generation, where they named two kernels; both run the mma.sync fused kernel now)
 @pytest.mark.parametrize("impl", ["tc", "mma"])
 @pytest.mark.parametrize("E", [192, 64])
 @pytest.mark.parametrize("case", [(2, 16, 32, 0), (2, 16, 32, 4), (3, 8, 8, 0), (1, 64, 64, 4), (5, 16, 16, 4), (16, 64, 64, 4)])
-def test_swin_attention_half_fused(case, E, impl, monkeypatch):
+def test_swin_attention_half_fused(case, E, impl):
     """norm1 + qkv + (shifted-)window attention + proj + residual as ONE kernel against plain torch on the same fp16
     operands, with the intermediate roundings of the unfused path (fp16 n1 / qkv / attention output); also the
     (mean, M2) pairs of the result per 8x8 window.  reference: models/swin_transformer.py:246-275,114-145.
-    The last case is the benchmark shape: 512 window pairs on 148 persistent CTAs, i.e. several tiles per CTA with the
+    The last case is the benchmark shape: 512 window pairs on 132 persistent CTAs, i.e. several tiles per CTA with the
     image changing inside a CTA's range (state carried from tile to tile: norm1 affine, weight ring, barrier phases)."""
     from resshift_b200.arch import relative_position_index, shifted_window_mask
     if case[0] == 16 and E == 64:
         pytest.skip("the multi-tile case is covered at the model's width")
-    monkeypatch.setenv("RS_SWIN_IMPL", impl)       # tc: tcgen05 kernel (swin_attn_tc.cuh); mma: mma.sync kernel (swin_attn_fused.cuh)
     N, H, W, shift = case
     heads = E // 32
     g = torch.Generator(device="cuda").manual_seed(E + H * 3 + shift + N)
@@ -482,7 +484,7 @@ def test_swin_attention_half_fused(case, E, impl, monkeypatch):
     for rep in range(2):
         y = torch.full_like(x, float("nan"))
         pout = torch.full((N, nW, E, 2), float("nan"), dtype=torch.float32, device="cuda")
-        # the tcgen05 kernel also finalises the image's 32 group (mean, rstd) on the last CTA to deliver its pairs
+        # tc: the image's 32 group (mean, rstd) of y are also reduced from the window pairs
         gst = torch.full((N, 32, 2), float("nan"), dtype=torch.float32, device="cuda") if impl == "tc" else None
         cnt = torch.zeros(N, dtype=torch.int32, device="cuda") if impl == "tc" else None
         _lib.check(G.L.rs_op_swin_attn(x.data_ptr(), N, H, W, E, heads, shift, part.data_ptr(), slots, gamma.data_ptr(), beta.data_ptr(),

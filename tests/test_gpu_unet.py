@@ -80,7 +80,7 @@ def test_forward_blocks_vs_golden(golden_dir):
 
 
 def test_norm2_fused_into_mlp_is_bit_identical_to_separate_groupnorm():
-    """The fused Swin MLP kernel applying norm2 to its X tile in shared memory (default) must reproduce, bit for bit,
+    """The fused Swin MLP kernel applying norm2 to its X tile in shared memory (RS_MLP_NORM_FUSE=1) must reproduce, bit for bit,
     the plan that runs gn_apply_kernel first (RS_MLP_NORM_FUSE=0): same partial sums, same affine, same rounding."""
     outs = []
     for fuse in ("1", "0"):
@@ -100,7 +100,7 @@ def test_norm2_fused_into_mlp_is_bit_identical_to_separate_groupnorm():
 
 
 def test_fused_swin_attention_plan_matches_four_launch_plan(monkeypatch):
-    """The tcgen05 Swin attention kernel (norm1 + qkv + window attention + proj + residual in one launch) against the
+    """The fused Swin attention kernel (norm1 + qkv + window attention + proj + residual in one launch) against the
     four-launch form of the same half, at plan level and WITH workspace reuse: forced on every level
     (RS_SWIN_FUSE_MIN_PAIRS=1: 18 blocks x 3 launches fewer) vs off.  Same roundings, different summation orders: the
     outputs agree to rounding; the fused plan is bit-reproducible and right against the oracle.  Batch 3 puts several
