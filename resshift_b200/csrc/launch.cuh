@@ -260,7 +260,9 @@ inline TileConfig pick_tile_config(int m_tiles, int cout16, int num_kb, int f_bn
             const int S = kSplits[si];
             // (S = 2 only: clusters of 4 CTAs; larger clusters of CTAs with ~200 KB of shared memory each schedule poorly)
             if (mode == 1 && (S != 2 || !allow_cluster_split || cg != 2 || occ != 1 || (cand / S) % 8 != 0)) continue;
-            if (mode == 1 && f_mode && std::strcmp(f_mode, "global") == 0) continue;
+            // cluster split-K only on request (RS_CONV_SPLITK_MODE=cluster): on the H100 every 8x8 / 16x16 denoiser conv that
+            // picked it ran 1.5-2.3x slower than the best global split-K or unsplit configuration (DESIGN.md §7)
+            if (mode == 1 && !(f_mode && std::strcmp(f_mode, "cluster") == 0)) continue;
             if (mode == 0 && S > 1 && f_mode && std::strcmp(f_mode, "cluster") == 0) continue;
             if (mode == 1 && (size_t)kConvBM * (cand * 4 + 16) + (size_t)kConvBM * (cand / S) * 2 + (size_t)4 * (cand / S) * 4 + 16 > (size_t)st * sbytes) continue;
             if (S > 1 && ((mode == 0 && !allow_split) || ms != 1 || num_kb / S < 6)) continue;
