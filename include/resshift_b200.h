@@ -203,6 +203,11 @@ int rs_op_groupnorm_apply_pairs(const void* x, int N, int H, int W, int C, int l
 /* group statistics gstat[N][32][2] = (mean, rstd) from (mean, M2) pairs part[N][slots][C][2] (rows_per_slot values each)
  * as a kernel of its own — what the first-stage plans run in front of a GroupNorm whose producer has hundreds of tiles */
 int rs_op_groupnorm_finalize(const float* part, int N, int slots, int C, int rows_per_slot, float eps, float* gstat, void* stream);
+/* single-head attention over all T positions of each image, out = softmax(q k^T C^-1/2) v (reference
+ * ldm/modules/diffusionmodules/model.py:180-199, AttnBlock.forward between the q/k/v convs and proj_out; the VQ-GAN
+ * plans run it for bottlenecks with H*W > 8192).  q, k, v fp16 [N][T][C] with row stride ld; out fp16 [N][T][C] dense.
+ * C in {128, 256, 512}, T % 64 == 0; O(T*C) memory, deterministic, one launch. */
+int rs_op_vq_attention(const void* q, const void* k, const void* v, int N, int T, int C, int ld, void* out, void* stream);
 /* window attention core (reference models/swin_transformer.py:114-145,251-275); qkv [N,H,W,3*heads*32] */
 int rs_op_expand_relpos(const float* table_225xh, float* dense_hx64x64, int heads, void* stream);
 int rs_op_window_attention(const void* qkv, int N, int H, int W, int heads, int shift, const float* bias_dense,

@@ -257,7 +257,7 @@ int build_inventory(rs_engine& e) {
 // ------------------------------------------------------------------------------------------------
 namespace {
 
-enum OpKind { OP_CONV, OP_GN, OP_ATTN, OP_UPSAMPLE, OP_MLP, OP_SOFTMAX, OP_FORK, OP_JOIN, OP_SWIN_ATTN };
+enum OpKind { OP_CONV, OP_GN, OP_ATTN, OP_UPSAMPLE, OP_MLP, OP_SOFTMAX, OP_FORK, OP_JOIN, OP_SWIN_ATTN, OP_VQ_ATTN };
 
 struct Tensor {
   size_t bytes = 0;
@@ -284,6 +284,8 @@ struct Op {
   MlpDesc mlp;
   // fused attention half of a Swin block (norm1 + qkv + window attention + proj + residual)
   SwinAttnDesc swin;
+  // fused attention over all positions of an image (VQ-GAN bottleneck with H*W > 8192, vq.inc)
+  VqAttnDesc vqa;
   std::string blk_name;
   std::string w2_name, b2_name;
   std::string w_name, b_name, g_name;   // parameter names resolved at bind
@@ -959,6 +961,11 @@ int bind_ops(rs_plan& P, std::vector<Op>& ops) {
       resolve(P, op.s_view);
       RS_CHECK(op.s_view.C % 8 == 0 && op.s_view.C <= 8192 && op.s_view.ld % 8 == 0, "softmax row length");
       ++P.launches;
+    } else if (op.kind == OP_VQ_ATTN) {
+      VqAttnDesc& a = op.vqa;
+      resolve(P, a.q); resolve(P, a.k); resolve(P, a.v); resolve(P, a.out);
+      int rc = vq_attn_finalize(a); if (rc) return rc;
+      ++P.launches;
     } else {
       resolve(P, op.u_in); resolve(P, op.u_out);
       ++P.launches;
@@ -978,8 +985,8 @@ struct Prof {
   ~Prof() { for (cudaEvent_t e : ev) cudaEventDestroy(e); }
 };
 
-// RS_SKIP_KINDS (timing ablation only — results are garbage): bit 0 conv3x3, 1 conv1x1 / linear, 2 GroupNorm, 3 window
-// attention, 4 upsample, 5 fused MLP.  The time a kernel family really costs inside the graph-replayed step is the
+// RS_SKIP_KINDS (timing ablation only — results are garbage): bit 0 conv3x3, 1 conv1x1 / linear, 2 GroupNorm, 3 attention
+// (window, fused Swin, fused VQ-GAN), 4 upsample, 5 fused MLP.  The time a kernel family really costs inside the graph-replayed step is the
 // difference between the full step and the step without it (per-launch events over-state small kernels).
 inline bool op_skipped(const Op& op) {
   static const int skip = env_int("RS_SKIP_KINDS", 0);
@@ -991,6 +998,7 @@ inline bool op_skipped(const Op& op) {
     case OP_UPSAMPLE: return (skip >> 4) & 1;
     case OP_MLP: return (skip >> 5) & 1;
     case OP_SWIN_ATTN: return (skip >> 3) & 1;
+    case OP_VQ_ATTN: return (skip >> 3) & 1;
     case OP_SOFTMAX: case OP_FORK: case OP_JOIN: return false;
   }
   return false;
@@ -1029,6 +1037,7 @@ int run_ops(rs_plan& P, const std::vector<Op>& ops, const float* film_base, long
       }
       case OP_MLP: rc = mlp_launch(op.mlp, st); break;
       case OP_SWIN_ATTN: rc = swin_attn_launch(op.swin, st); break;
+      case OP_VQ_ATTN: rc = vq_attn_launch(op.vqa, st); break;
       case OP_ATTN:
         rc = attn_launch(op.a_in, op.a_out, op.a_bias, P.e->cfg.swin_heads, P.e->cfg.swin_embed_dim, op.a_shift, st);
         break;
@@ -1306,6 +1315,8 @@ static void collect_profile(const rs_plan& P, const Prof& prof, double* ms, char
       snprintf(d, desc_stride, "%s", op.kind == OP_FORK ? "fork" : "join");
     } else if (op.kind == OP_SOFTMAX) {
       snprintf(d, desc_stride, "softmax %d", op.s_view.C);
+    } else if (op.kind == OP_VQ_ATTN) {
+      snprintf(d, desc_stride, "vq_attn T=%d C=%d N=%d", op.vqa.prm.T, op.vqa.q.C, op.vqa.q.N);
     } else {
       snprintf(d, desc_stride, "upsample %dx%d C=%d", op.u_in.H, op.u_in.W, op.u_in.C);
     }

@@ -15,6 +15,7 @@
 #include "norm_act.cuh"
 #include "window_attn.cuh"
 #include "swin_attn_fused.cuh"
+#include "vq_attn.cuh"
 
 namespace rs {
 
@@ -505,6 +506,9 @@ inline int conv_init() {   // once per process, outside any stream capture
     RS_CUDA_OK(cudaFuncSetAttribute(mlp_fused_sm90_kernel<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     RS_CUDA_OK(cudaFuncSetAttribute(swin_attn_fused_kernel<192>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SwinSmem<192>::total));
     RS_CUDA_OK(cudaFuncSetAttribute(swin_attn_fused_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SwinSmem<64>::total));
+    RS_CUDA_OK(cudaFuncSetAttribute(vq_attn_sm90_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, VqAttnSmem<128>::launch_bytes));
+    RS_CUDA_OK(cudaFuncSetAttribute(vq_attn_sm90_kernel<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, VqAttnSmem<256>::launch_bytes));
+    RS_CUDA_OK(cudaFuncSetAttribute(vq_attn_sm90_kernel<512>, cudaFuncAttributeMaxDynamicSharedMemorySize, VqAttnSmem<512>::launch_bytes));
     attr_set = true;
   }
   return 0;
@@ -759,6 +763,47 @@ inline int swin_attn_launch(const SwinAttnDesc& d, cudaStream_t st) {
       (void)launch_k(gn_finalize_kernel, dim3(32, d.x.N), dim3(256), (size_t)0, st, d.fin[k]);
       RS_CUDA_OK(cudaGetLastError());
     }
+  return 0;
+}
+
+// ---- fused VQ-GAN attention over all positions of an image (vq_attn.cuh) -----------------
+struct VqAttnDesc {
+  View q, k, v, out;                       // [N, H, W, C]; T = H * W positions per image
+  VqAttnParams prm;
+};
+inline int vq_attn_finalize(VqAttnDesc& d) {
+  VqAttnParams& p = d.prm;
+  std::memset(&p, 0, sizeof(p));
+  const int N = d.q.N, C = d.q.C;
+  const long long T = (long long)d.q.H * d.q.W;
+  RS_CHECK(C == 128 || C == 256 || C == 512, "fused VQ-GAN attention: C in {128, 256, 512}, got " + std::to_string(C));
+  RS_CHECK(T > 0 && T % kVqAttnBM == 0 && T <= (1LL << 30), "fused VQ-GAN attention: T = H * W must be a positive multiple of 64, got " + std::to_string(T));
+  RS_CHECK(N >= 1 && N <= 65535, "fused VQ-GAN attention: batch in [1, 65535]");
+  const View* vs[4] = {&d.q, &d.k, &d.v, &d.out};
+  for (const View* v : vs) {
+    RS_CHECK(v->N == N && (long long)v->H * v->W == T && v->C == C, "fused VQ-GAN attention: q, k, v, out must all be [N, T, C]");
+    RS_CHECK(v->ptr != nullptr && v->ld >= C && v->ld % 8 == 0, "fused VQ-GAN attention: rows of >= C elements, 16-byte aligned");
+  }
+  p.T = (int)T;
+  p.scale_log2 = (float)(1.4426950408889634 / std::sqrt((double)C));
+  CUtensorMap* maps[4] = {&p.tmQ, &p.tmK, &p.tmV, &p.tmO};
+  const int rows[4] = {kVqAttnBM, vq_attn_bk(C), vq_attn_bk(C), kVqAttnBM};
+  for (int i = 0; i < 4; ++i) {
+    const View& v = *vs[i];
+    int rc = encode_act_map(maps[i], v.ptr, C, (int)T, 1, N, v.ld, T * v.ld, v.sN(), rows[i], 1, 1, 64);
+    if (rc) return rc;
+  }
+  return 0;
+}
+inline int vq_attn_launch(const VqAttnDesc& d, cudaStream_t st) {
+  const dim3 grid((unsigned)(d.prm.T / kVqAttnBM), (unsigned)d.q.N);
+  switch (d.q.C) {
+    case 128: (void)launch_k(vq_attn_sm90_kernel<128>, grid, dim3(kVqAttnThreads), (size_t)VqAttnSmem<128>::launch_bytes, st, d.prm); break;
+    case 256: (void)launch_k(vq_attn_sm90_kernel<256>, grid, dim3(kVqAttnThreads), (size_t)VqAttnSmem<256>::launch_bytes, st, d.prm); break;
+    case 512: (void)launch_k(vq_attn_sm90_kernel<512>, grid, dim3(kVqAttnThreads), (size_t)VqAttnSmem<512>::launch_bytes, st, d.prm); break;
+    default: RS_CHECK(false, "fused VQ-GAN attention: C in {128, 256, 512}");
+  }
+  RS_CUDA_OK(cudaGetLastError());
   return 0;
 }
 

@@ -1,8 +1,9 @@
 """``VQModelTorch`` — same constructor, ``state_dict`` and call surface as the reference's
 ``ldm.models.autoencoder.VQModelTorch`` (reference ldm/models/autoencoder.py:12-47), the VQ-GAN first stage around the
 denoising loop (SURVEY.md §8f rank 1), executed by the sm_90a kernels of ``librs_b200.so``: the same wgmma
-implicit-GEMM conv / GroupNorm kernels as the denoiser, the 4096-token single-head attention as tensor-core GEMMs +
-a row softmax, nearest-codebook quantisation as one small kernel (csrc/vq.inc).
+implicit-GEMM conv / GroupNorm kernels as the denoiser, the bottleneck's single-head attention as tensor-core GEMMs + a
+row softmax up to 8192 positions and as one fused online-softmax kernel above (any image whose size is a multiple of
+8 * 2^(levels-1)), nearest-codebook quantisation as one small kernel (csrc/vq.inc, csrc/vq_attn.cuh).
 
 ``encode(x)`` / ``decode(h, force_not_quantize=False)`` / ``forward`` take and return fp32 NCHW CUDA tensors.  PyTorch
 owns every allocation; there is no eager / CPU fallback.
