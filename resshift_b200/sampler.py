@@ -8,6 +8,7 @@ PYTHONPATH, see INTEGRATION.md) is all that changes.  The VQ-GAN autoencoder is 
 (a PyTorch module; bookends stay in PyTorch).  Multi-GPU follows the reference: one process per GPU,
 contiguous batch slices per rank (sampler.py:273-277), same seed on every rank; on top of that rank 0 can
 broadcast the weights over NCCL (``broadcast_weights``) and results can be gathered (``gather_results``).
+``shard_tiles=True`` deals the tiles of each chunk across the ranks instead, bit-identical to one GPU (DESIGN.md §6).
 """
 from __future__ import annotations
 
@@ -24,6 +25,8 @@ import numpy as np
 import torch
 import torch.distributed as dist
 import torch.nn.functional as F
+
+from .parallel import gather_counts, shard_range
 
 
 # --------------------------------------------------------------------------------------------------
@@ -234,6 +237,17 @@ class BaseSampler:
 
 
 class ResShiftSampler(BaseSampler):
+    def __init__(self, configs, sf=4, use_amp=True, chop_size=128, chop_stride=128, chop_bs=1, padding_offset=16,
+                 seed=10000, shard_tiles=None):
+        """``shard_tiles``: deal the tiles of each chunk of images across the ranks instead of slicing the chunk by
+        image (``_run_shard``); ``None`` reads ``RS_SHARD_TILES`` (default 0), so unmodified reference scripts can turn
+        it on."""
+        if shard_tiles is None:
+            shard_tiles = os.environ.get("RS_SHARD_TILES", "0") not in ("", "0")
+        self.shard_tiles = bool(shard_tiles)
+        super().__init__(configs, sf=sf, use_amp=use_amp, chop_size=chop_size, chop_stride=chop_stride, chop_bs=chop_bs,
+                         padding_offset=padding_offset, seed=seed)
+
     def sample_func(self, y0, noise_repeat=False, mask=False):
         """y0: [n, c, h, w] in [-1, 1] -> [n, c, h*sf, w*sf] in [-1, 1] (reference sampler.py:119-165)."""
         if noise_repeat:
@@ -265,14 +279,12 @@ class ResShiftSampler(BaseSampler):
         are stacked on the batch axis per call exactly like ImageSpliterTh.__next__ (:940-960, `extra_bs`) — so the
         noise drawn per call matches the reference's — and overlaps are averaged (update / gather :962-979) by
         rs_op_tile_gather in the reference's accumulation order."""
-        from . import _lib
         ctx = torch.autocast("cuda") if self.use_amp else nullcontext()
         b, c, h, w = im_lq.shape
         if not (h > self.chop_size or w > self.chop_size):
             with ctx:
                 return self.sample_func(im_lq, noise_repeat=noise_repeat, mask=mask).float()
-        sf = self.sf
-        hs_list, ws_list, th, tw, groups = plan_tiles(h, w, self.chop_size, self.chop_stride, self.chop_bs)
+        _, _, th, tw, groups = plan_tiles(h, w, self.chop_size, self.chop_stride, self.chop_bs)
         tiles = []
         for group in groups:
             pch = torch.cat([im_lq[:, :, hs:hs + th, ws:ws + tw] for hs, ws in group], dim=0)
@@ -280,14 +292,132 @@ class ResShiftSampler(BaseSampler):
             with ctx:
                 res = self.sample_func(pch, noise_repeat=noise_repeat, mask=mch).float()
             tiles.extend(torch.split(res, b, dim=0))
-        tiles_t = torch.stack(tiles).contiguous()                                   # [T, b, c, th*sf, tw*sf]
-        out = torch.empty(b, tiles_t.shape[2], h * sf, w * sf, dtype=torch.float32, device=im_lq.device)
-        ys = torch.tensor([v * sf for v in hs_list], dtype=torch.int32, device=im_lq.device)
-        xs = torch.tensor([v * sf for v in ws_list], dtype=torch.int32, device=im_lq.device)
+        return self._overlap_average(torch.stack(tiles), h, w)
+
+    def _overlap_average(self, tiles, h, w):
+        """tiles [T, b, c, th*sf, tw*sf] of an [b, c, h, w] input, in plan_tiles order -> [b, c, h*sf, w*sf]: overlaps
+        averaged by rs_op_tile_gather in the reference's accumulation order."""
+        from . import _lib
+        sf = self.sf
+        hs_list, ws_list, th, tw, _ = plan_tiles(h, w, self.chop_size, self.chop_stride, self.chop_bs)
+        tiles_t = tiles.contiguous()
+        b = tiles_t.shape[1]
+        out = torch.empty(b, tiles_t.shape[2], h * sf, w * sf, dtype=torch.float32, device=tiles_t.device)
+        ys = torch.tensor([v * sf for v in hs_list], dtype=torch.int32, device=tiles_t.device)
+        xs = torch.tensor([v * sf for v in ws_list], dtype=torch.int32, device=tiles_t.device)
         _lib.check(_lib.lib.rs_op_tile_gather(tiles_t.data_ptr(), b, tiles_t.shape[2], h * sf, w * sf, th * sf, tw * sf,
                                               len(hs_list), len(ws_list), ys.data_ptr(), xs.data_ptr(), out.data_ptr(),
                                               _lib.current_stream()))
         return out
+
+    # -- tile sharding: the sample_func calls of a chunk dealt across ranks, bit-identical to one GPU ----------------
+    def _plan_units(self, shapes):
+        """Work units of a chunk whose shape groups have LQ sizes ``shapes`` [(h, w)], in the order a one-GPU run makes
+        its sample_func calls: (group, tile starts, tile h, tile w).  An image that fits in one tile is one unit with
+        the single start (0, 0)."""
+        units = []
+        for g, (h, w) in enumerate(shapes):
+            if h > self.chop_size or w > self.chop_size:
+                _, _, th, tw, groups = plan_tiles(h, w, self.chop_size, self.chop_stride, self.chop_bs)
+                units += [(g, starts, th, tw) for starts in groups]
+            else:
+                units.append((g, [(0, 0)], h, w))
+        return units
+
+    def _share_counts(self, shapes, world):
+        """counts[g][r]: tiles of shape group g that rank r runs (what parallel.gather_counts needs on every rank)."""
+        units = self._plan_units(shapes)
+        counts = [[0] * world for _ in shapes]
+        for r in range(world):
+            a, e = shard_range(len(units), world, r)
+            for g, starts, _, _ in units[a:e]:
+                counts[g][r] += len(starts)
+        return counts
+
+    def _latent_spec(self, n, h, w, dtype):
+        """Shape and dtype of z_y = encode_first_stage(y, up_sample=True) for an [n, 3, h, w] input (after the
+        padding_offset reflect-pad) of dtype ``dtype``, derived from the configs without running the encoder: the VQ
+        first stage keeps the data dtype (encode_first_stage) and downsamples by 2^(len(ch_mult) - 1)."""
+        sf = self.base_diffusion.sf
+        ae = self.configs.autoencoder.params
+        f = 2 ** (len(ae.ddconfig.ch_mult) - 1)
+        return (n, int(ae.embed_dim), int(h * sf) // f, int(w * sf) // f), dtype
+
+    def _check_shardable(self):
+        if not self.base_diffusion._native_ok(self.model, clip_denoised=(self.autoencoder is None), denoised_fn=None,
+                                              model_kwargs={"lq": None}):
+            raise RuntimeError(
+                "shard_tiles needs the fused sampling loop, whose noise can be drawn ahead of the encoder; this "
+                "configuration takes the generic per-step route (no autoencoder, a model other than this package's "
+                "UNetModelSwin, predict_type other than xstart, or T outside 2..64)")
+
+    def _sample_unit(self, y0, mask, noises, spec):
+        """sample_func with its noise given: reflect-pad, encode_first_stage(up_sample=True), sample_latent(noises=),
+        decode_first_stage, crop, clamp — the same steps, in the same order.  ``spec`` is the z_y shape and dtype the
+        noise was drawn for; it must be the real one."""
+        offset = self.padding_offset
+        ori_h, ori_w = y0.shape[2:]
+        flag_pad = not (ori_h % offset == 0 and ori_w % offset == 0)
+        if flag_pad:
+            pad_h = math.ceil(ori_h / offset) * offset - ori_h
+            pad_w = math.ceil(ori_w / offset) * offset - ori_w
+            y0 = F.pad(y0, pad=(0, pad_w, 0, pad_h), mode="reflect")
+            if mask is not None:
+                mask = F.pad(mask, pad=(0, pad_w, 0, pad_h), mode="reflect")
+        model_kwargs = {"lq": y0} if mask is None else {"lq": y0, "mask": mask}
+        diff = self.base_diffusion
+        z_y = diff.encode_first_stage(y0, self.autoencoder, up_sample=True)
+        assert (tuple(z_y.shape), z_y.dtype, z_y.is_contiguous()) == (spec[0], spec[1], True), \
+            f"derived z_y {spec} != real {tuple(z_y.shape)} {z_y.dtype}"
+        final = diff.sample_latent(z_y, self.model, model_kwargs, noises=noises)
+        with torch.no_grad():
+            results = diff.decode_first_stage(final, first_stage_model=self.autoencoder)
+        if flag_pad:
+            results = results[:, :, :ori_h * self.sf, :ori_w * self.sf]
+        return results.clamp_(-1.0, 1.0)
+
+    def _run_shard(self, lqs, masks, noise_repeat, world, rank):
+        """One rank's share of a chunk.  ``lqs`` / ``masks``: per shape group, [b, 3, h, w] in [-1, 1] and
+        [b, 1, h, w] or None.  The units of _plan_units are dealt as contiguous ranges (parallel.shard_range); every
+        rank walks all of them and draws each unit's T+1 noise tensors as GaussianDiffusion.draw_noises does (after
+        setup_seed with noise_repeat, as sample_func does), so the CUDA generator is where a one-GPU run has it, and runs
+        only its own units.  Nothing else in the chain draws random numbers.  Returns, per group, this rank's tiles
+        [n, b, 3, th*sf, tw*sf] in plan order (n may be 0)."""
+        self._check_shardable()
+        if any(lq is None for lq in lqs):
+            raise ValueError("shard_tiles needs the LQ image of every group")
+        units = self._plan_units([tuple(lq.shape[2:]) for lq in lqs])
+        a, e = shard_range(len(units), world, rank)
+        out = [[] for _ in lqs]
+        offset = self.padding_offset
+        ctx = torch.autocast("cuda") if self.use_amp else nullcontext()
+        for i, (g, starts, th, tw) in enumerate(units):
+            lq, mask = lqs[g], masks[g]
+            b = lq.shape[0]
+            with ctx:
+                if noise_repeat:
+                    self.setup_seed()
+                spec = self._latent_spec(b * len(starts), math.ceil(th / offset) * offset, math.ceil(tw / offset) * offset,
+                                         lq.dtype)
+                noises = self.base_diffusion.draw_noises(torch.empty(spec[0], dtype=spec[1], device=lq.device),
+                                                         noise_repeat=noise_repeat)
+                if not a <= i < e:
+                    continue
+                pch = torch.cat([lq[:, :, hs:hs + th, ws:ws + tw] for hs, ws in starts], dim=0)
+                mch = None if mask is None else torch.cat([mask[:, :, hs:hs + th, ws:ws + tw] for hs, ws in starts], dim=0)
+                res = self._sample_unit(pch, mch, noises, spec).float()
+            out[g].extend(torch.split(res, b, dim=0))
+        tile_hw = {g: (th, tw) for g, _, th, tw in units}
+        return [torch.stack(t) if t else
+                torch.empty((0,) + tuple(lq.shape[:2]) + (tile_hw[g][0] * self.sf, tile_hw[g][1] * self.sf), device=lq.device)
+                for g, (t, lq) in enumerate(zip(out, lqs))]
+
+    def _assemble(self, tiles, h, w):
+        """All tiles of one shape group [T, b, c, th*sf, tw*sf], in plan order -> [b, c, h*sf, w*sf]: what
+        _sample_tiled returns for that group."""
+        if not (h > self.chop_size or w > self.chop_size):
+            return tiles[0]
+        return self._overlap_average(tiles, h, w)
 
     def _process(self, im_lq, mask=None, noise_repeat=False, mask_back=True):
         """[b, c, h, w] in [-1, 1] -> [b, c, h*sf, w*sf] in [0, 1] (reference sampler.py:176-223)."""
@@ -303,6 +433,12 @@ class ResShiftSampler(BaseSampler):
         -> uint8 [b, h*sf, w*sf, 3] in BGR (what cv2.imwrite takes) or RGB order.  Ingest = (v / 255 - 0.5) / 0.5
         (reference datapipe default transform); emit = clamp, * 0.5 + 0.5, mask-back blend, round(v * 255)
         (sampler.py:218-223 + utils/util_image.tensor2img :216-273)."""
+        lq, mask = self._ingest_u8(lq_u8, mask_u8)
+        sr = self._sample_tiled(lq, mask=mask, noise_repeat=noise_repeat)
+        return self._emit_u8(sr, lq, mask, mask_back=mask_back, bgr=bgr)
+
+    @staticmethod
+    def _ingest_u8(lq_u8, mask_u8=None):
         from . import _lib
         b, h, w, _ = lq_u8.shape
         lq = torch.empty(b, 3, h, w, dtype=torch.float32, device=lq_u8.device)
@@ -311,8 +447,13 @@ class ResShiftSampler(BaseSampler):
         if mask_u8 is not None:
             mask = torch.empty(b, 1, h, w, dtype=torch.float32, device=lq_u8.device)
             _lib.check(_lib.lib.rs_op_ingest_u8(mask_u8.contiguous().data_ptr(), b, h, w, 1, mask.data_ptr(), _lib.current_stream()))
-        sr = self._sample_tiled(lq, mask=mask, noise_repeat=noise_repeat).contiguous()
-        out = torch.empty(b, h * self.sf, w * self.sf, 3, dtype=torch.uint8, device=lq_u8.device)
+        return lq, mask
+
+    def _emit_u8(self, sr, lq, mask, mask_back=True, bgr=True):
+        from . import _lib
+        sr = sr.contiguous()
+        b, _, h, w = lq.shape
+        out = torch.empty(b, h * self.sf, w * self.sf, 3, dtype=torch.uint8, device=lq.device)
         blend = mask_back and mask is not None
         if blend and self.sf != 1:
             raise ValueError("mask-back needs sf == 1 (as in the reference's inpainting tasks)")
@@ -321,8 +462,11 @@ class ResShiftSampler(BaseSampler):
         return out
 
     def inference(self, in_path, out_path, mask_path=None, mask_back=True, bs=1, noise_repeat=False):
-        """File / folder driver (reference sampler.py:167-308).  Image I/O through OpenCV."""
+        """File / folder driver (reference sampler.py:167-308).  Image I/O through OpenCV.  With ``shard_tiles`` every
+        rank reads the whole chunk and runs its share of the chunk's tiles (_run_shard); rank 0 assembles and writes."""
         import cv2
+        if self.shard_tiles:
+            self._check_shardable()
         in_path, out_path = Path(in_path), Path(out_path)
         if self.rank == 0:
             assert in_path.exists()
@@ -340,23 +484,50 @@ class ResShiftSampler(BaseSampler):
         exts = {".png", ".jpg", ".jpeg", ".bmp"}
         files = sorted(p for p in in_path.rglob("*") if p.suffix.lower() in exts) if in_path.is_dir() else [in_path]
         self.write_log(f"Find {len(files)} images in {in_path}")
+        def read_group(group):
+            paths, ims = zip(*group)
+            lq = torch.stack(ims).cuda()
+            mask = None
+            if mask_path is not None:
+                mp = Path(mask_path)
+                mask = torch.stack([read(mp / p.name if mp.is_dir() else mp, gray=True) for p in paths]).cuda()
+            return paths, lq, mask
+
         for i0 in range(0, len(files), bs):
             chunk = files[i0:i0 + bs]
-            micro = math.ceil(bs / self.num_gpus)                     # reference sampler.py:273-277
-            mine = chunk[self.rank * micro:(self.rank + 1) * micro]
-            for group in _same_shape_groups(mine, read):
-                paths, ims = zip(*group)
-                lq = torch.stack(ims).cuda()
-                mask = None
-                if mask_path is not None:
-                    mp = Path(mask_path)
-                    mask = torch.stack([read(mp / p.name if mp.is_dir() else mp, gray=True) for p in paths]).cuda()
-                sr = self._process_u8(lq, mask_u8=mask, noise_repeat=noise_repeat, mask_back=mask_back, bgr=True).cpu().numpy()
-                for p, im in zip(paths, sr):
-                    cv2.imwrite(str(out_path / f"{p.stem}.png"), im)
+            if self.shard_tiles:
+                self._inference_shards(_same_shape_groups(chunk, read), read_group, out_path, mask_back, noise_repeat)
+            else:
+                micro = math.ceil(bs / self.num_gpus)                     # reference sampler.py:273-277
+                mine = chunk[self.rank * micro:(self.rank + 1) * micro]
+                for group in _same_shape_groups(mine, read):
+                    paths, lq, mask = read_group(group)
+                    sr = self._process_u8(lq, mask_u8=mask, noise_repeat=noise_repeat, mask_back=mask_back, bgr=True).cpu().numpy()
+                    for p, im in zip(paths, sr):
+                        cv2.imwrite(str(out_path / f"{p.stem}.png"), im)
             if self.num_gpus > 1:
                 dist.barrier()
         self.write_log(f"Processing done, enjoy the results in {out_path}")
+
+    def _inference_shards(self, groups, read_group, out_path, mask_back, noise_repeat):
+        """One chunk in shard_tiles mode: this rank's tiles, one gather per shape group, assembly and writing on rank 0."""
+        import cv2
+        paths, lqs, masks = [], [], []
+        for group in groups:
+            p, lq_u8, mask_u8 = read_group(group)
+            lq, mask = self._ingest_u8(lq_u8, mask_u8)
+            paths.append(p)
+            lqs.append(lq)
+            masks.append(mask)
+        shares = self._run_shard(lqs, masks, noise_repeat, self.num_gpus, self.rank)
+        counts = self._share_counts([tuple(lq.shape[2:]) for lq in lqs], self.num_gpus)
+        for g, lq in enumerate(lqs):
+            tiles = gather_counts(shares[g], counts[g])
+            if self.rank != 0:
+                continue
+            sr = self._emit_u8(self._assemble(tiles, *lq.shape[2:]), lq, masks[g], mask_back=mask_back, bgr=True)
+            for p, im in zip(paths[g], sr.cpu().numpy()):
+                cv2.imwrite(str(out_path / f"{p.stem}.png"), im)
 
 
 def _same_shape_groups(paths, read):
