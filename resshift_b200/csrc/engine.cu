@@ -412,7 +412,9 @@ struct Builder {
   // a level with few window pairs is one long serial tile per CTA on a handful of SMs; below this many pairs the four
   // small launches, whose prologues overlap through PDL, are used instead.  At the benchmark shape (batch 16, the 64x64 and
   // 32x32 levels fused) the default measured 127.7 ms per 15-step loop against 134.8 ms with every level on four launches
-  // (H100 80GB HBM3 SXM, 700 W)
+  // (H100 80GB HBM3 SXM, 700 W).  With an earlier build of the wgmma kernel, thresholds 96 / 32 / 8 / 1 (also fusing
+  // the 16x16 and 8x8 levels) measured 135.3 / 134.1 / 135.3 / 135.6 ms, one run each: within the run-to-run spread,
+  // so 96 stays (H100 80GB HBM3 SXM, 400 W)
   const int fuse_swin_min_pairs = env_int("RS_SWIN_FUSE_MIN_PAIRS", 96);
   const bool fuse_stats = env_int("RS_GN_FUSE", 1) && !env_is("RS_CONV_EPI", "direct") && !env_is("RS_CONV_IMPL", "simt");
   Builder(rs_plan& p) : P(p), E(*p.e), cur(&p.ops) {}

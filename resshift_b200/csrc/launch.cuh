@@ -504,8 +504,8 @@ inline int conv_init() {   // once per process, outside any stream capture
     RS_CUDA_OK(cudaFuncSetAttribute(mlp_fused_sm90_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     RS_CUDA_OK(cudaFuncSetAttribute(mlp_fused_sm90_kernel<192>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     RS_CUDA_OK(cudaFuncSetAttribute(mlp_fused_sm90_kernel<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    RS_CUDA_OK(cudaFuncSetAttribute(swin_attn_fused_kernel<192>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SwinSmem<192>::total));
-    RS_CUDA_OK(cudaFuncSetAttribute(swin_attn_fused_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SwinSmem<64>::total));
+    RS_CUDA_OK(cudaFuncSetAttribute(swin_attn_fused_kernel<192>, cudaFuncAttributeMaxDynamicSharedMemorySize, SwinSmem<192>::launch_bytes));
+    RS_CUDA_OK(cudaFuncSetAttribute(swin_attn_fused_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, SwinSmem<64>::launch_bytes));
     RS_CUDA_OK(cudaFuncSetAttribute(vq_attn_sm90_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, VqAttnSmem<128>::launch_bytes));
     RS_CUDA_OK(cudaFuncSetAttribute(vq_attn_sm90_kernel<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, VqAttnSmem<256>::launch_bytes));
     RS_CUDA_OK(cudaFuncSetAttribute(vq_attn_sm90_kernel<512>, cudaFuncAttributeMaxDynamicSharedMemorySize, VqAttnSmem<512>::launch_bytes));
@@ -725,6 +725,8 @@ inline int swin_attn_finalize(SwinAttnDesc& d) {
   RS_CHECK(d.y.C == E && d.y.H == d.x.H && d.y.W == d.x.W && d.y.N == d.x.N, "fused Swin attention: output geometry");
   RS_CHECK(d.x.ld % 8 == 0 && d.y.ld % 8 == 0 && d.wqkv_ld % 8 == 0 && d.wproj_ld % 8 == 0, "fused Swin attention: 16-byte rows");
   RS_CHECK((d.gn_part && d.gn_slots > 0) || d.gn_gstat, "fused Swin attention: norm1 statistics");
+  int rc = encode_weight_map(&p.tmWqkv, d.wqkv, d.wqkv_ld, 3 * E, 64); if (rc) return rc;
+  rc = encode_weight_map(&p.tmWproj, d.wproj, d.wproj_ld, E, 64); if (rc) return rc;
   p.x = d.x.ptr; p.x_ld = d.x.ld; p.y = d.y.ptr; p.y_ld = d.y.ld;
   p.N = d.x.N; p.H = d.x.H; p.W = d.x.W; p.heads = d.heads; p.shift = d.shift; p.scale = 0.17677669529663687f;
   p.gn_part = d.gn_part; p.gn_slots = d.gn_slots; p.gn_gstat = d.gn_gstat; p.gamma = d.gamma; p.beta = d.beta; p.eps = 1e-5f;
@@ -755,8 +757,8 @@ inline int swin_attn_finalize(SwinAttnDesc& d) {
   return 0;
 }
 inline int swin_attn_launch(const SwinAttnDesc& d, cudaStream_t st) {
-  if (d.x.C == 192) (void)launch_k(swin_attn_fused_kernel<192>, dim3(d.grid), dim3(kSwinThreads), SwinSmem<192>::total, st, d.prm);
-  else (void)launch_k(swin_attn_fused_kernel<64>, dim3(d.grid), dim3(kSwinThreads), SwinSmem<64>::total, st, d.prm);
+  if (d.x.C == 192) (void)launch_k(swin_attn_fused_kernel<192>, dim3(d.grid), dim3(kSwinThreads), (size_t)SwinSmem<192>::launch_bytes, st, d.prm);
+  else (void)launch_k(swin_attn_fused_kernel<64>, dim3(d.grid), dim3(kSwinThreads), (size_t)SwinSmem<64>::launch_bytes, st, d.prm);
   RS_CUDA_OK(cudaGetLastError());
   for (int k = 0; k < 2; ++k)
     if (d.fin[k].gstat) {
