@@ -139,6 +139,23 @@ int rs_vq_encode(rs_plan* p, const float* x, float* h_out, void* stream);
  * ldm/modules/vqvae/quantize.py:271-284; skipped when force_not_quantize) -> post_quant_conv -> Decoder -> [B, 3, H, W] fp32.
  * idx_out: optional [B, H/f, W/f] int32 code indices. */
 int rs_vq_decode(rs_plan* p, const float* h, float* out, int32_t* idx_out, int force_not_quantize, void* stream);
+/* Each pass split at its mid-block attention, so that the query rows of that attention can be computed by several
+ * devices and exchanged in between.  rs_vq_encode = rs_vq_encode_begin + rs_vq_encode_end and rs_vq_decode =
+ * rs_vq_decode_begin + rs_vq_decode_end, the same launches in the same order.  _begin runs the input stage and every op
+ * up to and including the fused attention (the whole op list on plans without one: bottlenecks of <= 8192 positions);
+ * _end runs the rest and the output stage (quant_conv / the copy of the image). */
+int rs_vq_encode_begin(rs_plan* p, const float* x, void* stream);
+int rs_vq_encode_end(rs_plan* p, float* h_out, void* stream);
+int rs_vq_decode_begin(rs_plan* p, const float* h, int32_t* idx_out, int force_not_quantize, void* stream);
+int rs_vq_decode_end(rs_plan* p, float* out, void* stream);
+/* Query rows [row_begin, row_end) of every image that the plan's fused attention computes (default [0, T), T = the
+ * bottleneck's H*W); multiples of 64 inside [0, T].  An empty range skips the attention launch.  Rows outside the
+ * range keep whatever the attention output view held (the caller writes them between _begin and _end). */
+int rs_vq_set_attention_rows(rs_plan* p, int row_begin, int row_end);
+/* The fused attention's output as proj_out reads it (bound plans): fp16, element (n, t, c) at
+ * ptr + n * image_stride + t * row_stride + c (strides in elements), n < batch, t < T, c < C.  It holds the attention
+ * result from the end of _begin until _end reads it; nothing else in the plan writes it in between. */
+int rs_vq_attention_output(rs_plan* p, void** ptr, long long* row_stride, long long* image_stride, int32_t* T, int32_t* C);
 /* diagnostics: per-launch times (ms) and descriptions of the plan's op list on the inputs of the last encode/decode
  * call (counterpart of rs_plan_profile_ops for the first-stage plans) */
 int rs_vq_profile_ops(rs_plan* p, double* ms, char* desc, int desc_stride, int cap, int32_t* n_ops, void* stream);
@@ -208,6 +225,11 @@ int rs_op_groupnorm_finalize(const float* part, int N, int slots, int C, int row
  * plans run it for bottlenecks with H*W > 8192).  q, k, v fp16 [N][T][C] with row stride ld; out fp16 [N][T][C] dense.
  * C in {128, 256, 512}, T % 64 == 0; O(T*C) memory, deterministic, one launch. */
 int rs_op_vq_attention(const void* q, const void* k, const void* v, int N, int T, int C, int ld, void* out, void* stream);
+/* the same for the query rows [row_begin, row_end) of every image only (multiples of 64, non-empty, row_end <= T; keys
+ * and values are still all T positions).  Those rows of out are bit-identical to rs_op_vq_attention's; no other row of
+ * out is written, so ranges computed on different devices and copied together equal one full call. */
+int rs_op_vq_attention_rows(const void* q, const void* k, const void* v, int N, int T, int C, int ld, int row_begin,
+                            int row_end, void* out, void* stream);
 /* window attention core (reference models/swin_transformer.py:114-145,251-275); qkv [N,H,W,3*heads*32] */
 int rs_op_expand_relpos(const float* table_225xh, float* dense_hx64x64, int heads, void* stream);
 int rs_op_window_attention(const void* qkv, int N, int H, int W, int heads, int shift, const float* bias_dense,

@@ -90,6 +90,7 @@ _SIGNATURES = {
                                               C.c_int, _P, C.c_int, _P, C.c_int, _P]),
     "rs_op_expand_relpos": (C.c_int, [_P, _P, C.c_int, _P]),
     "rs_op_vq_attention": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P]),
+    "rs_op_vq_attention_rows": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P]),
     "rs_op_window_attention": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P, _P]),
     "rs_op_swin_attn": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, C.c_int, _P, _P, _P, _P, _P, _P, _P,
                                   _P, _P, _P, _P, _P]),
@@ -100,6 +101,13 @@ _SIGNATURES = {
     "rs_vq_plan_create": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(_P)]),
     "rs_vq_encode": (C.c_int, [_P, _P, _P, _P]),
     "rs_vq_decode": (C.c_int, [_P, _P, _P, _P, C.c_int, _P]),
+    "rs_vq_encode_begin": (C.c_int, [_P, _P, _P]),
+    "rs_vq_encode_end": (C.c_int, [_P, _P, _P]),
+    "rs_vq_decode_begin": (C.c_int, [_P, _P, _P, C.c_int, _P]),
+    "rs_vq_decode_end": (C.c_int, [_P, _P, _P]),
+    "rs_vq_set_attention_rows": (C.c_int, [_P, C.c_int, C.c_int]),
+    "rs_vq_attention_output": (C.c_int, [_P, C.POINTER(_P), C.POINTER(C.c_longlong), C.POINTER(C.c_longlong),
+                                         C.POINTER(C.c_int32), C.POINTER(C.c_int32)]),
     "rs_vq_profile_ops": (C.c_int, [_P, C.POINTER(C.c_double), C.c_char_p, C.c_int, C.c_int, C.POINTER(C.c_int32), _P]),
     "rs_op_bicubic_upsample": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P]),
     "rs_op_ingest_u8": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P]),

@@ -333,6 +333,7 @@ struct rs_plan {
   }
   int vq_which = -1;         // -1: denoiser plan; 0 / 1: VQ-GAN encode / decode plan (vq.inc)
   int imgH = 0, imgW = 0;    // VQ plans: image size (H, W above are the latent size)
+  int vq_attn_op = -1;       // VQ plans: index in ops of the fused bottleneck attention (-1: none, T <= 8192)
   // The schedule tables and the FiLM table live in this plan's workspace and are shared by rs_plan_forward (FiLM rows
   // 0..B-1 for the caller's timesteps) and by every sampler of the plan (rows 0..T-1 for its schedule): whoever wrote them
   // last owns them.  A sampler re-derives them when it is not the owner or when the weights changed since (weights_epoch).
@@ -1006,10 +1007,12 @@ inline bool op_skipped(const Op& op) {
   return false;
 }
 
-int run_ops(rs_plan& P, const std::vector<Op>& ops, const float* film_base, long long film_sN, cudaStream_t st0,
-            Prof* prof = nullptr) {
+// ops [first, last) of an op list
+int run_op_range(rs_plan& P, const Op* first, const Op* last, const float* film_base, long long film_sN, cudaStream_t st0,
+                 Prof* prof = nullptr) {
   const bool multi = prof == nullptr && !P.side.empty();       // per-op timing runs everything on the caller's stream
-  for (const Op& op : ops) {
+  for (const Op* it = first; it != last; ++it) {
+    const Op& op = *it;
     int rc = 0;
     if (op.kind == OP_FORK || op.kind == OP_JOIN) {
       if (multi) {
@@ -1061,6 +1064,11 @@ int run_ops(rs_plan& P, const std::vector<Op>& ops, const float* film_base, long
     if (rc) return rc;
   }
   return 0;
+}
+
+int run_ops(rs_plan& P, const std::vector<Op>& ops, const float* film_base, long long film_sN, cudaStream_t st0,
+            Prof* prof = nullptr) {
+  return run_op_range(P, ops.data(), ops.data() + ops.size(), film_base, film_sN, st0, prof);
 }
 
 // timestep embedding -> time_embed MLP -> all emb_layers at once, for `rows` timesteps
@@ -1318,7 +1326,12 @@ static void collect_profile(const rs_plan& P, const Prof& prof, double* ms, char
     } else if (op.kind == OP_SOFTMAX) {
       snprintf(d, desc_stride, "softmax %d", op.s_view.C);
     } else if (op.kind == OP_VQ_ATTN) {
-      snprintf(d, desc_stride, "vq_attn T=%d C=%d N=%d", op.vqa.prm.T, op.vqa.q.C, op.vqa.q.N);
+      // the query-row range only when it is not all T rows (the default launch keeps its description)
+      const VqAttnDesc& a = op.vqa;
+      if (a.row_begin == 0 && a.row_end == a.prm.T)
+        snprintf(d, desc_stride, "vq_attn T=%d C=%d N=%d", a.prm.T, a.q.C, a.q.N);
+      else
+        snprintf(d, desc_stride, "vq_attn T=%d C=%d N=%d rows=%d:%d", a.prm.T, a.q.C, a.q.N, a.row_begin, a.row_end);
     } else {
       snprintf(d, desc_stride, "upsample %dx%d C=%d", op.u_in.H, op.u_in.W, op.u_in.C);
     }

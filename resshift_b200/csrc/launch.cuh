@@ -771,8 +771,21 @@ inline int swin_attn_launch(const SwinAttnDesc& d, cudaStream_t st) {
 // ---- fused VQ-GAN attention over all positions of an image (vq_attn.cuh) -----------------
 struct VqAttnDesc {
   View q, k, v, out;                       // [N, H, W, C]; T = H * W positions per image
+  int row_begin = 0, row_end = -1;         // query rows [row_begin, row_end) of every image (-1: T); empty: no launch
   VqAttnParams prm;
 };
+// sets the query-row range of a (finalized or not) descriptor: multiples of 64 inside [0, T]; an empty range only if
+// allow_empty (a plan then skips the launch)
+inline int vq_attn_set_rows(VqAttnDesc& d, long long row_begin, long long row_end, bool allow_empty) {
+  const long long T = (long long)d.q.H * d.q.W;
+  RS_CHECK(row_begin >= 0 && row_begin <= row_end && row_end <= T,
+           "fused VQ-GAN attention: rows [" + std::to_string(row_begin) + ", " + std::to_string(row_end) + ") outside [0, T = " + std::to_string(T) + ")");
+  RS_CHECK(row_begin % kVqAttnBM == 0 && row_end % kVqAttnBM == 0, "fused VQ-GAN attention: row range bounds must be multiples of 64");
+  RS_CHECK(allow_empty || row_end > row_begin, "fused VQ-GAN attention: empty row range");
+  d.row_begin = (int)row_begin; d.row_end = (int)row_end;
+  d.prm.q_tile0 = (int)(row_begin / kVqAttnBM);
+  return 0;
+}
 inline int vq_attn_finalize(VqAttnDesc& d) {
   VqAttnParams& p = d.prm;
   std::memset(&p, 0, sizeof(p));
@@ -787,6 +800,7 @@ inline int vq_attn_finalize(VqAttnDesc& d) {
     RS_CHECK(v->ptr != nullptr && v->ld >= C && v->ld % 8 == 0, "fused VQ-GAN attention: rows of >= C elements, 16-byte aligned");
   }
   p.T = (int)T;
+  { int rc = vq_attn_set_rows(d, d.row_begin, d.row_end < 0 ? T : d.row_end, true); if (rc) return rc; }
   p.scale_log2 = (float)(1.4426950408889634 / std::sqrt((double)C));
   CUtensorMap* maps[4] = {&p.tmQ, &p.tmK, &p.tmV, &p.tmO};
   const int rows[4] = {kVqAttnBM, vq_attn_bk(C), vq_attn_bk(C), kVqAttnBM};
@@ -798,7 +812,8 @@ inline int vq_attn_finalize(VqAttnDesc& d) {
   return 0;
 }
 inline int vq_attn_launch(const VqAttnDesc& d, cudaStream_t st) {
-  const dim3 grid((unsigned)(d.prm.T / kVqAttnBM), (unsigned)d.q.N);
+  if (d.row_end == d.row_begin) return 0;
+  const dim3 grid((unsigned)((d.row_end - d.row_begin) / kVqAttnBM), (unsigned)d.q.N);
   switch (d.q.C) {
     case 128: (void)launch_k(vq_attn_sm90_kernel<128>, grid, dim3(kVqAttnThreads), (size_t)VqAttnSmem<128>::launch_bytes, st, d.prm); break;
     case 256: (void)launch_k(vq_attn_sm90_kernel<256>, grid, dim3(kVqAttnThreads), (size_t)VqAttnSmem<256>::launch_bytes, st, d.prm); break;

@@ -4,6 +4,11 @@
 // reference: AttnBlock.forward (ldm/modules/diffusionmodules/model.py:180-199; the MemoryEfficientAttnBlock path at
 // :205-268 computes the same).  q, k, v, out: fp16 [N][T][C] (row stride ld); one launch, grid (T / 64, N).
 //
+// A launch may cover a range of query rows [row_begin, row_end) (multiples of 64) instead of all T: grid
+// ((row_end - row_begin) / 64, N), CTA x takes query tile row_begin / 64 + x; K and V are always all T keys, and rows
+// outside the range are neither read as queries nor written.  A row's result depends only on its query and the full K, V
+// walked in the same order, so any partition of the rows over several launches (or GPUs) is bit-identical to one launch.
+//
 // A CTA owns 64 queries and walks the T keys in blocks of BK keys (vq_attn_bk: 32, or 16 at C = 512), in a fixed order,
 // with an online softmax (running row max and row sum in fp32), so memory is O(T C) and the result is bit-reproducible and
 // per image.  Warp 8 is the TMA producer: the Q tile once, then per key block the K block and the V block, each behind its
@@ -46,6 +51,7 @@ constexpr int kVqAttnConsumerRegs = 240;
 struct VqAttnParams {
   CUtensorMap tmQ, tmK, tmV, tmO;    // {C, T, 1, N}, boxes {64, 64 | BK, 1, 1}, 128-byte swizzle
   int T;
+  int q_tile0;                       // first query tile (row_begin / 64) of the launch's row range
   float scale_log2;                  // C^-1/2 * log2(e)
 };
 
@@ -100,7 +106,7 @@ __global__ void __launch_bounds__(kVqAttnThreads, 1) vq_attn_sm90_kernel(const _
   uint64_t* q_full = empty + kVqAttnStages;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int q0 = (int)blockIdx.x * kVqAttnBM, img = (int)blockIdx.y;
+  const int q0 = (p.q_tile0 + (int)blockIdx.x) * kVqAttnBM, img = (int)blockIdx.y;
   const int nblk = p.T / kBK;
 
   if (warp == kVqAttnTmaWarp && lane == 0) {

@@ -7,16 +7,22 @@ row softmax up to 8192 positions and as one fused online-softmax kernel above (a
 
 ``encode(x)`` / ``decode(h, force_not_quantize=False)`` / ``forward`` take and return fp32 NCHW CUDA tensors.  PyTorch
 owns every allocation; there is no eager / CPU fallback.
+
+``with vq.attention_team(member, size, exchange):`` splits the fused bottleneck attention's query rows over a team of
+processes (DESIGN.md §6): each member computes its share of the rows and ``exchange`` fills in the others', so the
+result is bit-identical to computing all rows here.
 """
 from __future__ import annotations
 
 import ctypes as C
-from typing import Dict, Optional, Tuple
+from contextlib import contextmanager
+from typing import Callable, Dict, List, Optional, Tuple
 
 import torch
 import torch.nn as nn
 
 from .. import _lib
+from ..parallel import shard_range
 from ..vq_arch import VQConfig, random_vq_state_dict, vq_param_spec
 
 
@@ -51,6 +57,9 @@ class VQModelTorch(nn.Module):
         self._packed_versions: Optional[Tuple] = None
         self._plans: Dict[Tuple[int, int, int, int], "_VQPlan"] = {}
         self.last_indices: Optional[torch.Tensor] = None
+        self._team: Optional[Tuple[int, int, Callable]] = None
+        # (which, row_begin, row_end) of every team-split attention since the last attention_team() entry: 0 encode, 1 decode
+        self.attention_rows: List[Tuple[int, int, int]] = []
 
     # ------------------------------------------------------------------ native plumbing
     def _ensure_engine(self, device: torch.device):
@@ -120,7 +129,13 @@ class VQModelTorch(nn.Module):
         plan = self.plan(0, b, hh, ww)
         xf = x.detach().float().contiguous()
         out = torch.empty(b, self.cfg.embed_dim, hh // f, ww // f, dtype=torch.float32, device=x.device)
-        _lib.check(_lib.lib.rs_vq_encode(plan.handle, xf.data_ptr(), out.data_ptr(), _lib.current_stream()))
+        stream = _lib.current_stream()
+        if self._team is not None and plan.attention is not None:
+            self._run_team_split(
+                plan, 0, lambda: _lib.check(_lib.lib.rs_vq_encode_begin(plan.handle, xf.data_ptr(), stream)),
+                lambda: _lib.check(_lib.lib.rs_vq_encode_end(plan.handle, out.data_ptr(), stream)))
+        else:
+            _lib.check(_lib.lib.rs_vq_encode(plan.handle, xf.data_ptr(), out.data_ptr(), stream))
         return out
 
     @torch.no_grad()
@@ -137,13 +152,54 @@ class VQModelTorch(nn.Module):
         hf = h.detach().float().contiguous()
         out = torch.empty(b, self.cfg.out_ch, lh * f, lw * f, dtype=torch.float32, device=h.device)
         idx = torch.empty(b, lh, lw, dtype=torch.int32, device=h.device)
-        _lib.check(_lib.lib.rs_vq_decode(plan.handle, hf.data_ptr(), out.data_ptr(), idx.data_ptr(), int(bool(force_not_quantize)),
-                                         _lib.current_stream()))
+        stream, fnq = _lib.current_stream(), int(bool(force_not_quantize))
+        if self._team is not None and plan.attention is not None:
+            self._run_team_split(
+                plan, 1, lambda: _lib.check(_lib.lib.rs_vq_decode_begin(plan.handle, hf.data_ptr(), idx.data_ptr(), fnq, stream)),
+                lambda: _lib.check(_lib.lib.rs_vq_decode_end(plan.handle, out.data_ptr(), stream)))
+        else:
+            _lib.check(_lib.lib.rs_vq_decode(plan.handle, hf.data_ptr(), out.data_ptr(), idx.data_ptr(), fnq, stream))
         self.last_indices = idx
         return out
 
     def forward(self, input, force_not_quantize=False):
         return self.decode(self.encode(input), force_not_quantize)
+
+    # ------------------------------------------------------------------ attention teams
+    @contextmanager
+    def attention_team(self, member: int, size: int, exchange: Callable[[torch.Tensor, int, int], None]):
+        """Inside this context, ``encode`` / ``decode`` on a plan with the fused bottleneck attention (more than 8192
+        positions) compute only this member's query rows of it: 64-row blocks ``parallel.shard_range(T / 64, size,
+        member)``.  After the first half of the pass, ``exchange(view, row_begin, row_end)`` is called with the attention
+        output ``view`` ([N, T, C] fp16, on the current stream) and this member's rows; it must write every other
+        member's rows into ``view``.  Then the pass finishes.  Every member must run the same calls on the same inputs.
+        The attention rows are independent, so the result is bit-identical to a call outside the context.  Rows computed
+        are recorded in ``attention_rows``.  Plans without the fused attention run as usual."""
+        if not (0 <= member < size):
+            raise ValueError(f"team member {member} of {size}")
+        if self._team is not None:
+            raise RuntimeError("attention_team contexts do not nest")
+        self._team = (member, size, exchange)
+        self.attention_rows = []
+        try:
+            yield self
+        finally:
+            self._team = None
+
+    def _run_team_split(self, plan: "_VQPlan", which: int, begin: Callable[[], None], end: Callable[[], None]):
+        member, size, exchange = self._team
+        view = plan.attention
+        t = view.shape[1]
+        b0, e0 = shard_range(t // 64, size, member)
+        rb, re = 64 * b0, 64 * e0
+        _lib.check(_lib.lib.rs_vq_set_attention_rows(plan.handle, rb, re))
+        try:
+            begin()
+        finally:
+            _lib.check(_lib.lib.rs_vq_set_attention_rows(plan.handle, 0, t))
+        exchange(view, rb, re)
+        end()
+        self.attention_rows.append((which, rb, re))
 
     def __del__(self):
         try:
@@ -167,6 +223,14 @@ class _VQPlan:
         self.workspace_ptr = (self.workspace.data_ptr() + 255) // 256 * 256
         _lib.check(_lib.lib.rs_plan_bind(h, self.workspace_ptr))
         self.launches = _lib.lib.rs_plan_num_launches(h)
+        # the fused attention's output [N, T, C] fp16 as a view of the workspace (None: the plan has no fused attention)
+        self.attention: Optional[torch.Tensor] = None
+        ptr, rstride, istride, t, cc = C.c_void_p(), C.c_longlong(), C.c_longlong(), C.c_int32(), C.c_int32()
+        if _lib.lib.rs_vq_attention_output(h, C.byref(ptr), C.byref(rstride), C.byref(istride), C.byref(t), C.byref(cc)) == 0:
+            off = ptr.value - self.workspace.data_ptr()
+            assert off % 2 == 0 and self.workspace.numel() % 2 == 0
+            self.attention = torch.as_strided(self.workspace.view(torch.float16), (batch, t.value, cc.value),
+                                              (istride.value, rstride.value, 1), off // 2)
 
     def __del__(self):
         try:

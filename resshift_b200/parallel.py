@@ -5,12 +5,14 @@ the T-step loop communicates.  Partitioning is the reference's (contiguous slice
 ceil(bs / world) per rank, reference sampler.py:273-277).  Collectives go through ``torch.distributed``
 (NCCL over NVLink on the GPU box, gloo in the CPU tests) — a broadcast of the flattened weights from
 rank 0 at start-up and an all-gather of the result shards at the end.  Tile sharding
-(``ResShiftSampler(shard_tiles=True)``) deals the tiles of a chunk instead and gathers them with ``gather_counts``.
+(``ResShiftSampler(shard_tiles=True)``) deals the tiles of a chunk instead and gathers them with ``gather_counts``;
+when a chunk has fewer units than ranks, each unit goes to a team of ranks (``attention_teams``) that splits the
+VQ-GAN bottleneck attention's query rows and exchanges them (``row_exchange``).
 """
 from __future__ import annotations
 
 import math
-from typing import Dict, List, Tuple
+from typing import Dict, List, Optional, Tuple
 
 import torch
 import torch.distributed as dist
@@ -68,3 +70,52 @@ def gather_counts(local: torch.Tensor, counts: List[int]) -> torch.Tensor:
     outs: List[torch.Tensor] = [torch.empty_like(pad) for _ in range(world)]
     dist.all_gather(outs, pad)
     return torch.cat([o[:n] for o, n in zip(outs, counts)], dim=0).to(local.device)
+
+
+def attention_teams(n_units: int, world: int) -> Optional[List[Tuple[int, int]]]:
+    """Ranks [start, end) of the team that runs unit u, for a chunk of ``n_units`` work units on ``world`` ranks with
+    fewer units than ranks: contiguous teams, in rank order, whose sizes differ by at most one (the larger ones first).
+    None when every rank has a unit of its own to run (``n_units >= world``)."""
+    if n_units < 1 or n_units >= world:
+        return None
+    base, extra = divmod(world, n_units)
+    teams, start = [], 0
+    for u in range(n_units):
+        size = base + (1 if u < extra else 0)
+        teams.append((start, start + size))
+        start += size
+    return teams
+
+
+def attention_row_ranges(n_rows: int, size: int) -> List[Tuple[int, int]]:
+    """[row_begin, row_end) of each of ``size`` team members for an attention over ``n_rows`` query rows (a multiple of
+    64): the 64-row blocks dealt as shard_range does."""
+    return [(64 * a, 64 * e) for a, e in (shard_range(n_rows // 64, size, m) for m in range(size))]
+
+
+def team_group(ranks: Tuple[int, ...], cache: Dict[Tuple[int, ...], object]):
+    """The process group of ``ranks``, created once.  dist.new_group must be entered by every rank of the default group,
+    in the same order: callers ask for every team of a chunk in team order on every rank."""
+    if ranks not in cache:
+        cache[ranks] = dist.new_group(list(ranks))
+    return cache[ranks]
+
+
+def row_exchange(group, size: int, member: int):
+    """``exchange(view, row_begin, row_end)`` for VQModelTorch.attention_team: all-gathers every member's rows of the
+    [N, T, C] attention output ``view`` inside ``group`` (this member's are [row_begin, row_end)) and writes the other
+    members' rows into ``view``.  Shares are padded to the largest for one ``all_gather``; under gloo the exchange is
+    staged through host memory, as gather_counts does."""
+    def exchange(view: torch.Tensor, row_begin: int, row_end: int) -> None:
+        n, t, c = view.shape
+        ranges = attention_row_ranges(t, size)
+        assert ranges[member] == (row_begin, row_end), (ranges, member, row_begin, row_end)
+        stage = torch.device("cpu") if dist.get_backend(group) == "gloo" else view.device
+        pad = torch.zeros((n, max(e - b for b, e in ranges), c), dtype=view.dtype, device=stage)
+        pad[:, :row_end - row_begin] = view[:, row_begin:row_end]
+        outs: List[torch.Tensor] = [torch.empty_like(pad) for _ in range(size)]
+        dist.all_gather(outs, pad, group=group)
+        for m, (b, e) in enumerate(ranges):
+            if m != member and e > b:
+                view[:, b:e] = outs[m][:, :e - b].to(view.device)
+    return exchange

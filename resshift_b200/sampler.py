@@ -8,7 +8,8 @@ PYTHONPATH, see INTEGRATION.md) is all that changes.  The VQ-GAN autoencoder is 
 (a PyTorch module; bookends stay in PyTorch).  Multi-GPU follows the reference: one process per GPU,
 contiguous batch slices per rank (sampler.py:273-277), same seed on every rank; on top of that rank 0 can
 broadcast the weights over NCCL (``broadcast_weights``) and results can be gathered (``gather_results``).
-``shard_tiles=True`` deals the tiles of each chunk across the ranks instead, bit-identical to one GPU (DESIGN.md §6).
+``shard_tiles=True`` deals the tiles of each chunk across the ranks instead, bit-identical to one GPU (DESIGN.md §6);
+a chunk with fewer units than ranks runs each unit on a team of ranks that splits its VQ-GAN bottleneck attention.
 """
 from __future__ import annotations
 
@@ -26,7 +27,7 @@ import torch
 import torch.distributed as dist
 import torch.nn.functional as F
 
-from .parallel import gather_counts, shard_range
+from .parallel import attention_teams, gather_counts, row_exchange, shard_range, team_group
 
 
 # --------------------------------------------------------------------------------------------------
@@ -334,6 +335,40 @@ class ResShiftSampler(BaseSampler):
                 counts[g][r] += len(starts)
         return counts
 
+    def _gather_counts(self, shapes, world):
+        """counts[g][r]: tiles of shape group g that rank r contributes to the gather.  With fewer units than ranks,
+        unit u is run by team u of parallel.attention_teams and only the team's first rank contributes its tiles;
+        otherwise _share_counts."""
+        units = self._plan_units(shapes)
+        teams = attention_teams(len(units), world)
+        if teams is None:
+            return self._share_counts(shapes, world)
+        counts = [[0] * world for _ in shapes]
+        for (g, starts, _, _), (first, _) in zip(units, teams):
+            counts[g][first] += len(starts)
+        return counts
+
+    def _run_team(self, lqs, masks, noise_repeat, world, rank):
+        """This rank's part of a chunk with fewer units than ranks: the rank runs its team's unit (team u runs unit u,
+        parallel.attention_teams) with the VQ-GAN bottleneck attention's query rows split across the team and exchanged
+        inside the team's process group, so every member ends with the whole unit, bit-identical to one GPU.  Noise is
+        drawn for every unit as _run_shard does.  Returns per group the tiles this rank contributes to the gather (the
+        team's first rank: the unit's tiles; the others: none).  Every rank of the default group must call this."""
+        self._check_shardable()
+        units = self._plan_units([tuple(lq.shape[2:]) for lq in lqs])
+        teams = attention_teams(len(units), world)
+        groups = self.__dict__.setdefault("_team_groups", {})
+        for first, end in teams:                     # every rank creates every multi-rank team's group, in team order
+            if end - first > 1:
+                team_group(tuple(range(first, end)), groups)
+        u = next(i for i, (first, end) in enumerate(teams) if first <= rank < end)
+        first, end = teams[u]
+        team = None
+        if end - first > 1:
+            member, size = rank - first, end - first
+            team = (member, size, row_exchange(team_group(tuple(range(first, end)), groups), size, member))
+        return self._run_units(lqs, masks, noise_repeat, units, u, u + 1, keep=rank == first, team=team)
+
     def _latent_spec(self, n, h, w, dtype):
         """Shape and dtype of z_y = encode_first_stage(y, up_sample=True) for an [n, 3, h, w] input (after the
         padding_offset reflect-pad) of dtype ``dtype``, derived from the configs without running the encoder: the VQ
@@ -388,6 +423,12 @@ class ResShiftSampler(BaseSampler):
             raise ValueError("shard_tiles needs the LQ image of every group")
         units = self._plan_units([tuple(lq.shape[2:]) for lq in lqs])
         a, e = shard_range(len(units), world, rank)
+        return self._run_units(lqs, masks, noise_repeat, units, a, e)
+
+    def _run_units(self, lqs, masks, noise_repeat, units, a, e, keep=True, team=None):
+        """Walks every unit of ``units``, drawing its noise, and runs units [a, e) (_run_shard).  ``keep``: return their
+        tiles, else empty shares (a team member other than the first).  ``team``: (member, size, exchange) to run the
+        units under the autoencoder's attention_team."""
         out = [[] for _ in lqs]
         offset = self.padding_offset
         ctx = torch.autocast("cuda") if self.use_amp else nullcontext()
@@ -405,8 +446,10 @@ class ResShiftSampler(BaseSampler):
                     continue
                 pch = torch.cat([lq[:, :, hs:hs + th, ws:ws + tw] for hs, ws in starts], dim=0)
                 mch = None if mask is None else torch.cat([mask[:, :, hs:hs + th, ws:ws + tw] for hs, ws in starts], dim=0)
-                res = self._sample_unit(pch, mch, noises, spec).float()
-            out[g].extend(torch.split(res, b, dim=0))
+                with self.autoencoder.attention_team(*team) if team is not None else nullcontext():
+                    res = self._sample_unit(pch, mch, noises, spec).float()
+            if keep:
+                out[g].extend(torch.split(res, b, dim=0))
         tile_hw = {g: (th, tw) for g, _, th, tw in units}
         return [torch.stack(t) if t else
                 torch.empty((0,) + tuple(lq.shape[:2]) + (tile_hw[g][0] * self.sf, tile_hw[g][1] * self.sf), device=lq.device)
@@ -510,7 +553,8 @@ class ResShiftSampler(BaseSampler):
         self.write_log(f"Processing done, enjoy the results in {out_path}")
 
     def _inference_shards(self, groups, read_group, out_path, mask_back, noise_repeat):
-        """One chunk in shard_tiles mode: this rank's tiles, one gather per shape group, assembly and writing on rank 0."""
+        """One chunk in shard_tiles mode: this rank's tiles (its own units, or with fewer units than ranks its team's
+        unit), one gather per shape group, assembly and writing on rank 0."""
         import cv2
         paths, lqs, masks = [], [], []
         for group in groups:
@@ -519,8 +563,16 @@ class ResShiftSampler(BaseSampler):
             paths.append(p)
             lqs.append(lq)
             masks.append(mask)
-        shares = self._run_shard(lqs, masks, noise_repeat, self.num_gpus, self.rank)
-        counts = self._share_counts([tuple(lq.shape[2:]) for lq in lqs], self.num_gpus)
+        shapes = [tuple(lq.shape[2:]) for lq in lqs]
+        # fewer units than ranks: teams of ranks share each unit's bottleneck attention instead of leaving ranks idle
+        teams = self.num_gpus > 1 and dist.is_initialized() and hasattr(self.autoencoder, "attention_team") and \
+            attention_teams(len(self._plan_units(shapes)), self.num_gpus) is not None
+        if teams:
+            shares = self._run_team(lqs, masks, noise_repeat, self.num_gpus, self.rank)
+            counts = self._gather_counts(shapes, self.num_gpus)
+        else:
+            shares = self._run_shard(lqs, masks, noise_repeat, self.num_gpus, self.rank)
+            counts = self._share_counts(shapes, self.num_gpus)
         for g, lq in enumerate(lqs):
             tiles = gather_counts(shares[g], counts[g])
             if self.rank != 0:
