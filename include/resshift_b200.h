@@ -12,6 +12,14 @@
  *   - pointers are raw device pointers unless the name says `host`.  Tensors at the boundary are
  *     contiguous fp32 NCHW, exactly what the reference module receives/returns.
  *   - one host thread per engine (the reference is one single-threaded process per GPU, sampler.py:66-77).
+ *     Different engines may be driven from different host threads at the same time, on the same or on different
+ *     devices (one-time per-device setup is thread-safe).
+ *   - devices: an engine belongs to the CUDA device that is current at rs_unet_set_arena (device memory of another
+ *     device is refused as its arena), and a plan to the device
+ *     that is current at rs_plan_bind, which must be its engine's.  A plan runs on the device it was bound on: every
+ *     entry point that enqueues work on a plan or its sampler (rs_plan_forward / _profile / _profile_ops / _probe,
+ *     rs_sampler_run / _run_host, rs_vq_encode / _decode and their _begin / _end halves, rs_vq_profile_ops)
+ *     returns an error when another device is current, and the stream passed in must belong to that device.
  */
 #ifndef RESSHIFT_B200_H
 #define RESSHIFT_B200_H

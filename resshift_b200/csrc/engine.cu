@@ -49,7 +49,8 @@ struct rs_engine {
   std::map<std::string, int> index;
   size_t arena_bytes = 0;
   uint8_t* arena = nullptr;
-  unsigned long long weights_epoch = 0;     // bumped by every rs_unet_load_param: tables derived from weights (FiLM) go stale
+  int device = -1;              // CUDA device that was current at rs_unet_set_arena (where the arena lives)
+  unsigned long long weights_epoch = 0;    // bumped by every rs_unet_load_param: tables derived from weights (FiLM) go stale
   // concatenated emb_layers ("FiLM") matrix: rows = sum 2*Cout over ResBlocks, K = time_embed_dim
   size_t film_w_off = 0, film_b_off = 0;
   int film_rows = 0;
@@ -318,6 +319,7 @@ struct rs_plan {
   int cin_pad = 0, fe_cpad = 0;
   float* out_f32 = nullptr;  // model output (fp32 NCHW), inside the state region
   bool bound = false;
+  int device = -1;           // CUDA device that was current at rs_plan_bind: the only one the plan runs on
   int launches = 0;
   // Low-resolution levels (a handful of output tiles per layer at batch 16: every kernel is latency-bound and leaves most
   // SMs idle) run as `branches` independent batch slices on concurrent streams; each slice's kernels depend only on its
@@ -1120,6 +1122,17 @@ int pack_lq_and_input(rs_plan& P, const float* x, const float* lq, const float* 
   return 0;
 }
 
+// A plan runs on the device it was bound on: its side streams, events, workspace, TMA descriptors and the engine's
+// arena all belong to that device.  Every run entry point checks the current device first.
+int check_plan_device(const rs_plan& P) {
+  int dev = -1;
+  RS_CUDA_OK(cudaGetDevice(&dev));
+  if (dev != P.device)
+    return fail(-1, "plan was bound on cuda:" + std::to_string(P.device) + " but cuda:" + std::to_string(dev) +
+                    " is current: a plan runs on the device it was bound on");
+  return 0;
+}
+
 }  // namespace
 
 // ------------------------------------------------------------------------------------------------
@@ -1157,7 +1170,16 @@ int rs_unet_param_info(const rs_engine* e, int index, char* name, size_t name_ca
 size_t rs_unet_arena_bytes(const rs_engine* e) { return e ? e->arena_bytes : 0; }
 int rs_unet_set_arena(rs_engine* e, void* arena_dev) {
   RS_CHECK(e && arena_dev && (reinterpret_cast<uintptr_t>(arena_dev) & 255) == 0, "arena must be 256-byte aligned");
+  int dev = -1;
+  RS_CUDA_OK(cudaGetDevice(&dev));
+  // the engine belongs to the current device, so device memory of another device cannot be its arena
+  cudaPointerAttributes attr{};
+  RS_CUDA_OK(cudaPointerGetAttributes(&attr, arena_dev));
+  RS_CHECK(attr.type != cudaMemoryTypeDevice || attr.device == dev,
+           "the arena is memory of cuda:" + std::to_string(attr.device) + " but cuda:" + std::to_string(dev) +
+           " is current: set the arena with its device current");
   e->arena = static_cast<uint8_t*>(arena_dev);
+  e->device = dev;
   return 0;
 }
 int rs_unet_load_param(rs_engine* e, const char* name, const float* src, void* stream) {
@@ -1206,6 +1228,12 @@ int rs_plan_num_launches(const rs_plan* p) { return p ? p->launches : 0; }
 int rs_plan_bind(rs_plan* p, void* workspace_dev) {
   RS_CHECK(p && workspace_dev && (reinterpret_cast<uintptr_t>(workspace_dev) & 255) == 0, "workspace must be 256-byte aligned");
   RS_CHECK(p->e->arena != nullptr, "rs_unet_set_arena before binding a plan");
+  int dev = -1;
+  RS_CUDA_OK(cudaGetDevice(&dev));
+  RS_CHECK(dev == p->e->device, "bind a plan on the device its engine's arena was set on (cuda:" +
+                                std::to_string(p->e->device) + "), not cuda:" + std::to_string(dev));
+  RS_CHECK(!p->bound || dev == p->device, "a bound plan can be rebound on its own device only");
+  p->device = dev;
   p->ws = static_cast<uint8_t*>(workspace_dev);
   if (p->vq_which >= 0) {
     p->out_f32 = reinterpret_cast<float*>(p->ws + p->off_state);
@@ -1242,9 +1270,10 @@ int rs_plan_forward(rs_plan* p, const float* x, const float* timesteps, const fl
   RS_CHECK(p && p->bound, "plan is not bound");
   RS_CHECK(p->vq_which < 0, "this is a VQ-GAN plan: use rs_vq_encode / rs_vq_decode");
   RS_CHECK(x && timesteps && lq && out, "null tensor");
+  int rc = check_plan_device(*p); if (rc) return rc;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   p->table_owner = nullptr;                       // FiLM rows 0..B-1 are overwritten below
-  int rc = run_embedding(*p, timesteps, p->B, st); if (rc) return rc;
+  rc = run_embedding(*p, timesteps, p->B, st); if (rc) return rc;
   rc = pack_lq_and_input(*p, x, lq, mask, nullptr, 0, st); if (rc) return rc;
   const float* film = reinterpret_cast<const float*>(p->ws + p->off_film);
   rc = run_ops(*p, p->ops, film, p->e->film_rows, st); if (rc) return rc;
@@ -1261,9 +1290,10 @@ int rs_plan_forward(rs_plan* p, const float* x, const float* timesteps, const fl
 int rs_plan_profile(rs_plan* p, const float* x, const float* timesteps, const float* lq, const float* mask,
                     double* ms_by_kind, double* conv_flops, int32_t* n_conv_launches, void* stream) {
   RS_CHECK(p && p->bound && ms_by_kind && p->vq_which < 0, "bad argument (needs a bound denoiser plan)");
+  int rc = check_plan_device(*p); if (rc) return rc;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   p->table_owner = nullptr;
-  int rc = run_embedding(*p, timesteps, p->B, st); if (rc) return rc;
+  rc = run_embedding(*p, timesteps, p->B, st); if (rc) return rc;
   rc = pack_lq_and_input(*p, x, lq, mask, nullptr, 0, st); if (rc) return rc;
   Prof prof;
   const float* film = reinterpret_cast<const float*>(p->ws + p->off_film);
@@ -1342,9 +1372,10 @@ static void collect_profile(const rs_plan& P, const Prof& prof, double* ms, char
 int rs_plan_profile_ops(rs_plan* p, const float* x, const float* timesteps, const float* lq, const float* mask,
                         double* ms, char* desc, int desc_stride, int cap, int32_t* n_ops, void* stream) {
   RS_CHECK(p && p->bound && ms && desc && n_ops, "bad argument");
+  int rc = check_plan_device(*p); if (rc) return rc;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   p->table_owner = nullptr;
-  int rc = run_embedding(*p, timesteps, p->B, st); if (rc) return rc;
+  rc = run_embedding(*p, timesteps, p->B, st); if (rc) return rc;
   rc = pack_lq_and_input(*p, x, lq, mask, nullptr, 0, st); if (rc) return rc;
   Prof prof;
   const float* film = reinterpret_cast<const float*>(p->ws + p->off_film);
@@ -1365,6 +1396,7 @@ __global__ void probe_kernel(const __half* src, long long sN, int ld, float* dst
 
 int rs_plan_probe(rs_plan* p, const char* block, float* dst, int32_t* channels, int32_t* h, int32_t* w, void* stream) {
   RS_CHECK(p && p->bound && block, "bad argument");
+  if (dst) { int rc = check_plan_device(*p); if (rc) return rc; }
   auto it = p->block_out.find(block);
   RS_CHECK(it != p->block_out.end(), std::string("unknown block ") + block);
   const View& v = it->second;
@@ -1494,8 +1526,9 @@ int rs_sampler_set_taps(rs_sampler* s, float* pred, float* sample) {
 int rs_sampler_run(rs_sampler* s, const float* z_y, const float* noises, const float* lq, const float* mask,
                    float* out_latent, int use_graph, void* stream) {
   RS_CHECK(s && z_y && noises && lq && out_latent, "null argument");
+  int rc = check_plan_device(*s->p); if (rc) return rc;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  int rc = sampler_prepare(*s, st); if (rc) return rc;
+  rc = sampler_prepare(*s, st); if (rc) return rc;
   if (!use_graph) return sampler_enqueue(*s, z_y, noises, lq, mask, out_latent, st);
   if (s->graph && (s->g_zy != z_y || s->g_noise != noises || s->g_lq != lq || s->g_mask != mask || s->g_out != out_latent)) {
     cudaGraphExecDestroy(s->graph); s->graph = nullptr;
@@ -1530,6 +1563,7 @@ int rs_sampler_run_host(rs_sampler* s, const float* z_y_h, const float* noises_h
                         float* out_h, void* staging, size_t staging_bytes, int use_graph, void* stream) {
   RS_CHECK(s && z_y_h && noises_h && lq_h && out_h && staging, "null argument");
   RS_CHECK(staging_bytes >= rs_sampler_staging_bytes(s), "staging buffer too small");
+  { int rc = check_plan_device(*s->p); if (rc) return rc; }
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const rs_plan& P = *s->p;
   const rs_unet_config& c = P.e->cfg;

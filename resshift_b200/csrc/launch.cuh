@@ -2,9 +2,11 @@
 #pragma once
 
 #include <algorithm>
+#include <atomic>
 #include <cstdlib>
 #include <cmath>
 #include <cstring>
+#include <mutex>
 #include <utility>
 #include <vector>
 
@@ -25,15 +27,18 @@ typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_
                                     CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 
 inline PFN_encodeTiled get_encode_tiled() {
-  static PFN_encodeTiled fn = nullptr;
-  if (!fn) {
+  static std::atomic<PFN_encodeTiled> fn{nullptr};     // plans may be bound from several host threads at once
+  PFN_encodeTiled f = fn.load(std::memory_order_acquire);
+  if (!f) {
     void* p = nullptr;
     cudaDriverEntryPointQueryResult q;
     if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess &&
-        q == cudaDriverEntryPointSuccess)
-      fn = reinterpret_cast<PFN_encodeTiled>(p);
+        q == cudaDriverEntryPointSuccess) {
+      f = reinterpret_cast<PFN_encodeTiled>(p);
+      fn.store(f, std::memory_order_release);
+    }
   }
-  return fn;
+  return f;
 }
 
 // NHWC fp16 view descriptor used by the host code.
@@ -123,18 +128,22 @@ inline cudaError_t launch_k(void (*kernel)(KArgs...), dim3 grid, dim3 block, siz
   return launch_kc(kernel, grid, block, smem, st, 1, std::forward<Args>(args)...);
 }
 
+// per-device state of the library is indexed by the CUDA device ordinal
+constexpr int kMaxDevices = 64;
+
 // streaming multiprocessors of the current device (grid sizes of persistent kernels, the wave model of the cost
-// estimates), read once per device; host-only previews without a device assume an H100 SXM (132)
+// estimates), read once per device; host-only previews without a device assume an H100 SXM (132).  Threads driving
+// different devices may ask at the same time: every slot is written with the same value, atomically.
 inline int num_sms() {
-  static int cache[64] = {};
+  static std::atomic<int> cache[kMaxDevices] = {};
   int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) { (void)cudaGetLastError(); return 132; }
-  if (cache[dev] == 0) {
-    int n = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= kMaxDevices) { (void)cudaGetLastError(); return 132; }
+  int n = cache[dev].load(std::memory_order_relaxed);
+  if (n == 0) {
     if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) { (void)cudaGetLastError(); n = 132; }
-    cache[dev] = n;
+    cache[dev].store(n, std::memory_order_relaxed);
   }
-  return cache[dev];
+  return n;
 }
 
 // shared memory of the conv epilogue's staging area: msub output tiles + per-warp GroupNorm partials + arrival flag
@@ -492,9 +501,18 @@ inline int conv_finalize(ConvDesc& d) {
   return 0;
 }
 
-inline int conv_init() {   // once per process, outside any stream capture
-  static bool attr_set = false;
-  if (!attr_set) {
+// Raises the dynamic shared-memory limit of every large kernel.  The runtime keeps function attributes per device, so
+// this runs once on every device the library launches on (the current one), outside any stream capture; host threads
+// driving different devices may call it at the same time.
+inline int conv_init() {
+  static std::atomic<bool> attr_set[kMaxDevices] = {};
+  static std::mutex mu;
+  int dev = 0;
+  RS_CUDA_OK(cudaGetDevice(&dev));
+  RS_CHECK(dev >= 0 && dev < kMaxDevices, "device ordinal out of range");
+  if (attr_set[dev].load(std::memory_order_acquire)) return 0;
+  std::lock_guard<std::mutex> lock(mu);
+  if (!attr_set[dev].load(std::memory_order_relaxed)) {
     for (int bn : kConvBNs)
       for (int ms = 1; ms <= 2; ++ms)
         if (ConvKernelFn k = conv_kernel_for(bn, ms))
@@ -509,7 +527,7 @@ inline int conv_init() {   // once per process, outside any stream capture
     RS_CUDA_OK(cudaFuncSetAttribute(vq_attn_sm90_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, VqAttnSmem<128>::launch_bytes));
     RS_CUDA_OK(cudaFuncSetAttribute(vq_attn_sm90_kernel<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, VqAttnSmem<256>::launch_bytes));
     RS_CUDA_OK(cudaFuncSetAttribute(vq_attn_sm90_kernel<512>, cudaFuncAttributeMaxDynamicSharedMemorySize, VqAttnSmem<512>::launch_bytes));
-    attr_set = true;
+    attr_set[dev].store(true, std::memory_order_release);
   }
   return 0;
 }

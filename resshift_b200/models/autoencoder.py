@@ -84,7 +84,8 @@ class VQModelTorch(nn.Module):
             nbytes = _lib.lib.rs_unet_arena_bytes(self._engine)
             self._arena = torch.zeros(nbytes + 256, dtype=torch.uint8, device=device)
             self._arena_ptr = (self._arena.data_ptr() + 255) // 256 * 256
-            _lib.check(_lib.lib.rs_unet_set_arena(self._engine, self._arena_ptr))
+            with torch.cuda.device(device):                   # the engine belongs to the arena's device
+                _lib.check(_lib.lib.rs_unet_set_arena(self._engine, self._arena_ptr))
             self._packed_versions = None
             self._plans.clear()
         return self._engine

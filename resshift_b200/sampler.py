@@ -10,6 +10,8 @@ contiguous batch slices per rank (sampler.py:273-277), same seed on every rank; 
 broadcast the weights over NCCL (``broadcast_weights``) and results can be gathered (``gather_results``).
 ``shard_tiles=True`` deals the tiles of each chunk across the ranks instead, bit-identical to one GPU (DESIGN.md §6);
 a chunk with fewer units than ranks runs each unit on a team of ranks that splits its VQ-GAN bottleneck attention.
+``devices=`` (or ``RS_DEVICES``) does the same inside one process: a pool of model replicas, one per listed GPU, each
+driven by its own thread (resshift_b200.device_pool).
 """
 from __future__ import annotations
 
@@ -27,6 +29,7 @@ import torch
 import torch.distributed as dist
 import torch.nn.functional as F
 
+from .device_pool import DevicePool, Replica, pool_devices
 from .parallel import attention_teams, gather_counts, row_exchange, shard_range, team_group
 
 
@@ -239,15 +242,47 @@ class BaseSampler:
 
 class ResShiftSampler(BaseSampler):
     def __init__(self, configs, sf=4, use_amp=True, chop_size=128, chop_stride=128, chop_bs=1, padding_offset=16,
-                 seed=10000, shard_tiles=None):
+                 seed=10000, shard_tiles=None, devices=None):
         """``shard_tiles``: deal the tiles of each chunk of images across the ranks instead of slicing the chunk by
         image (``_run_shard``); ``None`` reads ``RS_SHARD_TILES`` (default 0), so unmodified reference scripts can turn
-        it on."""
+        it on.
+
+        ``devices``: run ``inference`` on a pool of GPUs from this one process: ``"all"``, ``"0,2,3"`` or a list of
+        indices; the first is the primary (models, noise, assembly, output).  ``None`` reads ``RS_DEVICES`` (unset: no
+        pool).  The same device may be listed more than once: every entry is one model replica with its own stream.
+        Refused with ``WORLD_SIZE > 1``, on devices that differ in SM count or compute capability, and for
+        configurations that take the generic per-step route."""
+        self.devices = pool_devices(devices)
         if shard_tiles is None:
             shard_tiles = os.environ.get("RS_SHARD_TILES", "0") not in ("", "0")
         self.shard_tiles = bool(shard_tiles)
-        super().__init__(configs, sf=sf, use_amp=use_amp, chop_size=chop_size, chop_stride=chop_stride, chop_bs=chop_bs,
-                         padding_offset=padding_offset, seed=seed)
+        with torch.cuda.device(self.devices[0]) if self.devices else nullcontext():
+            super().__init__(configs, sf=sf, use_amp=use_amp, chop_size=chop_size, chop_stride=chop_stride,
+                             chop_bs=chop_bs, padding_offset=padding_offset, seed=seed)
+        self.pool = self._build_pool() if self.devices else None
+
+    def _build_pool(self):
+        """One replica per entry of ``self.devices``: the first uses this sampler's models, every other one gets the
+        denoiser and the VQ-GAN built from the same configs on its device, with this sampler's parameters copied over
+        device to device (each replica owns its library handles; modules holding them are never deep-copied)."""
+        self._check_shardable("a device pool")
+        replicas = []
+        for k, d in enumerate(self.devices):
+            if k == 0:
+                model, autoencoder = self.model, self.autoencoder
+            else:
+                with torch.cuda.device(d):
+                    model = instantiate_from_config(self.configs.model).cuda(d)
+                    self.load_model(model, self.model.state_dict())
+                    self.freeze_model(model)
+                    model = model.eval()
+                    autoencoder = instantiate_from_config(self.configs.autoencoder).cuda(d)
+                    self.load_model(autoencoder, self.autoencoder.state_dict())
+                    autoencoder = autoencoder.eval()
+            replicas.append(Replica(k, d, model, autoencoder, primary=self.devices[0]))
+        for d in sorted(set(self.devices)):                       # the parameter copies
+            torch.cuda.synchronize(d)
+        return DevicePool(replicas)
 
     def sample_func(self, y0, noise_repeat=False, mask=False):
         """y0: [n, c, h, w] in [-1, 1] -> [n, c, h*sf, w*sf] in [-1, 1] (reference sampler.py:119-165)."""
@@ -378,18 +413,20 @@ class ResShiftSampler(BaseSampler):
         f = 2 ** (len(ae.ddconfig.ch_mult) - 1)
         return (n, int(ae.embed_dim), int(h * sf) // f, int(w * sf) // f), dtype
 
-    def _check_shardable(self):
+    def _check_shardable(self, mode="shard_tiles"):
         if not self.base_diffusion._native_ok(self.model, clip_denoised=(self.autoencoder is None), denoised_fn=None,
                                               model_kwargs={"lq": None}):
             raise RuntimeError(
-                "shard_tiles needs the fused sampling loop, whose noise can be drawn ahead of the encoder; this "
+                f"{mode} needs the fused sampling loop, whose noise can be drawn ahead of the encoder; this "
                 "configuration takes the generic per-step route (no autoencoder, a model other than this package's "
                 "UNetModelSwin, predict_type other than xstart, or T outside 2..64)")
 
-    def _sample_unit(self, y0, mask, noises, spec):
+    def _sample_unit(self, y0, mask, noises, spec, replica=None):
         """sample_func with its noise given: reflect-pad, encode_first_stage(up_sample=True), sample_latent(noises=),
         decode_first_stage, crop, clamp — the same steps, in the same order.  ``spec`` is the z_y shape and dtype the
-        noise was drawn for; it must be the real one."""
+        noise was drawn for; it must be the real one.  ``replica``: a device_pool.Replica whose models run the unit
+        (default: this sampler's)."""
+        model, autoencoder = (self.model, self.autoencoder) if replica is None else (replica.model, replica.autoencoder)
         offset = self.padding_offset
         ori_h, ori_w = y0.shape[2:]
         flag_pad = not (ori_h % offset == 0 and ori_w % offset == 0)
@@ -401,12 +438,12 @@ class ResShiftSampler(BaseSampler):
                 mask = F.pad(mask, pad=(0, pad_w, 0, pad_h), mode="reflect")
         model_kwargs = {"lq": y0} if mask is None else {"lq": y0, "mask": mask}
         diff = self.base_diffusion
-        z_y = diff.encode_first_stage(y0, self.autoencoder, up_sample=True)
+        z_y = diff.encode_first_stage(y0, autoencoder, up_sample=True)
         assert (tuple(z_y.shape), z_y.dtype, z_y.is_contiguous()) == (spec[0], spec[1], True), \
             f"derived z_y {spec} != real {tuple(z_y.shape)} {z_y.dtype}"
-        final = diff.sample_latent(z_y, self.model, model_kwargs, noises=noises)
+        final = diff.sample_latent(z_y, model, model_kwargs, noises=noises)
         with torch.no_grad():
-            results = diff.decode_first_stage(final, first_stage_model=self.autoencoder)
+            results = diff.decode_first_stage(final, first_stage_model=autoencoder)
         if flag_pad:
             results = results[:, :, :ori_h * self.sf, :ori_w * self.sf]
         return results.clamp_(-1.0, 1.0)
@@ -430,26 +467,57 @@ class ResShiftSampler(BaseSampler):
         tiles, else empty shares (a team member other than the first).  ``team``: (member, size, exchange) to run the
         units under the autoencoder's attention_team."""
         out = [[] for _ in lqs]
+        for i, noises, spec in self._unit_noises(lqs, noise_repeat, units):
+            if not a <= i < e:
+                continue
+            g = units[i][0]
+            pch, mch = self._unit_input(lqs, masks, units[i])
+            res = self._run_unit(pch, mch, noises, spec, team=team)
+            if keep:
+                out[g].extend(torch.split(res, lqs[g].shape[0], dim=0))
+        return self._stack_shares(out, lqs, units)
+
+    def _unit_noises(self, lqs, noise_repeat, units):
+        """Yields (unit index, noises, z_y spec) for every unit of ``units`` in order: its T+1 noise tensors drawn as
+        GaussianDiffusion.draw_noises does (after setup_seed with noise_repeat, as sample_func does), on the device of
+        ``lqs``, so that the CUDA generator is where a one-GPU run has it whichever units run here."""
         offset = self.padding_offset
         ctx = torch.autocast("cuda") if self.use_amp else nullcontext()
         for i, (g, starts, th, tw) in enumerate(units):
-            lq, mask = lqs[g], masks[g]
-            b = lq.shape[0]
+            lq = lqs[g]
             with ctx:
                 if noise_repeat:
                     self.setup_seed()
-                spec = self._latent_spec(b * len(starts), math.ceil(th / offset) * offset, math.ceil(tw / offset) * offset,
-                                         lq.dtype)
+                spec = self._latent_spec(lq.shape[0] * len(starts), math.ceil(th / offset) * offset,
+                                         math.ceil(tw / offset) * offset, lq.dtype)
                 noises = self.base_diffusion.draw_noises(torch.empty(spec[0], dtype=spec[1], device=lq.device),
                                                          noise_repeat=noise_repeat)
-                if not a <= i < e:
-                    continue
-                pch = torch.cat([lq[:, :, hs:hs + th, ws:ws + tw] for hs, ws in starts], dim=0)
-                mch = None if mask is None else torch.cat([mask[:, :, hs:hs + th, ws:ws + tw] for hs, ws in starts], dim=0)
-                with self.autoencoder.attention_team(*team) if team is not None else nullcontext():
-                    res = self._sample_unit(pch, mch, noises, spec).float()
-            if keep:
-                out[g].extend(torch.split(res, b, dim=0))
+            yield i, noises, spec
+
+    @staticmethod
+    def _unit_input(lqs, masks, unit):
+        """The LQ tiles (and mask tiles or None) of one unit stacked on the batch axis, as sample_func receives them."""
+        g, starts, th, tw = unit
+        lq, mask = lqs[g], masks[g]
+        pch = torch.cat([lq[:, :, hs:hs + th, ws:ws + tw] for hs, ws in starts], dim=0)
+        mch = None if mask is None else torch.cat([mask[:, :, hs:hs + th, ws:ws + tw] for hs, ws in starts], dim=0)
+        return pch, mch
+
+    def _run_unit(self, pch, mch, noises, spec, team=None, replica=None):
+        """One unit: _sample_unit under autocast (and under the autoencoder's attention_team with ``team``), as fp32.
+        ``replica``: the device_pool.Replica that runs it (its models, on the current device and stream)."""
+        autoencoder = self.autoencoder if replica is None else replica.autoencoder
+        ctx = torch.autocast("cuda") if self.use_amp else nullcontext()
+        with ctx:
+            with autoencoder.attention_team(*team) if team is not None else nullcontext():
+                # shard mode keeps its four-argument call: code that wraps _sample_unit (e.g. to count the units a
+                # rank runs) sees the same call as before the pool existed; only pool units name their replica
+                if replica is None:
+                    return self._sample_unit(pch, mch, noises, spec).float()
+                return self._sample_unit(pch, mch, noises, spec, replica).float()
+
+    def _stack_shares(self, out, lqs, units):
+        """Per group, the tiles of ``out[g]`` stacked [n, b, 3, th*sf, tw*sf] (n may be 0)."""
         tile_hw = {g: (th, tw) for g, _, th, tw in units}
         return [torch.stack(t) if t else
                 torch.empty((0,) + tuple(lq.shape[:2]) + (tile_hw[g][0] * self.sf, tile_hw[g][1] * self.sf), device=lq.device)
@@ -506,7 +574,8 @@ class ResShiftSampler(BaseSampler):
 
     def inference(self, in_path, out_path, mask_path=None, mask_back=True, bs=1, noise_repeat=False):
         """File / folder driver (reference sampler.py:167-308).  Image I/O through OpenCV.  With ``shard_tiles`` every
-        rank reads the whole chunk and runs its share of the chunk's tiles (_run_shard); rank 0 assembles and writes."""
+        rank reads the whole chunk and runs its share of the chunk's tiles (_run_shard); rank 0 assembles and writes.
+        With a device pool the chunk's units run on the pool's replicas (_inference_pool)."""
         import cv2
         if self.shard_tiles:
             self._check_shardable()
@@ -538,7 +607,9 @@ class ResShiftSampler(BaseSampler):
 
         for i0 in range(0, len(files), bs):
             chunk = files[i0:i0 + bs]
-            if self.shard_tiles:
+            if self.pool is not None:
+                self._inference_pool(_same_shape_groups(chunk, read), read_group, out_path, mask_back, noise_repeat)
+            elif self.shard_tiles:
                 self._inference_shards(_same_shape_groups(chunk, read), read_group, out_path, mask_back, noise_repeat)
             else:
                 micro = math.ceil(bs / self.num_gpus)                     # reference sampler.py:273-277
@@ -555,14 +626,7 @@ class ResShiftSampler(BaseSampler):
     def _inference_shards(self, groups, read_group, out_path, mask_back, noise_repeat):
         """One chunk in shard_tiles mode: this rank's tiles (its own units, or with fewer units than ranks its team's
         unit), one gather per shape group, assembly and writing on rank 0."""
-        import cv2
-        paths, lqs, masks = [], [], []
-        for group in groups:
-            p, lq_u8, mask_u8 = read_group(group)
-            lq, mask = self._ingest_u8(lq_u8, mask_u8)
-            paths.append(p)
-            lqs.append(lq)
-            masks.append(mask)
+        paths, lqs, masks = self._read_chunk(groups, read_group)
         shapes = [tuple(lq.shape[2:]) for lq in lqs]
         # fewer units than ranks: teams of ranks share each unit's bottleneck attention instead of leaving ranks idle
         teams = self.num_gpus > 1 and dist.is_initialized() and hasattr(self.autoencoder, "attention_team") and \
@@ -577,9 +641,38 @@ class ResShiftSampler(BaseSampler):
             tiles = gather_counts(shares[g], counts[g])
             if self.rank != 0:
                 continue
-            sr = self._emit_u8(self._assemble(tiles, *lq.shape[2:]), lq, masks[g], mask_back=mask_back, bgr=True)
-            for p, im in zip(paths[g], sr.cpu().numpy()):
-                cv2.imwrite(str(out_path / f"{p.stem}.png"), im)
+            self._write_group(paths[g], tiles, lq, masks[g], out_path, mask_back)
+
+    def _inference_pool(self, groups, read_group, out_path, mask_back, noise_repeat):
+        """One chunk on the device pool: read and ingest on the primary, every unit's noise drawn there in one-GPU
+        order, the units run on the replicas (device_pool.DevicePool.run), then assembly and writing on the primary."""
+        with torch.cuda.device(self.pool.primary):
+            paths, lqs, masks = self._read_chunk(groups, read_group)
+            units = self._plan_units([tuple(lq.shape[2:]) for lq in lqs])
+            out = [[] for _ in lqs]
+            for (g, _, _, _), res in zip(units, self.pool.run(self, lqs, masks, noise_repeat, units)):
+                out[g].extend(torch.split(res, lqs[g].shape[0], dim=0))
+            for g, (tiles, lq) in enumerate(zip(self._stack_shares(out, lqs, units), lqs)):
+                self._write_group(paths[g], tiles, lq, masks[g], out_path, mask_back)
+
+    def _read_chunk(self, groups, read_group):
+        """Per shape group of a chunk: the paths, the LQ images [b, 3, h, w] and the masks [b, 1, h, w] or None, in
+        [-1, 1] on the current device."""
+        paths, lqs, masks = [], [], []
+        for group in groups:
+            p, lq_u8, mask_u8 = read_group(group)
+            lq, mask = self._ingest_u8(lq_u8, mask_u8)
+            paths.append(p)
+            lqs.append(lq)
+            masks.append(mask)
+        return paths, lqs, masks
+
+    def _write_group(self, paths, tiles, lq, mask, out_path, mask_back):
+        """Assembles one shape group from all its tiles (plan order) and writes its PNGs."""
+        import cv2
+        sr = self._emit_u8(self._assemble(tiles, *lq.shape[2:]), lq, mask, mask_back=mask_back, bgr=True)
+        for p, im in zip(paths, sr.cpu().numpy()):
+            cv2.imwrite(str(out_path / f"{p.stem}.png"), im)
 
 
 def _same_shape_groups(paths, read):
