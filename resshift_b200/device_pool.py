@@ -5,9 +5,9 @@ Every entry of the pool is a replica: a copy of the denoiser and the VQ-GAN on o
 plans and CUDA stream, driven by its own host thread.  The sampler's main thread walks the work units of a chunk in
 one-GPU order and draws each unit's noise on the primary device (the first entry), exactly as a one-GPU run does; the
 units then run on whichever replica is free.  A unit's output does not depend on the device that runs it, so the tiles
-that come back to the primary are the one-GPU tiles.  With fewer units than replicas, each unit runs on a team of
-replicas that splits its VQ-GAN bottleneck attention (``parallel.attention_teams``); the rows are exchanged in process
-by ``TeamExchange``.
+that come back to the primary are the one-GPU tiles.  With fewer units than replicas, the chunk's schedule
+(``parallel.unit_schedule``) runs each unit on a team of replicas that splits its VQ-GAN bottleneck attention; the rows
+are exchanged in process by ``TeamExchange``.
 
 The library's kernels pick their tile configurations from the device's SM count, so a pool refuses devices that differ
 in SM count or compute capability.
@@ -22,7 +22,7 @@ from typing import Callable, List, Optional, Sequence
 
 import torch
 
-from .parallel import attention_row_ranges, attention_teams
+from .parallel import attention_row_ranges
 
 
 def parse_devices(spec, count: int) -> List[int]:
@@ -189,14 +189,15 @@ class DevicePool:
     def run(self, sampler, lqs, masks, noise_repeat, units):
         """Runs every unit of ``units`` (ResShiftSampler._plan_units of the chunk ``lqs`` / ``masks`` on the primary
         device) and returns, per unit, its output [n * b, 3, th*sf, tw*sf] on the primary device.  Noise is drawn here,
-        on the calling thread, in unit order (ResShiftSampler._unit_noises); a unit goes to the next free replica, or
-        with fewer units than replicas to every member of its team.  An exception in any worker stops the others and
-        is raised here."""
+        on the calling thread, in unit order (ResShiftSampler._unit_noises); a unit goes to the next free replica, or,
+        when the chunk's schedule (ResShiftSampler._schedule) has teams, to every member of its team.  An exception in
+        any worker stops the others and is raised here."""
         n = len(self.replicas)
-        teams = attention_teams(len(units), n)
+        schedule = sampler._schedule(len(units), n)
+        teams = any(e - a > 1 for a, e in schedule)
         stop = threading.Event()
         errors: List[BaseException] = []
-        exchanges = [TeamExchange(e - a) for a, e in teams] if teams is not None else []
+        exchanges = [TeamExchange(e - a) for a, e in schedule] if teams else []
         lock = threading.Lock()
 
         def fail(exc):
@@ -206,10 +207,10 @@ class DevicePool:
             for x in exchanges:
                 x.barrier.abort()
 
-        if teams is None:                                       # deal units to whichever replica is free
+        if not teams:                                           # deal units to whichever replica is free
             shared = queue.Queue(maxsize=2 * n)
             inboxes = [shared] * n
-        else:                                                   # team u runs unit u
+        else:                                                   # unit u runs on its team's replicas
             inboxes = [queue.Queue() for _ in range(n)]
         results: List[Optional[tuple]] = [None] * len(units)      # (output on the primary, event completing it)
         threads = [threading.Thread(target=self._work, args=(r, sampler, inboxes[r], results, stop, fail),
@@ -224,13 +225,12 @@ class DevicePool:
                 pch, mch = sampler._unit_input(lqs, masks, units[i])
                 ready = torch.cuda.Event()
                 ready.record(main_stream)
-                if teams is None:
+                if not teams:
                     _put(shared, _Job(i, pch, mch, noises, spec, ready), stop)
                     continue
-                a, e = teams[i]
-                exchange = exchanges[i]
+                a, e = schedule[i]
                 for r in range(a, e):
-                    team = (r - a, e - a, exchange.member(r - a)) if e - a > 1 else None
+                    team = (r - a, e - a, exchanges[i].member(r - a)) if e - a > 1 else None
                     inboxes[r].put(_Job(i, pch, mch, noises, spec, ready, team, keep=r == a))
             for r in range(n):
                 if not _put(inboxes[r], None, stop):

@@ -5,8 +5,8 @@ the T-step loop communicates.  Partitioning is the reference's (contiguous slice
 ceil(bs / world) per rank, reference sampler.py:273-277).  Collectives go through ``torch.distributed``
 (NCCL over NVLink on the GPU box, gloo in the CPU tests) — a broadcast of the flattened weights from
 rank 0 at start-up and an all-gather of the result shards at the end.  Tile sharding
-(``ResShiftSampler(shard_tiles=True)``) deals the tiles of a chunk instead and gathers them with ``gather_counts``;
-when a chunk has fewer units than ranks, each unit goes to a team of ranks (``attention_teams``) that splits the
+(``ResShiftSampler(shard_tiles=True)``) deals the tiles of a chunk instead, by ``unit_schedule``, and gathers them with
+``gather_counts``; when a chunk has fewer units than ranks, the schedule gives each unit a team of ranks that splits the
 VQ-GAN bottleneck attention's query rows and exchanges them (``row_exchange``).
 """
 from __future__ import annotations
@@ -41,19 +41,8 @@ def broadcast_state_dict(sd: Dict[str, torch.Tensor], src: int = 0) -> None:
 
 def gather_shards(local: torch.Tensor, batch: int) -> torch.Tensor:
     """All-gather variable-length shards (padded to ceil(batch/world)) and return the global batch."""
-    if not (dist.is_available() and dist.is_initialized()) or dist.get_world_size() == 1:
-        return local
-    world, rank = dist.get_world_size(), dist.get_rank()
-    micro = math.ceil(batch / world)
-    pad = torch.zeros((micro,) + tuple(local.shape[1:]), dtype=local.dtype, device=local.device)
-    pad[:local.shape[0]] = local
-    outs: List[torch.Tensor] = [torch.empty_like(pad) for _ in range(world)]
-    dist.all_gather(outs, pad)
-    parts = []
-    for r in range(world):
-        s, e = shard_range(batch, world, r)
-        parts.append(outs[r][:e - s])
-    return torch.cat(parts, dim=0)
+    world = dist.get_world_size() if dist.is_available() and dist.is_initialized() else 1
+    return gather_counts(local, [e - s for s, e in (shard_range(batch, world, r) for r in range(world))])
 
 
 def gather_counts(local: torch.Tensor, counts: List[int]) -> torch.Tensor:
@@ -85,6 +74,15 @@ def attention_teams(n_units: int, world: int) -> Optional[List[Tuple[int, int]]]
         teams.append((start, start + size))
         start += size
     return teams
+
+
+def unit_schedule(n_units: int, world: int, teams: bool) -> List[Tuple[int, int]]:
+    """The executors (ranks, or a device pool's replicas) [a, e) that run each of a chunk's ``n_units`` work units;
+    executor a keeps the unit's tiles.  With ``teams`` and fewer units than executors, the attention_teams partition;
+    otherwise the units dealt as contiguous shard_range ranges, one executor each."""
+    if teams and 0 < n_units < world:
+        return attention_teams(n_units, world)
+    return [(r, r + 1) for r in range(world) for _ in range(*shard_range(n_units, world, r))]
 
 
 def attention_row_ranges(n_rows: int, size: int) -> List[Tuple[int, int]]:

@@ -30,7 +30,7 @@ import torch.distributed as dist
 import torch.nn.functional as F
 
 from .device_pool import DevicePool, Replica, pool_devices
-from .parallel import attention_teams, gather_counts, row_exchange, shard_range, team_group
+from .parallel import gather_counts, row_exchange, team_group, unit_schedule
 
 
 # --------------------------------------------------------------------------------------------------
@@ -157,6 +157,15 @@ def plan_tiles(h: int, w: int, patch: int, stride: int, chop_bs: int):
     return hs_list, ws_list, min(patch, h), min(patch, w), [starts[i:i + k] for i in range(0, len(starts), k)]
 
 
+def tile_counts(units, schedule, world: int):
+    """counts[g][r]: tiles of shape group g that executor r keeps, for ResShiftSampler._plan_units ``units`` run by
+    ``schedule`` (parallel.unit_schedule) — what parallel.gather_counts needs on every rank."""
+    counts = [[0] * world for _ in range(units[-1][0] + 1)]
+    for (g, starts, _, _), (a, _) in zip(units, schedule):
+        counts[g][a] += len(starts)
+    return counts
+
+
 class BaseSampler:
     def __init__(self, configs, sf=4, use_amp=True, chop_size=128, chop_stride=128, chop_bs=1, padding_offset=16,
                  seed=10000):
@@ -193,20 +202,27 @@ class BaseSampler:
 
     def build_model(self):
         self.base_diffusion = instantiate_from_config(self.configs.diffusion)
-        model = instantiate_from_config(self.configs.model).cuda()
         ckpt = self.configs.model.ckpt_path
         assert ckpt is not None
+        ae_cfg = self.configs.get("autoencoder", None)
+        ae_ckpt = None if ae_cfg is None else ae_cfg.get("ckpt_path", None)
+        self.model, self.autoencoder = self._instantiate_models(ckpt, ae_ckpt)
+
+    def _instantiate_models(self, ckpt, ae_ckpt):
+        """The denoiser (frozen) and the autoencoder (None when the configs have none) of the configs on the current
+        device, in eval mode, with the checkpoints ``ckpt`` / ``ae_ckpt`` (a path or a state dict; ``ae_ckpt`` may be
+        None) loaded."""
+        model = instantiate_from_config(self.configs.model).cuda()
         self.load_model(model, ckpt)
         self.freeze_model(model)
-        self.model = model.eval()
+        model.eval()
+        autoencoder = None
         if self.configs.get("autoencoder", None) is not None:
-            ae_cfg = self.configs.autoencoder
-            autoencoder = instantiate_from_config(ae_cfg).cuda()
-            if ae_cfg.get("ckpt_path", None) is not None:
-                self.load_model(autoencoder, ae_cfg.ckpt_path)
-            self.autoencoder = autoencoder.eval()
-        else:
-            self.autoencoder = None
+            autoencoder = instantiate_from_config(self.configs.autoencoder).cuda()
+            if ae_ckpt is not None:
+                self.load_model(autoencoder, ae_ckpt)
+            autoencoder.eval()
+        return model, autoencoder
 
     def load_model(self, model, ckpt_path):
         if isinstance(ckpt_path, dict):
@@ -244,7 +260,7 @@ class ResShiftSampler(BaseSampler):
     def __init__(self, configs, sf=4, use_amp=True, chop_size=128, chop_stride=128, chop_bs=1, padding_offset=16,
                  seed=10000, shard_tiles=None, devices=None):
         """``shard_tiles``: deal the tiles of each chunk of images across the ranks instead of slicing the chunk by
-        image (``_run_shard``); ``None`` reads ``RS_SHARD_TILES`` (default 0), so unmodified reference scripts can turn
+        image (``_run_rank``); ``None`` reads ``RS_SHARD_TILES`` (default 0), so unmodified reference scripts can turn
         it on.
 
         ``devices``: run ``inference`` on a pool of GPUs from this one process: ``"all"``, ``"0,2,3"`` or a list of
@@ -256,6 +272,7 @@ class ResShiftSampler(BaseSampler):
         if shard_tiles is None:
             shard_tiles = os.environ.get("RS_SHARD_TILES", "0") not in ("", "0")
         self.shard_tiles = bool(shard_tiles)
+        self._team_groups = {}                  # rank tuple -> process group of an attention team (parallel.team_group)
         with torch.cuda.device(self.devices[0]) if self.devices else nullcontext():
             super().__init__(configs, sf=sf, use_amp=use_amp, chop_size=chop_size, chop_stride=chop_stride,
                              chop_bs=chop_bs, padding_offset=padding_offset, seed=seed)
@@ -272,13 +289,7 @@ class ResShiftSampler(BaseSampler):
                 model, autoencoder = self.model, self.autoencoder
             else:
                 with torch.cuda.device(d):
-                    model = instantiate_from_config(self.configs.model).cuda(d)
-                    self.load_model(model, self.model.state_dict())
-                    self.freeze_model(model)
-                    model = model.eval()
-                    autoencoder = instantiate_from_config(self.configs.autoencoder).cuda(d)
-                    self.load_model(autoencoder, self.autoencoder.state_dict())
-                    autoencoder = autoencoder.eval()
+                    model, autoencoder = self._instantiate_models(self.model.state_dict(), self.autoencoder.state_dict())
             replicas.append(Replica(k, d, model, autoencoder, primary=self.devices[0]))
         for d in sorted(set(self.devices)):                       # the parameter copies
             torch.cuda.synchronize(d)
@@ -288,6 +299,15 @@ class ResShiftSampler(BaseSampler):
         """y0: [n, c, h, w] in [-1, 1] -> [n, c, h*sf, w*sf] in [-1, 1] (reference sampler.py:119-165)."""
         if noise_repeat:
             self.setup_seed()
+        if mask is False:      # reference quirk (`mask=False` default is "not None"); real callers pass None
+            mask = None
+        return self._pad_crop(y0, mask, lambda y, model_kwargs: self.base_diffusion.p_sample_loop(
+            y=y, model=self.model, first_stage_model=self.autoencoder, noise=None, noise_repeat=noise_repeat,
+            clip_denoised=(self.autoencoder is None), denoised_fn=None, model_kwargs=model_kwargs, progress=False))
+
+    def _pad_crop(self, y0, mask, run):
+        """``run(y0, model_kwargs)`` on y0 (and mask) reflect-padded to multiples of padding_offset, its result cropped to
+        the input's size times sf and clamped to [-1, 1] (reference sampler.py:130-165)."""
         offset = self.padding_offset
         ori_h, ori_w = y0.shape[2:]
         flag_pad = not (ori_h % offset == 0 and ori_w % offset == 0)
@@ -295,18 +315,15 @@ class ResShiftSampler(BaseSampler):
             pad_h = math.ceil(ori_h / offset) * offset - ori_h
             pad_w = math.ceil(ori_w / offset) * offset - ori_w
             y0 = F.pad(y0, pad=(0, pad_w, 0, pad_h), mode="reflect")
-            if mask is not None and mask is not False:
+            if mask is not None:
                 mask = F.pad(mask, pad=(0, pad_w, 0, pad_h), mode="reflect")
-        if mask is False:      # reference quirk (`mask=False` default is "not None"); real callers pass None
-            mask = None
-        model_kwargs = {"lq": y0} if mask is None else {"lq": y0, "mask": mask}
-        results = self.base_diffusion.p_sample_loop(
-            y=y0, model=self.model, first_stage_model=self.autoencoder, noise=None, noise_repeat=noise_repeat,
-            clip_denoised=(self.autoencoder is None), denoised_fn=None, model_kwargs=model_kwargs,
-            progress=False)
+        results = run(y0, {"lq": y0} if mask is None else {"lq": y0, "mask": mask})
         if flag_pad:
             results = results[:, :, :ori_h * self.sf, :ori_w * self.sf]
         return results.clamp_(-1.0, 1.0)
+
+    def _autocast(self):
+        return torch.autocast("cuda") if self.use_amp else nullcontext()
 
     # ---------------------------------------------------------------------------------------------
     def _sample_tiled(self, im_lq, mask=None, noise_repeat=False):
@@ -315,94 +332,67 @@ class ResShiftSampler(BaseSampler):
         are stacked on the batch axis per call exactly like ImageSpliterTh.__next__ (:940-960, `extra_bs`) — so the
         noise drawn per call matches the reference's — and overlaps are averaged (update / gather :962-979) by
         rs_op_tile_gather in the reference's accumulation order."""
-        ctx = torch.autocast("cuda") if self.use_amp else nullcontext()
         b, c, h, w = im_lq.shape
-        if not (h > self.chop_size or w > self.chop_size):
-            with ctx:
+        if self._one_tile(h, w):
+            with self._autocast():
                 return self.sample_func(im_lq, noise_repeat=noise_repeat, mask=mask).float()
-        _, _, th, tw, groups = plan_tiles(h, w, self.chop_size, self.chop_stride, self.chop_bs)
         tiles = []
-        for group in groups:
-            pch = torch.cat([im_lq[:, :, hs:hs + th, ws:ws + tw] for hs, ws in group], dim=0)
-            mch = None if mask is None else torch.cat([mask[:, :, hs:hs + th, ws:ws + tw] for hs, ws in group], dim=0)
-            with ctx:
+        for unit in self._plan_units([(h, w)]):
+            pch, mch = self._unit_input([im_lq], [mask], unit)
+            with self._autocast():
                 res = self.sample_func(pch, noise_repeat=noise_repeat, mask=mch).float()
             tiles.extend(torch.split(res, b, dim=0))
-        return self._overlap_average(torch.stack(tiles), h, w)
+        return self._assemble(torch.stack(tiles), h, w)
 
-    def _overlap_average(self, tiles, h, w):
-        """tiles [T, b, c, th*sf, tw*sf] of an [b, c, h, w] input, in plan_tiles order -> [b, c, h*sf, w*sf]: overlaps
-        averaged by rs_op_tile_gather in the reference's accumulation order."""
-        from . import _lib
-        sf = self.sf
-        hs_list, ws_list, th, tw, _ = plan_tiles(h, w, self.chop_size, self.chop_stride, self.chop_bs)
-        tiles_t = tiles.contiguous()
-        b = tiles_t.shape[1]
-        out = torch.empty(b, tiles_t.shape[2], h * sf, w * sf, dtype=torch.float32, device=tiles_t.device)
-        ys = torch.tensor([v * sf for v in hs_list], dtype=torch.int32, device=tiles_t.device)
-        xs = torch.tensor([v * sf for v in ws_list], dtype=torch.int32, device=tiles_t.device)
-        _lib.check(_lib.lib.rs_op_tile_gather(tiles_t.data_ptr(), b, tiles_t.shape[2], h * sf, w * sf, th * sf, tw * sf,
-                                              len(hs_list), len(ws_list), ys.data_ptr(), xs.data_ptr(), out.data_ptr(),
-                                              _lib.current_stream()))
-        return out
+    def _one_tile(self, h, w):
+        """Whether an [h, w] input runs whole, in one sample_func call, rather than tiled (reference sampler.py:186)."""
+        return not (h > self.chop_size or w > self.chop_size)
 
-    # -- tile sharding: the sample_func calls of a chunk dealt across ranks, bit-identical to one GPU ----------------
+    # -- the sample_func calls of a chunk as work units, scheduled across ranks or replicas, bit-identical to one GPU --
     def _plan_units(self, shapes):
         """Work units of a chunk whose shape groups have LQ sizes ``shapes`` [(h, w)], in the order a one-GPU run makes
         its sample_func calls: (group, tile starts, tile h, tile w).  An image that fits in one tile is one unit with
         the single start (0, 0)."""
         units = []
         for g, (h, w) in enumerate(shapes):
-            if h > self.chop_size or w > self.chop_size:
-                _, _, th, tw, groups = plan_tiles(h, w, self.chop_size, self.chop_stride, self.chop_bs)
-                units += [(g, starts, th, tw) for starts in groups]
-            else:
-                units.append((g, [(0, 0)], h, w))
+            _, _, th, tw, groups = plan_tiles(h, w, self.chop_size, self.chop_stride, self.chop_bs)
+            units += [(g, starts, th, tw) for starts in groups]
         return units
 
-    def _share_counts(self, shapes, world):
-        """counts[g][r]: tiles of shape group g that rank r runs (what parallel.gather_counts needs on every rank)."""
-        units = self._plan_units(shapes)
-        counts = [[0] * world for _ in shapes]
-        for r in range(world):
-            a, e = shard_range(len(units), world, r)
-            for g, starts, _, _ in units[a:e]:
-                counts[g][r] += len(starts)
-        return counts
+    def _schedule(self, n_units, world):
+        """parallel.unit_schedule of a chunk of ``n_units`` units on ``world`` executors.  Teams need executors that can
+        exchange attention rows (the ranks of a process group, or a pool's replicas in process) and an autoencoder that
+        can split its attention (VQModelTorch.attention_team)."""
+        teams = (self.pool is not None or dist.is_initialized()) and hasattr(self.autoencoder, "attention_team")
+        return unit_schedule(n_units, world, teams)
 
-    def _gather_counts(self, shapes, world):
-        """counts[g][r]: tiles of shape group g that rank r contributes to the gather.  With fewer units than ranks,
-        unit u is run by team u of parallel.attention_teams and only the team's first rank contributes its tiles;
-        otherwise _share_counts."""
-        units = self._plan_units(shapes)
-        teams = attention_teams(len(units), world)
-        if teams is None:
-            return self._share_counts(shapes, world)
-        counts = [[0] * world for _ in shapes]
-        for (g, starts, _, _), (first, _) in zip(units, teams):
-            counts[g][first] += len(starts)
-        return counts
-
-    def _run_team(self, lqs, masks, noise_repeat, world, rank):
-        """This rank's part of a chunk with fewer units than ranks: the rank runs its team's unit (team u runs unit u,
-        parallel.attention_teams) with the VQ-GAN bottleneck attention's query rows split across the team and exchanged
-        inside the team's process group, so every member ends with the whole unit, bit-identical to one GPU.  Noise is
-        drawn for every unit as _run_shard does.  Returns per group the tiles this rank contributes to the gather (the
-        team's first rank: the unit's tiles; the others: none).  Every rank of the default group must call this."""
+    def _run_rank(self, lqs, masks, noise_repeat, units, schedule, rank):
+        """One rank's part of a chunk in shard mode.  ``lqs`` / ``masks``: per shape group, [b, 3, h, w] in [-1, 1] and
+        [b, 1, h, w] or None; ``units``: their _plan_units; ``schedule``: the executors [a, e) of each unit
+        (_schedule).  The rank walks every unit and draws its noise (_unit_noises), so the CUDA generator is where a
+        one-GPU run has it, and runs the units whose range contains ``rank``: under the autoencoder's attention_team
+        when the range has more than one rank, with the query rows exchanged inside the team's process group, so every
+        member ends with the whole unit.  Nothing else in the chain draws random numbers.  Returns, per group, the tiles
+        of the units this rank keeps (rank == a) [n, b, 3, th*sf, tw*sf] in plan order (n may be 0).  With teams in the
+        schedule every rank of the default group must call this."""
         self._check_shardable()
-        units = self._plan_units([tuple(lq.shape[2:]) for lq in lqs])
-        teams = attention_teams(len(units), world)
-        groups = self.__dict__.setdefault("_team_groups", {})
-        for first, end in teams:                     # every rank creates every multi-rank team's group, in team order
-            if end - first > 1:
-                team_group(tuple(range(first, end)), groups)
-        u = next(i for i, (first, end) in enumerate(teams) if first <= rank < end)
-        first, end = teams[u]
-        team = None
-        if end - first > 1:
-            member, size = rank - first, end - first
-            team = (member, size, row_exchange(team_group(tuple(range(first, end)), groups), size, member))
-        return self._run_units(lqs, masks, noise_repeat, units, u, u + 1, keep=rank == first, team=team)
+        if any(lq is None for lq in lqs):
+            raise ValueError("shard_tiles needs the LQ image of every group")
+        for a, e in schedule:                        # every rank creates every multi-rank team's group, in team order
+            if e - a > 1:
+                team_group(tuple(range(a, e)), self._team_groups)
+        kept = [None] * len(units)
+        for i, noises, spec in self._unit_noises(lqs, noise_repeat, units):
+            a, e = schedule[i]
+            if not a <= rank < e:
+                continue
+            team = None
+            if e - a > 1:
+                team = (rank - a, e - a, row_exchange(team_group(tuple(range(a, e)), self._team_groups), e - a, rank - a))
+            res = self._run_unit(*self._unit_input(lqs, masks, units[i]), noises, spec, team=team)
+            if rank == a:
+                kept[i] = res
+        return self._stack_shares(kept, lqs, units)
 
     def _latent_spec(self, n, h, w, dtype):
         """Shape and dtype of z_y = encode_first_stage(y, up_sample=True) for an [n, 3, h, w] input (after the
@@ -421,71 +411,31 @@ class ResShiftSampler(BaseSampler):
                 "configuration takes the generic per-step route (no autoencoder, a model other than this package's "
                 "UNetModelSwin, predict_type other than xstart, or T outside 2..64)")
 
-    def _sample_unit(self, y0, mask, noises, spec, replica=None):
+    def _sample_unit(self, y0, mask, noises, spec, replica):
         """sample_func with its noise given: reflect-pad, encode_first_stage(up_sample=True), sample_latent(noises=),
         decode_first_stage, crop, clamp — the same steps, in the same order.  ``spec`` is the z_y shape and dtype the
-        noise was drawn for; it must be the real one.  ``replica``: a device_pool.Replica whose models run the unit
-        (default: this sampler's)."""
+        noise was drawn for; it must be the real one.  ``replica``: a device_pool.Replica whose models run the unit, or
+        None for this sampler's."""
         model, autoencoder = (self.model, self.autoencoder) if replica is None else (replica.model, replica.autoencoder)
-        offset = self.padding_offset
-        ori_h, ori_w = y0.shape[2:]
-        flag_pad = not (ori_h % offset == 0 and ori_w % offset == 0)
-        if flag_pad:
-            pad_h = math.ceil(ori_h / offset) * offset - ori_h
-            pad_w = math.ceil(ori_w / offset) * offset - ori_w
-            y0 = F.pad(y0, pad=(0, pad_w, 0, pad_h), mode="reflect")
-            if mask is not None:
-                mask = F.pad(mask, pad=(0, pad_w, 0, pad_h), mode="reflect")
-        model_kwargs = {"lq": y0} if mask is None else {"lq": y0, "mask": mask}
         diff = self.base_diffusion
-        z_y = diff.encode_first_stage(y0, autoencoder, up_sample=True)
-        assert (tuple(z_y.shape), z_y.dtype, z_y.is_contiguous()) == (spec[0], spec[1], True), \
-            f"derived z_y {spec} != real {tuple(z_y.shape)} {z_y.dtype}"
-        final = diff.sample_latent(z_y, model, model_kwargs, noises=noises)
-        with torch.no_grad():
-            results = diff.decode_first_stage(final, first_stage_model=autoencoder)
-        if flag_pad:
-            results = results[:, :, :ori_h * self.sf, :ori_w * self.sf]
-        return results.clamp_(-1.0, 1.0)
 
-    def _run_shard(self, lqs, masks, noise_repeat, world, rank):
-        """One rank's share of a chunk.  ``lqs`` / ``masks``: per shape group, [b, 3, h, w] in [-1, 1] and
-        [b, 1, h, w] or None.  The units of _plan_units are dealt as contiguous ranges (parallel.shard_range); every
-        rank walks all of them and draws each unit's T+1 noise tensors as GaussianDiffusion.draw_noises does (after
-        setup_seed with noise_repeat, as sample_func does), so the CUDA generator is where a one-GPU run has it, and runs
-        only its own units.  Nothing else in the chain draws random numbers.  Returns, per group, this rank's tiles
-        [n, b, 3, th*sf, tw*sf] in plan order (n may be 0)."""
-        self._check_shardable()
-        if any(lq is None for lq in lqs):
-            raise ValueError("shard_tiles needs the LQ image of every group")
-        units = self._plan_units([tuple(lq.shape[2:]) for lq in lqs])
-        a, e = shard_range(len(units), world, rank)
-        return self._run_units(lqs, masks, noise_repeat, units, a, e)
-
-    def _run_units(self, lqs, masks, noise_repeat, units, a, e, keep=True, team=None):
-        """Walks every unit of ``units``, drawing its noise, and runs units [a, e) (_run_shard).  ``keep``: return their
-        tiles, else empty shares (a team member other than the first).  ``team``: (member, size, exchange) to run the
-        units under the autoencoder's attention_team."""
-        out = [[] for _ in lqs]
-        for i, noises, spec in self._unit_noises(lqs, noise_repeat, units):
-            if not a <= i < e:
-                continue
-            g = units[i][0]
-            pch, mch = self._unit_input(lqs, masks, units[i])
-            res = self._run_unit(pch, mch, noises, spec, team=team)
-            if keep:
-                out[g].extend(torch.split(res, lqs[g].shape[0], dim=0))
-        return self._stack_shares(out, lqs, units)
+        def run(y, model_kwargs):
+            z_y = diff.encode_first_stage(y, autoencoder, up_sample=True)
+            assert (tuple(z_y.shape), z_y.dtype, z_y.is_contiguous()) == (spec[0], spec[1], True), \
+                f"derived z_y {spec} != real {tuple(z_y.shape)} {z_y.dtype}"
+            final = diff.sample_latent(z_y, model, model_kwargs, noises=noises)
+            with torch.no_grad():
+                return diff.decode_first_stage(final, first_stage_model=autoencoder)
+        return self._pad_crop(y0, mask, run)
 
     def _unit_noises(self, lqs, noise_repeat, units):
         """Yields (unit index, noises, z_y spec) for every unit of ``units`` in order: its T+1 noise tensors drawn as
         GaussianDiffusion.draw_noises does (after setup_seed with noise_repeat, as sample_func does), on the device of
         ``lqs``, so that the CUDA generator is where a one-GPU run has it whichever units run here."""
         offset = self.padding_offset
-        ctx = torch.autocast("cuda") if self.use_amp else nullcontext()
         for i, (g, starts, th, tw) in enumerate(units):
             lq = lqs[g]
-            with ctx:
+            with self._autocast():
                 if noise_repeat:
                     self.setup_seed()
                 spec = self._latent_spec(lq.shape[0] * len(starts), math.ceil(th / offset) * offset,
@@ -507,28 +457,37 @@ class ResShiftSampler(BaseSampler):
         """One unit: _sample_unit under autocast (and under the autoencoder's attention_team with ``team``), as fp32.
         ``replica``: the device_pool.Replica that runs it (its models, on the current device and stream)."""
         autoencoder = self.autoencoder if replica is None else replica.autoencoder
-        ctx = torch.autocast("cuda") if self.use_amp else nullcontext()
-        with ctx:
-            with autoencoder.attention_team(*team) if team is not None else nullcontext():
-                # shard mode keeps its four-argument call: code that wraps _sample_unit (e.g. to count the units a
-                # rank runs) sees the same call as before the pool existed; only pool units name their replica
-                if replica is None:
-                    return self._sample_unit(pch, mch, noises, spec).float()
-                return self._sample_unit(pch, mch, noises, spec, replica).float()
+        with self._autocast(), autoencoder.attention_team(*team) if team is not None else nullcontext():
+            return self._sample_unit(pch, mch, noises, spec, replica).float()
 
-    def _stack_shares(self, out, lqs, units):
-        """Per group, the tiles of ``out[g]`` stacked [n, b, 3, th*sf, tw*sf] (n may be 0)."""
-        tile_hw = {g: (th, tw) for g, _, th, tw in units}
-        return [torch.stack(t) if t else
-                torch.empty((0,) + tuple(lq.shape[:2]) + (tile_hw[g][0] * self.sf, tile_hw[g][1] * self.sf), device=lq.device)
+    def _stack_shares(self, results, lqs, units):
+        """Per group, the tiles of the units with an output in ``results`` (per unit, [n * b, 3, th*sf, tw*sf] or None)
+        stacked [n, b, 3, th*sf, tw*sf] in plan order (n may be 0)."""
+        out, empty = [[] for _ in lqs], {}
+        for (g, _, th, tw), res in zip(units, results):
+            empty[g] = (0,) + tuple(lqs[g].shape[:2]) + (th * self.sf, tw * self.sf)
+            if res is not None:
+                out[g].extend(torch.split(res, lqs[g].shape[0], dim=0))
+        return [torch.stack(t) if t else torch.empty(empty[g], device=lq.device)
                 for g, (t, lq) in enumerate(zip(out, lqs))]
 
     def _assemble(self, tiles, h, w):
-        """All tiles of one shape group [T, b, c, th*sf, tw*sf], in plan order -> [b, c, h*sf, w*sf]: what
-        _sample_tiled returns for that group."""
-        if not (h > self.chop_size or w > self.chop_size):
+        """All tiles of one shape group [T, b, c, th*sf, tw*sf], in plan order -> [b, c, h*sf, w*sf]: the tile of an
+        image that runs whole, else the overlaps averaged by rs_op_tile_gather in the reference's accumulation order."""
+        if self._one_tile(h, w):
             return tiles[0]
-        return self._overlap_average(tiles, h, w)
+        from . import _lib
+        sf = self.sf
+        hs_list = tile_starts(h, self.chop_size, self.chop_stride)
+        ws_list = tile_starts(w, self.chop_size, self.chop_stride)
+        tiles_t = tiles.contiguous()
+        b, c, th, tw = tiles_t.shape[1:]
+        out = torch.empty(b, c, h * sf, w * sf, dtype=torch.float32, device=tiles_t.device)
+        ys = torch.tensor([v * sf for v in hs_list], dtype=torch.int32, device=tiles_t.device)
+        xs = torch.tensor([v * sf for v in ws_list], dtype=torch.int32, device=tiles_t.device)
+        _lib.check(_lib.lib.rs_op_tile_gather(tiles_t.data_ptr(), b, c, h * sf, w * sf, th, tw, len(hs_list), len(ws_list),
+                                              ys.data_ptr(), xs.data_ptr(), out.data_ptr(), _lib.current_stream()))
+        return out
 
     def _process(self, im_lq, mask=None, noise_repeat=False, mask_back=True):
         """[b, c, h, w] in [-1, 1] -> [b, c, h*sf, w*sf] in [0, 1] (reference sampler.py:176-223)."""
@@ -574,7 +533,7 @@ class ResShiftSampler(BaseSampler):
 
     def inference(self, in_path, out_path, mask_path=None, mask_back=True, bs=1, noise_repeat=False):
         """File / folder driver (reference sampler.py:167-308).  Image I/O through OpenCV.  With ``shard_tiles`` every
-        rank reads the whole chunk and runs its share of the chunk's tiles (_run_shard); rank 0 assembles and writes.
+        rank reads the whole chunk and runs its part of the chunk's unit schedule (_run_rank); rank 0 assembles and writes.
         With a device pool the chunk's units run on the pool's replicas (_inference_pool)."""
         import cv2
         if self.shard_tiles:
@@ -624,24 +583,16 @@ class ResShiftSampler(BaseSampler):
         self.write_log(f"Processing done, enjoy the results in {out_path}")
 
     def _inference_shards(self, groups, read_group, out_path, mask_back, noise_repeat):
-        """One chunk in shard_tiles mode: this rank's tiles (its own units, or with fewer units than ranks its team's
-        unit), one gather per shape group, assembly and writing on rank 0."""
+        """One chunk in shard_tiles mode: this rank's part of the unit schedule, one gather per shape group, assembly and
+        writing on rank 0."""
         paths, lqs, masks = self._read_chunk(groups, read_group)
-        shapes = [tuple(lq.shape[2:]) for lq in lqs]
-        # fewer units than ranks: teams of ranks share each unit's bottleneck attention instead of leaving ranks idle
-        teams = self.num_gpus > 1 and dist.is_initialized() and hasattr(self.autoencoder, "attention_team") and \
-            attention_teams(len(self._plan_units(shapes)), self.num_gpus) is not None
-        if teams:
-            shares = self._run_team(lqs, masks, noise_repeat, self.num_gpus, self.rank)
-            counts = self._gather_counts(shapes, self.num_gpus)
-        else:
-            shares = self._run_shard(lqs, masks, noise_repeat, self.num_gpus, self.rank)
-            counts = self._share_counts(shapes, self.num_gpus)
-        for g, lq in enumerate(lqs):
-            tiles = gather_counts(shares[g], counts[g])
-            if self.rank != 0:
-                continue
-            self._write_group(paths[g], tiles, lq, masks[g], out_path, mask_back)
+        units = self._plan_units([tuple(lq.shape[2:]) for lq in lqs])
+        schedule = self._schedule(len(units), self.num_gpus)
+        shares = self._run_rank(lqs, masks, noise_repeat, units, schedule, self.rank)
+        for g, counts in enumerate(tile_counts(units, schedule, self.num_gpus)):
+            tiles = gather_counts(shares[g], counts)
+            if self.rank == 0:
+                self._write_group(paths[g], tiles, lqs[g], masks[g], out_path, mask_back)
 
     def _inference_pool(self, groups, read_group, out_path, mask_back, noise_repeat):
         """One chunk on the device pool: read and ingest on the primary, every unit's noise drawn there in one-GPU
@@ -649,11 +600,9 @@ class ResShiftSampler(BaseSampler):
         with torch.cuda.device(self.pool.primary):
             paths, lqs, masks = self._read_chunk(groups, read_group)
             units = self._plan_units([tuple(lq.shape[2:]) for lq in lqs])
-            out = [[] for _ in lqs]
-            for (g, _, _, _), res in zip(units, self.pool.run(self, lqs, masks, noise_repeat, units)):
-                out[g].extend(torch.split(res, lqs[g].shape[0], dim=0))
-            for g, (tiles, lq) in enumerate(zip(self._stack_shares(out, lqs, units), lqs)):
-                self._write_group(paths[g], tiles, lq, masks[g], out_path, mask_back)
+            tiles = self._stack_shares(self.pool.run(self, lqs, masks, noise_repeat, units), lqs, units)
+            for g, lq in enumerate(lqs):
+                self._write_group(paths[g], tiles[g], lq, masks[g], out_path, mask_back)
 
     def _read_chunk(self, groups, read_group):
         """Per shape group of a chunk: the paths, the LQ images [b, 3, h, w] and the masks [b, 1, h, w] or None, in

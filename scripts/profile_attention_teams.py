@@ -28,7 +28,7 @@ import torch.distributed as dist
 from resshift_b200 import _lib
 from resshift_b200.config import preset
 from resshift_b200.parallel import gather_counts
-from resshift_b200.sampler import ResShiftSampler, make_configs
+from resshift_b200.sampler import ResShiftSampler, make_configs, tile_counts
 from resshift_b200.vq_arch import random_vq_state_dict, vq_preset
 from resshift_b200.weights import random_state_dict
 
@@ -95,10 +95,12 @@ def team_worker(rank, world, port, steps, reps):
                       WORLD_SIZE=str(world))
     s = sampler(steps)                                        # setup_dist: NCCL, one GPU per rank
     lq = lq_tile()
+    units = s._plan_units([(512, 512)])
+    schedule = s._schedule(len(units), world)                # one unit: a team of every rank
 
     def team():
-        shares = s._run_team([lq], [None], False, world, rank)
-        tiles = gather_counts(shares[0], s._gather_counts([(512, 512)], world)[0])
+        shares = s._run_rank([lq], [None], False, units, schedule, rank)
+        tiles = gather_counts(shares[0], tile_counts(units, schedule, world)[0])
         return s._assemble(tiles, 512, 512) if rank == 0 else None
 
     def one():

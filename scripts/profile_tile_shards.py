@@ -24,7 +24,7 @@ import torch.distributed as dist
 
 from resshift_b200.config import preset
 from resshift_b200.parallel import gather_counts
-from resshift_b200.sampler import ResShiftSampler, make_configs, plan_tiles
+from resshift_b200.sampler import ResShiftSampler, make_configs, plan_tiles, tile_counts
 from resshift_b200.vq_arch import random_vq_state_dict, vq_preset
 from resshift_b200.weights import random_state_dict
 
@@ -84,9 +84,11 @@ def main():
     if rank == 0:
         print(f"time per unit: {', '.join(f'{t:.3f}' for t in unit_times)} s (first call includes plan creation)", flush=True)
 
+    schedule = s._schedule(len(units), world)
+
     def sharded():
-        shares = s._run_shard([lq], [None], False, world, rank)
-        tiles = gather_counts(shares[0], s._share_counts([(h, w)], world)[0])
+        shares = s._run_rank([lq], [None], False, units, schedule, rank)
+        tiles = gather_counts(shares[0], tile_counts(units, schedule, world)[0])
         return s._assemble(tiles, h, w) if rank == 0 else None
 
     def default():

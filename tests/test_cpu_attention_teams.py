@@ -8,8 +8,8 @@ import torch
 import torch.distributed as dist
 import torch.multiprocessing as mp
 
-from resshift_b200.parallel import attention_row_ranges, attention_teams, row_exchange, team_group
-from resshift_b200.sampler import ResShiftSampler
+from resshift_b200.parallel import attention_row_ranges, attention_teams, row_exchange, team_group, unit_schedule
+from resshift_b200.sampler import ResShiftSampler, tile_counts
 
 
 def _host_sampler(chop_size, chop_stride, chop_bs):
@@ -51,23 +51,29 @@ def test_row_blocks_are_covered_exactly_once(T):
     assert attention_row_ranges(16384, 3) == [(0, 5504), (5504, 11008), (11008, 16384)]
 
 
-def test_gather_counts_leader_only_with_fewer_units_than_ranks():
+def _counts(s, shapes, world, teams):
+    units = s._plan_units(shapes)
+    return tile_counts(units, unit_schedule(len(units), world, teams), world)
+
+
+def test_schedule_counts_leader_only_with_fewer_units_than_ranks():
     s = _host_sampler(64, 48, 5)
     shapes = [(200, 148), (60, 50), (64, 64)]              # units: 3 of the pair's tiles (5, 5, 2) + 1 + 1
     units = s._plan_units(shapes)
     assert len(units) == 5
     for world in (1, 2, 3, 4, 5, 6, 7, 8, 13):
-        counts = s._gather_counts(shapes, world)
+        counts = _counts(s, shapes, world, teams=True)
         if len(units) >= world:
-            assert counts == s._share_counts(shapes, world)
+            assert counts == _counts(s, shapes, world, teams=False)
             continue
-        teams = attention_teams(len(units), world)
+        teams = unit_schedule(len(units), world, True)
+        assert teams == attention_teams(len(units), world)
         firsts = {a for a, _ in teams}
         assert [sum(c) for c in counts] == [12, 1, 1]
         for g in range(len(shapes)):
             assert all(counts[g][r] == 0 for r in range(world) if r not in firsts)
-    assert s._gather_counts(shapes, 8) == [[5, 0, 5, 0, 2, 0, 0, 0], [0] * 6 + [1, 0], [0] * 7 + [1]]
-    assert s._gather_counts([(60, 50)], 3) == [[1, 0, 0]]
+    assert _counts(s, shapes, 8, teams=True) == [[5, 0, 5, 0, 2, 0, 0, 0], [0] * 6 + [1, 0], [0] * 7 + [1]]
+    assert _counts(s, [(60, 50)], 3, teams=True) == [[1, 0, 0]]
 
 
 def _exchange_worker(rank, world, port, q):

@@ -71,9 +71,9 @@ def _instrument(s):
     """Wraps s._sample_unit: records (replica index, batch, h, w) of every call."""
     ran, orig = [], s._sample_unit
 
-    def counted(*a):
-        ran.append((a[4].index if len(a) > 4 else None, a[0].shape[0]) + tuple(a[0].shape[2:]))
-        return orig(*a)
+    def counted(y0, mask, noises, spec, replica):
+        ran.append((None if replica is None else replica.index, y0.shape[0]) + tuple(y0.shape[2:]))
+        return orig(y0, mask, noises, spec, replica)
     s._sample_unit = counted
     return ran, orig
 
@@ -164,11 +164,11 @@ def test_worker_error_reaches_the_caller(samplers, tmp_path, kind, pool, failing
     _write(tmp_path, kind)
     calls, orig = [], s._sample_unit
 
-    def boom(*a):
-        calls.append(a[4].index)
-        if (failing == "second call" and len(calls) == 2) or (failing == "member 1" and a[4].index == 1):
+    def boom(y0, mask, noises, spec, replica):
+        calls.append(replica.index)
+        if (failing == "second call" and len(calls) == 2) or (failing == "member 1" and replica.index == 1):
             raise RuntimeError("boom in a pool worker")
-        return orig(*a)
+        return orig(y0, mask, noises, spec, replica)
     s._sample_unit = boom
     try:
         with pytest.raises(RuntimeError, match="boom in a pool worker"):

@@ -2,7 +2,7 @@
 every rank draws every unit's noise in the one-GPU order, and rank 0 averages the gathered tiles.  The output must be
 bit-identical to a one-GPU run of the default path, whatever the number of ranks.
 
-1. Virtual ranks in one process: each rank's share (_run_shard) after the same reseed, assembled in rank order, against
+1. Virtual ranks in one process: each rank's share (_run_rank) after the same reseed, assembled in rank order, against
    the default _sample_tiled.
 2. inference(bs=3) with two processes on one GPU under gloo, and 3. under NCCL on two GPUs: the PNG bytes against a
    one-GPU default inference().
@@ -54,7 +54,9 @@ CASES = [("tiny", 1, False), ("tiny", 1, True), ("tiny", 5, False), ("tiny", 5, 
 
 
 @pytest.mark.parametrize("kind,chop_bs,noise_repeat", CASES)
-def test_virtual_ranks_equal_one_gpu_default(samplers, kind, chop_bs, noise_repeat):
+def test_virtual_ranks_of_the_schedule_equal_one_gpu_default(samplers, kind, chop_bs, noise_repeat):
+    from resshift_b200.parallel import unit_schedule
+    from resshift_b200.sampler import tile_counts
     s = samplers[kind]
     s.chop_bs = chop_bs
     lqs, masks = _chunk(kind)
@@ -64,14 +66,15 @@ def test_virtual_ranks_equal_one_gpu_default(samplers, kind, chop_bs, noise_repe
     ran = []
     orig = s._sample_unit
 
-    def counted(y0, mask, noises, spec):
+    def counted(y0, mask, noises, spec, replica):
+        assert replica is None                                        # shard mode runs the sampler's own models
         ran.append(y0.shape[0])
         # the z_y shape and dtype derived from the configs (what every rank draws noise for) against the real encoder
         pad = s.padding_offset
         hp, wp = -(-y0.shape[2] // pad) * pad, -(-y0.shape[3] // pad) * pad
         z = s.base_diffusion.encode_first_stage(torch.zeros(y0.shape[0], 3, hp, wp, device="cuda"), s.autoencoder, up_sample=True)
         assert (tuple(z.shape), z.dtype) == spec
-        return orig(y0, mask, noises, spec)
+        return orig(y0, mask, noises, spec, replica)
 
     units = s._plan_units([tuple(lq.shape[2:]) for lq in lqs])
     if kind == "tiny":
@@ -79,13 +82,14 @@ def test_virtual_ranks_equal_one_gpu_default(samplers, kind, chop_bs, noise_repe
     s._sample_unit = counted
     try:
         for world in (1, 2, 5, 13):
+            schedule = unit_schedule(len(units), world, teams=False)  # virtual ranks cannot exchange attention rows
             ran.clear()
             shares = []
             for rank in range(world):
                 s.setup_seed()
-                shares.append(s._run_shard(lqs, masks, noise_repeat, world, rank))
+                shares.append(s._run_rank(lqs, masks, noise_repeat, units, schedule, rank))
             assert ran == [lqs[u[0]].shape[0] * len(u[1]) for u in units]      # each unit ran once, in order
-            counts = s._share_counts([tuple(lq.shape[2:]) for lq in lqs], world)
+            counts = tile_counts(units, schedule, world)
             for g, (lq, r) in enumerate(zip(lqs, ref)):
                 assert [sh[g].shape[0] for sh in shares] == counts[g]
                 out = s._assemble(torch.cat([sh[g] for sh in shares]), *lq.shape[2:])
@@ -164,7 +168,7 @@ def test_two_gpus_nccl_equal_one_gpu_default(tmp_path):
     _run_two_ranks(tmp_path, "nccl")
 
 
-def test_generic_route_is_refused_before_any_work(tmp_path, monkeypatch):
+def test_generic_route_is_refused_before_inference_or_run_rank_works(tmp_path, monkeypatch):
     """Without an autoencoder the reference clips x0 (clip_denoised=True), which takes the generic per-step route: its
     noise is drawn step by step inside the loop, so it cannot be drawn ahead for skipped units."""
     from resshift_b200.config import preset
@@ -186,4 +190,4 @@ def test_generic_route_is_refused_before_any_work(tmp_path, monkeypatch):
         s.inference(tmp_path / "in", tmp_path / "out", bs=3)
     assert not (tmp_path / "out").exists()
     with pytest.raises(RuntimeError, match="generic per-step route"):
-        s._run_shard([torch.zeros(1, 3, 64, 64, device="cuda")], [None], False, 2, 0)
+        s._run_rank([torch.zeros(1, 3, 64, 64, device="cuda")], [None], False, s._plan_units([(64, 64)]), [(0, 1)], 0)
