@@ -238,6 +238,11 @@ int rs_op_vq_attention(const void* q, const void* k, const void* v, int N, int T
  * out is written, so ranges computed on different devices and copied together equal one full call. */
 int rs_op_vq_attention_rows(const void* q, const void* k, const void* v, int N, int T, int C, int ld, int row_begin,
                             int row_end, void* out, void* stream);
+/* row softmax of the same attention for H*W <= 8192, in place on the fp16 score matrix: s[r][0:cols] =
+ * softmax(scale * s[r][0:cols]) for each of `rows` rows with row stride ld (elements); what lies beyond cols in a row is
+ * not touched.  Needs rows >= 1, cols a multiple of 8 in [8, 8192], ld >= cols and a multiple of 8, s 16-byte aligned;
+ * anything else returns an error. */
+int rs_op_softmax_rows(void* s, int rows, int cols, long long ld, float scale, void* stream);
 /* window attention core (reference models/swin_transformer.py:114-145,251-275); qkv [N,H,W,3*heads*32] */
 int rs_op_expand_relpos(const float* table_225xh, float* dense_hx64x64, int heads, void* stream);
 int rs_op_window_attention(const void* qkv, int N, int H, int W, int heads, int shift, const float* bias_dense,

@@ -91,6 +91,7 @@ _SIGNATURES = {
     "rs_op_expand_relpos": (C.c_int, [_P, _P, C.c_int, _P]),
     "rs_op_vq_attention": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P]),
     "rs_op_vq_attention_rows": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P]),
+    "rs_op_softmax_rows": (C.c_int, [_P, C.c_int, C.c_int, C.c_longlong, C.c_float, _P]),
     "rs_op_window_attention": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P, _P]),
     "rs_op_swin_attn": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, C.c_int, _P, _P, _P, _P, _P, _P, _P,
                                   _P, _P, _P, _P, _P]),

@@ -299,6 +299,11 @@ struct Op {
   std::vector<StatDst> stat_dst;        // conv: GroupNorm ops whose statistics this conv's epilogue produces
 };
 
+inline SoftmaxParams softmax_params(const Op& op) {
+  const View& s = op.s_view;
+  return SoftmaxParams{s.ptr, (long long)s.ld, s.N * s.H * s.W, s.C, op.s_scale};
+}
+
 }  // namespace
 
 struct rs_plan {
@@ -964,7 +969,7 @@ int bind_ops(rs_plan& P, std::vector<Op>& ops) {
       // stream structure only
     } else if (op.kind == OP_SOFTMAX) {
       resolve(P, op.s_view);
-      RS_CHECK(op.s_view.C % 8 == 0 && op.s_view.C <= 8192 && op.s_view.ld % 8 == 0, "softmax row length");
+      int rc = softmax_rows_check(softmax_params(op)); if (rc) return rc;
       ++P.launches;
     } else if (op.kind == OP_VQ_ATTN) {
       VqAttnDesc& a = op.vqa;
@@ -1049,7 +1054,7 @@ int run_op_range(rs_plan& P, const Op* first, const Op* last, const float* film_
         rc = attn_launch(op.a_in, op.a_out, op.a_bias, P.e->cfg.swin_heads, P.e->cfg.swin_embed_dim, op.a_shift, st);
         break;
       case OP_SOFTMAX: {
-        SoftmaxParams sp{op.s_view.ptr, (long long)op.s_view.ld, op.s_view.N * op.s_view.H * op.s_view.W, op.s_view.C, op.s_scale};
+        const SoftmaxParams sp = softmax_params(op);
         (void)launch_k(softmax_rows_kernel, dim3((unsigned)sp.rows), dim3(256), (size_t)0, st, sp);
         if (cudaGetLastError() != cudaSuccess) rc = fail(-2, "softmax launch failed");
         break;

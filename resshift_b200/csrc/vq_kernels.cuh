@@ -14,16 +14,28 @@ namespace rs {
 // reference: AttnBlock.forward, ldm/modules/diffusionmodules/model.py:190-192 (w_ * c^-0.5, softmax over keys).
 // One CTA per row; each thread keeps its (at most 32) elements in registers between the passes.
 // ------------------------------------------------------------------------------------------------
+constexpr int kSoftmaxMaxCols = 8192;             // the longest row: 256 threads x 4 vectors x 8 halves
 struct SoftmaxParams {
   __half* s; long long ld; int rows, cols; float scale;
 };
+// What the kernel computes correctly: rows that fit in its registers, read and written as 16-byte vectors from a
+// 16-byte aligned start.  Anything else would be silently wrong (columns dropped or misaligned), so both the plan and
+// the single-operator entry refuse it here.
+inline int softmax_rows_check(const SoftmaxParams& p) {
+  RS_CHECK(p.s != nullptr && (reinterpret_cast<uintptr_t>(p.s) & 15) == 0, "row softmax: S must be 16-byte aligned");
+  RS_CHECK(p.rows >= 1, "row softmax: rows >= 1");
+  RS_CHECK(p.cols >= 8 && p.cols <= kSoftmaxMaxCols && p.cols % 8 == 0,
+           "row softmax: cols must be a multiple of 8 in [8, 8192], got " + std::to_string(p.cols));
+  RS_CHECK(p.ld >= p.cols && p.ld % 8 == 0, "row softmax: row stride ld >= cols and a multiple of 8, got " + std::to_string(p.ld));
+  return 0;
+}
 __global__ void __launch_bounds__(256) softmax_rows_kernel(const SoftmaxParams p) {
   pdl_trigger();
   pdl_wait();
   __shared__ float s_red[8];
   __half* row = p.s + (long long)blockIdx.x * p.ld;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  constexpr int kMaxVec = 4;                      // 4 x 8 halves per thread: cols <= 8192
+  constexpr int kMaxVec = kSoftmaxMaxCols / (256 * 8);   // 4 x 8 halves per thread
   uint4 raw[kMaxVec];
   float v[kMaxVec][8];
   const int nvec = p.cols >> 3;
