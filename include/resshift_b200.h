@@ -18,7 +18,8 @@
  *     device is refused as its arena), and a plan to the device
  *     that is current at rs_plan_bind, which must be its engine's.  A plan runs on the device it was bound on: every
  *     entry point that enqueues work on a plan or its sampler (rs_plan_forward / _profile / _profile_ops / _probe,
- *     rs_sampler_run / _run_host, rs_vq_encode / _decode and their _begin / _end halves, rs_vq_profile_ops)
+ *     rs_sampler_run / _run_host, rs_vq_encode / _decode / _decode_code, rs_kl_encode / _decode, their _begin / _end
+ *     halves, rs_vq_profile_ops)
  *     returns an error when another device is current, and the stream passed in must belong to that device.
  */
 #ifndef RESSHIFT_B200_H
@@ -165,8 +166,36 @@ int rs_vq_set_attention_rows(rs_plan* p, int row_begin, int row_end);
  * result from the end of _begin until _end reads it; nothing else in the plan writes it in between. */
 int rs_vq_attention_output(rs_plan* p, void** ptr, long long* row_stride, long long* image_stride, int32_t* T, int32_t* C);
 /* diagnostics: per-launch times (ms) and descriptions of the plan's op list on the inputs of the last encode/decode
- * call (counterpart of rs_plan_profile_ops for the first-stage plans) */
+ * call (counterpart of rs_plan_profile_ops for the first-stage plans); VQ-GAN and KL plans */
 int rs_vq_profile_ops(rs_plan* p, double* ms, char* desc, int desc_stride, int cap, int32_t* n_ops, void* stream);
+/* VQModelTorch.decode_code (autoencoder.py:42-45) on a decode plan: idx [B, H/f, W/f] int32 code indices -> the codebook
+ * rows (quantize.embed_code) -> post_quant_conv -> Decoder -> out [B, 3, H, W] fp32; bit-identical to rs_vq_decode of
+ * those rows with force_not_quantize.  An index outside [0, n_embed) gives NaN at its position (nothing is read out of
+ * bounds). */
+int rs_vq_decode_code(rs_plan* p, const int32_t* idx, float* out, void* stream);
+
+/* ---- KL first stage: ldm.models.autoencoder.AutoencoderKLTorch (reference ldm/models/autoencoder.py:52-86) ----------
+ * The same Encoder / Decoder as the VQ-GAN with double_z: encoder.conv_out has 2 z_channels, quant_conv is
+ * [2 embed_dim, 2 z_channels, 1, 1], post_quant_conv [z_channels, embed_dim, 1, 1], no codebook (cfg->n_embed is
+ * ignored).  Parameters, arena, plans (rs_vq_plan_create with which = 0 / 1), rs_vq_set_attention_rows,
+ * rs_vq_attention_output and rs_vq_profile_ops work as for the VQ-GAN; the rs_vq_encode / _decode calls refuse KL
+ * plans and the rs_kl_* calls refuse VQ-GAN plans. */
+int rs_kl_create(const rs_vq_config* cfg, rs_engine** out);
+/* AutoencoderKLTorch.encode (autoencoder.py:65-76) with DiagonalGaussianDistribution
+ * (ldm/modules/distributions/distributions.py:24-37,61-62): x [B, 3, H, W] fp32 -> moments = quant_conv(Encoder(x))
+ * [B, 2 embed_dim, H/f, W/f]; mean, logvar = moments[:, :e], clamp(moments[:, e:], -30, 20);
+ * z_out [B, embed_dim, H/f, W/f] = mean + exp(0.5 logvar) * noise (sample()), or mean when noise is NULL (mode()).
+ * noise: [B, embed_dim, H/f, W/f] fp32 or NULL; moments_out: [B, 2 embed_dim, H/f, W/f] fp32 or NULL. */
+int rs_kl_encode(rs_plan* p, const float* x, const float* noise_or_null, float* z_out, float* moments_out_or_null,
+                 void* stream);
+/* AutoencoderKLTorch.decode (autoencoder.py:78-81): z [B, embed_dim, H/f, W/f] -> post_quant_conv -> Decoder ->
+ * out [B, 3, H, W] fp32 */
+int rs_kl_decode(rs_plan* p, const float* z, float* out, void* stream);
+/* the two halves of each pass, split at the mid-block attention as the rs_vq_*_begin / _end calls are */
+int rs_kl_encode_begin(rs_plan* p, const float* x, void* stream);
+int rs_kl_encode_end(rs_plan* p, const float* noise_or_null, float* z_out, float* moments_out_or_null, void* stream);
+int rs_kl_decode_begin(rs_plan* p, const float* z, void* stream);
+int rs_kl_decode_end(rs_plan* p, float* out, void* stream);
 
 /* ---- image edges of the sampler (reference sampler.py:176-223,286; utils/util_image.py:216-273,889-979) --------- */
 /* F.interpolate(x, scale_factor=sf, mode='bicubic') on fp32 NCHW (models/gaussian_diffusion.py:503-504) */

@@ -110,6 +110,14 @@ _SIGNATURES = {
     "rs_vq_attention_output": (C.c_int, [_P, C.POINTER(_P), C.POINTER(C.c_longlong), C.POINTER(C.c_longlong),
                                          C.POINTER(C.c_int32), C.POINTER(C.c_int32)]),
     "rs_vq_profile_ops": (C.c_int, [_P, C.POINTER(C.c_double), C.c_char_p, C.c_int, C.c_int, C.POINTER(C.c_int32), _P]),
+    "rs_vq_decode_code": (C.c_int, [_P, _P, _P, _P]),
+    "rs_kl_create": (C.c_int, [C.POINTER(VQConfigC), C.POINTER(_P)]),
+    "rs_kl_encode": (C.c_int, [_P, _P, _P, _P, _P, _P]),
+    "rs_kl_decode": (C.c_int, [_P, _P, _P, _P]),
+    "rs_kl_encode_begin": (C.c_int, [_P, _P, _P]),
+    "rs_kl_encode_end": (C.c_int, [_P, _P, _P, _P, _P]),
+    "rs_kl_decode_begin": (C.c_int, [_P, _P, _P]),
+    "rs_kl_decode_end": (C.c_int, [_P, _P, _P]),
     "rs_op_bicubic_upsample": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P]),
     "rs_op_ingest_u8": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P]),
     "rs_op_emit_u8": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P]),

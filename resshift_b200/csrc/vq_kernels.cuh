@@ -1,5 +1,6 @@
 // Small kernels of the VQ-GAN bookends and the image I/O edges (everything that is not a conv / GroupNorm / GEMM):
-// row softmax of the single-head attention, nearest-codebook quantisation, the two tiny 1x1 convs around the quantiser,
+// row softmax of the single-head attention, nearest-codebook quantisation, the two tiny 1x1 convs around the quantiser
+// (and around the KL first stage's posterior),
 // torch-compatible bicubic upsampling, uint8 <-> [-1, 1] conversion with mask blending, overlap-average tile scatter.
 #pragma once
 
@@ -115,11 +116,54 @@ __global__ void pointwise_conv_f32_kernel(const PointwiseParams p) {
 }
 
 // ------------------------------------------------------------------------------------------------
+// quant_conv and DiagonalGaussianDistribution of the KL first stage in one pass (reference
+// ldm/models/autoencoder.py:65-72, ldm/modules/distributions/distributions.py:24-37,61-62):
+//   moments = quant_conv(h)                        [N, 2E, HW]  (same fp32 accumulation as pointwise_conv_f32_kernel)
+//   mean, logvar = moments[:, :E], clamp(moments[:, E:], -30, 20);  std = exp(0.5 logvar)
+//   z = mean + std * noise   (noise given: sample())        z = mean   (noise == nullptr: mode())
+// The product and the sum are rounded separately, as torch evaluates `self.mean + self.std * randn`.
+// ------------------------------------------------------------------------------------------------
+struct KlPosteriorParams {
+  const float* h;            // [N, Cin, HW] fp32: the encoder's output (2 z_channels)
+  const __half* w; int w_ld; const float* b; int Cin, E;   // quant_conv [2E][Cin] (fp16, row stride w_ld), bias [2E]
+  const float* noise;        // [N, E, HW] fp32 or nullptr
+  float* z;                  // [N, E, HW]
+  float* moments;            // [N, 2E, HW] or nullptr
+  int N, HW;
+};
+__global__ void kl_posterior_kernel(const KlPosteriorParams p) {
+  pdl_trigger();
+  pdl_wait();
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (long long)p.N * p.HW) return;
+  const int n = (int)(i / p.HW), hw = (int)(i % p.HW);
+  float xin[16], m[16];
+  for (int c = 0; c < p.Cin; ++c) xin[c] = p.h[((long long)n * p.Cin + c) * p.HW + hw];
+  for (int co = 0; co < 2 * p.E; ++co) {
+    float acc = p.b[co];
+    for (int c = 0; c < p.Cin; ++c) acc = fmaf(__half2float(p.w[co * p.w_ld + c]), xin[c], acc);
+    m[co] = acc;
+    if (p.moments) p.moments[((long long)n * 2 * p.E + co) * p.HW + hw] = acc;
+  }
+  for (int c = 0; c < p.E; ++c) {
+    const long long o = ((long long)n * p.E + c) * p.HW + hw;
+    float zc = m[c];
+    if (p.noise) {
+      const float logvar = fminf(fmaxf(m[p.E + c], -30.0f), 20.0f);
+      zc = __fadd_rn(zc, __fmul_rn(expf(0.5f * logvar), p.noise[o]));
+    }
+    p.z[o] = zc;
+  }
+}
+
+// ------------------------------------------------------------------------------------------------
 // VectorQuantizer2.forward (reference ldm/modules/vqvae/quantize.py:271-284) fused with post_quant_conv
 // (ldm/models/autoencoder.py:33-38) and the layout change the decoder's first conv wants:
 //   idx = argmin_j ( |z|^2 + |e_j|^2 - 2 z.e_j )   (first minimum, fp32)
 //   out[pix, :] = post_quant_conv(e_idx)  as NHWC fp16 padded to Cpad channels.
 // One thread per latent position; the codebook streams through shared memory in chunks read by the whole CTA.
+// With idx_in (VQModelTorch.decode_code, autoencoder.py:42-45) the codes are given: e_idx is gathered from the codebook
+// (an index outside [0, n_e) gives NaN at that position) and z is not read.
 // ------------------------------------------------------------------------------------------------
 struct QuantizeParams {
   const float* z;            // [N, E, HW] fp32
@@ -129,6 +173,7 @@ struct QuantizeParams {
   const __half* pw; int pw_ld; const float* pb; int Cz;   // post_quant_conv [Cz][E] (fp16, row stride pw_ld), bias [Cz]
   __half* out; int Cpad;     // [N*HW, Cpad]
   int* idx_out;              // optional [N, HW]
+  const int* idx_in;         // optional [N, HW]: given codes (then quantize must be 0 and z may be null)
 };
 __global__ void __launch_bounds__(256) vq_quantize_kernel(const QuantizeParams p) {
   pdl_trigger();
@@ -140,7 +185,7 @@ __global__ void __launch_bounds__(256) vq_quantize_kernel(const QuantizeParams p
   const int n = live ? (int)(i / p.HW) : 0, hw = live ? (int)(i % p.HW) : 0;
   float zv[8];
   float zz = 0.f;
-  for (int c = 0; c < p.E; ++c) { zv[c] = live ? p.z[((long long)n * p.E + c) * p.HW + hw] : 0.f; }
+  for (int c = 0; c < p.E; ++c) { zv[c] = live && !p.idx_in ? p.z[((long long)n * p.E + c) * p.HW + hw] : 0.f; }
   for (int c = 0; c < p.E; ++c) zz += zv[c] * zv[c];          // torch.sum(z ** 2, dim=1): sequential over E
   int best = 0;
   if (p.quantize) {
@@ -166,7 +211,12 @@ __global__ void __launch_bounds__(256) vq_quantize_kernel(const QuantizeParams p
   }
   if (!live) return;
   float q[8];
-  for (int c = 0; c < p.E; ++c) q[c] = p.quantize ? p.codebook[(long long)best * p.E + c] : zv[c];
+  if (p.idx_in) {
+    const int code = p.idx_in[i];
+    for (int c = 0; c < p.E; ++c) q[c] = code >= 0 && code < p.n_e ? p.codebook[(long long)code * p.E + c] : __int_as_float(0x7fc00000);
+  } else {
+    for (int c = 0; c < p.E; ++c) q[c] = p.quantize ? p.codebook[(long long)best * p.E + c] : zv[c];
+  }
   if (p.idx_out) p.idx_out[i] = p.quantize ? best : -1;
   __half* o = p.out + i * p.Cpad;
   int co = 0;

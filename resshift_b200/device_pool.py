@@ -289,8 +289,9 @@ class DevicePool:
         dev = rep.device
         pch = job.pch.to(dev, non_blocking=True)
         mch = None if job.mch is None else job.mch.to(dev, non_blocking=True)
-        noises = job.noises.to(dev, non_blocking=True)
-        for t in (job.pch, job.mch, job.noises):                # read on primary_stream: not reused before that
+        # (the posterior noise, if any, stays on the CPU: the first stage copies it, as the reference's encode does)
+        noises = job.noises._replace(loop=job.noises.loop.to(dev, non_blocking=True))
+        for t in (job.pch, job.mch, job.noises.loop):           # read on primary_stream: not reused before that
             if t is not None:
                 t.record_stream(primary_stream)
         res = sampler._run_unit(pch, mch, noises, job.spec, team=job.team, replica=rep)

@@ -1,14 +1,18 @@
-"""``VQModelTorch`` — same constructor, ``state_dict`` and call surface as the reference's
-``ldm.models.autoencoder.VQModelTorch`` (reference ldm/models/autoencoder.py:12-47), the VQ-GAN first stage around the
-denoising loop (SURVEY.md §8f rank 1), executed by the sm_90a kernels of ``librs_b200.so``: the same wgmma
+"""``VQModelTorch``, ``AutoencoderKLTorch`` and ``EncoderKLTorch`` — same constructors, ``state_dict`` and call surface
+as the reference's ``ldm.models.autoencoder`` classes (reference ldm/models/autoencoder.py:12-112), the first stages
+around the denoising loop (SURVEY.md §8f rank 1), executed by the sm_90a kernels of ``librs_b200.so``: the same wgmma
 implicit-GEMM conv / GroupNorm kernels as the denoiser, the bottleneck's single-head attention as tensor-core GEMMs + a
 row softmax up to 8192 positions and as one fused online-softmax kernel above (any image whose size is a multiple of
-8 * 2^(levels-1)), nearest-codebook quantisation as one small kernel (csrc/vq.inc, csrc/vq_attn.cuh).
+8 * 2^(levels-1)), nearest-codebook quantisation (VQ) or quant_conv + posterior sampling (KL) as one small kernel
+(csrc/vq.inc, csrc/vq_attn.cuh, csrc/vq_kernels.cuh).
 
-``encode(x)`` / ``decode(h, force_not_quantize=False)`` / ``forward`` take and return fp32 NCHW CUDA tensors.  PyTorch
-owns every allocation; there is no eager / CPU fallback.
+``VQModelTorch``: ``encode(x)`` / ``decode(h, force_not_quantize=False)`` / ``decode_code(code_b)`` / ``forward``.
+``AutoencoderKLTorch``: ``encode(x, sample_posterior=True, return_moments=False)`` / ``decode(z)`` / ``forward``; the
+posterior noise is drawn as the reference draws it (``torch.randn`` on the CPU default generator) unless the caller
+passes it as ``posterior_noise=``.  All take and return fp32 NCHW CUDA tensors.  PyTorch owns every allocation; there
+is no eager / CPU fallback.
 
-``with vq.attention_team(member, size, exchange):`` splits the fused bottleneck attention's query rows over a team of
+``with ae.attention_team(member, size, exchange):`` splits the fused bottleneck attention's query rows over a team of
 processes (DESIGN.md §6): each member computes its share of the rows and ``exchange`` fills in the others', so the
 result is bit-identical to computing all rows here.
 """
@@ -23,27 +27,34 @@ import torch.nn as nn
 
 from .. import _lib
 from ..parallel import shard_range
-from ..vq_arch import VQConfig, random_vq_state_dict, vq_param_spec
+from ..vq_arch import VQConfig, kl_param_spec, random_kl_state_dict, random_vq_state_dict, vq_param_spec
 
 
 class _Node(nn.Module):
     """Anonymous container; only there so that ``state_dict`` keys match the reference's."""
 
 
-class VQModelTorch(nn.Module):
-    def __init__(self, ddconfig, n_embed, embed_dim, remap=None, sane_index_shape=False):
+def _config(ddconfig, embed_dim, n_embed=0, kl=False) -> VQConfig:
+    dd = dict(ddconfig)
+    return VQConfig(embed_dim=embed_dim, n_embed=n_embed, z_channels=dd["z_channels"], resolution=dd.get("resolution", 256),
+                    in_channels=dd.get("in_channels", 3), out_ch=dd.get("out_ch", 3), ch=dd["ch"],
+                    ch_mult=tuple(dd["ch_mult"]), num_res_blocks=dd["num_res_blocks"],
+                    attn_resolutions=tuple(dd.get("attn_resolutions", ())), dropout=dd.get("dropout", 0.0),
+                    double_z=dd.get("double_z", kl), kl=kl)
+
+
+class _FirstStage(nn.Module):
+    """What the first stages share: reference-named parameters, the native engine and its weight arena, one plan per
+    (pass, batch, image size), and attention teams.  ``_create`` is the engine constructor of the C ABI."""
+
+    _create = "rs_vq_create"
+    _name = "VQModelTorch"
+    _encoder_only = False          # the module holds the encoder's parameters only (the engine lists the decoder's too)
+
+    def __init__(self, cfg: VQConfig, spec, init: Dict[str, torch.Tensor]):
         super().__init__()
-        if remap is not None:
-            raise NotImplementedError("codebook remapping is not used by any shipped config")
-        dd = dict(ddconfig)
-        self.cfg = VQConfig(embed_dim=embed_dim, n_embed=n_embed, z_channels=dd["z_channels"], resolution=dd.get("resolution", 256),
-                            in_channels=dd.get("in_channels", 3), out_ch=dd.get("out_ch", 3), ch=dd["ch"],
-                            ch_mult=tuple(dd["ch_mult"]), num_res_blocks=dd["num_res_blocks"],
-                            attn_resolutions=tuple(dd.get("attn_resolutions", ())), dropout=dd.get("dropout", 0.0),
-                            double_z=dd.get("double_z", False))
-        self.sane_index_shape = sane_index_shape
-        self._spec = vq_param_spec(self.cfg)
-        init = random_vq_state_dict(self.cfg, seed=0)
+        self.cfg = cfg
+        self._spec = spec
         for name, shape, role in self._spec:
             *path, leaf = name.split(".")
             node = self
@@ -56,7 +67,6 @@ class VQModelTorch(nn.Module):
         self._arena: Optional[torch.Tensor] = None
         self._packed_versions: Optional[Tuple] = None
         self._plans: Dict[Tuple[int, int, int, int], "_VQPlan"] = {}
-        self.last_indices: Optional[torch.Tensor] = None
         self._team: Optional[Tuple[int, int, Callable]] = None
         # (which, row_begin, row_end) of every team-split attention since the last attention_team() entry: 0 encode, 1 decode
         self.attention_rows: List[Tuple[int, int, int]] = []
@@ -64,11 +74,11 @@ class VQModelTorch(nn.Module):
     # ------------------------------------------------------------------ native plumbing
     def _ensure_engine(self, device: torch.device):
         if device.type != "cuda":
-            raise RuntimeError("resshift_b200.VQModelTorch runs on CUDA only (no CPU fallback); call .cuda() first")
+            raise RuntimeError(f"resshift_b200.{self._name} runs on CUDA only (no CPU fallback); call .cuda() first")
         if self._engine is None:
             h = C.c_void_p()
             cfgc = _lib.make_vq_config(self.cfg)
-            _lib.check(_lib.lib.rs_vq_create(C.byref(cfgc), C.byref(h)))
+            _lib.check(getattr(_lib.lib, self._create)(C.byref(cfgc), C.byref(h)))
             self._engine = h
             n = _lib.lib.rs_unet_param_count(h)
             theirs = []
@@ -78,7 +88,7 @@ class VQModelTorch(nn.Module):
             for i in range(n):
                 _lib.check(_lib.lib.rs_unet_param_info(h, i, buf, 256, shape, C.byref(nd), C.byref(isb)))
                 theirs.append(buf.value.decode())
-            if sorted(theirs) != sorted(name for name, _, _ in self._spec):
+            if not self._inventory_matches(theirs):
                 raise _lib.RsError("parameter inventory of librs_b200 does not match resshift_b200.vq_arch")
         if self._arena is None or self._arena.device != device:
             nbytes = _lib.lib.rs_unet_arena_bytes(self._engine)
@@ -89,6 +99,10 @@ class VQModelTorch(nn.Module):
             self._packed_versions = None
             self._plans.clear()
         return self._engine
+
+    def _inventory_matches(self, theirs) -> bool:
+        mine = [name for name, _, _ in self._spec]
+        return set(mine) <= set(theirs) if self._encoder_only else sorted(theirs) == sorted(mine)
 
     def pack_weights(self, force: bool = False):
         params = dict(self.named_parameters())
@@ -117,54 +131,41 @@ class VQModelTorch(nn.Module):
             self._plans[key] = _VQPlan(self, which, batch, image_h, image_w, device)
         return self._plans[key]
 
-    # ------------------------------------------------------------------ reference call surface
-    @torch.no_grad()
-    def encode(self, x):
-        """x [B, 3, H, W] -> h [B, embed_dim, H/f, W/f] (reference autoencoder.py:28-31)."""
+    def _encode_plan(self, x, what):
+        """The encode plan of image batch ``x`` and ``x`` as contiguous fp32."""
         if x.device.type != "cuda":
-            raise RuntimeError("resshift_b200.VQModelTorch.encode needs CUDA tensors (no CPU fallback)")
+            raise RuntimeError(f"resshift_b200.{self._name}.{what} needs CUDA tensors (no CPU fallback)")
         b, c, hh, ww = x.shape
         if c != self.cfg.in_channels:
             raise ValueError(f"expected {self.cfg.in_channels} input channels, got {c}")
-        f = self.cfg.downscale
-        plan = self.plan(0, b, hh, ww)
-        xf = x.detach().float().contiguous()
-        out = torch.empty(b, self.cfg.embed_dim, hh // f, ww // f, dtype=torch.float32, device=x.device)
-        stream = _lib.current_stream()
-        if self._team is not None and plan.attention is not None:
-            self._run_team_split(
-                plan, 0, lambda: _lib.check(_lib.lib.rs_vq_encode_begin(plan.handle, xf.data_ptr(), stream)),
-                lambda: _lib.check(_lib.lib.rs_vq_encode_end(plan.handle, out.data_ptr(), stream)))
-        else:
-            _lib.check(_lib.lib.rs_vq_encode(plan.handle, xf.data_ptr(), out.data_ptr(), stream))
-        return out
+        return self.plan(0, b, hh, ww), x.detach().float().contiguous()
 
-    @torch.no_grad()
-    def decode(self, h, force_not_quantize=False):
-        """h [B, embed_dim, h, w] -> image [B, 3, h*f, w*f] (reference autoencoder.py:33-40); the code indices of the
-        last call stay available as ``self.last_indices`` ([B, h, w] int32, -1 when not quantised)."""
+    def _decode_plan(self, h, what):
+        """The decode plan of latent batch ``h`` and ``h`` as contiguous fp32."""
         if h.device.type != "cuda":
-            raise RuntimeError("resshift_b200.VQModelTorch.decode needs CUDA tensors (no CPU fallback)")
+            raise RuntimeError(f"resshift_b200.{self._name}.{what} needs CUDA tensors (no CPU fallback)")
         b, c, lh, lw = h.shape
         if c != self.cfg.embed_dim:
             raise ValueError(f"expected {self.cfg.embed_dim} latent channels, got {c}")
         f = self.cfg.downscale
-        plan = self.plan(1, b, lh * f, lw * f)
-        hf = h.detach().float().contiguous()
-        out = torch.empty(b, self.cfg.out_ch, lh * f, lw * f, dtype=torch.float32, device=h.device)
-        idx = torch.empty(b, lh, lw, dtype=torch.int32, device=h.device)
-        stream, fnq = _lib.current_stream(), int(bool(force_not_quantize))
-        if self._team is not None and plan.attention is not None:
-            self._run_team_split(
-                plan, 1, lambda: _lib.check(_lib.lib.rs_vq_decode_begin(plan.handle, hf.data_ptr(), idx.data_ptr(), fnq, stream)),
-                lambda: _lib.check(_lib.lib.rs_vq_decode_end(plan.handle, out.data_ptr(), stream)))
-        else:
-            _lib.check(_lib.lib.rs_vq_decode(plan.handle, hf.data_ptr(), out.data_ptr(), idx.data_ptr(), fnq, stream))
-        self.last_indices = idx
-        return out
+        return self.plan(1, b, lh * f, lw * f), h.detach().float().contiguous()
 
-    def forward(self, input, force_not_quantize=False):
-        return self.decode(self.encode(input), force_not_quantize)
+    def _latent(self, x):
+        b, _, hh, ww = x.shape
+        f = self.cfg.downscale
+        return torch.empty(b, self.cfg.embed_dim, hh // f, ww // f, dtype=torch.float32, device=x.device)
+
+    def _image(self, h):
+        b, _, lh, lw = h.shape
+        f = self.cfg.downscale
+        return torch.empty(b, self.cfg.out_ch, lh * f, lw * f, dtype=torch.float32, device=h.device)
+
+    def _run(self, plan: "_VQPlan", which: int, begin: Callable[[], None], end: Callable[[], None], whole: Callable[[], None]):
+        """One pass: split at the fused attention inside an attention team, else the single call ``whole``."""
+        if self._team is not None and plan.attention is not None:
+            self._run_team_split(plan, which, begin, end)
+        else:
+            whole()
 
     # ------------------------------------------------------------------ attention teams
     @contextmanager
@@ -211,10 +212,137 @@ class VQModelTorch(nn.Module):
             pass
 
 
-class _VQPlan:
-    """VQ-GAN engine bound to (encode | decode, batch, image H, image W): owns the workspace and the native plan."""
+class VQModelTorch(_FirstStage):
+    def __init__(self, ddconfig, n_embed, embed_dim, remap=None, sane_index_shape=False):
+        if remap is not None:
+            raise NotImplementedError("codebook remapping is not used by any shipped config")
+        cfg = _config(ddconfig, embed_dim, n_embed=n_embed)
+        super().__init__(cfg, vq_param_spec(cfg), random_vq_state_dict(cfg, seed=0))
+        self.sane_index_shape = sane_index_shape
+        self.last_indices: Optional[torch.Tensor] = None
 
-    def __init__(self, model: VQModelTorch, which: int, batch: int, image_h: int, image_w: int, device):
+    # ------------------------------------------------------------------ reference call surface
+    @torch.no_grad()
+    def encode(self, x):
+        """x [B, 3, H, W] -> h [B, embed_dim, H/f, W/f] (reference autoencoder.py:28-31)."""
+        plan, xf = self._encode_plan(x, "encode")
+        out = self._latent(x)
+        stream = _lib.current_stream()
+        self._run(plan, 0, lambda: _lib.check(_lib.lib.rs_vq_encode_begin(plan.handle, xf.data_ptr(), stream)),
+                  lambda: _lib.check(_lib.lib.rs_vq_encode_end(plan.handle, out.data_ptr(), stream)),
+                  lambda: _lib.check(_lib.lib.rs_vq_encode(plan.handle, xf.data_ptr(), out.data_ptr(), stream)))
+        return out
+
+    @torch.no_grad()
+    def decode(self, h, force_not_quantize=False):
+        """h [B, embed_dim, h, w] -> image [B, 3, h*f, w*f] (reference autoencoder.py:33-40); the code indices of the
+        last call stay available as ``self.last_indices`` ([B, h, w] int32, -1 when not quantised)."""
+        plan, hf = self._decode_plan(h, "decode")
+        b, _, lh, lw = h.shape
+        out = self._image(h)
+        idx = torch.empty(b, lh, lw, dtype=torch.int32, device=h.device)
+        stream, fnq = _lib.current_stream(), int(bool(force_not_quantize))
+        self._run(plan, 1, lambda: _lib.check(_lib.lib.rs_vq_decode_begin(plan.handle, hf.data_ptr(), idx.data_ptr(), fnq, stream)),
+                  lambda: _lib.check(_lib.lib.rs_vq_decode_end(plan.handle, out.data_ptr(), stream)),
+                  lambda: _lib.check(_lib.lib.rs_vq_decode(plan.handle, hf.data_ptr(), out.data_ptr(), idx.data_ptr(), fnq, stream)))
+        self.last_indices = idx
+        return out
+
+    @torch.no_grad()
+    def decode_code(self, code_b):
+        """code_b [B, h, w] integer code indices -> image [B, 3, h*f, w*f]: the codebook rows (quantize.embed_code), then
+        decode(..., force_not_quantize=True) (reference autoencoder.py:42-45), bit-identical to that call.  Indices
+        must lie in [0, n_embed); a position with any other index decodes from NaN."""
+        if code_b.device.type != "cuda":
+            raise RuntimeError("resshift_b200.VQModelTorch.decode_code needs CUDA tensors (no CPU fallback)")
+        if code_b.dim() != 3 or code_b.dtype.is_floating_point or code_b.dtype.is_complex:
+            raise ValueError(f"expected integer code indices [B, h, w], got {tuple(code_b.shape)} {code_b.dtype}")
+        b, lh, lw = code_b.shape
+        f = self.cfg.downscale
+        plan = self.plan(1, b, lh * f, lw * f)
+        idx = code_b.to(torch.int32).contiguous()
+        out = torch.empty(b, self.cfg.out_ch, lh * f, lw * f, dtype=torch.float32, device=code_b.device)
+        _lib.check(_lib.lib.rs_vq_decode_code(plan.handle, idx.data_ptr(), out.data_ptr(), _lib.current_stream()))
+        return out
+
+    def forward(self, input, force_not_quantize=False):
+        return self.decode(self.encode(input), force_not_quantize)
+
+
+class EncoderKLTorch(_FirstStage):
+    """The encoder half of the KL first stage (reference autoencoder.py:88-112): ``encode`` / ``forward`` as in
+    AutoencoderKLTorch; its ``state_dict`` holds only ``encoder.*`` and ``quant_conv.*``."""
+
+    _create = "rs_kl_create"
+    _name = "EncoderKLTorch"
+    _encoder_only = True
+    # encode() samples the posterior by default: ResShiftSampler draws that noise ahead of the unit (posterior_noise=)
+    samples_posterior = True
+
+    def __init__(self, ddconfig, embed_dim):
+        cfg = _config(ddconfig, embed_dim, kl=True)
+        spec = kl_param_spec(cfg)
+        if self._encoder_only:
+            spec = [e for e in spec if e[0].startswith(("encoder.", "quant_conv."))]
+        super().__init__(cfg, spec, random_kl_state_dict(cfg, seed=0))
+        self.embed_dim = embed_dim
+
+    @torch.no_grad()
+    def encode(self, x, sample_posterior=True, return_moments=False, posterior_noise=None):
+        """x [B, 3, H, W] -> z [B, embed_dim, H/f, W/f] (and the moments [B, 2 embed_dim, H/f, W/f] with
+        ``return_moments``) — reference autoencoder.py:65-76 with DiagonalGaussianDistribution
+        (ldm/modules/distributions/distributions.py:24-37,61-62): z = mean + exp(0.5 clamp(logvar, -30, 20)) * noise, or
+        the mean without ``sample_posterior``.  The noise is ``posterior_noise`` when given (a [B, embed_dim, H/f, W/f]
+        tensor), else ``torch.randn`` of that shape on the CPU default generator, as the reference draws it."""
+        plan, xf = self._encode_plan(x, "encode")
+        z = self._latent(x)
+        moments = torch.empty(z.shape[0], 2 * z.shape[1], *z.shape[2:], dtype=torch.float32, device=x.device) \
+            if return_moments else None
+        noise = None
+        if sample_posterior:
+            if posterior_noise is None:
+                posterior_noise = torch.randn(z.shape)         # the reference's draw: CPU generator, then to the device
+            if tuple(posterior_noise.shape) != tuple(z.shape):
+                raise ValueError(f"posterior_noise must have shape {tuple(z.shape)}, got {tuple(posterior_noise.shape)}")
+            noise = posterior_noise.to(device=x.device, dtype=torch.float32).contiguous()
+        stream = _lib.current_stream()
+        args = (_lib.ptr(noise), z.data_ptr(), _lib.ptr(moments), stream)
+        self._run(plan, 0, lambda: _lib.check(_lib.lib.rs_kl_encode_begin(plan.handle, xf.data_ptr(), stream)),
+                  lambda: _lib.check(_lib.lib.rs_kl_encode_end(plan.handle, *args)),
+                  lambda: _lib.check(_lib.lib.rs_kl_encode(plan.handle, xf.data_ptr(), *args)))
+        return (z, moments) if return_moments else z
+
+    def forward(self, x, sample_posterior=True, return_moments=False):
+        return self.encode(x, sample_posterior, return_moments)
+
+
+class AutoencoderKLTorch(EncoderKLTorch):
+    """KL first stage (reference autoencoder.py:52-86): Encoder with double_z, quant_conv to the posterior's moments,
+    post_quant_conv and Decoder."""
+
+    _name = "AutoencoderKLTorch"
+    _encoder_only = False
+
+    @torch.no_grad()
+    def decode(self, z):
+        """z [B, embed_dim, h, w] -> image [B, 3, h*f, w*f] (reference autoencoder.py:78-81)."""
+        plan, zf = self._decode_plan(z, "decode")
+        out = self._image(z)
+        stream = _lib.current_stream()
+        self._run(plan, 1, lambda: _lib.check(_lib.lib.rs_kl_decode_begin(plan.handle, zf.data_ptr(), stream)),
+                  lambda: _lib.check(_lib.lib.rs_kl_decode_end(plan.handle, out.data_ptr(), stream)),
+                  lambda: _lib.check(_lib.lib.rs_kl_decode(plan.handle, zf.data_ptr(), out.data_ptr(), stream)))
+        return out
+
+    def forward(self, input, sample_posterior=True):
+        return self.decode(self.encode(input, sample_posterior, return_moments=False))
+
+
+class _VQPlan:
+    """First-stage (VQ-GAN or KL) engine bound to (encode | decode, batch, image H, image W): owns the workspace and the
+    native plan."""
+
+    def __init__(self, model: _FirstStage, which: int, batch: int, image_h: int, image_w: int, device):
         self.model = model
         h = C.c_void_p()
         _lib.check(_lib.lib.rs_vq_plan_create(model._engine, batch, image_h, image_w, which, C.byref(h)))

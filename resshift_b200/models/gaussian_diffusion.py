@@ -123,8 +123,9 @@ class ResShiftDiffusion:
             noise = torch.randn_like(x_start)
         return _tab(self.etas, t, x_start) * (y - x_start) + x_start + _tab(self.sqrt_etas * self.kappa, t, x_start) * noise
 
-    def encode_first_stage(self, y, first_stage_model, up_sample=False):
-        """reference models/gaussian_diffusion.py:500-515 (PyTorch bookend)"""
+    def encode_first_stage(self, y, first_stage_model, up_sample=False, posterior_noise=None):
+        """reference models/gaussian_diffusion.py:500-515 (PyTorch bookend).  ``posterior_noise``: the noise of a first
+        stage that samples its posterior (AutoencoderKLTorch.encode(posterior_noise=)); None lets it draw its own."""
         data_dtype = y.dtype
         if up_sample and self.sf != 1:
             y = bicubic_upsample(y, self.sf)
@@ -134,7 +135,10 @@ class ResShiftDiffusion:
         if model_dtype != data_dtype:
             y = y.type(model_dtype)
         with torch.no_grad():
-            out = first_stage_model.encode(y) * self.scale_factor
+            if posterior_noise is None:
+                out = first_stage_model.encode(y) * self.scale_factor
+            else:
+                out = first_stage_model.encode(y, posterior_noise=posterior_noise) * self.scale_factor
         return out.type(data_dtype) if model_dtype != data_dtype else out
 
     def decode_first_stage(self, z_sample, first_stage_model=None, consistencydecoder=None):

@@ -16,13 +16,14 @@ driven by its own thread (resshift_b200.device_pool).
 from __future__ import annotations
 
 import importlib
+import inspect
 import math
 import os
 import random
 import re
 from contextlib import nullcontext
 from pathlib import Path
-from typing import Any, Optional
+from typing import Any, NamedTuple, Optional
 
 import numpy as np
 import torch
@@ -88,6 +89,7 @@ _NATIVE_TARGETS = {
     "models.unet.UNetModelSwin": "resshift_b200.models.unet.UNetModelSwin",
     "models.script_util.create_gaussian_diffusion": "resshift_b200.models.script_util.create_gaussian_diffusion",
     "ldm.models.autoencoder.VQModelTorch": "resshift_b200.models.autoencoder.VQModelTorch",
+    "ldm.models.autoencoder.AutoencoderKLTorch": "resshift_b200.models.autoencoder.AutoencoderKLTorch",
 }
 
 
@@ -155,6 +157,25 @@ def plan_tiles(h: int, w: int, patch: int, stride: int, chop_bs: int):
     starts = [(hs, ws) for hs in hs_list for ws in ws_list]
     k = max(1, int(chop_bs))
     return hs_list, ws_list, min(patch, h), min(patch, w), [starts[i:i + k] for i in range(0, len(starts), k)]
+
+
+class UnitNoise(NamedTuple):
+    """The random numbers of one work unit, drawn ahead of it in one-GPU order (ResShiftSampler._unit_noises): the
+    loop's T+1 noise tensors [T+1, n, c, h, w] on the device, and the first stage's posterior noise [n, c, h, w] on the
+    CPU for an autoencoder that samples one (AutoencoderKLTorch), else None."""
+    loop: torch.Tensor
+    posterior: Optional[torch.Tensor]
+
+
+def _unsupported_posterior(autoencoder) -> bool:
+    """Whether ``autoencoder.encode`` samples a posterior (it takes ``sample_posterior``, as the reference's KL first
+    stages do) without accepting that noise from the caller: its draws would follow the units a rank runs."""
+    if autoencoder is None or getattr(autoencoder, "samples_posterior", False):
+        return False
+    try:
+        return "sample_posterior" in inspect.signature(autoencoder.encode).parameters
+    except (TypeError, ValueError):
+        return False
 
 
 def tile_counts(units, schedule, world: int):
@@ -396,14 +417,20 @@ class ResShiftSampler(BaseSampler):
 
     def _latent_spec(self, n, h, w, dtype):
         """Shape and dtype of z_y = encode_first_stage(y, up_sample=True) for an [n, 3, h, w] input (after the
-        padding_offset reflect-pad) of dtype ``dtype``, derived from the configs without running the encoder: the VQ
-        first stage keeps the data dtype (encode_first_stage) and downsamples by 2^(len(ch_mult) - 1)."""
+        padding_offset reflect-pad) of dtype ``dtype``, derived from the configs without running the encoder: the first
+        stage (VQ or KL: both have ``embed_dim`` latent channels) keeps the data dtype (encode_first_stage) and
+        downsamples by 2^(len(ch_mult) - 1)."""
         sf = self.base_diffusion.sf
         ae = self.configs.autoencoder.params
         f = 2 ** (len(ae.ddconfig.ch_mult) - 1)
         return (n, int(ae.embed_dim), int(h * sf) // f, int(w * sf) // f), dtype
 
     def _check_shardable(self, mode="shard_tiles"):
+        if _unsupported_posterior(self.autoencoder):
+            raise RuntimeError(
+                f"{mode} needs every random number of a unit drawn ahead of it in one-GPU order; this autoencoder "
+                f"({type(self.autoencoder).__name__}) samples its posterior inside encode and cannot take that noise "
+                "(use resshift_b200.models.autoencoder.AutoencoderKLTorch)")
         if not self.base_diffusion._native_ok(self.model, clip_denoised=(self.autoencoder is None), denoised_fn=None,
                                               model_kwargs={"lq": None}):
             raise RuntimeError(
@@ -412,27 +439,31 @@ class ResShiftSampler(BaseSampler):
                 "UNetModelSwin, predict_type other than xstart, or T outside 2..64)")
 
     def _sample_unit(self, y0, mask, noises, spec, replica):
-        """sample_func with its noise given: reflect-pad, encode_first_stage(up_sample=True), sample_latent(noises=),
-        decode_first_stage, crop, clamp — the same steps, in the same order.  ``spec`` is the z_y shape and dtype the
-        noise was drawn for; it must be the real one.  ``replica``: a device_pool.Replica whose models run the unit, or
+        """sample_func with its noise given (a UnitNoise): reflect-pad, encode_first_stage(up_sample=True) with the
+        posterior noise, sample_latent(noises=), decode_first_stage, crop, clamp — the same steps, in the same order.
+        ``spec`` is the z_y shape and dtype the noise was drawn for; it must be the real one.  ``replica``: a device_pool.Replica whose models run the unit, or
         None for this sampler's."""
         model, autoencoder = (self.model, self.autoencoder) if replica is None else (replica.model, replica.autoencoder)
         diff = self.base_diffusion
 
         def run(y, model_kwargs):
-            z_y = diff.encode_first_stage(y, autoencoder, up_sample=True)
+            z_y = diff.encode_first_stage(y, autoencoder, up_sample=True, posterior_noise=noises.posterior)
             assert (tuple(z_y.shape), z_y.dtype, z_y.is_contiguous()) == (spec[0], spec[1], True), \
                 f"derived z_y {spec} != real {tuple(z_y.shape)} {z_y.dtype}"
-            final = diff.sample_latent(z_y, model, model_kwargs, noises=noises)
+            final = diff.sample_latent(z_y, model, model_kwargs, noises=noises.loop)
             with torch.no_grad():
                 return diff.decode_first_stage(final, first_stage_model=autoencoder)
         return self._pad_crop(y0, mask, run)
 
     def _unit_noises(self, lqs, noise_repeat, units):
-        """Yields (unit index, noises, z_y spec) for every unit of ``units`` in order: its T+1 noise tensors drawn as
+        """Yields (unit index, UnitNoise, z_y spec) for every unit of ``units`` in order: its T+1 noise tensors drawn as
         GaussianDiffusion.draw_noises does (after setup_seed with noise_repeat, as sample_func does), on the device of
-        ``lqs``, so that the CUDA generator is where a one-GPU run has it whichever units run here."""
+        ``lqs``, so that the CUDA generator is where a one-GPU run has it whichever units run here.  For an
+        autoencoder that samples its posterior (AutoencoderKLTorch), the unit's posterior noise is drawn too, as its
+        encode would draw it (torch.randn on the CPU generator, after that setup_seed), so that generator also follows
+        the one-GPU run."""
         offset = self.padding_offset
+        posterior = getattr(self.autoencoder, "samples_posterior", False)
         for i, (g, starts, th, tw) in enumerate(units):
             lq = lqs[g]
             with self._autocast():
@@ -440,9 +471,10 @@ class ResShiftSampler(BaseSampler):
                     self.setup_seed()
                 spec = self._latent_spec(lq.shape[0] * len(starts), math.ceil(th / offset) * offset,
                                          math.ceil(tw / offset) * offset, lq.dtype)
+                post = torch.randn(spec[0]) if posterior else None
                 noises = self.base_diffusion.draw_noises(torch.empty(spec[0], dtype=spec[1], device=lq.device),
                                                          noise_repeat=noise_repeat)
-            yield i, noises, spec
+            yield i, UnitNoise(noises, post), spec
 
     @staticmethod
     def _unit_input(lqs, masks, unit):

@@ -31,6 +31,7 @@ class VQConfig:
     attn_resolutions: Sequence[int] = ()
     dropout: float = 0.0
     double_z: bool = False
+    kl: bool = False            # AutoencoderKLTorch: double_z encoder, posterior moments, no codebook (n_embed unused)
 
     def __post_init__(self):
         self.ch_mult = tuple(int(v) for v in self.ch_mult)
@@ -39,7 +40,7 @@ class VQConfig:
         self.num_res_blocks = tuple(int(v) for v in self.num_res_blocks)
         self.attn_resolutions = tuple(int(v) for v in self.attn_resolutions)
         # what this implementation covers (every shipped yaml satisfies these)
-        assert not self.double_z and self.dropout == 0 and len(self.attn_resolutions) == 0
+        assert self.double_z == self.kl and self.dropout == 0 and len(self.attn_resolutions) == 0
         assert len(self.num_res_blocks) == len(self.ch_mult)
 
     @property
@@ -51,12 +52,14 @@ class VQConfig:
         return 2 ** (self.levels - 1)
 
     def ddconfig(self) -> dict:
-        return {"double_z": False, "z_channels": self.z_channels, "resolution": self.resolution,
+        return {"double_z": self.double_z, "z_channels": self.z_channels, "resolution": self.resolution,
                 "in_channels": self.in_channels, "out_ch": self.out_ch, "ch": self.ch, "ch_mult": list(self.ch_mult),
                 "num_res_blocks": list(self.num_res_blocks), "attn_resolutions": list(self.attn_resolutions),
                 "dropout": 0.0, "padding_mode": "zeros"}
 
     def to_kwargs(self) -> dict:
+        if self.kl:
+            return {"ddconfig": self.ddconfig(), "embed_dim": self.embed_dim}
         return {"ddconfig": self.ddconfig(), "n_embed": self.n_embed, "embed_dim": self.embed_dim}
 
 
@@ -68,6 +71,17 @@ def vq_preset(name: str) -> VQConfig:
                         num_res_blocks=(1, 2, 3, 4))
     if name == "tiny":                                  # not shipped: same topology, narrow, for fast tests
         return VQConfig(n_embed=512, resolution=64, ch=32, ch_mult=(1, 2, 4), num_res_blocks=(1, 2, 2))
+    raise KeyError(name)
+
+
+def kl_preset(name: str) -> VQConfig:
+    """KL first stages (AutoencoderKLTorch); no shipped ResShift config uses one, so these are test configurations."""
+    if name == "f8":                                    # Stable-Diffusion-style f8 KL autoencoder
+        return VQConfig(embed_dim=4, z_channels=4, resolution=256, ch=128, ch_mult=(1, 2, 4, 4), num_res_blocks=(2, 2, 2, 2),
+                        double_z=True, kl=True)
+    if name == "tiny":                                  # the VQ "tiny" topology with a KL bottleneck
+        return VQConfig(embed_dim=4, z_channels=4, resolution=64, ch=32, ch_mult=(1, 2, 4), num_res_blocks=(1, 2, 2),
+                        double_z=True, kl=True)
     raise KeyError(name)
 
 
@@ -124,6 +138,20 @@ def decoder_blocks(cfg: VQConfig):
 
 
 def vq_param_spec(cfg: VQConfig) -> Spec:
+    """VQModelTorch's state_dict inventory (reference ldm/models/autoencoder.py:21-26)."""
+    assert not cfg.kl
+    return _first_stage_spec(cfg)
+
+
+def kl_param_spec(cfg: VQConfig) -> Spec:
+    """AutoencoderKLTorch's state_dict inventory (reference ldm/models/autoencoder.py:58-62): the encoder ends in
+    2 z_channels, quant_conv maps them to the 2 embed_dim moments, and there is no codebook."""
+    assert cfg.kl
+    return _first_stage_spec(cfg)
+
+
+def _first_stage_spec(cfg: VQConfig) -> Spec:
+    z_out = 2 * cfg.z_channels if cfg.double_z else cfg.z_channels
     s: Spec = []
     # encoder
     s += _conv("encoder.conv_in", cfg.in_channels, cfg.ch, 3)
@@ -134,7 +162,7 @@ def vq_param_spec(cfg: VQConfig) -> Spec:
             s += _conv(f"encoder.down.{i}.downsample.conv", blocks[-1][1], blocks[-1][1], 3)
     top = cfg.ch * cfg.ch_mult[-1]
     s += _resblock("encoder.mid.block_1", top, top) + _attn("encoder.mid.attn_1", top) + _resblock("encoder.mid.block_2", top, top)
-    s += _gn("encoder.norm_out", top) + _conv("encoder.conv_out", top, cfg.z_channels, 3)
+    s += _gn("encoder.norm_out", top) + _conv("encoder.conv_out", top, z_out, 3)
     # decoder (state_dict order follows module registration: conv_in, mid, up.0 .. up.L-1, norm_out, conv_out)
     s += _conv("decoder.conv_in", cfg.z_channels, top, 3)
     s += _resblock("decoder.mid.block_1", top, top) + _attn("decoder.mid.attn_1", top) + _resblock("decoder.mid.block_2", top, top)
@@ -146,9 +174,13 @@ def vq_param_spec(cfg: VQConfig) -> Spec:
         if up:
             s += _conv(f"decoder.up.{i}.upsample.conv", blocks[-1][1], blocks[-1][1], 3)
     s += _gn("decoder.norm_out", cfg.ch * cfg.ch_mult[0]) + _conv("decoder.conv_out", cfg.ch * cfg.ch_mult[0], cfg.out_ch, 3)
-    # quantiser and the two 1x1 convs around it
-    s += [("quantize.embedding.weight", (cfg.n_embed, cfg.embed_dim), "codebook")]
-    s += _conv("quant_conv", cfg.z_channels, cfg.embed_dim, 1) + _conv("post_quant_conv", cfg.embed_dim, cfg.z_channels, 1)
+    # quantiser (VQ) and the two 1x1 convs around it / around the posterior (KL)
+    if cfg.kl:
+        s += _conv("quant_conv", z_out, 2 * cfg.embed_dim, 1)
+    else:
+        s += [("quantize.embedding.weight", (cfg.n_embed, cfg.embed_dim), "codebook")]
+        s += _conv("quant_conv", cfg.z_channels, cfg.embed_dim, 1)
+    s += _conv("post_quant_conv", cfg.embed_dim, cfg.z_channels, 1)
     return s
 
 
@@ -156,9 +188,18 @@ def random_vq_state_dict(cfg: VQConfig, seed: int = 0) -> Dict[str, torch.Tensor
     """Deterministic synthetic weights (same values in the build container and on the GPU box): fan-in scaled convs with a
     reduced gain on the residual-branch outputs so activations stay in fp16 range, and a codebook with the spread of
     the latents it quantises (the reference's uniform(+-1/n_e) init would make every code equally near)."""
+    return _random_state_dict(vq_param_spec(cfg), seed)
+
+
+def random_kl_state_dict(cfg: VQConfig, seed: int = 0) -> Dict[str, torch.Tensor]:
+    """Deterministic synthetic weights of AutoencoderKLTorch, drawn as random_vq_state_dict draws them."""
+    return _random_state_dict(kl_param_spec(cfg), seed)
+
+
+def _random_state_dict(spec: Spec, seed: int) -> Dict[str, torch.Tensor]:
     g = torch.Generator().manual_seed(seed)
     sd: Dict[str, torch.Tensor] = {}
-    for name, shape, role in vq_param_spec(cfg):
+    for name, shape, role in spec:
         if role in ("conv3", "conv1"):
             fan_in = math.prod(shape[1:])
             gain = 0.35 if name.endswith(("conv2.weight", "proj_out.weight")) else 1.0
