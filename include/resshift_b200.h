@@ -35,8 +35,11 @@ extern "C" {
 #define RS_MAX_LEVELS 8
 
 /* Keyword arguments of UNetModelSwin.__init__ (reference models/unet.py:632-657) that shipped yaml
- * files vary.  Unsupported variants (dims != 2, resblock_updown, patch_norm, dropout > 0,
- * use_scale_shift_norm = False) are rejected by rs_unet_create. */
+ * files vary.  The constructor options the shipped files leave at one value are in rs_unet_options.
+ * Covered: dims = 2 (the struct has no field for it), cond_lq = True (the reference cannot run
+ * cond_lq = False), any dropout (identity at inference), cond_mask with or without an LQ feature
+ * extractor.  Refused by rs_unet_create / rs_unet_create_ex: window_size != 8 and head dims
+ * (swin_embed_dim / swin_heads) other than 32, the specialisations of the attention kernels. */
 typedef struct rs_unet_config {
   int32_t image_size;
   int32_t in_channels;
@@ -55,6 +58,15 @@ typedef struct rs_unet_config {
   int32_t cond_mask;
   int32_t lq_size;
 } rs_unet_config;
+
+/* The remaining UNetModelSwin.__init__ options, each 0 or 1.  rs_unet_create uses the values of every
+ * shipped yaml: {use_scale_shift_norm 1, resblock_updown 0, conv_resample 1, patch_norm 0}. */
+typedef struct rs_unet_options {
+  int32_t use_scale_shift_norm;   /* 0: ResBlock adds emb_layers(emb) to h before out_layers (unet.py:202-205) */
+  int32_t resblock_updown;        /* 1: ResBlocks with down / up = True resample (unet.py:187-193)            */
+  int32_t conv_resample;          /* 0: Downsample = 2x2 average pool, Upsample = nearest 2x, no conv         */
+  int32_t patch_norm;             /* 1: GroupNorm32 after patch_embed.proj and patch_unembed.proj              */
+} rs_unet_options;
 
 /* ``autoencoder.params`` of the shipped yaml files: VQModelTorch(ddconfig, n_embed, embed_dim)
  * (reference ldm/models/autoencoder.py:12-26; ddconfig -> ldm/modules/diffusionmodules/model.py:452-470,563-581).
@@ -80,6 +92,7 @@ const char* rs_last_error(void);
 
 /* ---- denoiser: models.unet.UNetModelSwin (reference models/unet.py:603-912) ------------------ */
 int rs_unet_create(const rs_unet_config* cfg, rs_engine** out);
+int rs_unet_create_ex(const rs_unet_config* cfg, const rs_unet_options* opts, rs_engine** out);
 void rs_unet_destroy(rs_engine* e);
 /* state_dict inventory (reference key names / shapes; utils/util_net.py:86-98 relies on them) */
 int rs_unet_param_count(const rs_engine* e);

@@ -31,6 +31,12 @@ class UNetConfigC(C.Structure):
     ]
 
 
+class UNetOptionsC(C.Structure):
+    """Mirror of ``rs_unet_options``."""
+    _fields_ = [("use_scale_shift_norm", C.c_int32), ("resblock_updown", C.c_int32), ("conv_resample", C.c_int32),
+                ("patch_norm", C.c_int32)]
+
+
 class VQConfigC(C.Structure):
     """Mirror of ``rs_vq_config``."""
     _fields_ = [
@@ -46,6 +52,7 @@ _SIGNATURES = {
     "rs_version": (C.c_int, []),
     "rs_last_error": (C.c_char_p, []),
     "rs_unet_create": (C.c_int, [C.POINTER(UNetConfigC), C.POINTER(_P)]),
+    "rs_unet_create_ex": (C.c_int, [C.POINTER(UNetConfigC), C.POINTER(UNetOptionsC), C.POINTER(_P)]),
     "rs_unet_destroy": (None, [_P]),
     "rs_unet_param_count": (C.c_int, [_P]),
     "rs_unet_param_info": (C.c_int, [_P, C.c_int, C.c_char_p, C.c_size_t, C.POINTER(C.c_int32), C.POINTER(C.c_int32),
@@ -176,6 +183,13 @@ def make_config(cfg) -> UNetConfigC:
     c.window_size, c.mlp_ratio = cfg.window_size, float(cfg.mlp_ratio)
     c.cond_mask, c.lq_size = int(cfg.cond_mask), cfg.lq_size
     return c
+
+
+def make_options(cfg) -> UNetOptionsC:
+    o = UNetOptionsC()
+    o.use_scale_shift_norm, o.resblock_updown = int(cfg.use_scale_shift_norm), int(cfg.resblock_updown)
+    o.conv_resample, o.patch_norm = int(cfg.conv_resample), int(cfg.patch_norm)
+    return o
 
 
 def make_vq_config(cfg) -> VQConfigC:

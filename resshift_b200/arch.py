@@ -39,11 +39,11 @@ def _gn(name: str, c: int) -> List[Spec]:
     return [(f"{name}.weight", (c,), "gn_w"), (f"{name}.bias", (c,), "gn_b")]
 
 
-def _resblock(name: str, cin: int, cout: int, emb: int) -> List[Spec]:
+def _resblock(name: str, cin: int, cout: int, emb: int, scale_shift: bool = True) -> List[Spec]:
     s: List[Spec] = []
     s += _gn(f"{name}.in_layers.0", cin)
     s += _conv(f"{name}.in_layers.2", cin, cout, 3)
-    s += _linear(f"{name}.emb_layers.1", emb, 2 * cout)
+    s += _linear(f"{name}.emb_layers.1", emb, (2 if scale_shift else 1) * cout)
     s += _gn(f"{name}.out_layers.0", cout)
     s += _conv(f"{name}.out_layers.3", cout, cout, 3)
     if cin != cout:
@@ -65,7 +65,11 @@ def _basic_layer(name: str, cfg: UNetConfig, c: int, res: int) -> List[Spec]:
     hidden = int(e * cfg.mlp_ratio)
     s: List[Spec] = []
     s += _conv(f"{name}.patch_embed.proj", c, e, 1)
+    if cfg.patch_norm:
+        s += _gn(f"{name}.patch_embed.norm", e)
     s += _conv(f"{name}.patch_unembed.proj", e, c, 1)
+    if cfg.patch_norm:
+        s += _gn(f"{name}.patch_unembed.norm", c)
     for i in range(cfg.swin_depth):
         b = f"{name}.blocks.{i}"
         if i % 2 == 1 and shift > 0:
@@ -87,8 +91,12 @@ def unet_block_plan(cfg: UNetConfig):
 
     Returns ``(input_blocks, middle, output_blocks)``; every block is a list of layer tuples
     ``("conv", cin, cout)``, ``("res", cin, cout)``, ``("swin", c, res)``,
-    ``("down", c)``, ``("up", c)``; restates reference models/unet.py:704-857.
+    ``("down", c)``, ``("up", c)`` (a conv, or with ``conv_resample=False`` a parameterless pool / upsample), or with
+    ``resblock_updown`` ``("res_down", c)``, ``("res_up", c)`` (ResBlocks with down / up = True);
+    restates reference models/unet.py:704-857.
     """
+    down = "res_down" if cfg.resblock_updown else "down"
+    up = "res_up" if cfg.resblock_updown else "up"
     mc = cfg.model_channels
     ch = int(cfg.channel_mult[0] * mc)
     in_ch = cfg.in_channels + cfg.lq_feat_channels
@@ -104,7 +112,7 @@ def unet_block_plan(cfg: UNetConfig):
             input_blocks.append(layers)
             chans.append(ch)
         if level != len(cfg.channel_mult) - 1:
-            input_blocks.append([("down", ch)])
+            input_blocks.append([(down, ch)])
             chans.append(ch)
             ds //= 2
     middle = [("res", ch, ch), ("swin", ch, ds), ("res", ch, ch)]
@@ -117,7 +125,7 @@ def unet_block_plan(cfg: UNetConfig):
             if ds in cfg.attention_resolutions and i == 0:
                 layers.append(("swin", ch, ds))
             if level and i == cfg.num_res_blocks[level]:
-                layers.append(("up", ch))
+                layers.append((up, ch))
                 ds *= 2
             output_blocks.append(layers)
     return input_blocks, middle, output_blocks
@@ -144,12 +152,14 @@ def unet_param_spec(cfg: UNetConfig) -> List[Spec]:
             if kind == "conv":
                 out += _conv(f"{prefix}.{j}", layer[1], layer[2], 3)
             elif kind == "res":
-                out += _resblock(f"{prefix}.{j}", layer[1], layer[2], emb)
+                out += _resblock(f"{prefix}.{j}", layer[1], layer[2], emb, cfg.use_scale_shift_norm)
+            elif kind in ("res_down", "res_up"):
+                out += _resblock(f"{prefix}.{j}", layer[1], layer[1], emb, cfg.use_scale_shift_norm)
             elif kind == "swin":
                 out += _basic_layer(f"{prefix}.{j}", cfg, layer[1], layer[2])
-            elif kind == "down":
+            elif kind == "down" and cfg.conv_resample:
                 out += _conv(f"{prefix}.{j}.op", layer[1], layer[1], 3)
-            elif kind == "up":
+            elif kind == "up" and cfg.conv_resample:
                 out += _conv(f"{prefix}.{j}.conv", layer[1], layer[1], 3)
         return out
 

@@ -45,11 +45,19 @@ class UNetConfig:
         self.num_res_blocks = tuple(int(v) for v in self.num_res_blocks)
         self.channel_mult = tuple(int(v) for v in self.channel_mult)
         self.attention_resolutions = tuple(int(v) for v in self.attention_resolutions)
-        # What this implementation covers (every shipped yaml satisfies these).
-        assert self.dims == 2 and self.conv_resample and not self.resblock_updown
-        assert self.use_scale_shift_norm and not self.patch_norm and self.dropout == 0
+        # What this implementation covers: every constructor option the reference can run, except the attention kernels'
+        # specialisations.  dropout is the identity at inference.
         assert len(self.num_res_blocks) == len(self.channel_mult)
-        assert self.cond_lq, "the ResShift denoiser is always conditioned on the LQ image"
+        if self.dims != 2:
+            raise ValueError(f"dims={self.dims}: only 2-D UNets are covered (every ResShift config uses dims=2)")
+        if not self.cond_lq:
+            raise ValueError("cond_lq=False: the reference cannot run it either (it widens the first conv by the LQ "
+                             "channels but skips the concatenation when lq is None)")
+        if self.window_size != 8:
+            raise ValueError(f"window_size={self.window_size}: the window-attention kernels are specialised for 8x8 windows")
+        if self.swin_embed_dim % self.swin_heads or self.swin_embed_dim // self.swin_heads != 32:
+            raise ValueError(f"head dim {self.swin_embed_dim / self.swin_heads:g}: the window-attention kernels are "
+                             f"specialised for a head dim of 32 (num_head_channels=32)")
 
     # -- derived quantities (reference models/unet.py:689-709) -----------------
     @property

@@ -63,8 +63,9 @@ struct ConvParams {
                          //    shared memory and are summed through distributed shared memory (no scratch, no second kernel)
   int msub;              // 128-pixel sub-tiles per CTA (1 or 2): two sub-tiles share every weight tile (fewer operand bytes per MMA)
   // epilogue
-  const float* bias;                 // [Cout] fp32 or nullptr
-  const __half* residual;            // optional, same pixel grid as the output
+  const float* bias;                 // [Cout] fp32 or nullptr; with bias_sN > 0 one row per image
+  int bias_sN;                       // elements between the bias rows of consecutive images (0: one row for all)
+  const __half* residual;           // optional, same pixel grid as the output
   long long res_sN, res_sH, res_sW;  // strides in elements
   __half* out;                       // NHWC fp16 view (may be nullptr when out_f32 is set)
   long long out_sN, out_sH, out_sW;
@@ -292,8 +293,21 @@ __global__ void __launch_bounds__(kConvThreads, (BN * MS <= 128) ? 2 : 1) conv_g
         // Swizzle<B,4,3>: the 16-byte unit index is XORed with address bits [7, 7+B); row pitch is 2*bc bytes
         auto swz_of = [&](int r) { return (bc == 64) ? (r & 7) : (bc == 32 ? ((r >> 1) & 3) : ((r >> 2) & 1)); };
         float* wsum_all = reinterpret_cast<float*>(sepi + (size_t)MS * sub_bytes);
-        for (int i = etid; i < BN; i += 32 * kConvEpiWarps)
-          s_bias[i] = (p.bias && col0 + i < p.Cout) ? __ldg(p.bias + col0 + i) : 0.f;
+        // per-image bias (one sub-tile per CTA only: conv_finalize never pairs it with msub = 2): s_bias holds [bn][BN],
+        // one row per image of the tile; with tiles of at most 8 images, rows rA and rB = rA + 8 share an image
+        const bool bias_rows = MS == 1 && p.bias_sN != 0;
+        if (!bias_rows) {
+          for (int i = etid; i < BN; i += 32 * kConvEpiWarps)
+            s_bias[i] = (p.bias && col0 + i < p.Cout) ? __ldg(p.bias + col0 + i) : 0.f;
+        } else {
+          const int nb = mt0 / (p.tiles_w * p.tiles_h) * p.bn;     // first image of the tile
+          for (int il = 0; il < p.bn; ++il) {
+            const int n = nb + il;
+            for (int c = etid; c < BN; c += 32 * kConvEpiWarps)
+              s_bias[il * BN + c] = (col0 + c < p.Cout && n < p.Nimg) ? __ldg(p.bias + n * p.bias_sN + col0 + c) : 0.f;
+          }
+        }
+        const float* s_bias_row = s_bias + (bias_rows ? (rA / (p.bw * p.bh)) * BN : 0);
         if (p.tma_res && etid == 0) {
           mbar_arrive_expect_tx(res_bar, (uint32_t)(MS * sub_bytes));
           for (int sub = 0; sub < MS; ++sub) {
@@ -312,7 +326,7 @@ __global__ void __launch_bounds__(kConvThreads, (BN * MS <= 128) ? 2 : 1) conv_g
 #pragma unroll
           for (int j = 0; j < BN / 8; ++j) {
             const int c = 8 * j + 2 * (lane & 3);
-            const float2 b2 = *reinterpret_cast<const float2*>(s_bias + c);
+            const float2 b2 = *reinterpret_cast<const float2*>(s_bias_row + c);
             uint8_t* blk = sblk + (size_t)(c >> bshift) * blk_bytes + 4 * (lane & 3);
             const int u = (c & (bc - 1)) >> 3;         // 16-byte unit of columns 8j..8j+7 inside the block
 #pragma unroll
@@ -397,7 +411,7 @@ __global__ void __launch_bounds__(kConvThreads, (BN * MS <= 128) ? 2 : 1) conv_g
                 const int col = col0 + 8 * j + 2 * (lane & 3) + e;
                 if (col >= p.Cout) continue;
                 float f = acc[sub][4 * j + 2 * hr + e];
-                if (p.bias) f += __ldg(p.bias + col);
+                if (p.bias) f += __ldg(p.bias + n * p.bias_sN + col);
                 if (p.act == ACT_GELU) f = gelu_erf_f(f);
                 else if (p.act == ACT_SILU) f = silu_f(f);
                 if (rrow) f += __half2float(rrow[col]);
@@ -450,7 +464,7 @@ __global__ void __launch_bounds__(kConvThreads, (BN * MS <= 128) ? 2 : 1) conv_g
         if (ok) {
           if (p.bias) {
 #pragma unroll
-            for (int j = 0; j < 8; ++j) acc[j] += __ldg(p.bias + col + j);
+            for (int j = 0; j < 8; ++j) acc[j] += __ldg(p.bias + n * p.bias_sN + col + j);
           }
           if (p.act == ACT_GELU) {
 #pragma unroll
@@ -572,7 +586,7 @@ __global__ void conv_simt_kernel(const __grid_constant__ ConvParams p, const __g
         acc = fmaf(av.y, wv.y, acc);
       }
     }
-    if (p.bias) acc += p.bias[co];
+    if (p.bias) acc += p.bias[n * p.bias_sN + co];
     if (p.act == ACT_GELU) acc = gelu_erf_f(acc);
     else if (p.act == ACT_SILU) acc = silu_f(acc);
     if (p.residual) acc += __half2float(p.residual[n * p.res_sN + h * p.res_sH + w * p.res_sW + co]);

@@ -19,6 +19,7 @@ struct PackInputParams {
   const float* x; int Cx;             // [N, Cx, H, W] fp32
   const float* scale_tab; int scale_idx;   // optional per-step table; value 1/sqrt(eta*kappa^2+1)
   const float* lq_nchw; int Cl;       // [N, Cl, H, W] fp32 or nullptr
+  const float* mask_nchw;             // [N, 1, H, W] fp32 after lq_nchw (cond_mask without feature extractor) or nullptr
   const __half* lq_nhwc; int lq_ld;   // [N*H*W, Cl] fp16 or nullptr
   __half* out; int Cpad;              // [N*H*W, Cpad]
   int N, HW;
@@ -40,6 +41,7 @@ __global__ void pack_input_kernel(const PackInputParams p) {
   for (; c < p.Cx; ++c) o[c] = __float2half_rn(p.x[((long long)n * p.Cx + c) * p.HW + hw] * sc);
   if (p.lq_nchw) {
     for (int j = 0; j < p.Cl; ++j, ++c) o[c] = __float2half_rn(p.lq_nchw[((long long)n * p.Cl + j) * p.HW + hw]);
+    if (p.mask_nchw) o[c++] = __float2half_rn(p.mask_nchw[(long long)n * p.HW + hw]);
   } else if (p.lq_nhwc) {
     for (int j = 0; j < p.Cl; ++j, ++c) o[c] = p.lq_nhwc[pix * p.lq_ld + j];
   }
@@ -69,13 +71,42 @@ __global__ void pack_image_kernel(const PackImageParams p) {
 }
 
 // ------------------------------------------------------------------------------------------------
-// nearest x2 upsample, NHWC fp16 (reference Upsample.forward, models/unet.py:71-81)
+// 2x resampling, NHWC fp16 views, 16-byte vectors: nearest x2 upsample (reference Upsample.forward,
+// models/unet.py:71-81) and 2x2 average pool (Downsample without conv, avg_pool2d, :83-108)
 // ------------------------------------------------------------------------------------------------
 struct UpsampleParams {
-  const __half* x; long long x_sN; int x_ld;   // [N, H, W, C] view
-  __half* y;                                   // [N, 2H, 2W, C] contiguous
+  const __half* x; long long x_sN; int x_ld;   // [N, H, W, C] view (the input, for both directions)
+  __half* y; long long y_sN; int y_ld;         // [N, 2H, 2W, C] (upsample) or [N, H/2, W/2, C] (pool) view
   int N, H, W, C;
 };
+__global__ void avgpool2x2_kernel(const UpsampleParams p) {
+  pdl_trigger();
+  pdl_wait();
+  const int vecs = p.C >> 3, Ho = p.H / 2, Wo = p.W / 2;
+  const long long total = (long long)p.N * Ho * Wo * vecs;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total;
+       i += (long long)gridDim.x * blockDim.x) {
+    const int v = (int)(i % vecs);
+    long long q = i / vecs;
+    const int ox = (int)(q % Wo); q /= Wo;
+    const int oy = (int)(q % Ho); q /= Ho;
+    const int n = (int)q;
+    const __half* src = p.x + n * p.x_sN + ((long long)(2 * oy) * p.W + 2 * ox) * p.x_ld + v * 8;
+    float acc[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const uint4 raw = *reinterpret_cast<const uint4*>(src + ((long long)(k >> 1) * p.W + (k & 1)) * p.x_ld);
+      const __half2* h = reinterpret_cast<const __half2*>(&raw);
+#pragma unroll
+      for (int j = 0; j < 4; ++j) { const float2 f = __half22float2(h[j]); acc[2 * j] += f.x; acc[2 * j + 1] += f.y; }
+    }
+    uint4 o;
+    __half2* oh = reinterpret_cast<__half2*>(&o);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) oh[j] = __floats2half2_rn(0.25f * acc[2 * j], 0.25f * acc[2 * j + 1]);
+    *reinterpret_cast<uint4*>(p.y + n * p.y_sN + ((long long)oy * Wo + ox) * p.y_ld + v * 8) = o;
+  }
+}
 __global__ void upsample2x_kernel(const UpsampleParams p) {
   pdl_trigger();
   pdl_wait();
@@ -89,7 +120,7 @@ __global__ void upsample2x_kernel(const UpsampleParams p) {
     const int oy = (int)(q % (2 * p.H)); q /= 2 * p.H;
     const int n = (int)q;
     const uint4 raw = *reinterpret_cast<const uint4*>(p.x + n * p.x_sN + ((long long)(oy >> 1) * p.W + (ox >> 1)) * p.x_ld + v * 8);
-    *reinterpret_cast<uint4*>(p.y + (((long long)n * 2 * p.H + oy) * 2 * p.W + ox) * p.C + v * 8) = raw;
+    *reinterpret_cast<uint4*>(p.y + n * p.y_sN + ((long long)oy * 2 * p.W + ox) * p.y_ld + v * 8) = raw;
   }
 }
 
@@ -109,6 +140,14 @@ __global__ void timestep_embedding_kernel(const float* __restrict__ t, float* __
   out[(long long)b * dim + k] = cosf(a);
   out[(long long)b * dim + half_dim + k] = sinf(a);
   if ((dim & 1) && k == 0) out[(long long)b * dim + dim - 1] = 0.f;
+}
+
+// out = a + b (fp32, load time: the folded bias of a ResBlock without scale-shift norm)
+__global__ void add_f32_kernel(const float* __restrict__ a, const float* __restrict__ b, float* __restrict__ out, int n) {
+  pdl_trigger();
+  pdl_wait();
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) out[i] = a[i] + b[i];
 }
 
 // out[b, o] = bias[o] + sum_k act(x[b, k]) * W[o, k];  W fp16 row-major [O, K], x/out fp32.
@@ -193,7 +232,7 @@ __global__ void prior_sample_kernel(const float* __restrict__ zy, const float* _
 struct SplitKReduceParams {
   const float* partial;     // [S][N*HW][C]
   int S, N, HW, C;
-  const float* bias;
+  const float* bias; int bias_sN;         // bias_sN > 0: one bias row per image
   const __half* residual; long long res_sN; int res_ld;
   __half* out; long long out_sN; int out_ld;
   int act;
@@ -224,7 +263,7 @@ __global__ void __launch_bounds__(256) splitk_reduce_kernel(const __grid_constan
     const int c = c_begin + vec * 8;
     float bs[8];
 #pragma unroll
-    for (int j = 0; j < 8; ++j) bs[j] = p.bias ? p.bias[c + j] : 0.f;
+    for (int j = 0; j < 8; ++j) bs[j] = p.bias ? p.bias[n * p.bias_sN + c + j] : 0.f;
     for (int r = r0 + rl; r < r1; r += lanes) {
       const long long pix = (long long)n * p.HW + r;
       float acc[8];

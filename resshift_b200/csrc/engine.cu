@@ -45,6 +45,7 @@ struct rs_engine {
   int kind = 0;                 // 0: UNetModelSwin denoiser, 1: VQ-GAN first stage (vq.inc); the parameter store is shared
   rs_vq_config vq{};
   rs_unet_config cfg;
+  rs_unet_options opt{1, 0, 1, 0};
   std::vector<Param> params;
   std::map<std::string, int> index;
   size_t arena_bytes = 0;
@@ -84,7 +85,9 @@ struct rs_engine {
 // ------------------------------------------------------------------------------------------------
 namespace {
 
-struct Layer { int kind; int a, b; };   // kind: 0 conv(cin,cout) 1 res(cin,cout) 2 swin(c,res) 3 down(c) 4 up(c)
+// kind: 0 conv(cin,cout) 1 res(cin,cout) 2 swin(c,res) 3 down(c) 4 up(c) 5 res with down=True(c) 6 res with up=True(c)
+struct Layer { int kind; int a, b; };
+enum { L_CONV = 0, L_RES, L_SWIN, L_DOWN, L_UP, L_RES_DOWN, L_RES_UP };
 struct Topology {
   std::vector<std::vector<Layer>> input_blocks, output_blocks;
   std::vector<Layer> middle;
@@ -108,7 +111,7 @@ Topology build_topology(const rs_engine& e) {
       chans.push_back(ch);
     }
     if (level != c.n_levels - 1) {
-      t.input_blocks.push_back({{3, ch, ch}});
+      t.input_blocks.push_back({{e.opt.resblock_updown ? L_RES_DOWN : L_DOWN, ch, ch}});
       chans.push_back(ch);
       ds /= 2;
     }
@@ -121,7 +124,7 @@ Topology build_topology(const rs_engine& e) {
       std::vector<Layer> layers{{1, ch + ich, mc * c.channel_mult[level]}};
       ch = mc * c.channel_mult[level];
       if (e.has_attn(ds) && i == 0) layers.push_back({2, ch, ds});
-      if (level && i == c.num_res_blocks[level]) { layers.push_back({4, ch, ch}); ds *= 2; }
+      if (level && i == c.num_res_blocks[level]) { layers.push_back({e.opt.resblock_updown ? L_RES_UP : L_UP, ch, ch}); ds *= 2; }
       t.output_blocks.push_back(layers);
     }
   }
@@ -151,22 +154,25 @@ void add_layers(rs_engine& e, const std::string& prefix, const std::vector<Layer
   for (size_t j = 0; j < layers.size(); ++j) {
     const Layer& L = layers[j];
     const std::string p = prefix + "." + std::to_string(j);
-    if (L.kind == 0) {
+    if (L.kind == L_CONV) {
       add_conv(e, p, L.a, L.b, 3);
-    } else if (L.kind == 1) {
+    } else if (L.kind == L_RES || L.kind == L_RES_DOWN || L.kind == L_RES_UP) {
+      const int cout = L.kind == L_RES ? L.b : L.a;
       add_gn(e, p + ".in_layers.0", L.a);
-      add_conv(e, p + ".in_layers.2", L.a, L.b, 3);
-      add_linear(e, p + ".emb_layers.1", e.time_dim(), 2 * L.b);
-      add_gn(e, p + ".out_layers.0", L.b);
-      add_conv(e, p + ".out_layers.3", L.b, L.b, 3);
-      if (L.a != L.b) add_conv(e, p + ".skip_connection", L.a, L.b, 1);
-    } else if (L.kind == 2) {
+      add_conv(e, p + ".in_layers.2", L.a, cout, 3);
+      add_linear(e, p + ".emb_layers.1", e.time_dim(), (e.opt.use_scale_shift_norm ? 2 : 1) * cout);
+      add_gn(e, p + ".out_layers.0", cout);
+      add_conv(e, p + ".out_layers.3", cout, cout, 3);
+      if (L.a != cout) add_conv(e, p + ".skip_connection", L.a, cout, 1);
+    } else if (L.kind == L_SWIN) {
       const int E = c.swin_embed_dim, res = L.b;
       const int win = res <= c.window_size ? res : c.window_size;
       const int shift = res <= c.window_size ? 0 : c.window_size / 2;
       const int hidden = (int)(E * c.mlp_ratio);
       add_conv(e, p + ".patch_embed.proj", L.a, E, 1);
+      if (e.opt.patch_norm) add_gn(e, p + ".patch_embed.norm", E);
       add_conv(e, p + ".patch_unembed.proj", E, L.a, 1);
+      if (e.opt.patch_norm) add_gn(e, p + ".patch_unembed.norm", L.a);
       for (int i = 0; i < c.swin_depth; ++i) {
         const std::string b = p + ".blocks." + std::to_string(i);
         if (i % 2 == 1 && shift > 0) {
@@ -182,10 +188,10 @@ void add_layers(rs_engine& e, const std::string& prefix, const std::vector<Layer
         add_conv(e, b + ".mlp.fc1", E, hidden, 1);
         add_conv(e, b + ".mlp.fc2", hidden, E, 1);
       }
-    } else if (L.kind == 3) {
-      add_conv(e, p + ".op", L.a, L.a, 3);
-    } else if (L.kind == 4) {
-      add_conv(e, p + ".conv", L.a, L.a, 3);
+    } else if (L.kind == L_DOWN) {
+      if (e.opt.conv_resample) add_conv(e, p + ".op", L.a, L.a, 3);
+    } else if (L.kind == L_UP) {
+      if (e.opt.conv_resample) add_conv(e, p + ".conv", L.a, L.a, 3);
     }
   }
 }
@@ -224,9 +230,13 @@ int build_inventory(rs_engine& e) {
   e.film_rows = rows;
   off = align_up(off, 256);
   e.film_b_off = off;
+  // Without scale-shift norm the FiLM row of a ResBlock is emb_out, added to in_layers.2's output by that conv's epilogue
+  // in place of its bias: the table's bias there is emb_layers.1.bias + in_layers.2.bias (rs_unet_load_param folds them),
+  // and both parameters keep slots of their own below.
   for (Param& p : e.params) {
     if (p.role == R_BIAS && p.name.find(".emb_layers.1.bias") != std::string::npos) {
-      p.off = off; p.bytes = (size_t)p.shape[0] * 4; off += p.bytes;
+      if (e.opt.use_scale_shift_norm) { p.off = off; p.bytes = (size_t)p.shape[0] * 4; }
+      off += (size_t)p.shape[0] * 4;
     }
   }
   off = align_up(off, 256);
@@ -273,8 +283,10 @@ struct Op {
   GnDesc gn;
   // attention
   View a_in, a_out; const float* a_bias = nullptr; int a_shift = 0;
-  // upsample
-  View u_in, u_out;
+  // 2x resampling: nearest upsample, or (u_pool) 2x2 average pool
+  View u_in, u_out; bool u_pool = false;
+  // conv whose bias is a FiLM-table row (ResBlock without scale-shift norm): its offset in a row, first image, or -1
+  int bias_film_off = -1, bias_film_n0 = 0;
   // row softmax (VQ-GAN attention): in place on s_view [rows = N*H*W][cols = C]
   View s_view; float s_scale = 1.f;
   // conv whose "weight" matrix is an activation tensor of the plan (per-image attention GEMMs), or whose INPUT is a
@@ -432,10 +444,11 @@ struct Builder {
   int opi() const { return (int)(P.fe_ops.size() + P.ops.size()); }
 
   void conv(const View& in, const std::string& name, int ksize, int stride, int cout, const View* out,
-            const View* res, int act, bool out_f32 = false, int pad_lo = 1) {
+            const View* res, int act, bool out_f32 = false, int pad_lo = 1, int bias_film_off = -1) {
     Op op; op.kind = OP_CONV;
     op.conv.in = in; op.conv.ksize = ksize; op.conv.stride = stride; op.conv.Cout = cout; op.conv.act = act;
     op.conv.pad_lo = pad_lo;
+    op.bias_film_off = bias_film_off; op.bias_film_n0 = cur_batch0; op.conv.bias_per_image = bias_film_off >= 0;
     if (out) { op.conv.out = *out; op.conv.has_out = true; } else op.conv.has_out = false;
     if (res) { op.conv.res = *res; op.conv.has_res = true; }
     op.w_name = name + ".weight"; op.b_name = name + ".bias";
@@ -539,23 +552,43 @@ struct Builder {
     if (x.tens >= 0) note_writer(x, x.C, /*win_slots=*/1);
     return true;
   }
-  void upsample(const View& in, const View& out) {
-    Op op; op.kind = OP_UPSAMPLE; op.u_in = in; op.u_out = out;
+  // a writer that delivers no GroupNorm statistics: a consumer of this range takes them from gn_stats_kernel
+  void forget_writers(const View& out, int C) {
+    auto it = writers.find(out.tens);
+    if (it == writers.end()) return;
+    auto& ws = it->second;
+    ws.erase(std::remove_if(ws.begin(), ws.end(), [&](const Writer& w) { return overlaps(w, out, C); }), ws.end());
+  }
+  void upsample(const View& in, const View& out, bool pool = false) {
+    Op op; op.kind = OP_UPSAMPLE; op.u_in = in; op.u_out = out; op.u_pool = pool;
     const int i = opi();
     P.touch(in, i); P.touch(out, i);
     op.stream = cur_stream;
     cur->push_back(op);
+    forget_writers(out, out.C);
   }
   void marker(OpKind k) { Op op; op.kind = k; cur->push_back(op); }
 
   // ResBlock (reference models/unet.py:186-206)
-  void res_block(const View& x, const std::string& p, int cout, const View& out) {
-    View t1 = P.make_view(x.N, x.H, x.W, x.C);
-    gn(x, p + ".in_layers.0", t1, 1, -1);
+  // updown: 0, or -1 / +1 for a ResBlock with down / up = True: h_upd and x_upd resample the GroupNorm + SiLU output and x
+  // (2x2 average pool / nearest 2x, :187-193).  Without scale-shift norm, h + emb_out is in_layers.2's epilogue bias.
+  void res_block(const View& x_in, const std::string& p, int cout, const View& out, int updown = 0) {
+    const bool ss = E.opt.use_scale_shift_norm != 0;
+    View t1 = P.make_view(x_in.N, x_in.H, x_in.W, x_in.C);
+    gn(x_in, p + ".in_layers.0", t1, 1, -1);
+    View x = x_in;
+    if (updown) {
+      const int Ho = updown > 0 ? 2 * x_in.H : x_in.H / 2, Wo = updown > 0 ? 2 * x_in.W : x_in.W / 2;
+      View t1r = P.make_view(x_in.N, Ho, Wo, x_in.C);
+      upsample(t1, t1r, updown < 0);
+      t1 = t1r;
+      x = P.make_view(x_in.N, Ho, Wo, x_in.C);
+      upsample(x_in, x, updown < 0);
+    }
     View h1 = P.make_view(x.N, x.H, x.W, cout);
-    conv(t1, p + ".in_layers.2", 3, 1, cout, &h1, nullptr, ACT_NONE);
+    conv(t1, p + ".in_layers.2", 3, 1, cout, &h1, nullptr, ACT_NONE, false, 1, ss ? -1 : E.film_row_of.at(p));
     View t2 = P.make_view(x.N, x.H, x.W, cout);
-    gn(h1, p + ".out_layers.0", t2, 1, E.film_row_of.at(p));
+    gn(h1, p + ".out_layers.0", t2, 1, ss ? E.film_row_of.at(p) : -1);
     if (x.C != cout) {
       conv(x, p + ".skip_connection", 1, 1, cout, &out, nullptr, ACT_NONE);
       conv(t2, p + ".out_layers.3", 3, 1, cout, &out, &out, ACT_NONE);     // in-place accumulate
@@ -571,7 +604,15 @@ struct Builder {
     RS_CHECK(win == 8 && x.H % 8 == 0 && x.W % 8 == 0, "the window-attention kernel covers 8x8 windows only");
     const int shift_odd = ctor_res <= c.window_size ? 0 : c.window_size / 2;
     View e = P.make_view(x.N, x.H, x.W, Ed);
-    conv(x, p + ".patch_embed.proj", 1, 1, Ed, &e, nullptr, ACT_NONE);
+    if (E.opt.patch_norm) {
+      // PatchEmbed.norm (reference models/swin_transformer.py:452-502).  Its output comes from no conv epilogue, so the
+      // first block's norm1 takes its statistics from gn_stats_kernel and that block runs the four-launch form
+      View e0 = P.make_view(x.N, x.H, x.W, Ed);
+      conv(x, p + ".patch_embed.proj", 1, 1, Ed, &e0, nullptr, ACT_NONE);
+      gn(e0, p + ".patch_embed.norm", e, 0, -1);
+    } else {
+      conv(x, p + ".patch_embed.proj", 1, 1, Ed, &e, nullptr, ACT_NONE);
+    }
     for (int i = 0; i < c.swin_depth; ++i) {
       const std::string b = p + ".blocks." + std::to_string(i);
       // x = x + proj(attn(qkv(norm1(x)))): one kernel (swin_attn_fused.cuh), or the four-launch sequence
@@ -601,7 +642,15 @@ struct Builder {
         conv(f, b + ".mlp.fc2", 1, 1, Ed, &e, &e, ACT_NONE);              // x = x + mlp
       }
     }
-    conv(e, p + ".patch_unembed.proj", 1, 1, x.C, &out, nullptr, ACT_NONE);
+    if (E.opt.patch_norm) {
+      // PatchUnEmbed.norm (:504-527), written into the block's destination (possibly a channel slice of a concat buffer)
+      View u = P.make_view(x.N, x.H, x.W, x.C);
+      conv(e, p + ".patch_unembed.proj", 1, 1, x.C, &u, nullptr, ACT_NONE);
+      gn(u, p + ".patch_unembed.norm", out, 0, -1);
+      forget_writers(out, x.C);
+    } else {
+      conv(e, p + ".patch_unembed.proj", 1, 1, x.C, &out, nullptr, ACT_NONE);
+    }
     return 0;
   }
 
@@ -611,18 +660,25 @@ struct Builder {
       const std::string p = prefix + "." + std::to_string(j);
       const bool last = (j + 1 == layers.size());
       View out;
-      if (L.kind == 0) {
+      if (L.kind == L_CONV) {
         out = last ? dest : P.make_view(h.N, h.H, h.W, L.b);
         conv(h, p, 3, 1, L.b, &out, nullptr, ACT_NONE);
-      } else if (L.kind == 1) {
+      } else if (L.kind == L_RES) {
         out = last ? dest : P.make_view(h.N, h.H, h.W, L.b);
         res_block(h, p, L.b, out);
-      } else if (L.kind == 2) {
+      } else if (L.kind == L_SWIN) {
         out = last ? dest : P.make_view(h.N, h.H, h.W, h.C);
         int rc = basic_layer(h, p, L.b, out); if (rc) return rc;
-      } else if (L.kind == 3) {
+      } else if (L.kind == L_RES_DOWN || L.kind == L_RES_UP) {     // always the last layer of its block
         out = dest;
-        conv(h, p + ".op", 3, 2, L.a, &out, nullptr, ACT_NONE);
+        res_block(h, p, L.a, out, L.kind == L_RES_DOWN ? -1 : 1);
+      } else if (L.kind == L_DOWN) {
+        out = dest;
+        if (E.opt.conv_resample) conv(h, p + ".op", 3, 2, L.a, &out, nullptr, ACT_NONE);
+        else upsample(h, out, /*pool=*/true);
+      } else if (!E.opt.conv_resample) {
+        out = dest;
+        upsample(h, out);
       } else {
         View u = P.make_view(h.N, 2 * h.H, 2 * h.W, h.C);
         upsample(h, u);
@@ -741,7 +797,7 @@ int build_plan(rs_plan& P) {
   {
     int hh = P.H, ww = P.W;
     for (int i = 0; i < n_in; ++i) {
-      for (const Layer& L : topo.input_blocks[i]) if (L.kind == 3) { hh /= 2; ww /= 2; }
+      for (const Layer& L : topo.input_blocks[i]) if (L.kind == L_DOWN || L.kind == L_RES_DOWN) { hh /= 2; ww /= 2; }
       in_h[i] = hh; in_w[i] = ww;
     }
   }
@@ -774,7 +830,8 @@ int build_plan(rs_plan& P) {
   // one block of the topology: as a whole, or as `branches` batch slices on their own streams
   auto run = [&](const View& hin, const std::string& prefix, const std::vector<Layer>& layers, const View& dest, View* hout) -> int {
     bool low = P.branches > 1 && is_low(hin.H, hin.W);
-    if (P.branches > 1 && !low && layers.size() == 1 && layers[0].kind == 3) low = is_low(hin.H / 2, hin.W / 2);   // the stride-2 conv entering the section
+    if (P.branches > 1 && !low && layers.size() == 1 && (layers[0].kind == L_DOWN || layers[0].kind == L_RES_DOWN))
+      low = is_low(hin.H / 2, hin.W / 2);   // the stride-2 conv entering the section
     if (!low) {
       leave();
       return b.run_block(hin, prefix, layers, dest, hout);
@@ -1040,7 +1097,15 @@ int run_op_range(rs_plan& P, const Op* first, const Op* last, const float* film_
     if (op_skipped(op)) { if (prof) { cudaEventRecord(prof->get(), st); prof->kind.push_back((int)op.kind); cudaEventRecord(prof->get(), st); } continue; }
     if (prof) { cudaEventRecord(prof->get(), st); prof->kind.push_back((int)op.kind); }
     switch (op.kind) {
-      case OP_CONV: rc = conv_launch(op.conv, st); break;
+      case OP_CONV: {
+        if (op.bias_film_off < 0) { rc = conv_launch(op.conv, st); break; }
+        ConvDesc d = op.conv;           // bias = this launch's FiLM row(s), resolved like a GroupNorm's film
+        const float* row = film_base + op.bias_film_off + (long long)op.bias_film_n0 * film_sN;
+        if (d.prm.bias) { d.prm.bias = row; d.prm.bias_sN = (int)film_sN; }
+        if (d.prm.splitk > 1 && !d.prm.splitk_cluster) { d.red.bias = row; d.red.bias_sN = (int)film_sN; }
+        rc = conv_launch(d, st);
+        break;
+      }
       case OP_GN: {
         GnDesc g = op.gn;
         if (g.film_off >= 0) { g.film = film_base + g.film_off + (long long)g.film_n0 * film_sN; g.film_sN = film_sN; }
@@ -1060,10 +1125,12 @@ int run_op_range(rs_plan& P, const Op* first, const Op* last, const float* film_
         break;
       }
       case OP_UPSAMPLE: {
-        UpsampleParams u{op.u_in.ptr, op.u_in.sN(), op.u_in.ld, op.u_out.ptr, op.u_in.N, op.u_in.H, op.u_in.W, op.u_in.C};
-        const long long total = (long long)u.N * 4 * u.H * u.W * (u.C / 8);
-        (void)launch_k(upsample2x_kernel, dim3((unsigned)std::min<long long>((total + 255) / 256, num_sms() * 16)), dim3(256), (size_t)(0), st, u);
-        if (cudaGetLastError() != cudaSuccess) rc = fail(-2, "upsample launch failed");
+        UpsampleParams u{op.u_in.ptr, op.u_in.sN(), op.u_in.ld, op.u_out.ptr, op.u_out.sN(), op.u_out.ld,
+                         op.u_in.N, op.u_in.H, op.u_in.W, op.u_in.C};
+        const long long total = (long long)u.N * (op.u_pool ? u.H * u.W / 4 : 4 * u.H * u.W) * (u.C / 8);
+        (void)launch_k(op.u_pool ? avgpool2x2_kernel : upsample2x_kernel,
+                       dim3((unsigned)std::min<long long>((total + 255) / 256, num_sms() * 16)), dim3(256), (size_t)(0), st, u);
+        if (cudaGetLastError() != cudaSuccess) rc = fail(-2, "resample launch failed");
         break;
       }
     }
@@ -1119,8 +1186,10 @@ int pack_lq_and_input(rs_plan& P, const float* x, const float* lq, const float* 
     int rc = run_ops(P, P.fe_ops, nullptr, 0, st); if (rc) return rc;
     pp.lq_nhwc = P.lq_feat.ptr; pp.lq_ld = P.lq_feat.ld; pp.Cl = P.lq_feat.C;
   } else {
-    RS_CHECK(!c.cond_mask, "cond_mask with lq_size == image_size is not covered");
+    // no feature extractor: cat([x, lq, mask]) straight into the packed input (reference models/unet.py:876-882)
+    RS_CHECK(!c.cond_mask || mask != nullptr, "this model is mask-conditioned: mask must be given");
     pp.lq_nchw = lq; pp.Cl = 3;
+    pp.mask_nchw = c.cond_mask ? mask : nullptr;
   }
   (void)launch_k(pack_input_kernel, dim3((unsigned)((npix + 255) / 256)), dim3(256), (size_t)(0), st, pp);
   RS_CUDA_OK(cudaGetLastError());
@@ -1148,17 +1217,25 @@ extern "C" {
 int rs_version(void) { return 100; }
 const char* rs_last_error(void) { return g_last_error.c_str(); }
 
-int rs_unet_create(const rs_unet_config* cfg, rs_engine** out) {
-  RS_CHECK(cfg && out, "null argument");
+int rs_unet_create_ex(const rs_unet_config* cfg, const rs_unet_options* opts, rs_engine** out) {
+  RS_CHECK(cfg && opts && out, "null argument");
   RS_CHECK(cfg->n_levels >= 1 && cfg->n_levels <= RS_MAX_LEVELS, "n_levels");
   RS_CHECK(cfg->swin_embed_dim == cfg->swin_heads * 32, "head_dim must be 32 (num_head_channels: 32 in every shipped yaml)");
+  RS_CHECK(cfg->window_size == 8, "window_size must be 8: the window-attention kernels are specialised for 8x8 windows");
   RS_CHECK(cfg->model_channels % 32 == 0 && cfg->swin_embed_dim % 32 == 0, "GroupNorm32 needs channels % 32 == 0");
   RS_CHECK(cfg->lq_size >= cfg->image_size, "lq_size < image_size is not covered");
+  for (int v : {opts->use_scale_shift_norm, opts->resblock_updown, opts->conv_resample, opts->patch_norm})
+    RS_CHECK(v == 0 || v == 1, "rs_unet_options fields are 0 or 1");
   auto e = std::make_unique<rs_engine>();
   e->cfg = *cfg;
+  e->opt = *opts;
   int rc = build_inventory(*e); if (rc) return rc;
   *out = e.release();
   return 0;
+}
+int rs_unet_create(const rs_unet_config* cfg, rs_engine** out) {
+  const rs_unet_options shipped{1, 0, 1, 0};
+  return rs_unet_create_ex(cfg, &shipped, out);
 }
 void rs_unet_destroy(rs_engine* e) { delete e; }
 int rs_unet_param_count(const rs_engine* e) { return e ? (int)e->params.size() : 0; }
@@ -1209,6 +1286,22 @@ int rs_unet_load_param(rs_engine* e, const char* name, const float* src, void* s
     long long n = 1;
     for (int v : p->shape) n *= v;
     (void)launch_k(copy_f32_kernel, dim3((unsigned)((n + 255) / 256)), dim3(256), (size_t)(0), st, src, reinterpret_cast<float*>(e->arena + p->off), n);
+  }
+  if (!e->opt.use_scale_shift_norm) {
+    // the FiLM table's bias of a ResBlock is emb_layers.1.bias + in_layers.2.bias (build_inventory); whichever of the two
+    // is loaded last leaves the sum right
+    const std::string nm(name);
+    for (const char* suffix : {".emb_layers.1.bias", ".in_layers.2.bias"}) {
+      const size_t ls = std::strlen(suffix);
+      if (nm.size() <= ls || nm.compare(nm.size() - ls, ls, suffix) != 0) continue;
+      const std::string blk = nm.substr(0, nm.size() - ls);
+      auto it = e->film_row_of.find(blk);
+      if (it == e->film_row_of.end()) continue;
+      const int n = p->shape[0];
+      (void)launch_k(add_f32_kernel, dim3((unsigned)((n + 255) / 256)), dim3(256), (size_t)(0), st,
+                     (const float*)e->at<float>(blk + ".emb_layers.1.bias"), (const float*)e->at<float>(blk + ".in_layers.2.bias"),
+                     reinterpret_cast<float*>(e->arena + e->film_b_off) + it->second, n);
+    }
   }
   RS_CUDA_OK(cudaGetLastError());
   return 0;
@@ -1368,7 +1461,7 @@ static void collect_profile(const rs_plan& P, const Prof& prof, double* ms, char
       else
         snprintf(d, desc_stride, "vq_attn T=%d C=%d N=%d rows=%d:%d", a.prm.T, a.q.C, a.q.N, a.row_begin, a.row_end);
     } else {
-      snprintf(d, desc_stride, "upsample %dx%d C=%d", op.u_in.H, op.u_in.W, op.u_in.C);
+      snprintf(d, desc_stride, "%s %dx%d C=%d", op.u_pool ? "avgpool" : "upsample", op.u_in.H, op.u_in.W, op.u_in.C);
     }
   }
 }

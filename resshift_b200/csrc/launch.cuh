@@ -168,8 +168,9 @@ struct ConvDesc {
   const __half* wt = nullptr;   // [Cout][taps][ipad]
   int ipad = 0;
   const float* bias = nullptr;
+  bool bias_per_image = false;    // the bias is a per-image row set per launch (prm.bias / prm.bias_sN): size its tile
   int Cout = 0;
-  View out;                // NHWC fp16 output view (ptr may be null when out_f32 is used)
+  View out;               // NHWC fp16 output view (ptr may be null when out_f32 is used)
   bool has_out = true;
   View res; bool has_res = false;
   float* out_f32 = nullptr;
@@ -198,7 +199,7 @@ struct TileConfig { int BN = 0, msub = 1, stages = 2, occ = 1, cg = 1, splitk = 
 // multicast).  Shallow rings are additionally latency-bound (~3000 cycles per load).  The epilogue (~18 cycles per
 // column + set-up) hides under a co-resident CTA; whole waves are counted.
 inline TileConfig pick_tile_config(int m_tiles, int cout16, int num_kb, int f_bn, bool allow_split = false, bool allow_persist = false,
-                                   bool allow_cluster_split = false) {
+                                   bool allow_cluster_split = false, bool allow_msub2 = true) {
   const int f_msub = env_int("RS_CONV_MSUB", 0), f_occ = env_int("RS_CONV_OCC", 0), f_stages = env_int("RS_CONV_STAGES", 0);
   const int f_cg = env_int("RS_CONV_CG", 0);
   TileConfig best, bestp;      // best one-tile-per-CTA configuration (ranking model below), best persistent one
@@ -233,7 +234,7 @@ inline TileConfig pick_tile_config(int m_tiles, int cout16, int num_kb, int f_bn
         }
       }
       for (int ms = 1; ms <= 2; ++ms) {
-        if (ms == 2 && (f_msub != 2 || cg == 2 || m_tiles % 2 || !conv_kernel_for(cand, 2))) continue;   // msub = 2 only on request
+        if (ms == 2 && (f_msub != 2 || !allow_msub2 || cg == 2 || m_tiles % 2 || !conv_kernel_for(cand, 2))) continue;   // msub = 2 only on request
         const int sbytes = ms * kConvBM * kConvBK * 2 + cand * kConvBK * 2;
         for (int occ = 1; occ <= 2; ++occ) {
           if (f_occ && occ != f_occ) continue;
@@ -342,14 +343,16 @@ inline int conv_finalize(ConvDesc& d) {
   const int cout16 = (d.Cout + 15) / 16 * 16;
   const int num_kb = p.num_taps * p.kchunks;
   const bool contiguous_tiles = (p.bw == Wout) || (p.bh == 1);
-  const bool can_split = d.allow_split && d.partial != nullptr && contiguous_tiles && p.bn <= 2 && d.has_out && !d.out_f32;
+  // (the SIMT cross-check kernel computes whole outputs, bias / residual / activation included: it never splits K)
+  const bool simt = env_is("RS_CONV_IMPL", "simt");
+  const bool can_split = d.allow_split && d.partial != nullptr && contiguous_tiles && p.bn <= 2 && d.has_out && !d.out_f32 && !simt;
   const int want_persist = env_int("RS_CONV_PERSIST", -1);           // 0 / 1 disables / forces the persistent kernel
   // (the persistent kernel batches its GroupNorm arrivals in a shared list of kGnListCap (sink, image) entries)
   const bool persist_ok = d.has_out && !d.out_f32 && want_persist != 0 && !env_is("RS_CONV_EPI", "direct") &&
                           !env_is("RS_CONV_IMPL", "simt") && env_int("RS_CONV_MSUB", 0) != 2;
-  const bool can_cluster_split = d.allow_split && contiguous_tiles && p.bn <= 2 && d.has_out && !d.out_f32 && d.Cout % 8 == 0;
+  const bool can_cluster_split = d.allow_split && contiguous_tiles && p.bn <= 2 && d.has_out && !d.out_f32 && d.Cout % 8 == 0 && !simt;
   const TileConfig tc = pick_tile_config(m_tiles, cout16, num_kb, d.bn_override ? d.bn_override : env_int("RS_CONV_BN", 0), can_split,
-                                         persist_ok && want_persist != 1, can_cluster_split);
+                                         persist_ok && want_persist != 1, can_cluster_split, !d.bias_per_image);
   const int BN = tc.BN, msub = tc.msub, stages = tc.stages, cg = tc.cg;
   p.cg = cg;
   p.splitk = tc.splitk; p.partial = d.partial; p.splitk_cluster = tc.cluster_split;
@@ -360,7 +363,10 @@ inline int conv_finalize(ConvDesc& d) {
   p.stages = stages;
   p.epi_off = 0;
   p.bar_off = stages * stage_bytes;
-  d.smem = (size_t)stages * stage_bytes + 1024 + 256 + 1024;   // ring + alignment slack + barriers + bias tile
+  // bias tile: [BN] floats, or [bn][BN] when every image has its own bias row
+  RS_CHECK(!d.bias_per_image || (p.bn <= 8 && msub == 1), "per-image bias needs one sub-tile of at most 8 images");
+  const size_t bias_tile = d.bias_per_image ? std::max<size_t>(1024, (size_t)p.bn * BN * sizeof(float)) : 1024;
+  d.smem = (size_t)stages * stage_bytes + 1024 + 256 + bias_tile;   // ring + alignment slack + barriers + bias tile
   RS_CHECK(d.smem <= 227 * 1024, "shared memory budget exceeded");
   d.grid = (cg == 2 ? ((m_tiles + 1) / 2) * p.n_tiles * 2 : (m_tiles / msub) * p.n_tiles) * p.splitk;
   // taps
@@ -384,7 +390,7 @@ inline int conv_finalize(ConvDesc& d) {
       }
   }
   // epilogue
-  p.bias = d.bias; p.act = d.act;
+  p.bias = d.bias; p.bias_sN = 0; p.act = d.act;
   if (d.has_res) {
     RS_CHECK(d.res.H == Hout && d.res.W == Wout && d.res.N == N && d.res.C >= d.Cout, "residual geometry");
     p.residual = d.res.ptr; p.res_sN = d.res.sN(); p.res_sH = d.res.sH(); p.res_sW = d.res.sW();
@@ -425,12 +431,12 @@ inline int conv_finalize(ConvDesc& d) {
       // the staging area (output tile + statistics scratch) follows the ring: the producer refills the ring while the
       // consumers drain the previous tile
       const size_t extra = conv_persist_extra_bytes(BN);
-      const int st = (int)std::min<size_t>(8, ((size_t)227 * 1024 - extra) / (size_t)stage_bytes);
+      const int st = (int)std::min<size_t>(8, ((size_t)227 * 1024 - extra - (bias_tile - 1024)) / (size_t)stage_bytes);
       RS_CHECK(st >= 2, "persistent conv: shared memory budget");
       p.stages = std::min(st, std::max(2, num_kb));
       p.epi_off = p.stages * stage_bytes;
       p.bar_off = p.epi_off + (int)conv_epi_bytes(BN, 1);
-      d.smem = (size_t)p.bar_off + 256 + 1024 + 1024;
+      d.smem = (size_t)p.bar_off + 256 + bias_tile + 1024;
       RS_CHECK(d.smem <= 227 * 1024, "persistent conv: shared memory budget");
       d.grid = cg * std::min(units, workers);
     }

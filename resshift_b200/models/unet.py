@@ -74,8 +74,8 @@ class UNetModelSwin(nn.Module):
             raise RuntimeError("resshift_b200.UNetModelSwin runs on CUDA only (no CPU fallback); call .cuda() first")
         if self._engine is None:
             h = C.c_void_p()
-            cfgc = _lib.make_config(self.cfg)
-            _lib.check(_lib.lib.rs_unet_create(C.byref(cfgc), C.byref(h)))
+            cfgc, optc = _lib.make_config(self.cfg), _lib.make_options(self.cfg)
+            _lib.check(_lib.lib.rs_unet_create_ex(C.byref(cfgc), C.byref(optc), C.byref(h)))
             self._engine = h
             n = _lib.lib.rs_unet_param_count(h)
             mine = sorted(name for name, _, _ in self._spec)
