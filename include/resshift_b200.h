@@ -238,19 +238,22 @@ int rs_op_conv2d(const void* x, int N, int H, int W, int C, int ld, const void* 
                  int Cout, int ksize, int stride, const void* residual, int res_ld, void* out, int out_ld,
                  float* out_f32_nchw, int act, int bn, void* stream);
 /* conv2d + GroupNorm statistics of its output: part[N][slots][cstride][2] = (mean, M2) of the stored values per image /
- * 128-pixel tile slot / channel at channel offset coff; with gstat + counter (uint32[N], zeroed by the caller) the last
- * CTA of each image also writes gstat[N][32][2] = (group mean, group rstd) once slots * expected_channels channel-slots
- * arrived (expected_channels = 0: cstride).  reference: the GroupNorm32 that follows every conv (models/basic_ops.py:15-17) */
+ * 128-pixel tile slot / channel at channel offset coff; with gstat, a finalisation kernel after the conv also writes
+ * gstat[N][32][2] = (group mean, group rstd) of all cstride channels of part (cstride % 32 == 0).  counter is accepted
+ * for compatibility and not read; expected_channels must be 0 or cstride, anything else returns an error.
+ * reference: the GroupNorm32 that follows every conv (models/basic_ops.py:15-17) */
 int rs_op_conv2d_stats(const void* x, int N, int H, int W, int C, int ld, const void* w_packed, int Ipad, const float* bias,
                        int Cout, int ksize, int stride, const void* residual, int res_ld, void* out, int out_ld, int act,
                        int bn, float* part, int cstride, int coff, int32_t* slots_out, float* gstat, void* counter,
                        int expected_channels, void* stream);
-/* conv2d that may split its K loop over several CTAs (layers with few output tiles); scratch: 8*N*Ho*Wo*Cout floats */
+/* conv2d that may split its K loop over several CTAs (layers with few output tiles); scratch: 8*N*Ho*Wo*Cout floats;
+ * part / gstat as rs_op_conv2d_stats, counter not read */
 int rs_op_conv2d_splitk(const void* x, int N, int H, int W, int C, int ld, const void* w_packed, int Ipad, const float* bias,
                         int Cout, int ksize, int stride, const void* residual, int res_ld, void* out, int out_ld, int act,
                         float* part, int cstride, int coff, float* scratch, int32_t* splits_out, float* gstat, void* counter,
                         void* stream);
-/* profiling aid: `iters` launches of the same conv; per-CTA timeline of the last one in dbg (8 x u64 per CTA) */
+/* profiling aid: `iters` launches of the same conv; per-CTA timeline of the last one in dbg (8 x u64 per CTA);
+ * info[7] = grid, BN, stages, shared memory bytes, CTAs per tile group, split-K factor, persistent kernel (0 / 1) */
 int rs_op_conv2d_timeline(const void* x, int N, int H, int W, int C, int ld, const void* w_packed, int Ipad, const float* bias,
                           int Cout, int ksize, int stride, void* out, int out_ld, int bn, int iters, void* dbg,
                           int32_t* info, float* splitk_scratch_or_null, void* stream);
@@ -305,8 +308,8 @@ int rs_op_swin_attn(const void* x, int N, int H, int W, int E, int heads, int sh
 int rs_op_mlp(const void* x, int N, int H, int W, int E, int Hd, const void* w1_packed, const float* b1,
               const void* w2_packed, const float* b2, const void* residual, void* out, void* dbg_timeline_or_null,
               void* stream);
-/* host-only: tile configuration the conv launcher picks: out[9] = BN, msub, stages, CTAs/SM, estimated cycles,
-   CTAs per tile group (1 or 2), split-K factor, persistent kernel (0 / 1), cluster split-K (0 / 1) */
+/* host-only: tile configuration the conv launcher picks: out[8] = BN, msub, stages, CTAs/SM, estimated cycles,
+   CTAs per tile group (1 or 2), split-K factor, persistent kernel (0 / 1) */
 int rs_debug_tile_config(int m_tiles, int cout, int num_kblocks, int32_t* out);
 /* nearest x2 (reference models/unet.py:71-81) */
 int rs_op_upsample2x(const void* x, int N, int H, int W, int C, void* y, void* stream);

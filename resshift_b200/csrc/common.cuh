@@ -160,7 +160,7 @@ __device__ __forceinline__ void tma_load_4d(void* dst, const CUtensorMap* m, uin
       : "memory");
 }
 
-// ---- clusters: rank, cluster-wide barrier, distributed shared memory, TMA multicast ----
+// ---- clusters: rank, cluster-wide barrier, remote shared-memory addresses, TMA multicast ----
 __device__ __forceinline__ uint32_t cluster_ctarank() {
   uint32_t r;
   asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
@@ -175,13 +175,6 @@ __device__ __forceinline__ uint32_t mapa_u32(uint32_t addr, uint32_t rank) {
   uint32_t r;
   asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(addr), "r"(rank));
   return r;
-}
-// 16-byte load from the shared memory of another CTA of the cluster (address from mapa_u32)
-__device__ __forceinline__ float4 ld_shared_cluster_f4(uint32_t cluster_addr) {
-  float4 v;
-  asm volatile("ld.shared::cluster.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(cluster_addr)
-               : "memory");
-  return v;
 }
 // 2-D tile load written to the same shared-memory offset of every CTA in `cta_mask`; each destination CTA's barrier at
 // the offset of `bar` receives the bytes that landed there

@@ -59,8 +59,6 @@ struct ConvParams {
   int splitk;            // > 1: the K loop is cut into `splitk` ranges, one CTA (or pair) each; the epilogue then only
                          //      stores fp32 partial accumulators to `partial` and splitk_reduce_kernel finishes the layer
   float* partial;        // [splitk][Nimg*Hout*Wout pixels][Cout] fp32
-  int splitk_cluster;    // 1 (pair mode only): the S K-ranges of a tile are ONE cluster of 2*S CTAs; partial tiles stay in
-                         //    shared memory and are summed through distributed shared memory (no scratch, no second kernel)
   int msub;              // 128-pixel sub-tiles per CTA (1 or 2): two sub-tiles share every weight tile (fewer operand bytes per MMA)
   // epilogue
   const float* bias;                 // [Cout] fp32 or nullptr; with bias_sN > 0 one row per image
@@ -80,7 +78,7 @@ struct ConvParams {
   int epi_bc;                        // staging block width in columns: 64 / 32 / 16 (swizzle 128B / 64B / 32B),
                                      // the largest that divides BN so a block never spills into the next channel tile
   // fused GroupNorm statistics of the OUTPUT for up to two consumers (gn_stats.cuh): per image / 128-pixel tile slot /
-  // channel the pair (mean, M2) of the stored fp16 values; the last CTA to finish an image reduces its 32 groups
+  // channel the pair (mean, M2) of the stored fp16 values
   GnSink sink[2];
   int gn_slots;
   // persistent mode: CTAs (pairs) walk work units u = worker, worker + #workers, ...; the producer loads the next
@@ -117,8 +115,7 @@ __global__ void __launch_bounds__(kConvThreads, (BN * MS <= 128) ? 2 : 1) conv_g
     dbg[0] = global_timer_ns(); dbg[7] = smid;
   }
 
-  // pair mode: the cluster is one CTA pair — or, with splitk_cluster, the S pairs (K ranges) of one tile: cluster rank =
-  // 2 * split + (rank inside the pair)
+  // pair mode: the cluster is one CTA pair, cluster rank = rank inside the pair
   const int cg = p.cg;
   const uint32_t crank = cg == 2 ? cluster_ctarank() : 0;
   const uint32_t rank = crank & 1;
@@ -252,17 +249,7 @@ __global__ void __launch_bounds__(kConvThreads, (BN * MS <= 128) ? 2 : 1) conv_g
       // complete (its staged tile has been read by the TMA store)
       named_bar_sync(1, 32 * kConvEpiWarps);
 
-      if (p.splitk > 1 && p.splitk_cluster) {
-        // ---------- cluster split-K, step 1: this K range's fp32 partial tile -> own shared memory ----------
-        // (row pitch BN*4 + 16 B spreads the rows over the banks)
-        const int pitch = BN * 4 + 16;
-#pragma unroll
-        for (int j = 0; j < BN / 8; ++j) {
-          const int c = 8 * j + 2 * (lane & 3);
-          *reinterpret_cast<float2*>(smem + (size_t)rA * pitch + c * 4) = make_float2(acc[0][4 * j], acc[0][4 * j + 1]);
-          *reinterpret_cast<float2*>(smem + (size_t)rB * pitch + c * 4) = make_float2(acc[0][4 * j + 2], acc[0][4 * j + 3]);
-        }
-      } else if (p.splitk > 1) {
+      if (p.splitk > 1) {
         // ---------- split-K: raw fp32 partial sums, finished by splitk_reduce_kernel ----------
         int tw, th, w0, h0, n0;
         tile_origin(mt0, tw, th, w0, h0, n0);
@@ -372,7 +359,6 @@ __global__ void __launch_bounds__(kConvThreads, (BN * MS <= 128) ? 2 : 1) conv_g
           tma_store_commit();
         }
         if (want_stats) {
-          int* s_flag = reinterpret_cast<int*>(wsum_all + (size_t)MS * 8 * BN);
           for (int sub = 0; sub < MS; ++sub) {
             int tw, th, w0, h0, n0;
             tile_origin(mt0 + sub, tw, th, w0, h0, n0);
@@ -381,13 +367,6 @@ __global__ void __launch_bounds__(kConvThreads, (BN * MS <= 128) ? 2 : 1) conv_g
             if (n0 < p.Nimg)                                           // (else: padding tile of an odd pair)
               write_quad_pairs(wsum_all + (size_t)sub * 8 * BN, BN, ncols, col0, p.bn, n0, p.Nimg, slot, p.gn_slots, p.sink[0], p.sink[1],
                                etid, 32 * kConvEpiWarps);
-            if (p.sink[0].gstat || p.sink[1].gstat) {                  // producer-side finalisation (large tensors only)
-              const GnSink* const sk[4] = {&p.sink[0], &p.sink[0], p.sink[1].part ? &p.sink[1] : nullptr, p.sink[1].part ? &p.sink[1] : nullptr};
-              const int n1 = (p.bn == 2 && n0 + 1 < p.Nimg) ? n0 + 1 : -1;
-              const int im[4] = {n0 < p.Nimg ? n0 : -1, n0 < p.Nimg ? n1 : -1, n0 < p.Nimg ? n0 : -1, n0 < p.Nimg ? n1 : -1};
-              const unsigned int ad[4] = {(unsigned)ncols, (unsigned)ncols, (unsigned)ncols, (unsigned)ncols};
-              gn_arrive<4>(sk, im, ad, p.gn_slots, 128.0f / (float)p.bn, etid, 32 * kConvEpiWarps, 1, s_flag);
-            }
           }
         }
         if (etid == 0) tma_store_wait_read();
@@ -420,99 +399,6 @@ __global__ void __launch_bounds__(kConvThreads, (BN * MS <= 128) ? 2 : 1) conv_g
               }
             }
           }
-        }
-      }
-    }
-  }
-
-  if (p.splitk > 1 && p.splitk_cluster) {
-    // ---------- cluster split-K, step 2: sum the S partial tiles through distributed shared memory ----------
-    // K range `split` finishes columns [split * BN/S, (split + 1) * BN/S) of the tile for its CTA's 128 pixels:
-    // fixed summation order (range 0, 1, ...), then the usual epilogue work (bias / activation / residual / fp16
-    // store / GroupNorm partials of the stored values).  Deterministic, no global scratch, no second kernel.
-    cluster_sync_all();                                   // every K range's partial tile is in its CTA's shared memory
-    if (warp < kConvEpiWarps) {
-      const int etid = threadIdx.x;
-      const int S = p.splitk, cw = BN / S, upr = cw >> 3;
-      const int pitch = BN * 4 + 16;
-      const int cbase = split * cw;
-      int n_tile, mt0;
-      unit_tiles(unit0, n_tile, mt0);
-      const int col0 = n_tile * BN;
-      __half* s_out = reinterpret_cast<__half*>(smem + (size_t)kConvBM * pitch);        // [128][cw] stored values
-      float* s_col = reinterpret_cast<float*>(s_out + (size_t)kConvBM * cw);            // [2 halves][cw][2]
-      int tw, th, w0, h0, n0;
-      tile_origin(mt0, tw, th, w0, h0, n0);
-      const uint32_t dump0 = smem_u32(smem);
-      for (int u = etid; u < kConvBM * upr; u += 32 * kConvEpiWarps) {
-        const int rr = u / upr, cu = u - rr * upr;
-        const int ct = cbase + cu * 8;                    // column inside the BN tile
-        float acc[8];
-#pragma unroll
-        for (int j = 0; j < 8; ++j) acc[j] = 0.f;
-        for (int sp = 0; sp < S; ++sp) {
-          const uint32_t a = mapa_u32(dump0 + (uint32_t)(rr * pitch + ct * 4), (uint32_t)(sp * 2) + rank);
-          const float4 x0 = ld_shared_cluster_f4(a), x1 = ld_shared_cluster_f4(a + 16);
-          acc[0] += x0.x; acc[1] += x0.y; acc[2] += x0.z; acc[3] += x0.w;
-          acc[4] += x1.x; acc[5] += x1.y; acc[6] += x1.z; acc[7] += x1.w;
-        }
-        const int lw = rr % p.bw, lh = (rr / p.bw) % p.bh, ln = rr / (p.bw * p.bh);
-        const int w = w0 + lw, h = h0 + lh, n = n0 + ln;
-        const int col = col0 + ct;
-        const bool ok = (w < p.Wout) && (h < p.Hout) && (n < p.Nimg) && (col < p.Cout);   // Cout % 8 == 0
-        uint4 o = make_uint4(0, 0, 0, 0);
-        if (ok) {
-          if (p.bias) {
-#pragma unroll
-            for (int j = 0; j < 8; ++j) acc[j] += __ldg(p.bias + n * p.bias_sN + col + j);
-          }
-          if (p.act == ACT_GELU) {
-#pragma unroll
-            for (int j = 0; j < 8; ++j) acc[j] = gelu_erf_f(acc[j]);
-          } else if (p.act == ACT_SILU) {
-#pragma unroll
-            for (int j = 0; j < 8; ++j) acc[j] = silu_f(acc[j]);
-          }
-          if (p.residual) {
-            const uint4 rv = *reinterpret_cast<const uint4*>(p.residual + n * p.res_sN + h * p.res_sH + w * p.res_sW + col);
-            const __half2* rh = reinterpret_cast<const __half2*>(&rv);
-#pragma unroll
-            for (int j = 0; j < 4; ++j) { const float2 f = __half22float2(rh[j]); acc[2 * j] += f.x; acc[2 * j + 1] += f.y; }
-          }
-          __half2* oh = reinterpret_cast<__half2*>(&o);
-#pragma unroll
-          for (int j = 0; j < 4; ++j) oh[j] = __floats2half2_rn(acc[2 * j], acc[2 * j + 1]);
-          *reinterpret_cast<uint4*>(p.out + n * p.out_sN + h * p.out_sH + w * p.out_sW + col) = o;
-        }
-        *reinterpret_cast<uint4*>(s_out + (size_t)rr * cw + cu * 8) = o;                  // zeros outside the tensor
-      }
-      if (p.sink[0].part != nullptr) {
-        named_bar_sync(1, 32 * kConvEpiWarps);
-        // (mean, M2) of the stored values per column over the two 64-row halves (pivot = first row, rows in order)
-        for (int t = etid; t < 2 * cw; t += 32 * kConvEpiWarps) {
-          const int half = t / cw, c = t - half * cw;
-          const __half* col = s_out + (size_t)(half * 64) * cw + c;
-          const float pv = __half2float(col[0]);
-          float s1 = 0.f, s2 = 0.f;
-          for (int rr = 1; rr < 64; ++rr) {
-            const float d = __half2float(col[(size_t)rr * cw]) - pv;
-            s1 += d; s2 = fmaf(d, d, s2);
-          }
-          s_col[(half * cw + c) * 2] = pv + s1 * (1.0f / 64.0f);
-          s_col[(half * cw + c) * 2 + 1] = fmaxf(s2 - s1 * s1 * (1.0f / 64.0f), 0.f);
-        }
-        named_bar_sync(1, 32 * kConvEpiWarps);
-        const int slot = th * p.tiles_w + tw;
-        const int ncols = max(0, min(cw, p.Cout - (col0 + cbase)));
-        if (n0 < p.Nimg)
-          write_tile_pairs(s_col, cw, ncols, col0 + cbase, p.bn, n0, p.Nimg, slot, p.gn_slots, p.sink[0], p.sink[1], etid, 32 * kConvEpiWarps);
-        if (p.sink[0].gstat || p.sink[1].gstat) {
-          int* s_flag = reinterpret_cast<int*>(s_col + 4 * cw);
-          const GnSink* const sk[4] = {&p.sink[0], &p.sink[0], p.sink[1].part ? &p.sink[1] : nullptr, p.sink[1].part ? &p.sink[1] : nullptr};
-          const int n1 = (p.bn == 2 && n0 + 1 < p.Nimg) ? n0 + 1 : -1;
-          const int im[4] = {n0 < p.Nimg ? n0 : -1, n0 < p.Nimg ? n1 : -1, n0 < p.Nimg ? n0 : -1, n0 < p.Nimg ? n1 : -1};
-          const unsigned int ad[4] = {(unsigned)ncols, (unsigned)ncols, (unsigned)ncols, (unsigned)ncols};
-          gn_arrive<4>(sk, im, ad, p.gn_slots, 128.0f / (float)p.bn, etid, 32 * kConvEpiWarps, 1, s_flag);
         }
       }
     }

@@ -244,7 +244,7 @@ struct SplitKReduceParams {
 __global__ void __launch_bounds__(256) splitk_reduce_kernel(const __grid_constant__ SplitKReduceParams p) {
   pdl_trigger();
   pdl_wait();
-  extern __shared__ float s_red[];       // [lanes][cols_per_cta][3] = (rows, mean, M2) per row-lane and column; + 4 flags
+  extern __shared__ float s_red[];       // [lanes][cols_per_cta][3] = (rows, mean, M2) per row-lane and column
   const int c_begin = blockIdx.z * p.cols_per_cta;
   const int ccols = min(p.cols_per_cta, p.C - c_begin);
   const int vecs = ccols >> 3;
@@ -339,12 +339,6 @@ __global__ void __launch_bounds__(256) splitk_reduce_kernel(const __grid_constan
         dst[0] = mean; dst[1] = m2;
       }
   }
-  if (!(p.sink[0].gstat || p.sink[1].gstat)) return;
-  int* s_flag = reinterpret_cast<int*>(s_red + (size_t)lanes * ccols * 3);
-  const GnSink* const sk[2] = {&p.sink[0], p.sink[1].part ? &p.sink[1] : nullptr};
-  const int im[2] = {n, n};
-  const unsigned int ad[2] = {(unsigned)ccols, (unsigned)ccols};
-  gn_arrive<2>(sk, im, ad, p.slots, (float)p.rows_per_slot, threadIdx.x, blockDim.x, 1, s_flag);
 }
 
 // ------------------------------------------------------------------------------------------------

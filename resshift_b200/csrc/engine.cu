@@ -268,7 +268,7 @@ int build_inventory(rs_engine& e) {
 // ------------------------------------------------------------------------------------------------
 namespace {
 
-enum OpKind { OP_CONV, OP_GN, OP_ATTN, OP_UPSAMPLE, OP_MLP, OP_SOFTMAX, OP_FORK, OP_JOIN, OP_SWIN_ATTN, OP_VQ_ATTN };
+enum OpKind { OP_CONV, OP_GN, OP_ATTN, OP_UPSAMPLE, OP_MLP, OP_SOFTMAX, OP_SWIN_ATTN, OP_VQ_ATTN };
 
 struct Tensor {
   size_t bytes = 0;
@@ -285,8 +285,8 @@ struct Op {
   View a_in, a_out; const float* a_bias = nullptr; int a_shift = 0;
   // 2x resampling: nearest upsample, or (u_pool) 2x2 average pool
   View u_in, u_out; bool u_pool = false;
-  // conv whose bias is a FiLM-table row (ResBlock without scale-shift norm): its offset in a row, first image, or -1
-  int bias_film_off = -1, bias_film_n0 = 0;
+  // conv whose bias is a FiLM-table row (ResBlock without scale-shift norm): its offset in a row, or -1
+  int bias_film_off = -1;
   // row softmax (VQ-GAN attention): in place on s_view [rows = N*H*W][cols = C]
   View s_view; float s_scale = 1.f;
   // conv whose "weight" matrix is an activation tensor of the plan (per-image attention GEMMs), or whose INPUT is a
@@ -306,8 +306,7 @@ struct Op {
   int gn_index = -1;                    // GroupNorm: index of its [N][32][2] group statistics / [N] arrival counters
   bool to_f32 = false;                  // conv: writes the fp32 NCHW model output
   int split_tens = -1;                  // conv: workspace tensor holding split-K partial sums (or -1)
-  int stream = 0;                       // 0: the caller's stream; k > 0: side stream k of the plan (concurrent batch slices)
-  struct StatDst { int list; int op; int coff; int img_off; };
+  struct StatDst { int list; int op; int coff; };
   std::vector<StatDst> stat_dst;        // conv: GroupNorm ops whose statistics this conv's epilogue produces
 };
 
@@ -338,18 +337,6 @@ struct rs_plan {
   bool bound = false;
   int device = -1;           // CUDA device that was current at rs_plan_bind: the only one the plan runs on
   int launches = 0;
-  // Low-resolution levels (a handful of output tiles per layer at batch 16: every kernel is latency-bound and leaves most
-  // SMs idle) run as `branches` independent batch slices on concurrent streams; each slice's kernels depend only on its
-  // own predecessors, so two (or four) of these small kernels share the machine.  Streams / events belong to the plan;
-  // fork / join are event edges, so the structure is captured into the sampler's CUDA graph as parallel branches.
-  int branches = 1;
-  std::vector<cudaStream_t> side;          // branches - 1 side streams
-  std::vector<cudaEvent_t> ev;             // [0] fork, [k] join of side stream k
-  std::vector<std::pair<int, int>> sections;   // [first, last] global op index of every concurrent section
-  ~rs_plan() {
-    for (cudaStream_t s : side) cudaStreamDestroy(s);
-    for (cudaEvent_t e : ev) cudaEventDestroy(e);
-  }
   int vq_which = -1;         // -1: denoiser plan; 0 / 1: VQ-GAN encode / decode plan (vq.inc)
   int imgH = 0, imgW = 0;    // VQ plans: image size (H, W above are the latent size)
   int vq_attn_op = -1;       // VQ plans: index in ops of the fused bottleneck attention (-1: none, T <= 8192)
@@ -372,9 +359,6 @@ struct rs_plan {
   static View slice(const View& base, int c0, int C) {
     View v = base; v.off = base.off + c0; v.c0 = base.c0 + c0; v.C = C; return v;
   }
-  static View batch(const View& base, int n0, int n) {       // images [n0, n0 + n) of the view
-    View v = base; v.off = base.off + (long long)n0 * base.sN(); v.n0 = base.n0 + n0; v.N = n; return v;
-  }
   void touch(const View& v, int opi) {
     if (v.tens < 0) return;
     Tensor& t = tensors[v.tens];
@@ -392,8 +376,6 @@ struct Builder {
   int n_gn = 0;
   struct Writer { int c0; int C; int n0; int N; int list; int op; int win_slots; };
   std::map<int, std::vector<Writer>> writers;      // tensor id -> latest writers by (channel range, image range)
-  int cur_stream = 0;                              // ops are tagged with the stream of the batch slice being built
-  int cur_batch0 = 0;                              // ... and with its first image inside the plan's batch (per-image FiLM rows)
   static bool overlaps(const Writer& w, const View& v, int C) {
     return w.c0 < v.c0 + C && v.c0 < w.c0 + w.C && w.n0 < v.n0 + v.N && v.n0 < w.n0 + w.N;
   }
@@ -448,15 +430,15 @@ struct Builder {
     Op op; op.kind = OP_CONV;
     op.conv.in = in; op.conv.ksize = ksize; op.conv.stride = stride; op.conv.Cout = cout; op.conv.act = act;
     op.conv.pad_lo = pad_lo;
-    op.bias_film_off = bias_film_off; op.bias_film_n0 = cur_batch0; op.conv.bias_per_image = bias_film_off >= 0;
+    op.bias_film_off = bias_film_off; op.conv.bias_per_image = bias_film_off >= 0;
     if (out) { op.conv.out = *out; op.conv.has_out = true; } else op.conv.has_out = false;
     if (res) { op.conv.res = *res; op.conv.has_res = true; }
     op.w_name = name + ".weight"; op.b_name = name + ".bias";
     op.to_f32 = out_f32;
     if (out && !out_f32 && env_int("RS_CONV_SPLITK", 0) != 1) {       // split-K for layers with too few tiles
       const TileConfig tc = conv_preview_config(in.N, in.H, in.W, in.C, cout, ksize, stride, true);
-      if (tc.splitk > 1) op.conv.allow_split = true;
-      if (tc.splitk > 1 && !tc.cluster_split) {       // (cluster split-K reduces through shared memory: no scratch)
+      if (tc.splitk > 1) {
+        op.conv.allow_split = true;
         const size_t bytes = (size_t)tc.splitk * in.N * (in.H / stride) * (in.W / stride) * cout * sizeof(float);
         op.split_tens = P.new_tensor(bytes);
         Tensor& tz = P.tensors[op.split_tens];
@@ -465,14 +447,12 @@ struct Builder {
     }
     const int i = opi();
     P.touch(in, i); if (out) P.touch(*out, i); if (res) P.touch(*res, i);
-    op.stream = cur_stream;
     cur->push_back(op);
     if (out && !out_f32 && out->tens >= 0) note_writer(*out, cout);   // the latest writer of this (channel, image) range
   }
   void gn(const View& in, const std::string& name, const View& out, int silu, int film_off, float eps = 1e-5f) {
     Op op; op.kind = OP_GN;
     op.gn.in = in; op.gn.out = out; op.gn.silu = silu; op.gn.film_off = film_off; op.gn.eps = eps;
-    op.gn.film_n0 = cur_batch0;
     op.g_name = name;
     // can the producers' epilogues deliver the statistics?  (every channel of every image of the view written by a
     // conv / MLP of this plan)
@@ -488,17 +468,15 @@ struct Builder {
     stats_off += align_up((size_t)in.N * op.gn.slots * in.C * 2 * sizeof(float), 256);
     const int i = opi();
     P.touch(in, i); P.touch(out, i);
-    op.stream = cur_stream;
     cur->push_back(op);
     for (const Writer& w : prod)
-      list(w.list)[w.op].stat_dst.push_back({list_id(), (int)cur->size() - 1, w.c0 - in.c0, w.n0 - in.n0});
+      list(w.list)[w.op].stat_dst.push_back({list_id(), (int)cur->size() - 1, w.c0 - in.c0});
   }
   void attn(const View& qkv, const View& out, const std::string& blk, int shift) {
     Op op; op.kind = OP_ATTN; op.a_in = qkv; op.a_out = out; op.a_shift = shift;
     op.w_name = blk + ".attn.relative_position_bias_table";
     const int i = opi();
     P.touch(qkv, i); P.touch(out, i);
-    op.stream = cur_stream;
     cur->push_back(op);
   }
   // norm_name non-empty: `in` is the un-normalised tensor and the kernel applies that GroupNorm to its X tile itself
@@ -522,10 +500,9 @@ struct Builder {
     }
     const int i = opi();
     P.touch(in, i); P.touch(out, i); P.touch(res, i);
-    op.stream = cur_stream;
     cur->push_back(op);
     for (const Writer& w : prod)
-      list(w.list)[w.op].stat_dst.push_back({list_id(), (int)cur->size() - 1, w.c0 - in.c0, w.n0 - in.n0});
+      list(w.list)[w.op].stat_dst.push_back({list_id(), (int)cur->size() - 1, w.c0 - in.c0});
     if (out.tens >= 0) note_writer(out, E);
     return true;
   }
@@ -545,10 +522,9 @@ struct Builder {
     stats_off += align_up((size_t)x.N * op.gn.slots * x.C * 2 * sizeof(float), 256);
     const int i = opi();
     P.touch(x, i);
-    op.stream = cur_stream;
     cur->push_back(op);
     for (const Writer& w : prod)
-      list(w.list)[w.op].stat_dst.push_back({list_id(), (int)cur->size() - 1, w.c0 - x.c0, w.n0 - x.n0});
+      list(w.list)[w.op].stat_dst.push_back({list_id(), (int)cur->size() - 1, w.c0 - x.c0});
     if (x.tens >= 0) note_writer(x, x.C, /*win_slots=*/1);
     return true;
   }
@@ -563,11 +539,9 @@ struct Builder {
     Op op; op.kind = OP_UPSAMPLE; op.u_in = in; op.u_out = out; op.u_pool = pool;
     const int i = opi();
     P.touch(in, i); P.touch(out, i);
-    op.stream = cur_stream;
     cur->push_back(op);
     forget_writers(out, out.C);
   }
-  void marker(OpKind k) { Op op; op.kind = k; cur->push_back(op); }
 
   // ResBlock (reference models/unet.py:186-206)
   // updown: 0, or -1 / +1 for a ResBlock with down / up = True: h_upd and x_upd resample the GroupNorm + SiLU output and x
@@ -719,14 +693,6 @@ int finish_layout(rs_plan& P, Builder& b, size_t state_bytes, bool unet) {
   P.off_state = region(2 * align_up(lat, 256));
   // persistent tensors first, then liveness-packed temporaries (RS_NO_REUSE=1 keeps every tensor
   // alive for the whole forward so that rs_plan_probe can read any block output afterwards)
-  // tensors born or last used inside a concurrent section stay allocated for the whole section: its batch slices run
-  // on different streams, so "op index order" no longer implies "executed before"
-  for (const auto& sec : P.sections)
-    for (Tensor& tz : P.tensors) {
-      if (tz.last < 0) continue;
-      if (tz.first >= sec.first && tz.first <= sec.second) tz.first = sec.first;
-      if (tz.last >= sec.first && tz.last <= sec.second) tz.last = sec.second;
-    }
   if (env_int("RS_NO_REUSE", 0)) for (Tensor& tz : P.tensors) tz.persistent = true;
   for (Tensor& tz : P.tensors) if (tz.persistent) tz.off = region(tz.bytes);
   P.off_temps = off;
@@ -807,47 +773,6 @@ int build_plan(rs_plan& P) {
     const int ctot = topo.output_blocks[j][0].a;       // ch + ich
     cat[j] = P.make_view(B, in_h[k], in_w[k], ctot);
   }
-  // ---- concurrent batch slices for the few-tile levels (see rs_plan::branches) --------------------------------
-  // (the tile planner re-splits every half-batch layer until it fills the machine again, so the slices do not actually
-  // share it and only the launch count doubles; selectable, OFF by default)
-  {
-    int nb = env_int("RS_LOWRES_STREAMS", 1);
-    if (nb < 1) nb = 1;
-    while (nb > 1 && (B % nb != 0 || B / nb < 1)) --nb;
-    P.branches = nb;
-  }
-  const long long low_tiles = env_int("RS_LOWRES_TILES", 64);       // a level is "few-tile" when batch * H * W / 128 <= this
-  auto is_low = [&](int hh, int ww) { return (long long)B * hh * ww / 128 <= low_tiles; };
-  bool in_sec = false;
-  int sec_first = 0;
-  auto leave = [&]() {
-    if (!in_sec) return;
-    const int last = b.opi() - 1;
-    b.marker(OP_JOIN);
-    P.sections.push_back({sec_first, last});
-    in_sec = false;
-  };
-  // one block of the topology: as a whole, or as `branches` batch slices on their own streams
-  auto run = [&](const View& hin, const std::string& prefix, const std::vector<Layer>& layers, const View& dest, View* hout) -> int {
-    bool low = P.branches > 1 && is_low(hin.H, hin.W);
-    if (P.branches > 1 && !low && layers.size() == 1 && (layers[0].kind == L_DOWN || layers[0].kind == L_RES_DOWN))
-      low = is_low(hin.H / 2, hin.W / 2);   // the stride-2 conv entering the section
-    if (!low) {
-      leave();
-      return b.run_block(hin, prefix, layers, dest, hout);
-    }
-    if (!in_sec) { b.marker(OP_FORK); sec_first = b.opi(); in_sec = true; }
-    const int per = B / P.branches;
-    for (int k = 0; k < P.branches; ++k) {
-      View tmp;
-      b.cur_stream = k; b.cur_batch0 = k * per;
-      int rc = b.run_block(rs_plan::batch(hin, k * per, per), prefix, layers, rs_plan::batch(dest, k * per, per), &tmp);
-      b.cur_stream = 0; b.cur_batch0 = 0;
-      if (rc) return rc;
-    }
-    *hout = dest;
-    return 0;
-  };
   // encoder
   View h = P.xin;
   for (int i = 0; i < n_in; ++i) {
@@ -856,14 +781,14 @@ int build_plan(rs_plan& P) {
     View dest = rs_plan::slice(cat[j], cat[j].C - ich, ich);
     // the input view of the first conv must expose the padded channel count (weights are zero-padded)
     View hin = h;
-    int rc = run(hin, "input_blocks." + std::to_string(i), topo.input_blocks[i], dest, &h);
+    int rc = b.run_block(hin, "input_blocks." + std::to_string(i), topo.input_blocks[i], dest, &h);
     if (rc) return rc;
     P.block_out["input_blocks." + std::to_string(i)] = h;
   }
   // middle: writes into the h-slice of cat[0]
   {
     View dest = rs_plan::slice(cat[0], 0, cat[0].C - topo.in_block_ch[n_in - 1]);
-    int rc = run(h, "middle_block", topo.middle, dest, &h); if (rc) return rc;
+    int rc = b.run_block(h, "middle_block", topo.middle, dest, &h); if (rc) return rc;
     P.block_out["middle_block"] = h;
   }
   // decoder
@@ -877,12 +802,11 @@ int build_plan(rs_plan& P) {
       const Layer& L0 = topo.output_blocks[j][0];
       dest = P.make_view(B, cat[j].H, cat[j].W, L0.b);
     }
-    int rc = run(cat[j], "output_blocks." + std::to_string(j), topo.output_blocks[j], dest, &h);
+    int rc = b.run_block(cat[j], "output_blocks." + std::to_string(j), topo.output_blocks[j], dest, &h);
     if (rc) return rc;
     P.block_out["output_blocks." + std::to_string(j)] = h;
     final_h = h;
   }
-  leave();
   // head (reference models/unet.py:859-863,894)
   View t = P.make_view(B, final_h.H, final_h.W, final_h.C);
   b.gn(final_h, "out.0", t, 1, -1);
@@ -896,31 +820,23 @@ void resolve(rs_plan& P, View& v) {
 }
 
 // statistics destination of a producer: the consuming GroupNorm's pair buffer (+ group statistics / arrival counters)
-// (img_off: a producer that covers only images [img_off, ...) of the consumer — a batch slice on a side stream)
 // Who reduces the (mean, M2) pairs to the image's 32 (mean, rstd)?
 //   * few tile slots (the denoiser's maps, <= 32 slots): every consumer CTA combines them itself — a finalisation step on
 //     the producer's tail sits on every producer CTA;
 //   * many slots (the VQ-GAN's 128x128 / 256x256 maps, RS_GN_FINALIZE_SLOTS moves the threshold): gn_finalize_kernel, a
-//     small launch in front of the consumer (default), or — RS_GN_PRODUCER_FINALIZE=1 — the last producer CTA of each
-//     image (arrival counters; on a persistent conv the CTAs all finish together, so ONE of them ends up reducing every
-//     image).
+//     small launch in front of the consumer, or, for a GroupNorm without a fusable producer, the last gn_stats_kernel CTA
+//     of each image (arrival counters).  (The last producer CTA of an image would do it at the cost of a counter round
+//     trip on every tile, and on a persistent conv the CTAs all finish together, so ONE of them would reduce every image.)
 bool gn_finalizes(const Op& g) {
   static const int thr = env_int("RS_GN_FINALIZE_SLOTS", 64);
   return g.gn.slots > thr && !g.gn.win_slots;      // (the fused Swin attention kernel delivers pairs only)
 }
-bool gn_producer_finalizes(const Op& g) {
-  static const int on = env_int("RS_GN_PRODUCER_FINALIZE", 0);
-  // (the fused Swin attention kernel delivers window pairs only: its consumers combine them)
-  if (g.gn.win_slots) return false;
-  // (a GroupNorm without a fusable producer runs gn_stats_kernel, whose few CTAs per image arrive themselves)
-  return gn_finalizes(g) && (on != 0 || !g.gn.fused);
-}
-GnSink make_sink(rs_plan& P, const Op& g, int coff, int img_off = 0, bool consumer = false) {
+GnSink make_sink(rs_plan& P, const Op& g, int coff, bool consumer = false) {
   GnSink s{};
-  s.part = reinterpret_cast<float*>(P.ws + P.off_stats + g.stats_off) + (size_t)img_off * g.gn.slots * g.gn.in.C * 2;
-  if (gn_producer_finalizes(g) || (consumer && gn_finalizes(g))) {
-    s.gstat = reinterpret_cast<float*>(P.ws + P.off_gstat) + (size_t)g.gn_index * P.B * 64 + (size_t)img_off * 64;
-    s.counter = reinterpret_cast<unsigned int*>(P.ws + P.off_counters) + (size_t)g.gn_index * P.B + img_off;
+  s.part = reinterpret_cast<float*>(P.ws + P.off_stats + g.stats_off);
+  if (consumer && gn_finalizes(g)) {
+    s.gstat = reinterpret_cast<float*>(P.ws + P.off_gstat) + (size_t)g.gn_index * P.B * 64;
+    s.counter = reinterpret_cast<unsigned int*>(P.ws + P.off_counters) + (size_t)g.gn_index * P.B;
   }
   s.cstride = g.gn.in.C; s.coff = coff; s.expected = (unsigned)(g.gn.slots * g.gn.in.C); s.eps = g.gn.eps;
   return s;
@@ -934,7 +850,7 @@ int bind_ops(rs_plan& P, std::vector<Op>& ops) {
         op.conv.sink[i] = GnSink{};
         if (i < (int)op.stat_dst.size()) {
           const Op::StatDst& sd = op.stat_dst[i];
-          op.conv.sink[i] = make_sink(P, (sd.list == 0 ? P.fe_ops : P.ops)[sd.op], sd.coff, sd.img_off);
+          op.conv.sink[i] = make_sink(P, (sd.list == 0 ? P.fe_ops : P.ops)[sd.op], sd.coff);
         }
       }
       ConvDesc& d = op.conv;
@@ -959,15 +875,15 @@ int bind_ops(rs_plan& P, std::vector<Op>& ops) {
       if (d.in.C < d.ipad && d.in.ld >= d.ipad && d.in.tens == P.xin.tens) d.in.C = d.ipad;
       if (d.in.C < d.ipad && P.fe_in.tens >= 0 && d.in.tens == P.fe_in.tens) d.in.C = d.ipad;
       int rc = conv_finalize(d); if (rc) return rc;
-      P.launches += (d.prm.splitk > 1 && !d.prm.splitk_cluster) ? 2 : 1;
+      P.launches += d.prm.splitk > 1 ? 2 : 1;
     } else if (op.kind == OP_GN) {
       resolve(P, op.gn.in); resolve(P, op.gn.out);
       op.gn.gamma = E.at<float>(op.g_name + ".weight"); op.gn.beta = E.at<float>(op.g_name + ".bias");
       RS_CHECK(op.gn.gamma && op.gn.beta, "missing GroupNorm parameters " + op.g_name);
       {
-        const GnSink sk = make_sink(P, op, 0, 0, true);
+        const GnSink sk = make_sink(P, op, 0, true);
         op.gn.part = sk.part; op.gn.gstat = sk.gstat; op.gn.counter = sk.counter;
-        op.gn.finalize_kernel = op.gn.fused && gn_finalizes(op) && !gn_producer_finalizes(op);
+        op.gn.finalize_kernel = op.gn.fused && gn_finalizes(op);
       }
       P.launches += (op.gn.fused ? 1 : 2) + (op.gn.finalize_kernel ? 1 : 0);
     } else if (op.kind == OP_MLP) {
@@ -988,7 +904,7 @@ int bind_ops(rs_plan& P, std::vector<Op>& ops) {
         m.sink[i] = GnSink{};
         if (i < (int)op.stat_dst.size()) {
           const Op::StatDst& sd = op.stat_dst[i];
-          m.sink[i] = make_sink(P, (sd.list == 0 ? P.fe_ops : P.ops)[sd.op], sd.coff, sd.img_off);
+          m.sink[i] = make_sink(P, (sd.list == 0 ? P.fe_ops : P.ops)[sd.op], sd.coff);
         }
       }
       int rc = mlp_finalize(m); if (rc) return rc;
@@ -1017,13 +933,11 @@ int bind_ops(rs_plan& P, std::vector<Op>& ops) {
         w.sink[i] = GnSink{};
         if (i < (int)op.stat_dst.size()) {
           const Op::StatDst& sd = op.stat_dst[i];
-          w.sink[i] = make_sink(P, (sd.list == 0 ? P.fe_ops : P.ops)[sd.op], sd.coff, sd.img_off);
+          w.sink[i] = make_sink(P, (sd.list == 0 ? P.fe_ops : P.ops)[sd.op], sd.coff);
         }
       }
       int rc = swin_attn_finalize(w); if (rc) return rc;
       ++P.launches;
-    } else if (op.kind == OP_FORK || op.kind == OP_JOIN) {
-      // stream structure only
     } else if (op.kind == OP_SOFTMAX) {
       resolve(P, op.s_view);
       int rc = softmax_rows_check(softmax_params(op)); if (rc) return rc;
@@ -1066,49 +980,32 @@ inline bool op_skipped(const Op& op) {
     case OP_MLP: return (skip >> 5) & 1;
     case OP_SWIN_ATTN: return (skip >> 3) & 1;
     case OP_VQ_ATTN: return (skip >> 3) & 1;
-    case OP_SOFTMAX: case OP_FORK: case OP_JOIN: return false;
+    case OP_SOFTMAX: return false;
   }
   return false;
 }
 
 // ops [first, last) of an op list
-int run_op_range(rs_plan& P, const Op* first, const Op* last, const float* film_base, long long film_sN, cudaStream_t st0,
+int run_op_range(rs_plan& P, const Op* first, const Op* last, const float* film_base, long long film_sN, cudaStream_t st,
                  Prof* prof = nullptr) {
-  const bool multi = prof == nullptr && !P.side.empty();       // per-op timing runs everything on the caller's stream
   for (const Op* it = first; it != last; ++it) {
     const Op& op = *it;
     int rc = 0;
-    if (op.kind == OP_FORK || op.kind == OP_JOIN) {
-      if (multi) {
-        if (op.kind == OP_FORK) {
-          RS_CUDA_OK(cudaEventRecord(P.ev[0], st0));
-          for (cudaStream_t s : P.side) RS_CUDA_OK(cudaStreamWaitEvent(s, P.ev[0], 0));
-        } else {
-          for (size_t k = 0; k < P.side.size(); ++k) {
-            RS_CUDA_OK(cudaEventRecord(P.ev[k + 1], P.side[k]));
-            RS_CUDA_OK(cudaStreamWaitEvent(st0, P.ev[k + 1], 0));
-          }
-        }
-      }
-      if (prof) { cudaEventRecord(prof->get(), st0); prof->kind.push_back((int)OP_UPSAMPLE); cudaEventRecord(prof->get(), st0); }
-      continue;
-    }
-    cudaStream_t st = (multi && op.stream > 0 && op.stream <= (int)P.side.size()) ? P.side[op.stream - 1] : st0;
     if (op_skipped(op)) { if (prof) { cudaEventRecord(prof->get(), st); prof->kind.push_back((int)op.kind); cudaEventRecord(prof->get(), st); } continue; }
     if (prof) { cudaEventRecord(prof->get(), st); prof->kind.push_back((int)op.kind); }
     switch (op.kind) {
       case OP_CONV: {
         if (op.bias_film_off < 0) { rc = conv_launch(op.conv, st); break; }
         ConvDesc d = op.conv;           // bias = this launch's FiLM row(s), resolved like a GroupNorm's film
-        const float* row = film_base + op.bias_film_off + (long long)op.bias_film_n0 * film_sN;
+        const float* row = film_base + op.bias_film_off;
         if (d.prm.bias) { d.prm.bias = row; d.prm.bias_sN = (int)film_sN; }
-        if (d.prm.splitk > 1 && !d.prm.splitk_cluster) { d.red.bias = row; d.red.bias_sN = (int)film_sN; }
+        if (d.prm.splitk > 1) { d.red.bias = row; d.red.bias_sN = (int)film_sN; }
         rc = conv_launch(d, st);
         break;
       }
       case OP_GN: {
         GnDesc g = op.gn;
-        if (g.film_off >= 0) { g.film = film_base + g.film_off + (long long)g.film_n0 * film_sN; g.film_sN = film_sN; }
+        if (g.film_off >= 0) { g.film = film_base + g.film_off; g.film_sN = film_sN; }
         rc = gn_launch(g, st);
         break;
       }
@@ -1140,9 +1037,9 @@ int run_op_range(rs_plan& P, const Op* first, const Op* last, const float* film_
   return 0;
 }
 
-int run_ops(rs_plan& P, const std::vector<Op>& ops, const float* film_base, long long film_sN, cudaStream_t st0,
+int run_ops(rs_plan& P, const std::vector<Op>& ops, const float* film_base, long long film_sN, cudaStream_t st,
             Prof* prof = nullptr) {
-  return run_op_range(P, ops.data(), ops.data() + ops.size(), film_base, film_sN, st0, prof);
+  return run_op_range(P, ops.data(), ops.data() + ops.size(), film_base, film_sN, st, prof);
 }
 
 // timestep embedding -> time_embed MLP -> all emb_layers at once, for `rows` timesteps
@@ -1196,7 +1093,7 @@ int pack_lq_and_input(rs_plan& P, const float* x, const float* lq, const float* 
   return 0;
 }
 
-// A plan runs on the device it was bound on: its side streams, events, workspace, TMA descriptors and the engine's
+// A plan runs on the device it was bound on: its workspace, TMA descriptors and the engine's
 // arena all belong to that device.  Every run entry point checks the current device first.
 int check_plan_device(const rs_plan& P) {
   int dev = -1;
@@ -1343,18 +1240,6 @@ int rs_plan_bind(rs_plan* p, void* workspace_dev) {
   if (p->fe_in.tens >= 0) { resolve(*p, p->fe_in); resolve(*p, p->lq_feat); }
   for (auto& kv : p->block_out) resolve(*p, kv.second);
   p->launches = 0;
-  if (p->branches > 1 && p->side.empty() && !p->sections.empty()) {
-    for (int k = 1; k < p->branches; ++k) {
-      cudaStream_t s = nullptr;
-      RS_CUDA_OK(cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking));
-      p->side.push_back(s);
-    }
-    for (int k = 0; k < p->branches; ++k) {
-      cudaEvent_t e = nullptr;
-      RS_CUDA_OK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-      p->ev.push_back(e);
-    }
-  }
   int rc = conv_init(); if (rc) return rc;
   rc = bind_ops(*p, p->fe_ops); if (rc) return rc;
   rc = bind_ops(*p, p->ops); if (rc) return rc;
@@ -1449,8 +1334,6 @@ static void collect_profile(const rs_plan& P, const Prof& prof, double* ms, char
       snprintf(d, desc_stride, "attn %dx%d shift=%d", op.a_in.H, op.a_in.W, op.a_shift);
     } else if (op.kind == OP_SWIN_ATTN) {
       snprintf(d, desc_stride, "swin_attn %dx%d shift=%d grid=%d", op.swin.x.H, op.swin.x.W, op.swin.shift, op.swin.grid);
-    } else if (op.kind == OP_FORK || op.kind == OP_JOIN) {
-      snprintf(d, desc_stride, "%s", op.kind == OP_FORK ? "fork" : "join");
     } else if (op.kind == OP_SOFTMAX) {
       snprintf(d, desc_stride, "softmax %d", op.s_view.C);
     } else if (op.kind == OP_VQ_ATTN) {

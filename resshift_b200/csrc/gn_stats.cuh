@@ -7,9 +7,11 @@
 //   1. every producer tile writes, per (image, tile slot, channel), the pair (mean, M2) of the fp16 values it STORED
 //      (M2 = sum of squared deviations from that local mean).  Local sums are taken around a pivot (the first row of the
 //      tile), so a channel with |mean| >> std loses nothing to cancellation (E[x^2] - mean^2 in fp32 does).
-//   2. the LAST producer CTA to finish an image (an integer arrival counter per (GroupNorm, image) decides who that is;
-//      the arithmetic does not depend on who) combines the pairs of each of the 32 groups — Chan et al.'s parallel
-//      variance formula, again around a pivot — into gstat[image][group] = (mean, rstd).
+//   2. the pairs of each of the 32 groups are combined — Chan et al.'s parallel variance formula, again around a pivot —
+//      into gstat[image][group] = (mean, rstd): by every consumer CTA itself on small maps (few tile slots), or on maps
+//      with many slots by gn_finalize_kernel, a small launch in front of the consumer, or by the last CTA of
+//      gn_stats_kernel to finish an image (an integer arrival counter per (GroupNorm, image) decides who that is; the
+//      arithmetic does not depend on who) when no producer epilogue delivers the pairs.
 //   3. consumers (gn_apply_kernel, the fused MLP's and the qkv GEMM's in-shared-memory operand transform) read the 32
 //      pairs of their image and fold gamma / beta (/ FiLM) into a per-channel affine.
 //
@@ -25,7 +27,7 @@ namespace rs {
 // encoder block and, later, the decoder's concat GroupNorm)
 struct GnSink {
   float* part;            // [N][slots][cstride][2] = (mean, M2) per image / tile slot / channel; nullptr: no statistics
-  float* gstat;           // [N][32][2] = (group mean, group rstd), written by the last-arriving producer CTA
+  float* gstat;           // [N][32][2] = (group mean, group rstd), written by the last-arriving gn_stats_kernel CTA
   unsigned int* counter;  // [N] channel-slots delivered so far (zeroed before every forward)
   int cstride;            // channel count of the consumer's tensor (this producer may cover only a slice of it)
   int coff;               // first channel of this producer's slice
@@ -147,46 +149,6 @@ __device__ __forceinline__ void gn_arrive(const GnSink* const (&sink)[kMax], con
   named_bar_sync(bar_id, nthreads);               // s_flag may be rewritten by the next tile
 }
 
-// Deferred arrivals of a persistent producer: instead of one arrival (barrier + GPU-scope atomic round trip + barrier,
-// during which the epilogue warps idle) per output tile, thread 0 records (sink, image, channels) in a small
-// shared list — merging repeats — and the CTA arrives ONCE for every entry after its last tile.
-constexpr int kGnListCap = 64;
-struct GnArriveList {
-  int cnt;
-  int over;                       // set by thread 0 when the list cannot take another tile's entries: arrive now instead
-  short sink[kGnListCap];
-  short img[kGnListCap];
-  unsigned int add[kGnListCap];
-  int flag[kGnListCap];
-};
-__device__ __forceinline__ void gn_list_add(GnArriveList* L, int d, int img, unsigned int add) {   // thread 0 only
-  for (int j = 0; j < L->cnt; ++j)
-    if (L->sink[j] == d && L->img[j] == img) { L->add[j] += add; return; }
-  const int j = L->cnt++;
-  L->sink[j] = (short)d; L->img[j] = (short)img; L->add[j] = add;
-}
-// all `nthreads` threads of the epilogue group, after the CTA's last tile (every pair store precedes the first barrier)
-__device__ __forceinline__ void gn_list_arrive(GnArriveList* L, const GnSink& s0, const GnSink& s1, int slots, float ns, int tid,
-                                               int nthreads, int bar_id) {
-  named_bar_sync(bar_id, nthreads);
-  const int cnt = L->cnt;
-  for (int j = tid; j < cnt; j += nthreads) {
-    const GnSink& s = L->sink[j] == 0 ? s0 : s1;
-    const unsigned int old = atom_add_acq_rel_gpu(s.counter + L->img[j], L->add[j]);
-    L->flag[j] = (old + L->add[j] == s.expected) ? 1 : 0;
-  }
-  named_bar_sync(bar_id, nthreads);
-  const int warp = tid >> 5, lane = tid & 31, nwarps = nthreads >> 5;
-  for (int j = 0; j < cnt; ++j) {
-    if (!L->flag[j]) continue;
-    const GnSink& s = L->sink[j] == 0 ? s0 : s1;
-    const int cpg = s.cstride / 32;
-    for (int g = warp; g < 32; g += 4 * nwarps) gn_finalize_groups<4>(s.part, L->img[j], slots, s.cstride, g, nwarps, cpg, ns, s.eps, s.gstat, lane);
-  }
-  named_bar_sync(bar_id, nthreads);
-  if (tid == 0) L->cnt = 0;
-}
-
 // (mean, M2) of the `rows` fp16 values x[r * pitch_h] (r = 0 .. rows-1) read through `ld(r)` -> float2 (two adjacent
 // columns), around the pivot ld(0).  Returns mean / M2 per column.
 template <typename Ld>
@@ -270,35 +232,6 @@ __device__ __forceinline__ void write_quad_pairs(const float* wq, int BN, int nc
         if (n0 + 1 < Nimg) {
           float* dst1 = s.part + (((size_t)(n0 + 1) * slots + slot) * s.cstride + ch) * 2;
           dst1[0] = mb; dst1[1] = qb;
-        }
-      }
-    }
-  }
-}
-
-// Final write of one tile's pairs from wstat[2 halves][BN][2] (as produced above, or by a plain [128][cw] column pass)
-// into up to two sinks.  bn = images per tile (1: both halves belong to image n0 and are merged, ns = 128; 2: half h
-// belongs to image n0 + h, ns = 64).  Thread `tid` of `nthreads` walks the tile's `ncols` valid columns.
-__device__ __forceinline__ void write_tile_pairs(const float* wstat, int BN, int ncols, int col0, int bn, int n0, int Nimg, int slot,
-                                                 int slots, const GnSink& s0, const GnSink& s1, int tid, int nthreads) {
-  for (int cc = tid; cc < ncols; cc += nthreads) {
-    const float m0 = wstat[((size_t)0 * BN + cc) * 2], q0 = wstat[((size_t)0 * BN + cc) * 2 + 1];
-    const float m1 = wstat[((size_t)1 * BN + cc) * 2], q1 = wstat[((size_t)1 * BN + cc) * 2 + 1];
-#pragma unroll
-    for (int d = 0; d < 2; ++d) {
-      const GnSink& s = d == 0 ? s0 : s1;
-      if (!s.part) continue;
-      const size_t ch = (size_t)s.coff + col0 + cc;
-      float* dst = s.part + (((size_t)n0 * slots + slot) * s.cstride + ch) * 2;
-      if (bn == 1) {
-        float m, q;
-        chan_merge_equal(64.f, m0, q0, m1, q1, m, q);
-        dst[0] = m; dst[1] = q;
-      } else {
-        dst[0] = m0; dst[1] = q0;
-        if (n0 + 1 < Nimg) {
-          float* dst1 = s.part + (((size_t)(n0 + 1) * slots + slot) * s.cstride + ch) * 2;
-          dst1[0] = m1; dst1[1] = q1;
         }
       }
     }

@@ -146,9 +146,9 @@ inline int num_sms() {
   return n;
 }
 
-// shared memory of the conv epilogue's staging area: msub output tiles + per-warp GroupNorm partials + arrival flag
+// shared memory of the conv epilogue's staging area: msub output tiles + per-warp GroupNorm partials
 inline size_t conv_epi_bytes(int BN, int msub) {
-  return (size_t)msub * ((size_t)BN * kConvBM * 2 + (size_t)4 * BN * 2 * sizeof(float)) + 16;
+  return (size_t)msub * ((size_t)BN * kConvBM * 2 + (size_t)4 * BN * 2 * sizeof(float));
 }
 // what a persistent conv CTA needs beyond its operand ring: staging area, barriers, bias tile, alignment slack
 inline size_t conv_persist_extra_bytes(int BN) { return (conv_epi_bytes(BN, 1) + 1023) / 1024 * 1024 + 256 + 1024 + 1024; }
@@ -190,7 +190,7 @@ struct ConvDesc {
   int grid = 0; size_t smem = 0;
 };
 
-struct TileConfig { int BN = 0, msub = 1, stages = 2, occ = 1, cg = 1, splitk = 1, persist = 0, cluster_split = 0; double est_cycles = 1e30; };
+struct TileConfig { int BN = 0, msub = 1, stages = 2, occ = 1, cg = 1, splitk = 1, persist = 0; double est_cycles = 1e30; };
 
 // Cost model that ranks tile configurations (its constants come from the throughput figures of the H100 SXM and have not
 // been calibrated against timelines).  Per 64-channel k-block and 128-pixel tile the tensor pipe needs 4*BN cycles
@@ -199,7 +199,7 @@ struct TileConfig { int BN = 0, msub = 1, stages = 2, occ = 1, cg = 1, splitk = 
 // multicast).  Shallow rings are additionally latency-bound (~3000 cycles per load).  The epilogue (~18 cycles per
 // column + set-up) hides under a co-resident CTA; whole waves are counted.
 inline TileConfig pick_tile_config(int m_tiles, int cout16, int num_kb, int f_bn, bool allow_split = false, bool allow_persist = false,
-                                   bool allow_cluster_split = false, bool allow_msub2 = true) {
+                                   bool allow_msub2 = true) {
   const int f_msub = env_int("RS_CONV_MSUB", 0), f_occ = env_int("RS_CONV_OCC", 0), f_stages = env_int("RS_CONV_STAGES", 0);
   const int f_cg = env_int("RS_CONV_CG", 0);
   TileConfig best, bestp;      // best one-tile-per-CTA configuration (ranking model below), best persistent one
@@ -244,7 +244,7 @@ inline TileConfig pick_tile_config(int m_tiles, int cout16, int num_kb, int f_bn
           // the staged epilogue (output tile + statistics scratch) reuses the ring: it must be at least that large
           // (short-K layers with wide channel tiles in pair mode: 2 stages x (16 KB + BN/2 x 128 B) < BN x 288 B)
           {
-            const int st_need = (int)(((size_t)ms * ((size_t)cand * kConvBM * 2 + (size_t)4 * cand * 2 * sizeof(float)) + 16 + sbytes - 1) / sbytes);
+            const int st_need = (int)((conv_epi_bytes(cand, ms) + sbytes - 1) / sbytes);
             if (st_need > budget / sbytes) continue;
             st = std::max(st, st_need);
           }
@@ -263,36 +263,24 @@ inline TileConfig pick_tile_config(int m_tiles, int cout16, int num_kb, int f_bn
           // split-K: S CTAs (pairs) share one output tile's K loop; costs an fp32 round trip + a small reduce kernel
           const int f_split = env_int("RS_CONV_SPLITK", 0);
           const int kSplits[6] = {1, 2, 3, 4, 6, 8};
-          // split-K flavours: 0 = none / global (fp32 partials in HBM scratch + splitk_reduce_kernel), 1 = cluster (the S
-          // pairs of a tile are one cluster of 2S CTAs and reduce through distributed shared memory: pair mode)
-          const char* f_mode = std::getenv("RS_CONV_SPLITK_MODE");
-          for (int mode = 0; mode < 2; ++mode)
           for (int si = 0; si < 6; ++si) {
             const int S = kSplits[si];
-            // (S = 2 only: clusters of 4 CTAs; larger clusters of CTAs with ~200 KB of shared memory each schedule poorly)
-            if (mode == 1 && (S != 2 || !allow_cluster_split || cg != 2 || occ != 1 || (cand / S) % 8 != 0)) continue;
-            // cluster split-K only on request (RS_CONV_SPLITK_MODE=cluster): on the H100 every 8x8 / 16x16 denoiser conv that
-            // picked it ran 1.5-2.3x slower than the best global split-K or unsplit configuration (DESIGN.md §7)
-            if (mode == 1 && !(f_mode && std::strcmp(f_mode, "cluster") == 0)) continue;
-            if (mode == 0 && S > 1 && f_mode && std::strcmp(f_mode, "cluster") == 0) continue;
-            if (mode == 1 && (size_t)kConvBM * (cand * 4 + 16) + (size_t)kConvBM * (cand / S) * 2 + (size_t)4 * (cand / S) * 4 + 16 > (size_t)st * sbytes) continue;
-            if (S > 1 && ((mode == 0 && !allow_split) || ms != 1 || num_kb / S < 6)) continue;
-            if (f_split && (allow_split || allow_cluster_split) && ms == 1 && num_kb / f_split >= 6 && S != f_split) continue;
+            if (S > 1 && (!allow_split || ms != 1 || num_kb / S < 6)) continue;
+            if (f_split && allow_split && ms == 1 && num_kb / f_split >= 6 && S != f_split) continue;
             const double waves = std::ceil((double)units * S / slots);
             const double kbs = std::ceil((double)num_kb / S);
             const double round = kbs * kb_cycles + (occ == 2 ? 0.5 * epi : epi);
-            // global: fp32 partials written once by the conv epilogue and read once by the reduce kernel (assumed ~2 KB/clk
-            // chip-wide each way), plus a second kernel launch / drain (a fixed cost for the pair);
-            // cluster: a cluster barrier and one pass over the tile through distributed shared memory
+            // fp32 partials written once by the conv epilogue and read once by the reduce kernel (assumed ~2 KB/clk
+            // chip-wide each way), plus a second kernel launch / drain (a fixed cost for the pair)
             const double part_bytes = 4.0 * m_tiles * 128.0 * cout16 * S;
-            const double total = waves * round + (S == 1 ? 0.0 : mode == 1 ? 6000.0 : 19000.0 + 2.0 * part_bytes / 2048.0);
+            const double total = waves * round + (S == 1 ? 0.0 : 19000.0 + 2.0 * part_bytes / 2048.0);
             if (total < best.est_cycles) {
               best.est_cycles = total; best.BN = cand; best.msub = ms;
-              best.stages = std::max(std::min(st, (int)std::max(2.0, kbs)), std::min(st, (int)(((size_t)ms * ((size_t)cand * kConvBM * 2 + (size_t)4 * cand * 2 * sizeof(float)) + 16 + sbytes - 1) / sbytes)));
-              best.occ = occ; best.cg = cg; best.splitk = S; best.persist = 0; best.cluster_split = (S > 1 && mode == 1) ? 1 : 0;
+              best.stages = std::max(std::min(st, (int)std::max(2.0, kbs)), std::min(st, (int)((conv_epi_bytes(cand, ms) + sbytes - 1) / sbytes)));
+              best.occ = occ; best.cg = cg; best.splitk = S; best.persist = 0;
               // what a wave really costs (timelines r1_s25): co-resident CTAs run in lockstep, so set-up, the first
               // operand round trip and the whole epilogue are exposed once per wave
-              best_real = waves * (kbs * kb_cycles + epi + 5000.0) + (S == 1 ? 0.0 : mode == 1 ? 6000.0 : 19000.0 + 2.0 * part_bytes / 2048.0);
+              best_real = waves * (kbs * kb_cycles + epi + 5000.0) + (S == 1 ? 0.0 : 19000.0 + 2.0 * part_bytes / 2048.0);
             }
           }
         }
@@ -315,7 +303,7 @@ inline TileConfig conv_preview_config(int N, int Hin, int Win, int Cin, int Cout
   const bool contiguous = (bw == Wout) || (bh == 1);
   const int num_kb = ksize * ksize * ((Cin + kConvBK - 1) / kConvBK);
   const bool sp = allow_split && contiguous && bn <= 2;
-  return pick_tile_config(m_tiles, (Cout + 15) / 16 * 16, num_kb, env_int("RS_CONV_BN", 0), sp, false, sp && Cout % 8 == 0);
+  return pick_tile_config(m_tiles, (Cout + 15) / 16 * 16, num_kb, env_int("RS_CONV_BN", 0), sp);
 }
 
 inline int conv_finalize(ConvDesc& d) {
@@ -347,15 +335,13 @@ inline int conv_finalize(ConvDesc& d) {
   const bool simt = env_is("RS_CONV_IMPL", "simt");
   const bool can_split = d.allow_split && d.partial != nullptr && contiguous_tiles && p.bn <= 2 && d.has_out && !d.out_f32 && !simt;
   const int want_persist = env_int("RS_CONV_PERSIST", -1);           // 0 / 1 disables / forces the persistent kernel
-  // (the persistent kernel batches its GroupNorm arrivals in a shared list of kGnListCap (sink, image) entries)
   const bool persist_ok = d.has_out && !d.out_f32 && want_persist != 0 && !env_is("RS_CONV_EPI", "direct") &&
                           !env_is("RS_CONV_IMPL", "simt") && env_int("RS_CONV_MSUB", 0) != 2;
-  const bool can_cluster_split = d.allow_split && contiguous_tiles && p.bn <= 2 && d.has_out && !d.out_f32 && d.Cout % 8 == 0 && !simt;
   const TileConfig tc = pick_tile_config(m_tiles, cout16, num_kb, d.bn_override ? d.bn_override : env_int("RS_CONV_BN", 0), can_split,
-                                         persist_ok && want_persist != 1, can_cluster_split, !d.bias_per_image);
+                                         persist_ok && want_persist != 1, !d.bias_per_image);
   const int BN = tc.BN, msub = tc.msub, stages = tc.stages, cg = tc.cg;
   p.cg = cg;
-  p.splitk = tc.splitk; p.partial = d.partial; p.splitk_cluster = tc.cluster_split;
+  p.splitk = tc.splitk; p.partial = d.partial;
   RS_CHECK(conv_kernel_for(BN, msub) != nullptr, "no valid tile configuration");
   p.BN = BN; p.n_tiles = (cout16 + BN - 1) / BN;
   p.msub = msub;
@@ -415,8 +401,7 @@ inline int conv_finalize(ConvDesc& d) {
     }
     // the staging area (column blocks + per-warp GN partials) must fit in the operand ring
     // (the persistent kernel stages in buffers of its own, sized below)
-    const size_t need = (size_t)msub * ((size_t)BN * kConvBM * 2 + (size_t)4 * BN * 2 * sizeof(float)) + 16;
-    RS_CHECK(tc.persist || need <= (size_t)stages * stage_bytes, "epilogue staging does not fit in the pipeline shared memory");
+    RS_CHECK(tc.persist || conv_epi_bytes(BN, msub) <= (size_t)stages * stage_bytes, "epilogue staging does not fit in the pipeline shared memory");
   }
   // persistent variant (conv_persist.cuh) when the cost model chose it (every SM / pair gets at least two tiles), or
   // when RS_CONV_PERSIST = 1 forces it for any eligible layer
@@ -458,11 +443,7 @@ inline int conv_finalize(ConvDesc& d) {
     GnSink none[2] = {};
     if (p.tma_out) fill_sinks(p.sink); else { p.sink[0] = none[0]; p.sink[1] = none[1]; }
   }
-  if (p.splitk > 1 && p.splitk_cluster) {
-    // cluster split-K: the conv kernel finishes the layer itself (DSMEM reduce + direct epilogue), statistics included
-    fill_sinks(p.sink);
-    RS_CHECK(cg == 2 && d.Cout % 8 == 0 && (BN / p.splitk) % 8 == 0, "cluster split-K configuration");
-  } else if (p.splitk > 1) {
+  if (p.splitk > 1) {
     // the conv kernel only produces fp32 partial sums; bias / activation / residual / fp16 store / GroupNorm statistics
     // happen in the reduce kernel, one CTA per (128-pixel slot, image)
     SplitKReduceParams& r = d.red;
@@ -482,7 +463,7 @@ inline int conv_finalize(ConvDesc& d) {
     r.cols_per_cta = cpc;
     d.red_grid_z = (d.Cout + cpc - 1) / cpc;
     const int lanes = 256 / std::max(1, cpc / 8);
-    d.red_smem = (size_t)std::max(1, lanes) * cpc * 3 * sizeof(float) + 16;
+    d.red_smem = (size_t)std::max(1, lanes) * cpc * 3 * sizeof(float);
   }
   // tensor maps + SIMT mirrors
   ConvSimtSrc& s = d.simt;
@@ -546,9 +527,8 @@ inline int conv_launch(const ConvDesc& d, cudaStream_t st) {
   } else {
     const ConvKernelFn k = conv_kernel_for(d.prm.BN, d.prm.msub);
     RS_CHECK(k != nullptr, "no conv kernel for this channel tile");
-    const int cluster = d.prm.cg == 2 ? (d.prm.splitk_cluster ? 2 * d.prm.splitk : 2) : 1;
-    (void)launch_kc(k, dim3(d.grid), dim3(kConvThreads), (size_t)(d.smem), st, cluster, d.prm);
-    if (d.prm.splitk > 1 && !d.prm.splitk_cluster)
+    (void)launch_kc(k, dim3(d.grid), dim3(kConvThreads), (size_t)(d.smem), st, d.prm.cg, d.prm);
+    if (d.prm.splitk > 1)
       (void)launch_k(splitk_reduce_kernel, dim3(d.red_grid_x, d.prm.Nimg, d.red_grid_z), dim3(256), d.red_smem, st, d.red);
   }
   RS_CUDA_OK(cudaGetLastError());
@@ -570,10 +550,9 @@ struct GnDesc {
   const float* gamma = nullptr; const float* beta = nullptr;
   const float* film = nullptr; long long film_sN = 0;   // resolved per launch for FiLM layers
   int film_off = -1;      // offset of this layer's [2C] slice inside an embedding row, or -1
-  int film_n0 = 0;        // first image of this (batch-sliced) op inside the plan's batch: row offset into per-image FiLM
   int silu = 0;
   float* part = nullptr;  // [N][slots][C][2] (mean, M2) pairs
-  float* gstat = nullptr; // [N][32][2] (mean, rstd), finalised by the last producer CTA of each image
+  float* gstat = nullptr; // [N][32][2] (mean, rstd), finalised by gn_finalize_kernel or the last gn_stats_kernel CTA
   unsigned int* counter = nullptr;   // [N]
   float eps = 1e-5f;
   int slots = 0;

@@ -321,6 +321,8 @@ __global__ void __launch_bounds__(kMlpThreads, 1) mlp_fused_sm90_kernel(const __
     const int slot = th * p.tiles_w + tw;
     if (n0 < p.Nimg)
       write_quad_pairs(wsum, E, E, 0, p.bn, n0, p.Nimg, slot, p.gn_slots, p.sink[0], p.sink[1], etid, kCons);
+    // (no plan gives an MLP sink group statistics; without this branch ptxas spills loop state of the <128> / <192>
+    // instances in the main loop, so it stays)
     if (p.sink[0].gstat || p.sink[1].gstat) {
       int* s_flag = reinterpret_cast<int*>(wsum + 8 * E);
       const GnSink* const sk[4] = {&p.sink[0], &p.sink[0], p.sink[1].part ? &p.sink[1] : nullptr, p.sink[1].part ? &p.sink[1] : nullptr};

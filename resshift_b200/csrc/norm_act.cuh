@@ -4,10 +4,11 @@
 // (models/unet.py:144-148,168-175,198-202: GN -> SiLU, and GN*(1+scale)+shift -> SiLU) and in
 // SwinTransformerBlock (models/swin_transformer.py:248,279: plain GN), final head (unet.py:859-863).
 //
-// Statistics (gn_stats.cuh): every producer tile delivers (mean, M2) pairs per (image, slot, channel); the last producer
-// CTA of an image reduces them to gstat[image][group] = (mean, rstd).  Producers are
+// Statistics (gn_stats.cuh): every producer tile delivers (mean, M2) pairs per (image, slot, channel).  Producers are
 //   * the epilogue of the conv / GEMM / MLP kernel that wrote the tensor (one slot per 128-pixel tile), or
-//   * gn_stats_kernel below (one slot per CTA) for tensors that have no fusable producer.
+//   * gn_stats_kernel below (one slot per CTA) for tensors that have no fusable producer; with group statistics
+//     requested, its last CTA of an image reduces the pairs to gstat[image][group] = (mean, rstd).
+// The pairs of a fused producer are reduced by the consumer itself or by gn_finalize_kernel (many tile slots).
 // gn_apply_kernel folds (mean, rstd, gamma, beta, FiLM) into a per-(image, channel) affine a*x+b in shared memory,
 // then streams x -> y = act(a*x+b) with 128-bit accesses.
 #pragma once

@@ -20,7 +20,7 @@ KNOBS = ("RS_CONV_BN", "RS_CONV_CG", "RS_CONV_OCC", "RS_CONV_SPLITK")
 
 def time_conv(t, iters=24):
     x, wp, ipad, b, out, scratch, dbg, (N, H, W, Ci, Co, k) = t
-    info = (C.c_int32 * 8)()
+    info = (C.c_int32 * 7)()
     st = _lib.current_stream()
     rc = L.rs_op_conv2d_timeline(x.data_ptr(), N, H, W, Ci, Ci, wp.data_ptr(), ipad, b.data_ptr(), Co, k, 1,
                                  out.data_ptr(), Co, 0, 3, dbg.data_ptr(), info, scratch.data_ptr(), st)
@@ -34,7 +34,7 @@ def time_conv(t, iters=24):
                             out.data_ptr(), Co, 0, iters, dbg.data_ptr(), info, scratch.data_ptr(), st)
     e1.record()
     torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / iters * 1e3, (info[1], info[4], info[5], info[2], info[0], info[6], info[7])
+    return e0.elapsed_time(e1) / iters * 1e3, (info[1], info[4], info[5], info[2], info[0], info[6])
 
 
 def main():
@@ -80,7 +80,7 @@ def main():
         best = results[0]
         total_def += t_def; total_best += best[0]
         top = "  ".join(f"[{r[0]:.1f}us BN={r[1]} cg={r[2]} occ={r[3]} S={r[4]} st={r[5]}]" for r in results[:4])
-        print(f"{HW}x{HW} Cin={Ci} Cout={Co} k={k}: default {t_def:.1f}us (BN={cfg_def[0]} cg={cfg_def[1]} S={cfg_def[2]}{'c' if cfg_def[5] else ''} st={cfg_def[3]} grid={cfg_def[4]}{' persist' if cfg_def[6] else ''})"
+        print(f"{HW}x{HW} Cin={Ci} Cout={Co} k={k}: default {t_def:.1f}us (BN={cfg_def[0]} cg={cfg_def[1]} S={cfg_def[2]} st={cfg_def[3]} grid={cfg_def[4]}{' persist' if cfg_def[5] else ''})"
               f" | best {top}", flush=True)
     print(f"sum default {total_def:.1f} us, sum best {total_best:.1f} us")
 

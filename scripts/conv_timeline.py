@@ -22,7 +22,7 @@ def run(N, H, W, Ci, Co, k, bn=0, iters=20, tag=""):
     b = torch.randn(Co, device="cuda")
     wp, ipad = G.pack_weight(w)
     out = torch.empty(N, H, W, Co, dtype=torch.float16, device="cuda")
-    info = (C.c_int32 * 8)()
+    info = (C.c_int32 * 7)()
     scratch = torch.empty(8 * N * H * W * Co, dtype=torch.float32, device="cuda") if os.environ.get("TL_SPLIT") else None
     dbg = torch.zeros(8 * 8192, dtype=torch.int64, device="cuda")
     st = _lib.current_stream()

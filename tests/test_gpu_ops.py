@@ -153,14 +153,15 @@ def _combine_pairs(pairs, hw):
     return mean_c.float(), (m2 / hw).float()
 
 
-@pytest.mark.parametrize("variant", ["cg1", "cg2", "persist_cg2", "splitk_global", "splitk_cluster"])
+@pytest.mark.parametrize("variant", ["cg1", "cg2", "persist_cg2", "splitk_global"])
 @pytest.mark.parametrize("case", [(16, 64, 64, 64, 160, 3, 30.0), (3, 16, 16, 160, 320, 3, 0.5), (16, 8, 8, 320, 640, 3, -30.0),
                                   (5, 8, 8, 64, 192, 1, 30.0)])
-def test_conv_statistics_finalised_by_last_cta(case, variant):
-    """Producer -> consumer GroupNorm without a statistics pass: the conv epilogue delivers (mean, M2) pairs, the last CTA
-    to finish an image writes gstat[N][32] = (mean, rstd), rs_op_groupnorm_apply consumes it.  Checked against
-    F.group_norm (fp32) of the STORED fp16 conv output, including channels whose mean (conv bias +-30) dwarfs their
-    spread — the case a single-pass E[x^2] - mean^2 loses.  reference: GroupNorm32, models/basic_ops.py:15-17."""
+def test_conv_statistics_to_group_stats(case, variant):
+    """Producer -> consumer GroupNorm without a statistics pass: the conv epilogue delivers (mean, M2) pairs, the
+    finalisation kernel the op enqueues behind it writes gstat[N][32] = (mean, rstd), rs_op_groupnorm_apply consumes
+    it.  Checked against F.group_norm (fp32) of the STORED fp16 conv output, including channels whose mean (conv bias
+    +-30) dwarfs their spread — the case a single-pass E[x^2] - mean^2 loses.  reference: GroupNorm32,
+    models/basic_ops.py:15-17."""
     import ctypes as C
     N, H, W, Ci, Co, k, bias_mean = case
     if variant.startswith("splitk") and H > 16:
@@ -176,8 +177,7 @@ def test_conv_statistics_finalised_by_last_cta(case, variant):
     beta = 0.2 * torch.randn(Co, device="cuda", generator=g)
     env = {"cg1": {"RS_CONV_CG": "1", "RS_CONV_PERSIST": "0"}, "cg2": {"RS_CONV_CG": "2", "RS_CONV_PERSIST": "0"},
            "persist_cg2": {"RS_CONV_CG": "2", "RS_CONV_PERSIST": "1"},
-           "splitk_global": {"RS_CONV_SPLITK": "2", "RS_CONV_SPLITK_MODE": "global"},
-           "splitk_cluster": {"RS_CONV_SPLITK": "2", "RS_CONV_SPLITK_MODE": "cluster"}}[variant]
+           "splitk_global": {"RS_CONV_SPLITK": "2"}}[variant]
     os.environ.update(env)
     try:
         results = []
@@ -217,7 +217,7 @@ def test_conv_statistics_finalised_by_last_cta(case, variant):
         for kk in env:
             os.environ.pop(kk, None)
     out, gstat, y = results[0]
-    assert torch.equal(gstat, results[1][1]) and torch.equal(y, results[1][2])           # deterministic whoever arrives last
+    assert torch.equal(gstat, results[1][1]) and torch.equal(y, results[1][2])           # deterministic
     assert not torch.isnan(gstat).any()
     of = G.nchw32(out)                                                                  # [N, Co, H, W] fp32 of the stored values
     grp = of.reshape(N, 32, -1).double()
@@ -269,17 +269,13 @@ def test_conv2d_persistent_matches_one_tile_per_cta(case, cg):
     assert (G.nchw32(outs[1]) - ref).abs().max().item() <= _tol(ref)
 
 
-@pytest.mark.parametrize("mode", ["global", "cluster"])
 @pytest.mark.parametrize("force", [0, 2, 4])
 @pytest.mark.parametrize("case", [(16, 8, 8, 640, 640, 3), (3, 16, 16, 320, 320, 3), (5, 8, 8, 192, 192, 1), (2, 16, 16, 960, 320, 3)])
-def test_conv2d_split_k(case, force, mode):
-    """Layers with few output tiles split their K loop over several CTAs (pairs).  `global`: fp32 partial sums go to a
-    scratch buffer and the reduce kernel combines them in a fixed order, applies bias / residual and emits the GroupNorm
-    partial statistics.  `cluster`: the K ranges of a tile form one thread-block cluster, keep their partial tiles in
-    shared memory and finish the layer themselves through distributed shared memory (no scratch, no second kernel)."""
+def test_conv2d_split_k(case, force):
+    """Layers with few output tiles split their K loop over several CTAs (pairs): fp32 partial sums go to a scratch
+    buffer and the reduce kernel combines them in a fixed order, applies bias / residual and emits the GroupNorm partial
+    statistics."""
     import ctypes as C
-    if mode == "cluster" and force == 4:
-        pytest.skip("cluster split-K is limited to two K ranges (clusters of 4 CTAs)")
     N, H, W, Ci, Co, k = case
     g = torch.Generator(device="cuda").manual_seed(sum(case))
     x = G.nhwc16(torch.randn(N, Ci, H, W, device="cuda", generator=g))
@@ -290,7 +286,6 @@ def test_conv2d_split_k(case, force, mode):
     scratch = torch.empty(8 * N * H * W * Co, dtype=torch.float32, device="cuda")
     if force:
         os.environ["RS_CONV_SPLITK"] = str(force)
-    os.environ["RS_CONV_SPLITK_MODE"] = mode
     try:
         outs, parts, used = [], [], []
         for rep in range(2):
@@ -304,8 +299,7 @@ def test_conv2d_split_k(case, force, mode):
             outs.append(out); parts.append(part.clone()); used.append(S.value)
     finally:
         os.environ.pop("RS_CONV_SPLITK", None)
-        os.environ.pop("RS_CONV_SPLITK_MODE", None)
-    print(f"[split-k] case {case} forced {force} mode {mode}: S = {used[0]}")
+    print(f"[split-k] case {case} forced {force}: S = {used[0]}")
     assert torch.equal(outs[0], outs[1]) and torch.equal(parts[0][~torch.isnan(parts[0])], parts[1][~torch.isnan(parts[1])])
     ref = G.ref_conv(x, w, b, residual=res)
     st = G.err_stats(G.nchw32(outs[0]), ref)
@@ -319,13 +313,10 @@ def test_conv2d_split_k(case, force, mode):
     assert ((var_c - v_ref).abs() / (v_ref + 1e-6)).max().item() <= 1e-4
 
 
-@pytest.mark.parametrize("hsplit", [1, 2])
 @pytest.mark.parametrize("case", [(2, 16, 16, 192, 768), (1, 64, 64, 64, 256), (3, 8, 8, 192, 768), (4, 32, 32, 192, 768)])
-def test_fused_mlp(case, hsplit, monkeypatch):
+def test_fused_mlp(case):
     """out = residual + fc2(GELU(fc1(x))) in one kernel (hidden activations stay on chip, rounded to fp16 like the
-    unfused path rounds its stored intermediate).  RS_MLP_HSPLIT is set both ways: the kernel has no hidden-dimension
-    split, so the results must not depend on it."""
-    monkeypatch.setenv("RS_MLP_HSPLIT", str(hsplit))
+    unfused path rounds its stored intermediate)."""
     N, H, W, E, Hd = case
     g = torch.Generator(device="cuda").manual_seed(sum(case))
     x = G.nhwc16(torch.randn(N, E, H, W, device="cuda", generator=g))
