@@ -38,8 +38,9 @@ extern "C" {
  * files vary.  The constructor options the shipped files leave at one value are in rs_unet_options.
  * Covered: dims = 2 (the struct has no field for it), cond_lq = True (the reference cannot run
  * cond_lq = False), any dropout (identity at inference), cond_mask with or without an LQ feature
- * extractor.  Refused by rs_unet_create / rs_unet_create_ex: window_size != 8 and head dims
- * (swin_embed_dim / swin_heads) other than 32, the specialisations of the attention kernels. */
+ * extractor, window_size 8 or 16, head dims (swin_embed_dim / swin_heads) of 32 or 64.  Refused by
+ * rs_unet_create / rs_unet_create_ex: any other window_size or head dim (the window-attention
+ * kernels are instantiated for those four combinations). */
 typedef struct rs_unet_config {
   int32_t image_size;
   int32_t in_channels;
@@ -288,10 +289,16 @@ int rs_op_vq_attention_rows(const void* q, const void* k, const void* v, int N, 
  * not touched.  Needs rows >= 1, cols a multiple of 8 in [8, 8192], ld >= cols and a multiple of 8, s 16-byte aligned;
  * anything else returns an error. */
 int rs_op_softmax_rows(void* s, int rows, int cols, long long ld, float scale, void* stream);
-/* window attention core (reference models/swin_transformer.py:114-145,251-275); qkv [N,H,W,3*heads*32] */
+/* window attention core (reference models/swin_transformer.py:114-145,251-275); qkv [N,H,W,3*heads*32], 8x8 windows */
 int rs_op_expand_relpos(const float* table_225xh, float* dense_hx64x64, int heads, void* stream);
 int rs_op_window_attention(const void* qkv, int N, int H, int W, int heads, int shift, const float* bias_dense,
                            void* out, void* stream);
+/* the same for window 8 or 16 and head_dim 32 or 64: table [(2 window - 1)^2, heads] -> dense
+ * [heads][window^2][window^2]; qkv [N,H,W,3*heads*head_dim] -> out [N,H,W,heads*head_dim]; H and W multiples of window,
+ * shift 0 or window / 2.  RS_ATTN_IMPL=simt runs the fp32 cross-check kernel instead of the tensor-core instance. */
+int rs_op_expand_relpos_ex(const float* table, float* dense, int heads, int window, void* stream);
+int rs_op_window_attention_ex(const void* qkv, int N, int H, int W, int heads, int window, int head_dim, int shift,
+                              const float* bias_dense, void* out, void* stream);
 /* fused attention half of a Swin block: y = x + proj(window_attention(qkv(norm1(x)))) (reference
  * models/swin_transformer.py:246-275 with WindowAttention.forward :114-145); x NHWC fp16 [N,H,W,E] (in place when
  * y == x), norm1 statistics as the producers' (mean, M2) pairs gn_part[N][gn_slots][E][2], weights packed fp16;

@@ -96,10 +96,12 @@ _SIGNATURES = {
     "rs_op_groupnorm_apply_pairs": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P, _P, C.c_longlong,
                                               C.c_int, _P, C.c_int, _P, C.c_int, _P]),
     "rs_op_expand_relpos": (C.c_int, [_P, _P, C.c_int, _P]),
+    "rs_op_expand_relpos_ex": (C.c_int, [_P, _P, C.c_int, C.c_int, _P]),
     "rs_op_vq_attention": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P]),
     "rs_op_vq_attention_rows": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P]),
     "rs_op_softmax_rows": (C.c_int, [_P, C.c_int, C.c_int, C.c_longlong, C.c_float, _P]),
     "rs_op_window_attention": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P, _P]),
+    "rs_op_window_attention_ex": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P, _P]),
     "rs_op_swin_attn": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, C.c_int, _P, _P, _P, _P, _P, _P, _P,
                                   _P, _P, _P, _P, _P]),
     "rs_op_mlp": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P, _P, _P, _P, _P, _P, _P]),

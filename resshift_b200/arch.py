@@ -59,6 +59,15 @@ def swin_geometry(cfg: UNetConfig, res: int) -> Tuple[int, int]:
     return cfg.window_size, cfg.window_size // 2
 
 
+def latent_multiple(cfg: UNetConfig) -> int:
+    """What H and W of a latent must be multiples of: every level's map (H / 2^level) is tiled by that level's window."""
+    import math
+    m = 1
+    for level in range(len(cfg.channel_mult)):
+        m = math.lcm(m, swin_geometry(cfg, cfg.image_size >> level)[0] << level)
+    return m
+
+
 def _basic_layer(name: str, cfg: UNetConfig, c: int, res: int) -> List[Spec]:
     e, heads = cfg.swin_embed_dim, cfg.swin_heads
     win, shift = swin_geometry(cfg, res)

@@ -53,11 +53,12 @@ class UNetConfig:
         if not self.cond_lq:
             raise ValueError("cond_lq=False: the reference cannot run it either (it widens the first conv by the LQ "
                              "channels but skips the concatenation when lq is None)")
-        if self.window_size != 8:
-            raise ValueError(f"window_size={self.window_size}: the window-attention kernels are specialised for 8x8 windows")
-        if self.swin_embed_dim % self.swin_heads or self.swin_embed_dim // self.swin_heads != 32:
+        if self.window_size not in (8, 16):
+            raise ValueError(f"window_size={self.window_size}: the window-attention kernels are instantiated for 8x8 and "
+                             f"16x16 windows")
+        if self.swin_embed_dim % self.swin_heads or self.swin_embed_dim // self.swin_heads not in (32, 64):
             raise ValueError(f"head dim {self.swin_embed_dim / self.swin_heads:g}: the window-attention kernels are "
-                             f"specialised for a head dim of 32 (num_head_channels=32)")
+                             f"instantiated for head dims of 32 and 64 (num_head_channels 32 or 64)")
 
     # -- derived quantities (reference models/unet.py:689-709) -----------------
     @property

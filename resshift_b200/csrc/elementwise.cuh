@@ -362,16 +362,17 @@ __global__ void pack_conv_weight_kernel(const float* __restrict__ src, __half* _
   }
 }
 
-// relative_position_bias_table [(2w-1)^2, heads] -> dense [heads][64][64] fp32 (window 8)
+// relative_position_bias_table [(2w-1)^2, heads] -> dense [heads][w*w][w*w] fp32
 // (reference models/swin_transformer.py:93-103 for the index, :127-130 for the gather)
-__global__ void expand_relpos_kernel(const float* __restrict__ table, float* __restrict__ dst, int heads) {
+__global__ void expand_relpos_kernel(const float* __restrict__ table, float* __restrict__ dst, int heads, int w) {
   pdl_trigger();
   pdl_wait();
+  const int T = w * w;
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= heads * 64 * 64) return;
-  const int h = i / 4096, r = (i / 64) % 64, c = i % 64;
-  const int dy = (r >> 3) - (c >> 3) + 7, dx = (r & 7) - (c & 7) + 7;
-  dst[i] = table[(dy * 15 + dx) * heads + h];
+  if (i >= heads * T * T) return;
+  const int h = i / (T * T), r = (i / T) % T, c = i % T;
+  const int dy = r / w - c / w + w - 1, dx = r % w - c % w + w - 1;
+  dst[i] = table[(dy * (2 * w - 1) + dx) * heads + h];
 }
 
 __global__ void copy_f32_kernel(const float* __restrict__ src, float* __restrict__ dst, long long n) {

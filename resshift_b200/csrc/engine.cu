@@ -11,6 +11,7 @@
 //     kernels; in the sampling loop the table for all T steps is computed once.
 #include <map>
 #include <memory>
+#include <numeric>
 #include <string>
 #include <vector>
 
@@ -196,6 +197,13 @@ void add_layers(rs_engine& e, const std::string& prefix, const std::vector<Layer
   }
 }
 
+// window side w of a relative_position_bias_table [(2w-1)^2, heads]
+int relpos_window(const Param& p) {
+  int w = 1;
+  while ((2 * w - 1) * (2 * w - 1) < p.shape[0]) ++w;
+  return w;
+}
+
 int build_inventory(rs_engine& e) {
   const rs_unet_config& c = e.cfg;
   add_linear(e, "time_embed.0", c.model_channels, e.time_dim());
@@ -251,8 +259,10 @@ int build_inventory(rs_engine& e) {
         p.bytes = (size_t)p.shape[0] * p.ipad * 2; break;
       case R_BIAS: case R_GN_W: case R_GN_B:
         p.bytes = (size_t)p.shape[0] * 4; break;
-      case R_RELPOS:
-        p.bytes = (size_t)c.swin_heads * 64 * 64 * 4; break;
+      case R_RELPOS: {    // expanded at load time to dense [heads][w*w][w*w] fp32
+        const int w = relpos_window(p);
+        p.bytes = (size_t)c.swin_heads * w * w * w * w * 4; break;
+      }
       default: p.bytes = 0; break;     // buffers are derived, not stored
     }
     if (p.bytes) { p.off = off; off = align_up(off + p.bytes, 256); }
@@ -282,7 +292,7 @@ struct Op {
   ConvDesc conv;
   GnDesc gn;
   // attention
-  View a_in, a_out; const float* a_bias = nullptr; int a_shift = 0;
+  View a_in, a_out; const float* a_bias = nullptr; int a_window = 8, a_shift = 0;
   // 2x resampling: nearest upsample, or (u_pool) 2x2 average pool
   View u_in, u_out; bool u_pool = false;
   // conv whose bias is a FiLM-table row (ResBlock without scale-shift norm): its offset in a row, or -1
@@ -472,8 +482,8 @@ struct Builder {
     for (const Writer& w : prod)
       list(w.list)[w.op].stat_dst.push_back({list_id(), (int)cur->size() - 1, w.c0 - in.c0});
   }
-  void attn(const View& qkv, const View& out, const std::string& blk, int shift) {
-    Op op; op.kind = OP_ATTN; op.a_in = qkv; op.a_out = out; op.a_shift = shift;
+  void attn(const View& qkv, const View& out, const std::string& blk, int window, int shift) {
+    Op op; op.kind = OP_ATTN; op.a_in = qkv; op.a_out = out; op.a_window = window; op.a_shift = shift;
     op.w_name = blk + ".attn.relative_position_bias_table";
     const int i = opi();
     P.touch(qkv, i); P.touch(out, i);
@@ -575,7 +585,9 @@ struct Builder {
     const rs_unet_config& c = E.cfg;
     const int Ed = c.swin_embed_dim, hidden = (int)(Ed * c.mlp_ratio);
     const int win = ctor_res <= c.window_size ? ctor_res : c.window_size;
-    RS_CHECK(win == 8 && x.H % 8 == 0 && x.W % 8 == 0, "the window-attention kernel covers 8x8 windows only");
+    RS_CHECK((win == 8 || win == 16) && x.H % win == 0 && x.W % win == 0,
+             "a " + std::to_string(x.H) + "x" + std::to_string(x.W) + " level with " + std::to_string(win) + "x" + std::to_string(win) +
+             " windows: the window-attention kernels cover 8x8 and 16x16 windows that tile the level");
     const int shift_odd = ctor_res <= c.window_size ? 0 : c.window_size / 2;
     View e = P.make_view(x.N, x.H, x.W, Ed);
     if (E.opt.patch_norm) {
@@ -592,15 +604,15 @@ struct Builder {
       // x = x + proj(attn(qkv(norm1(x)))): one kernel (swin_attn_fused.cuh), or the four-launch sequence
       // (a level with few window pairs is one long serial tile per CTA on a handful of SMs: below fuse_swin_min_pairs the
       //  four small launches, whose prologues overlap through PDL, are faster in the graph)
-      const int win_pairs = (x.N * (x.H / 8) * (x.W / 8) + 1) / 2;
-      if (!(fuse_swin_attn && win_pairs >= fuse_swin_min_pairs && swin_attn_supported(Ed, c.swin_heads, x.H, x.W) &&
+      const int win_pairs = (x.N * (x.H / win) * (x.W / win) + 1) / 2;
+      if (!(fuse_swin_attn && win_pairs >= fuse_swin_min_pairs && swin_attn_supported(Ed, c.swin_heads, x.H, x.W, win) &&
             swin_attn(e, b, c.swin_heads, (i % 2) ? shift_odd : 0))) {
         View n1 = P.make_view(x.N, x.H, x.W, Ed);
         gn(e, b + ".norm1", n1, 0, -1);
         View qkv = P.make_view(x.N, x.H, x.W, 3 * Ed);
         conv(n1, b + ".attn.qkv", 1, 1, 3 * Ed, &qkv, nullptr, ACT_NONE);
         View a = P.make_view(x.N, x.H, x.W, Ed);
-        attn(qkv, a, b, (i % 2) ? shift_odd : 0);
+        attn(qkv, a, b, win, (i % 2) ? shift_odd : 0);
         conv(a, b + ".attn.proj", 1, 1, Ed, &e, &e, ACT_NONE);              // x = shortcut + attn
       }
       const bool mlp_ok = fuse_mlp && mlp_supported(Ed, hidden, x.H, x.W, x.N);
@@ -1013,7 +1025,7 @@ int run_op_range(rs_plan& P, const Op* first, const Op* last, const float* film_
       case OP_SWIN_ATTN: rc = swin_attn_launch(op.swin, st); break;
       case OP_VQ_ATTN: rc = vq_attn_launch(op.vqa, st); break;
       case OP_ATTN:
-        rc = attn_launch(op.a_in, op.a_out, op.a_bias, P.e->cfg.swin_heads, P.e->cfg.swin_embed_dim, op.a_shift, st);
+        rc = attn_launch(op.a_in, op.a_out, op.a_bias, P.e->cfg.swin_heads, P.e->cfg.swin_embed_dim, op.a_window, op.a_shift, st);
         break;
       case OP_SOFTMAX: {
         const SoftmaxParams sp = softmax_params(op);
@@ -1117,8 +1129,10 @@ const char* rs_last_error(void) { return g_last_error.c_str(); }
 int rs_unet_create_ex(const rs_unet_config* cfg, const rs_unet_options* opts, rs_engine** out) {
   RS_CHECK(cfg && opts && out, "null argument");
   RS_CHECK(cfg->n_levels >= 1 && cfg->n_levels <= RS_MAX_LEVELS, "n_levels");
-  RS_CHECK(cfg->swin_embed_dim == cfg->swin_heads * 32, "head_dim must be 32 (num_head_channels: 32 in every shipped yaml)");
-  RS_CHECK(cfg->window_size == 8, "window_size must be 8: the window-attention kernels are specialised for 8x8 windows");
+  RS_CHECK(cfg->swin_heads > 0 && (cfg->swin_embed_dim == cfg->swin_heads * 32 || cfg->swin_embed_dim == cfg->swin_heads * 64),
+           "head_dim (swin_embed_dim / heads) must be 32 or 64: the window-attention kernels are instantiated for those");
+  RS_CHECK(cfg->window_size == 8 || cfg->window_size == 16,
+           "window_size must be 8 or 16: the window-attention kernels are instantiated for 8x8 and 16x16 windows");
   RS_CHECK(cfg->model_channels % 32 == 0 && cfg->swin_embed_dim % 32 == 0, "GroupNorm32 needs channels % 32 == 0");
   RS_CHECK(cfg->lq_size >= cfg->image_size, "lq_size < image_size is not covered");
   for (int v : {opts->use_scale_shift_norm, opts->resblock_updown, opts->conv_resample, opts->patch_norm})
@@ -1176,9 +1190,10 @@ int rs_unet_load_param(rs_engine* e, const char* name, const float* src, void* s
     (void)launch_k(pack_conv_weight_kernel, dim3((unsigned)std::min<long long>((total + 255) / 256, 4096)), dim3(256), (size_t)(0), st, 
         src, reinterpret_cast<__half*>(e->arena + p->off), O, I, KH, KW, p->ipad);
   } else if (p->role == R_RELPOS) {
-    RS_CHECK(p->shape[0] == 225, "relative position table must be 15x15 (window 8)");
-    (void)launch_k(expand_relpos_kernel, dim3((e->cfg.swin_heads * 4096 + 255) / 256), dim3(256), (size_t)(0), st,
-        src, reinterpret_cast<float*>(e->arena + p->off), e->cfg.swin_heads);
+    const int w = relpos_window(*p);
+    RS_CHECK(w == 8 || w == 16, "relative position table must be 15x15 (window 8) or 31x31 (window 16)");
+    (void)launch_k(expand_relpos_kernel, dim3((e->cfg.swin_heads * w * w * w * w + 255) / 256), dim3(256), (size_t)(0), st,
+        src, reinterpret_cast<float*>(e->arena + p->off), e->cfg.swin_heads, w);
   } else {
     long long n = 1;
     for (int v : p->shape) n *= v;
@@ -1207,9 +1222,16 @@ int rs_unet_load_param(rs_engine* e, const char* name, const float* src, void* s
 int rs_plan_create(rs_engine* e, int batch, int height, int width, rs_plan** out) {
   RS_CHECK(e && out && batch > 0, "bad argument");
   RS_CHECK(e->kind == 0, "this engine is a VQ-GAN first stage: use rs_vq_plan_create");
-  const int down = 1 << (e->cfg.n_levels - 1);
-  RS_CHECK(height % (8 * down) == 0 && width % (8 * down) == 0,
-           "latent H and W must be multiples of window_size * 2^(levels-1) (64 for the shipped configs)");
+  // every level's H and W must be multiples of that level's window (the constructor-time rule: the level's nominal
+  // resolution where that is not larger than window_size, else window_size)
+  int mult = 1;
+  for (int l = 0; l < e->cfg.n_levels; ++l) {
+    const int res = e->cfg.image_size >> l;
+    mult = std::lcm(mult, (res <= e->cfg.window_size ? res : e->cfg.window_size) << l);
+  }
+  RS_CHECK(height % mult == 0 && width % mult == 0,
+           "latent H and W must be multiples of " + std::to_string(mult) + " for this model: each level's window (at most "
+           "window_size) times the level's downsampling (64 for the shipped configs)");
   auto p = std::make_unique<rs_plan>();
   p->e = e; p->B = batch; p->H = height; p->W = width;
   int rc = build_plan(*p); if (rc) return rc;
@@ -1331,7 +1353,7 @@ static void collect_profile(const rs_plan& P, const Prof& prof, double* ms, char
     } else if (op.kind == OP_MLP) {
       snprintf(d, desc_stride, "mlp %dx%d E=%d Hd=%d grid=%d", op.mlp.in.H, op.mlp.in.W, op.mlp.E, op.mlp.Hd, op.mlp.grid);
     } else if (op.kind == OP_ATTN) {
-      snprintf(d, desc_stride, "attn %dx%d shift=%d", op.a_in.H, op.a_in.W, op.a_shift);
+      snprintf(d, desc_stride, "attn %dx%d window=%d shift=%d", op.a_in.H, op.a_in.W, op.a_window, op.a_shift);
     } else if (op.kind == OP_SWIN_ATTN) {
       snprintf(d, desc_stride, "swin_attn %dx%d shift=%d grid=%d", op.swin.x.H, op.swin.x.W, op.swin.shift, op.swin.grid);
     } else if (op.kind == OP_SOFTMAX) {

@@ -504,7 +504,10 @@ inline int conv_init() {
       for (int ms = 1; ms <= 2; ++ms)
         if (ConvKernelFn k = conv_kernel_for(bn, ms))
           RS_CUDA_OK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    RS_CUDA_OK(cudaFuncSetAttribute(window_attn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));
+    RS_CUDA_OK(cudaFuncSetAttribute(window_attn_kernel<8, 32>, cudaFuncAttributeMaxDynamicSharedMemorySize, kAttnMaxSmem));
+    RS_CUDA_OK(cudaFuncSetAttribute(window_attn_kernel<8, 64>, cudaFuncAttributeMaxDynamicSharedMemorySize, kAttnMaxSmem));
+    RS_CUDA_OK(cudaFuncSetAttribute(window_attn_kernel<16, 32>, cudaFuncAttributeMaxDynamicSharedMemorySize, kAttnMaxSmem));
+    RS_CUDA_OK(cudaFuncSetAttribute(window_attn_kernel<16, 64>, cudaFuncAttributeMaxDynamicSharedMemorySize, kAttnMaxSmem));
     RS_CUDA_OK(cudaFuncSetAttribute(mlp_fused_sm90_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     RS_CUDA_OK(cudaFuncSetAttribute(mlp_fused_sm90_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     RS_CUDA_OK(cudaFuncSetAttribute(mlp_fused_sm90_kernel<192>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
@@ -717,14 +720,15 @@ struct SwinAttnDesc {
   GnFinalizeParams fin[2] = {};
   int grid = 0;
 };
-inline bool swin_attn_supported(int E, int heads, int H, int W) {
-  return (E == 192 || E == 64) && heads * 32 == E && H % 8 == 0 && W % 8 == 0;
+// (8x8 windows and 32-wide heads only: every other level takes the four-launch form around window_attn_kernel)
+inline bool swin_attn_supported(int E, int heads, int H, int W, int window) {
+  return window == 8 && (E == 192 || E == 64) && heads * 32 == E && H % 8 == 0 && W % 8 == 0;
 }
 inline int swin_attn_finalize(SwinAttnDesc& d) {
   SwinAttnParams& p = d.prm;
   std::memset(&p, 0, sizeof(p));
   const int E = d.x.C;
-  RS_CHECK(swin_attn_supported(E, d.heads, d.x.H, d.x.W), "fused Swin attention: E in {64, 192}, head_dim 32, H and W multiples of 8");
+  RS_CHECK(swin_attn_supported(E, d.heads, d.x.H, d.x.W, 8), "fused Swin attention: E in {64, 192}, head_dim 32, H and W multiples of 8");
   RS_CHECK(d.y.C == E && d.y.H == d.x.H && d.y.W == d.x.W && d.y.N == d.x.N, "fused Swin attention: output geometry");
   RS_CHECK(d.x.ld % 8 == 0 && d.y.ld % 8 == 0 && d.wqkv_ld % 8 == 0 && d.wproj_ld % 8 == 0, "fused Swin attention: 16-byte rows");
   RS_CHECK((d.gn_part && d.gn_slots > 0) || d.gn_gstat, "fused Swin attention: norm1 statistics");
@@ -827,27 +831,44 @@ inline int vq_attn_launch(const VqAttnDesc& d, cudaStream_t st) {
   return 0;
 }
 
-inline size_t attn_smem_bytes(int E) {
-  return (size_t)2 * 3 * 64 * kAttnPad * 2 + (size_t)64 * (E + 8) * 2 + 64 * sizeof(int);
-}
-
-inline int attn_launch(const View& qkv, const View& out, const float* bias, int heads, int E, int shift,
-                       cudaStream_t st) {
-  RS_CHECK(qkv.H % 8 == 0 && qkv.W % 8 == 0, "window attention needs H, W multiples of 8");
-  RS_CHECK(E == heads * 32 && E % 8 == 0, "window attention kernel is specialised for head_dim 32");
-  const int windows = qkv.N * (qkv.H / 8) * (qkv.W / 8);
+// one launch of the window-attention core: the instance of window_attn_kernel for (window side, head width), or the
+// SIMT cross-check under RS_ATTN_IMPL=simt
+template <int WS, int HD>
+inline int attn_launch_instance(WinAttnParams& p, int windows, cudaStream_t st) {
   // heads per CTA: all of them when there are plenty of windows, fewer (more CTAs) otherwise
+  const int heads = p.heads;
   int hpc = heads;
   while (hpc > 1 && (long long)windows * (heads / hpc) < 4 * num_sms() && hpc % 2 == 0) hpc /= 2;
   if (hpc > 1 && (long long)windows * (heads / hpc) < 4 * num_sms() && heads % hpc == 0) hpc = 1;
-  WinAttnParams p{qkv.ptr, qkv.ld, out.ptr, out.ld, bias, qkv.N, qkv.H, qkv.W, heads, E, shift, 0.17677669529663687f, hpc};
+  p.hpc = hpc;
+  // (at WS = 8 sized for the output channels of all heads: an upper bound of what hpc heads stage)
+  const size_t smem = window_attn_smem_bytes<WS, HD>(WS == 8 ? heads : hpc);
+  RS_CHECK(smem <= (size_t)kAttnMaxSmem, "attention tile does not fit in shared memory");   // limit raised in conv_init()
+  (void)launch_k(window_attn_kernel<WS, HD>, dim3(windows, heads / hpc), dim3(WS == 8 ? 128 : 256), smem, st, p);
+  return 0;
+}
+
+inline int attn_launch(const View& qkv, const View& out, const float* bias, int heads, int E, int window, int shift,
+                       cudaStream_t st) {
+  RS_CHECK(window == 8 || window == 16, "window attention kernels: window_size 8 or 16, got " + std::to_string(window));
+  RS_CHECK(heads > 0 && E % heads == 0 && (E / heads == 32 || E / heads == 64),
+           "window attention kernels: head_dim 32 or 64");
+  RS_CHECK(qkv.H % window == 0 && qkv.W % window == 0,
+           "window attention needs H, W multiples of the window (" + std::to_string(window) + ")");
+  RS_CHECK(shift == 0 || shift == window / 2, "window attention: shift is 0 or half the window");
+  const int hd = E / heads;
+  const int windows = qkv.N * (qkv.H / window) * (qkv.W / window);
+  WinAttnParams p{qkv.ptr, qkv.ld, out.ptr, out.ld, bias, qkv.N, qkv.H, qkv.W, heads, E, shift,
+                  hd == 32 ? 0.17677669529663687f : 0.125f, heads, window, hd};
+  int rc = 0;
   if (env_is("RS_ATTN_IMPL", "simt")) {
-    (void)launch_k(window_attn_simt_kernel, dim3(windows, heads), dim3(64), (size_t)0, st, p);
+    (void)launch_k(window_attn_simt_kernel, dim3(windows, heads), dim3(window * window), (size_t)0, st, p);
+  } else if (window == 8) {
+    rc = hd == 32 ? attn_launch_instance<8, 32>(p, windows, st) : attn_launch_instance<8, 64>(p, windows, st);
   } else {
-    const size_t smem = attn_smem_bytes(E);
-    RS_CHECK(smem <= 160 * 1024, "attention tile does not fit in shared memory");   // limit raised in conv_init()
-    (void)launch_k(window_attn_kernel, dim3(windows, heads / hpc), dim3(128), smem, st, p);
+    rc = hd == 32 ? attn_launch_instance<16, 32>(p, windows, st) : attn_launch_instance<16, 64>(p, windows, st);
   }
+  if (rc) return rc;
   RS_CUDA_OK(cudaGetLastError());
   return 0;
 }

@@ -15,7 +15,7 @@ import torch
 import torch.nn as nn
 
 from .. import _lib
-from ..arch import unet_param_spec, relative_position_index, shifted_window_mask
+from ..arch import latent_multiple, unet_param_spec, relative_position_index, shifted_window_mask
 from ..config import UNetConfig
 from ..weights import random_state_dict
 
@@ -119,6 +119,11 @@ class UNetModelSwin(nn.Module):
         self._packed_versions = versions
 
     def plan(self, batch: int, height: int, width: int) -> "_Plan":
+        mult = latent_multiple(self.cfg)
+        if height % mult or width % mult:
+            raise ValueError(f"latent {height}x{width}: H and W must be multiples of {mult} for this model (each level's "
+                             f"window, at most window_size={self.cfg.window_size}, times the level's downsampling); "
+                             f"ResShiftSampler pads to multiples of padding_offset, which must be a multiple of {mult}")
         device = next(self.parameters()).device
         self._ensure_engine(device)
         self.pack_weights()
