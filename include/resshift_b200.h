@@ -253,6 +253,32 @@ int rs_op_conv2d_splitk(const void* x, int N, int H, int W, int C, int ld, const
                         int Cout, int ksize, int stride, const void* residual, int res_ld, void* out, int out_ld, int act,
                         float* part, int cstride, int coff, float* scratch, int32_t* splits_out, float* gstat, void* counter,
                         void* stream);
+/* Every option of the conv launcher.  The three entries above are rs_op_conv2d_ex with some fields left at their
+ * neutral values (NULL / 0, pad_lo = 1). */
+typedef struct rs_conv_args {
+  const void* x; int32_t N, H, W, C, ld;        /* NHWC fp16 input view, row stride ld                              */
+  const void* w_packed; int32_t ipad;           /* fp16 [Cout][k*k][ipad] from rs_op_pack_conv_weight                */
+  const float* bias; int32_t bias_sN;           /* [Cout] fp32 or NULL; bias_sN > 0: one row per image at
+                                                   bias + n * bias_sN (tiles of at most 8 images, one sub-tile)       */
+  int32_t cout, ksize, stride;
+  int32_t pad_lo;                               /* stride 2 only: 1 = padding 1 on every side, 0 = pad (0, 1, 0, 1)  */
+  const void* residual; int32_t res_ld;         /* optional fp16 view on the output grid                             */
+  void* out; int32_t out_ld;                    /* fp16 output view, or NULL with out_f32_nchw                       */
+  float* out_f32_nchw;                          /* optional fp32 NCHW output [N, Cout, Ho, Wo]                       */
+  int32_t act;                                  /* 0 none, 1 GELU(erf), 2 SiLU                                       */
+  int32_t bn;                                   /* channel-tile width; 0 lets the library choose                     */
+  int32_t msub;                                 /* 128-pixel sub-tiles per CTA: 0 lets the library choose (RS_CONV_MSUB=2
+                                                   asks for two where the layer can take them); 1 or 2 is required   */
+  float* part[2];                               /* GroupNorm statistics sinks part[i][N][slots][cstride[i]][2] or NULL */
+  int32_t cstride[2], coff[2];
+  float* gstat;                                 /* optional [N][32][2] group (mean, rstd) of all channels of sink 0  */
+  float* splitk_scratch;                        /* non-NULL allows split-K: 8 * N * Ho * Wo * Cout floats            */
+} rs_conv_args;
+/* info[12] (optional) = the configuration launched: grid, BN, msub, stages, CTAs per tile group, split-K factor,
+ * persistent (0 / 1), staging block width of the TMA epilogue (0: direct epilogue), pixel box bw / bh / bn, statistics
+ * slots per image.  A configuration that cannot be launched as required (bn without a compiled instance, msub = 2 with a
+ * bn that has no two-sub-tile instance, or on a layer that cannot take two sub-tiles) returns an error. */
+int rs_op_conv2d_ex(const rs_conv_args* a, int32_t* info, void* stream);
 /* profiling aid: `iters` launches of the same conv; per-CTA timeline of the last one in dbg (8 x u64 per CTA);
  * info[7] = grid, BN, stages, shared memory bytes, CTAs per tile group, split-K factor, persistent kernel (0 / 1) */
 int rs_op_conv2d_timeline(const void* x, int N, int H, int W, int C, int ld, const void* w_packed, int Ipad, const float* bias,
@@ -315,6 +341,14 @@ int rs_op_swin_attn(const void* x, int N, int H, int W, int E, int heads, int sh
 int rs_op_mlp(const void* x, int N, int H, int W, int E, int Hd, const void* w1_packed, const float* b1,
               const void* w2_packed, const float* b2, const void* residual, void* out, void* dbg_timeline_or_null,
               void* stream);
+/* the same with the block's norm2 fused in front (x is then the un-normalised tensor, Hd >= 4 E): its group statistics
+ * either as gn_gstat[N][32][2] = (mean, rstd), or as the producers' (mean, M2) pairs gn_part[N][gn_slots][E][2]
+ * (gn_gstat NULL), with gn_gamma / gn_beta [E]; all four NULL: no input norm.  part[i] (optional): (mean, M2) pairs of
+ * out, part[i][N][slots][cstride[i]][2] at channel offset coff[i]; *slots_out = slots per image. */
+int rs_op_mlp_ex(const void* x, int N, int H, int W, int E, int Hd, const void* w1_packed, const float* b1,
+                 const void* w2_packed, const float* b2, const void* residual, void* out, const float* gn_gstat,
+                 const float* gn_part, int gn_slots, const float* gn_gamma, const float* gn_beta, float* const part[2],
+                 const int32_t cstride[2], const int32_t coff[2], int32_t* slots_out, void* stream);
 /* host-only: tile configuration the conv launcher picks: out[8] = BN, msub, stages, CTAs/SM, estimated cycles,
    CTAs per tile group (1 or 2), split-K factor, persistent kernel (0 / 1) */
 int rs_debug_tile_config(int m_tiles, int cout, int num_kblocks, int32_t* out);

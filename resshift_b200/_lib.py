@@ -46,6 +46,19 @@ class VQConfigC(C.Structure):
     ]
 
 
+class ConvArgsC(C.Structure):
+    """Mirror of ``rs_conv_args``."""
+    _fields_ = [
+        ("x", C.c_void_p), ("N", C.c_int32), ("H", C.c_int32), ("W", C.c_int32), ("C", C.c_int32), ("ld", C.c_int32),
+        ("w_packed", C.c_void_p), ("ipad", C.c_int32), ("bias", C.c_void_p), ("bias_sN", C.c_int32),
+        ("cout", C.c_int32), ("ksize", C.c_int32), ("stride", C.c_int32), ("pad_lo", C.c_int32),
+        ("residual", C.c_void_p), ("res_ld", C.c_int32), ("out", C.c_void_p), ("out_ld", C.c_int32),
+        ("out_f32_nchw", C.c_void_p), ("act", C.c_int32), ("bn", C.c_int32), ("msub", C.c_int32),
+        ("part", C.c_void_p * 2), ("cstride", C.c_int32 * 2), ("coff", C.c_int32 * 2),
+        ("gstat", C.c_void_p), ("splitk_scratch", C.c_void_p),
+    ]
+
+
 # every symbol include/resshift_b200.h declares: (restype, argtypes)
 _P = C.c_void_p
 _SIGNATURES = {
@@ -85,6 +98,7 @@ _SIGNATURES = {
     "rs_op_conv2d_splitk": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, C.c_int, _P, C.c_int, C.c_int,
                                       C.c_int, _P, C.c_int, _P, C.c_int, C.c_int, _P, C.c_int, C.c_int, _P,
                                       C.POINTER(C.c_int32), _P, _P, _P]),
+    "rs_op_conv2d_ex": (C.c_int, [C.POINTER(ConvArgsC), C.POINTER(C.c_int32), _P]),
     "rs_op_conv2d_timeline": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, C.c_int, _P, C.c_int, C.c_int,
                                         C.c_int, _P, C.c_int, C.c_int, C.c_int, _P, C.POINTER(C.c_int32), _P, _P]),
     "rs_op_groupnorm": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P, _P, C.c_longlong, C.c_int,
@@ -105,6 +119,8 @@ _SIGNATURES = {
     "rs_op_swin_attn": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, C.c_int, _P, _P, _P, _P, _P, _P, _P,
                                   _P, _P, _P, _P, _P]),
     "rs_op_mlp": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P, _P, _P, _P, _P, _P, _P]),
+    "rs_op_mlp_ex": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P, _P, _P, _P, _P, _P, _P, C.c_int, _P, _P,
+                               C.POINTER(_P), C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(C.c_int32), _P]),
     "rs_debug_tile_config": (C.c_int, [C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int32)]),
     "rs_op_upsample2x": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P]),
     "rs_vq_create": (C.c_int, [C.POINTER(VQConfigC), C.POINTER(_P)]),

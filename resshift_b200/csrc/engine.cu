@@ -1345,9 +1345,11 @@ static void collect_profile(const rs_plan& P, const Prof& prof, double* ms, char
     char* d = desc + (size_t)i * desc_stride;
     if (op.kind == OP_CONV) {
       const ConvParams& c = op.conv.prm;
-      snprintf(d, desc_stride, "conv%dx%d s%d %dx%d Cin=%d Cout=%d grid=%d BN=%d st=%d %s cg=%d ms=%d sk=%d box=%dx%dx%d",
+      snprintf(d, desc_stride, "conv%dx%d s%d %dx%d Cin=%d Cout=%d grid=%d BN=%d st=%d %s cg=%d ms=%d sk=%d box=%dx%dx%d "
+               "N=%d persist=%d pad=%d act=%d res=%d f32=%d",
                op.conv.ksize, op.conv.ksize, op.conv.stride, c.Hout, c.Wout, op.conv.in.C, c.Cout, op.conv.grid, c.BN, c.stages,
-               op.w_name.c_str(), c.cg, c.msub, c.splitk, c.bw, c.bh, c.bn);
+               op.w_name.c_str(), c.cg, c.msub, c.splitk, c.bw, c.bh, c.bn, c.Nimg, c.persist, op.conv.pad_lo, op.conv.act,
+               (int)op.conv.has_res, (int)(op.conv.out_f32 != nullptr));
     } else if (op.kind == OP_GN) {
       snprintf(d, desc_stride, "gn %dx%d C=%d fused=%d %s", op.gn.in.H, op.gn.in.W, op.gn.in.C, (int)op.gn.fused, op.g_name.c_str());
     } else if (op.kind == OP_MLP) {

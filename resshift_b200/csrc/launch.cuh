@@ -176,6 +176,7 @@ struct ConvDesc {
   float* out_f32 = nullptr;
   int act = ACT_NONE;
   int bn_override = 0;
+  int msub_request = 0;           // sub-tiles per CTA asked for (0: RS_CONV_MSUB, else the cost model)
   unsigned long long* dbg = nullptr;
   float* partial = nullptr;       // split-K scratch [S][pixels][Cout] fp32 (caller-provided when the plan chose S > 1)
   bool allow_split = false;
@@ -199,8 +200,8 @@ struct TileConfig { int BN = 0, msub = 1, stages = 2, occ = 1, cg = 1, splitk = 
 // multicast).  Shallow rings are additionally latency-bound (~3000 cycles per load).  The epilogue (~18 cycles per
 // column + set-up) hides under a co-resident CTA; whole waves are counted.
 inline TileConfig pick_tile_config(int m_tiles, int cout16, int num_kb, int f_bn, bool allow_split = false, bool allow_persist = false,
-                                   bool allow_msub2 = true) {
-  const int f_msub = env_int("RS_CONV_MSUB", 0), f_occ = env_int("RS_CONV_OCC", 0), f_stages = env_int("RS_CONV_STAGES", 0);
+                                   bool allow_msub2 = true, int msub_request = 0) {
+  const int f_msub = msub_request ? msub_request : env_int("RS_CONV_MSUB", 0), f_occ = env_int("RS_CONV_OCC", 0), f_stages = env_int("RS_CONV_STAGES", 0);
   const int f_cg = env_int("RS_CONV_CG", 0);
   TileConfig best, bestp;      // best one-tile-per-CTA configuration (ranking model below), best persistent one
   double best_real = 1e30;     // realistic estimate of `best` (see the end of the function)
@@ -208,8 +209,12 @@ inline TileConfig pick_tile_config(int m_tiles, int cout16, int num_kb, int f_bn
     if (f_bn ? (cand != std::min(f_bn, std::min(cout16, 256))) : (cout16 % cand != 0)) continue;
     if (!conv_bn_supported(cand)) continue;
     const int n_tiles = (cout16 + cand - 1) / cand;
+    // msub = 2 only on request (RS_CONV_MSUB=2 or the descriptor), and then wherever the layer can take it (one CTA per
+    // tile, an even tile count, a channel tile with that instance); otherwise one sub-tile
+    const bool ms2_cand = f_msub == 2 && allow_msub2 && m_tiles % 2 == 0 && conv_kernel_for(cand, 2);
     for (int cg = 1; cg <= 2; ++cg) {
       if (f_cg && cg != f_cg && !(f_cg == 2 && m_tiles < 2)) continue;   // a single tile cannot form a pair
+      if (cg == 2 && ms2_cand && f_cg != 2) continue;
       if (cg == 2 && (cand % 16 != 0 || m_tiles < 2)) continue;
       // persistent mode: one CTA (pair) per SM walks ceil(units / workers) tiles; the producer fetches the next tile's
       // operands while the consumers run the epilogue, so a tile costs about max(main loop, epilogue) and set-up / first
@@ -233,8 +238,9 @@ inline TileConfig pick_tile_config(int m_tiles, int cout16, int num_kb, int f_bn
           }
         }
       }
+      const bool ms2 = ms2_cand && cg == 1;
       for (int ms = 1; ms <= 2; ++ms) {
-        if (ms == 2 && (f_msub != 2 || !allow_msub2 || cg == 2 || m_tiles % 2 || !conv_kernel_for(cand, 2))) continue;   // msub = 2 only on request
+        if (ms == 2 ? !ms2 : ms2) continue;
         const int sbytes = ms * kConvBM * kConvBK * 2 + cand * kConvBK * 2;
         for (int occ = 1; occ <= 2; ++occ) {
           if (f_occ && occ != f_occ) continue;
@@ -336,9 +342,9 @@ inline int conv_finalize(ConvDesc& d) {
   const bool can_split = d.allow_split && d.partial != nullptr && contiguous_tiles && p.bn <= 2 && d.has_out && !d.out_f32 && !simt;
   const int want_persist = env_int("RS_CONV_PERSIST", -1);           // 0 / 1 disables / forces the persistent kernel
   const bool persist_ok = d.has_out && !d.out_f32 && want_persist != 0 && !env_is("RS_CONV_EPI", "direct") &&
-                          !env_is("RS_CONV_IMPL", "simt") && env_int("RS_CONV_MSUB", 0) != 2;
+                          !env_is("RS_CONV_IMPL", "simt") && (d.msub_request ? d.msub_request : env_int("RS_CONV_MSUB", 0)) != 2;
   const TileConfig tc = pick_tile_config(m_tiles, cout16, num_kb, d.bn_override ? d.bn_override : env_int("RS_CONV_BN", 0), can_split,
-                                         persist_ok && want_persist != 1, !d.bias_per_image);
+                                         persist_ok && want_persist != 1, !d.bias_per_image, d.msub_request);
   const int BN = tc.BN, msub = tc.msub, stages = tc.stages, cg = tc.cg;
   p.cg = cg;
   p.splitk = tc.splitk; p.partial = d.partial;

@@ -64,19 +64,72 @@ def conv2d(x_nhwc, w, bias, stride=1, residual=None, act=0, out_f32=False, bn=0,
 
 
 def ref_conv(x_nhwc16, w, bias, stride=1, residual=None, act=0):
-    """fp32 torch reference on the fp16-rounded operands."""
-    x = nchw32(x_nhwc16)
-    wq = w.half().float()
+    """float64 torch reference (NCHW) on the fp16-rounded operands: no TF32, no fp32 accumulation error of its own."""
+    x = nchw32(x_nhwc16).double()
+    wq = w.half().double()
     if wq.dim() == 2:
         wq = wq[:, :, None, None]
-    y = F.conv2d(x, wq, bias, stride=stride, padding=wq.shape[-1] // 2)
+    y = F.conv2d(x, wq, None if bias is None else bias.double(), stride=stride, padding=wq.shape[-1] // 2)
     if act == 1:
         y = F.gelu(y)
     elif act == 2:
         y = F.silu(y)
     if residual is not None:
-        y = y + nchw32(residual)
+        y = y + nchw32(residual).double()
     return y
+
+
+def ulp16(v: torch.Tensor) -> torch.Tensor:
+    """Spacing of fp16 numbers at |v| (float64; the subnormal spacing 2^-24 below 2^-14)."""
+    e = torch.floor(torch.log2(v.double().abs().clamp(min=2.0 ** -14)))
+    return torch.exp2(e - 10)
+
+
+def accumulation_ratio(got, ref, mag, fp16=True, slack=None):
+    """max over elements of (|got - ref| - rounding - slack) / mag: the accumulation error relative to the magnitudes that
+    entered each output (rounding = half an fp16 ulp of the stored value, or one fp32 rounding for fp32 outputs)."""
+    err = (got.double() - ref).abs()
+    rnd = 0.5 * ulp16(ref) if fp16 else 2.0 ** -24 * ref.abs()
+    if slack is not None:
+        rnd = rnd + slack
+    return ((err - rnd).clamp(min=0) / mag.clamp(min=1e-30)).max().item()
+
+
+def assert_within(tag, got, ref, mag, kappa, slack=None, fp16=True):
+    """|got - ref| <= 1/2 ulp16(ref) + kappa * mag (+ slack) per element; ulp taken at |ref| + the error allowance so that
+    a value pushed across a power of two may round to the coarser spacing.  NaN fails."""
+    allow = kappa * mag + (0 if slack is None else slack)
+    err = (got.double() - ref).abs()
+    rnd = 0.5 * ulp16(ref.abs() + allow) if fp16 else 2.0 ** -24 * (ref.abs() + allow)
+    bad = ~(err <= rnd + allow)
+    ratio = accumulation_ratio(got, ref, mag, fp16, slack)
+    print(f"[bound] {tag}: max (|d| - rounding) / mag = {ratio:.3e}")
+    assert not bad.any(), f"{tag}: {int(bad.sum())} of {bad.numel()} elements outside the bound (ratio {ratio:.3e})"
+    return ratio
+
+
+def check_slot_pairs(tag, part, out16, bw, bh, slots, cstride, coff):
+    """(mean, M2) pairs part[N][slots][cstride][2] of the stored fp16 output out16 [N, H, W, C] (slot = (bw x bh) box of
+    one image, row-major over the map) at channel offset coff, against float64 statistics of the same values; the bounds
+    of test_gpu_ops.py's combined statistics.  Channels outside [coff, coff + C) must still hold their NaN fill."""
+    N, H, W, Co = out16.shape
+    o = out16.double()
+    t = o.reshape(N, H // bh, bh, W // bw, bw, Co).permute(0, 1, 3, 2, 4, 5).reshape(N, slots, bh * bw, Co)
+    mean = t.mean(dim=2)
+    m2 = ((t - mean[:, :, None]) ** 2).sum(dim=2)
+    p = part[:N * slots * cstride * 2].view(N, slots, cstride, 2)
+    got = p[:, :, coff:coff + Co].double()
+    assert torch.isfinite(got).all(), f"{tag}: missing statistics"
+    rest = torch.cat([p[:, :, :coff], p[:, :, coff + Co:]], dim=2)
+    assert torch.isnan(rest).all(), f"{tag}: statistics written outside the sink's channel slice"
+    assert torch.isnan(part[N * slots * cstride * 2:]).all(), f"{tag}: statistics written beyond the slots"
+    assert (got[..., 0] - mean).abs().max().item() <= 1e-5 * (1 + o.abs().max().item()), tag
+    assert ((got[..., 1] - m2).abs() / (m2 + 1e-6 * bw * bh)).max().item() <= 1e-4, tag
+
+
+def bits(t: torch.Tensor) -> torch.Tensor:
+    """The raw bits of a float tensor (NaN fills compare equal)."""
+    return t.view(torch.int16 if t.element_size() == 2 else torch.int32)
 
 
 def err_stats(got: torch.Tensor, ref: torch.Tensor) -> dict:

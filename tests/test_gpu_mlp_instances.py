@@ -1,0 +1,228 @@
+"""The fused Swin MLP (mlp_fused_sm90_kernel<E>, E in {64, 128, 192, 256}) through rs_op_mlp_ex against float64, and the
+two model-level paths around it (the <256> instance inside a plan, and the unfused fc1 / fc2 fallback of E = 96).
+
+The reference is float64 with the kernel's fp16 roundings: of the (normalised) input X, of the hidden activations
+H = fp16(GELU(X W1^T + b1)), and of the output fp16(res + b2 + H W2^T).  Per element
+|got - ref| <= 1/2 ulp16(ref) + KAPPA * mag2 + slack, with mag2 = |H| |W2|^T + |b2| + |res| and slack = sum_j |W2_ij| e_j
+over the hidden values whose float64 value lies so close to an fp16 rounding boundary (closer than the first GEMM's
+allowance KAPPA * (|X| |W1|^T + |b1|) x 1.13) that the kernel may have rounded it to the neighbour (e_j = that spacing).
+The fused norm2 must be bit-identical to rs_op_groupnorm_apply / _apply_pairs followed by the plain MLP."""
+import ctypes as C
+
+import pytest
+import torch
+import torch.nn.functional as F
+
+pytestmark = pytest.mark.gpu
+
+if torch.cuda.is_available():
+    from tests import gpu_util as G
+    from resshift_b200 import _lib
+
+# the conv tests' allowance (test_gpu_conv_instances.py: 6.6 times the largest ratio observed there).  On an H100 80GB HBM3
+# (700 W) no MLP output exceeded 1/2 ulp16 + slack at all: every deviation from the float64 reference was explained by
+# hidden values rounded to the neighbouring fp16 number, so the slack term dominates this bound
+KAPPA = 2.0 ** -18
+ACT_GAIN = 1.13
+# (N, H, W): 8x8 with an odd batch (two images per 128-pixel tile, the second tile half padding), 16x16, 64x64, 32x64
+MAPS = {"8x8_n3": (3, 8, 8), "16x16_n2": (2, 16, 16), "64x64_n1": (1, 64, 64), "32x64_n2": (2, 32, 64)}
+CASES = [(E, r, m, norm) for E in (64, 128, 192, 256) for r in (4, 2) for m in MAPS
+         for norm in (("none", "gstat", "pairs") if r == 4 else ("none",))]
+
+
+def _box(H, W):
+    def p2(x, cap):
+        p = 1
+        while p * 2 <= cap and x % (p * 2) == 0:
+            p *= 2
+        return p
+    bw = p2(W, 128)
+    bh = p2(H, 128 // bw)
+    return bw, bh, (W // bw) * (H // bh)
+
+
+def _mlp(x, res, w1p, b1, w2p, b2, E, Hd, gstat=None, part=None, slots=0, gamma=None, beta=None, sinks=()):
+    N, H, W, _ = x.shape
+    out = torch.full_like(x, float("nan"))
+    parts = (C.c_void_p * 2)(*[s[0].data_ptr() for s in sinks] + [None] * (2 - len(sinks)))
+    cst = (C.c_int32 * 2)(*[s[1] for s in sinks] + [0] * (2 - len(sinks)))
+    cof = (C.c_int32 * 2)(*[s[2] for s in sinks] + [0] * (2 - len(sinks)))
+    slots_out = C.c_int32()
+    _lib.check(_lib.lib.rs_op_mlp_ex(x.data_ptr(), N, H, W, E, Hd, w1p.data_ptr(), b1.data_ptr(), w2p.data_ptr(), b2.data_ptr(),
+                                     _lib.ptr(res), out.data_ptr(), _lib.ptr(gstat), _lib.ptr(part), slots, _lib.ptr(gamma),
+                                     _lib.ptr(beta), parts, cst, cof, C.byref(slots_out), G.stream()))
+    torch.cuda.synchronize()
+    return out, slots_out.value
+
+
+def _group_stats(x, N):
+    """float64 per-(image, group) mean and rstd of fp16 x [N, H, W, E] (GroupNorm32, eps 1e-5)."""
+    xg = x.double().reshape(N, -1, 32, x.shape[-1] // 32).permute(0, 2, 1, 3).reshape(N, 32, -1)
+    mean = xg.mean(dim=2)
+    return mean, (xg.var(dim=2, unbiased=False) + 1e-5).rsqrt()
+
+
+def _slot_pairs(x, bw, bh, slots):
+    """(mean, M2) pairs [N][slots][E][2] of x per tile slot, what a producing kernel delivers."""
+    N, H, W, E = x.shape
+    t = x.float().reshape(N, H // bh, bh, W // bw, bw, E).permute(0, 1, 3, 2, 4, 5).reshape(N, slots, bh * bw, E)
+    m = t.mean(dim=2)
+    return torch.stack([m, ((t - m[:, :, None]) ** 2).sum(dim=2)], dim=-1).contiguous()
+
+
+def _reference(xin, res, w1, b1, w2, b2):
+    """float64 output, mag2 and slack (module docstring) of the MLP on the fp16 input xin [M, E]."""
+    x = xin.double()
+    w1q, w2q = w1.half().double(), w2.half().double()
+    pre = x @ w1q.T + b1.double()
+    dh = KAPPA * ACT_GAIN * (x.abs() @ w1q.abs().T + b1.double().abs()) + 2.0 ** -21 * pre.abs()
+    h64 = F.gelu(pre)
+    h16 = h64.half()
+    hc = h16.cpu()                                          # (fp16 nextafter on the CPU)
+    inf = torch.full_like(hc, float("inf"))
+    up, dn = (torch.nextafter(hc, s * inf).to(h16.device).double() for s in (1, -1))
+    hq = h16.double()
+    near = (h64 + dh >= 0.5 * (hq + up)) | (h64 - dh <= 0.5 * (hq + dn))
+    e = torch.where(near, torch.maximum(up - hq, hq - dn), torch.zeros_like(hq))
+    out = hq @ w2q.T + b2.double() + res.double()
+    mag = hq.abs() @ w2q.abs().T + b2.double().abs() + res.double().abs()
+    return out, mag, e @ w2q.abs().T
+
+
+@pytest.mark.parametrize("E,ratio,map_,norm", CASES, ids=[f"E{e}-Hd{r}E-{m}-{n}" for e, r, m, n in CASES])
+def test_fused_mlp(E, ratio, map_, norm):
+    """Output against float64, output statistics sinks per slot, two launches bit-identical; with the fused norm2,
+    bit-identical to the separate GroupNorm apply followed by the plain MLP."""
+    N, H, W = MAPS[map_]
+    Hd = ratio * E
+    seed = E * 7 + ratio * 3 + H + W + len(norm)
+    g = torch.Generator(device="cuda").manual_seed(seed)
+    x = (torch.randn(N, H, W, E, device="cuda", generator=g) * 1.5 + 0.3).half()
+    res = torch.randn(N, H, W, E, device="cuda", generator=g).half()
+    w1 = torch.randn(Hd, E, device="cuda", generator=g) / E ** 0.5
+    b1 = torch.randn(Hd, device="cuda", generator=g) * 0.5
+    w2 = torch.randn(E, Hd, device="cuda", generator=g) / Hd ** 0.5
+    b2 = torch.randn(E, device="cuda", generator=g) * 0.5
+    gamma = 1 + 0.2 * torch.randn(E, device="cuda", generator=g)
+    beta = 0.2 * torch.randn(E, device="cuda", generator=g)
+    w1p, _ = G.pack_weight(w1)
+    w2p, _ = G.pack_weight(w2)
+    bw, bh, slots = _box(H, W)
+    n_sinks = CASES.index((E, ratio, map_, norm)) % 3
+    norm_args, xin = {}, x
+    if norm != "none":
+        mean, rstd = _group_stats(x, N)
+        if norm == "gstat":
+            gst = torch.stack([mean, rstd], dim=-1).float().contiguous()
+            norm_args = dict(gstat=gst, gamma=gamma, beta=beta)
+            xin = torch.empty_like(x)
+            _lib.check(_lib.lib.rs_op_groupnorm_apply(x.data_ptr(), N, H, W, E, E, gamma.data_ptr(), beta.data_ptr(), None, 0, 0,
+                                                      xin.data_ptr(), E, gst.data_ptr(), G.stream()))
+        else:
+            pairs = _slot_pairs(x, bw, bh, slots)
+            norm_args = dict(part=pairs, slots=slots, gamma=gamma, beta=beta)
+            xin = torch.empty_like(x)
+            _lib.check(_lib.lib.rs_op_groupnorm_apply_pairs(x.data_ptr(), N, H, W, E, E, gamma.data_ptr(), beta.data_ptr(), None, 0,
+                                                            0, xin.data_ptr(), E, pairs.data_ptr(), slots, G.stream()))
+        torch.cuda.synchronize()
+        # the separate normalisation itself, against float64 GroupNorm32 (fp32 arithmetic, one fp16 rounding)
+        xn = (x.double().reshape(N, -1, 32, E // 32) - mean[:, None, :, None]) * rstd[:, None, :, None]
+        xn = xn.reshape(N, H, W, E) * gamma.double() + beta.double()
+        mag = (x.double().reshape(N, -1, 32, E // 32) * rstd[:, None, :, None]).reshape(N, H, W, E).abs() * gamma.double().abs()
+        G.assert_within(f"norm2 {norm}", xin, xn, mag + xn.abs(), 2.0 ** -16)
+
+    def sinks():
+        return [(torch.full((N * slots * (E + 32 * i + 8) * 2 + 64,), float("nan"), device="cuda"), E + 32 * i + 8, 8 * i)
+                for i in range(n_sinks)]
+    runs = []
+    for _ in range(2):
+        sk = sinks()
+        out, nslots = _mlp(x, res, w1p, b1, w2p, b2, E, Hd, sinks=sk, **norm_args)
+        runs.append((out, sk))
+    assert nslots == slots
+    (out, sk), (out2, sk2) = runs
+    assert torch.equal(G.bits(out), G.bits(out2))
+    assert all(torch.equal(G.bits(a[0]), G.bits(b[0])) for a, b in zip(sk, sk2))
+    if norm != "none":
+        sep_sinks = sinks()
+        sep, _ = _mlp(xin, res, w1p, b1, w2p, b2, E, Hd, sinks=sep_sinks)
+        assert torch.equal(G.bits(out), G.bits(sep)), "fused norm2 differs from GroupNorm apply + MLP"
+        assert all(torch.equal(G.bits(a[0]), G.bits(b[0])) for a, b in zip(sk, sep_sinks))
+    ref, mag, slack = _reference(xin.reshape(-1, E), res.reshape(-1, E), w1, b1, w2, b2)
+    G.assert_within(f"mlp E={E} Hd={Hd} {map_} {norm}", out.reshape(-1, E), ref, mag, KAPPA, slack=slack)
+    for i, (part, cstride, coff) in enumerate(sk):
+        G.check_slot_pairs(f"mlp sink {i}", part, out, bw, bh, slots, cstride, coff)
+
+
+def test_refusals():
+    """Widths without an instance, hidden sizes that are not whole 64-column chunks, and the fused norm2 with Hd < 4E
+    (its scratch lives in the bias table) are refused."""
+    g = torch.Generator(device="cuda").manual_seed(1)
+
+    def attempt(E, Hd, norm=False):
+        x = torch.randn(2, 16, 16, E, device="cuda", generator=g).half()
+        w1p, _ = G.pack_weight(torch.randn(Hd, E, device="cuda", generator=g))
+        w2p, _ = G.pack_weight(torch.randn(E, Hd, device="cuda", generator=g))
+        b1, b2 = torch.zeros(Hd, device="cuda"), torch.zeros(E, device="cuda")
+        kw = {}
+        if norm:
+            kw = dict(gstat=torch.zeros(2, 32, 2, device="cuda"), gamma=torch.ones(E, device="cuda"), beta=torch.zeros(E, device="cuda"))
+        with pytest.raises(_lib.RsError, match="fused MLP"):
+            _mlp(x, None, w1p, b1, w2p, b2, E, Hd, **kw)
+    attempt(96, 384)
+    attempt(64, 4 * 64 + 32)
+    attempt(128, 256, norm=True)
+    attempt(192, 384, norm=True)
+
+
+# ---------------------------------------------------------------------------------------------- model level
+
+def _unet_vs_oracle(ucfg, expect_mlp_e):
+    from oracle import unet_variants_oracle as uo
+    from resshift_b200.models.unet import UNetModelSwin
+    from resshift_b200.weights import random_state_dict
+    sd = random_state_dict(ucfg, 0)
+    m = UNetModelSwin(**ucfg.to_kwargs())
+    m.load_state_dict(sd, strict=True)
+    m = m.cuda().eval()
+    g = torch.Generator().manual_seed(4)
+    x = torch.randn(2, ucfg.in_channels, 64, 64, generator=g)
+    lq = torch.rand(2, 3, 64, 64, generator=g) * 2 - 1
+    t = torch.tensor([0, 3])
+    out = m(x.cuda(), t.cuda(), lq=lq.cuda())
+    ref = uo.unet_forward(sd, ucfg, x, t, lq=lq)            # fp32 on the CPU
+    d = (out.float().cpu() - ref).abs()
+    print(f"[unet] swin_embed_dim={ucfg.swin_embed_dim} mlp_ratio={ucfg.mlp_ratio}: max|d|={d.max():.3e} mean|d|={d.mean():.3e}")
+    assert not torch.isnan(out).any()
+    assert d.max().item() <= 1e-2 and d.mean().item() <= 2.5e-3          # test_gpu_unet_variants.py's forward bounds
+    plan = m.plan(2, 64, 64)
+    cap, stride = 2048, 256
+    ms = (C.c_double * cap)()
+    desc = C.create_string_buffer(cap * stride)
+    n = C.c_int32()
+    xc, tc, lqc = x.cuda(), t.float().cuda(), lq.cuda()
+    _lib.check(_lib.lib.rs_plan_profile_ops(plan.handle, xc.data_ptr(), tc.data_ptr(), lqc.data_ptr(), None, ms, desc, stride, cap,
+                                            C.byref(n), _lib.current_stream()))
+    rows = [desc.raw[i * stride:(i + 1) * stride].split(b"\0")[0].decode() for i in range(n.value)]
+    mlps = [r for r in rows if r.startswith("mlp")]
+    if expect_mlp_e:
+        assert mlps and all(f"E={expect_mlp_e} " in r for r in mlps), mlps
+    else:
+        assert mlps == [], mlps
+
+
+def test_unet_swin_embed_256_runs_the_256_instance():
+    """A tiny-width UNetModelSwin with swin_embed_dim = 256: the only way a plan reaches mlp_fused_sm90_kernel<256>."""
+    import dataclasses
+    from resshift_b200.config import preset
+    ucfg, _ = preset("tiny")
+    _unet_vs_oracle(dataclasses.replace(ucfg, swin_embed_dim=256), 256)
+
+
+def test_unet_reference_default_swin_width_takes_the_unfused_mlp():
+    """The reference constructor's own defaults, swin_embed_dim = 96 and mlp_ratio = 2.0 (hidden 192): no fused MLP
+    instance, the fc1 / fc2 convs instead."""
+    import dataclasses
+    from resshift_b200.config import preset
+    ucfg, _ = preset("tiny")
+    _unet_vs_oracle(dataclasses.replace(ucfg, swin_embed_dim=96, mlp_ratio=2.0), None)
