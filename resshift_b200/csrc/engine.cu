@@ -12,7 +12,9 @@
 #include <map>
 #include <memory>
 #include <numeric>
+#include <optional>
 #include <string>
+#include <variant>
 #include <vector>
 
 #include "../../include/resshift_b200.h"
@@ -42,8 +44,24 @@ struct Param {
 
 using namespace rs;
 
+namespace {
+enum class EngineKind { Denoiser, VqGan, Kl };   // the denoiser or a first stage around it (vq.inc)
+enum class Pass { Denoiser, Encode, Decode };    // a plan's program: the denoiser's forward, a first stage's encoder / decoder
+const char* kind_name(EngineKind k) {
+  switch (k) {
+    case EngineKind::Denoiser: return "a UNetModelSwin denoiser";
+    case EngineKind::VqGan: return "a VQ-GAN first stage";
+    case EngineKind::Kl: return "a KL first stage";
+  }
+  return "an engine of unknown kind";
+}
+// launches a bound plan makes outside its op list: the denoiser's timestep embedding (4) and input packing (1-2); a first
+// stage's counter reset, input packing or quantiser, and output copy
+constexpr int kDenoiserOuterLaunches = 6, kEncodeOuterLaunches = 3, kDecodeOuterLaunches = 3;
+}  // namespace
+
 struct rs_engine {
-  int kind = 0;                 // 0: UNetModelSwin denoiser, 1: VQ-GAN first stage (vq.inc); the parameter store is shared
+  EngineKind kind = EngineKind::Denoiser;   // the parameter store is shared by all kinds
   rs_vq_config vq{};
   rs_unet_config cfg;
   rs_unet_options opt{1, 0, 1, 0};
@@ -78,6 +96,11 @@ struct rs_engine {
   template <typename T> T* at(const std::string& n) const {
     const Param* p = find(n);
     return p ? reinterpret_cast<T*>(arena + p->off) : nullptr;
+  }
+  const __half* packed(const std::string& n, int* ld) const {   // a packed fp16 weight matrix and its row length
+    const Param* p = find(n);
+    if (p) *ld = p->ipad;
+    return at<__half>(n);
   }
 };
 
@@ -278,8 +301,6 @@ int build_inventory(rs_engine& e) {
 // ------------------------------------------------------------------------------------------------
 namespace {
 
-enum OpKind { OP_CONV, OP_GN, OP_ATTN, OP_UPSAMPLE, OP_MLP, OP_SOFTMAX, OP_SWIN_ATTN, OP_VQ_ATTN };
-
 struct Tensor {
   size_t bytes = 0;
   int first = 1 << 30, last = -1;
@@ -287,42 +308,54 @@ struct Tensor {
   bool persistent = false;
 };
 
-struct Op {
-  OpKind kind;
-  ConvDesc conv;
-  GnDesc gn;
-  // attention
-  View a_in, a_out; const float* a_bias = nullptr; int a_window = 8, a_shift = 0;
-  // 2x resampling: nearest upsample, or (u_pool) 2x2 average pool
-  View u_in, u_out; bool u_pool = false;
-  // conv whose bias is a FiLM-table row (ResBlock without scale-shift norm): its offset in a row, or -1
-  int bias_film_off = -1;
-  // row softmax (VQ-GAN attention): in place on s_view [rows = N*H*W][cols = C]
-  View s_view; float s_scale = 1.f;
-  // conv whose "weight" matrix is an activation tensor of the plan (per-image attention GEMMs), or whose INPUT is a
-  // weight matrix of the arena viewed as pixels (the transposed value projection): see vq.inc
+// The GroupNorm statistics a consumer reads (a GroupNorm op, the fused MLP's norm2, the fused Swin attention's norm1):
+// (mean, M2) pairs [N][slots][C][2] of `in` from its producers' epilogues (fused) or from gn_stats_kernel
+struct GnLink {
+  View in;
+  bool fused = false;
+  int slots = 0;           // pair slots per image: 128-pixel conv tiles, 8x8 windows (win_slots), or gn_chunks (unfused)
+  bool win_slots = false;  // the producer is the fused Swin attention kernel: one slot per 8x8 window (64 values each)
+  size_t stats_off = 0;    // offset of the pair buffer inside the stats region
+  int gn_index = -1;       // index of its [N][32][2] group statistics / [N] arrival counters
+  float eps = 1e-5f;
+};
+struct StatDst { GnLink to; int coff; };            // a consumer a producer's epilogue delivers to, at its channel coff
+struct Producer { std::vector<StatDst> stat_dst; };   // conv, fused MLP, fused Swin attention: up to two consumers
+
+// The payload of each op kind; parameter names are resolved at bind
+struct ConvOp : Producer {
+  ConvDesc d;
+  std::string w_name, b_name;   // (b_name empty: no bias)
+  int bias_film_off = -1;       // the bias is a FiLM-table row (ResBlock without scale-shift norm): its offset in a row
+  bool to_f32 = false;          // writes the fp32 NCHW model output
+  int split_tens = -1;          // workspace tensor holding split-K partial sums (or -1)
+  // VQ-GAN attention GEMMs (vq.inc): "weights" that are an activation tensor [Cout rows][K] of the plan, and / or input
+  // "pixels" that are the rows of the arena's weight matrix in_param (the transposed value projection)
   View w_view; bool w_is_view = false;
   std::string in_param;
-  // fused MLP
-  MlpDesc mlp;
-  // fused attention half of a Swin block (norm1 + qkv + window attention + proj + residual)
-  SwinAttnDesc swin;
-  // fused attention over all positions of an image (VQ-GAN bottleneck with H*W > 8192, vq.inc)
-  VqAttnDesc vqa;
-  std::string blk_name;
-  std::string w2_name, b2_name;
-  std::string w_name, b_name, g_name;   // parameter names resolved at bind
-  size_t stats_off = 0;                 // GroupNorm: offset of its (mean, M2) pair buffer inside the stats region
-  int gn_index = -1;                    // GroupNorm: index of its [N][32][2] group statistics / [N] arrival counters
-  bool to_f32 = false;                  // conv: writes the fp32 NCHW model output
-  int split_tens = -1;                  // conv: workspace tensor holding split-K partial sums (or -1)
-  struct StatDst { int list; int op; int coff; };
-  std::vector<StatDst> stat_dst;        // conv: GroupNorm ops whose statistics this conv's epilogue produces
 };
+struct GnOp { GnDesc d; GnLink stats; std::string name; };   // d.in / fused / slots / eps come from stats at bind
+struct WinAttnOp { View qkv, out; int window = 8, shift = 0; std::string bias_name; const float* bias = nullptr; };
+struct ResampleOp { View in, out; bool pool = false; };     // 2x nearest upsample, or (pool) 2x2 average pool
+struct MlpOp : Producer { MlpDesc d; std::string name, norm_name; std::optional<GnLink> norm2; };   // norm2: in the kernel
+struct SwinOp : Producer { SwinAttnDesc d; std::string blk; GnLink norm1; };
+struct SoftmaxOp { View view; float scale = 1.f; };         // in place on view [rows = N*H*W][cols = C]
 
-inline SoftmaxParams softmax_params(const Op& op) {
-  const View& s = op.s_view;
-  return SoftmaxParams{s.ptr, (long long)s.ld, s.N * s.H * s.W, s.C, op.s_scale};
+// an op is its kind's payload and nothing else: the alternatives follow OpKind
+enum OpKind { OP_CONV, OP_GN, OP_ATTN, OP_UPSAMPLE, OP_MLP, OP_SOFTMAX, OP_SWIN_ATTN, OP_VQ_ATTN };
+using OpPayload = std::variant<ConvOp, GnOp, WinAttnOp, ResampleOp, MlpOp, SoftmaxOp, SwinOp, VqAttnDesc>;
+template <OpKind K, typename T> constexpr bool payload_of = std::is_same_v<std::variant_alternative_t<K, OpPayload>, T>;
+static_assert(std::variant_size_v<OpPayload> == OP_VQ_ATTN + 1 && payload_of<OP_CONV, ConvOp> && payload_of<OP_GN, GnOp> &&
+              payload_of<OP_ATTN, WinAttnOp> && payload_of<OP_UPSAMPLE, ResampleOp> && payload_of<OP_MLP, MlpOp> &&
+              payload_of<OP_SOFTMAX, SoftmaxOp> && payload_of<OP_SWIN_ATTN, SwinOp> && payload_of<OP_VQ_ATTN, VqAttnDesc>);
+using Op = OpPayload;
+inline OpKind kind_of(const Op& op) { return static_cast<OpKind>(op.index()); }
+// the payload of an op of kind T (read under that kind's case only)
+template <typename T, typename O> auto& payload(O& op) { return *std::get_if<T>(&op); }
+
+inline SoftmaxParams softmax_params(const SoftmaxOp& s) {
+  const View& v = s.view;
+  return SoftmaxParams{v.ptr, (long long)v.ld, v.N * v.H * v.W, v.C, s.scale};
 }
 
 }  // namespace
@@ -347,7 +380,7 @@ struct rs_plan {
   bool bound = false;
   int device = -1;           // CUDA device that was current at rs_plan_bind: the only one the plan runs on
   int launches = 0;
-  int vq_which = -1;         // -1: denoiser plan; 0 / 1: VQ-GAN encode / decode plan (vq.inc)
+  Pass pass = Pass::Denoiser;
   int imgH = 0, imgW = 0;    // VQ plans: image size (H, W above are the latent size)
   int vq_attn_op = -1;       // VQ plans: index in ops of the fused bottleneck attention (-1: none, T <= 8192)
   // The schedule tables and the FiLM table live in this plan's workspace and are shared by rs_plan_forward (FiLM rows
@@ -393,9 +426,15 @@ struct Builder {
     return w.c0 >= v.c0 && w.c0 + w.C <= v.c0 + v.C && w.n0 >= v.n0 && w.n0 + w.N <= v.n0 + v.N;
   }
   void note_writer(const View& out, int C, int win_slots = 0) {
-    auto& ws = writers[out.tens];
-    ws.erase(std::remove_if(ws.begin(), ws.end(), [&](const Writer& w) { return overlaps(w, out, C); }), ws.end());
-    ws.push_back({out.c0, C, out.n0, out.N, list_id(), (int)cur->size() - 1, win_slots});
+    forget_writers(out, C);
+    writers[out.tens].push_back({out.c0, C, out.n0, out.N, list_id(), (int)cur->size() - 1, win_slots});
+  }
+  // the op a writer names: a conv, fused MLP or fused Swin attention (the kinds that note writers)
+  Producer& producer(const Writer& w) {
+    Op& op = list(w.list)[w.op];
+    if (ConvOp* c = std::get_if<ConvOp>(&op)) return *c;
+    if (MlpOp* m = std::get_if<MlpOp>(&op)) return *m;
+    return payload<SwinOp>(op);
   }
   // producers of every (channel, image) of `in` whose epilogues can deliver GroupNorm statistics (empty: not fusable)
   std::vector<Writer> covering_writers(const View& in) {
@@ -409,10 +448,24 @@ struct Builder {
         for (const Writer& w : it->second)
           if (inside(w, in)) { prod.push_back(w); covered += (long long)w.C * w.N; }
       bool ok = covered == (long long)in.C * in.N;
-      for (const Writer& w : prod) ok = ok && list(w.list)[w.op].stat_dst.size() < 2 && w.win_slots == prod[0].win_slots;
+      for (const Writer& w : prod) ok = ok && producer(w).stat_dst.size() < 2 && w.win_slots == prod[0].win_slots;
       if (!ok) prod.clear();
     }
     return prod;
+  }
+  // The statistics of a GroupNorm over `in`, with its pair buffer and group-statistics index reserved: from the producers'
+  // epilogues when they can deliver them (the consumer is added to their stat_dst), else from gn_stats_kernel in gn_chunks
+  // slots, or, with fused_only, none (nullopt)
+  std::optional<GnLink> link_stats(const View& in, float eps, bool fused_only) {
+    const std::vector<Writer> prod = covering_writers(in);
+    if (prod.empty() && fused_only) return std::nullopt;
+    GnLink s{in, !prod.empty(), 0, !prod.empty() && prod[0].win_slots, stats_off, n_gn++, eps};
+    if (s.win_slots) s.slots = (in.H / 8) * (in.W / 8);
+    else if (s.fused) s.slots = conv_tile_slots(in.H, in.W);
+    else { int rows; gn_chunks(in.H * in.W, in.N, &s.slots, &rows); }
+    stats_off += align_up((size_t)in.N * s.slots * in.C * 2 * sizeof(float), 256);
+    for (const Writer& w : prod) producer(w).stat_dst.push_back({s, w.c0 - in.c0});
+    return s;
   }
   const bool fuse_mlp = env_int("RS_MLP_FUSE", 1) && !env_is("RS_CONV_IMPL", "simt");
   // norm2 applied inside the fused MLP kernel (bit-identical to the separate pass; RS_MLP_NORM_FUSE=1, off by default:
@@ -437,18 +490,18 @@ struct Builder {
 
   void conv(const View& in, const std::string& name, int ksize, int stride, int cout, const View* out,
             const View* res, int act, bool out_f32 = false, int pad_lo = 1, int bias_film_off = -1) {
-    Op op; op.kind = OP_CONV;
-    op.conv.in = in; op.conv.ksize = ksize; op.conv.stride = stride; op.conv.Cout = cout; op.conv.act = act;
-    op.conv.pad_lo = pad_lo;
-    op.bias_film_off = bias_film_off; op.conv.bias_per_image = bias_film_off >= 0;
-    if (out) { op.conv.out = *out; op.conv.has_out = true; } else op.conv.has_out = false;
-    if (res) { op.conv.res = *res; op.conv.has_res = true; }
+    ConvOp op;
+    op.d.in = in; op.d.ksize = ksize; op.d.stride = stride; op.d.Cout = cout; op.d.act = act;
+    op.d.pad_lo = pad_lo;
+    op.bias_film_off = bias_film_off; op.d.bias_per_image = bias_film_off >= 0;
+    if (out) { op.d.out = *out; op.d.has_out = true; } else op.d.has_out = false;
+    if (res) { op.d.res = *res; op.d.has_res = true; }
     op.w_name = name + ".weight"; op.b_name = name + ".bias";
     op.to_f32 = out_f32;
     if (out && !out_f32 && env_int("RS_CONV_SPLITK", 0) != 1) {       // split-K for layers with too few tiles
       const TileConfig tc = conv_preview_config(in.N, in.H, in.W, in.C, cout, ksize, stride, true);
       if (tc.splitk > 1) {
-        op.conv.allow_split = true;
+        op.d.allow_split = true;
         const size_t bytes = (size_t)tc.splitk * in.N * (in.H / stride) * (in.W / stride) * cout * sizeof(float);
         op.split_tens = P.new_tensor(bytes);
         Tensor& tz = P.tensors[op.split_tens];
@@ -457,84 +510,56 @@ struct Builder {
     }
     const int i = opi();
     P.touch(in, i); if (out) P.touch(*out, i); if (res) P.touch(*res, i);
-    cur->push_back(op);
+    cur->push_back(std::move(op));
     if (out && !out_f32 && out->tens >= 0) note_writer(*out, cout);   // the latest writer of this (channel, image) range
   }
   void gn(const View& in, const std::string& name, const View& out, int silu, int film_off, float eps = 1e-5f) {
-    Op op; op.kind = OP_GN;
-    op.gn.in = in; op.gn.out = out; op.gn.silu = silu; op.gn.film_off = film_off; op.gn.eps = eps;
-    op.g_name = name;
-    // can the producers' epilogues deliver the statistics?  (every channel of every image of the view written by a
-    // conv / MLP of this plan)
-    std::vector<Writer> prod = covering_writers(in);
-    op.gn.win_slots = !prod.empty() && prod[0].win_slots;
-    const int tile_slots = op.gn.win_slots ? (in.H / 8) * (in.W / 8) : conv_tile_slots(in.H, in.W);
-    int chunks, rows;
-    gn_chunks(in.H * in.W, in.N, &chunks, &rows);
-    op.gn.fused = !prod.empty();
-    op.gn.slots = op.gn.fused ? tile_slots : chunks;
-    op.stats_off = stats_off;
-    op.gn_index = n_gn++;
-    stats_off += align_up((size_t)in.N * op.gn.slots * in.C * 2 * sizeof(float), 256);
+    GnOp op;
+    op.d.out = out; op.d.silu = silu; op.d.film_off = film_off;
+    op.stats = *link_stats(in, eps, /*fused_only=*/false);
+    op.name = name;
     const int i = opi();
     P.touch(in, i); P.touch(out, i);
-    cur->push_back(op);
-    for (const Writer& w : prod)
-      list(w.list)[w.op].stat_dst.push_back({list_id(), (int)cur->size() - 1, w.c0 - in.c0});
+    cur->push_back(std::move(op));
   }
   void attn(const View& qkv, const View& out, const std::string& blk, int window, int shift) {
-    Op op; op.kind = OP_ATTN; op.a_in = qkv; op.a_out = out; op.a_window = window; op.a_shift = shift;
-    op.w_name = blk + ".attn.relative_position_bias_table";
+    WinAttnOp op; op.qkv = qkv; op.out = out; op.window = window; op.shift = shift;
+    op.bias_name = blk + ".attn.relative_position_bias_table";
     const int i = opi();
     P.touch(qkv, i); P.touch(out, i);
-    cur->push_back(op);
+    cur->push_back(std::move(op));
   }
   // norm_name non-empty: `in` is the un-normalised tensor and the kernel applies that GroupNorm to its X tile itself
   // (returns false, adding nothing, when the statistics cannot come from the producers' epilogues)
   bool mlp(const View& in, const std::string& name, int E, int Hd, const View& out, const View& res,
            const std::string& norm_name = std::string()) {
-    Op op; op.kind = OP_MLP;
-    op.mlp.in = in; op.mlp.out = out; op.mlp.res = res; op.mlp.has_res = true; op.mlp.E = E; op.mlp.Hd = Hd;
-    op.w_name = name + ".fc1.weight"; op.b_name = name + ".fc1.bias";
-    op.w2_name = name + ".fc2.weight"; op.b2_name = name + ".fc2.bias";
-    std::vector<Writer> prod;
+    MlpOp op;
+    op.d.in = in; op.d.out = out; op.d.res = res; op.d.has_res = true; op.d.E = E; op.d.Hd = Hd;
+    op.name = name;
     if (!norm_name.empty()) {
-      prod = covering_writers(in);
-      if (prod.empty() || Hd < 4 * E) return false;
-      op.g_name = norm_name;
-      op.gn.win_slots = prod[0].win_slots;
-      op.gn.in = in; op.gn.fused = true; op.gn.slots = op.gn.win_slots ? (in.H / 8) * (in.W / 8) : conv_tile_slots(in.H, in.W);
-      op.stats_off = stats_off;
-      op.gn_index = n_gn++;
-      stats_off += align_up((size_t)in.N * op.gn.slots * in.C * 2 * sizeof(float), 256);
+      if (Hd < 4 * E) return false;
+      op.norm2 = link_stats(in, 1e-5f, /*fused_only=*/true);
+      if (!op.norm2) return false;
+      op.norm_name = norm_name;
     }
     const int i = opi();
     P.touch(in, i); P.touch(out, i); P.touch(res, i);
-    cur->push_back(op);
-    for (const Writer& w : prod)
-      list(w.list)[w.op].stat_dst.push_back({list_id(), (int)cur->size() - 1, w.c0 - in.c0});
+    cur->push_back(std::move(op));
     if (out.tens >= 0) note_writer(out, E);
     return true;
   }
   // x <- x + proj(window_attention(qkv(norm1(x)))) in one kernel (swin_attn_fused.cuh); false when the statistics of x
   // cannot come from its producers' epilogues
   bool swin_attn(const View& x, const std::string& blk, int heads, int shift) {
-    std::vector<Writer> prod = covering_writers(x);
-    if (prod.empty()) return false;
-    Op op; op.kind = OP_SWIN_ATTN;
-    op.swin.x = x; op.swin.y = x; op.swin.heads = heads; op.swin.shift = shift;
-    op.blk_name = blk;
-    op.g_name = blk + ".norm1";
-    op.gn.win_slots = prod[0].win_slots;
-    op.gn.in = x; op.gn.fused = true; op.gn.slots = op.gn.win_slots ? (x.H / 8) * (x.W / 8) : conv_tile_slots(x.H, x.W);
-    op.stats_off = stats_off;
-    op.gn_index = n_gn++;
-    stats_off += align_up((size_t)x.N * op.gn.slots * x.C * 2 * sizeof(float), 256);
+    const std::optional<GnLink> norm1 = link_stats(x, 1e-5f, /*fused_only=*/true);
+    if (!norm1) return false;
+    SwinOp op;
+    op.d.x = x; op.d.y = x; op.d.heads = heads; op.d.shift = shift;
+    op.blk = blk;
+    op.norm1 = *norm1;
     const int i = opi();
     P.touch(x, i);
-    cur->push_back(op);
-    for (const Writer& w : prod)
-      list(w.list)[w.op].stat_dst.push_back({list_id(), (int)cur->size() - 1, w.c0 - x.c0});
+    cur->push_back(std::move(op));
     if (x.tens >= 0) note_writer(x, x.C, /*win_slots=*/1);
     return true;
   }
@@ -546,10 +571,9 @@ struct Builder {
     ws.erase(std::remove_if(ws.begin(), ws.end(), [&](const Writer& w) { return overlaps(w, out, C); }), ws.end());
   }
   void upsample(const View& in, const View& out, bool pool = false) {
-    Op op; op.kind = OP_UPSAMPLE; op.u_in = in; op.u_out = out; op.u_pool = pool;
     const int i = opi();
     P.touch(in, i); P.touch(out, i);
-    cur->push_back(op);
+    cur->push_back(ResampleOp{in, out, pool});
     forget_writers(out, out.C);
   }
 
@@ -839,137 +863,130 @@ void resolve(rs_plan& P, View& v) {
 //     small launch in front of the consumer, or, for a GroupNorm without a fusable producer, the last gn_stats_kernel CTA
 //     of each image (arrival counters).  (The last producer CTA of an image would do it at the cost of a counter round
 //     trip on every tile, and on a persistent conv the CTAs all finish together, so ONE of them would reduce every image.)
-bool gn_finalizes(const Op& g) {
+bool gn_finalizes(const GnLink& g) {
   static const int thr = env_int("RS_GN_FINALIZE_SLOTS", 64);
-  return g.gn.slots > thr && !g.gn.win_slots;      // (the fused Swin attention kernel delivers pairs only)
+  return g.slots > thr && !g.win_slots;      // (the fused Swin attention kernel delivers pairs only)
 }
-GnSink make_sink(rs_plan& P, const Op& g, int coff, bool consumer = false) {
+GnSink make_sink(rs_plan& P, const GnLink& g, int coff, bool consumer = false) {
   GnSink s{};
   s.part = reinterpret_cast<float*>(P.ws + P.off_stats + g.stats_off);
   if (consumer && gn_finalizes(g)) {
     s.gstat = reinterpret_cast<float*>(P.ws + P.off_gstat) + (size_t)g.gn_index * P.B * 64;
     s.counter = reinterpret_cast<unsigned int*>(P.ws + P.off_counters) + (size_t)g.gn_index * P.B;
   }
-  s.cstride = g.gn.in.C; s.coff = coff; s.expected = (unsigned)(g.gn.slots * g.gn.in.C); s.eps = g.gn.eps;
+  s.cstride = g.in.C; s.coff = coff; s.expected = (unsigned)(g.slots * g.in.C); s.eps = g.eps;
   return s;
+}
+// the statistics sinks of a producer's epilogue: one per consumer it delivers to
+void bind_sinks(rs_plan& P, const Producer& pr, GnSink (&sink)[2]) {
+  for (int i = 0; i < 2; ++i)
+    sink[i] = i < (int)pr.stat_dst.size() ? make_sink(P, pr.stat_dst[i].to, pr.stat_dst[i].coff) : GnSink{};
 }
 
 int bind_ops(rs_plan& P, std::vector<Op>& ops) {
   rs_engine& E = *P.e;
   for (Op& op : ops) {
-    if (op.kind == OP_CONV) {
-      for (int i = 0; i < 2; ++i) {
-        op.conv.sink[i] = GnSink{};
-        if (i < (int)op.stat_dst.size()) {
-          const Op::StatDst& sd = op.stat_dst[i];
-          op.conv.sink[i] = make_sink(P, (sd.list == 0 ? P.fe_ops : P.ops)[sd.op], sd.coff);
+    int rc = 0, launches = 1;
+    switch (kind_of(op)) {
+      case OP_CONV: {
+        ConvOp& c = payload<ConvOp>(op);
+        ConvDesc& d = c.d;
+        bind_sinks(P, c, d.sink);
+        resolve(P, d.in); if (d.has_out) resolve(P, d.out); if (d.has_res) resolve(P, d.res);
+        if (!c.in_param.empty()) {          // the "pixels" are the rows of a weight matrix of the arena
+          const Param* wp = E.find(c.in_param);
+          RS_CHECK(wp != nullptr && wp->ipad == d.in.ld, "missing / mismatching parameter " + c.in_param);
+          d.in.ptr = E.at<__half>(c.in_param);
         }
-      }
-      ConvDesc& d = op.conv;
-      resolve(P, d.in); if (d.has_out) resolve(P, d.out); if (d.has_res) resolve(P, d.res);
-      if (!op.in_param.empty()) {          // the "pixels" are the rows of a weight matrix of the arena
-        const Param* wp = E.find(op.in_param);
-        RS_CHECK(wp != nullptr && wp->ipad == d.in.ld, "missing / mismatching parameter " + op.in_param);
-        d.in.ptr = E.at<__half>(op.in_param);
-      }
-      if (op.w_is_view) {                  // the "weights" are an activation tensor [Cout rows][K], K-major
-        resolve(P, op.w_view);
-        d.wt = op.w_view.ptr; d.ipad = op.w_view.ld;
-        d.bias = op.b_name.empty() ? nullptr : E.at<float>(op.b_name);
-      } else {
-        const Param* w = E.find(op.w_name);
-        RS_CHECK(w != nullptr, "missing parameter " + op.w_name);
-        d.wt = E.at<__half>(op.w_name); d.ipad = w->ipad; d.bias = E.at<float>(op.b_name);
-      }
-      d.out_f32 = op.to_f32 ? P.out_f32 : nullptr;
-      d.partial = op.split_tens >= 0 ? reinterpret_cast<float*>(P.ws + P.tensors[op.split_tens].off) : nullptr;
-      // the first conv reads the channel-padded packed input: expose the padded width to the kernel
-      if (d.in.C < d.ipad && d.in.ld >= d.ipad && d.in.tens == P.xin.tens) d.in.C = d.ipad;
-      if (d.in.C < d.ipad && P.fe_in.tens >= 0 && d.in.tens == P.fe_in.tens) d.in.C = d.ipad;
-      int rc = conv_finalize(d); if (rc) return rc;
-      P.launches += d.prm.splitk > 1 ? 2 : 1;
-    } else if (op.kind == OP_GN) {
-      resolve(P, op.gn.in); resolve(P, op.gn.out);
-      op.gn.gamma = E.at<float>(op.g_name + ".weight"); op.gn.beta = E.at<float>(op.g_name + ".bias");
-      RS_CHECK(op.gn.gamma && op.gn.beta, "missing GroupNorm parameters " + op.g_name);
-      {
-        const GnSink sk = make_sink(P, op, 0, true);
-        op.gn.part = sk.part; op.gn.gstat = sk.gstat; op.gn.counter = sk.counter;
-        op.gn.finalize_kernel = op.gn.fused && gn_finalizes(op);
-      }
-      P.launches += (op.gn.fused ? 1 : 2) + (op.gn.finalize_kernel ? 1 : 0);
-    } else if (op.kind == OP_MLP) {
-      MlpDesc& m = op.mlp;
-      resolve(P, m.in); resolve(P, m.out); resolve(P, m.res);
-      m.w1 = E.at<__half>(op.w_name); m.b1 = E.at<float>(op.b_name);
-      m.w2 = E.at<__half>(op.w2_name); m.b2 = E.at<float>(op.b2_name);
-      RS_CHECK(m.w1 && m.w2 && m.b1 && m.b2, "missing MLP parameters " + op.w_name);
-      const Param* w1p = E.find(op.w_name); const Param* w2p = E.find(op.w2_name);
-      RS_CHECK(w1p->ipad == m.E && w2p->ipad == m.Hd, "MLP weight padding");
-      if (!op.g_name.empty()) {
-        const GnSink sk = make_sink(P, op, 0);
-        m.gn_in_gstat = sk.gstat; m.gn_in_part = sk.part; m.gn_in_slots = op.gn.slots;
-        m.gn_in_gamma = E.at<float>(op.g_name + ".weight"); m.gn_in_beta = E.at<float>(op.g_name + ".bias");
-        RS_CHECK(m.gn_in_gamma && m.gn_in_beta, "missing GroupNorm parameters " + op.g_name);
-      }
-      for (int i = 0; i < 2; ++i) {
-        m.sink[i] = GnSink{};
-        if (i < (int)op.stat_dst.size()) {
-          const Op::StatDst& sd = op.stat_dst[i];
-          m.sink[i] = make_sink(P, (sd.list == 0 ? P.fe_ops : P.ops)[sd.op], sd.coff);
+        if (c.w_is_view) {                  // the "weights" are an activation tensor [Cout rows][K], K-major
+          resolve(P, c.w_view);
+          d.wt = c.w_view.ptr; d.ipad = c.w_view.ld;
+          d.bias = c.b_name.empty() ? nullptr : E.at<float>(c.b_name);
+        } else {
+          d.wt = E.packed(c.w_name, &d.ipad); d.bias = E.at<float>(c.b_name);
+          RS_CHECK(d.wt != nullptr, "missing parameter " + c.w_name);
         }
+        d.out_f32 = c.to_f32 ? P.out_f32 : nullptr;
+        d.partial = c.split_tens >= 0 ? reinterpret_cast<float*>(P.ws + P.tensors[c.split_tens].off) : nullptr;
+        // the first conv reads the channel-padded packed input: expose the padded width to the kernel
+        if (d.in.C < d.ipad && d.in.ld >= d.ipad && d.in.tens == P.xin.tens) d.in.C = d.ipad;
+        if (d.in.C < d.ipad && P.fe_in.tens >= 0 && d.in.tens == P.fe_in.tens) d.in.C = d.ipad;
+        rc = conv_finalize(d);
+        launches = d.prm.splitk > 1 ? 2 : 1;
+        break;
       }
-      int rc = mlp_finalize(m); if (rc) return rc;
-      ++P.launches;
-    } else if (op.kind == OP_ATTN) {
-      resolve(P, op.a_in); resolve(P, op.a_out);
-      op.a_bias = E.at<float>(op.w_name);
-      RS_CHECK(op.a_bias != nullptr, "missing " + op.w_name);
-      ++P.launches;
-    } else if (op.kind == OP_SWIN_ATTN) {
-      SwinAttnDesc& w = op.swin;
-      resolve(P, w.x); resolve(P, w.y);
-      const std::string& b = op.blk_name;
-      const Param* wq = E.find(b + ".attn.qkv.weight"); const Param* wp = E.find(b + ".attn.proj.weight");
-      RS_CHECK(wq && wp, "missing attention parameters of " + b);
-      w.wqkv = E.at<__half>(b + ".attn.qkv.weight"); w.wqkv_ld = wq->ipad; w.bqkv = E.at<float>(b + ".attn.qkv.bias");
-      w.wproj = E.at<__half>(b + ".attn.proj.weight"); w.wproj_ld = wp->ipad; w.bproj = E.at<float>(b + ".attn.proj.bias");
-      w.relbias = E.at<float>(b + ".attn.relative_position_bias_table");
-      w.gamma = E.at<float>(b + ".norm1.weight"); w.beta = E.at<float>(b + ".norm1.bias");
-      RS_CHECK(w.bqkv && w.bproj && w.relbias && w.gamma && w.beta, "missing attention parameters of " + b);
-      {
-        const GnSink sk = make_sink(P, op, 0);
-        w.gn_part = sk.part; w.gn_slots = op.gn.slots; w.gn_gstat = sk.gstat;
+      case OP_GN: {
+        GnOp& g = payload<GnOp>(op);
+        GnDesc& d = g.d;
+        d.in = g.stats.in; d.fused = g.stats.fused; d.slots = g.stats.slots; d.eps = g.stats.eps;
+        resolve(P, d.in); resolve(P, d.out);
+        d.gamma = E.at<float>(g.name + ".weight"); d.beta = E.at<float>(g.name + ".bias");
+        RS_CHECK(d.gamma && d.beta, "missing GroupNorm parameters " + g.name);
+        const GnSink sk = make_sink(P, g.stats, 0, true);
+        d.part = sk.part; d.gstat = sk.gstat; d.counter = sk.counter;
+        d.finalize_kernel = d.fused && gn_finalizes(g.stats);
+        launches = (d.fused ? 1 : 2) + (d.finalize_kernel ? 1 : 0);
+        break;
       }
-      for (int i = 0; i < 2; ++i) {
-        w.sink[i] = GnSink{};
-        if (i < (int)op.stat_dst.size()) {
-          const Op::StatDst& sd = op.stat_dst[i];
-          w.sink[i] = make_sink(P, (sd.list == 0 ? P.fe_ops : P.ops)[sd.op], sd.coff);
+      case OP_ATTN: {
+        WinAttnOp& a = payload<WinAttnOp>(op);
+        resolve(P, a.qkv); resolve(P, a.out);
+        a.bias = E.at<float>(a.bias_name);
+        RS_CHECK(a.bias != nullptr, "missing " + a.bias_name);
+        break;
+      }
+      case OP_UPSAMPLE: resolve(P, payload<ResampleOp>(op).in); resolve(P, payload<ResampleOp>(op).out); break;
+      case OP_MLP: {
+        MlpOp& mo = payload<MlpOp>(op);
+        MlpDesc& m = mo.d;
+        resolve(P, m.in); resolve(P, m.out); resolve(P, m.res);
+        int ld1 = 0, ld2 = 0;
+        m.w1 = E.packed(mo.name + ".fc1.weight", &ld1); m.b1 = E.at<float>(mo.name + ".fc1.bias");
+        m.w2 = E.packed(mo.name + ".fc2.weight", &ld2); m.b2 = E.at<float>(mo.name + ".fc2.bias");
+        RS_CHECK(m.w1 && m.w2 && m.b1 && m.b2, "missing MLP parameters " + mo.name + ".fc1.weight");
+        RS_CHECK(ld1 == m.E && ld2 == m.Hd, "MLP weight padding");
+        if (mo.norm2) {
+          const GnSink sk = make_sink(P, *mo.norm2, 0);
+          m.gn_in_gstat = sk.gstat; m.gn_in_part = sk.part; m.gn_in_slots = mo.norm2->slots;
+          m.gn_in_gamma = E.at<float>(mo.norm_name + ".weight"); m.gn_in_beta = E.at<float>(mo.norm_name + ".bias");
+          RS_CHECK(m.gn_in_gamma && m.gn_in_beta, "missing GroupNorm parameters " + mo.norm_name);
         }
+        bind_sinks(P, mo, m.sink);
+        rc = mlp_finalize(m);
+        break;
       }
-      int rc = swin_attn_finalize(w); if (rc) return rc;
-      ++P.launches;
-    } else if (op.kind == OP_SOFTMAX) {
-      resolve(P, op.s_view);
-      int rc = softmax_rows_check(softmax_params(op)); if (rc) return rc;
-      ++P.launches;
-    } else if (op.kind == OP_VQ_ATTN) {
-      VqAttnDesc& a = op.vqa;
-      resolve(P, a.q); resolve(P, a.k); resolve(P, a.v); resolve(P, a.out);
-      int rc = vq_attn_finalize(a); if (rc) return rc;
-      ++P.launches;
-    } else {
-      resolve(P, op.u_in); resolve(P, op.u_out);
-      ++P.launches;
+      case OP_SOFTMAX: resolve(P, payload<SoftmaxOp>(op).view); rc = softmax_rows_check(softmax_params(payload<SoftmaxOp>(op))); break;
+      case OP_SWIN_ATTN: {
+        SwinOp& so = payload<SwinOp>(op);
+        SwinAttnDesc& w = so.d;
+        resolve(P, w.x); resolve(P, w.y);
+        const std::string& b = so.blk;
+        w.wqkv = E.packed(b + ".attn.qkv.weight", &w.wqkv_ld); w.bqkv = E.at<float>(b + ".attn.qkv.bias");
+        w.wproj = E.packed(b + ".attn.proj.weight", &w.wproj_ld); w.bproj = E.at<float>(b + ".attn.proj.bias");
+        w.relbias = E.at<float>(b + ".attn.relative_position_bias_table");
+        w.gamma = E.at<float>(b + ".norm1.weight"); w.beta = E.at<float>(b + ".norm1.bias");
+        RS_CHECK(w.wqkv && w.wproj && w.bqkv && w.bproj && w.relbias && w.gamma && w.beta, "missing attention parameters of " + b);
+        const GnSink sk = make_sink(P, so.norm1, 0);
+        w.gn_part = sk.part; w.gn_slots = so.norm1.slots; w.gn_gstat = sk.gstat;
+        bind_sinks(P, so, w.sink);
+        rc = swin_attn_finalize(w);
+        break;
+      }
+      case OP_VQ_ATTN: {
+        VqAttnDesc& a = payload<VqAttnDesc>(op);
+        resolve(P, a.q); resolve(P, a.k); resolve(P, a.v); resolve(P, a.out);
+        rc = vq_attn_finalize(a);
+        break;
+      }
     }
+    if (rc) return rc;
+    P.launches += launches;
   }
   return 0;
 }
 
 struct Prof {
-  std::vector<cudaEvent_t> ev;     // pairs
-  std::vector<int> kind;
+  std::vector<cudaEvent_t> ev;     // a pair per op run, skipped or not
   int used = 0;
   cudaEvent_t get() {
     if (used == (int)ev.size()) { cudaEvent_t e; cudaEventCreate(&e); ev.push_back(e); }
@@ -984,14 +1001,12 @@ struct Prof {
 inline bool op_skipped(const Op& op) {
   static const int skip = env_int("RS_SKIP_KINDS", 0);
   if (!skip) return false;
-  switch (op.kind) {
-    case OP_CONV: return (skip >> (op.conv.ksize == 3 ? 0 : 1)) & 1;
+  switch (kind_of(op)) {
+    case OP_CONV: return (skip >> (payload<ConvOp>(op).d.ksize == 3 ? 0 : 1)) & 1;
     case OP_GN: return (skip >> 2) & 1;
-    case OP_ATTN: return (skip >> 3) & 1;
+    case OP_ATTN: case OP_SWIN_ATTN: case OP_VQ_ATTN: return (skip >> 3) & 1;
     case OP_UPSAMPLE: return (skip >> 4) & 1;
     case OP_MLP: return (skip >> 5) & 1;
-    case OP_SWIN_ATTN: return (skip >> 3) & 1;
-    case OP_VQ_ATTN: return (skip >> 3) & 1;
     case OP_SOFTMAX: return false;
   }
   return false;
@@ -1003,41 +1018,44 @@ int run_op_range(rs_plan& P, const Op* first, const Op* last, const float* film_
   for (const Op* it = first; it != last; ++it) {
     const Op& op = *it;
     int rc = 0;
-    if (op_skipped(op)) { if (prof) { cudaEventRecord(prof->get(), st); prof->kind.push_back((int)op.kind); cudaEventRecord(prof->get(), st); } continue; }
-    if (prof) { cudaEventRecord(prof->get(), st); prof->kind.push_back((int)op.kind); }
-    switch (op.kind) {
+    if (op_skipped(op)) { if (prof) { cudaEventRecord(prof->get(), st); cudaEventRecord(prof->get(), st); } continue; }
+    if (prof) cudaEventRecord(prof->get(), st);
+    switch (kind_of(op)) {
       case OP_CONV: {
-        if (op.bias_film_off < 0) { rc = conv_launch(op.conv, st); break; }
-        ConvDesc d = op.conv;           // bias = this launch's FiLM row(s), resolved like a GroupNorm's film
-        const float* row = film_base + op.bias_film_off;
+        const ConvOp& c = payload<ConvOp>(op);
+        if (c.bias_film_off < 0) { rc = conv_launch(c.d, st); break; }
+        ConvDesc d = c.d;               // bias = this launch's FiLM row(s), resolved like a GroupNorm's film
+        const float* row = film_base + c.bias_film_off;
         if (d.prm.bias) { d.prm.bias = row; d.prm.bias_sN = (int)film_sN; }
         if (d.prm.splitk > 1) { d.red.bias = row; d.red.bias_sN = (int)film_sN; }
         rc = conv_launch(d, st);
         break;
       }
       case OP_GN: {
-        GnDesc g = op.gn;
+        GnDesc g = payload<GnOp>(op).d;
         if (g.film_off >= 0) { g.film = film_base + g.film_off; g.film_sN = film_sN; }
         rc = gn_launch(g, st);
         break;
       }
-      case OP_MLP: rc = mlp_launch(op.mlp, st); break;
-      case OP_SWIN_ATTN: rc = swin_attn_launch(op.swin, st); break;
-      case OP_VQ_ATTN: rc = vq_attn_launch(op.vqa, st); break;
-      case OP_ATTN:
-        rc = attn_launch(op.a_in, op.a_out, op.a_bias, P.e->cfg.swin_heads, P.e->cfg.swin_embed_dim, op.a_window, op.a_shift, st);
+      case OP_MLP: rc = mlp_launch(payload<MlpOp>(op).d, st); break;
+      case OP_SWIN_ATTN: rc = swin_attn_launch(payload<SwinOp>(op).d, st); break;
+      case OP_VQ_ATTN: rc = vq_attn_launch(payload<VqAttnDesc>(op), st); break;
+      case OP_ATTN: {
+        const WinAttnOp& a = payload<WinAttnOp>(op);
+        rc = attn_launch(a.qkv, a.out, a.bias, P.e->cfg.swin_heads, P.e->cfg.swin_embed_dim, a.window, a.shift, st);
         break;
+      }
       case OP_SOFTMAX: {
-        const SoftmaxParams sp = softmax_params(op);
+        const SoftmaxParams sp = softmax_params(payload<SoftmaxOp>(op));
         (void)launch_k(softmax_rows_kernel, dim3((unsigned)sp.rows), dim3(256), (size_t)0, st, sp);
         if (cudaGetLastError() != cudaSuccess) rc = fail(-2, "softmax launch failed");
         break;
       }
       case OP_UPSAMPLE: {
-        UpsampleParams u{op.u_in.ptr, op.u_in.sN(), op.u_in.ld, op.u_out.ptr, op.u_out.sN(), op.u_out.ld,
-                         op.u_in.N, op.u_in.H, op.u_in.W, op.u_in.C};
-        const long long total = (long long)u.N * (op.u_pool ? u.H * u.W / 4 : 4 * u.H * u.W) * (u.C / 8);
-        (void)launch_k(op.u_pool ? avgpool2x2_kernel : upsample2x_kernel,
+        const ResampleOp& r = payload<ResampleOp>(op);
+        UpsampleParams u{r.in.ptr, r.in.sN(), r.in.ld, r.out.ptr, r.out.sN(), r.out.ld, r.in.N, r.in.H, r.in.W, r.in.C};
+        const long long total = (long long)u.N * (r.pool ? u.H * u.W / 4 : 4 * u.H * u.W) * (u.C / 8);
+        (void)launch_k(r.pool ? avgpool2x2_kernel : upsample2x_kernel,
                        dim3((unsigned)std::min<long long>((total + 255) / 256, num_sms() * 16)), dim3(256), (size_t)(0), st, u);
         if (cudaGetLastError() != cudaSuccess) rc = fail(-2, "resample launch failed");
         break;
@@ -1114,6 +1132,17 @@ int check_plan_device(const rs_plan& P) {
     return fail(-1, "plan was bound on cuda:" + std::to_string(P.device) + " but cuda:" + std::to_string(dev) +
                     " is current: a plan runs on the device it was bound on");
   return 0;
+}
+
+// One forward of the denoiser on the caller's inputs: FiLM rows 0..B-1 for its timesteps, the packed input, the op list
+// (with a CUDA-event pair around every op when prof is given)
+int run_forward(rs_plan& P, const float* x, const float* timesteps, const float* lq, const float* mask, cudaStream_t st,
+                Prof* prof = nullptr) {
+  int rc = check_plan_device(P); if (rc) return rc;
+  P.table_owner = nullptr;                       // FiLM rows 0..B-1 are overwritten below
+  rc = run_embedding(P, timesteps, P.B, st); if (rc) return rc;
+  rc = pack_lq_and_input(P, x, lq, mask, nullptr, 0, st); if (rc) return rc;
+  return run_ops(P, P.ops, reinterpret_cast<const float*>(P.ws + P.off_film), P.e->film_rows, st, prof);
 }
 
 }  // namespace
@@ -1221,7 +1250,7 @@ int rs_unet_load_param(rs_engine* e, const char* name, const float* src, void* s
 
 int rs_plan_create(rs_engine* e, int batch, int height, int width, rs_plan** out) {
   RS_CHECK(e && out && batch > 0, "bad argument");
-  RS_CHECK(e->kind == 0, "this engine is a VQ-GAN first stage: use rs_vq_plan_create");
+  RS_CHECK(e->kind == EngineKind::Denoiser, std::string("this engine is ") + kind_name(e->kind) + ": use rs_vq_plan_create");
   // every level's H and W must be multiples of that level's window (the constructor-time rule: the level's nominal
   // resolution where that is not larger than window_size, else window_size)
   int mult = 1;
@@ -1252,7 +1281,7 @@ int rs_plan_bind(rs_plan* p, void* workspace_dev) {
   RS_CHECK(!p->bound || dev == p->device, "a bound plan can be rebound on its own device only");
   p->device = dev;
   p->ws = static_cast<uint8_t*>(workspace_dev);
-  if (p->vq_which >= 0) {
+  if (p->pass != Pass::Denoiser) {
     p->out_f32 = reinterpret_cast<float*>(p->ws + p->off_state);
   } else {
     const size_t lat = align_up((size_t)p->B * std::max(p->e->cfg.in_channels, p->e->cfg.out_channels) * p->H * p->W * 4, 256);
@@ -1265,7 +1294,7 @@ int rs_plan_bind(rs_plan* p, void* workspace_dev) {
   int rc = conv_init(); if (rc) return rc;
   rc = bind_ops(*p, p->fe_ops); if (rc) return rc;
   rc = bind_ops(*p, p->ops); if (rc) return rc;
-  p->launches += p->vq_which >= 0 ? 3 : 6;   // denoiser: embedding (4) + pack (1-2); VQ: counter reset, pack / quantise, output copy
+  p->launches += p->pass == Pass::Denoiser ? kDenoiserOuterLaunches : p->pass == Pass::Encode ? kEncodeOuterLaunches : kDecodeOuterLaunches;
   p->bound = true;
   return 0;
 }
@@ -1273,15 +1302,10 @@ int rs_plan_bind(rs_plan* p, void* workspace_dev) {
 int rs_plan_forward(rs_plan* p, const float* x, const float* timesteps, const float* lq, const float* mask, float* out,
                     void* stream) {
   RS_CHECK(p && p->bound, "plan is not bound");
-  RS_CHECK(p->vq_which < 0, "this is a VQ-GAN plan: use rs_vq_encode / rs_vq_decode");
+  RS_CHECK(p->pass == Pass::Denoiser, std::string("this plan belongs to ") + kind_name(p->e->kind) + ": use its encode / decode calls");
   RS_CHECK(x && timesteps && lq && out, "null tensor");
-  int rc = check_plan_device(*p); if (rc) return rc;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  p->table_owner = nullptr;                       // FiLM rows 0..B-1 are overwritten below
-  rc = run_embedding(*p, timesteps, p->B, st); if (rc) return rc;
-  rc = pack_lq_and_input(*p, x, lq, mask, nullptr, 0, st); if (rc) return rc;
-  const float* film = reinterpret_cast<const float*>(p->ws + p->off_film);
-  rc = run_ops(*p, p->ops, film, p->e->film_rows, st); if (rc) return rc;
+  int rc = run_forward(*p, x, timesteps, lq, mask, st); if (rc) return rc;
   const long long n = (long long)p->B * p->e->cfg.out_channels * p->H * p->W;
   (void)launch_k(copy_f32_kernel, dim3((unsigned)((n + 255) / 256)), dim3(256), (size_t)(0), st, p->out_f32, out, n);
   RS_CUDA_OK(cudaGetLastError());
@@ -1294,38 +1318,38 @@ int rs_plan_forward(rs_plan* p, const float* x, const float* timesteps, const fl
 // Swin attention) in that forward.
 int rs_plan_profile(rs_plan* p, const float* x, const float* timesteps, const float* lq, const float* mask,
                     double* ms_by_kind, double* conv_flops, int32_t* n_conv_launches, void* stream) {
-  RS_CHECK(p && p->bound && ms_by_kind && p->vq_which < 0, "bad argument (needs a bound denoiser plan)");
-  int rc = check_plan_device(*p); if (rc) return rc;
+  RS_CHECK(p && p->bound && ms_by_kind && p->pass == Pass::Denoiser, "bad argument (needs a bound denoiser plan)");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  p->table_owner = nullptr;
-  rc = run_embedding(*p, timesteps, p->B, st); if (rc) return rc;
-  rc = pack_lq_and_input(*p, x, lq, mask, nullptr, 0, st); if (rc) return rc;
   Prof prof;
-  const float* film = reinterpret_cast<const float*>(p->ws + p->off_film);
-  rc = run_ops(*p, p->ops, film, p->e->film_rows, st, &prof); if (rc) return rc;
+  int rc = run_forward(*p, x, timesteps, lq, mask, st, &prof); if (rc) return rc;
   RS_CUDA_OK(cudaStreamSynchronize(st));
   for (int k = 0; k < 4; ++k) ms_by_kind[k] = 0.0;
-  for (size_t i = 0; i < prof.kind.size(); ++i) {
+  double fl = 0.0; int nc = 0;
+  for (size_t i = 0; i < p->ops.size(); ++i) {
+    const Op& op = p->ops[i];
     float ms = 0.f;
     cudaEventElapsedTime(&ms, prof.ev[2 * i], prof.ev[2 * i + 1]);
-    const int kd = prof.kind[i];
-    // (the fused Swin attention kernel is a GEMM kernel: qkv + QK^T + PV + proj; it counts with the GEMM family)
-    ms_by_kind[(kd == (int)OP_MLP || kd == (int)OP_SWIN_ATTN) ? 0 : kd] += ms;
-  }
-  double fl = 0.0; int nc = 0;
-  for (const Op& op : p->ops) if (op.kind == OP_MLP) {
-    fl += 4.0 * (double)op.mlp.in.N * op.mlp.in.H * op.mlp.in.W * op.mlp.E * (double)op.mlp.Hd;
-    ++nc;
-  } else if (op.kind == OP_CONV) {
-    const ConvParams& c = op.conv.prm;
-    const int cin_real = op.conv.in.tens == p->xin.tens ? p->e->cfg.in_channels + p->e->lq_feat_ch() : op.conv.in.C;
-    fl += 2.0 * (double)c.Nimg * c.Hout * c.Wout * c.Cout * (double)c.num_taps * cin_real;
-    ++nc;
-  } else if (op.kind == OP_SWIN_ATTN) {
-    // per token: qkv 2 E 3E + proj 2 E E + (QK^T + PV over the 64 keys of its window) 4 * 64 * E
-    const double M = (double)op.swin.x.N * op.swin.x.H * op.swin.x.W, Ed = (double)op.swin.x.C;
-    fl += M * (8.0 * Ed * Ed + 256.0 * Ed);
-    ++nc;
+    int family = 0;          // GEMM kernels (FLOPs counted), GroupNorm, attention, resample
+    switch (kind_of(op)) {
+      case OP_CONV: {
+        const ConvDesc& d = payload<ConvOp>(op).d;
+        const ConvParams& c = d.prm;
+        const int cin_real = d.in.tens == p->xin.tens ? p->e->cfg.in_channels + p->e->lq_feat_ch() : d.in.C;
+        fl += 2.0 * (double)c.Nimg * c.Hout * c.Wout * c.Cout * (double)c.num_taps * cin_real;
+        break;
+      }
+      case OP_MLP: { const MlpDesc& m = payload<MlpOp>(op).d; fl += 4.0 * (double)m.in.N * m.in.H * m.in.W * m.E * (double)m.Hd; break; }
+      case OP_SWIN_ATTN: {   // a GEMM kernel: per token qkv 2 E 3E + proj 2 E E + (QK^T + PV over the 64 keys of its window) 4 * 64 * E
+        const View& xv = payload<SwinOp>(op).d.x;
+        fl += (double)xv.N * xv.H * xv.W * (8.0 * xv.C * xv.C + 256.0 * xv.C);
+        break;
+      }
+      case OP_GN: family = 1; break;
+      case OP_ATTN: case OP_SOFTMAX: case OP_VQ_ATTN: family = 2; break;    // (no softmax / VQ-GAN attention in a denoiser)
+      case OP_UPSAMPLE: family = 3; break;
+    }
+    ms_by_kind[family] += ms;
+    nc += family == 0;
   }
   if (conv_flops) *conv_flops = fl;
   if (n_conv_launches) *n_conv_launches = nc;
@@ -1334,41 +1358,41 @@ int rs_plan_profile(rs_plan* p, const float* x, const float* timesteps, const fl
 
 // per-operator times + one-line descriptions of a profiled run_ops() pass
 static void collect_profile(const rs_plan& P, const Prof& prof, double* ms, char* desc, int desc_stride, int cap, int32_t* n_ops) {
-  const rs_plan* p = &P;
-  const int n = std::min<int>((int)p->ops.size(), cap);
+  const int n = std::min<int>((int)P.ops.size(), cap);
   *n_ops = n;
   for (int i = 0; i < n; ++i) {
     float t = 0.f;
     cudaEventElapsedTime(&t, prof.ev[2 * i], prof.ev[2 * i + 1]);
     ms[i] = t;
-    const Op& op = p->ops[i];
+    const Op& op = P.ops[i];
     char* d = desc + (size_t)i * desc_stride;
-    if (op.kind == OP_CONV) {
-      const ConvParams& c = op.conv.prm;
-      snprintf(d, desc_stride, "conv%dx%d s%d %dx%d Cin=%d Cout=%d grid=%d BN=%d st=%d %s cg=%d ms=%d sk=%d box=%dx%dx%d "
-               "N=%d persist=%d pad=%d act=%d res=%d f32=%d",
-               op.conv.ksize, op.conv.ksize, op.conv.stride, c.Hout, c.Wout, op.conv.in.C, c.Cout, op.conv.grid, c.BN, c.stages,
-               op.w_name.c_str(), c.cg, c.msub, c.splitk, c.bw, c.bh, c.bn, c.Nimg, c.persist, op.conv.pad_lo, op.conv.act,
-               (int)op.conv.has_res, (int)(op.conv.out_f32 != nullptr));
-    } else if (op.kind == OP_GN) {
-      snprintf(d, desc_stride, "gn %dx%d C=%d fused=%d %s", op.gn.in.H, op.gn.in.W, op.gn.in.C, (int)op.gn.fused, op.g_name.c_str());
-    } else if (op.kind == OP_MLP) {
-      snprintf(d, desc_stride, "mlp %dx%d E=%d Hd=%d grid=%d", op.mlp.in.H, op.mlp.in.W, op.mlp.E, op.mlp.Hd, op.mlp.grid);
-    } else if (op.kind == OP_ATTN) {
-      snprintf(d, desc_stride, "attn %dx%d window=%d shift=%d", op.a_in.H, op.a_in.W, op.a_window, op.a_shift);
-    } else if (op.kind == OP_SWIN_ATTN) {
-      snprintf(d, desc_stride, "swin_attn %dx%d shift=%d grid=%d", op.swin.x.H, op.swin.x.W, op.swin.shift, op.swin.grid);
-    } else if (op.kind == OP_SOFTMAX) {
-      snprintf(d, desc_stride, "softmax %d", op.s_view.C);
-    } else if (op.kind == OP_VQ_ATTN) {
-      // the query-row range only when it is not all T rows (the default launch keeps its description)
-      const VqAttnDesc& a = op.vqa;
-      if (a.row_begin == 0 && a.row_end == a.prm.T)
-        snprintf(d, desc_stride, "vq_attn T=%d C=%d N=%d", a.prm.T, a.q.C, a.q.N);
-      else
-        snprintf(d, desc_stride, "vq_attn T=%d C=%d N=%d rows=%d:%d", a.prm.T, a.q.C, a.q.N, a.row_begin, a.row_end);
-    } else {
-      snprintf(d, desc_stride, "%s %dx%d C=%d", op.u_pool ? "avgpool" : "upsample", op.u_in.H, op.u_in.W, op.u_in.C);
+    switch (kind_of(op)) {
+      case OP_CONV: {
+        const ConvDesc& cd = payload<ConvOp>(op).d;
+        const ConvParams& c = cd.prm;
+        snprintf(d, desc_stride, "conv%dx%d s%d %dx%d Cin=%d Cout=%d grid=%d BN=%d st=%d %s cg=%d ms=%d sk=%d box=%dx%dx%d "
+                 "N=%d persist=%d pad=%d act=%d res=%d f32=%d",
+                 cd.ksize, cd.ksize, cd.stride, c.Hout, c.Wout, cd.in.C, c.Cout, cd.grid, c.BN, c.stages,
+                 payload<ConvOp>(op).w_name.c_str(), c.cg, c.msub, c.splitk, c.bw, c.bh, c.bn, c.Nimg, c.persist, cd.pad_lo,
+                 cd.act, (int)cd.has_res, (int)(cd.out_f32 != nullptr));
+        break;
+      }
+      case OP_GN: {
+        const GnLink& g = payload<GnOp>(op).stats;
+        snprintf(d, desc_stride, "gn %dx%d C=%d fused=%d %s", g.in.H, g.in.W, g.in.C, (int)g.fused, payload<GnOp>(op).name.c_str());
+        break;
+      }
+      case OP_MLP: { const MlpDesc& m = payload<MlpOp>(op).d; snprintf(d, desc_stride, "mlp %dx%d E=%d Hd=%d grid=%d", m.in.H, m.in.W, m.E, m.Hd, m.grid); break; }
+      case OP_ATTN: { const WinAttnOp& a = payload<WinAttnOp>(op); snprintf(d, desc_stride, "attn %dx%d window=%d shift=%d", a.qkv.H, a.qkv.W, a.window, a.shift); break; }
+      case OP_SWIN_ATTN: { const SwinAttnDesc& w = payload<SwinOp>(op).d; snprintf(d, desc_stride, "swin_attn %dx%d shift=%d grid=%d", w.x.H, w.x.W, w.shift, w.grid); break; }
+      case OP_SOFTMAX: snprintf(d, desc_stride, "softmax %d", payload<SoftmaxOp>(op).view.C); break;
+      case OP_VQ_ATTN: {     // the query-row range only when it is not all T rows (the default launch keeps its description)
+        const VqAttnDesc& a = payload<VqAttnDesc>(op);
+        if (a.row_begin == 0 && a.row_end == a.prm.T) snprintf(d, desc_stride, "vq_attn T=%d C=%d N=%d", a.prm.T, a.q.C, a.q.N);
+        else snprintf(d, desc_stride, "vq_attn T=%d C=%d N=%d rows=%d:%d", a.prm.T, a.q.C, a.q.N, a.row_begin, a.row_end);
+        break;
+      }
+      case OP_UPSAMPLE: { const ResampleOp& r = payload<ResampleOp>(op); snprintf(d, desc_stride, "%s %dx%d C=%d", r.pool ? "avgpool" : "upsample", r.in.H, r.in.W, r.in.C); break; }
     }
   }
 }
@@ -1377,14 +1401,9 @@ static void collect_profile(const rs_plan& P, const Prof& prof, double* ms, char
 int rs_plan_profile_ops(rs_plan* p, const float* x, const float* timesteps, const float* lq, const float* mask,
                         double* ms, char* desc, int desc_stride, int cap, int32_t* n_ops, void* stream) {
   RS_CHECK(p && p->bound && ms && desc && n_ops, "bad argument");
-  int rc = check_plan_device(*p); if (rc) return rc;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  p->table_owner = nullptr;
-  rc = run_embedding(*p, timesteps, p->B, st); if (rc) return rc;
-  rc = pack_lq_and_input(*p, x, lq, mask, nullptr, 0, st); if (rc) return rc;
   Prof prof;
-  const float* film = reinterpret_cast<const float*>(p->ws + p->off_film);
-  rc = run_ops(*p, p->ops, film, p->e->film_rows, st, &prof); if (rc) return rc;
+  int rc = run_forward(*p, x, timesteps, lq, mask, st, &prof); if (rc) return rc;
   RS_CUDA_OK(cudaStreamSynchronize(st));
   collect_profile(*p, prof, ms, desc, desc_stride, cap, n_ops);
   return 0;
@@ -1492,7 +1511,7 @@ extern "C" {
 
 int rs_sampler_create(rs_plan* p, int steps, const double* sqrt_etas, double kappa, const int32_t* tmap, rs_sampler** out) {
   RS_CHECK(p && p->bound && sqrt_etas && out, "bad argument (plan must be bound)");
-  RS_CHECK(p->vq_which < 0, "samplers are built on denoiser plans");
+  RS_CHECK(p->pass == Pass::Denoiser, std::string("samplers are built on denoiser plans: this plan belongs to ") + kind_name(p->e->kind));
   RS_CHECK(steps >= 2 && steps <= p->max_rows && steps <= 1024, "steps out of range for this plan");
   auto s = std::make_unique<rs_sampler>();
   s->p = p; s->T = steps; s->kappa = kappa;

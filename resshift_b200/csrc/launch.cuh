@@ -312,6 +312,20 @@ inline TileConfig conv_preview_config(int N, int Hin, int Win, int Cin, int Cout
   return pick_tile_config(m_tiles, (Cout + 15) / 16 * 16, num_kb, env_int("RS_CONV_BN", 0), sp);
 }
 
+// The statistics sinks a producer's kernel receives: the set ones of `sink` first; an unset `expected` becomes slots (the
+// producer's pair slots per image) x cstride, an unset eps GroupNorm32's 1e-5
+inline void compact_sinks(const GnSink (&sink)[2], int slots, GnSink (&out)[2]) {
+  out[0] = GnSink{}; out[1] = GnSink{};
+  int k = 0;
+  for (const GnSink& s : sink) {
+    if (!s.part) continue;
+    out[k] = s;
+    if (out[k].expected == 0) out[k].expected = (unsigned)(slots * s.cstride);
+    if (out[k].eps == 0.f) out[k].eps = 1e-5f;
+    ++k;
+  }
+}
+
 inline int conv_finalize(ConvDesc& d) {
   ConvParams& p = d.prm;
   std::memset(&p, 0, sizeof(p));
@@ -434,21 +448,7 @@ inline int conv_finalize(ConvDesc& d) {
   }
   p.gn_slots = p.tiles_w * p.tiles_h;
   RS_CHECK(!(d.sink[0].part || d.sink[1].part) || p.bn <= 2, "fused GroupNorm statistics need tiles of at most two images");
-  auto fill_sinks = [&](GnSink* dst) {
-    int k = 0;
-    for (int i = 0; i < 2; ++i) {
-      dst[i] = GnSink{};
-      if (!d.sink[i].part) continue;
-      dst[k] = d.sink[i];
-      if (dst[k].expected == 0) dst[k].expected = (unsigned)(p.gn_slots * dst[k].cstride);
-      if (dst[k].eps == 0.f) dst[k].eps = 1e-5f;
-      ++k;
-    }
-  };
-  {
-    GnSink none[2] = {};
-    if (p.tma_out) fill_sinks(p.sink); else { p.sink[0] = none[0]; p.sink[1] = none[1]; }
-  }
+  if (p.tma_out) compact_sinks(d.sink, p.gn_slots, p.sink);
   if (p.splitk > 1) {
     // the conv kernel only produces fp32 partial sums; bias / activation / residual / fp16 store / GroupNorm statistics
     // happen in the reduce kernel, one CTA per (128-pixel slot, image)
@@ -459,7 +459,7 @@ inline int conv_finalize(ConvDesc& d) {
     if (d.has_res) { r.residual = d.res.ptr; r.res_sN = d.res.sN(); r.res_ld = d.res.ld; }
     r.out = d.out.ptr; r.out_sN = d.out.sN(); r.out_ld = d.out.ld;
     r.rows_per_slot = p.bw * p.bh; r.slots = p.tiles_w * p.tiles_h;
-    fill_sinks(r.sink);
+    compact_sinks(d.sink, p.gn_slots, r.sink);
     RS_CHECK(d.Cout % 8 == 0 && d.Cout <= 2048, "split-K reduce needs Cout % 8 == 0");
     p.bias = nullptr; p.residual = nullptr; p.act = ACT_NONE; p.sink[0] = GnSink{}; p.sink[1] = GnSink{};
     d.red_grid_x = r.slots;
@@ -566,7 +566,6 @@ struct GnDesc {
   float eps = 1e-5f;
   int slots = 0;
   bool fused = false;     // statistics already delivered by the producing kernels' epilogues
-  bool win_slots = false; // the producer is the fused Swin attention kernel: one slot per 8x8 window (64 values each)
   bool finalize_kernel = false;   // fused statistics with many slots: reduce part -> gstat with gn_finalize_kernel first
 };
 
@@ -685,17 +684,7 @@ inline int mlp_finalize(MlpDesc& d) {
   RS_CHECK(!(d.gn_in_gstat || d.gn_in_part) || (d.gn_in_gamma && d.gn_in_beta && d.Hd >= 4 * d.E && d.E % 32 == 0),
            "fused MLP: input GroupNorm arguments");
   p.gn_slots = p.tiles_w * p.tiles_h;
-  {
-    int k = 0;
-    p.sink[0] = GnSink{}; p.sink[1] = GnSink{};
-    for (int i = 0; i < 2; ++i) {
-      if (!d.sink[i].part) continue;
-      p.sink[k] = d.sink[i];
-      if (p.sink[k].expected == 0) p.sink[k].expected = (unsigned)(p.gn_slots * p.sink[k].cstride);
-      if (p.sink[k].eps == 0.f) p.sink[k].eps = 1e-5f;
-      ++k;
-    }
-  }
+  compact_sinks(d.sink, p.gn_slots, p.sink);
   return 0;
 }
 
@@ -746,19 +735,12 @@ inline int swin_attn_finalize(SwinAttnDesc& d) {
   p.wqkv = d.wqkv; p.wqkv_ld = d.wqkv_ld; p.bqkv = d.bqkv; p.relbias = d.relbias;
   p.wproj = d.wproj; p.wproj_ld = d.wproj_ld; p.bproj = d.bproj;
   p.total_windows = d.x.N * (d.x.H / 8) * (d.x.W / 8);
-  {
-    int k = 0;
-    for (int i = 0; i < 2; ++i) {
-      if (!d.sink[i].part) continue;
-      p.sink[k] = d.sink[i];
-      if (p.sink[k].expected == 0) p.sink[k].expected = (unsigned)((d.x.H / 8) * (d.x.W / 8) * p.sink[k].cstride);
-      if (p.sink[k].eps == 0.f) p.sink[k].eps = 1e-5f;
-      ++k;
-    }
-  }
+  // the kernel's epilogue writes one (mean, M2) pair per 8x8 window of 64 tokens, not per 128-pixel conv tile: its
+  // slots are windows
+  const int nW = (d.x.H / 8) * (d.x.W / 8);
+  compact_sinks(d.sink, nW, p.sink);
   const int pairs = (p.total_windows + 1) / 2;
   d.grid = std::min(pairs, num_sms());
-  const int nW = (d.x.H / 8) * (d.x.W / 8);
   for (int k = 0; k < 2; ++k) {
     d.fin[k] = GnFinalizeParams{};
     if (p.sink[k].gstat) {
