@@ -69,6 +69,27 @@ typedef struct rs_unet_options {
   int32_t patch_norm;             /* 1: GroupNorm32 after patch_embed.proj and patch_unembed.proj              */
 } rs_unet_options;
 
+/* Keyword arguments of UNetModel.__init__ (reference models/unet.py:373-393), the global-attention UNet.  x has
+ * out_channels channels; the LQ image (3 channels) is concatenated to it, so in_channels - out_channels is 3 (lq at
+ * the latent size) or 12 (lq at twice the latent size, through F.pixel_unshuffle(lq, 2), :569-573).  num_heads /
+ * num_head_channels as in the reference (num_head_channels -1: num_heads heads; output blocks then have ONE head, since
+ * the reference builds them without num_heads, :517-523).  Refused by rs_unetmodel_create, with the reason in the
+ * message: head dims other than 32, 64 or 128, channel counts GroupNorm32 cannot split, any other in_channels. */
+typedef struct rs_unetmodel_config {
+  int32_t image_size;
+  int32_t in_channels;
+  int32_t model_channels;
+  int32_t out_channels;
+  int32_t n_levels;
+  int32_t channel_mult[RS_MAX_LEVELS];
+  int32_t num_res_blocks[RS_MAX_LEVELS];
+  int32_t n_attn;
+  int32_t attention_resolutions[RS_MAX_LEVELS];
+  int32_t num_heads;
+  int32_t num_head_channels;
+  int32_t use_new_attention_order;
+} rs_unetmodel_config;
+
 /* ``autoencoder.params`` of the shipped yaml files: VQModelTorch(ddconfig, n_embed, embed_dim)
  * (reference ldm/models/autoencoder.py:12-26; ddconfig -> ldm/modules/diffusionmodules/model.py:452-470,563-581).
  * Covered: double_z = False, attn_resolutions = [], dropout = 0 (every shipped config). */
@@ -94,6 +115,11 @@ const char* rs_last_error(void);
 /* ---- denoiser: models.unet.UNetModelSwin (reference models/unet.py:603-912) ------------------ */
 int rs_unet_create(const rs_unet_config* cfg, rs_engine** out);
 int rs_unet_create_ex(const rs_unet_config* cfg, const rs_unet_options* opts, rs_engine** out);
+/* models.unet.UNetModel (reference models/unet.py:346-601).  opts: use_scale_shift_norm, resblock_updown and
+ * conv_resample as for UNetModelSwin; patch_norm must be 0.  The engine works with every entry point below
+ * (parameters, plans, forward / profile / probe, samplers); rs_plan_forward's lq is [B, 3, H, W] or [B, 3, 2H, 2W]
+ * as in_channels says, and mask must be NULL.  Its AttentionBlocks run unet_attn (rs_op_unet_attention). */
+int rs_unetmodel_create(const rs_unetmodel_config* cfg, const rs_unet_options* opts, rs_engine** out);
 void rs_unet_destroy(rs_engine* e);
 /* state_dict inventory (reference key names / shapes; utils/util_net.py:86-98 relies on them) */
 int rs_unet_param_count(const rs_engine* e);
@@ -310,7 +336,12 @@ int rs_op_vq_attention(const void* q, const void* k, const void* v, int N, int T
  * out is written, so ranges computed on different devices and copied together equal one full call. */
 int rs_op_vq_attention_rows(const void* q, const void* k, const void* v, int N, int T, int C, int ld, int row_begin,
                             int row_end, void* out, void* stream);
-/* row softmax of the same attention for H*W <= 8192, in place on the fp16 score matrix: s[r][0:cols] =
+/* multi-head attention over all T positions of each image, out = softmax(q k^T head_dim^-1/2) v per head (reference
+ * models/unet.py:265-344, QKVAttentionLegacy / QKVAttention between the qkv conv and proj_out).  qkv fp16 [N][T][3C]
+ * dense, C = heads * head_dim, split legacy-order (per head: q, k, v) or, with new_order, qkv-first (q | k | v, each
+ * [heads][head_dim]); out fp16 [N][T][C] dense.  head_dim 32, 64 or 128, any T >= 1; deterministic, one launch. */
+int rs_op_unet_attention(const void* qkv, int N, int T, int heads, int head_dim, int new_order, void* out, void* stream);
+/* row softmax of the VQ-GAN attention above for H*W <= 8192, in place on the fp16 score matrix: s[r][0:cols] =
  * softmax(scale * s[r][0:cols]) for each of `rows` rows with row stride ld (elements); what lies beyond cols in a row is
  * not touched.  Needs rows >= 1, cols a multiple of 8 in [8, 8192], ld >= cols and a multiple of 8, s 16-byte aligned;
  * anything else returns an error. */

@@ -37,6 +37,17 @@ class UNetOptionsC(C.Structure):
                 ("patch_norm", C.c_int32)]
 
 
+class UNetModelConfigC(C.Structure):
+    """Mirror of ``rs_unetmodel_config``."""
+    _fields_ = [
+        ("image_size", C.c_int32), ("in_channels", C.c_int32), ("model_channels", C.c_int32),
+        ("out_channels", C.c_int32), ("n_levels", C.c_int32),
+        ("channel_mult", C.c_int32 * RS_MAX_LEVELS), ("num_res_blocks", C.c_int32 * RS_MAX_LEVELS),
+        ("n_attn", C.c_int32), ("attention_resolutions", C.c_int32 * RS_MAX_LEVELS),
+        ("num_heads", C.c_int32), ("num_head_channels", C.c_int32), ("use_new_attention_order", C.c_int32),
+    ]
+
+
 class VQConfigC(C.Structure):
     """Mirror of ``rs_vq_config``."""
     _fields_ = [
@@ -66,6 +77,7 @@ _SIGNATURES = {
     "rs_last_error": (C.c_char_p, []),
     "rs_unet_create": (C.c_int, [C.POINTER(UNetConfigC), C.POINTER(_P)]),
     "rs_unet_create_ex": (C.c_int, [C.POINTER(UNetConfigC), C.POINTER(UNetOptionsC), C.POINTER(_P)]),
+    "rs_unetmodel_create": (C.c_int, [C.POINTER(UNetModelConfigC), C.POINTER(UNetOptionsC), C.POINTER(_P)]),
     "rs_unet_destroy": (None, [_P]),
     "rs_unet_param_count": (C.c_int, [_P]),
     "rs_unet_param_info": (C.c_int, [_P, C.c_int, C.c_char_p, C.c_size_t, C.POINTER(C.c_int32), C.POINTER(C.c_int32),
@@ -113,7 +125,8 @@ _SIGNATURES = {
     "rs_op_expand_relpos_ex": (C.c_int, [_P, _P, C.c_int, C.c_int, _P]),
     "rs_op_vq_attention": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P]),
     "rs_op_vq_attention_rows": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P]),
-    "rs_op_softmax_rows": (C.c_int, [_P, C.c_int, C.c_int, C.c_longlong, C.c_float, _P]),
+    "rs_op_unet_attention": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P]),
+    "rs_op_softmax_rows":(C.c_int, [_P, C.c_int, C.c_int, C.c_longlong, C.c_float, _P]),
     "rs_op_window_attention": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P, _P]),
     "rs_op_window_attention_ex": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P, _P]),
     "rs_op_swin_attn": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, C.c_int, _P, _P, _P, _P, _P, _P, _P,
@@ -206,8 +219,24 @@ def make_config(cfg) -> UNetConfigC:
 def make_options(cfg) -> UNetOptionsC:
     o = UNetOptionsC()
     o.use_scale_shift_norm, o.resblock_updown = int(cfg.use_scale_shift_norm), int(cfg.resblock_updown)
-    o.conv_resample, o.patch_norm = int(cfg.conv_resample), int(cfg.patch_norm)
+    o.conv_resample, o.patch_norm = int(cfg.conv_resample), int(getattr(cfg, "patch_norm", False))
     return o
+
+
+def make_unetmodel_config(cfg) -> UNetModelConfigC:
+    c = UNetModelConfigC()
+    c.image_size, c.in_channels, c.model_channels, c.out_channels = cfg.image_size, cfg.in_channels, cfg.model_channels, cfg.out_channels
+    c.n_levels = len(cfg.channel_mult)
+    for i, v in enumerate(cfg.channel_mult):
+        c.channel_mult[i] = int(v)
+    for i, v in enumerate(cfg.num_res_blocks):
+        c.num_res_blocks[i] = int(v)
+    c.n_attn = len(cfg.attention_resolutions)
+    for i, v in enumerate(cfg.attention_resolutions):
+        c.attention_resolutions[i] = int(v)
+    c.num_heads, c.num_head_channels = cfg.num_heads, cfg.num_head_channels
+    c.use_new_attention_order = int(cfg.use_new_attention_order)
+    return c
 
 
 def make_vq_config(cfg) -> VQConfigC:

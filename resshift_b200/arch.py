@@ -21,7 +21,7 @@ from __future__ import annotations
 
 from typing import List, Tuple
 
-from .config import UNetConfig
+from .config import UNetConfig, UNetModelConfig
 
 Spec = Tuple[str, Tuple[int, ...], str]
 
@@ -59,9 +59,12 @@ def swin_geometry(cfg: UNetConfig, res: int) -> Tuple[int, int]:
     return cfg.window_size, cfg.window_size // 2
 
 
-def latent_multiple(cfg: UNetConfig) -> int:
-    """What H and W of a latent must be multiples of: every level's map (H / 2^level) is tiled by that level's window."""
+def latent_multiple(cfg) -> int:
+    """What H and W of a latent must be multiples of: every level's map (H / 2^level) is tiled by that level's window
+    (UNetModel: the levels only have to halve evenly)."""
     import math
+    if isinstance(cfg, UNetModelConfig):
+        return 2 ** (len(cfg.channel_mult) - 1)
     m = 1
     for level in range(len(cfg.channel_mult)):
         m = math.lcm(m, swin_geometry(cfg, cfg.image_size >> level)[0] << level)
@@ -170,6 +173,85 @@ def unet_param_spec(cfg: UNetConfig) -> List[Spec]:
                 out += _conv(f"{prefix}.{j}.op", layer[1], layer[1], 3)
             elif kind == "up" and cfg.conv_resample:
                 out += _conv(f"{prefix}.{j}.conv", layer[1], layer[1], 3)
+        return out
+
+    for i, layers in enumerate(input_blocks):
+        s += emit(f"input_blocks.{i}", layers)
+    s += emit("middle_block", middle)
+    for i, layers in enumerate(output_blocks):
+        s += emit(f"output_blocks.{i}", layers)
+    ch0 = int(cfg.channel_mult[0] * cfg.model_channels)
+    s += _gn("out.0", ch0)
+    s += _conv("out.2", ch0, cfg.out_channels, 3)
+    return s
+
+
+def unetmodel_block_plan(cfg: UNetModelConfig):
+    """Topology of UNetModel (reference models/unet.py:426-541) in the form of ``unet_block_plan``, with
+    ``("attn", c, heads)`` for an AttentionBlock: one after EVERY ResBlock of an attention level, and in the middle."""
+    down = "res_down" if cfg.resblock_updown else "down"
+    up = "res_up" if cfg.resblock_updown else "up"
+    mc = cfg.model_channels
+    ch = int(cfg.channel_mult[0] * mc)
+    input_blocks = [[("conv", cfg.in_channels, ch)]]
+    chans = [ch]
+    ds = cfg.image_size
+    for level, mult in enumerate(cfg.channel_mult):
+        for _ in range(cfg.num_res_blocks[level]):
+            layers = [("res", ch, int(mult * mc))]
+            ch = int(mult * mc)
+            if ds in cfg.attention_resolutions:
+                layers.append(("attn", ch, cfg.heads(ch, False)))
+            input_blocks.append(layers)
+            chans.append(ch)
+        if level != len(cfg.channel_mult) - 1:
+            input_blocks.append([(down, ch)])
+            chans.append(ch)
+            ds //= 2
+    middle = [("res", ch, ch), ("attn", ch, cfg.heads(ch, False)), ("res", ch, ch)]
+    output_blocks = []
+    for level, mult in list(enumerate(cfg.channel_mult))[::-1]:
+        for i in range(cfg.num_res_blocks[level] + 1):
+            ich = chans.pop()
+            layers = [("res", ch + ich, int(mc * mult))]
+            ch = int(mc * mult)
+            if ds in cfg.attention_resolutions:
+                layers.append(("attn", ch, cfg.heads(ch, True)))
+            if level and i == cfg.num_res_blocks[level]:
+                layers.append((up, ch))
+                ds *= 2
+            output_blocks.append(layers)
+    return input_blocks, middle, output_blocks
+
+
+def unetmodel_param_spec(cfg: UNetModelConfig) -> List[Spec]:
+    """UNetModel's ``state_dict`` (reference models/unet.py:416-547); AttentionBlock :246-255 (qkv / proj_out are conv1d
+    weights [O, I, 1])."""
+    emb = cfg.time_embed_dim
+    s: List[Spec] = []
+    s += _linear("time_embed.0", cfg.model_channels, emb)
+    s += _linear("time_embed.2", emb, emb)
+    input_blocks, middle, output_blocks = unetmodel_block_plan(cfg)
+
+    def emit(prefix: str, layers):
+        out: List[Spec] = []
+        for j, layer in enumerate(layers):
+            kind, p = layer[0], f"{prefix}.{j}"
+            if kind == "conv":
+                out += _conv(p, layer[1], layer[2], 3)
+            elif kind == "res":
+                out += _resblock(p, layer[1], layer[2], emb, cfg.use_scale_shift_norm)
+            elif kind in ("res_down", "res_up"):
+                out += _resblock(p, layer[1], layer[1], emb, cfg.use_scale_shift_norm)
+            elif kind == "attn":
+                c = layer[1]
+                out += _gn(f"{p}.norm", c)
+                out += [(f"{p}.qkv.weight", (3 * c, c, 1), "conv1"), (f"{p}.qkv.bias", (3 * c,), "bias")]
+                out += [(f"{p}.proj_out.weight", (c, c, 1), "conv1"), (f"{p}.proj_out.bias", (c,), "bias")]
+            elif kind == "down" and cfg.conv_resample:
+                out += _conv(f"{p}.op", layer[1], layer[1], 3)
+            elif kind == "up" and cfg.conv_resample:
+                out += _conv(f"{p}.conv", layer[1], layer[1], 3)
         return out
 
     for i, layers in enumerate(input_blocks):

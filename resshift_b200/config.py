@@ -98,6 +98,88 @@ class UNetConfig:
 
 
 @dataclass
+class UNetModelConfig:
+    """Exactly the keyword arguments of ``UNetModel.__init__`` (reference models/unet.py:373-393), the global-attention
+    UNet.  What the native kernels cannot run is refused here with the reason."""
+    image_size: int = 64
+    in_channels: int = 6
+    model_channels: int = 160
+    out_channels: int = 3
+    num_res_blocks: Sequence[int] = (2, 2, 2, 2)
+    attention_resolutions: Sequence[int] = (64, 32, 16, 8)
+    cond_lq: bool = True
+    dropout: float = 0.0
+    channel_mult: Sequence[int] = (1, 2, 4, 8)
+    conv_resample: bool = True
+    dims: int = 2
+    num_classes: Optional[int] = None
+    use_fp16: bool = False
+    num_heads: int = 1
+    num_head_channels: int = -1
+    use_scale_shift_norm: bool = False
+    resblock_updown: bool = False
+    use_new_attention_order: bool = False
+
+    def __post_init__(self):
+        if isinstance(self.num_res_blocks, int):
+            self.num_res_blocks = (self.num_res_blocks,) * len(self.channel_mult)
+        self.num_res_blocks = tuple(int(v) for v in self.num_res_blocks)
+        self.channel_mult = tuple(int(v) for v in self.channel_mult)
+        self.attention_resolutions = tuple(int(v) for v in self.attention_resolutions)
+        if len(self.num_res_blocks) != len(self.channel_mult):
+            raise ValueError("num_res_blocks and channel_mult must have the same length")
+        if self.dims != 2:
+            raise ValueError(f"dims={self.dims}: only 2-D UNets are covered (every ResShift config uses dims=2)")
+        if self.num_classes is not None:
+            raise ValueError("num_classes: class-conditional UNetModel is not covered (the ResShift sampler never passes "
+                             "labels, so the reference's own `y is not None` assert would fire)")
+        if not self.cond_lq:
+            raise ValueError("cond_lq=False: the ResShift sampler always passes lq, and the reference asserts cond_lq then")
+        if self.in_channels - self.out_channels not in (3, 12):
+            raise ValueError(f"in_channels={self.in_channels}, out_channels={self.out_channels}: x has out_channels "
+                             f"channels and lq is a 3-channel image, so in_channels must be out_channels + 3 (lq at the "
+                             f"latent size) or out_channels + 12 (lq at twice it, through pixel_unshuffle)")
+        if self.model_channels % 32:
+            raise ValueError(f"model_channels={self.model_channels}: GroupNorm32 needs channel counts divisible by 32")
+        for ch, output_block in self.attention_layers():
+            heads = self.heads(ch, output_block)
+            if heads <= 0 or ch % heads or ch // heads not in (32, 64, 128):
+                where = "an output block" if output_block else "an input / the middle block"
+                raise ValueError(f"AttentionBlock of {where} over {ch} channels with {heads} head(s): the attention kernel "
+                                 f"is instantiated for head dims 32, 64 and 128; set num_head_channels to 32, 64 or 128 "
+                                 f"(with num_head_channels=-1 output blocks have one head over all their channels)")
+
+    def heads(self, ch: int, output_block: bool) -> int:
+        """AttentionBlock heads (reference :239-245); output blocks are built without num_heads (:517-523)."""
+        if self.num_head_channels != -1:
+            return ch // self.num_head_channels
+        return 1 if output_block else self.num_heads
+
+    def attention_layers(self):
+        """(channels, in an output block) of every AttentionBlock."""
+        from .arch import unetmodel_block_plan
+        ins, mid, outs = unetmodel_block_plan(self)
+        return ([(l[1], False) for b in ins + [mid] for l in b if l[0] == "attn"]
+                + [(l[1], True) for b in outs for l in b if l[0] == "attn"])
+
+    @property
+    def lq_factor(self) -> int:
+        """1: lq enters at the latent size; 2: at twice it, through F.pixel_unshuffle(lq, 2) (reference :569-573)."""
+        return 2 if self.in_channels - self.out_channels == 12 else 1
+
+    @property
+    def time_embed_dim(self) -> int:
+        return self.model_channels * 4
+
+    def to_kwargs(self) -> dict:
+        d = asdict(self)
+        d["num_res_blocks"] = list(self.num_res_blocks)
+        d["channel_mult"] = list(self.channel_mult)
+        d["attention_resolutions"] = list(self.attention_resolutions)
+        return d
+
+
+@dataclass
 class DiffusionConfig:
     normalize_input: bool = True
     schedule_name: str = "exponential"

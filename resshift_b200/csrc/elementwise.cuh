@@ -23,6 +23,7 @@ struct PackInputParams {
   const __half* lq_nhwc; int lq_ld;   // [N*H*W, Cl] fp16 or nullptr
   __half* out; int Cpad;              // [N*H*W, Cpad]
   int N, HW;
+  int lq_unshuffle, W;                // 1: lq_nchw is [N, Cl / 4, 2H, 2W], packed as F.pixel_unshuffle(lq, 2) (channel 4c + 2dy + dx)
   unsigned int* zero_ptr; int zero_n; // GroupNorm arrival counters of the forward that follows (gn_stats.cuh): reset here
 };
 
@@ -39,7 +40,12 @@ __global__ void pack_input_kernel(const PackInputParams p) {
   __half* o = p.out + pix * p.Cpad;
   int c = 0;
   for (; c < p.Cx; ++c) o[c] = __float2half_rn(p.x[((long long)n * p.Cx + c) * p.HW + hw] * sc);
-  if (p.lq_nchw) {
+  if (p.lq_nchw && p.lq_unshuffle) {
+    const int y = hw / p.W, xx = hw % p.W;
+    const long long W2 = 2LL * p.W, plane = 4LL * p.HW;
+    for (int j = 0; j < p.Cl; ++j, ++c)
+      o[c] = __float2half_rn(p.lq_nchw[((long long)n * (p.Cl / 4) + j / 4) * plane + (2 * y + ((j >> 1) & 1)) * W2 + 2 * xx + (j & 1)]);
+  } else if (p.lq_nchw) {
     for (int j = 0; j < p.Cl; ++j, ++c) o[c] = __float2half_rn(p.lq_nchw[((long long)n * p.Cl + j) * p.HW + hw]);
     if (p.mask_nchw) o[c++] = __float2half_rn(p.mask_nchw[(long long)n * p.HW + hw]);
   } else if (p.lq_nhwc) {

@@ -65,6 +65,10 @@ struct rs_engine {
   rs_vq_config vq{};
   rs_unet_config cfg;
   rs_unet_options opt{1, 0, 1, 0};
+  // UNetModel (rs_unetmodel_create): global-attention blocks instead of Swin layers, no feature extractor; cfg then holds
+  // its levels with in_channels = out_channels (the channels of x) and lq_size = image_size
+  bool unetmodel = false;
+  rs_unetmodel_config um{};
   std::vector<Param> params;
   std::map<std::string, int> index;
   size_t arena_bytes = 0;
@@ -84,7 +88,17 @@ struct rs_engine {
     return s;
   }
   int lq_in_ch() const { return cfg.cond_mask ? 4 : 3; }
-  int lq_feat_ch() const { return fe_stages() == 0 ? lq_in_ch() : 16 << fe_stages(); }
+  int lq_feat_ch() const {
+    if (unetmodel) return um.in_channels - um.out_channels;
+    return fe_stages() == 0 ? lq_in_ch() : 16 << fe_stages();
+  }
+  // UNetModel: the LQ image enters at the latent size (1) or at twice it through pixel_unshuffle (2)
+  int lq_factor() const { return unetmodel && lq_feat_ch() == 4 * lq_in_ch() ? 2 : 1; }
+  // heads of a UNetModel AttentionBlock over ch channels; output blocks are built without num_heads (unet.py:517-523)
+  int attn_heads(int ch, bool output_block) const {
+    if (um.num_head_channels != -1) return ch / um.num_head_channels;
+    return output_block ? 1 : um.num_heads;
+  }
   bool has_attn(int ds) const {
     for (int i = 0; i < cfg.n_attn; ++i) if (cfg.attention_resolutions[i] == ds) return true;
     return false;
@@ -110,8 +124,9 @@ struct rs_engine {
 namespace {
 
 // kind: 0 conv(cin,cout) 1 res(cin,cout) 2 swin(c,res) 3 down(c) 4 up(c) 5 res with down=True(c) 6 res with up=True(c)
+// 7 UNetModel AttentionBlock(c,heads)
 struct Layer { int kind; int a, b; };
-enum { L_CONV = 0, L_RES, L_SWIN, L_DOWN, L_UP, L_RES_DOWN, L_RES_UP };
+enum { L_CONV = 0, L_RES, L_SWIN, L_DOWN, L_UP, L_RES_DOWN, L_RES_UP, L_ATTN };
 struct Topology {
   std::vector<std::vector<Layer>> input_blocks, output_blocks;
   std::vector<Layer> middle;
@@ -126,11 +141,18 @@ Topology build_topology(const rs_engine& e) {
   t.input_blocks.push_back({{0, c.in_channels + e.lq_feat_ch(), ch}});
   std::vector<int> chans{ch};
   int ds = c.image_size;
+  // UNetModel (reference models/unet.py:426-541): an AttentionBlock after EVERY ResBlock of an attention level; the
+  // Swin UNet puts a BasicLayer after the first one only
+  auto add_attn = [&](std::vector<Layer>& layers, int jj, int chn, bool output_block) {
+    if (!e.has_attn(ds)) return;
+    if (e.unetmodel) layers.push_back({L_ATTN, chn, e.attn_heads(chn, output_block)});
+    else if (jj == 0) layers.push_back({L_SWIN, chn, ds});
+  };
   for (int level = 0; level < c.n_levels; ++level) {
     for (int jj = 0; jj < c.num_res_blocks[level]; ++jj) {
       std::vector<Layer> layers{{1, ch, c.channel_mult[level] * mc}};
       ch = c.channel_mult[level] * mc;
-      if (e.has_attn(ds) && jj == 0) layers.push_back({2, ch, ds});
+      add_attn(layers, jj, ch, false);
       t.input_blocks.push_back(layers);
       chans.push_back(ch);
     }
@@ -141,13 +163,13 @@ Topology build_topology(const rs_engine& e) {
     }
   }
   t.in_block_ch = chans;
-  t.middle = {{1, ch, ch}, {2, ch, ds}, {1, ch, ch}};
+  t.middle = {{1, ch, ch}, {e.unetmodel ? L_ATTN : L_SWIN, ch, e.unetmodel ? e.attn_heads(ch, false) : ds}, {1, ch, ch}};
   for (int level = c.n_levels - 1; level >= 0; --level) {
     for (int i = 0; i <= c.num_res_blocks[level]; ++i) {
       const int ich = chans.back(); chans.pop_back();
       std::vector<Layer> layers{{1, ch + ich, mc * c.channel_mult[level]}};
       ch = mc * c.channel_mult[level];
-      if (e.has_attn(ds) && i == 0) layers.push_back({2, ch, ds});
+      add_attn(layers, i, ch, true);
       if (level && i == c.num_res_blocks[level]) { layers.push_back({e.opt.resblock_updown ? L_RES_UP : L_UP, ch, ch}); ds *= 2; }
       t.output_blocks.push_back(layers);
     }
@@ -212,6 +234,13 @@ void add_layers(rs_engine& e, const std::string& prefix, const std::vector<Layer
         add_conv(e, b + ".mlp.fc1", E, hidden, 1);
         add_conv(e, b + ".mlp.fc2", hidden, E, 1);
       }
+    } else if (L.kind == L_ATTN) {
+      // AttentionBlock (reference models/unet.py:230-255): qkv and proj_out are conv1d weights [O, I, 1], packed as 1x1 convs
+      add_gn(e, p + ".norm", L.a);
+      add_param(e, p + ".qkv.weight", {3 * L.a, L.a, 1}, R_CONV1);
+      add_param(e, p + ".qkv.bias", {3 * L.a}, R_BIAS);
+      add_param(e, p + ".proj_out.weight", {L.a, L.a, 1}, R_CONV1);
+      add_param(e, p + ".proj_out.bias", {L.a}, R_BIAS);
     } else if (L.kind == L_DOWN) {
       if (e.opt.conv_resample) add_conv(e, p + ".op", L.a, L.a, 3);
     } else if (L.kind == L_UP) {
@@ -276,7 +305,7 @@ int build_inventory(rs_engine& e) {
     switch (p.role) {
       case R_CONV3: case R_CONV1:
         p.ipad = (p.shape[1] + 7) / 8 * 8;
-        p.bytes = (size_t)p.shape[0] * p.shape[2] * p.shape[3] * p.ipad * 2; break;
+        p.bytes = (size_t)p.shape[0] * (p.shape.size() == 4 ? p.shape[2] * p.shape[3] : 1) * p.ipad * 2; break;   // (conv1d [O, I, 1])
       case R_LINEAR:
         p.ipad = (p.shape[1] + 7) / 8 * 8;
         p.bytes = (size_t)p.shape[0] * p.ipad * 2; break;
@@ -342,12 +371,13 @@ struct SwinOp : Producer { SwinAttnDesc d; std::string blk; GnLink norm1; };
 struct SoftmaxOp { View view; float scale = 1.f; };         // in place on view [rows = N*H*W][cols = C]
 
 // an op is its kind's payload and nothing else: the alternatives follow OpKind
-enum OpKind { OP_CONV, OP_GN, OP_ATTN, OP_UPSAMPLE, OP_MLP, OP_SOFTMAX, OP_SWIN_ATTN, OP_VQ_ATTN };
-using OpPayload = std::variant<ConvOp, GnOp, WinAttnOp, ResampleOp, MlpOp, SoftmaxOp, SwinOp, VqAttnDesc>;
+enum OpKind { OP_CONV, OP_GN, OP_ATTN, OP_UPSAMPLE, OP_MLP, OP_SOFTMAX, OP_SWIN_ATTN, OP_VQ_ATTN, OP_UNET_ATTN };
+using OpPayload = std::variant<ConvOp, GnOp, WinAttnOp, ResampleOp, MlpOp, SoftmaxOp, SwinOp, VqAttnDesc, UnetAttnDesc>;
 template <OpKind K, typename T> constexpr bool payload_of = std::is_same_v<std::variant_alternative_t<K, OpPayload>, T>;
-static_assert(std::variant_size_v<OpPayload> == OP_VQ_ATTN + 1 && payload_of<OP_CONV, ConvOp> && payload_of<OP_GN, GnOp> &&
+static_assert(std::variant_size_v<OpPayload> == OP_UNET_ATTN + 1 && payload_of<OP_CONV, ConvOp> && payload_of<OP_GN, GnOp> &&
               payload_of<OP_ATTN, WinAttnOp> && payload_of<OP_UPSAMPLE, ResampleOp> && payload_of<OP_MLP, MlpOp> &&
-              payload_of<OP_SOFTMAX, SoftmaxOp> && payload_of<OP_SWIN_ATTN, SwinOp> && payload_of<OP_VQ_ATTN, VqAttnDesc>);
+              payload_of<OP_SOFTMAX, SoftmaxOp> && payload_of<OP_SWIN_ATTN, SwinOp> && payload_of<OP_VQ_ATTN, VqAttnDesc> &&
+              payload_of<OP_UNET_ATTN, UnetAttnDesc>);
 using Op = OpPayload;
 inline OpKind kind_of(const Op& op) { return static_cast<OpKind>(op.index()); }
 // the payload of an op of kind T (read under that kind's case only)
@@ -664,6 +694,22 @@ struct Builder {
     return 0;
   }
 
+  // AttentionBlock of UNetModel (reference models/unet.py:257-263): out = x + proj_out(attention(qkv(norm(x)))) as four
+  // launches; norm takes its statistics from x's producers, proj_out's epilogue delivers those of out to its consumers
+  void unet_attn_block(const View& x, const std::string& p, int heads, const View& out) {
+    View n = P.make_view(x.N, x.H, x.W, x.C);
+    gn(x, p + ".norm", n, 0, -1);
+    View qkv = P.make_view(x.N, x.H, x.W, 3 * x.C);
+    conv(n, p + ".qkv", 1, 1, 3 * x.C, &qkv, nullptr, ACT_NONE);
+    View a = P.make_view(x.N, x.H, x.W, x.C);
+    UnetAttnDesc op;
+    op.qkv = qkv; op.out = a; op.heads = heads; op.new_order = E.um.use_new_attention_order != 0;
+    const int i = opi();
+    P.touch(qkv, i); P.touch(a, i);
+    cur->push_back(std::move(op));
+    conv(a, p + ".proj_out", 1, 1, x.C, &out, &x, ACT_NONE);
+  }
+
   int run_block(View h, const std::string& prefix, const std::vector<Layer>& layers, const View& dest, View* result) {
     for (size_t j = 0; j < layers.size(); ++j) {
       const Layer& L = layers[j];
@@ -679,6 +725,9 @@ struct Builder {
       } else if (L.kind == L_SWIN) {
         out = last ? dest : P.make_view(h.N, h.H, h.W, h.C);
         int rc = basic_layer(h, p, L.b, out); if (rc) return rc;
+      } else if (L.kind == L_ATTN) {
+        out = last ? dest : P.make_view(h.N, h.H, h.W, h.C);
+        unet_attn_block(h, p, L.b, out);
       } else if (L.kind == L_RES_DOWN || L.kind == L_RES_UP) {     // always the last layer of its block
         out = dest;
         res_block(h, p, L.a, out, L.kind == L_RES_DOWN ? -1 : 1);
@@ -767,7 +816,7 @@ int build_plan(rs_plan& P) {
 
   // ---- feature extractor (reference models/unet.py:689-702), hoisted out of the sampling loop ----
   const int fes = E.fe_stages();
-  P.lqH = P.H << fes; P.lqW = P.W << fes;
+  P.lqH = (P.H << fes) * E.lq_factor(); P.lqW = (P.W << fes) * E.lq_factor();
   if (fes > 0) {
     b.cur = &P.fe_ops;
     P.fe_cpad = 8;
@@ -978,6 +1027,12 @@ int bind_ops(rs_plan& P, std::vector<Op>& ops) {
         rc = vq_attn_finalize(a);
         break;
       }
+      case OP_UNET_ATTN: {
+        UnetAttnDesc& a = payload<UnetAttnDesc>(op);
+        resolve(P, a.qkv); resolve(P, a.out);
+        rc = unet_attn_finalize(a);
+        break;
+      }
     }
     if (rc) return rc;
     P.launches += launches;
@@ -996,7 +1051,7 @@ struct Prof {
 };
 
 // RS_SKIP_KINDS (timing ablation only — results are garbage): bit 0 conv3x3, 1 conv1x1 / linear, 2 GroupNorm, 3 attention
-// (window, fused Swin, fused VQ-GAN), 4 upsample, 5 fused MLP.  The time a kernel family really costs inside the graph-replayed step is the
+// (window, fused Swin, fused VQ-GAN, UNetModel), 4 upsample, 5 fused MLP.  The time a kernel family really costs inside the graph-replayed step is the
 // difference between the full step and the step without it (per-launch events over-state small kernels).
 inline bool op_skipped(const Op& op) {
   static const int skip = env_int("RS_SKIP_KINDS", 0);
@@ -1004,7 +1059,7 @@ inline bool op_skipped(const Op& op) {
   switch (kind_of(op)) {
     case OP_CONV: return (skip >> (payload<ConvOp>(op).d.ksize == 3 ? 0 : 1)) & 1;
     case OP_GN: return (skip >> 2) & 1;
-    case OP_ATTN: case OP_SWIN_ATTN: case OP_VQ_ATTN: return (skip >> 3) & 1;
+    case OP_ATTN: case OP_SWIN_ATTN: case OP_VQ_ATTN: case OP_UNET_ATTN: return (skip >> 3) & 1;
     case OP_UPSAMPLE: return (skip >> 4) & 1;
     case OP_MLP: return (skip >> 5) & 1;
     case OP_SOFTMAX: return false;
@@ -1040,6 +1095,7 @@ int run_op_range(rs_plan& P, const Op* first, const Op* last, const float* film_
       case OP_MLP: rc = mlp_launch(payload<MlpOp>(op).d, st); break;
       case OP_SWIN_ATTN: rc = swin_attn_launch(payload<SwinOp>(op).d, st); break;
       case OP_VQ_ATTN: rc = vq_attn_launch(payload<VqAttnDesc>(op), st); break;
+      case OP_UNET_ATTN: rc = unet_attn_launch(payload<UnetAttnDesc>(op), st); break;
       case OP_ATTN: {
         const WinAttnOp& a = payload<WinAttnOp>(op);
         rc = attn_launch(a.qkv, a.out, a.bias, P.e->cfg.swin_heads, P.e->cfg.swin_embed_dim, a.window, a.shift, st);
@@ -1113,10 +1169,13 @@ int pack_lq_and_input(rs_plan& P, const float* x, const float* lq, const float* 
     int rc = run_ops(P, P.fe_ops, nullptr, 0, st); if (rc) return rc;
     pp.lq_nhwc = P.lq_feat.ptr; pp.lq_ld = P.lq_feat.ld; pp.Cl = P.lq_feat.C;
   } else {
-    // no feature extractor: cat([x, lq, mask]) straight into the packed input (reference models/unet.py:876-882)
+    // no feature extractor: cat([x, lq, mask]) straight into the packed input (reference models/unet.py:876-882); a
+    // UNetModel's lq at twice the latent size goes through pixel_unshuffle(lq, 2) on the way (:569-573)
     RS_CHECK(!c.cond_mask || mask != nullptr, "this model is mask-conditioned: mask must be given");
-    pp.lq_nchw = lq; pp.Cl = 3;
+    RS_CHECK(!E.unetmodel || mask == nullptr, "UNetModel.forward takes no mask");
+    pp.lq_nchw = lq; pp.Cl = E.unetmodel ? E.lq_feat_ch() : 3;
     pp.mask_nchw = c.cond_mask ? mask : nullptr;
+    pp.lq_unshuffle = E.lq_factor() == 2; pp.W = P.W;
   }
   (void)launch_k(pack_input_kernel, dim3((unsigned)((npix + 255) / 256)), dim3(256), (size_t)(0), st, pp);
   RS_CUDA_OK(cudaGetLastError());
@@ -1176,6 +1235,47 @@ int rs_unet_create_ex(const rs_unet_config* cfg, const rs_unet_options* opts, rs
 int rs_unet_create(const rs_unet_config* cfg, rs_engine** out) {
   const rs_unet_options shipped{1, 0, 1, 0};
   return rs_unet_create_ex(cfg, &shipped, out);
+}
+int rs_unetmodel_create(const rs_unetmodel_config* cfg, const rs_unet_options* opts, rs_engine** out) {
+  RS_CHECK(cfg && opts && out, "null argument");
+  RS_CHECK(cfg->n_levels >= 1 && cfg->n_levels <= RS_MAX_LEVELS && cfg->n_attn >= 0 && cfg->n_attn <= RS_MAX_LEVELS, "n_levels / n_attn");
+  RS_CHECK(opts->patch_norm == 0, "UNetModel has no patch norm: rs_unet_options.patch_norm must be 0");
+  for (int v : {opts->use_scale_shift_norm, opts->resblock_updown, opts->conv_resample})
+    RS_CHECK(v == 0 || v == 1, "rs_unet_options fields are 0 or 1");
+  RS_CHECK(cfg->use_new_attention_order == 0 || cfg->use_new_attention_order == 1, "use_new_attention_order is 0 or 1");
+  RS_CHECK(cfg->out_channels > 0 && (cfg->in_channels - cfg->out_channels == 3 || cfg->in_channels - cfg->out_channels == 12),
+           "in_channels must be out_channels + 3 (lq at the latent size) or out_channels + 12 (lq at twice the latent size, "
+           "pixel_unshuffle): x has out_channels channels and lq is a 3-channel image");
+  RS_CHECK(cfg->num_head_channels == -1 || cfg->num_head_channels > 0, "num_head_channels is -1 or positive");
+  RS_CHECK(cfg->num_head_channels != -1 || cfg->num_heads > 0, "num_heads must be positive");
+  RS_CHECK(cfg->model_channels > 0 && cfg->model_channels % 32 == 0, "GroupNorm32 needs model_channels % 32 == 0");
+  for (int l = 0; l < cfg->n_levels; ++l)
+    RS_CHECK(cfg->channel_mult[l] > 0 && cfg->num_res_blocks[l] >= 0, "channel_mult / num_res_blocks");
+  auto e = std::make_unique<rs_engine>();
+  e->unetmodel = true;
+  e->um = *cfg;
+  e->opt = *opts;
+  rs_unet_config& c = e->cfg;
+  std::memset(&c, 0, sizeof(c));
+  c.image_size = cfg->image_size; c.in_channels = cfg->out_channels; c.model_channels = cfg->model_channels;
+  c.out_channels = cfg->out_channels; c.n_levels = cfg->n_levels; c.n_attn = cfg->n_attn; c.lq_size = cfg->image_size;
+  for (int l = 0; l < RS_MAX_LEVELS; ++l) {
+    c.channel_mult[l] = cfg->channel_mult[l]; c.num_res_blocks[l] = cfg->num_res_blocks[l];
+    c.attention_resolutions[l] = cfg->attention_resolutions[l];
+  }
+  // every AttentionBlock's head dim must have a unet_attn instance (the output blocks' single heads included)
+  Topology t = build_topology(*e);
+  std::vector<Layer> all = t.middle;
+  for (const std::vector<Layer>& blk : t.input_blocks) all.insert(all.end(), blk.begin(), blk.end());
+  for (const std::vector<Layer>& blk : t.output_blocks) all.insert(all.end(), blk.begin(), blk.end());
+  for (const Layer& L : all)
+    RS_CHECK(L.kind != L_ATTN || (L.b > 0 && L.a % L.b == 0 && unet_attn_head_dim_ok(L.a / L.b)),
+             "an AttentionBlock over " + std::to_string(L.a) + " channels with " + std::to_string(L.b) +
+             " head(s): the attention kernel is instantiated for head dims 32, 64 and 128; set num_head_channels to "
+             "32, 64 or 128 (with num_head_channels -1, output blocks have one head over all their channels)");
+  int rc = build_inventory(*e); if (rc) return rc;
+  *out = e.release();
+  return 0;
 }
 void rs_unet_destroy(rs_engine* e) { delete e; }
 int rs_unet_param_count(const rs_engine* e) { return e ? (int)e->params.size() : 0; }
@@ -1253,14 +1353,16 @@ int rs_plan_create(rs_engine* e, int batch, int height, int width, rs_plan** out
   RS_CHECK(e->kind == EngineKind::Denoiser, std::string("this engine is ") + kind_name(e->kind) + ": use rs_vq_plan_create");
   // every level's H and W must be multiples of that level's window (the constructor-time rule: the level's nominal
   // resolution where that is not larger than window_size, else window_size)
+  // (a UNetModel's levels only need to halve evenly)
   int mult = 1;
   for (int l = 0; l < e->cfg.n_levels; ++l) {
     const int res = e->cfg.image_size >> l;
-    mult = std::lcm(mult, (res <= e->cfg.window_size ? res : e->cfg.window_size) << l);
+    mult = e->unetmodel ? 1 << l : std::lcm(mult, (res <= e->cfg.window_size ? res : e->cfg.window_size) << l);
   }
   RS_CHECK(height % mult == 0 && width % mult == 0,
-           "latent H and W must be multiples of " + std::to_string(mult) + " for this model: each level's window (at most "
-           "window_size) times the level's downsampling (64 for the shipped configs)");
+           "latent H and W must be multiples of " + std::to_string(mult) + " for this model: " +
+           (e->unetmodel ? std::string("2^(levels - 1)") : std::string("each level's window (at most window_size) times the "
+                                                                          "level's downsampling (64 for the shipped configs)")));
   auto p = std::make_unique<rs_plan>();
   p->e = e; p->B = batch; p->H = height; p->W = width;
   int rc = build_plan(*p); if (rc) return rc;
@@ -1345,7 +1447,7 @@ int rs_plan_profile(rs_plan* p, const float* x, const float* timesteps, const fl
         break;
       }
       case OP_GN: family = 1; break;
-      case OP_ATTN: case OP_SOFTMAX: case OP_VQ_ATTN: family = 2; break;    // (no softmax / VQ-GAN attention in a denoiser)
+      case OP_ATTN: case OP_SOFTMAX: case OP_VQ_ATTN: case OP_UNET_ATTN: family = 2; break;    // (no softmax / VQ-GAN attention in a denoiser)
       case OP_UPSAMPLE: family = 3; break;
     }
     ms_by_kind[family] += ms;
@@ -1393,6 +1495,12 @@ static void collect_profile(const rs_plan& P, const Prof& prof, double* ms, char
         break;
       }
       case OP_UPSAMPLE: { const ResampleOp& r = payload<ResampleOp>(op); snprintf(d, desc_stride, "%s %dx%d C=%d", r.pool ? "avgpool" : "upsample", r.in.H, r.in.W, r.in.C); break; }
+      case OP_UNET_ATTN: {
+        const UnetAttnDesc& a = payload<UnetAttnDesc>(op);
+        snprintf(d, desc_stride, "unet_attn T=%d heads=%d D=%d N=%d order=%s", a.prm.T, a.heads, a.out.C / a.heads, a.qkv.N,
+                 a.new_order ? "new" : "legacy");
+        break;
+      }
     }
   }
 }

@@ -18,6 +18,7 @@
 #include "window_attn.cuh"
 #include "swin_attn_fused.cuh"
 #include "vq_attn.cuh"
+#include "unet_attn.cuh"
 
 namespace rs {
 
@@ -523,6 +524,9 @@ inline int conv_init() {
     RS_CUDA_OK(cudaFuncSetAttribute(vq_attn_sm90_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, VqAttnSmem<128>::launch_bytes));
     RS_CUDA_OK(cudaFuncSetAttribute(vq_attn_sm90_kernel<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, VqAttnSmem<256>::launch_bytes));
     RS_CUDA_OK(cudaFuncSetAttribute(vq_attn_sm90_kernel<512>, cudaFuncAttributeMaxDynamicSharedMemorySize, VqAttnSmem<512>::launch_bytes));
+    RS_CUDA_OK(cudaFuncSetAttribute(unet_attn_sm90_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, UnetAttnSmem<32>::launch_bytes));
+    RS_CUDA_OK(cudaFuncSetAttribute(unet_attn_sm90_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, UnetAttnSmem<64>::launch_bytes));
+    RS_CUDA_OK(cudaFuncSetAttribute(unet_attn_sm90_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, UnetAttnSmem<128>::launch_bytes));
     attr_set[dev].store(true, std::memory_order_release);
   }
   return 0;
@@ -814,6 +818,46 @@ inline int vq_attn_launch(const VqAttnDesc& d, cudaStream_t st) {
     case 256: (void)launch_k(vq_attn_sm90_kernel<256>, grid, dim3(kVqAttnThreads), (size_t)VqAttnSmem<256>::launch_bytes, st, d.prm); break;
     case 512: (void)launch_k(vq_attn_sm90_kernel<512>, grid, dim3(kVqAttnThreads), (size_t)VqAttnSmem<512>::launch_bytes, st, d.prm); break;
     default: RS_CHECK(false, "fused VQ-GAN attention: C in {128, 256, 512}");
+  }
+  RS_CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+// ---- multi-head attention over all positions of a level (unet_attn.cuh): UNetModel's AttentionBlock -----------------
+struct UnetAttnDesc {
+  View qkv, out;                           // [N, H, W, 3C] (the qkv conv's output), [N, H, W, C]
+  int heads = 1;
+  bool new_order = false;                  // QKVAttention (split qkv, then heads) instead of QKVAttentionLegacy
+  UnetAttnParams prm;
+};
+inline bool unet_attn_head_dim_ok(int D) { return D == 32 || D == 64 || D == 128; }
+inline int unet_attn_finalize(UnetAttnDesc& d) {
+  UnetAttnParams& p = d.prm;
+  std::memset(&p, 0, sizeof(p));
+  const int N = d.qkv.N, C = d.out.C;
+  const long long T = (long long)d.qkv.H * d.qkv.W;
+  RS_CHECK(d.heads > 0 && C % d.heads == 0 && unet_attn_head_dim_ok(C / d.heads),
+           "UNetModel attention: head dim (channels / heads) must be 32, 64 or 128");
+  const int D = C / d.heads;
+  RS_CHECK(d.qkv.C == 3 * C && d.out.N == N && (long long)d.out.H * d.out.W == T, "UNetModel attention: qkv [N, T, 3C] -> out [N, T, C]");
+  RS_CHECK(T >= 1 && T <= (1LL << 30) && N >= 1 && N <= 65535 && d.heads <= 65535, "UNetModel attention: T >= 1, batch and heads <= 65535");
+  RS_CHECK(d.qkv.ptr && d.out.ptr && d.qkv.ld % 8 == 0 && d.out.ld % 2 == 0 && d.out.ld >= C, "UNetModel attention: views");
+  p.out = d.out.ptr; p.out_sN = d.out.sN(); p.out_ld = d.out.ld;
+  p.T = (int)T;
+  p.head_stride = d.new_order ? D : 3 * D;
+  p.k_col0 = d.new_order ? C : D;
+  p.v_col0 = d.new_order ? 2 * C : 2 * D;
+  p.scale_log2 = (float)(1.4426950408889634 / std::sqrt((double)D));
+  return encode_act_map(&p.tm, d.qkv.ptr, 3 * C, (int)T, 1, N, d.qkv.ld, T * d.qkv.ld, d.qkv.sN(), kUnetAttnBK, 1, 1, 64);
+}
+inline int unet_attn_launch(const UnetAttnDesc& d, cudaStream_t st) {
+  const long long T = (long long)d.qkv.H * d.qkv.W;
+  const dim3 grid((unsigned)((T + kUnetAttnCtaRows - 1) / kUnetAttnCtaRows), (unsigned)d.heads, (unsigned)d.qkv.N);
+  switch (d.out.C / d.heads) {
+    case 32: (void)launch_k(unet_attn_sm90_kernel<32>, grid, dim3(kUnetAttnThreads), (size_t)UnetAttnSmem<32>::launch_bytes, st, d.prm); break;
+    case 64: (void)launch_k(unet_attn_sm90_kernel<64>, grid, dim3(kUnetAttnThreads), (size_t)UnetAttnSmem<64>::launch_bytes, st, d.prm); break;
+    case 128: (void)launch_k(unet_attn_sm90_kernel<128>, grid, dim3(kUnetAttnThreads), (size_t)UnetAttnSmem<128>::launch_bytes, st, d.prm); break;
+    default: RS_CHECK(false, "UNetModel attention: head dim 32, 64 or 128");
   }
   RS_CUDA_OK(cudaGetLastError());
   return 0;

@@ -23,7 +23,7 @@ import torch
 import torch.nn.functional as F
 
 from .. import _lib
-from .unet import UNetModelSwin
+from .unet import UNetModel, UNetModelSwin
 
 
 class ModelMeanType(enum.Enum):
@@ -205,7 +205,7 @@ class ResShiftDiffusion:
 
     # ------------------------------------------------------------------ the loop
     def _native_ok(self, model, clip_denoised, denoised_fn, model_kwargs) -> bool:
-        return (isinstance(model, UNetModelSwin) and self.model_mean_type == ModelMeanType.START_X
+        return (isinstance(model, (UNetModelSwin, UNetModel)) and self.model_mean_type == ModelMeanType.START_X
                 and not clip_denoised and denoised_fn is None and self.normalize_input and self.latent_flag
                 and model_kwargs is not None and "lq" in model_kwargs
                 and 2 <= self.num_timesteps <= 64)       # rs_sampler_create: 2 <= T <= FiLM-table rows of a plan
@@ -213,15 +213,20 @@ class ResShiftDiffusion:
     @staticmethod
     def _check_native_inputs(model: UNetModelSwin, z_y, lq, mask):
         """Same contract as UNetModelSwin.forward (reference models/unet.py:865-882 asserts `mask is not None` iff
-        cond_mask): the library receives raw pointers, so every shape is checked here."""
+        cond_mask; UNetModel.forward takes no mask and its lq is at the latent size or twice it, :569-573): the library
+        receives raw pointers, so every shape is checked here."""
         cfg = model.cfg
         B, Cc, H, W = z_y.shape
-        if Cc != cfg.in_channels:
-            raise ValueError(f"latent has {Cc} channels, the model expects {cfg.in_channels}")
-        exp_lq = (B, 3, H << cfg.fe_stages, W << cfg.fe_stages)
+        latent_ch = cfg.out_channels if isinstance(model, UNetModel) else cfg.in_channels
+        if Cc != latent_ch:
+            raise ValueError(f"latent has {Cc} channels, the model expects {latent_ch}")
+        exp_lq = model.lq_shape(B, H, W)
         if tuple(lq.shape) != exp_lq:
             raise ValueError(f"lq must have shape {exp_lq}, got {tuple(lq.shape)}")
-        if cfg.cond_mask:
+        if isinstance(model, UNetModel):
+            if mask is not None:
+                raise ValueError("UNetModel takes no mask (its forward has no mask parameter)")
+        elif cfg.cond_mask:
             if mask is None:
                 raise ValueError("this model is mask-conditioned (cond_mask=True): pass model_kwargs['mask']")
             exp_m = (B, 1) + exp_lq[2:]

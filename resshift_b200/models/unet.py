@@ -1,6 +1,6 @@
-"""``UNetModelSwin`` — same constructor, ``state_dict`` and call surface as the reference's
-``models.unet.UNetModelSwin`` (reference models/unet.py:603-912), with the forward pass executed by
-the sm_90a kernels of ``librs_b200.so`` through the C ABI (include/resshift_b200.h).
+"""``UNetModelSwin`` and ``UNetModel`` — same constructors, ``state_dict`` and call surface as the reference's
+``models.unet.UNetModelSwin`` (reference models/unet.py:603-912) and ``models.unet.UNetModel`` (:346-601), with the
+forward pass executed by the sm_90a kernels of ``librs_b200.so`` through the C ABI (include/resshift_b200.h).
 
 PyTorch owns every allocation (parameters, packed-weight arena, workspace, outputs); the library only
 enqueues kernels on the current CUDA stream.  There is no eager / CPU fallback: calling the module
@@ -15,8 +15,8 @@ import torch
 import torch.nn as nn
 
 from .. import _lib
-from ..arch import latent_multiple, unet_param_spec, relative_position_index, shifted_window_mask
-from ..config import UNetConfig
+from ..arch import latent_multiple, unet_param_spec, unetmodel_param_spec
+from ..config import UNetConfig, UNetModelConfig
 from ..weights import random_state_dict
 
 
@@ -24,28 +24,15 @@ class _Node(nn.Module):
     """Anonymous container; only there so that ``state_dict`` keys match the reference's."""
 
 
-class UNetModelSwin(nn.Module):
-    def __init__(self, image_size, in_channels, model_channels, out_channels, num_res_blocks,
-                 attention_resolutions, dropout=0, channel_mult=(1, 2, 4, 8), conv_resample=True, dims=2,
-                 use_fp16=False, num_heads=1, num_head_channels=-1, use_scale_shift_norm=False,
-                 resblock_updown=False, swin_depth=2, swin_embed_dim=96, window_size=8, mlp_ratio=2.0,
-                 patch_norm=False, cond_lq=True, cond_mask=False, lq_size=256):
-        super().__init__()
-        self.cfg = UNetConfig(
-            image_size=image_size, in_channels=in_channels, model_channels=model_channels,
-            out_channels=out_channels, num_res_blocks=num_res_blocks,
-            attention_resolutions=tuple(attention_resolutions), dropout=dropout, channel_mult=tuple(channel_mult),
-            conv_resample=conv_resample, dims=dims, use_fp16=use_fp16, num_heads=num_heads,
-            num_head_channels=num_head_channels, use_scale_shift_norm=use_scale_shift_norm,
-            resblock_updown=resblock_updown, swin_depth=swin_depth, swin_embed_dim=swin_embed_dim,
-            window_size=window_size, mlp_ratio=mlp_ratio, patch_norm=patch_norm, cond_lq=cond_lq,
-            cond_mask=cond_mask, lq_size=lq_size)
-        # attributes the reference exposes
-        self.image_size, self.in_channels, self.model_channels = image_size, in_channels, model_channels
-        self.out_channels, self.cond_lq, self.cond_mask = out_channels, cond_lq, cond_mask
-        self.dtype = torch.float32
+class _NativeDenoiser(nn.Module):
+    """What both denoisers share: parameters registered under the reference's names, the native engine, its packed
+    weight arena, and one plan (workspace) per (batch, H, W).  Subclasses set ``cfg`` and define ``_create_engine``,
+    ``_latent_rule``, ``lq_shape`` and ``forward``."""
 
-        self._spec = unet_param_spec(self.cfg)
+    _ZEROED: Tuple[str, ...] = ()         # parameters the reference's zero_module zeroes (name suffixes)
+
+    def _register_params(self, spec):
+        self._spec = spec
         init = random_state_dict(self.cfg, seed=0)
         for name, shape, role in self._spec:
             *path, leaf = name.split(".")
@@ -58,8 +45,8 @@ class UNetModelSwin(nn.Module):
             if role.startswith("buf_"):
                 node.register_buffer(leaf, value)
             else:
-                if name.endswith("out_layers.3.weight") or name.endswith("out_layers.3.bias"):
-                    value = torch.zeros_like(value)         # zero_module (reference models/unet.py:172-174)
+                if name.endswith(self._ZEROED):
+                    value = torch.zeros_like(value)
                 node.register_parameter(leaf, nn.Parameter(value))
 
         # native state (created lazily on the first CUDA call)
@@ -71,11 +58,10 @@ class UNetModelSwin(nn.Module):
     # ------------------------------------------------------------------ native plumbing
     def _ensure_engine(self, device: torch.device):
         if device.type != "cuda":
-            raise RuntimeError("resshift_b200.UNetModelSwin runs on CUDA only (no CPU fallback); call .cuda() first")
+            raise RuntimeError(f"resshift_b200.{type(self).__name__} runs on CUDA only (no CPU fallback); call .cuda() first")
         if self._engine is None:
             h = C.c_void_p()
-            cfgc, optc = _lib.make_config(self.cfg), _lib.make_options(self.cfg)
-            _lib.check(_lib.lib.rs_unet_create_ex(C.byref(cfgc), C.byref(optc), C.byref(h)))
+            self._create_engine(h)
             self._engine = h
             n = _lib.lib.rs_unet_param_count(h)
             mine = sorted(name for name, _, _ in self._spec)
@@ -121,9 +107,9 @@ class UNetModelSwin(nn.Module):
     def plan(self, batch: int, height: int, width: int) -> "_Plan":
         mult = latent_multiple(self.cfg)
         if height % mult or width % mult:
-            raise ValueError(f"latent {height}x{width}: H and W must be multiples of {mult} for this model (each level's "
-                             f"window, at most window_size={self.cfg.window_size}, times the level's downsampling); "
-                             f"ResShiftSampler pads to multiples of padding_offset, which must be a multiple of {mult}")
+            raise ValueError(f"latent {height}x{width}: H and W must be multiples of {mult} for this model "
+                             f"({self._latent_rule()}); ResShiftSampler pads to multiples of padding_offset, which must "
+                             f"be a multiple of {mult}")
         device = next(self.parameters()).device
         self._ensure_engine(device)
         self.pack_weights()
@@ -135,22 +121,16 @@ class UNetModelSwin(nn.Module):
     def num_launches(self, batch, height, width) -> int:
         return _lib.lib.rs_plan_num_launches(self.plan(batch, height, width).handle)
 
-    # ------------------------------------------------------------------ reference call surface
-    @torch.no_grad()
-    def forward(self, x, timesteps, lq=None, mask=None):
-        """x [N, C, H, W]; timesteps [N]; lq [N, 3, h, w]; mask [N, 1, h, w] or None -> [N, out_ch, H, W] fp32
-        (reference models/unet.py:865-895; the reference returns fp16 under autocast, this returns fp32)."""
-        if lq is None:
-            raise ValueError("UNetModelSwin is LQ-conditioned (cond_lq=True in every shipped config): pass lq=")
+    def _run_forward(self, x, timesteps, lq, mask):
         if x.device.type != "cuda":
-            raise RuntimeError("resshift_b200.UNetModelSwin.forward needs CUDA tensors (no CPU fallback)")
+            raise RuntimeError(f"resshift_b200.{type(self).__name__}.forward needs CUDA tensors (no CPU fallback)")
         n, _, h, w = x.shape
         plan = self.plan(n, h, w)
         xf = x.detach().float().contiguous()
         tf = timesteps.detach().to(device=x.device, dtype=torch.float32).contiguous()
         lqf = lq.detach().float().contiguous()
         mf = mask.detach().float().contiguous() if mask is not None else None
-        exp_lq = (n, 3, h << self.cfg.fe_stages, w << self.cfg.fe_stages)
+        exp_lq = self.lq_shape(n, h, w)
         if tuple(lqf.shape) != exp_lq:
             raise ValueError(f"lq must have shape {exp_lq}, got {tuple(lqf.shape)}")
         out = torch.empty(n, self.cfg.out_channels, h, w, dtype=torch.float32, device=x.device)
@@ -183,10 +163,102 @@ class UNetModelSwin(nn.Module):
             pass
 
 
+class UNetModelSwin(_NativeDenoiser):
+    _ZEROED = ("out_layers.3.weight", "out_layers.3.bias")     # zero_module (reference models/unet.py:172-174)
+
+    def __init__(self, image_size, in_channels, model_channels, out_channels, num_res_blocks,
+                 attention_resolutions, dropout=0, channel_mult=(1, 2, 4, 8), conv_resample=True, dims=2,
+                 use_fp16=False, num_heads=1, num_head_channels=-1, use_scale_shift_norm=False,
+                 resblock_updown=False, swin_depth=2, swin_embed_dim=96, window_size=8, mlp_ratio=2.0,
+                 patch_norm=False, cond_lq=True, cond_mask=False, lq_size=256):
+        super().__init__()
+        self.cfg = UNetConfig(
+            image_size=image_size, in_channels=in_channels, model_channels=model_channels,
+            out_channels=out_channels, num_res_blocks=num_res_blocks,
+            attention_resolutions=tuple(attention_resolutions), dropout=dropout, channel_mult=tuple(channel_mult),
+            conv_resample=conv_resample, dims=dims, use_fp16=use_fp16, num_heads=num_heads,
+            num_head_channels=num_head_channels, use_scale_shift_norm=use_scale_shift_norm,
+            resblock_updown=resblock_updown, swin_depth=swin_depth, swin_embed_dim=swin_embed_dim,
+            window_size=window_size, mlp_ratio=mlp_ratio, patch_norm=patch_norm, cond_lq=cond_lq,
+            cond_mask=cond_mask, lq_size=lq_size)
+        # attributes the reference exposes
+        self.image_size, self.in_channels, self.model_channels = image_size, in_channels, model_channels
+        self.out_channels, self.cond_lq, self.cond_mask = out_channels, cond_lq, cond_mask
+        self.dtype = torch.float32
+        self._register_params(unet_param_spec(self.cfg))
+
+    def _create_engine(self, handle):
+        cfgc, optc = _lib.make_config(self.cfg), _lib.make_options(self.cfg)
+        _lib.check(_lib.lib.rs_unet_create_ex(C.byref(cfgc), C.byref(optc), C.byref(handle)))
+
+    def _latent_rule(self) -> str:
+        return f"each level's window, at most window_size={self.cfg.window_size}, times the level's downsampling"
+
+    def lq_shape(self, n, h, w):
+        return (n, 3, h << self.cfg.fe_stages, w << self.cfg.fe_stages)
+
+    # ------------------------------------------------------------------ reference call surface
+    @torch.no_grad()
+    def forward(self, x, timesteps, lq=None, mask=None):
+        """x [N, C, H, W]; timesteps [N]; lq [N, 3, h, w]; mask [N, 1, h, w] or None -> [N, out_ch, H, W] fp32
+        (reference models/unet.py:865-895; the reference returns fp16 under autocast, this returns fp32)."""
+        if lq is None:
+            raise ValueError("UNetModelSwin is LQ-conditioned (cond_lq=True in every shipped config): pass lq=")
+        return self._run_forward(x, timesteps, lq, mask)
+
+
+class UNetModel(_NativeDenoiser):
+    """The reference's global-attention UNet.  Its AttentionBlocks run as GroupNorm, qkv conv, the multi-head attention
+    kernel (csrc/unet_attn.cuh) and proj_out with the block input as residual."""
+    _ZEROED = ("out_layers.3.weight", "out_layers.3.bias", "proj_out.weight", "proj_out.bias")   # zero_module (:172-174, :255)
+
+    def __init__(self, image_size, in_channels, model_channels, out_channels, num_res_blocks, attention_resolutions,
+                 cond_lq=True, dropout=0, channel_mult=(1, 2, 4, 8), conv_resample=True, dims=2, num_classes=None,
+                 use_fp16=False, num_heads=1, num_head_channels=-1, use_scale_shift_norm=False, resblock_updown=False,
+                 use_new_attention_order=False):
+        super().__init__()
+        self.cfg = UNetModelConfig(
+            image_size=image_size, in_channels=in_channels, model_channels=model_channels, out_channels=out_channels,
+            num_res_blocks=num_res_blocks, attention_resolutions=tuple(attention_resolutions), cond_lq=cond_lq,
+            dropout=dropout, channel_mult=tuple(channel_mult), conv_resample=conv_resample, dims=dims,
+            num_classes=num_classes, use_fp16=use_fp16, num_heads=num_heads, num_head_channels=num_head_channels,
+            use_scale_shift_norm=use_scale_shift_norm, resblock_updown=resblock_updown,
+            use_new_attention_order=use_new_attention_order)
+        # attributes the reference exposes
+        self.image_size, self.in_channels, self.model_channels = image_size, in_channels, model_channels
+        self.out_channels, self.cond_lq, self.num_classes = out_channels, cond_lq, num_classes
+        self.num_heads, self.num_head_channels = num_heads, num_head_channels
+        self.dtype = torch.float32
+        self._register_params(unetmodel_param_spec(self.cfg))
+
+    def _create_engine(self, handle):
+        cfgc, optc = _lib.make_unetmodel_config(self.cfg), _lib.make_options(self.cfg)
+        _lib.check(_lib.lib.rs_unetmodel_create(C.byref(cfgc), C.byref(optc), C.byref(handle)))
+
+    def _latent_rule(self) -> str:
+        return "2^(levels - 1): every level halves evenly"
+
+    def lq_shape(self, n, h, w):
+        f = self.cfg.lq_factor
+        return (n, 3, h * f, w * f)
+
+    @torch.no_grad()
+    def forward(self, x, timesteps, y=None, lq=None):
+        """x [N, out_channels, H, W]; timesteps [N]; lq [N, 3, H, W] or [N, 3, 2H, 2W] as in_channels says
+        -> [N, out_channels, H, W] fp32 (reference models/unet.py:549-585)."""
+        if y is not None:
+            raise ValueError("y: class-conditional UNetModel is not covered (num_classes must be None)")
+        if lq is None:
+            raise ValueError("UNetModel is LQ-conditioned (cond_lq=True): pass lq=")
+        if x.shape[1] != self.cfg.out_channels:
+            raise ValueError(f"x must have out_channels={self.cfg.out_channels} channels, got {x.shape[1]}")
+        return self._run_forward(x, timesteps, lq, None)
+
+
 class _Plan:
     """Engine bound to (batch, H, W): owns the workspace tensor and the native plan handle."""
 
-    def __init__(self, model: UNetModelSwin, batch: int, height: int, width: int, device):
+    def __init__(self, model: _NativeDenoiser, batch: int, height: int, width: int, device):
         self.model = model
         h = C.c_void_p()
         _lib.check(_lib.lib.rs_plan_create(model._engine, batch, height, width, C.byref(h)))

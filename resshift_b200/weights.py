@@ -14,16 +14,18 @@ from typing import Dict
 
 import torch
 
-from .arch import unet_param_spec, relative_position_index, shifted_window_mask, swin_geometry
-from .config import UNetConfig
+from .arch import unet_param_spec, unetmodel_param_spec, relative_position_index, shifted_window_mask, swin_geometry
+from .config import UNetConfig, UNetModelConfig
 
-_BRANCH_OUT = ("out_layers.3.weight", "attn.proj.weight", "mlp.fc2.weight")
+_BRANCH_OUT = ("out_layers.3.weight", "attn.proj.weight", "mlp.fc2.weight", "proj_out.weight")
 
 
-def random_state_dict(cfg: UNetConfig, seed: int = 0) -> Dict[str, torch.Tensor]:
+def random_state_dict(cfg, seed: int = 0) -> Dict[str, torch.Tensor]:
+    """For a UNetConfig (UNetModelSwin) or a UNetModelConfig (UNetModel)."""
     g = torch.Generator().manual_seed(seed)
     sd: Dict[str, torch.Tensor] = {}
-    for name, shape, role in unet_param_spec(cfg):
+    spec = unetmodel_param_spec(cfg) if isinstance(cfg, UNetModelConfig) else unet_param_spec(cfg)
+    for name, shape, role in spec:
         if role in ("conv3", "conv1", "linear"):
             fan_in = math.prod(shape[1:])
             gain = 0.35 if name.endswith(_BRANCH_OUT) else 1.0
