@@ -372,13 +372,10 @@ int rs_op_swin_attn(const void* x, int N, int H, int W, int E, int heads, int sh
 int rs_op_mlp(const void* x, int N, int H, int W, int E, int Hd, const void* w1_packed, const float* b1,
               const void* w2_packed, const float* b2, const void* residual, void* out, void* dbg_timeline_or_null,
               void* stream);
-/* the same with the block's norm2 fused in front (x is then the un-normalised tensor, Hd >= 4 E): its group statistics
- * either as gn_gstat[N][32][2] = (mean, rstd), or as the producers' (mean, M2) pairs gn_part[N][gn_slots][E][2]
- * (gn_gstat NULL), with gn_gamma / gn_beta [E]; all four NULL: no input norm.  part[i] (optional): (mean, M2) pairs of
- * out, part[i][N][slots][cstride[i]][2] at channel offset coff[i]; *slots_out = slots per image. */
+/* the same with the output's GroupNorm statistics: part[i] (optional): (mean, M2) pairs of out,
+ * part[i][N][slots][cstride[i]][2] at channel offset coff[i]; *slots_out = slots per image. */
 int rs_op_mlp_ex(const void* x, int N, int H, int W, int E, int Hd, const void* w1_packed, const float* b1,
-                 const void* w2_packed, const float* b2, const void* residual, void* out, const float* gn_gstat,
-                 const float* gn_part, int gn_slots, const float* gn_gamma, const float* gn_beta, float* const part[2],
+                 const void* w2_packed, const float* b2, const void* residual, void* out, float* const part[2],
                  const int32_t cstride[2], const int32_t coff[2], int32_t* slots_out, void* stream);
 /* host-only: tile configuration the conv launcher picks: out[8] = BN, msub, stages, CTAs/SM, estimated cycles,
    CTAs per tile group (1 or 2), split-K factor, persistent kernel (0 / 1) */

@@ -337,7 +337,7 @@ struct Tensor {
   bool persistent = false;
 };
 
-// The GroupNorm statistics a consumer reads (a GroupNorm op, the fused MLP's norm2, the fused Swin attention's norm1):
+// The GroupNorm statistics a consumer reads (a GroupNorm op, the fused Swin attention's norm1):
 // (mean, M2) pairs [N][slots][C][2] of `in` from its producers' epilogues (fused) or from gn_stats_kernel
 struct GnLink {
   View in;
@@ -364,9 +364,11 @@ struct ConvOp : Producer {
   std::string in_param;
 };
 struct GnOp { GnDesc d; GnLink stats; std::string name; };   // d.in / fused / slots / eps come from stats at bind
-struct WinAttnOp { View qkv, out; int window = 8, shift = 0; std::string bias_name; const float* bias = nullptr; };
+struct WinAttnOp {   // (simt: the SIMT cross-check kernel instead of a window_attn_kernel instance)
+  View qkv, out; int window = 8, shift = 0; bool simt = false; std::string bias_name; const float* bias = nullptr;
+};
 struct ResampleOp { View in, out; bool pool = false; };     // 2x nearest upsample, or (pool) 2x2 average pool
-struct MlpOp : Producer { MlpDesc d; std::string name, norm_name; std::optional<GnLink> norm2; };   // norm2: in the kernel
+struct MlpOp : Producer { MlpDesc d; std::string name; };
 struct SwinOp : Producer { SwinAttnDesc d; std::string blk; GnLink norm1; };
 struct SoftmaxOp { View view; float scale = 1.f; };         // in place on view [rows = N*H*W][cols = C]
 
@@ -392,6 +394,7 @@ inline SoftmaxParams softmax_params(const SoftmaxOp& s) {
 
 struct rs_plan {
   rs_engine* e = nullptr;
+  Overrides ovr;             // the environment's kernel-choice overrides when the plan was created: its every decision follows them
   int B = 0, H = 0, W = 0, lqH = 0, lqW = 0;
   std::vector<Tensor> tensors;
   std::vector<Op> fe_ops, ops;
@@ -497,21 +500,11 @@ struct Builder {
     for (const Writer& w : prod) producer(w).stat_dst.push_back({s, w.c0 - in.c0});
     return s;
   }
-  const bool fuse_mlp = env_int("RS_MLP_FUSE", 1) && !env_is("RS_CONV_IMPL", "simt");
-  // norm2 applied inside the fused MLP kernel (bit-identical to the separate pass; RS_MLP_NORM_FUSE=1, off by default:
-  // not measured faster)
-  const bool fuse_mlp_norm = env_int("RS_MLP_NORM_FUSE", 0) != 0;
-  // norm1 + qkv + window attention + proj + residual as one kernel per Swin block (swin_attn_fused.cuh; RS_SWIN_FUSE=0:
-  // four launches)
-  const bool fuse_swin_attn = env_int("RS_SWIN_FUSE", 1) != 0 && !env_is("RS_CONV_IMPL", "simt") && !env_is("RS_ATTN_IMPL", "simt");
-  // a level with few window pairs is one long serial tile per CTA on a handful of SMs; below this many pairs the four
-  // small launches, whose prologues overlap through PDL, are used instead.  At the benchmark shape (batch 16, the 64x64 and
-  // 32x32 levels fused) the default measured 127.7 ms per 15-step loop against 134.8 ms with every level on four launches
-  // (H100 80GB HBM3 SXM, 700 W).  With an earlier build of the wgmma kernel, thresholds 96 / 32 / 8 / 1 (also fusing
-  // the 16x16 and 8x8 levels) measured 135.3 / 134.1 / 135.3 / 135.6 ms, one run each: within the run-to-run spread,
-  // so 96 stays (H100 80GB HBM3 SXM, 400 W)
-  const int fuse_swin_min_pairs = env_int("RS_SWIN_FUSE_MIN_PAIRS", 96);
-  const bool fuse_stats = env_int("RS_GN_FUSE", 1) && !env_is("RS_CONV_EPI", "direct") && !env_is("RS_CONV_IMPL", "simt");
+  // the fused kernels run only where the overrides leave the wgmma conv and attention kernels in place
+  const bool fuse_mlp = !P.ovr.conv_simt;
+  // norm1 + qkv + window attention + proj + residual as one kernel per Swin block (swin_attn_fused.cuh)
+  const bool fuse_swin_attn = !P.ovr.conv_simt && !P.ovr.attn_simt;
+  const bool fuse_stats = !P.ovr.conv_direct && !P.ovr.conv_simt;
   Builder(rs_plan& p) : P(p), E(*p.e), cur(&p.ops) {}
   int list_id() const { return cur == &P.fe_ops ? 0 : 1; }
   std::vector<Op>& list(int id) { return id == 0 ? P.fe_ops : P.ops; }
@@ -528,8 +521,8 @@ struct Builder {
     if (res) { op.d.res = *res; op.d.has_res = true; }
     op.w_name = name + ".weight"; op.b_name = name + ".bias";
     op.to_f32 = out_f32;
-    if (out && !out_f32 && env_int("RS_CONV_SPLITK", 0) != 1) {       // split-K for layers with too few tiles
-      const TileConfig tc = conv_preview_config(in.N, in.H, in.W, in.C, cout, ksize, stride, true);
+    if (out && !out_f32 && P.ovr.conv_splitk != 1) {       // split-K for layers with too few tiles
+      const TileConfig tc = conv_preview_config(P.ovr, in.N, in.H, in.W, in.C, cout, ksize, stride, true);
       if (tc.splitk > 1) {
         op.d.allow_split = true;
         const size_t bytes = (size_t)tc.splitk * in.N * (in.H / stride) * (in.W / stride) * cout * sizeof(float);
@@ -553,30 +546,20 @@ struct Builder {
     cur->push_back(std::move(op));
   }
   void attn(const View& qkv, const View& out, const std::string& blk, int window, int shift) {
-    WinAttnOp op; op.qkv = qkv; op.out = out; op.window = window; op.shift = shift;
+    WinAttnOp op; op.qkv = qkv; op.out = out; op.window = window; op.shift = shift; op.simt = P.ovr.attn_simt;
     op.bias_name = blk + ".attn.relative_position_bias_table";
     const int i = opi();
     P.touch(qkv, i); P.touch(out, i);
     cur->push_back(std::move(op));
   }
-  // norm_name non-empty: `in` is the un-normalised tensor and the kernel applies that GroupNorm to its X tile itself
-  // (returns false, adding nothing, when the statistics cannot come from the producers' epilogues)
-  bool mlp(const View& in, const std::string& name, int E, int Hd, const View& out, const View& res,
-           const std::string& norm_name = std::string()) {
+  void mlp(const View& in, const std::string& name, int E, int Hd, const View& out, const View& res) {
     MlpOp op;
     op.d.in = in; op.d.out = out; op.d.res = res; op.d.has_res = true; op.d.E = E; op.d.Hd = Hd;
     op.name = name;
-    if (!norm_name.empty()) {
-      if (Hd < 4 * E) return false;
-      op.norm2 = link_stats(in, 1e-5f, /*fused_only=*/true);
-      if (!op.norm2) return false;
-      op.norm_name = norm_name;
-    }
     const int i = opi();
     P.touch(in, i); P.touch(out, i); P.touch(res, i);
     cur->push_back(std::move(op));
     if (out.tens >= 0) note_writer(out, E);
-    return true;
   }
   // x <- x + proj(window_attention(qkv(norm1(x)))) in one kernel (swin_attn_fused.cuh); false when the statistics of x
   // cannot come from its producers' epilogues
@@ -656,10 +639,10 @@ struct Builder {
     for (int i = 0; i < c.swin_depth; ++i) {
       const std::string b = p + ".blocks." + std::to_string(i);
       // x = x + proj(attn(qkv(norm1(x)))): one kernel (swin_attn_fused.cuh), or the four-launch sequence
-      // (a level with few window pairs is one long serial tile per CTA on a handful of SMs: below fuse_swin_min_pairs the
-      //  four small launches, whose prologues overlap through PDL, are faster in the graph)
+      // (a level with few window pairs is one long serial tile per CTA on a handful of SMs: below swin_fuse_min_pairs
+      //  (Overrides) the four small launches, whose prologues overlap through PDL, are faster in the graph)
       const int win_pairs = (x.N * (x.H / win) * (x.W / win) + 1) / 2;
-      if (!(fuse_swin_attn && win_pairs >= fuse_swin_min_pairs && swin_attn_supported(Ed, c.swin_heads, x.H, x.W, win) &&
+      if (!(fuse_swin_attn && win_pairs >= P.ovr.swin_fuse_min_pairs && swin_attn_supported(Ed, c.swin_heads, x.H, x.W, win) &&
             swin_attn(e, b, c.swin_heads, (i % 2) ? shift_odd : 0))) {
         View n1 = P.make_view(x.N, x.H, x.W, Ed);
         gn(e, b + ".norm1", n1, 0, -1);
@@ -669,12 +652,9 @@ struct Builder {
         attn(qkv, a, b, win, (i % 2) ? shift_odd : 0);
         conv(a, b + ".attn.proj", 1, 1, Ed, &e, &e, ACT_NONE);              // x = shortcut + attn
       }
-      const bool mlp_ok = fuse_mlp && mlp_supported(Ed, hidden, x.H, x.W, x.N);
-      // x = x + fc2(gelu(fc1(norm2(x)))) in one kernel, norm2 applied to the X tile in shared memory
-      if (mlp_ok && fuse_mlp_norm && mlp(e, b + ".mlp", Ed, hidden, e, e, b + ".norm2")) continue;
       View n2 = P.make_view(x.N, x.H, x.W, Ed);
       gn(e, b + ".norm2", n2, 0, -1);
-      if (mlp_ok) {
+      if (fuse_mlp && mlp_supported(Ed, hidden, x.H, x.W, x.N)) {
         mlp(n2, b + ".mlp", Ed, hidden, e, e);                            // x = x + fc2(gelu(fc1(n2))), one kernel
       } else {
         View f = P.make_view(x.N, x.H, x.W, hidden);
@@ -778,7 +758,7 @@ int finish_layout(rs_plan& P, Builder& b, size_t state_bytes, bool unet) {
   P.off_state = region(2 * align_up(lat, 256));
   // persistent tensors first, then liveness-packed temporaries (RS_NO_REUSE=1 keeps every tensor
   // alive for the whole forward so that rs_plan_probe can read any block output afterwards)
-  if (env_int("RS_NO_REUSE", 0)) for (Tensor& tz : P.tensors) tz.persistent = true;
+  if (P.ovr.no_reuse) for (Tensor& tz : P.tensors) tz.persistent = true;
   for (Tensor& tz : P.tensors) if (tz.persistent) tz.off = region(tz.bytes);
   P.off_temps = off;
   {
@@ -908,13 +888,13 @@ void resolve(rs_plan& P, View& v) {
 // Who reduces the (mean, M2) pairs to the image's 32 (mean, rstd)?
 //   * few tile slots (the denoiser's maps, <= 32 slots): every consumer CTA combines them itself — a finalisation step on
 //     the producer's tail sits on every producer CTA;
-//   * many slots (the VQ-GAN's 128x128 / 256x256 maps, RS_GN_FINALIZE_SLOTS moves the threshold): gn_finalize_kernel, a
+//   * many slots (more than kGnFinalizeSlots: the VQ-GAN's 128x128 / 256x256 maps): gn_finalize_kernel, a
 //     small launch in front of the consumer, or, for a GroupNorm without a fusable producer, the last gn_stats_kernel CTA
 //     of each image (arrival counters).  (The last producer CTA of an image would do it at the cost of a counter round
 //     trip on every tile, and on a persistent conv the CTAs all finish together, so ONE of them would reduce every image.)
+constexpr int kGnFinalizeSlots = 64;
 bool gn_finalizes(const GnLink& g) {
-  static const int thr = env_int("RS_GN_FINALIZE_SLOTS", 64);
-  return g.slots > thr && !g.win_slots;      // (the fused Swin attention kernel delivers pairs only)
+  return g.slots > kGnFinalizeSlots && !g.win_slots;      // (the fused Swin attention kernel delivers pairs only)
 }
 GnSink make_sink(rs_plan& P, const GnLink& g, int coff, bool consumer = false) {
   GnSink s{};
@@ -960,7 +940,9 @@ int bind_ops(rs_plan& P, std::vector<Op>& ops) {
         // the first conv reads the channel-padded packed input: expose the padded width to the kernel
         if (d.in.C < d.ipad && d.in.ld >= d.ipad && d.in.tens == P.xin.tens) d.in.C = d.ipad;
         if (d.in.C < d.ipad && P.fe_in.tens >= 0 && d.in.tens == P.fe_in.tens) d.in.C = d.ipad;
-        rc = conv_finalize(d);
+        rc = conv_finalize(d, P.ovr); if (rc) return rc;
+        RS_CHECK(d.prm.splitk == 1 || (size_t)d.prm.splitk * d.prm.Nimg * d.prm.Hout * d.prm.Wout * d.Cout * sizeof(float) <=
+                                       P.tensors[c.split_tens].bytes, "split-K scratch of " + c.w_name + " too small for the split chosen");
         launches = d.prm.splitk > 1 ? 2 : 1;
         break;
       }
@@ -994,12 +976,6 @@ int bind_ops(rs_plan& P, std::vector<Op>& ops) {
         m.w2 = E.packed(mo.name + ".fc2.weight", &ld2); m.b2 = E.at<float>(mo.name + ".fc2.bias");
         RS_CHECK(m.w1 && m.w2 && m.b1 && m.b2, "missing MLP parameters " + mo.name + ".fc1.weight");
         RS_CHECK(ld1 == m.E && ld2 == m.Hd, "MLP weight padding");
-        if (mo.norm2) {
-          const GnSink sk = make_sink(P, *mo.norm2, 0);
-          m.gn_in_gstat = sk.gstat; m.gn_in_part = sk.part; m.gn_in_slots = mo.norm2->slots;
-          m.gn_in_gamma = E.at<float>(mo.norm_name + ".weight"); m.gn_in_beta = E.at<float>(mo.norm_name + ".bias");
-          RS_CHECK(m.gn_in_gamma && m.gn_in_beta, "missing GroupNorm parameters " + mo.norm_name);
-        }
         bind_sinks(P, mo, m.sink);
         rc = mlp_finalize(m);
         break;
@@ -1041,7 +1017,7 @@ int bind_ops(rs_plan& P, std::vector<Op>& ops) {
 }
 
 struct Prof {
-  std::vector<cudaEvent_t> ev;     // a pair per op run, skipped or not
+  std::vector<cudaEvent_t> ev;     // a pair per op run
   int used = 0;
   cudaEvent_t get() {
     if (used == (int)ev.size()) { cudaEvent_t e; cudaEventCreate(&e); ev.push_back(e); }
@@ -1050,30 +1026,12 @@ struct Prof {
   ~Prof() { for (cudaEvent_t e : ev) cudaEventDestroy(e); }
 };
 
-// RS_SKIP_KINDS (timing ablation only — results are garbage): bit 0 conv3x3, 1 conv1x1 / linear, 2 GroupNorm, 3 attention
-// (window, fused Swin, fused VQ-GAN, UNetModel), 4 upsample, 5 fused MLP.  The time a kernel family really costs inside the graph-replayed step is the
-// difference between the full step and the step without it (per-launch events over-state small kernels).
-inline bool op_skipped(const Op& op) {
-  static const int skip = env_int("RS_SKIP_KINDS", 0);
-  if (!skip) return false;
-  switch (kind_of(op)) {
-    case OP_CONV: return (skip >> (payload<ConvOp>(op).d.ksize == 3 ? 0 : 1)) & 1;
-    case OP_GN: return (skip >> 2) & 1;
-    case OP_ATTN: case OP_SWIN_ATTN: case OP_VQ_ATTN: case OP_UNET_ATTN: return (skip >> 3) & 1;
-    case OP_UPSAMPLE: return (skip >> 4) & 1;
-    case OP_MLP: return (skip >> 5) & 1;
-    case OP_SOFTMAX: return false;
-  }
-  return false;
-}
-
 // ops [first, last) of an op list
 int run_op_range(rs_plan& P, const Op* first, const Op* last, const float* film_base, long long film_sN, cudaStream_t st,
                  Prof* prof = nullptr) {
   for (const Op* it = first; it != last; ++it) {
     const Op& op = *it;
     int rc = 0;
-    if (op_skipped(op)) { if (prof) { cudaEventRecord(prof->get(), st); cudaEventRecord(prof->get(), st); } continue; }
     if (prof) cudaEventRecord(prof->get(), st);
     switch (kind_of(op)) {
       case OP_CONV: {
@@ -1098,7 +1056,7 @@ int run_op_range(rs_plan& P, const Op* first, const Op* last, const float* film_
       case OP_UNET_ATTN: rc = unet_attn_launch(payload<UnetAttnDesc>(op), st); break;
       case OP_ATTN: {
         const WinAttnOp& a = payload<WinAttnOp>(op);
-        rc = attn_launch(a.qkv, a.out, a.bias, P.e->cfg.swin_heads, P.e->cfg.swin_embed_dim, a.window, a.shift, st);
+        rc = attn_launch(a.qkv, a.out, a.bias, P.e->cfg.swin_heads, P.e->cfg.swin_embed_dim, a.window, a.shift, a.simt, st);
         break;
       }
       case OP_SOFTMAX: {
@@ -1364,7 +1322,7 @@ int rs_plan_create(rs_engine* e, int batch, int height, int width, rs_plan** out
            (e->unetmodel ? std::string("2^(levels - 1)") : std::string("each level's window (at most window_size) times the "
                                                                           "level's downsampling (64 for the shipped configs)")));
   auto p = std::make_unique<rs_plan>();
-  p->e = e; p->B = batch; p->H = height; p->W = width;
+  p->e = e; p->ovr = read_overrides(); p->B = batch; p->H = height; p->W = width;
   int rc = build_plan(*p); if (rc) return rc;
   *out = p.release();
   return 0;

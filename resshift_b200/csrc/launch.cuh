@@ -90,31 +90,52 @@ inline int encode_weight_map(CUtensorMap* m, const __half* base, int Ktot, int C
   return 0;
 }
 
-inline int env_int(const char* name, int dflt) {
-  const char* v = std::getenv(name);
-  return v ? std::atoi(v) : dflt;
-}
-inline bool env_is(const char* name, const char* val) {
-  const char* v = std::getenv(name);
-  return v && std::strcmp(v, val) == 0;
+// The kernel-choice overrides of the environment (INTEGRATION.md): test hooks and tuning aids, none set in production.
+// A plan reads them once, when it is created, and every later decision of that plan (layout, tile configurations at
+// bind, the kernels it launches) follows that snapshot; a single-operator entry point reads them per call.
+struct Overrides {
+  bool conv_simt = false;     // RS_CONV_IMPL=simt: the SIMT cross-check conv kernel (no fused MLP / Swin attention / statistics)
+  bool attn_simt = false;     // RS_ATTN_IMPL=simt: the SIMT cross-check window-attention kernel (no fused Swin attention)
+  bool conv_direct = false;   // RS_CONV_EPI=direct: per-thread stores instead of the staged TMA epilogue
+  // RS_CONV_{BN,CG,OCC,MSUB,SPLITK}: forced tile configuration (0: the cost model's pick); RS_CONV_PERSIST 0 / 1
+  // disables / forces the persistent kernel (-1: the cost model)
+  int conv_bn = 0, conv_cg = 0, conv_occ = 0, conv_msub = 0, conv_splitk = 0, conv_persist = -1;
+  bool no_reuse = false;      // RS_NO_REUSE=1: no workspace aliasing, every block output stays readable (rs_plan_probe)
+  // RS_SWIN_FUSE_MIN_PAIRS: a Swin level with fewer pairs of 8x8 windows keeps the four-launch attention half.  A level with
+  // few window pairs is one long serial tile per CTA on a handful of SMs; below this many pairs the four small launches,
+  // whose prologues overlap through PDL, are used instead.  At the benchmark shape (batch 16, the 64x64 and 32x32 levels
+  // fused) the default measured 127.7 ms per 15-step loop against 134.8 ms with every level on four launches (H100 80GB
+  // HBM3 SXM, 700 W).  With an earlier build of the wgmma kernel, thresholds 96 / 32 / 8 / 1 (also fusing the 16x16 and
+  // 8x8 levels) measured 135.3 / 134.1 / 135.3 / 135.6 ms, one run each: within the run-to-run spread, so 96 stays
+  // (H100 80GB HBM3 SXM, 400 W)
+  int swin_fuse_min_pairs = 96;
+};
+inline Overrides read_overrides() {
+  auto var = [](const char* name) { return std::getenv(name); };
+  auto num = [&](const char* name, int dflt) { const char* v = var(name); return v ? std::atoi(v) : dflt; };
+  auto is = [&](const char* name, const char* val) { const char* v = var(name); return v && std::strcmp(v, val) == 0; };
+  Overrides o;
+  o.conv_simt = is("RS_CONV_IMPL", "simt");
+  o.attn_simt = is("RS_ATTN_IMPL", "simt");
+  o.conv_direct = is("RS_CONV_EPI", "direct");
+  o.conv_bn = num("RS_CONV_BN", 0); o.conv_cg = num("RS_CONV_CG", 0); o.conv_occ = num("RS_CONV_OCC", 0);
+  o.conv_msub = num("RS_CONV_MSUB", 0); o.conv_splitk = num("RS_CONV_SPLITK", 0); o.conv_persist = num("RS_CONV_PERSIST", -1);
+  o.no_reuse = num("RS_NO_REUSE", 0) != 0;
+  o.swin_fuse_min_pairs = num("RS_SWIN_FUSE_MIN_PAIRS", o.swin_fuse_min_pairs);
+  return o;
 }
 
 // All kernels go through this launcher: cudaLaunchKernelEx with the programmatic-stream-serialization
 // attribute (PDL), so kernel N+1's prologue overlaps kernel N's tail, also inside captured graphs.
-// RS_PDL=0 turns the attribute off.
 template <typename... KArgs, typename... Args>
 inline cudaError_t launch_kc(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st,
                              int cluster_x, Args&&... args) {
-  static const int use_pdl = env_int("RS_PDL", 1);
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = st;
   cudaLaunchAttribute attr[2];
-  int n = 0;
-  if (use_pdl) {
-    attr[n].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[n].val.programmaticStreamSerializationAllowed = 1;
-    ++n;
-  }
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[0].val.programmaticStreamSerializationAllowed = 1;
+  int n = 1;
   if (cluster_x > 1) {
     attr[n].id = cudaLaunchAttributeClusterDimension;
     attr[n].val.clusterDim.x = cluster_x; attr[n].val.clusterDim.y = 1; attr[n].val.clusterDim.z = 1;
@@ -189,6 +210,7 @@ struct ConvDesc {
   // filled by finalize()
   ConvParams prm;
   ConvSimtSrc simt;
+  bool simt_kernel = false;       // launch the SIMT cross-check kernel (RS_CONV_IMPL=simt) instead of the wgmma one
   int grid = 0; size_t smem = 0;
 };
 
@@ -200,10 +222,9 @@ struct TileConfig { int BN = 0, msub = 1, stages = 2, occ = 1, cg = 1, splitk = 
 // read by wgmma (A once, B once per warpgroup); a CTA pair (cg = 2) fetches only half of B from L2 per CTA (TMA
 // multicast).  Shallow rings are additionally latency-bound (~3000 cycles per load).  The epilogue (~18 cycles per
 // column + set-up) hides under a co-resident CTA; whole waves are counted.
-inline TileConfig pick_tile_config(int m_tiles, int cout16, int num_kb, int f_bn, bool allow_split = false, bool allow_persist = false,
-                                   bool allow_msub2 = true, int msub_request = 0) {
-  const int f_msub = msub_request ? msub_request : env_int("RS_CONV_MSUB", 0), f_occ = env_int("RS_CONV_OCC", 0), f_stages = env_int("RS_CONV_STAGES", 0);
-  const int f_cg = env_int("RS_CONV_CG", 0);
+inline TileConfig pick_tile_config(const Overrides& o, int m_tiles, int cout16, int num_kb, int f_bn, bool allow_split = false,
+                                   bool allow_persist = false, bool allow_msub2 = true, int msub_request = 0) {
+  const int f_msub = msub_request ? msub_request : o.conv_msub, f_occ = o.conv_occ, f_cg = o.conv_cg;
   TileConfig best, bestp;      // best one-tile-per-CTA configuration (ranking model below), best persistent one
   double best_real = 1e30;     // realistic estimate of `best` (see the end of the function)
   for (int cand = std::min(cout16, 256); cand >= 16; cand -= 16) {
@@ -255,7 +276,6 @@ inline TileConfig pick_tile_config(int m_tiles, int cout16, int num_kb, int f_bn
             if (st_need > budget / sbytes) continue;
             st = std::max(st, st_need);
           }
-          if (f_stages) st = f_stages;
           if (st < 2 || (size_t)st * sbytes + 2304 > (size_t)(occ == 2 ? 113 : 227) * 1024) continue;
           const double smem_cycles = (sbytes + ms * kConvBM * kConvBK * 2.0 + 2.0 * cand * kConvBK * 2.0) / 128.0;
           // SM time for every resident CTA to advance one k-block: tensor / smem work of each, or the load latency
@@ -268,7 +288,7 @@ inline TileConfig pick_tile_config(int m_tiles, int cout16, int num_kb, int f_bn
           const long long units = (long long)((m_tiles + cg * ms - 1) / (cg * ms)) * n_tiles;   // CTAs or CTA pairs
           const double slots = (cg == 2 ? num_sms() / 2 : num_sms()) * (double)occ;
           // split-K: S CTAs (pairs) share one output tile's K loop; costs an fp32 round trip + a small reduce kernel
-          const int f_split = env_int("RS_CONV_SPLITK", 0);
+          const int f_split = o.conv_splitk;
           const int kSplits[6] = {1, 2, 3, 4, 6, 8};
           for (int si = 0; si < 6; ++si) {
             const int S = kSplits[si];
@@ -301,7 +321,8 @@ inline TileConfig pick_tile_config(int m_tiles, int cout16, int num_kb, int f_bn
 }
 
 // geometry-only preview of the configuration conv_finalize() will choose (used at plan time to size split-K scratch)
-inline TileConfig conv_preview_config(int N, int Hin, int Win, int Cin, int Cout, int ksize, int stride, bool allow_split) {
+inline TileConfig conv_preview_config(const Overrides& o, int N, int Hin, int Win, int Cin, int Cout, int ksize, int stride,
+                                      bool allow_split) {
   const int Hout = Hin / stride, Wout = Win / stride;
   const int bw = pow2_floor_div(Wout, kConvBM);
   const int bh = pow2_floor_div(Hout, kConvBM / bw);
@@ -310,7 +331,7 @@ inline TileConfig conv_preview_config(int N, int Hin, int Win, int Cin, int Cout
   const bool contiguous = (bw == Wout) || (bh == 1);
   const int num_kb = ksize * ksize * ((Cin + kConvBK - 1) / kConvBK);
   const bool sp = allow_split && contiguous && bn <= 2;
-  return pick_tile_config(m_tiles, (Cout + 15) / 16 * 16, num_kb, env_int("RS_CONV_BN", 0), sp);
+  return pick_tile_config(o, m_tiles, (Cout + 15) / 16 * 16, num_kb, o.conv_bn, sp);
 }
 
 // The statistics sinks a producer's kernel receives: the set ones of `sink` first; an unset `expected` becomes slots (the
@@ -327,7 +348,7 @@ inline void compact_sinks(const GnSink (&sink)[2], int slots, GnSink (&out)[2]) 
   }
 }
 
-inline int conv_finalize(ConvDesc& d) {
+inline int conv_finalize(ConvDesc& d, const Overrides& o) {
   ConvParams& p = d.prm;
   std::memset(&p, 0, sizeof(p));
   const int Hin = d.in.H, Win = d.in.W;
@@ -353,12 +374,13 @@ inline int conv_finalize(ConvDesc& d) {
   const int num_kb = p.num_taps * p.kchunks;
   const bool contiguous_tiles = (p.bw == Wout) || (p.bh == 1);
   // (the SIMT cross-check kernel computes whole outputs, bias / residual / activation included: it never splits K)
-  const bool simt = env_is("RS_CONV_IMPL", "simt");
+  const bool simt = o.conv_simt;
+  d.simt_kernel = simt;
   const bool can_split = d.allow_split && d.partial != nullptr && contiguous_tiles && p.bn <= 2 && d.has_out && !d.out_f32 && !simt;
-  const int want_persist = env_int("RS_CONV_PERSIST", -1);           // 0 / 1 disables / forces the persistent kernel
-  const bool persist_ok = d.has_out && !d.out_f32 && want_persist != 0 && !env_is("RS_CONV_EPI", "direct") &&
-                          !env_is("RS_CONV_IMPL", "simt") && (d.msub_request ? d.msub_request : env_int("RS_CONV_MSUB", 0)) != 2;
-  const TileConfig tc = pick_tile_config(m_tiles, cout16, num_kb, d.bn_override ? d.bn_override : env_int("RS_CONV_BN", 0), can_split,
+  const int want_persist = o.conv_persist;                           // 0 / 1 disables / forces the persistent kernel
+  const bool persist_ok = d.has_out && !d.out_f32 && want_persist != 0 && !o.conv_direct && !simt &&
+                          (d.msub_request ? d.msub_request : o.conv_msub) != 2;
+  const TileConfig tc = pick_tile_config(o, m_tiles, cout16, num_kb, d.bn_override ? d.bn_override : o.conv_bn, can_split,
                                          persist_ok && want_persist != 1, !d.bias_per_image, d.msub_request);
   const int BN = tc.BN, msub = tc.msub, stages = tc.stages, cg = tc.cg;
   p.cg = cg;
@@ -410,7 +432,7 @@ inline int conv_finalize(ConvDesc& d) {
   p.out_f32_nchw = d.out_f32;
   p.dbg = d.dbg;
   // staged epilogue (TMA store / TMA residual load) for fp16 NHWC outputs
-  p.tma_out = (d.has_out && !d.out_f32 && p.splitk == 1 && !env_is("RS_CONV_EPI", "direct") && !env_is("RS_CONV_IMPL", "simt")) ? 1 : 0;
+  p.tma_out = (d.has_out && !d.out_f32 && p.splitk == 1 && !o.conv_direct && !simt) ? 1 : 0;
   p.tma_res = (p.tma_out && d.has_res) ? 1 : 0;
   p.epi_bc = (BN % 64 == 0) ? 64 : (BN % 32 == 0 ? 32 : 16);
   if (p.tma_out) {
@@ -483,12 +505,12 @@ inline int conv_finalize(ConvDesc& d) {
     const __half* base = d.in.ptr + (long long)hp * d.in.sH() + (long long)wp * d.in.sW();
     const long long sW = d.in.sW() * d.stride, sH = d.in.sH() * d.stride, sN = d.in.sN();
     s.ptr[i] = base; s.sN[i] = sN; s.sH[i] = sH; s.sW[i] = sW; s.H[i] = Hout; s.W[i] = Wout;
-    if (!env_is("RS_CONV_IMPL", "simt")) {
+    if (!simt) {
       int rc = encode_act_map(&p.tmA[i], base, d.in.C, Wout, Hout, N, sW, sH, sN, p.bw, p.bh, p.bn);
       if (rc) return rc;
     }
   }
-  if (!env_is("RS_CONV_IMPL", "simt")) {
+  if (!simt) {
     int rc = encode_weight_map(&p.tmB, d.wt, p.num_taps * d.ipad, d.Cout, BN / cg);   // pair mode: each CTA loads half
     if (rc) return rc;
   }
@@ -533,7 +555,7 @@ inline int conv_init() {
 }
 
 inline int conv_launch(const ConvDesc& d, cudaStream_t st) {
-  if (env_is("RS_CONV_IMPL", "simt")) {
+  if (d.simt_kernel) {
     const long long npix = (long long)d.prm.Nimg * d.prm.Hout * d.prm.Wout;
     const int warps = 8;
     (void)launch_k(conv_simt_kernel, dim3((unsigned)((npix + warps - 1) / warps)), dim3(warps * 32), (size_t)(0), st, d.prm, d.simt);
@@ -636,10 +658,6 @@ struct MlpDesc {
   const __half* w2 = nullptr; const float* b2 = nullptr;    // fc2: [E][Hd] fp16
   int E = 0, Hd = 0;
   GnSink sink[2] = {};
-  // optional fused input GroupNorm (plain affine): `in` is then the un-normalised tensor
-  const float* gn_in_gstat = nullptr;      // finalised group statistics, or
-  const float* gn_in_part = nullptr; int gn_in_slots = 0;   // the producers' (mean, M2) pairs to combine in the kernel
-  const float* gn_in_gamma = nullptr; const float* gn_in_beta = nullptr;
   MlpParams prm;
   int grid = 0; size_t smem = 0;
 };
@@ -664,7 +682,7 @@ inline int mlp_finalize(MlpDesc& d) {
   p.tiles_w = W / p.bw; p.tiles_h = H / p.bh;
   const int tiles_n = (N + p.bn - 1) / p.bn;
   p.Wout = W; p.Hout = H; p.Nimg = N;
-  // ring slots for the weight tiles: as many as fit next to X, one hidden chunk and the bias / affine tables
+  // ring slots for the weight tiles: as many as fit next to X, one hidden chunk and the bias tables
   const int slot = std::max(kMlpHc, d.E) * kConvBK * 2;
   const int fixed = MlpSmem(d.E, d.Hd, 0).total + 1024;     // + alignment slack
   p.ring = std::min(8, (227 * 1024 - fixed) / slot);
@@ -683,10 +701,6 @@ inline int mlp_finalize(MlpDesc& d) {
     rc = encode_act_map(&p.tmRes, d.res.ptr, d.E, W, H, N, d.res.sW(), d.res.sH(), d.res.sN(), p.bw, p.bh, p.bn, 64);
     if (rc) return rc;
   }
-  p.gn_in_gstat = d.gn_in_gstat; p.gn_in_part = d.gn_in_part; p.gn_in_slots = d.gn_in_slots;
-  p.gn_in_gamma = d.gn_in_gamma; p.gn_in_beta = d.gn_in_beta; p.gn_in_eps = 1e-5f;
-  RS_CHECK(!(d.gn_in_gstat || d.gn_in_part) || (d.gn_in_gamma && d.gn_in_beta && d.Hd >= 4 * d.E && d.E % 32 == 0),
-           "fused MLP: input GroupNorm arguments");
   p.gn_slots = p.tiles_w * p.tiles_h;
   compact_sinks(d.sink, p.gn_slots, p.sink);
   return 0;
@@ -863,8 +877,8 @@ inline int unet_attn_launch(const UnetAttnDesc& d, cudaStream_t st) {
   return 0;
 }
 
-// one launch of the window-attention core: the instance of window_attn_kernel for (window side, head width), or the
-// SIMT cross-check under RS_ATTN_IMPL=simt
+// one launch of the window-attention core: the instance of window_attn_kernel for (window side, head width), or with
+// simt the SIMT cross-check (RS_ATTN_IMPL=simt)
 template <int WS, int HD>
 inline int attn_launch_instance(WinAttnParams& p, int windows, cudaStream_t st) {
   // heads per CTA: all of them when there are plenty of windows, fewer (more CTAs) otherwise
@@ -881,7 +895,7 @@ inline int attn_launch_instance(WinAttnParams& p, int windows, cudaStream_t st) 
 }
 
 inline int attn_launch(const View& qkv, const View& out, const float* bias, int heads, int E, int window, int shift,
-                       cudaStream_t st) {
+                       bool simt, cudaStream_t st) {
   RS_CHECK(window == 8 || window == 16, "window attention kernels: window_size 8 or 16, got " + std::to_string(window));
   RS_CHECK(heads > 0 && E % heads == 0 && (E / heads == 32 || E / heads == 64),
            "window attention kernels: head_dim 32 or 64");
@@ -893,7 +907,7 @@ inline int attn_launch(const View& qkv, const View& out, const float* bias, int 
   WinAttnParams p{qkv.ptr, qkv.ld, out.ptr, out.ld, bias, qkv.N, qkv.H, qkv.W, heads, E, shift,
                   hd == 32 ? 0.17677669529663687f : 0.125f, heads, window, hd};
   int rc = 0;
-  if (env_is("RS_ATTN_IMPL", "simt")) {
+  if (simt) {
     (void)launch_k(window_attn_simt_kernel, dim3(windows, heads), dim3(window * window), (size_t)0, st, p);
   } else if (window == 8) {
     rc = hd == 32 ? attn_launch_instance<8, 32>(p, windows, st) : attn_launch_instance<8, 64>(p, windows, st);

@@ -13,8 +13,7 @@
 //
 // then the staged epilogue of conv_gemm.cuh (+ b2, + residual through a TMA load, fp16, TMA store, GroupNorm partials).
 // Warp 8 is the TMA producer: X once, then per chunk the fc1 weight tiles followed by the fc2 weight tiles, through one
-// ring of slots in the order the consumers use them.  Optionally the Swin block's norm2 is applied to the X tile in shared
-// memory first (same arithmetic as gn_apply_kernel, so the operand is bit-identical to the separate pass).
+// ring of slots in the order the consumers use them.  The Swin block's norm2 runs in front of this kernel (gn_apply_kernel).
 #pragma once
 
 #include "common.cuh"
@@ -36,19 +35,11 @@ struct MlpParams {
   int Wout, Hout, Nimg;
   int has_res;
   GnSink sink[2]; int gn_slots;      // fused GroupNorm statistics of the output (gn_stats.cuh)
-  // optional fused input GroupNorm (the Swin block's norm2, models/swin_transformer.py:279): X is then the UN-normalised
-  // tensor and the CTA applies  a*x + b  (per image, per channel) to its X tile in shared memory before the first GEMM
-  const float* gn_in_gstat;          // [N][32][2] finalised by the producer, or nullptr
-  const float* gn_in_part;           // [N][gn_in_slots][E][2] (mean, M2) pairs, combined here when gn_in_gstat == nullptr
-  int gn_in_slots;
-  float gn_in_eps;
-  const float* gn_in_gamma;          // [E]
-  const float* gn_in_beta;           // [E]
 };
 
 // shared-memory layout (offsets from the 1024-aligned base)
 struct MlpSmem {
-  int x, h, ring, bars, b1, b2, ab, total;
+  int x, h, ring, bars, b1, b2, total;
   __host__ __device__ MlpSmem(int E, int Hd, int ring_depth) {
     const int slot = (E > kMlpHc ? E : kMlpHc) * kConvBK * 2;
     x = 0;                                          // E/64 tiles of [128 rows x 64] (the staging area at the end)
@@ -57,8 +48,7 @@ struct MlpSmem {
     bars = ring + ring_depth * slot;
     b1 = bars + 1024;
     b2 = b1 + Hd * 4;
-    ab = b2 + E * 4;                                // [2][E][2] input-GN affine, then [2][32][2] group (mean, rstd)
-    total = ab + (4 * E + 128) * 4;
+    total = b2 + E * 4;
   }
 };
 
@@ -83,7 +73,6 @@ __global__ void __launch_bounds__(kMlpThreads, 1) mlp_fused_sm90_kernel(const __
   uint64_t* res_bar = x_full + 1;
   float* s_b1 = reinterpret_cast<float*>(smem + L.b1);
   float* s_b2 = reinterpret_cast<float*>(smem + L.b2);
-  float* s_ab = reinterpret_cast<float*>(smem + L.ab);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int chunks = p.Hd / kMlpHc;
@@ -91,7 +80,6 @@ __global__ void __launch_bounds__(kMlpThreads, 1) mlp_fused_sm90_kernel(const __
   const int tw = mt % p.tiles_w; mt /= p.tiles_w;
   const int th = mt % p.tiles_h; mt /= p.tiles_h;
   const int w0 = tw * p.bw, h0 = th * p.bh, n0 = mt * p.bn;
-  const bool gn_in = p.gn_in_gstat || p.gn_in_part;
 
   if (warp == kMlpTmaWarp && lane == 0) {
     tma_prefetch_desc(&p.tmX); tma_prefetch_desc(&p.tmW1); tma_prefetch_desc(&p.tmW2);
@@ -139,72 +127,10 @@ __global__ void __launch_bounds__(kMlpThreads, 1) mlp_fused_sm90_kernel(const __
   const int rA = 64 * wg + 16 * (warp & 3) + (lane >> 2), rB = rA + 8;
   const int etid = threadIdx.x;
   constexpr int kCons = 32 * kConvEpiWarps;
-  if (gn_in) {
-    // ---- fused input GroupNorm: statistics -> per-(image, channel) affine (same arithmetic and order as gn_apply_kernel) ----
-    const int cpg = E / 32;
-    const int nimg = p.bn;                                       // images this tile touches (1 or 2)
-    float* s_mr = s_ab + 2 * E * 2;                              // [2][32][2] group (mean, rstd)
-    if (p.gn_in_gstat) {
-      if (etid < 32 * nimg) {
-        const int img = etid >> 5, g = etid & 31;
-        float2 mr = make_float2(0.f, 0.f);
-        if (n0 + img < p.Nimg) mr = ldcg_f2(p.gn_in_gstat + ((size_t)(n0 + img) * 32 + g) * 2);
-        s_mr[(img * 32 + g) * 2] = mr.x; s_mr[(img * 32 + g) * 2 + 1] = mr.y;
-      }
-    } else {
-      float* s_ch = s_b1;                                        // scratch [2][E][2] (bias1 is loaded afterwards; Hd >= 4E)
-      const float ns = (float)(p.Hout * p.Wout) / (float)p.gn_in_slots;
-      for (int idx = etid; idx < nimg * E; idx += kCons) {
-        const int img = idx / E, c = idx - img * E;
-        float2 mq = make_float2(0.f, 0.f);
-        if (n0 + img < p.Nimg)
-          mq = gn_channel_from_pairs(p.gn_in_part + (size_t)(n0 + img) * p.gn_in_slots * E * 2 + (size_t)c * 2, p.gn_in_slots, E, ns);
-        s_ch[(img * E + c) * 2] = mq.x; s_ch[(img * E + c) * 2 + 1] = mq.y;
-      }
-      named_bar_sync(1, kCons);
-      if (etid < 32 * nimg) {
-        const int img = etid >> 5, g = etid & 31;
-        float chp[2 * 8];                                        // cpg <= 8 (E <= 256)
-        for (int j = 0; j < cpg; ++j) { chp[2 * j] = s_ch[(img * E + g * cpg + j) * 2]; chp[2 * j + 1] = s_ch[(img * E + g * cpg + j) * 2 + 1]; }
-        const float2 mr = gn_group_from_channels(chp, cpg, (float)(p.Hout * p.Wout), p.gn_in_eps);
-        s_mr[(img * 32 + g) * 2] = mr.x; s_mr[(img * 32 + g) * 2 + 1] = mr.y;
-      }
-    }
-    named_bar_sync(1, kCons);
-    for (int idx = etid; idx < nimg * E; idx += kCons) {
-      const int img = idx / E, c = idx - img * E, g = c / cpg;
-      const float a = s_mr[(img * 32 + g) * 2 + 1] * __ldg(p.gn_in_gamma + c);
-      const float b = __ldg(p.gn_in_beta + c) - s_mr[(img * 32 + g) * 2] * a;
-      s_ab[(img * E + c) * 2] = a; s_ab[(img * E + c) * 2 + 1] = b;
-    }
-    named_bar_sync(1, kCons);                                    // the scratch aliasing the bias area is free again
-  }
   for (int i = etid; i < p.Hd; i += kCons) s_b1[i] = __ldg(p.bias1 + i);
   for (int i = etid; i < E; i += kCons) s_b2[i] = __ldg(p.bias2 + i);
   mbar_wait(x_full, 0);
-  if (gn_in) {
-    // in place: 128 rows x kx x eight 16-byte units (8 channels each); unit u of row rr sits at (u ^ (rr & 7))
-    const int rows_per_img = p.bw * p.bh;                         // bn == 2: rows 0..63 -> image n0, 64..127 -> n0 + 1
-    for (int idx = etid; idx < kx * kConvBM * 8; idx += kCons) {
-      const int kb = idx / (kConvBM * 8), rem = idx - kb * (kConvBM * 8);
-      const int rr = rem >> 3, us = rem & 7;
-      const int ch = kb * 64 + ((us ^ (rr & 7)) << 3);
-      const float* ab = s_ab + ((size_t)(p.bn == 2 && rr >= rows_per_img ? E : 0) + ch) * 2;
-      uint4* ptr = reinterpret_cast<uint4*>(sX + (size_t)kb * kTile + rr * 128 + us * 16);
-      uint4 raw = *ptr;
-      __half2* hh = reinterpret_cast<__half2*>(&raw);
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        float2 f = __half22float2(hh[j]);
-        f.x = fmaf(f.x, ab[(2 * j) * 2], ab[(2 * j) * 2 + 1]);
-        f.y = fmaf(f.y, ab[(2 * j + 1) * 2], ab[(2 * j + 1) * 2 + 1]);
-        hh[j] = __floats2half2_rn(f.x, f.y);
-      }
-      *ptr = raw;
-    }
-    fence_proxy_async_smem();                                     // the tensor core reads X through the async proxy
-  }
-  named_bar_sync(1, kCons);                                       // biases (and the normalised X tile) visible
+  named_bar_sync(1, kCons);                                       // biases visible
 
   const uint32_t sX0 = smem_u32(sX), sH0 = smem_u32(sH), sR0 = smem_u32(sRing);
   int stage = 0; uint32_t phase = 0;

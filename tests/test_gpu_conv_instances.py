@@ -31,7 +31,7 @@ KAPPA = 2.0 ** -18
 ACT_GAIN = 1.13
 INFO_KEYS = ("grid", "BN", "msub", "stages", "cg", "splitk", "persist", "epi_bc", "bw", "bh", "box_n", "gn_slots")
 _ENV = ("RS_CONV_CG", "RS_CONV_MSUB", "RS_CONV_PERSIST", "RS_CONV_SPLITK", "RS_CONV_EPI", "RS_CONV_IMPL", "RS_CONV_BN",
-        "RS_CONV_OCC", "RS_CONV_STAGES")
+        "RS_CONV_OCC")
 # forced modes: environment and the (cg, msub, persist) the entry must report; msub is required through rs_conv_args
 MODES = {
     "one_tile": ({"RS_CONV_CG": 1, "RS_CONV_PERSIST": 0}, (1, 1, 0)),
