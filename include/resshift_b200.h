@@ -326,6 +326,35 @@ int rs_op_groupnorm_apply_pairs(const void* x, int N, int H, int W, int C, int l
 /* group statistics gstat[N][32][2] = (mean, rstd) from (mean, M2) pairs part[N][slots][C][2] (rows_per_slot values each)
  * as a kernel of its own — what the first-stage plans run in front of a GroupNorm whose producer has hundreds of tiles */
 int rs_op_groupnorm_finalize(const float* part, int N, int slots, int C, int rows_per_slot, float eps, float* gstat, void* stream);
+/* GroupNorm statistics routes of rs_op_groupnorm_ex: where the (mean, M2) pairs part[N][slots][C][2] come from and who
+ * reduces them to the group statistics.  A plan picks one per GroupNorm by shape (rs_plan_profile_ops names it). */
+#define RS_GN_GSTAT 0         /* the caller's gstat[N][32][2] = (group mean, group rstd): apply only                    */
+#define RS_GN_CONV_PAIRS 1    /* the caller's pairs in equal slots (a conv / MLP epilogue: one per 128-pixel tile),
+                                 combined by every apply CTA                                                            */
+#define RS_GN_WINDOW_PAIRS 2  /* the same from the fused Swin attention: slots = (H/8)(W/8) windows of 64 pixels        */
+#define RS_GN_FINALIZE 3      /* the caller's pairs reduced into the caller's gstat by a finalisation kernel, then apply */
+#define RS_GN_STATS_PAIRS 4   /* a statistics kernel writes part (slots 0: the library's chunking), apply combines      */
+#define RS_GN_STATS_GSTAT 5   /* ... and its last CTA per image reduces into gstat (arrival counters[N], zeroed here)    */
+/* Every option of the GroupNorm launcher.  rs_op_groupnorm, _apply and _apply_pairs are rs_op_groupnorm_ex with
+ * routes RS_GN_STATS_GSTAT, RS_GN_GSTAT and RS_GN_CONV_PAIRS. */
+typedef struct rs_gn_args {
+  const void* x; int32_t x_ld;                  /* NHWC fp16 input view [N][H][W][C], row stride x_ld >= C            */
+  void* y; int32_t y_ld;                        /* output view; channels outside [0, C) of each row are not written    */
+  int32_t N, H, W, C;                           /* C a multiple of 32, at most 2048                                    */
+  const float* gamma; const float* beta;        /* [C]                                                                 */
+  const float* film; long long film_sN;         /* optional FiLM rows: scale film[n sN + c], shift film[n sN + C + c];
+                                                   film_sN = 0 shares one row between all images                       */
+  int32_t silu;                                 /* 1: SiLU after the affine                                            */
+  float eps;                                    /* > 0 (GroupNorm32: 1e-5 in the UNet, 1e-6 in the VQ-GAN / KL)        */
+  int32_t route;                                /* RS_GN_*                                                             */
+  float* part; int32_t slots;                   /* pairs [N][slots][C][2]: given (pairs / finalize routes) or written   */
+  float* gstat;                                 /* [N][32][2] (mean, rstd): given (RS_GN_GSTAT) or written              */
+  uint32_t* counter;                            /* [N] arrival counters of RS_GN_STATS_GSTAT                           */
+} rs_gn_args;
+/* info[8] (optional) = route, slots, rows per slot, statistics-kernel CTAs per image (0: none), finalisation kernel
+ * ran (0 / 1), apply CTAs per image and channel slice, rows per apply CTA, channel slices.  The route is launched as
+ * asked or refused with a message, never replaced by another. */
+int rs_op_groupnorm_ex(const rs_gn_args* a, int32_t* info, void* stream);
 /* single-head attention over all T positions of each image, out = softmax(q k^T C^-1/2) v (reference
  * ldm/modules/diffusionmodules/model.py:180-199, AttnBlock.forward between the q/k/v convs and proj_out; the VQ-GAN
  * plans run it for bottlenecks with H*W > 8192).  q, k, v fp16 [N][T][C] with row stride ld; out fp16 [N][T][C] dense.

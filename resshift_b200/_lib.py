@@ -70,6 +70,21 @@ class ConvArgsC(C.Structure):
     ]
 
 
+# GroupNorm statistics routes (RS_GN_*)
+GN_GSTAT, GN_CONV_PAIRS, GN_WINDOW_PAIRS, GN_FINALIZE, GN_STATS_PAIRS, GN_STATS_GSTAT = range(6)
+
+
+class GnArgsC(C.Structure):
+    """Mirror of ``rs_gn_args``."""
+    _fields_ = [
+        ("x", C.c_void_p), ("x_ld", C.c_int32), ("y", C.c_void_p), ("y_ld", C.c_int32),
+        ("N", C.c_int32), ("H", C.c_int32), ("W", C.c_int32), ("C", C.c_int32),
+        ("gamma", C.c_void_p), ("beta", C.c_void_p), ("film", C.c_void_p), ("film_sN", C.c_longlong),
+        ("silu", C.c_int32), ("eps", C.c_float), ("route", C.c_int32),
+        ("part", C.c_void_p), ("slots", C.c_int32), ("gstat", C.c_void_p), ("counter", C.c_void_p),
+    ]
+
+
 # every symbol include/resshift_b200.h declares: (restype, argtypes)
 _P = C.c_void_p
 _SIGNATURES = {
@@ -119,6 +134,7 @@ _SIGNATURES = {
     "rs_op_groupnorm_apply": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P, _P, C.c_longlong, C.c_int,
                                         _P, C.c_int, _P, _P]),
     "rs_op_groupnorm_finalize": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, _P, _P]),
+    "rs_op_groupnorm_ex": (C.c_int, [C.POINTER(GnArgsC), C.POINTER(C.c_int32), _P]),
     "rs_op_groupnorm_apply_pairs": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P, _P, C.c_longlong,
                                               C.c_int, _P, C.c_int, _P, C.c_int, _P]),
     "rs_op_expand_relpos": (C.c_int, [_P, _P, C.c_int, _P]),

@@ -1416,8 +1416,9 @@ int rs_plan_profile(rs_plan* p, const float* x, const float* timesteps, const fl
   return 0;
 }
 
-// per-operator times + one-line descriptions of a profiled run_ops() pass
-static void collect_profile(const rs_plan& P, const Prof& prof, double* ms, char* desc, int desc_stride, int cap, int32_t* n_ops) {
+// per-operator times + one-line descriptions of a profiled run_ops() pass (film_sN: the FiLM row stride it ran with)
+static void collect_profile(const rs_plan& P, const Prof& prof, double* ms, char* desc, int desc_stride, int cap, int32_t* n_ops,
+                            long long film_sN) {
   const int n = std::min<int>((int)P.ops.size(), cap);
   *n_ops = n;
   for (int i = 0; i < n; ++i) {
@@ -1437,9 +1438,16 @@ static void collect_profile(const rs_plan& P, const Prof& prof, double* ms, char
                  cd.act, (int)cd.has_res, (int)(cd.out_f32 != nullptr));
         break;
       }
-      case OP_GN: {
-        const GnLink& g = payload<GnOp>(op).stats;
-        snprintf(d, desc_stride, "gn %dx%d C=%d fused=%d %s", g.in.H, g.in.W, g.in.C, (int)g.fused, payload<GnOp>(op).name.c_str());
+      case OP_GN: {   // everything rs_op_groupnorm_ex needs to replay it, and the launch geometry it should report
+        const GnOp& o = payload<GnOp>(op);
+        const GnLink& g = o.stats;
+        const GnGeometry geo = gn_geometry(o.d);
+        const char* route = g.win_slots ? "window_pairs" : g.fused ? (gn_finalizes(g) ? "finalize" : "conv_pairs")
+                                                                   : (gn_finalizes(g) ? "stats_gstat" : "stats_pairs");
+        const char* film = o.d.film_off < 0 ? "none" : film_sN > 0 ? "image" : "shared";
+        snprintf(d, desc_stride, "gn %dx%d C=%d N=%d route=%s slots=%d eps=%g silu=%d film=%s@%d apply=%d rows=%d csplit=%d %s",
+                 g.in.H, g.in.W, g.in.C, g.in.N, route, geo.slots, (double)g.eps, o.d.silu, film, o.d.film_off, geo.apply_ctas,
+                 geo.apply_rows, geo.csplit, o.name.c_str());
         break;
       }
       case OP_MLP: { const MlpDesc& m = payload<MlpOp>(op).d; snprintf(d, desc_stride, "mlp %dx%d E=%d Hd=%d grid=%d", m.in.H, m.in.W, m.E, m.Hd, m.grid); break; }
@@ -1471,7 +1479,7 @@ int rs_plan_profile_ops(rs_plan* p, const float* x, const float* timesteps, cons
   Prof prof;
   int rc = run_forward(*p, x, timesteps, lq, mask, st, &prof); if (rc) return rc;
   RS_CUDA_OK(cudaStreamSynchronize(st));
-  collect_profile(*p, prof, ms, desc, desc_stride, cap, n_ops);
+  collect_profile(*p, prof, ms, desc, desc_stride, cap, n_ops, p->e->film_rows);
   return 0;
 }
 

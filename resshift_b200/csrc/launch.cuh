@@ -603,49 +603,72 @@ inline void gn_chunks(int HW, int N, int* chunks, int* rows) {
   *chunks = c; *rows = HW / c;
 }
 
+// The launch geometry of one GroupNorm (host only; gn_launch launches exactly this)
+struct GnGeometry {
+  int slots = 0;          // pair slots per image (the producers', or gn_stats_kernel's CTAs per image)
+  int rows_per_slot = 0;
+  int stats_ctas = 0;     // gn_stats_kernel CTAs per image (0: the producers delivered the pairs)
+  bool finalize = false;  // gn_finalize_kernel runs in front of the apply
+  int apply_ctas = 0;     // gn_apply_kernel grid.x (row blocks per image)
+  int apply_rows = 0;     // rows per apply CTA
+  int csplit = 1;         // gn_apply_kernel grid.z (channel slices)
+};
+
+inline GnGeometry gn_geometry(const GnDesc& g) {
+  const int C = g.in.C, HW = g.in.H * g.in.W, N = g.in.N;
+  GnGeometry r;
+  r.slots = g.slots;
+  if (!g.fused) {         // gn_stats_kernel: the caller's slot count, or enough CTAs to fill the machine
+    int chunks, rows;
+    gn_chunks(HW, N, &chunks, &rows);
+    if (r.slots <= 0) r.slots = chunks;
+    r.stats_ctas = r.slots;
+  }
+  r.rows_per_slot = r.slots > 0 ? HW / r.slots : 0;
+  r.finalize = g.fused && g.finalize_kernel;
+  // apply: ~4 CTAs per SM in total, all resident at once (each CTA re-derives the per-channel affine from the
+  // partials — a latency, not a bandwidth cost), at least 16 rows each
+  int actas = std::max(1, std::min((HW + 15) / 16, (num_sms() * 4 + N - 1) / N));
+  r.apply_rows = (HW + actas - 1) / actas;
+  r.apply_ctas = (HW + r.apply_rows - 1) / r.apply_rows;
+  // small tensors: split the channels too (slices aligned to GroupNorm groups and to 8-channel vectors) until there
+  // are ~1.5 CTAs per SM — a 8x8 C=640 layer would otherwise run on 64 CTAs
+  const int cpg = C / 32;
+  int unit = cpg; while (unit % 8) unit += cpg;                     // lcm(8, channels per group)
+  for (int cs = 2; r.apply_ctas * N * r.csplit < num_sms() * 3 / 2 && cs <= C / unit; ++cs)
+    if (C % cs == 0 && (C / cs) % unit == 0) r.csplit = cs;
+  return r;
+}
+
 inline int gn_launch(const GnDesc& g, cudaStream_t st) {
   const int C = g.in.C, HW = g.in.H * g.in.W, N = g.in.N;
   RS_CHECK(C % 32 == 0 && C % 8 == 0 && C <= 2048, "GroupNorm channel count");
   RS_CHECK(g.in.ld % 8 == 0 && g.out.ld % 8 == 0, "GroupNorm view alignment");
-  int chunks, rows;
-  gn_chunks(HW, N, &chunks, &rows);
-  int slots = g.slots;
   RS_CHECK(g.gstat != nullptr || g.part != nullptr, "GroupNorm needs a statistics buffer");
+  const GnGeometry geo = gn_geometry(g);
+  const int slots = geo.slots;
   if (!g.fused) {
-    slots = chunks;
     const int lanes = 256 / (C / 8);
     RS_CHECK(g.part != nullptr && (g.gstat == nullptr || g.counter != nullptr), "GroupNorm statistics buffers");
+    RS_CHECK(HW % slots == 0, "GroupNorm statistics slots must divide H*W");
     GnStatsParams sp{};
     sp.x = g.in.ptr; sp.sN = g.in.sN(); sp.ld = g.in.ld; sp.C = C; sp.HW = HW; sp.N = N;
     sp.sink.part = g.part; sp.sink.gstat = g.gstat; sp.sink.counter = g.counter; sp.sink.cstride = C; sp.sink.coff = 0;
     sp.sink.expected = (unsigned)(slots * C); sp.sink.eps = g.eps;
-    sp.slots = slots; sp.rows_per_slot = rows;
-    (void)launch_k(gn_stats_kernel, dim3(chunks, N), dim3(256), (size_t)lanes * C * 3 * sizeof(float) + 16, st, sp);
+    sp.slots = slots; sp.rows_per_slot = geo.rows_per_slot;
+    (void)launch_k(gn_stats_kernel, dim3(geo.stats_ctas, N), dim3(256), (size_t)lanes * C * 3 * sizeof(float) + 16, st, sp);
     RS_CUDA_OK(cudaGetLastError());
   }
-  if (g.fused && g.finalize_kernel) {
+  if (geo.finalize) {
     RS_CHECK(g.part != nullptr && g.gstat != nullptr && slots > 0 && HW % slots == 0, "GroupNorm finalisation buffers");
-    GnFinalizeParams fp{g.part, g.gstat, slots, C, (float)(HW / slots), g.eps};
+    GnFinalizeParams fp{g.part, g.gstat, slots, C, (float)geo.rows_per_slot, g.eps};
     (void)launch_k(gn_finalize_kernel, dim3(32, N), dim3(256), (size_t)0, st, fp);
     RS_CUDA_OK(cudaGetLastError());
   }
-  // apply: ~4 CTAs per SM in total, all resident at once (each CTA re-derives the per-channel affine from the
-  // partials — a latency, not a bandwidth cost), at least 16 rows each
-  int actas = std::max(1, std::min((HW + 15) / 16, (num_sms() * 4 + N - 1) / N));
-  const int arows = (HW + actas - 1) / actas;
-  actas = (HW + arows - 1) / arows;
-  // small tensors: split the channels too (slices aligned to GroupNorm groups and to 8-channel vectors) until there
-  // are ~1.5 CTAs per SM — a 8x8 C=640 layer would otherwise run on 64 CTAs
-  int csplit = 1;
-  {
-    const int cpg = C / 32;
-    int unit = cpg; while (unit % 8) unit += cpg;                   // lcm(8, channels per group)
-    for (int cs = 2; actas * N * csplit < num_sms() * 3 / 2 && cs <= C / unit; ++cs)
-      if (C % cs == 0 && (C / cs) % unit == 0) csplit = cs;
-  }
   GnApplyParams ap{g.in.ptr, g.in.sN(), g.in.ld, g.out.ptr, g.out.sN(), g.out.ld, C, HW, N, g.gstat, g.part, slots, g.eps,
-                   g.gamma, g.beta, g.film, g.film_sN, g.silu, arows, C / csplit};
-  (void)launch_k(gn_apply_kernel, dim3(actas, N, csplit), dim3(256), (size_t)(4 * (C / csplit) + 64) * sizeof(float), st, ap);
+                   g.gamma, g.beta, g.film, g.film_sN, g.silu, geo.apply_rows, C / geo.csplit};
+  (void)launch_k(gn_apply_kernel, dim3(geo.apply_ctas, N, geo.csplit), dim3(256),
+                 (size_t)(4 * (C / geo.csplit) + 64) * sizeof(float), st, ap);
   RS_CUDA_OK(cudaGetLastError());
   return 0;
 }
