@@ -90,6 +90,23 @@ typedef struct rs_unetmodel_config {
   int32_t use_new_attention_order;
 } rs_unetmodel_config;
 
+/* Keyword arguments of UNetModelConv.__init__ (reference models/unet.py:1026-1040), the attention- and GroupNorm-free
+ * UNet of ResBlockConv blocks (:914-1004).  As for UNetModel, x has out_channels channels and in_channels - out_channels
+ * is 3 (lq at the latent size) or 12 (lq at twice it, pixel_unshuffle).  Refused by rs_unetconv_create, with the reason
+ * in the message: dims != 2, cond_lq == 0, any other in_channels, channel counts the conv kernels cannot take
+ * (model_channels * channel_mult not a multiple of 8).  Latent H and W must be multiples of 2^(n_levels - 1)
+ * (rs_plan_create). */
+typedef struct rs_unetconv_config {
+  int32_t in_channels;
+  int32_t model_channels;
+  int32_t out_channels;
+  int32_t n_levels;
+  int32_t channel_mult[RS_MAX_LEVELS];
+  int32_t num_res_blocks[RS_MAX_LEVELS];
+  int32_t cond_lq;
+  int32_t dims;
+} rs_unetconv_config;
+
 /* ``autoencoder.params`` of the shipped yaml files: VQModelTorch(ddconfig, n_embed, embed_dim)
  * (reference ldm/models/autoencoder.py:12-26; ddconfig -> ldm/modules/diffusionmodules/model.py:452-470,563-581).
  * Covered: double_z = False, attn_resolutions = [], dropout = 0 (every shipped config). */
@@ -120,6 +137,10 @@ int rs_unet_create_ex(const rs_unet_config* cfg, const rs_unet_options* opts, rs
  * (parameters, plans, forward / profile / probe, samplers); rs_plan_forward's lq is [B, 3, H, W] or [B, 3, 2H, 2W]
  * as in_channels says, and mask must be NULL.  Its AttentionBlocks run unet_attn (rs_op_unet_attention). */
 int rs_unetmodel_create(const rs_unetmodel_config* cfg, const rs_unet_options* opts, rs_engine** out);
+/* models.unet.UNetModelConv (reference models/unet.py:1006-1181).  opts as for rs_unetmodel_create (patch_norm must be
+ * 0); every entry point below works with it, with rs_plan_forward's lq and mask as for UNetModel.  Its ResBlockConv
+ * blocks read every tensor raw and through SiLU: the producing conv / resample writes both (rs_conv_args.silu_out). */
+int rs_unetconv_create(const rs_unetconv_config* cfg, const rs_unet_options* opts, rs_engine** out);
 void rs_unet_destroy(rs_engine* e);
 /* state_dict inventory (reference key names / shapes; utils/util_net.py:86-98 relies on them) */
 int rs_unet_param_count(const rs_engine* e);
@@ -285,7 +306,7 @@ typedef struct rs_conv_args {
   const void* x; int32_t N, H, W, C, ld;        /* NHWC fp16 input view, row stride ld                              */
   const void* w_packed; int32_t ipad;           /* fp16 [Cout][k*k][ipad] from rs_op_pack_conv_weight                */
   const float* bias; int32_t bias_sN;           /* [Cout] fp32 or NULL; bias_sN > 0: one row per image at
-                                                   bias + n * bias_sN (tiles of at most 8 images, one sub-tile)       */
+                                                   bias + n * bias_sN (one sub-tile)                                  */
   int32_t cout, ksize, stride;
   int32_t pad_lo;                               /* stride 2 only: 1 = padding 1 on every side, 0 = pad (0, 1, 0, 1)  */
   const void* residual; int32_t res_ld;         /* optional fp16 view on the output grid                             */
@@ -299,6 +320,12 @@ typedef struct rs_conv_args {
   int32_t cstride[2], coff[2];
   float* gstat;                                 /* optional [N][32][2] group (mean, rstd) of all channels of sink 0  */
   float* splitk_scratch;                        /* non-NULL allows split-K: 8 * N * Ho * Wo * Cout floats            */
+  void* silu_out; int32_t silu_ld;              /* optional second fp16 output view: SiLU of every fp16 value stored to
+                                                   out (needs out), row stride silu_ld                               */
+  const float* film; int32_t film_sN;           /* optional FiLM after the activation: with v = fp16(act(acc + bias)),
+                                                   out = fp16(v * (1 + film[n film_sN + c]) + film[n film_sN + cout + c]);
+                                                   film_sN 0 shares one row; no residual or statistics sinks, one
+                                                   sub-tile, cout % 8 == 0 (silu_out too)                            */
 } rs_conv_args;
 /* info[12] (optional) = the configuration launched: grid, BN, msub, stages, CTAs per tile group, split-K factor,
  * persistent (0 / 1), staging block width of the TMA epilogue (0: direct epilogue), pixel box bw / bh / bn, statistics
@@ -411,6 +438,11 @@ int rs_op_mlp_ex(const void* x, int N, int H, int W, int E, int Hd, const void* 
 int rs_debug_tile_config(int m_tiles, int cout, int num_kblocks, int32_t* out);
 /* nearest x2 (reference models/unet.py:71-81) */
 int rs_op_upsample2x(const void* x, int N, int H, int W, int C, void* y, void* stream);
+/* the same with an optional second output silu_y (NULL: none) = SiLU of every fp16 value stored to y; dense NHWC, C % 8 == 0 */
+int rs_op_upsample2x_ex(const void* x, int N, int H, int W, int C, void* y, void* silu_y, void* stream);
+/* 2x2 average pool (Downsample without conv, reference models/unet.py:83-108): x [N,H,W,C] -> y [N,H/2,W/2,C] dense
+ * NHWC fp16, H and W even, C % 8 == 0; silu_y as rs_op_upsample2x_ex */
+int rs_op_avgpool2x2(const void* x, int N, int H, int W, int C, void* y, void* silu_y, void* stream);
 
 #ifdef __cplusplus
 }

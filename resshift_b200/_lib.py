@@ -48,6 +48,15 @@ class UNetModelConfigC(C.Structure):
     ]
 
 
+class UNetConvConfigC(C.Structure):
+    """Mirror of ``rs_unetconv_config``."""
+    _fields_ = [
+        ("in_channels", C.c_int32), ("model_channels", C.c_int32), ("out_channels", C.c_int32), ("n_levels", C.c_int32),
+        ("channel_mult", C.c_int32 * RS_MAX_LEVELS), ("num_res_blocks", C.c_int32 * RS_MAX_LEVELS),
+        ("cond_lq", C.c_int32), ("dims", C.c_int32),
+    ]
+
+
 class VQConfigC(C.Structure):
     """Mirror of ``rs_vq_config``."""
     _fields_ = [
@@ -67,6 +76,7 @@ class ConvArgsC(C.Structure):
         ("out_f32_nchw", C.c_void_p), ("act", C.c_int32), ("bn", C.c_int32), ("msub", C.c_int32),
         ("part", C.c_void_p * 2), ("cstride", C.c_int32 * 2), ("coff", C.c_int32 * 2),
         ("gstat", C.c_void_p), ("splitk_scratch", C.c_void_p),
+        ("silu_out", C.c_void_p), ("silu_ld", C.c_int32), ("film", C.c_void_p), ("film_sN", C.c_int32),
     ]
 
 
@@ -93,6 +103,7 @@ _SIGNATURES = {
     "rs_unet_create": (C.c_int, [C.POINTER(UNetConfigC), C.POINTER(_P)]),
     "rs_unet_create_ex": (C.c_int, [C.POINTER(UNetConfigC), C.POINTER(UNetOptionsC), C.POINTER(_P)]),
     "rs_unetmodel_create": (C.c_int, [C.POINTER(UNetModelConfigC), C.POINTER(UNetOptionsC), C.POINTER(_P)]),
+    "rs_unetconv_create": (C.c_int, [C.POINTER(UNetConvConfigC), C.POINTER(UNetOptionsC), C.POINTER(_P)]),
     "rs_unet_destroy": (None, [_P]),
     "rs_unet_param_count": (C.c_int, [_P]),
     "rs_unet_param_info": (C.c_int, [_P, C.c_int, C.c_char_p, C.c_size_t, C.POINTER(C.c_int32), C.POINTER(C.c_int32),
@@ -152,6 +163,8 @@ _SIGNATURES = {
                                C.POINTER(_P), C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(C.c_int32), _P]),
     "rs_debug_tile_config": (C.c_int, [C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int32)]),
     "rs_op_upsample2x": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P]),
+    "rs_op_upsample2x_ex": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P, _P]),
+    "rs_op_avgpool2x2": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P, _P]),
     "rs_vq_create": (C.c_int, [C.POINTER(VQConfigC), C.POINTER(_P)]),
     "rs_vq_plan_create": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(_P)]),
     "rs_vq_encode": (C.c_int, [_P, _P, _P, _P]),
@@ -252,6 +265,18 @@ def make_unetmodel_config(cfg) -> UNetModelConfigC:
         c.attention_resolutions[i] = int(v)
     c.num_heads, c.num_head_channels = cfg.num_heads, cfg.num_head_channels
     c.use_new_attention_order = int(cfg.use_new_attention_order)
+    return c
+
+
+def make_unetconv_config(cfg) -> UNetConvConfigC:
+    c = UNetConvConfigC()
+    c.in_channels, c.model_channels, c.out_channels = cfg.in_channels, cfg.model_channels, cfg.out_channels
+    c.n_levels = len(cfg.channel_mult)
+    for i, v in enumerate(cfg.channel_mult):
+        c.channel_mult[i] = int(v)
+    for i, v in enumerate(cfg.num_res_blocks):
+        c.num_res_blocks[i] = int(v)
+    c.cond_lq, c.dims = int(cfg.cond_lq), int(cfg.dims)
     return c
 
 

@@ -21,7 +21,7 @@ from __future__ import annotations
 
 from typing import List, Tuple
 
-from .config import UNetConfig, UNetModelConfig
+from .config import UNetConfig, UNetModelConfig, UNetModelConvConfig
 
 Spec = Tuple[str, Tuple[int, ...], str]
 
@@ -63,7 +63,7 @@ def latent_multiple(cfg) -> int:
     """What H and W of a latent must be multiples of: every level's map (H / 2^level) is tiled by that level's window
     (UNetModel: the levels only have to halve evenly)."""
     import math
-    if isinstance(cfg, UNetModelConfig):
+    if isinstance(cfg, (UNetModelConfig, UNetModelConvConfig)):
         return 2 ** (len(cfg.channel_mult) - 1)
     m = 1
     for level in range(len(cfg.channel_mult)):
@@ -262,6 +262,80 @@ def unetmodel_param_spec(cfg: UNetModelConfig) -> List[Spec]:
     ch0 = int(cfg.channel_mult[0] * cfg.model_channels)
     s += _gn("out.0", ch0)
     s += _conv("out.2", ch0, cfg.out_channels, 3)
+    return s
+
+
+def unetconv_block_plan(cfg: UNetModelConvConfig):
+    """Topology of UNetModelConv (reference models/unet.py:1064-1146) in the form of ``unet_block_plan``: ``res`` layers
+    are ResBlockConv, no attention, two ResBlockConv in the middle."""
+    down = "res_down" if cfg.resblock_updown else "down"
+    up = "res_up" if cfg.resblock_updown else "up"
+    mc = cfg.model_channels
+    ch = int(cfg.channel_mult[0] * mc)
+    input_blocks = [[("conv", cfg.in_channels, ch)]]
+    chans = [ch]
+    for level, mult in enumerate(cfg.channel_mult):
+        for _ in range(cfg.num_res_blocks[level]):
+            input_blocks.append([("res", ch, int(mult * mc))])
+            ch = int(mult * mc)
+            chans.append(ch)
+        if level != len(cfg.channel_mult) - 1:
+            input_blocks.append([(down, ch)])
+            chans.append(ch)
+    middle = [("res", ch, ch), ("res", ch, ch)]
+    output_blocks = []
+    for level, mult in list(enumerate(cfg.channel_mult))[::-1]:
+        for i in range(cfg.num_res_blocks[level] + 1):
+            ich = chans.pop()
+            layers = [("res", ch + ich, int(mc * mult))]
+            ch = int(mc * mult)
+            if level and i == cfg.num_res_blocks[level]:
+                layers.append((up, ch))
+            output_blocks.append(layers)
+    return input_blocks, middle, output_blocks
+
+
+def _resblock_conv(name: str, cin: int, cout: int, emb: int, scale_shift: bool) -> List[Spec]:
+    """ResBlockConv (reference models/unet.py:914-982): in_layers = [SiLU, conv], out_layers = [SiLU, conv]."""
+    s: List[Spec] = []
+    s += _conv(f"{name}.in_layers.1", cin, cout, 3)
+    s += _linear(f"{name}.emb_layers.1", emb, (2 if scale_shift else 1) * cout)
+    s += _conv(f"{name}.out_layers.1", cout, cout, 3)
+    if cin != cout:
+        s += _conv(f"{name}.skip_connection", cin, cout, 1)
+    return s
+
+
+def unetconv_param_spec(cfg: UNetModelConvConfig) -> List[Spec]:
+    """UNetModelConv's ``state_dict`` (reference models/unet.py:1057-1151): no GroupNorm parameters, head ``out.1``."""
+    emb = cfg.time_embed_dim
+    s: List[Spec] = []
+    s += _linear("time_embed.0", cfg.model_channels, emb)
+    s += _linear("time_embed.2", emb, emb)
+    input_blocks, middle, output_blocks = unetconv_block_plan(cfg)
+
+    def emit(prefix: str, layers):
+        out: List[Spec] = []
+        for j, layer in enumerate(layers):
+            kind, p = layer[0], f"{prefix}.{j}"
+            if kind == "conv":
+                out += _conv(p, layer[1], layer[2], 3)
+            elif kind == "res":
+                out += _resblock_conv(p, layer[1], layer[2], emb, cfg.use_scale_shift_norm)
+            elif kind in ("res_down", "res_up"):
+                out += _resblock_conv(p, layer[1], layer[1], emb, cfg.use_scale_shift_norm)
+            elif kind == "down" and cfg.conv_resample:
+                out += _conv(f"{p}.op", layer[1], layer[1], 3)
+            elif kind == "up" and cfg.conv_resample:
+                out += _conv(f"{p}.conv", layer[1], layer[1], 3)
+        return out
+
+    for i, layers in enumerate(input_blocks):
+        s += emit(f"input_blocks.{i}", layers)
+    s += emit("middle_block", middle)
+    for i, layers in enumerate(output_blocks):
+        s += emit(f"output_blocks.{i}", layers)
+    s += _conv("out.1", int(cfg.channel_mult[0] * cfg.model_channels), cfg.out_channels, 3)
     return s
 
 

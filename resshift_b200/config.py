@@ -180,6 +180,62 @@ class UNetModelConfig:
 
 
 @dataclass
+class UNetModelConvConfig:
+    """Exactly the keyword arguments of ``UNetModelConv.__init__`` (reference models/unet.py:1026-1040), the UNet of
+    attention- and GroupNorm-free ``ResBlockConv`` blocks.  What the native kernels cannot run is refused here with the
+    reason.  ``use_fp16`` is accepted and has no effect: precision is fixed by the kernels."""
+    in_channels: int = 6
+    model_channels: int = 160
+    out_channels: int = 3
+    num_res_blocks: Sequence[int] = (2, 2, 2, 2)
+    cond_lq: bool = True
+    channel_mult: Sequence[int] = (1, 2, 4, 8)
+    conv_resample: bool = True
+    dims: int = 2
+    use_scale_shift_norm: bool = False
+    resblock_updown: bool = False
+    use_fp16: bool = False
+
+    def __post_init__(self):
+        if isinstance(self.num_res_blocks, int):
+            self.num_res_blocks = (self.num_res_blocks,) * len(self.channel_mult)
+        self.num_res_blocks = tuple(int(v) for v in self.num_res_blocks)
+        self.channel_mult = tuple(int(v) for v in self.channel_mult)
+        if len(self.num_res_blocks) != len(self.channel_mult):
+            raise ValueError("num_res_blocks and channel_mult must have the same length")
+        if not 1 <= len(self.channel_mult) <= 8:
+            raise ValueError(f"{len(self.channel_mult)} levels: the engine takes 1 to 8")
+        if self.dims != 2:
+            raise ValueError(f"dims={self.dims}: only 2-D UNets are covered (every ResShift config uses dims=2)")
+        if not self.cond_lq:
+            raise ValueError("cond_lq=False: the ResShift sampler always passes lq, and the reference asserts cond_lq then")
+        if self.in_channels - self.out_channels not in (3, 12):
+            raise ValueError(f"in_channels={self.in_channels}, out_channels={self.out_channels}: x has out_channels "
+                             f"channels and lq is a 3-channel image, so in_channels must be out_channels + 3 (lq at the "
+                             f"latent size) or out_channels + 12 (lq at twice it, through pixel_unshuffle)")
+        for level, mult in enumerate(self.channel_mult):
+            if mult <= 0 or self.model_channels <= 0 or (self.model_channels * mult) % 8:
+                raise ValueError(f"level {level} has {self.model_channels * mult} channels: the conv kernels read and "
+                                 f"write 16-byte channel rows, so model_channels * channel_mult must be a positive "
+                                 f"multiple of 8")
+
+    @property
+    def lq_factor(self) -> int:
+        """1: lq enters at the latent size; 2: at twice it, through F.pixel_unshuffle(lq, 2) (reference :1166-1167)."""
+        return 2 if self.in_channels - self.out_channels == 12 else 1
+
+    @property
+    def time_embed_dim(self) -> int:
+        return self.model_channels * 4
+
+    def to_kwargs(self) -> dict:
+        d = asdict(self)
+        d["num_res_blocks"] = list(self.num_res_blocks)
+        d["channel_mult"] = list(self.channel_mult)
+        return d
+
+
+@dataclass
 class DiffusionConfig:
     normalize_input: bool = True
     schedule_name: str = "exponential"

@@ -85,13 +85,25 @@ struct ConvParams {
   // unit's operands while the consumers run the epilogue of the current one (staging area outside the ring)
   int persist;
   int num_units;         // (pixel tiles or tile pairs) x channel tiles
+  // second, activated output (ResBlockConv reads every block output raw and through SiLU): silu_out = SiLU(v) of the
+  // fp16 value v stored to `out`, an NHWC fp16 view of its own (staged epilogue: through tmSilu from the same tile).
+  // Only the EX instances of the wgmma kernel (and the SIMT / split-K kernels) read silu_out and film.
+  __half* silu_out;
+  long long silu_sN, silu_sH, silu_sW;
+  CUtensorMap tmSilu;
+  // FiLM after the activation (ResBlockConv with scale-shift norm): v = fp16(act(acc + bias)), stored as
+  // fp16(v * (1 + film[n][c]) + film[n][Cout + c]) (the reference's autocast forward rounds there too); rows film_sN apart
+  // (0: one row for all images); no residual, one sub-tile.  Applied after the accumulators are dead.
+  const float* film;
+  int film_sN;
 };
 
 #ifdef __CUDACC__
 
 // Every (BN, MS) instance has the same structure; BN and the sub-tile count are template parameters because the
-// accumulators live in registers (BN / 2 floats per thread and sub-tile).
-template <int BN, int MS>
+// accumulators live in registers (BN / 2 floats per thread and sub-tile).  EX instances (one sub-tile) also have the
+// epilogue's FiLM and SiLU-output passes; the others compile without them, so the convs that use neither run the same code.
+template <int BN, int MS, bool EX = false>
 __global__ void __launch_bounds__(kConvThreads, (BN * MS <= 128) ? 2 : 1) conv_gemm_sm90_kernel(const __grid_constant__ ConvParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   // carve: [stages][MS x A 16 KB | B BN*128 B] (+ staging area when persistent), then barriers, then the bias tile
@@ -329,6 +341,29 @@ __global__ void __launch_bounds__(kConvThreads, (BN * MS <= 128) ? 2 : 1) conv_g
           }
         }
         named_bar_sync(1, 32 * kConvEpiWarps);         // the staged tile is complete
+        if (EX && MS == 1 && p.film) {
+          // FiLM on the staged fp16 values, in place once the accumulators are dead (conv_finalize: no residual, one
+          // sub-tile); every 16-byte unit reads its image's scale and shift rows
+          const int nb = mt0 / (p.tiles_w * p.tiles_h) * p.bn;     // first image of the tile
+          const int upr = bc / 8;                                  // 16-byte units per row of a block
+          for (int i = etid; i < nblk * kConvBM * upr; i += 32 * kConvEpiWarps) {
+            const int b = i / (kConvBM * upr), r = (i / upr) % kConvBM, up = i % upr;
+            const int c = col0 + b * bc + ((up ^ swz_of(r)) << 3), n = nb + r / (p.bw * p.bh);
+            if (c >= p.Cout || n >= p.Nimg) continue;                // (columns / images the stores clip)
+            uint4* unit = reinterpret_cast<uint4*>(sepi + (size_t)b * blk_bytes + r * (2 * bc) + (up << 4));
+            const float* row = p.film + (long long)n * p.film_sN + c;
+            uint4 v = *unit;
+            __half2* h = reinterpret_cast<__half2*>(&v);
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+              const float2 f = __half22float2(h[k]);
+              h[k] = __floats2half2_rn(fmaf(f.x, 1.f + __ldg(row + 2 * k), __ldg(row + p.Cout + 2 * k)),
+                                       fmaf(f.y, 1.f + __ldg(row + 2 * k + 1), __ldg(row + p.Cout + 2 * k + 1)));
+            }
+            *unit = v;
+          }
+          named_bar_sync(1, 32 * kConvEpiWarps);
+        }
         const bool want_stats = p.sink[0].part != nullptr;
         if (want_stats) {
           // statistics of the values as stored (gn_stats.cuh): warp (quad, column parity) reads back 32 rows x 16 columns
@@ -367,6 +402,35 @@ __global__ void __launch_bounds__(kConvThreads, (BN * MS <= 128) ? 2 : 1) conv_g
             if (n0 < p.Nimg)                                           // (else: padding tile of an odd pair)
               write_quad_pairs(wsum_all + (size_t)sub * 8 * BN, BN, ncols, col0, p.bn, n0, p.Nimg, slot, p.gn_slots, p.sink[0], p.sink[1],
                                etid, 32 * kConvEpiWarps);
+          }
+        }
+        if (EX && p.silu_out) {
+          // the second output from the same staged tile: once the store above has read it, SiLU of every stored fp16
+          // value in place (the staging layout is elementwise), then the same boxes through tmSilu
+          if (etid == 0) tma_store_wait_read();
+          named_bar_sync(1, 32 * kConvEpiWarps);
+          uint4* sv = reinterpret_cast<uint4*>(sepi);
+          for (int i = etid; i < MS * sub_bytes / 16; i += 32 * kConvEpiWarps) {
+            uint4 v = sv[i];
+            __half2* h = reinterpret_cast<__half2*>(&v);
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+              const float2 f = __half22float2(h[k]);
+              h[k] = __floats2half2_rn(silu_f(f.x), silu_f(f.y));
+            }
+            sv[i] = v;
+          }
+          fence_proxy_async_smem();
+          named_bar_sync(1, 32 * kConvEpiWarps);
+          if (etid == 0) {
+            for (int sub = 0; sub < MS; ++sub) {
+              int tw, th, w0, h0, n0;
+              tile_origin(mt0 + sub, tw, th, w0, h0, n0);
+              for (int b = 0; b < nblk; ++b)
+                if (col0 + b * bc < p.Cout)
+                  tma_store_4d(&p.tmSilu, sepi + (size_t)sub * sub_bytes + (size_t)b * blk_bytes, col0 + b * bc, w0, h0, n0);
+            }
+            tma_store_commit();
           }
         }
         if (etid == 0) tma_store_wait_read();
@@ -412,23 +476,25 @@ __global__ void __launch_bounds__(kConvThreads, (BN * MS <= 128) ? 2 : 1) conv_g
 // kernel instance of a (channel-tile width, sub-tiles per CTA) configuration, nullptr if none is compiled
 using ConvKernelFn = void (*)(const ConvParams);
 template <int BN>
-inline ConvKernelFn conv_kernel_ms(int msub) {
+inline ConvKernelFn conv_kernel_ms(int msub, bool ex) {
+  if (ex) return msub == 1 ? conv_gemm_sm90_kernel<BN, 1, true> : nullptr;
   if (msub == 1) return conv_gemm_sm90_kernel<BN, 1>;
   if constexpr (BN <= 128) { if (msub == 2) return conv_gemm_sm90_kernel<BN, 2>; }
   return nullptr;
 }
-inline ConvKernelFn conv_kernel_for(int bn, int msub) {
+// ex: the conv writes a SiLU output or applies FiLM rows (one sub-tile only)
+inline ConvKernelFn conv_kernel_for(int bn, int msub, bool ex = false) {
   switch (bn) {
-    case 16: return conv_kernel_ms<16>(msub);
-    case 32: return conv_kernel_ms<32>(msub);
-    case 48: return conv_kernel_ms<48>(msub);
-    case 64: return conv_kernel_ms<64>(msub);
-    case 80: return conv_kernel_ms<80>(msub);
-    case 96: return conv_kernel_ms<96>(msub);
-    case 128: return conv_kernel_ms<128>(msub);
-    case 160: return conv_kernel_ms<160>(msub);
-    case 192: return conv_kernel_ms<192>(msub);
-    case 256: return conv_kernel_ms<256>(msub);
+    case 16: return conv_kernel_ms<16>(msub, ex);
+    case 32: return conv_kernel_ms<32>(msub, ex);
+    case 48: return conv_kernel_ms<48>(msub, ex);
+    case 64: return conv_kernel_ms<64>(msub, ex);
+    case 80: return conv_kernel_ms<80>(msub, ex);
+    case 96: return conv_kernel_ms<96>(msub, ex);
+    case 128: return conv_kernel_ms<128>(msub, ex);
+    case 160: return conv_kernel_ms<160>(msub, ex);
+    case 192: return conv_kernel_ms<192>(msub, ex);
+    case 256: return conv_kernel_ms<256>(msub, ex);
     default: return nullptr;
   }
 }
@@ -477,7 +543,11 @@ __global__ void conv_simt_kernel(const __grid_constant__ ConvParams p, const __g
     else if (p.act == ACT_SILU) acc = silu_f(acc);
     if (p.residual) acc += __half2float(p.residual[n * p.res_sN + h * p.res_sH + w * p.res_sW + co]);
     if (p.out_f32_nchw) p.out_f32_nchw[(((long long)n * p.Cout + co) * p.Hout + h) * p.Wout + w] = acc;
-    if (p.out) p.out[n * p.out_sN + h * p.out_sH + w * p.out_sW + co] = __float2half_rn(acc);
+    __half v = __float2half_rn(acc);
+    if (p.film)      // on the fp16 value, as the wgmma kernel's epilogues do
+      v = __float2half_rn(fmaf(__half2float(v), 1.f + p.film[(long long)n * p.film_sN + co], p.film[(long long)n * p.film_sN + p.Cout + co]));
+    if (p.out) p.out[n * p.out_sN + h * p.out_sH + w * p.out_sW + co] = v;
+    if (p.silu_out) p.silu_out[n * p.silu_sN + h * p.silu_sH + w * p.silu_sW + co] = __float2half_rn(silu_f(__half2float(v)));
   }
 }
 

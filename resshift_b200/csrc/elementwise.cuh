@@ -84,7 +84,14 @@ struct UpsampleParams {
   const __half* x; long long x_sN; int x_ld;   // [N, H, W, C] view (the input, for both directions)
   __half* y; long long y_sN; int y_ld;         // [N, 2H, 2W, C] (upsample) or [N, H/2, W/2, C] (pool) view
   int N, H, W, C;
+  __half* s; long long s_sN; int s_ld;         // optional second output on y's grid: SiLU of every fp16 value stored to y
 };
+__device__ __forceinline__ uint4 silu_h8(uint4 v) {
+  __half2* h = reinterpret_cast<__half2*>(&v);
+#pragma unroll
+  for (int k = 0; k < 4; ++k) { const float2 f = __half22float2(h[k]); h[k] = __floats2half2_rn(silu_f(f.x), silu_f(f.y)); }
+  return v;
+}
 __global__ void avgpool2x2_kernel(const UpsampleParams p) {
   pdl_trigger();
   pdl_wait();
@@ -111,6 +118,7 @@ __global__ void avgpool2x2_kernel(const UpsampleParams p) {
 #pragma unroll
     for (int j = 0; j < 4; ++j) oh[j] = __floats2half2_rn(0.25f * acc[2 * j], 0.25f * acc[2 * j + 1]);
     *reinterpret_cast<uint4*>(p.y + n * p.y_sN + ((long long)oy * Wo + ox) * p.y_ld + v * 8) = o;
+    if (p.s) *reinterpret_cast<uint4*>(p.s + n * p.s_sN + ((long long)oy * Wo + ox) * p.s_ld + v * 8) = silu_h8(o);
   }
 }
 __global__ void upsample2x_kernel(const UpsampleParams p) {
@@ -127,6 +135,7 @@ __global__ void upsample2x_kernel(const UpsampleParams p) {
     const int n = (int)q;
     const uint4 raw = *reinterpret_cast<const uint4*>(p.x + n * p.x_sN + ((long long)(oy >> 1) * p.W + (ox >> 1)) * p.x_ld + v * 8);
     *reinterpret_cast<uint4*>(p.y + n * p.y_sN + ((long long)oy * 2 * p.W + ox) * p.y_ld + v * 8) = raw;
+    if (p.s) *reinterpret_cast<uint4*>(p.s + n * p.s_sN + ((long long)oy * 2 * p.W + ox) * p.s_ld + v * 8) = silu_h8(raw);
   }
 }
 
@@ -245,6 +254,8 @@ struct SplitKReduceParams {
   int rows_per_slot, slots;
   int cols_per_cta;         // multiple of 8; grid.z = ceil(C / cols_per_cta)
   GnSink sink[2];           // fused GroupNorm statistics of the result (gn_stats.cuh)
+  __half* silu_out; long long silu_sN; int silu_ld;   // optional: SiLU of the stored fp16 result (ConvParams::silu_out)
+  const float* film; int film_sN;                     // optional FiLM after the activation (ConvParams::film)
 };
 
 __global__ void __launch_bounds__(256) splitk_reduce_kernel(const __grid_constant__ SplitKReduceParams p) {
@@ -310,6 +321,30 @@ __global__ void __launch_bounds__(256) splitk_reduce_kernel(const __grid_constan
           for (int j = 0; j < 8; ++j) { const float d = st[j] - pv[j]; s1[j] += d; s2[j] = fmaf(d, d, s2[j]); }
         }
         ++cnt;
+      }
+    }
+    if (p.film || p.silu_out) {
+      // FiLM on the stored fp16 values and their SiLU, in a pass of their own over this thread's rows (as the conv
+      // epilogue does; conv_finalize gives FiLM neither a residual nor statistics sinks)
+      float fs[8], fh[8];
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        fs[j] = p.film ? 1.f + p.film[(long long)n * p.film_sN + c + j] : 1.f;
+        fh[j] = p.film ? p.film[(long long)n * p.film_sN + p.C + c + j] : 0.f;
+      }
+      for (int r = r0 + rl; r < r1; r += lanes) {
+        uint4* dst = reinterpret_cast<uint4*>(p.out + n * p.out_sN + (long long)r * p.out_ld + c);
+        uint4 o = *dst;
+        if (p.film) {
+          __half2* oh = reinterpret_cast<__half2*>(&o);
+#pragma unroll
+          for (int j = 0; j < 4; ++j) {
+            const float2 f = __half22float2(oh[j]);
+            oh[j] = __floats2half2_rn(fmaf(f.x, fs[2 * j], fh[2 * j]), fmaf(f.y, fs[2 * j + 1], fh[2 * j + 1]));
+          }
+          *dst = o;
+        }
+        if (p.silu_out) *reinterpret_cast<uint4*>(p.silu_out + n * p.silu_sN + (long long)r * p.silu_ld + c) = silu_h8(o);
       }
     }
     if (want_stats) {

@@ -69,6 +69,9 @@ struct rs_engine {
   // its levels with in_channels = out_channels (the channels of x) and lq_size = image_size
   bool unetmodel = false;
   rs_unetmodel_config um{};
+  // UNetModelConv (rs_unetconv_create): a UNetModel-style engine (unetmodel set, no attention levels) whose ResBlocks are
+  // ResBlockConv — SiLU and conv without GroupNorm — and whose head is conv3x3(SiLU(h))
+  bool conv_blocks = false;
   std::vector<Param> params;
   std::map<std::string, int> index;
   size_t arena_bytes = 0;
@@ -163,7 +166,8 @@ Topology build_topology(const rs_engine& e) {
     }
   }
   t.in_block_ch = chans;
-  t.middle = {{1, ch, ch}, {e.unetmodel ? L_ATTN : L_SWIN, ch, e.unetmodel ? e.attn_heads(ch, false) : ds}, {1, ch, ch}};
+  if (e.conv_blocks) t.middle = {{1, ch, ch}, {1, ch, ch}};      // two ResBlockConv (reference models/unet.py:1103-1116)
+  else t.middle = {{1, ch, ch}, {e.unetmodel ? L_ATTN : L_SWIN, ch, e.unetmodel ? e.attn_heads(ch, false) : ds}, {1, ch, ch}};
   for (int level = c.n_levels - 1; level >= 0; --level) {
     for (int i = 0; i <= c.num_res_blocks[level]; ++i) {
       const int ich = chans.back(); chans.pop_back();
@@ -202,6 +206,13 @@ void add_layers(rs_engine& e, const std::string& prefix, const std::vector<Layer
     const std::string p = prefix + "." + std::to_string(j);
     if (L.kind == L_CONV) {
       add_conv(e, p, L.a, L.b, 3);
+    } else if ((L.kind == L_RES || L.kind == L_RES_DOWN || L.kind == L_RES_UP) && e.conv_blocks) {
+      // ResBlockConv (reference models/unet.py:914-982): in_layers = [SiLU, conv], out_layers = [SiLU, conv]
+      const int cout = L.kind == L_RES ? L.b : L.a;
+      add_conv(e, p + ".in_layers.1", L.a, cout, 3);
+      add_linear(e, p + ".emb_layers.1", e.time_dim(), (e.opt.use_scale_shift_norm ? 2 : 1) * cout);
+      add_conv(e, p + ".out_layers.1", cout, cout, 3);
+      if (L.a != cout) add_conv(e, p + ".skip_connection", L.a, cout, 1);
     } else if (L.kind == L_RES || L.kind == L_RES_DOWN || L.kind == L_RES_UP) {
       const int cout = L.kind == L_RES ? L.b : L.a;
       add_gn(e, p + ".in_layers.0", L.a);
@@ -270,8 +281,12 @@ int build_inventory(rs_engine& e) {
   for (size_t i = 0; i < t.input_blocks.size(); ++i) add_layers(e, "input_blocks." + std::to_string(i), t.input_blocks[i]);
   add_layers(e, "middle_block", t.middle);
   for (size_t i = 0; i < t.output_blocks.size(); ++i) add_layers(e, "output_blocks." + std::to_string(i), t.output_blocks[i]);
-  add_gn(e, "out.0", c.channel_mult[0] * c.model_channels);
-  add_conv(e, "out.2", c.channel_mult[0] * c.model_channels, c.out_channels, 3);
+  if (e.conv_blocks) {
+    add_conv(e, "out.1", c.channel_mult[0] * c.model_channels, c.out_channels, 3);
+  } else {
+    add_gn(e, "out.0", c.channel_mult[0] * c.model_channels);
+    add_conv(e, "out.2", c.channel_mult[0] * c.model_channels, c.out_channels, 3);
+  }
 
   // arena layout.  emb_layers weights / biases first, contiguous, in ResBlock order, so that all of
   // them form ONE [film_rows, time_dim] matrix for a single small-linear launch.
@@ -356,6 +371,7 @@ struct ConvOp : Producer {
   ConvDesc d;
   std::string w_name, b_name;   // (b_name empty: no bias)
   int bias_film_off = -1;       // the bias is a FiLM-table row (ResBlock without scale-shift norm): its offset in a row
+  int film_off = -1;            // FiLM after the activation (ResBlockConv with scale-shift norm): its [2 Cout] slice of a row
   bool to_f32 = false;          // writes the fp32 NCHW model output
   int split_tens = -1;          // workspace tensor holding split-K partial sums (or -1)
   // VQ-GAN attention GEMMs (vq.inc): "weights" that are an activation tensor [Cout rows][K] of the plan, and / or input
@@ -367,7 +383,8 @@ struct GnOp { GnDesc d; GnLink stats; std::string name; };   // d.in / fused / s
 struct WinAttnOp {   // (simt: the SIMT cross-check kernel instead of a window_attn_kernel instance)
   View qkv, out; int window = 8, shift = 0; bool simt = false; std::string bias_name; const float* bias = nullptr;
 };
-struct ResampleOp { View in, out; bool pool = false; };     // 2x nearest upsample, or (pool) 2x2 average pool
+struct ResampleOp { View in, out; bool pool = false; View silu; bool has_silu = false; };   // 2x nearest upsample, or (pool) 2x2
+                                                                                            // average pool (+ SiLU twin of out)
 struct MlpOp : Producer { MlpDesc d; std::string name; };
 struct SwinOp : Producer { SwinAttnDesc d; std::string blk; GnLink norm1; };
 struct SoftmaxOp { View view; float scale = 1.f; };         // in place on view [rows = N*H*W][cols = C]
@@ -511,12 +528,27 @@ struct Builder {
 
   int opi() const { return (int)(P.fe_ops.size() + P.ops.size()); }
 
+  // SiLU twins (UNetModelConv): a tensor whose every value a ResBlockConv or the head also reads through SiLU has a twin
+  // tensor of the same layout holding SiLU of it.  Whoever writes a view of such a tensor (conv epilogue, resample) writes
+  // the same view of the twin; with_twin() is the one place that decides which tensors have one.
+  std::map<int, int> twin_of;                      // tensor id -> its twin's
+  View with_twin(const View& v) {
+    if (!twin_of.count(v.tens)) twin_of[v.tens] = P.new_tensor(P.tensors[v.tens].bytes);
+    return v;
+  }
+  bool has_twin(const View& v) const { return twin_of.count(v.tens) != 0; }
+  View twin(const View& v) const { View t = v; t.tens = twin_of.at(v.tens); return t; }
+
+  // partial: `out` is a partial value that a later op accumulates into (no twin written)
   void conv(const View& in, const std::string& name, int ksize, int stride, int cout, const View* out,
-            const View* res, int act, bool out_f32 = false, int pad_lo = 1, int bias_film_off = -1) {
+            const View* res, int act, bool out_f32 = false, int pad_lo = 1, int bias_film_off = -1, int film_off = -1,
+            bool partial = false) {
     ConvOp op;
     op.d.in = in; op.d.ksize = ksize; op.d.stride = stride; op.d.Cout = cout; op.d.act = act;
     op.d.pad_lo = pad_lo;
     op.bias_film_off = bias_film_off; op.d.bias_per_image = bias_film_off >= 0;
+    op.film_off = film_off; op.d.film = film_off >= 0;
+    if (out && !out_f32 && !partial && has_twin(*out)) { op.d.silu_out = twin(*out); op.d.has_silu = true; }
     if (out) { op.d.out = *out; op.d.has_out = true; } else op.d.has_out = false;
     if (res) { op.d.res = *res; op.d.has_res = true; }
     op.w_name = name + ".weight"; op.b_name = name + ".bias";
@@ -533,6 +565,7 @@ struct Builder {
     }
     const int i = opi();
     P.touch(in, i); if (out) P.touch(*out, i); if (res) P.touch(*res, i);
+    if (op.d.has_silu) P.touch(op.d.silu_out, i);
     cur->push_back(std::move(op));
     if (out && !out_f32 && out->tens >= 0) note_writer(*out, cout);   // the latest writer of this (channel, image) range
   }
@@ -586,7 +619,9 @@ struct Builder {
   void upsample(const View& in, const View& out, bool pool = false) {
     const int i = opi();
     P.touch(in, i); P.touch(out, i);
-    cur->push_back(ResampleOp{in, out, pool});
+    ResampleOp r{in, out, pool};
+    if (has_twin(out)) { r.silu = twin(out); r.has_silu = true; P.touch(r.silu, i); }
+    cur->push_back(r);
     forget_writers(out, out.C);
   }
 
@@ -615,6 +650,32 @@ struct Builder {
       conv(t2, p + ".out_layers.3", 3, 1, cout, &out, &out, ACT_NONE);     // in-place accumulate
     } else {
       conv(t2, p + ".out_layers.3", 3, 1, cout, &out, &x, ACT_NONE);
+    }
+  }
+  // ResBlockConv (reference models/unet.py:984-1004): y = skip(x) + out_conv(SiLU(in_conv(SiLU(x)) + emb_out)), or with
+  // scale-shift norm y = skip(x) + out_conv(SiLU(in_conv(SiLU(x))) * (1 + scale) + shift) (out_layers[0] is the SiLU, and
+  // no SiLU follows the FiLM).  SiLU(x) is x's twin; in_conv's epilogue adds emb_out as its per-image bias and applies the
+  // SiLU (and the FiLM).  updown: h_upd / x_upd resample SiLU(x) and x (:985-990).  out_conv's epilogue writes y and its twin.
+  void res_block_conv(const View& x_in, const std::string& p, int cout, const View& out, int updown = 0) {
+    const bool ss = E.opt.use_scale_shift_norm != 0;
+    const int row = E.film_row_of.at(p);
+    View s = twin(x_in);
+    View x = x_in;
+    if (updown) {
+      const int Ho = updown > 0 ? 2 * x_in.H : x_in.H / 2, Wo = updown > 0 ? 2 * x_in.W : x_in.W / 2;
+      View sr = P.make_view(x_in.N, Ho, Wo, x_in.C);
+      upsample(s, sr, updown < 0);
+      s = sr;
+      x = P.make_view(x_in.N, Ho, Wo, x_in.C);
+      upsample(x_in, x, updown < 0);
+    }
+    View h = P.make_view(x.N, x.H, x.W, cout);
+    conv(s, p + ".in_layers.1", 3, 1, cout, &h, nullptr, ACT_SILU, false, 1, ss ? -1 : row, ss ? row : -1);
+    if (x.C != cout) {
+      conv(x, p + ".skip_connection", 1, 1, cout, &out, nullptr, ACT_NONE, false, 1, -1, -1, /*partial=*/true);
+      conv(h, p + ".out_layers.1", 3, 1, cout, &out, &out, ACT_NONE);     // in-place accumulate
+    } else {
+      conv(h, p + ".out_layers.1", 3, 1, cout, &out, &x, ACT_NONE);
     }
   }
   // BasicLayer (reference models/swin_transformer.py:427-442) with SwinTransformerBlock.forward (:238-281)
@@ -695,10 +756,19 @@ struct Builder {
       const Layer& L = layers[j];
       const std::string p = prefix + "." + std::to_string(j);
       const bool last = (j + 1 == layers.size());
+      // an output inside the block: with a twin when a ResBlockConv reads it next (block outputs are the caller's dest)
+      auto inner = [&](int c) {
+        const View v = P.make_view(h.N, h.H, h.W, c);
+        const int nk = last ? -1 : layers[j + 1].kind;
+        return E.conv_blocks && (nk == L_RES || nk == L_RES_DOWN || nk == L_RES_UP) ? with_twin(v) : v;
+      };
       View out;
       if (L.kind == L_CONV) {
-        out = last ? dest : P.make_view(h.N, h.H, h.W, L.b);
+        out = last ? dest : inner(L.b);
         conv(h, p, 3, 1, L.b, &out, nullptr, ACT_NONE);
+      } else if (L.kind == L_RES && E.conv_blocks) {
+        out = last ? dest : inner(L.b);
+        res_block_conv(h, p, L.b, out);
       } else if (L.kind == L_RES) {
         out = last ? dest : P.make_view(h.N, h.H, h.W, L.b);
         res_block(h, p, L.b, out);
@@ -710,7 +780,8 @@ struct Builder {
         unet_attn_block(h, p, L.b, out);
       } else if (L.kind == L_RES_DOWN || L.kind == L_RES_UP) {     // always the last layer of its block
         out = dest;
-        res_block(h, p, L.a, out, L.kind == L_RES_DOWN ? -1 : 1);
+        if (E.conv_blocks) res_block_conv(h, p, L.a, out, L.kind == L_RES_DOWN ? -1 : 1);
+        else res_block(h, p, L.a, out, L.kind == L_RES_DOWN ? -1 : 1);
       } else if (L.kind == L_DOWN) {
         out = dest;
         if (E.opt.conv_resample) conv(h, p + ".op", 3, 2, L.a, &out, nullptr, ACT_NONE);
@@ -837,6 +908,7 @@ int build_plan(rs_plan& P) {
     const int k = n_in - 1 - j;
     const int ctot = topo.output_blocks[j][0].a;       // ch + ich
     cat[j] = P.make_view(B, in_h[k], in_w[k], ctot);
+    if (E.conv_blocks) b.with_twin(cat[j]);            // read by a ResBlockConv: every slice writer also writes SiLU of it
   }
   // encoder
   View h = P.xin;
@@ -866,16 +938,21 @@ int build_plan(rs_plan& P) {
     } else {
       const Layer& L0 = topo.output_blocks[j][0];
       dest = P.make_view(B, cat[j].H, cat[j].W, L0.b);
+      if (E.conv_blocks) b.with_twin(dest);            // the head reads SiLU(h)
     }
     int rc = b.run_block(cat[j], "output_blocks." + std::to_string(j), topo.output_blocks[j], dest, &h);
     if (rc) return rc;
     P.block_out["output_blocks." + std::to_string(j)] = h;
     final_h = h;
   }
-  // head (reference models/unet.py:859-863,894)
-  View t = P.make_view(B, final_h.H, final_h.W, final_h.C);
-  b.gn(final_h, "out.0", t, 1, -1);
-  b.conv(t, "out.2", 3, 1, c.out_channels, nullptr, nullptr, ACT_NONE, /*out_f32=*/true);
+  // head (reference models/unet.py:859-863,894; UNetModelConv :1148-1151: conv3x3(SiLU(h)))
+  if (E.conv_blocks) {
+    b.conv(b.twin(final_h), "out.1", 3, 1, c.out_channels, nullptr, nullptr, ACT_NONE, /*out_f32=*/true);
+  } else {
+    View t = P.make_view(B, final_h.H, final_h.W, final_h.C);
+    b.gn(final_h, "out.0", t, 1, -1);
+    b.conv(t, "out.2", 3, 1, c.out_channels, nullptr, nullptr, ACT_NONE, /*out_f32=*/true);
+  }
 
   return finish_layout(P, b, (size_t)B * std::max(c.in_channels, c.out_channels) * P.H * P.W * sizeof(float), true);
 }
@@ -922,6 +999,7 @@ int bind_ops(rs_plan& P, std::vector<Op>& ops) {
         ConvDesc& d = c.d;
         bind_sinks(P, c, d.sink);
         resolve(P, d.in); if (d.has_out) resolve(P, d.out); if (d.has_res) resolve(P, d.res);
+        if (d.has_silu) resolve(P, d.silu_out);
         if (!c.in_param.empty()) {          // the "pixels" are the rows of a weight matrix of the arena
           const Param* wp = E.find(c.in_param);
           RS_CHECK(wp != nullptr && wp->ipad == d.in.ld, "missing / mismatching parameter " + c.in_param);
@@ -966,7 +1044,12 @@ int bind_ops(rs_plan& P, std::vector<Op>& ops) {
         RS_CHECK(a.bias != nullptr, "missing " + a.bias_name);
         break;
       }
-      case OP_UPSAMPLE: resolve(P, payload<ResampleOp>(op).in); resolve(P, payload<ResampleOp>(op).out); break;
+      case OP_UPSAMPLE: {
+        ResampleOp& r = payload<ResampleOp>(op);
+        resolve(P, r.in); resolve(P, r.out);
+        if (r.has_silu) resolve(P, r.silu);
+        break;
+      }
       case OP_MLP: {
         MlpOp& mo = payload<MlpOp>(op);
         MlpDesc& m = mo.d;
@@ -1036,11 +1119,18 @@ int run_op_range(rs_plan& P, const Op* first, const Op* last, const float* film_
     switch (kind_of(op)) {
       case OP_CONV: {
         const ConvOp& c = payload<ConvOp>(op);
-        if (c.bias_film_off < 0) { rc = conv_launch(c.d, st); break; }
-        ConvDesc d = c.d;               // bias = this launch's FiLM row(s), resolved like a GroupNorm's film
-        const float* row = film_base + c.bias_film_off;
-        if (d.prm.bias) { d.prm.bias = row; d.prm.bias_sN = (int)film_sN; }
-        if (d.prm.splitk > 1) { d.red.bias = row; d.red.bias_sN = (int)film_sN; }
+        if (c.bias_film_off < 0 && c.film_off < 0) { rc = conv_launch(c.d, st); break; }
+        ConvDesc d = c.d;               // bias / FiLM = this launch's FiLM-table row(s), resolved like a GroupNorm's film
+        if (c.bias_film_off >= 0) {
+          const float* row = film_base + c.bias_film_off;
+          if (d.prm.bias) { d.prm.bias = row; d.prm.bias_sN = (int)film_sN; }
+          if (d.prm.splitk > 1) { d.red.bias = row; d.red.bias_sN = (int)film_sN; }
+        }
+        if (c.film_off >= 0) {
+          const float* row = film_base + c.film_off;
+          if (d.prm.splitk > 1) { d.red.film = row; d.red.film_sN = (int)film_sN; }
+          else { d.prm.film = row; d.prm.film_sN = (int)film_sN; }
+        }
         rc = conv_launch(d, st);
         break;
       }
@@ -1068,6 +1158,7 @@ int run_op_range(rs_plan& P, const Op* first, const Op* last, const float* film_
       case OP_UPSAMPLE: {
         const ResampleOp& r = payload<ResampleOp>(op);
         UpsampleParams u{r.in.ptr, r.in.sN(), r.in.ld, r.out.ptr, r.out.sN(), r.out.ld, r.in.N, r.in.H, r.in.W, r.in.C};
+        if (r.has_silu) { u.s = r.silu.ptr; u.s_sN = r.silu.sN(); u.s_ld = r.silu.ld; }
         const long long total = (long long)u.N * (r.pool ? u.H * u.W / 4 : 4 * u.H * u.W) * (u.C / 8);
         (void)launch_k(r.pool ? avgpool2x2_kernel : upsample2x_kernel,
                        dim3((unsigned)std::min<long long>((total + 255) / 256, num_sms() * 16)), dim3(256), (size_t)(0), st, u);
@@ -1235,6 +1326,45 @@ int rs_unetmodel_create(const rs_unetmodel_config* cfg, const rs_unet_options* o
   *out = e.release();
   return 0;
 }
+int rs_unetconv_create(const rs_unetconv_config* cfg, const rs_unet_options* opts, rs_engine** out) {
+  RS_CHECK(cfg && opts && out, "null argument");
+  RS_CHECK(cfg->n_levels >= 1 && cfg->n_levels <= RS_MAX_LEVELS, "n_levels must be 1 .. " + std::to_string(RS_MAX_LEVELS));
+  RS_CHECK(opts->patch_norm == 0, "UNetModelConv has no patch norm: rs_unet_options.patch_norm must be 0");
+  for (int v : {opts->use_scale_shift_norm, opts->resblock_updown, opts->conv_resample})
+    RS_CHECK(v == 0 || v == 1, "rs_unet_options fields are 0 or 1");
+  RS_CHECK(cfg->dims == 2, "dims=" + std::to_string(cfg->dims) + ": only 2-D UNets are covered (set dims=2)");
+  RS_CHECK(cfg->cond_lq == 1, "cond_lq must be 1: the ResShift sampler always passes lq, and the reference asserts cond_lq then");
+  RS_CHECK(cfg->out_channels > 0 && (cfg->in_channels - cfg->out_channels == 3 || cfg->in_channels - cfg->out_channels == 12),
+           "in_channels must be out_channels + 3 (lq at the latent size) or out_channels + 12 (lq at twice the latent size, "
+           "pixel_unshuffle): x has out_channels channels and lq is a 3-channel image");
+  RS_CHECK(cfg->model_channels > 0, "model_channels must be positive");
+  for (int l = 0; l < cfg->n_levels; ++l) {
+    RS_CHECK(cfg->channel_mult[l] > 0 && cfg->num_res_blocks[l] >= 0, "channel_mult / num_res_blocks");
+    RS_CHECK(cfg->model_channels * cfg->channel_mult[l] % 8 == 0,
+             "level " + std::to_string(l) + " has " + std::to_string(cfg->model_channels * cfg->channel_mult[l]) +
+             " channels: the conv kernels read and write 16-byte channel rows, so model_channels * channel_mult must be a "
+             "multiple of 8");
+  }
+  auto e = std::make_unique<rs_engine>();
+  e->unetmodel = true;
+  e->conv_blocks = true;
+  e->opt = *opts;
+  rs_unetmodel_config& u = e->um;               // the UNetModel-style input handling (x + lq, no feature extractor)
+  u.in_channels = cfg->in_channels; u.out_channels = cfg->out_channels; u.model_channels = cfg->model_channels;
+  u.n_levels = cfg->n_levels; u.n_attn = 0; u.num_heads = 1; u.num_head_channels = -1;
+  rs_unet_config& c = e->cfg;
+  std::memset(&c, 0, sizeof(c));
+  c.image_size = 64; c.lq_size = 64;            // (no image_size: unused without attention levels and feature extractor)
+  c.in_channels = cfg->out_channels; c.model_channels = cfg->model_channels; c.out_channels = cfg->out_channels;
+  c.n_levels = cfg->n_levels; c.n_attn = 0;
+  for (int l = 0; l < RS_MAX_LEVELS; ++l) {
+    c.channel_mult[l] = u.channel_mult[l] = cfg->channel_mult[l];
+    c.num_res_blocks[l] = u.num_res_blocks[l] = cfg->num_res_blocks[l];
+  }
+  int rc = build_inventory(*e); if (rc) return rc;
+  *out = e.release();
+  return 0;
+}
 void rs_unet_destroy(rs_engine* e) { delete e; }
 int rs_unet_param_count(const rs_engine* e) { return e ? (int)e->params.size() : 0; }
 int rs_unet_param_info(const rs_engine* e, int index, char* name, size_t name_cap, int32_t shape[4], int32_t* ndim,
@@ -1290,7 +1420,8 @@ int rs_unet_load_param(rs_engine* e, const char* name, const float* src, void* s
     // the FiLM table's bias of a ResBlock is emb_layers.1.bias + in_layers.2.bias (build_inventory); whichever of the two
     // is loaded last leaves the sum right
     const std::string nm(name);
-    for (const char* suffix : {".emb_layers.1.bias", ".in_layers.2.bias"}) {
+    const char* in_bias = e->conv_blocks ? ".in_layers.1.bias" : ".in_layers.2.bias";    // (ResBlockConv: in_layers.1)
+    for (const char* suffix : {".emb_layers.1.bias", in_bias}) {
       const size_t ls = std::strlen(suffix);
       if (nm.size() <= ls || nm.compare(nm.size() - ls, ls, suffix) != 0) continue;
       const std::string blk = nm.substr(0, nm.size() - ls);
@@ -1298,7 +1429,7 @@ int rs_unet_load_param(rs_engine* e, const char* name, const float* src, void* s
       if (it == e->film_row_of.end()) continue;
       const int n = p->shape[0];
       (void)launch_k(add_f32_kernel, dim3((unsigned)((n + 255) / 256)), dim3(256), (size_t)(0), st,
-                     (const float*)e->at<float>(blk + ".emb_layers.1.bias"), (const float*)e->at<float>(blk + ".in_layers.2.bias"),
+                     (const float*)e->at<float>(blk + ".emb_layers.1.bias"), (const float*)e->at<float>(blk + in_bias),
                      reinterpret_cast<float*>(e->arena + e->film_b_off) + it->second, n);
     }
   }
@@ -1436,6 +1567,10 @@ static void collect_profile(const rs_plan& P, const Prof& prof, double* ms, char
                  cd.ksize, cd.ksize, cd.stride, c.Hout, c.Wout, cd.in.C, c.Cout, cd.grid, c.BN, c.stages,
                  payload<ConvOp>(op).w_name.c_str(), c.cg, c.msub, c.splitk, c.bw, c.bh, c.bn, c.Nimg, c.persist, cd.pad_lo,
                  cd.act, (int)cd.has_res, (int)(cd.out_f32 != nullptr));
+        if (cd.has_silu || cd.film) {       // (UNetModelConv only: the other plans' rows keep their form)
+          const size_t len = std::strlen(d);
+          snprintf(d + len, desc_stride - len, " silu=%d film=%d", (int)cd.has_silu, (int)cd.film);
+        }
         break;
       }
       case OP_GN: {   // everything rs_op_groupnorm_ex needs to replay it, and the launch geometry it should report
@@ -1460,7 +1595,11 @@ static void collect_profile(const rs_plan& P, const Prof& prof, double* ms, char
         else snprintf(d, desc_stride, "vq_attn T=%d C=%d N=%d rows=%d:%d", a.prm.T, a.q.C, a.q.N, a.row_begin, a.row_end);
         break;
       }
-      case OP_UPSAMPLE: { const ResampleOp& r = payload<ResampleOp>(op); snprintf(d, desc_stride, "%s %dx%d C=%d", r.pool ? "avgpool" : "upsample", r.in.H, r.in.W, r.in.C); break; }
+      case OP_UPSAMPLE: {
+        const ResampleOp& r = payload<ResampleOp>(op);
+        snprintf(d, desc_stride, "%s %dx%d C=%d%s", r.pool ? "avgpool" : "upsample", r.in.H, r.in.W, r.in.C, r.has_silu ? " silu=1" : "");
+        break;
+      }
       case OP_UNET_ATTN: {
         const UnetAttnDesc& a = payload<UnetAttnDesc>(op);
         snprintf(d, desc_stride, "unet_attn T=%d heads=%d D=%d N=%d order=%s", a.prm.T, a.heads, a.out.C / a.heads, a.qkv.N,

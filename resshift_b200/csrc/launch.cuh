@@ -195,6 +195,8 @@ struct ConvDesc {
   View out;               // NHWC fp16 output view (ptr may be null when out_f32 is used)
   bool has_out = true;
   View res; bool has_res = false;
+  View silu_out; bool has_silu = false;   // second output: SiLU of the stored fp16 output (same grid and channels)
+  bool film = false;      // FiLM rows after the activation, set per launch (prm.film / red.film)
   float* out_f32 = nullptr;
   int act = ACT_NONE;
   int bn_override = 0;
@@ -378,14 +380,18 @@ inline int conv_finalize(ConvDesc& d, const Overrides& o) {
   d.simt_kernel = simt;
   const bool can_split = d.allow_split && d.partial != nullptr && contiguous_tiles && p.bn <= 2 && d.has_out && !d.out_f32 && !simt;
   const int want_persist = o.conv_persist;                           // 0 / 1 disables / forces the persistent kernel
-  const bool persist_ok = d.has_out && !d.out_f32 && want_persist != 0 && !o.conv_direct && !simt &&
+  // per-image bias rows of a box of more than 8 images (maps of fewer than 16 pixels per 128-pixel box): the direct
+  // epilogue, which reads them per element (the staged one holds one row per 16 accumulator rows)
+  const bool bias_direct = d.bias_per_image && p.bn > 8;
+  RS_CHECK(!bias_direct || (!d.has_silu && !d.film), "per-image bias on boxes of more than 8 images cannot take silu_out or FiLM");
+  const bool persist_ok = d.has_out && !d.out_f32 && want_persist != 0 && !o.conv_direct && !simt && !bias_direct &&
                           (d.msub_request ? d.msub_request : o.conv_msub) != 2;
   const TileConfig tc = pick_tile_config(o, m_tiles, cout16, num_kb, d.bn_override ? d.bn_override : o.conv_bn, can_split,
-                                         persist_ok && want_persist != 1, !d.bias_per_image, d.msub_request);
+                                         persist_ok && want_persist != 1, !d.bias_per_image && !d.film && !d.has_silu, d.msub_request);
   const int BN = tc.BN, msub = tc.msub, stages = tc.stages, cg = tc.cg;
   p.cg = cg;
   p.splitk = tc.splitk; p.partial = d.partial;
-  RS_CHECK(conv_kernel_for(BN, msub) != nullptr, "no valid tile configuration");
+  RS_CHECK(conv_kernel_for(BN, msub, d.has_silu || d.film) != nullptr, "no valid tile configuration");
   p.BN = BN; p.n_tiles = (cout16 + BN - 1) / BN;
   p.msub = msub;
   const int stage_bytes = msub * kConvBM * kConvBK * 2 + BN * kConvBK * 2;
@@ -393,8 +399,11 @@ inline int conv_finalize(ConvDesc& d, const Overrides& o) {
   p.epi_off = 0;
   p.bar_off = stages * stage_bytes;
   // bias tile: [BN] floats, or [bn][BN] when every image has its own bias row
-  RS_CHECK(!d.bias_per_image || (p.bn <= 8 && msub == 1), "per-image bias needs one sub-tile of at most 8 images");
-  const size_t bias_tile = d.bias_per_image ? std::max<size_t>(1024, (size_t)p.bn * BN * sizeof(float)) : 1024;
+  RS_CHECK(!d.bias_per_image || msub == 1, "per-image bias needs one sub-tile per CTA");
+  RS_CHECK(!d.film || (msub == 1 && d.Cout % 8 == 0), "FiLM rows need one sub-tile per CTA and Cout % 8 == 0");
+  RS_CHECK(!d.film || (!d.has_res && d.has_out && !d.out_f32 && !d.sink[0].part && !d.sink[1].part),
+           "FiLM rows need an fp16 output and no residual or statistics sinks");
+  const size_t bias_tile = d.bias_per_image && !bias_direct ? std::max<size_t>(1024, (size_t)p.bn * BN * sizeof(float)) : 1024;
   d.smem = (size_t)stages * stage_bytes + 1024 + 256 + bias_tile;   // ring + alignment slack + barriers + bias tile
   RS_CHECK(d.smem <= 227 * 1024, "shared memory budget exceeded");
   d.grid = (cg == 2 ? ((m_tiles + 1) / 2) * p.n_tiles * 2 : (m_tiles / msub) * p.n_tiles) * p.splitk;
@@ -429,10 +438,17 @@ inline int conv_finalize(ConvDesc& d, const Overrides& o) {
     p.out = d.out.ptr; p.out_sN = d.out.sN(); p.out_sH = d.out.sH(); p.out_sW = d.out.sW();
     RS_CHECK(d.out.ld % 8 == 0 && (reinterpret_cast<uintptr_t>(d.out.ptr) & 15) == 0, "output alignment");
   }
+  if (d.has_silu) {
+    RS_CHECK(d.has_out && !d.out_f32 && d.Cout % 8 == 0, "the SiLU output needs an fp16 output and Cout % 8 == 0");
+    RS_CHECK(d.silu_out.H == Hout && d.silu_out.W == Wout && d.silu_out.N == N, "SiLU output geometry");
+    RS_CHECK(d.silu_out.ld % 8 == 0 && (reinterpret_cast<uintptr_t>(d.silu_out.ptr) & 15) == 0, "SiLU output alignment");
+    p.silu_out = d.silu_out.ptr; p.silu_sN = d.silu_out.sN(); p.silu_sH = d.silu_out.sH(); p.silu_sW = d.silu_out.sW();
+  }
   p.out_f32_nchw = d.out_f32;
   p.dbg = d.dbg;
   // staged epilogue (TMA store / TMA residual load) for fp16 NHWC outputs
-  p.tma_out = (d.has_out && !d.out_f32 && p.splitk == 1 && !o.conv_direct && !simt) ? 1 : 0;
+  // (the direct epilogue has no SiLU output or FiLM: such convs keep the staged epilogue under RS_CONV_EPI=direct)
+  p.tma_out = (d.has_out && !d.out_f32 && p.splitk == 1 && (!o.conv_direct || d.has_silu || d.film) && !simt && !bias_direct) ? 1 : 0;
   p.tma_res = (p.tma_out && d.has_res) ? 1 : 0;
   p.epi_bc = (BN % 64 == 0) ? 64 : (BN % 32 == 0 ? 32 : 16);
   if (p.tma_out) {
@@ -440,6 +456,11 @@ inline int conv_finalize(ConvDesc& d, const Overrides& o) {
     if (rc) return rc;
     if (p.tma_res) {
       rc = encode_act_map(&p.tmRes, d.res.ptr, d.Cout, Wout, Hout, N, d.res.sW(), d.res.sH(), d.res.sN(), p.bw, p.bh, p.bn, p.epi_bc);
+      if (rc) return rc;
+    }
+    if (d.has_silu) {
+      rc = encode_act_map(&p.tmSilu, d.silu_out.ptr, d.Cout, Wout, Hout, N, d.silu_out.sW(), d.silu_out.sH(), d.silu_out.sN(),
+                          p.bw, p.bh, p.bn, p.epi_bc);
       if (rc) return rc;
     }
     // the staging area (column blocks + per-warp GN partials) must fit in the operand ring
@@ -483,8 +504,10 @@ inline int conv_finalize(ConvDesc& d, const Overrides& o) {
     r.out = d.out.ptr; r.out_sN = d.out.sN(); r.out_ld = d.out.ld;
     r.rows_per_slot = p.bw * p.bh; r.slots = p.tiles_w * p.tiles_h;
     compact_sinks(d.sink, p.gn_slots, r.sink);
+    if (d.has_silu) { r.silu_out = d.silu_out.ptr; r.silu_sN = d.silu_out.sN(); r.silu_ld = d.silu_out.ld; }
     RS_CHECK(d.Cout % 8 == 0 && d.Cout <= 2048, "split-K reduce needs Cout % 8 == 0");
     p.bias = nullptr; p.residual = nullptr; p.act = ACT_NONE; p.sink[0] = GnSink{}; p.sink[1] = GnSink{};
+    p.silu_out = nullptr;
     d.red_grid_x = r.slots;
     // column blocks so that the reduce kernel fills the machine even with one slot per image
     int cpc = d.Cout;
@@ -531,8 +554,9 @@ inline int conv_init() {
   if (!attr_set[dev].load(std::memory_order_relaxed)) {
     for (int bn : kConvBNs)
       for (int ms = 1; ms <= 2; ++ms)
-        if (ConvKernelFn k = conv_kernel_for(bn, ms))
-          RS_CUDA_OK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+        for (bool ex : {false, true})
+          if (ConvKernelFn k = conv_kernel_for(bn, ms, ex))
+            RS_CUDA_OK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     RS_CUDA_OK(cudaFuncSetAttribute(window_attn_kernel<8, 32>, cudaFuncAttributeMaxDynamicSharedMemorySize, kAttnMaxSmem));
     RS_CUDA_OK(cudaFuncSetAttribute(window_attn_kernel<8, 64>, cudaFuncAttributeMaxDynamicSharedMemorySize, kAttnMaxSmem));
     RS_CUDA_OK(cudaFuncSetAttribute(window_attn_kernel<16, 32>, cudaFuncAttributeMaxDynamicSharedMemorySize, kAttnMaxSmem));
@@ -560,7 +584,7 @@ inline int conv_launch(const ConvDesc& d, cudaStream_t st) {
     const int warps = 8;
     (void)launch_k(conv_simt_kernel, dim3((unsigned)((npix + warps - 1) / warps)), dim3(warps * 32), (size_t)(0), st, d.prm, d.simt);
   } else {
-    const ConvKernelFn k = conv_kernel_for(d.prm.BN, d.prm.msub);
+    const ConvKernelFn k = conv_kernel_for(d.prm.BN, d.prm.msub, d.has_silu || d.film);
     RS_CHECK(k != nullptr, "no conv kernel for this channel tile");
     (void)launch_kc(k, dim3(d.grid), dim3(kConvThreads), (size_t)(d.smem), st, d.prm.cg, d.prm);
     if (d.prm.splitk > 1)

@@ -23,7 +23,7 @@ import torch
 import torch.nn.functional as F
 
 from .. import _lib
-from .unet import UNetModel, UNetModelSwin
+from .unet import UNetModel, UNetModelConv, UNetModelSwin
 
 
 class ModelMeanType(enum.Enum):
@@ -205,7 +205,7 @@ class ResShiftDiffusion:
 
     # ------------------------------------------------------------------ the loop
     def _native_ok(self, model, clip_denoised, denoised_fn, model_kwargs) -> bool:
-        return (isinstance(model, (UNetModelSwin, UNetModel)) and self.model_mean_type == ModelMeanType.START_X
+        return (isinstance(model, (UNetModelSwin, UNetModel, UNetModelConv)) and self.model_mean_type == ModelMeanType.START_X
                 and not clip_denoised and denoised_fn is None and self.normalize_input and self.latent_flag
                 and model_kwargs is not None and "lq" in model_kwargs
                 and 2 <= self.num_timesteps <= 64)       # rs_sampler_create: 2 <= T <= FiLM-table rows of a plan
@@ -217,15 +217,16 @@ class ResShiftDiffusion:
         receives raw pointers, so every shape is checked here."""
         cfg = model.cfg
         B, Cc, H, W = z_y.shape
-        latent_ch = cfg.out_channels if isinstance(model, UNetModel) else cfg.in_channels
+        plain_lq = isinstance(model, (UNetModel, UNetModelConv))     # x + lq concatenated, no feature extractor or mask
+        latent_ch = cfg.out_channels if plain_lq else cfg.in_channels
         if Cc != latent_ch:
             raise ValueError(f"latent has {Cc} channels, the model expects {latent_ch}")
         exp_lq = model.lq_shape(B, H, W)
         if tuple(lq.shape) != exp_lq:
             raise ValueError(f"lq must have shape {exp_lq}, got {tuple(lq.shape)}")
-        if isinstance(model, UNetModel):
+        if plain_lq:
             if mask is not None:
-                raise ValueError("UNetModel takes no mask (its forward has no mask parameter)")
+                raise ValueError(f"{type(model).__name__} takes no mask (its forward has no mask parameter)")
         elif cfg.cond_mask:
             if mask is None:
                 raise ValueError("this model is mask-conditioned (cond_mask=True): pass model_kwargs['mask']")

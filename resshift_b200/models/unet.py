@@ -1,5 +1,6 @@
-"""``UNetModelSwin`` and ``UNetModel`` — same constructors, ``state_dict`` and call surface as the reference's
-``models.unet.UNetModelSwin`` (reference models/unet.py:603-912) and ``models.unet.UNetModel`` (:346-601), with the
+"""``UNetModelSwin``, ``UNetModel`` and ``UNetModelConv`` — same constructors, ``state_dict`` and call surface as the
+reference's ``models.unet.UNetModelSwin`` (reference models/unet.py:603-912), ``models.unet.UNetModel`` (:346-601) and
+``models.unet.UNetModelConv`` (:1006-1181), with the
 forward pass executed by the sm_90a kernels of ``librs_b200.so`` through the C ABI (include/resshift_b200.h).
 
 PyTorch owns every allocation (parameters, packed-weight arena, workspace, outputs); the library only
@@ -15,8 +16,8 @@ import torch
 import torch.nn as nn
 
 from .. import _lib
-from ..arch import latent_multiple, unet_param_spec, unetmodel_param_spec
-from ..config import UNetConfig, UNetModelConfig
+from ..arch import latent_multiple, unet_param_spec, unetconv_param_spec, unetmodel_param_spec
+from ..config import UNetConfig, UNetModelConfig, UNetModelConvConfig
 from ..weights import random_state_dict
 
 
@@ -250,6 +251,48 @@ class UNetModel(_NativeDenoiser):
             raise ValueError("y: class-conditional UNetModel is not covered (num_classes must be None)")
         if lq is None:
             raise ValueError("UNetModel is LQ-conditioned (cond_lq=True): pass lq=")
+        if x.shape[1] != self.cfg.out_channels:
+            raise ValueError(f"x must have out_channels={self.cfg.out_channels} channels, got {x.shape[1]}")
+        return self._run_forward(x, timesteps, lq, None)
+
+
+class UNetModelConv(_NativeDenoiser):
+    """The reference's attention- and GroupNorm-free UNet of ResBlockConv blocks (reference models/unet.py:1006-1181).
+    Every tensor a ResBlockConv or the head reads is read raw and through SiLU: the conv or resample that produces it
+    writes both."""
+    _ZEROED = ("out_layers.1.weight", "out_layers.1.bias")       # zero_module (reference models/unet.py:968-972)
+
+    def __init__(self, in_channels, model_channels, out_channels, num_res_blocks, cond_lq=True, channel_mult=(1, 2, 4, 8),
+                 conv_resample=True, dims=2, use_scale_shift_norm=False, resblock_updown=False, use_fp16=False):
+        super().__init__()
+        self.cfg = UNetModelConvConfig(
+            in_channels=in_channels, model_channels=model_channels, out_channels=out_channels,
+            num_res_blocks=num_res_blocks, cond_lq=cond_lq, channel_mult=tuple(channel_mult), conv_resample=conv_resample,
+            dims=dims, use_scale_shift_norm=use_scale_shift_norm, resblock_updown=resblock_updown, use_fp16=use_fp16)
+        # attributes the reference exposes
+        self.in_channels, self.model_channels, self.out_channels = in_channels, model_channels, out_channels
+        self.num_res_blocks, self.channel_mult = list(self.cfg.num_res_blocks), channel_mult
+        self.conv_resample, self.cond_lq = conv_resample, cond_lq
+        self.dtype = torch.float32
+        self._register_params(unetconv_param_spec(self.cfg))
+
+    def _create_engine(self, handle):
+        cfgc, optc = _lib.make_unetconv_config(self.cfg), _lib.make_options(self.cfg)
+        _lib.check(_lib.lib.rs_unetconv_create(C.byref(cfgc), C.byref(optc), C.byref(handle)))
+
+    def _latent_rule(self) -> str:
+        return "2^(levels - 1): every level halves evenly"
+
+    def lq_shape(self, n, h, w):
+        f = self.cfg.lq_factor
+        return (n, 3, h * f, w * f)
+
+    @torch.no_grad()
+    def forward(self, x, timesteps, lq=None):
+        """x [N, out_channels, H, W]; timesteps [N]; lq [N, 3, H, W] or [N, 3, 2H, 2W] as in_channels says
+        -> [N, out_channels, H, W] fp32 (reference models/unet.py:1153-1181)."""
+        if lq is None:
+            raise ValueError("UNetModelConv is LQ-conditioned (cond_lq=True): pass lq=")
         if x.shape[1] != self.cfg.out_channels:
             raise ValueError(f"x must have out_channels={self.cfg.out_channels} channels, got {x.shape[1]}")
         return self._run_forward(x, timesteps, lq, None)

@@ -88,6 +88,7 @@ def load_yaml(path) -> Cfg:
 _NATIVE_TARGETS = {
     "models.unet.UNetModelSwin": "resshift_b200.models.unet.UNetModelSwin",
     "models.unet.UNetModel": "resshift_b200.models.unet.UNetModel",
+    "models.unet.UNetModelConv": "resshift_b200.models.unet.UNetModelConv",
     "models.script_util.create_gaussian_diffusion": "resshift_b200.models.script_util.create_gaussian_diffusion",
     "ldm.models.autoencoder.VQModelTorch": "resshift_b200.models.autoencoder.VQModelTorch",
     "ldm.models.autoencoder.AutoencoderKLTorch": "resshift_b200.models.autoencoder.AutoencoderKLTorch",
@@ -114,8 +115,9 @@ def instantiate_from_config(config):
 
 def make_configs(ucfg, dcfg, autoencoder: Optional[dict] = None, state_dict: Any = None) -> Cfg:
     """Programmatic equivalent of a configs/*.yaml for this package's targets."""
-    from .config import UNetModelConfig
-    target = "UNetModel" if isinstance(ucfg, UNetModelConfig) else "UNetModelSwin"
+    from .config import UNetModelConfig, UNetModelConvConfig
+    target = ("UNetModel" if isinstance(ucfg, UNetModelConfig) else
+              "UNetModelConv" if isinstance(ucfg, UNetModelConvConfig) else "UNetModelSwin")
     return Cfg.wrap({
         "model": {"target": f"resshift_b200.models.unet.{target}", "ckpt_path": state_dict, "params": ucfg.to_kwargs()},
         "diffusion": {"target": "resshift_b200.models.script_util.create_gaussian_diffusion", "params": dcfg.to_kwargs()},

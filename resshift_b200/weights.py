@@ -14,17 +14,25 @@ from typing import Dict
 
 import torch
 
-from .arch import unet_param_spec, unetmodel_param_spec, relative_position_index, shifted_window_mask, swin_geometry
-from .config import UNetConfig, UNetModelConfig
+from .arch import (unet_param_spec, unetconv_param_spec, unetmodel_param_spec, relative_position_index, shifted_window_mask,
+                   swin_geometry)
+from .config import UNetConfig, UNetModelConfig, UNetModelConvConfig
 
-_BRANCH_OUT = ("out_layers.3.weight", "attn.proj.weight", "mlp.fc2.weight", "proj_out.weight")
+_BRANCH_OUT = ("out_layers.3.weight", "attn.proj.weight", "mlp.fc2.weight", "proj_out.weight", "out_layers.1.weight")
+
+
+def param_spec(cfg):
+    """The ``state_dict`` inventory of the denoiser a config describes."""
+    if isinstance(cfg, UNetModelConvConfig):
+        return unetconv_param_spec(cfg)
+    return unetmodel_param_spec(cfg) if isinstance(cfg, UNetModelConfig) else unet_param_spec(cfg)
 
 
 def random_state_dict(cfg, seed: int = 0) -> Dict[str, torch.Tensor]:
-    """For a UNetConfig (UNetModelSwin) or a UNetModelConfig (UNetModel)."""
+    """For a UNetConfig (UNetModelSwin), a UNetModelConfig (UNetModel) or a UNetModelConvConfig (UNetModelConv)."""
     g = torch.Generator().manual_seed(seed)
     sd: Dict[str, torch.Tensor] = {}
-    spec = unetmodel_param_spec(cfg) if isinstance(cfg, UNetModelConfig) else unet_param_spec(cfg)
+    spec = param_spec(cfg)
     for name, shape, role in spec:
         if role in ("conv3", "conv1", "linear"):
             fan_in = math.prod(shape[1:])
