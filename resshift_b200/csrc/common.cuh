@@ -176,6 +176,12 @@ __device__ __forceinline__ uint32_t mapa_u32(uint32_t addr, uint32_t rank) {
   asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(addr), "r"(rank));
   return r;
 }
+// two floats from the shared memory of a CTA of the cluster (address from mapa_u32)
+__device__ __forceinline__ float2 ld_dsmem_f32x2(uint32_t addr) {
+  float2 v;
+  asm volatile("ld.shared::cluster.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"(addr) : "memory");
+  return v;
+}
 // 2-D tile load written to the same shared-memory offset of every CTA in `cta_mask`; each destination CTA's barrier at
 // the offset of `bar` receives the bytes that landed there
 __device__ __forceinline__ void tma_load_2d_mc(void* dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1, uint16_t cta_mask) {
@@ -205,6 +211,10 @@ __device__ __forceinline__ void st_shared_v4(uint32_t addr, uint32_t a, uint32_t
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
+}
+// counts toward named barrier `id` without waiting for it (the other side of a bar.sync by the remaining threads)
+__device__ __forceinline__ void named_bar_arrive(int id, int nthreads) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
 
 // ----------------------------------------------------------------------------------------

@@ -166,6 +166,26 @@ __device__ __forceinline__ void pivot_stats2(Ld ld, int rows, float2& mean, floa
   m2 = make_float2(fmaxf(s2.x - s1.x * s1.x * inv, 0.f), fmaxf(s2.y - s1.y * s1.y * inv, 0.f));
 }
 
+// One step of warp_chunk_stats' transpose-reduce: lanes that differ in bit 2 * kHalf exchange halves of their first
+// 2 * kHalf columns.  The step width is a template argument so that every sv / sq index is a compile-time constant:
+// written as one loop over (half >>= 1, bit >>= 1), nvcc kept a run-time index and put sv / sq in local memory, which
+// in the MMA kernels (most of L1 carved out as shared memory) went to L2 and cost about 10 us per 128-row tile of the
+// fused MLP at E = 192.
+template <int kHalf>
+__device__ __forceinline__ void warp_xor_step(float (&sv)[16], float (&sq)[16], int lane) {
+  constexpr int bit = 2 * kHalf;
+  const bool upper = (lane & bit) != 0;
+#pragma unroll
+  for (int j = 0; j < kHalf; ++j) {
+    const float send_s = upper ? sv[j] : sv[j + kHalf];
+    const float keep_s = upper ? sv[j + kHalf] : sv[j];
+    sv[j] = keep_s + __shfl_xor_sync(0xffffffffu, send_s, bit);
+    const float send_q = upper ? sq[j] : sq[j + kHalf];
+    const float keep_q = upper ? sq[j + kHalf] : sq[j];
+    sq[j] = keep_q + __shfl_xor_sync(0xffffffffu, send_q, bit);
+  }
+}
+
 // Statistics of one epilogue chunk while the accumulator tile drains: this warp's 32 rows x 16 columns, the values
 // exactly as stored (o0 / o1 = the two 16-byte units of fp16 the lane writes).  Transpose-reduce over the 32 lanes
 // (16 shuffles per moment, fixed tree), then (sum, sum of squares) -> (mean, M2) right here: over 32 fp16 values the
@@ -183,19 +203,10 @@ __device__ __forceinline__ void warp_chunk_stats(const uint4& o0, const uint4& o
   }
 #pragma unroll
   for (int j = 0; j < 16; ++j) sq[j] = sv[j] * sv[j];
-#pragma unroll
-  for (int half = 8, bit = 16; half >= 1; half >>= 1, bit >>= 1) {
-    const bool upper = (lane & bit) != 0;
-#pragma unroll
-    for (int j = 0; j < half; ++j) {
-      const float send_s = upper ? sv[j] : sv[j + half];
-      const float keep_s = upper ? sv[j + half] : sv[j];
-      sv[j] = keep_s + __shfl_xor_sync(0xffffffffu, send_s, bit);
-      const float send_q = upper ? sq[j] : sq[j + half];
-      const float keep_q = upper ? sq[j + half] : sq[j];
-      sq[j] = keep_q + __shfl_xor_sync(0xffffffffu, send_q, bit);
-    }
-  }
+  warp_xor_step<8>(sv, sq, lane);
+  warp_xor_step<4>(sv, sq, lane);
+  warp_xor_step<2>(sv, sq, lane);
+  warp_xor_step<1>(sv, sq, lane);
   sv[0] += __shfl_xor_sync(0xffffffffu, sv[0], 1);
   sq[0] += __shfl_xor_sync(0xffffffffu, sq[0], 1);
   if ((lane & 1) == 0) {

@@ -737,7 +737,17 @@ inline int mlp_finalize(MlpDesc& d) {
   d.smem = (size_t)MlpSmem(d.E, d.Hd, p.ring).total + 1024;
   RS_CHECK(d.smem <= 227 * 1024, "fused MLP: shared memory budget exceeded");
   p.has_res = d.has_res ? 1 : 0;
-  d.grid = p.tiles_w * p.tiles_h * tiles_n;
+  // Few tiles leave most SMs idle (batch 16: 32 tiles at 16x16, 8 at 8x8): split each tile's hidden chunks over a
+  // cluster of p.split CTAs, the smallest divisor of the chunk count that brings the grid to half the SMs, else the
+  // largest, and at most 4.  Measured at batch 16, E = 192, hidden 768 (DESIGN.md §7), us per launch for S = 1 / 2 / 3
+  // / 4 / 6: 8x8 38.4 / 31.0 / 29.0 / 28.7 / 30.1, 16x16 38.7 / 31.4 / 29.9 / 44.8 / 49.6; 32x32 (128 tiles) is
+  // fastest unsplit.  The reduction needs the ring to hold a 128 x E fp32 partial.
+  const int tiles = p.tiles_w * p.tiles_h * tiles_n, chunks = d.Hd / kMlpHc;
+  p.split = 1;
+  if (p.ring * slot >= kConvBM * d.E * 4)
+    for (int s = 2; s <= 4 && tiles * p.split < num_sms() / 2; ++s)
+      if (chunks % s == 0) p.split = s;
+  d.grid = tiles * p.split;
   int rc = encode_act_map(&p.tmX, d.in.ptr, d.E, W, H, N, d.in.sW(), d.in.sH(), d.in.sN(), p.bw, p.bh, p.bn, 64);
   if (rc) return rc;
   rc = encode_weight_map(&p.tmW1, d.w1, d.E, d.Hd, kMlpHc); if (rc) return rc;
@@ -755,10 +765,10 @@ inline int mlp_finalize(MlpDesc& d) {
 
 inline int mlp_launch(const MlpDesc& d, cudaStream_t st) {
   switch (d.E) {
-    case 64: (void)launch_k(mlp_fused_sm90_kernel<64>, dim3(d.grid), dim3(kMlpThreads), d.smem, st, d.prm); break;
-    case 128: (void)launch_k(mlp_fused_sm90_kernel<128>, dim3(d.grid), dim3(kMlpThreads), d.smem, st, d.prm); break;
-    case 192: (void)launch_k(mlp_fused_sm90_kernel<192>, dim3(d.grid), dim3(kMlpThreads), d.smem, st, d.prm); break;
-    case 256: (void)launch_k(mlp_fused_sm90_kernel<256>, dim3(d.grid), dim3(kMlpThreads), d.smem, st, d.prm); break;
+    case 64: (void)launch_kc(mlp_fused_sm90_kernel<64>, dim3(d.grid), dim3(kMlpThreads), d.smem, st, d.prm.split, d.prm); break;
+    case 128: (void)launch_kc(mlp_fused_sm90_kernel<128>, dim3(d.grid), dim3(kMlpThreads), d.smem, st, d.prm.split, d.prm); break;
+    case 192: (void)launch_kc(mlp_fused_sm90_kernel<192>, dim3(d.grid), dim3(kMlpThreads), d.smem, st, d.prm.split, d.prm); break;
+    case 256: (void)launch_kc(mlp_fused_sm90_kernel<256>, dim3(d.grid), dim3(kMlpThreads), d.smem, st, d.prm.split, d.prm); break;
     default: RS_CHECK(false, "fused MLP: embedding width");
   }
   RS_CUDA_OK(cudaGetLastError());
