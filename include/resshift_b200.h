@@ -412,17 +412,30 @@ int rs_op_window_attention(const void* qkv, int N, int H, int W, int heads, int 
 int rs_op_expand_relpos_ex(const float* table, float* dense, int heads, int window, void* stream);
 int rs_op_window_attention_ex(const void* qkv, int N, int H, int W, int heads, int window, int head_dim, int shift,
                               const float* bias_dense, void* out, void* stream);
+/* the same with the launch given explicitly: hpc heads per CTA of the tensor-core instance (0: the launcher's rule, which
+ * the plans use; otherwise a divisor of heads), simt != 0 for the fp32 cross-check (hpc 0 or 1).  A configuration is
+ * launched as asked or refused with a message naming the argument.  info[5] (may be NULL): SIMT kernel (0 / 1), heads
+ * per CTA, grid x (windows), grid y (head groups), dynamic shared memory in bytes. */
+int rs_op_window_attention_cfg(const void* qkv, int N, int H, int W, int heads, int window, int head_dim, int shift,
+                               const float* bias_dense, void* out, int hpc, int simt, int32_t* info, void* stream);
 /* fused attention half of a Swin block: y = x + proj(window_attention(qkv(norm1(x)))) (reference
  * models/swin_transformer.py:246-275 with WindowAttention.forward :114-145); x NHWC fp16 [N,H,W,E] (in place when
- * y == x), norm1 statistics as the producers' (mean, M2) pairs gn_part[N][gn_slots][E][2], weights packed fp16;
- * part_out (optional): pairs of y per 8x8 window, [N][(H/8)*(W/8)][E][2]; gstat_out (optional, needs part_out; counters
- * [N] are accepted for compatibility and not used): the 32 group (mean, rstd) of y per image, reduced from the window
- * pairs by a finalisation kernel after the attention kernel.  relbias_dense must be the output of rs_op_expand_relpos
- * (relative_position_bias_table gathered by relative_position_index, :82-97,130-133). */
+ * y == x), norm1 statistics as the producers' (mean, M2) pairs gn_part[N][gn_slots][E][2] (gn_slots equal boxes of each
+ * image), weights packed fp16; part_out (optional): pairs of y per 8x8 window of the shifted partition,
+ * [N][(H/8)*(W/8)][E][2].  relbias_dense must be the output of rs_op_expand_relpos (relative_position_bias_table
+ * gathered by relative_position_index, :82-97,130-133).  gstat_out_null and counters_null must be NULL: the group
+ * statistics of y are the consuming GroupNorm's to combine from part_out. */
 int rs_op_swin_attn(const void* x, int N, int H, int W, int E, int heads, int shift, const float* gn_part, int gn_slots,
                     const float* gamma, const float* beta, const void* wqkv_packed, const float* bqkv, const float* relbias_dense,
-                    const void* wproj_packed, const float* bproj, void* y, float* part_out, float* gstat_out_or_null,
-                    uint32_t* counters_or_null, void* stream);
+                    const void* wproj_packed, const float* bproj, void* y, float* part_out, float* gstat_out_null,
+                    uint32_t* counters_null, void* stream);
+/* the same on a persistent grid of `grid` CTAs (0: min(window pairs, SMs), what the plans run; otherwise at most the
+ * number of window pairs), each walking a contiguous run of pairs.  info[3] (may be NULL): grid, window pairs per CTA
+ * at most, windows per image. */
+int rs_op_swin_attn_ex(const void* x, int N, int H, int W, int E, int heads, int shift, const float* gn_part, int gn_slots,
+                       const float* gamma, const float* beta, const void* wqkv_packed, const float* bqkv,
+                       const float* relbias_dense, const void* wproj_packed, const float* bproj, void* y, float* part_out,
+                       int grid, int32_t* info, void* stream);
 /* fused Swin MLP (reference models/swin_transformer.py:17-33,279): out = residual + fc2(GELU(fc1(x))) in one kernel,
  * E in {64, 128, 192, 256}, Hd % 64 == 0; dbg_timeline_or_null must be NULL */
 int rs_op_mlp(const void* x, int N, int H, int W, int E, int Hd, const void* w1_packed, const float* b1,

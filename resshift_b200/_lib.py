@@ -156,8 +156,12 @@ _SIGNATURES = {
     "rs_op_softmax_rows":(C.c_int, [_P, C.c_int, C.c_int, C.c_longlong, C.c_float, _P]),
     "rs_op_window_attention": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P, _P]),
     "rs_op_window_attention_ex": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P, _P]),
+    "rs_op_window_attention_cfg": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P,
+                                             C.c_int, C.c_int, C.POINTER(C.c_int32), _P]),
     "rs_op_swin_attn": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, C.c_int, _P, _P, _P, _P, _P, _P, _P,
                                   _P, _P, _P, _P, _P]),
+    "rs_op_swin_attn_ex": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, C.c_int, _P, _P, _P, _P, _P,
+                                     _P, _P, _P, _P, C.c_int, C.POINTER(C.c_int32), _P]),
     "rs_op_mlp": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P, _P, _P, _P, _P, _P, _P]),
     "rs_op_mlp_ex": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P, _P, _P, _P, _P,
                                C.POINTER(_P), C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(C.c_int32), _P]),

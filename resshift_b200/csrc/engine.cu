@@ -1075,7 +1075,7 @@ int bind_ops(rs_plan& P, std::vector<Op>& ops) {
         w.gamma = E.at<float>(b + ".norm1.weight"); w.beta = E.at<float>(b + ".norm1.bias");
         RS_CHECK(w.wqkv && w.wproj && w.bqkv && w.bproj && w.relbias && w.gamma && w.beta, "missing attention parameters of " + b);
         const GnSink sk = make_sink(P, so.norm1, 0);
-        w.gn_part = sk.part; w.gn_slots = so.norm1.slots; w.gn_gstat = sk.gstat;
+        w.gn_part = sk.part; w.gn_slots = so.norm1.slots;
         bind_sinks(P, so, w.sink);
         rc = swin_attn_finalize(w);
         break;
@@ -1586,8 +1586,20 @@ static void collect_profile(const rs_plan& P, const Prof& prof, double* ms, char
         break;
       }
       case OP_MLP: { const MlpDesc& m = payload<MlpOp>(op).d; snprintf(d, desc_stride, "mlp %dx%d E=%d Hd=%d grid=%d", m.in.H, m.in.W, m.E, m.Hd, m.grid); break; }
-      case OP_ATTN: { const WinAttnOp& a = payload<WinAttnOp>(op); snprintf(d, desc_stride, "attn %dx%d window=%d shift=%d", a.qkv.H, a.qkv.W, a.window, a.shift); break; }
-      case OP_SWIN_ATTN: { const SwinAttnDesc& w = payload<SwinOp>(op).d; snprintf(d, desc_stride, "swin_attn %dx%d shift=%d grid=%d", w.x.H, w.x.W, w.shift, w.grid); break; }
+      case OP_ATTN: {       // everything rs_op_window_attention_cfg needs to replay it, and the heads per CTA it should report
+        const WinAttnOp& a = payload<WinAttnOp>(op);
+        const int heads = P.e->cfg.swin_heads, hd = P.e->cfg.swin_embed_dim / heads;
+        const int hpc = a.simt ? 1 : attn_default_hpc(heads, (long long)a.qkv.N * (a.qkv.H / a.window) * (a.qkv.W / a.window));
+        snprintf(d, desc_stride, "attn %dx%d window=%d shift=%d N=%d heads=%d head_dim=%d hpc=%d simt=%d", a.qkv.H, a.qkv.W,
+                 a.window, a.shift, a.qkv.N, heads, hd, hpc, (int)a.simt);
+        break;
+      }
+      case OP_SWIN_ATTN: {  // ... rs_op_swin_attn_ex, with the persistent grid it should report
+        const SwinAttnDesc& w = payload<SwinOp>(op).d;
+        snprintf(d, desc_stride, "swin_attn %dx%d shift=%d grid=%d N=%d E=%d heads=%d slots=%d", w.x.H, w.x.W, w.shift, w.grid,
+                 w.x.N, w.x.C, w.heads, w.gn_slots);
+        break;
+      }
       case OP_SOFTMAX: snprintf(d, desc_stride, "softmax %d", payload<SoftmaxOp>(op).view.C); break;
       case OP_VQ_ATTN: {     // the query-row range only when it is not all T rows (the default launch keeps its description)
         const VqAttnDesc& a = payload<VqAttnDesc>(op);

@@ -779,16 +779,14 @@ inline int mlp_launch(const MlpDesc& d, cudaStream_t st) {
 struct SwinAttnDesc {
   View x, y;                               // input / output token tensors [N, H, W, E] (y may alias x)
   int heads = 0, shift = 0;
-  const float* gn_part = nullptr; int gn_slots = 0; const float* gn_gstat = nullptr;
+  const float* gn_part = nullptr; int gn_slots = 0;
   const float* gamma = nullptr; const float* beta = nullptr;
   const __half* wqkv = nullptr; int wqkv_ld = 0; const float* bqkv = nullptr;
   const float* relbias = nullptr;
   const __half* wproj = nullptr; int wproj_ld = 0; const float* bproj = nullptr;
-  GnSink sink[2] = {};
+  GnSink sink[2] = {};                     // window pairs of y only: the consumer combines them
   SwinAttnParams prm;
-  // the kernel delivers window pairs; a sink with group statistics gets them from gn_finalize_kernel right after it
-  GnFinalizeParams fin[2] = {};
-  int grid = 0;
+  int grid = 0;                            // persistent CTAs: swin_attn_finalize sets min(pairs, SMs)
 };
 // (8x8 windows and 32-wide heads only: every other level takes the four-launch form around window_attn_kernel)
 inline bool swin_attn_supported(int E, int heads, int H, int W, int window) {
@@ -801,12 +799,14 @@ inline int swin_attn_finalize(SwinAttnDesc& d) {
   RS_CHECK(swin_attn_supported(E, d.heads, d.x.H, d.x.W, 8), "fused Swin attention: E in {64, 192}, head_dim 32, H and W multiples of 8");
   RS_CHECK(d.y.C == E && d.y.H == d.x.H && d.y.W == d.x.W && d.y.N == d.x.N, "fused Swin attention: output geometry");
   RS_CHECK(d.x.ld % 8 == 0 && d.y.ld % 8 == 0 && d.wqkv_ld % 8 == 0 && d.wproj_ld % 8 == 0, "fused Swin attention: 16-byte rows");
-  RS_CHECK((d.gn_part && d.gn_slots > 0) || d.gn_gstat, "fused Swin attention: norm1 statistics");
+  RS_CHECK(d.gn_part && d.gn_slots > 0, "fused Swin attention: norm1 statistics");
+  RS_CHECK(d.x.H * d.x.W % d.gn_slots == 0,
+           "fused Swin attention: norm1 slots must divide H*W = " + std::to_string(d.x.H * d.x.W) + ", got " + std::to_string(d.gn_slots));
   int rc = encode_weight_map(&p.tmWqkv, d.wqkv, d.wqkv_ld, 3 * E, 64); if (rc) return rc;
   rc = encode_weight_map(&p.tmWproj, d.wproj, d.wproj_ld, E, 64); if (rc) return rc;
   p.x = d.x.ptr; p.x_ld = d.x.ld; p.y = d.y.ptr; p.y_ld = d.y.ld;
   p.N = d.x.N; p.H = d.x.H; p.W = d.x.W; p.heads = d.heads; p.shift = d.shift; p.scale = 0.17677669529663687f;
-  p.gn_part = d.gn_part; p.gn_slots = d.gn_slots; p.gn_gstat = d.gn_gstat; p.gamma = d.gamma; p.beta = d.beta; p.eps = 1e-5f;
+  p.gn_part = d.gn_part; p.gn_slots = d.gn_slots; p.gamma = d.gamma; p.beta = d.beta; p.eps = 1e-5f;
   p.wqkv = d.wqkv; p.wqkv_ld = d.wqkv_ld; p.bqkv = d.bqkv; p.relbias = d.relbias;
   p.wproj = d.wproj; p.wproj_ld = d.wproj_ld; p.bproj = d.bproj;
   p.total_windows = d.x.N * (d.x.H / 8) * (d.x.W / 8);
@@ -816,25 +816,12 @@ inline int swin_attn_finalize(SwinAttnDesc& d) {
   compact_sinks(d.sink, nW, p.sink);
   const int pairs = (p.total_windows + 1) / 2;
   d.grid = std::min(pairs, num_sms());
-  for (int k = 0; k < 2; ++k) {
-    d.fin[k] = GnFinalizeParams{};
-    if (p.sink[k].gstat) {
-      RS_CHECK(p.sink[k].coff == 0 && p.sink[k].cstride == E, "fused Swin attention: group statistics of a channel slice");
-      d.fin[k] = GnFinalizeParams{p.sink[k].part, p.sink[k].gstat, nW, E, 64.0f, p.sink[k].eps};
-    }
-    p.sink[k].gstat = nullptr; p.sink[k].counter = nullptr;
-  }
   return 0;
 }
 inline int swin_attn_launch(const SwinAttnDesc& d, cudaStream_t st) {
   if (d.x.C == 192) (void)launch_k(swin_attn_fused_kernel<192>, dim3(d.grid), dim3(kSwinThreads), (size_t)SwinSmem<192>::launch_bytes, st, d.prm);
   else (void)launch_k(swin_attn_fused_kernel<64>, dim3(d.grid), dim3(kSwinThreads), (size_t)SwinSmem<64>::launch_bytes, st, d.prm);
   RS_CUDA_OK(cudaGetLastError());
-  for (int k = 0; k < 2; ++k)
-    if (d.fin[k].gstat) {
-      (void)launch_k(gn_finalize_kernel, dim3(32, d.x.N), dim3(256), (size_t)0, st, d.fin[k]);
-      RS_CUDA_OK(cudaGetLastError());
-    }
   return 0;
 }
 
@@ -934,42 +921,57 @@ inline int unet_attn_launch(const UnetAttnDesc& d, cudaStream_t st) {
   return 0;
 }
 
-// one launch of the window-attention core: the instance of window_attn_kernel for (window side, head width), or with
-// simt the SIMT cross-check (RS_ATTN_IMPL=simt)
-template <int WS, int HD>
-inline int attn_launch_instance(WinAttnParams& p, int windows, cudaStream_t st) {
-  // heads per CTA: all of them when there are plenty of windows, fewer (more CTAs) otherwise
-  const int heads = p.heads;
+// heads per CTA of window_attn_kernel when the caller does not ask for a count: all of them when there are plenty of
+// windows, fewer (more CTAs) otherwise
+inline int attn_default_hpc(int heads, long long windows) {
   int hpc = heads;
-  while (hpc > 1 && (long long)windows * (heads / hpc) < 4 * num_sms() && hpc % 2 == 0) hpc /= 2;
-  if (hpc > 1 && (long long)windows * (heads / hpc) < 4 * num_sms() && heads % hpc == 0) hpc = 1;
-  p.hpc = hpc;
+  while (hpc > 1 && windows * (heads / hpc) < 4 * num_sms() && hpc % 2 == 0) hpc /= 2;
+  if (hpc > 1 && windows * (heads / hpc) < 4 * num_sms() && heads % hpc == 0) hpc = 1;
+  return hpc;
+}
+
+// what one launch of the window-attention core runs: the SIMT cross-check (one head per CTA) or the instance of
+// window_attn_kernel with hpc heads per CTA
+struct AttnLaunch { bool simt; int hpc; dim3 grid; size_t smem; };
+
+// one launch of the window-attention core: the instance of window_attn_kernel for (window side, head width), or with
+// simt the SIMT cross-check (RS_ATTN_IMPL=simt).  hpc = heads per CTA (0: attn_default_hpc); *info = what was launched
+template <int WS, int HD>
+inline int attn_launch_instance(WinAttnParams& p, int windows, int hpc, AttnLaunch* info, cudaStream_t st) {
+  const int heads = p.heads;
+  p.hpc = hpc ? hpc : attn_default_hpc(heads, windows);
   // (at WS = 8 sized for the output channels of all heads: an upper bound of what hpc heads stage)
-  const size_t smem = window_attn_smem_bytes<WS, HD>(WS == 8 ? heads : hpc);
+  const size_t smem = window_attn_smem_bytes<WS, HD>(WS == 8 ? heads : p.hpc);
   RS_CHECK(smem <= (size_t)kAttnMaxSmem, "attention tile does not fit in shared memory");   // limit raised in conv_init()
-  (void)launch_k(window_attn_kernel<WS, HD>, dim3(windows, heads / hpc), dim3(WS == 8 ? 128 : 256), smem, st, p);
+  const dim3 grid(windows, heads / p.hpc);
+  if (info) *info = AttnLaunch{false, p.hpc, grid, smem};
+  (void)launch_k(window_attn_kernel<WS, HD>, grid, dim3(WS == 8 ? 128 : 256), smem, st, p);
   return 0;
 }
 
 inline int attn_launch(const View& qkv, const View& out, const float* bias, int heads, int E, int window, int shift,
-                       bool simt, cudaStream_t st) {
+                       bool simt, cudaStream_t st, int hpc = 0, AttnLaunch* info = nullptr) {
   RS_CHECK(window == 8 || window == 16, "window attention kernels: window_size 8 or 16, got " + std::to_string(window));
   RS_CHECK(heads > 0 && E % heads == 0 && (E / heads == 32 || E / heads == 64),
            "window attention kernels: head_dim 32 or 64");
   RS_CHECK(qkv.H % window == 0 && qkv.W % window == 0,
            "window attention needs H, W multiples of the window (" + std::to_string(window) + ")");
   RS_CHECK(shift == 0 || shift == window / 2, "window attention: shift is 0 or half the window");
+  RS_CHECK(hpc >= 0 && (hpc == 0 || heads % hpc == 0),
+           "window attention: hpc must divide heads = " + std::to_string(heads) + ", got " + std::to_string(hpc));
+  RS_CHECK(!simt || hpc <= 1, "window attention: hpc must be 0 or 1 for the SIMT kernel (one head per CTA)");
   const int hd = E / heads;
   const int windows = qkv.N * (qkv.H / window) * (qkv.W / window);
   WinAttnParams p{qkv.ptr, qkv.ld, out.ptr, out.ld, bias, qkv.N, qkv.H, qkv.W, heads, E, shift,
                   hd == 32 ? 0.17677669529663687f : 0.125f, heads, window, hd};
   int rc = 0;
   if (simt) {
+    if (info) *info = AttnLaunch{true, 1, dim3(windows, heads), 0};
     (void)launch_k(window_attn_simt_kernel, dim3(windows, heads), dim3(window * window), (size_t)0, st, p);
   } else if (window == 8) {
-    rc = hd == 32 ? attn_launch_instance<8, 32>(p, windows, st) : attn_launch_instance<8, 64>(p, windows, st);
+    rc = hd == 32 ? attn_launch_instance<8, 32>(p, windows, hpc, info, st) : attn_launch_instance<8, 64>(p, windows, hpc, info, st);
   } else {
-    rc = hd == 32 ? attn_launch_instance<16, 32>(p, windows, st) : attn_launch_instance<16, 64>(p, windows, st);
+    rc = hd == 32 ? attn_launch_instance<16, 32>(p, windows, hpc, info, st) : attn_launch_instance<16, 64>(p, windows, hpc, info, st);
   }
   if (rc) return rc;
   RS_CUDA_OK(cudaGetLastError());

@@ -42,8 +42,8 @@ struct SwinAttnParams {
   int N, H, W, heads;
   int shift;                            // 0 or 4
   float scale;                          // head_dim^-0.5
-  // norm1: producers' pairs (gn_part, gn_slots) or finalised group statistics (gn_gstat)
-  const float* gn_part; int gn_slots; const float* gn_gstat;
+  // norm1: the producers' (mean, M2) pairs gn_part[N][gn_slots][E][2]
+  const float* gn_part; int gn_slots;
   const float* gamma; const float* beta; float eps;
   const __half* wqkv; int wqkv_ld;      // [3E][E] fp16, row stride wqkv_ld
   const float* bqkv;                    // [3E]
@@ -195,25 +195,18 @@ __global__ void __launch_bounds__(kSwinThreads, 1) swin_attn_fused_kernel(const 
     // ---- norm1 affine of the window's image (recomputed only when the image changes) ----
     if (n_img != cur_img) {                                 // uniform over the warpgroup
       constexpr int cpg = kE / 32;
-      if (p.gn_gstat) {
-        if (wt < 32) {
-          const float2 mr = ldcg_f2(p.gn_gstat + ((size_t)n_img * 32 + wt) * 2);
-          sMR[wt * 2] = mr.x; sMR[wt * 2 + 1] = mr.y;
-        }
-      } else {
-        const float ns = (float)HW / (float)p.gn_slots;
-        for (int c = wt; c < kE; c += 128) {
-          const float2 mq = gn_channel_from_pairs(p.gn_part + (size_t)n_img * p.gn_slots * kE * 2 + (size_t)c * 2, p.gn_slots, kE, ns);
-          sScr[c * 2] = mq.x; sScr[c * 2 + 1] = mq.y;
-        }
-        wg_sync();
-        if (wt < 32) {
-          float chp[2 * cpg];
+      const float ns = (float)HW / (float)p.gn_slots;
+      for (int c = wt; c < kE; c += 128) {
+        const float2 mq = gn_channel_from_pairs(p.gn_part + (size_t)n_img * p.gn_slots * kE * 2 + (size_t)c * 2, p.gn_slots, kE, ns);
+        sScr[c * 2] = mq.x; sScr[c * 2 + 1] = mq.y;
+      }
+      wg_sync();
+      if (wt < 32) {
+        float chp[2 * cpg];
 #pragma unroll
-          for (int k = 0; k < cpg; ++k) { chp[2 * k] = sScr[(wt * cpg + k) * 2]; chp[2 * k + 1] = sScr[(wt * cpg + k) * 2 + 1]; }
-          const float2 mr = gn_group_from_channels(chp, cpg, (float)HW, p.eps);
-          sMR[wt * 2] = mr.x; sMR[wt * 2 + 1] = mr.y;
-        }
+        for (int k = 0; k < cpg; ++k) { chp[2 * k] = sScr[(wt * cpg + k) * 2]; chp[2 * k + 1] = sScr[(wt * cpg + k) * 2 + 1]; }
+        const float2 mr = gn_group_from_channels(chp, cpg, (float)HW, p.eps);
+        sMR[wt * 2] = mr.x; sMR[wt * 2 + 1] = mr.y;
       }
       wg_sync();
       for (int c = wt; c < kE; c += 128) {

@@ -40,11 +40,12 @@ for tot, share, n, avg, desc in rows:
         E = int(re.search(r"E=(\d+)", desc).group(1))
         fl = 2.0 * px * E * 4 * E * 2
     elif desc.startswith("swin_attn"):
-        E = 192
+        E = int(re.search(r"E=(\d+)", desc).group(1))
         fl = px * (8.0 * E * E + 256.0 * E)
     elif desc.startswith("attn"):
-        E = 192
-        fl = px * 256.0 * E
+        E = int(re.search(r"heads=(\d+)", desc).group(1)) * int(re.search(r"head_dim=(\d+)", desc).group(1))
+        T = int(re.search(r"window=(\d+)", desc).group(1)) ** 2
+        fl = px * 4.0 * T * E
         by = px * (3 * E + E) * 2.0
     elif desc.startswith("gn"):
         C = int(re.search(r"C=(\d+)", desc).group(1))

@@ -1,6 +1,6 @@
 """GPU parity of the window-attention core's four instances (windows of 8 or 16, heads of 32 or 64) and of UNetModelSwin
-built with 16x16 windows and / or 64-wide heads: the core against fp32 torch on the same fp16 operands and against the
-SIMT cross-check; whole forwards against the reference's goldens (tests/golden/unet_windows.npz) and the fp32 oracle; the
+built with 16x16 windows and / or 64-wide heads: the core and the SIMT cross-check per element against float64 (the
+bounds of tests/test_gpu_attention.py); whole forwards against the reference's goldens (tests/golden/unet_windows.npz) and the fp32 oracle; the
 fused 4-step loop; a 128x128 latent; batch independence; graph replay; the sampler's padding.  Bounds are those of
 test_gpu_unet.py and test_gpu_ops.py."""
 import hashlib
@@ -16,7 +16,6 @@ from oracle import unet_variants_oracle as uo
 from oracle.make_golden_variants import OUT_STRIDE, trajectory_inputs, variant_inputs
 from oracle.make_golden_windows import LOOP_MODEL, WINDOWS, windows_config
 from resshift_b200 import _lib
-from resshift_b200.arch import relative_position_index, shifted_window_mask
 from resshift_b200.weights import random_state_dict
 
 FWD_MAX, FWD_MEAN = 1e-2, 2.5e-3
@@ -53,47 +52,22 @@ def _core(qkv, table, heads, ws, hd, shift, impl):
     return out
 
 
-def _core_reference(qkv, table, heads, ws, hd, shift):
-    """roll / partition / attention core / reverse / roll in fp32 (reference models/swin_transformer.py:114-145,251-275)."""
-    N, H, W, _ = qkv.shape
-    E, T = heads * hd, ws * ws
-    y = qkv.float().permute(0, 3, 1, 2)
-    if shift:
-        y = torch.roll(y, (-shift, -shift), (2, 3))
-    yw = y.reshape(N, 3 * E, H // ws, ws, W // ws, ws).permute(0, 2, 4, 3, 5, 1).reshape(-1, T, 3, heads, hd)
-    q, k, v = (yw[:, :, i].transpose(1, 2) for i in range(3))
-    attn = (q * hd ** -0.5) @ k.transpose(-2, -1)
-    idx = relative_position_index(ws).reshape(-1).to(qkv.device)
-    attn = attn + table[idx].view(T, T, heads).permute(2, 0, 1)[None]
-    if shift:
-        m = shifted_window_mask(H, W, ws, shift).to(qkv.device)
-        attn = (attn.view(-1, m.shape[0], heads, T, T) + m[None, :, None]).view(-1, heads, T, T)
-    o = (attn.softmax(-1) @ v).transpose(1, 2).reshape(-1, T, E)
-    o = o.view(N, H // ws, W // ws, ws, ws, E).permute(0, 5, 1, 3, 2, 4).reshape(N, E, H, W)
-    if shift:
-        o = torch.roll(o, (shift, shift), (2, 3))
-    return o.permute(0, 2, 3, 1)
-
-
 # (windows along H, windows along W): one window, rectangular with odd counts both ways, the last row of windows masked
 @pytest.mark.parametrize("shifted", [False, True])
 @pytest.mark.parametrize("grid", [(1, 1), (3, 1), (2, 5), (4, 4)])
 @pytest.mark.parametrize("heads", [1, 3, 6])
 @pytest.mark.parametrize("ws,hd", INSTANCES)
 def test_core_instances_vs_fp32_and_simt(ws, hd, heads, grid, shifted):
+    """Each instance and the SIMT cross-check per element against float64 (tests/test_gpu_attention.py); the
+    RS_ATTN_IMPL-selected rs_op_window_attention_ex gives the same bits as the explicit launch."""
+    from tests.test_gpu_attention import WindowCase
     if shifted and grid == (1, 1):
         pytest.skip("no shifted windows at a single-window resolution")
-    N, H, W, shift = 3, grid[0] * ws, grid[1] * ws, ws // 2 if shifted else 0
-    qkv, table = _core_inputs(N, H, W, heads, ws, hd, seed=ws * 100 + hd + heads + H + shift)
-    out = _core(qkv, table, heads, ws, hd, shift, "mma")
-    simt = _core(qkv, table, heads, ws, hd, shift, "simt")
-    ref = _core_reference(qkv, table, heads, ws, hd, shift)
-    tol = 4e-3 * ref.abs().max().item() + 2e-3
-    for tag, got in (("tensor core", out), ("simt", simt)):
-        assert not torch.isnan(got).any(), tag
-        d = (got.float() - ref).abs().max().item()
-        assert d <= tol, (tag, d, tol)
-    assert (out.float() - simt.float()).abs().max().item() <= tol
+    shift = ws // 2 if shifted else 0
+    L = WindowCase("randn", 3, grid[0], grid[1], heads, ws, hd, shift, seed=ws * 100 + hd + heads + grid[0] * ws + shift)
+    for impl in ("mma", "simt"):
+        out, _ = L.check(f"core {impl} ws={ws} hd={hd} heads={heads} grid={grid} shift={shift}", simt=impl == "simt")
+        assert torch.equal(out, _core(L.qkv, L.table, heads, ws, hd, shift, impl)), impl
 
 
 @pytest.mark.parametrize("shift", [0, 4])

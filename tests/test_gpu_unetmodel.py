@@ -1,10 +1,9 @@
 """GPU tests of the reference's global-attention UNetModel on the native kernels: the multi-head attention kernel
-(csrc/unet_attn.cuh) against fp32 torch on the same fp16 operands over head dims, head counts, sequence lengths and
-both head orders, its determinism and per-image independence; every fixture of tests/golden/unetmodel.npz against the
+(csrc/unet_attn.cuh) per element against float64 on the same fp16 operands over head dims, head counts, sequence
+lengths and both head orders, its determinism and per-image independence; every fixture of tests/golden/unetmodel.npz against the
 reference and the fp32 oracle; the fused 4-step loop with graph replay; a 64x128 latent; ResShiftSampler end to end
 from a ``models.unet.UNetModel`` config, one GPU and a device pool.  Bounds are those of test_gpu_ops.py (kernel) and
 test_gpu_unet.py (models)."""
-import math
 
 import numpy as np
 import pytest
@@ -32,41 +31,14 @@ def _attn(qkv, N, T, heads, D, new_order):
     return out
 
 
-def _attn_ref(qkv, N, T, heads, D, new_order):
-    """fp32 torch on the fp16 operands, one (image, head) at a time."""
-    C = heads * D
-    x = qkv.float().view(N, T, 3 * C)
-    out = torch.empty(N, T, C, dtype=torch.float32, device="cuda")
-    for h in range(heads):
-        if new_order:
-            q, k, v = x[..., D * h:D * (h + 1)], x[..., C + D * h:C + D * (h + 1)], x[..., 2 * C + D * h:2 * C + D * (h + 1)]
-        else:
-            b = 3 * D * h
-            q, k, v = x[..., b:b + D], x[..., b + D:b + 2 * D], x[..., b + 2 * D:b + 3 * D]
-        for n in range(N):
-            s = (q[n] @ k[n].t()) / math.sqrt(D)
-            out[n, :, D * h:D * (h + 1)] = torch.softmax(s, dim=-1) @ v[n]
-    return out
-
-
-def _tol(ref):
-    return 2e-3 * ref.abs().max().item() + 2e-3
-
-
 @pytest.mark.parametrize("new_order", [False, True])
 @pytest.mark.parametrize("T", [1, 15, 63, 64, 65, 1000, 4096, 16384])
 @pytest.mark.parametrize("heads", [1, 2, 5, 8])
 @pytest.mark.parametrize("D", [32, 64, 128])
 def test_unet_attention_vs_fp32(D, heads, T, new_order):
-    N = 3
-    g = torch.Generator(device="cuda").manual_seed(1000 * D + 10 * heads + T % 97)
-    qkv = (torch.randn(N, T, 3 * heads * D, device="cuda", generator=g) * 1.5).half()
-    out = _attn(qkv, N, T, heads, D, new_order)
-    ref = _attn_ref(qkv, N, T, heads, D, new_order)
-    torch.cuda.synchronize()
-    d = (out.float() - ref).abs()
-    assert not torch.isnan(out).any()
-    assert d.max().item() <= _tol(ref), (d.max().item(), _tol(ref))
+    """Per element against float64 on the fp16 operands (the bound of tests/test_gpu_attention.py)."""
+    from tests.test_gpu_attention import unet_case
+    unet_case("randn", 3, T, heads, D, new_order, seed=1000 * D + 10 * heads + T % 97)
 
 
 @pytest.mark.parametrize("D,heads,T", [(32, 5, 4096), (64, 2, 1000), (128, 1, 65)])
