@@ -276,6 +276,61 @@ int rs_op_tile_gather(const float* tiles, int N, int C, int H, int W, int th, in
 /* p_sample update (reference models/gaussian_diffusion.py:361-364 with :218-221) */
 int rs_p_sample(const float* x_t, const float* x0_pred, const float* noise, float* x_next, float coef1,
                 float coef2, float std, int t_is_zero, long long numel, void* stream);
+/* The step the sampler's loop launches: x_next = coef1[t] x_t + coef2[t] x0 + [t != 0] std[t] noise, all [N, C, HW]
+ * fp32, with the coefficients read from T-entry device tables at t.  With next_in (t > 0 only) it also writes
+ * fp16(x_next * in_scale[t - 1]) into channels [0, C) of the next denoiser input [N*HW][next_cpad] and leaves every other
+ * channel as it was; counters[0, n_counters) are zeroed (the next forward's GroupNorm arrival counters).  t outside
+ * [0, T), next_cpad < C and more counters than launched threads are refused. */
+typedef struct rs_p_sample_args {
+  const float* x_t; const float* x0; const float* noise; float* x_next;
+  const float* coef1; const float* coef2; const float* stdv; const float* in_scale;   /* [T] fp32 device tables */
+  int32_t T, t, N, C, HW;
+  void* next_in; int32_t next_cpad;             /* optional fp16 [N*HW][next_cpad]                                     */
+  uint32_t* counters; int32_t n_counters;       /* optional                                                             */
+} rs_p_sample_args;
+int rs_op_p_sample_ex(const rs_p_sample_args* a, void* stream);
+/* The denoiser's input packing: out[N*HW][Cpad] fp16 = cat([fp16(x * scale_tab[scale_idx]), lq, mask], channels) + zero
+ * padding (scale 1 without scale_tab).  lq is one of: lq_nchw [N, Cl, HW] fp32 (optionally followed by mask_nchw
+ * [N, 1, HW]); lq_nchw [N, Cl / 4, 2H, 2W] packed as pixel_unshuffle(lq, 2) (lq_unshuffle, W = the latent width); the
+ * feature extractor's fp16 output lq_nhwc [N*HW][lq_ld]; or none.  Refused: Cpad below the channels written, Cl % 4 != 0
+ * with unshuffle, a mask with unshuffle or lq_nhwc or without lq_nchw, lq_ld < Cl, scale_idx outside [0, scale_n), both
+ * LQ forms at once, and more counters than launched threads. */
+typedef struct rs_pack_input_args {
+  const float* x; int32_t Cx;                   /* [N, Cx, HW] fp32                                                    */
+  const float* scale_tab; int32_t scale_n, scale_idx;
+  const float* lq_nchw; int32_t Cl;
+  const float* mask_nchw;
+  const void* lq_nhwc; int32_t lq_ld;
+  void* out; int32_t Cpad;
+  int32_t N, HW;
+  int32_t lq_unshuffle, W;
+  uint32_t* counters; int32_t n_counters;
+} rs_pack_input_args;
+int rs_op_pack_input(const rs_pack_input_args* a, void* stream);
+/* The feature extractor's (and first stage's) input packing: out[N*HW][Cpad] fp16 = cat([a [N, Ca, HW], b [N, Cb, HW]])
+ * + zero padding; b may be NULL with Cb = 0. */
+int rs_op_pack_image(const float* a, int Ca, const float* b, int Cb, void* out, int Cpad, int N, int HW, void* stream);
+/* The timestep path of a bound denoiser plan for `rows` (1 .. max(batch, 64)) device fp32 timesteps: the sinusoid
+ * [rows, model_channels], time_embed.0 after SiLU [rows, 4 model_channels], time_embed.2 [rows, 4 model_channels] and the
+ * FiLM rows of every ResBlock [rows, film_rows] (the emb_layers.1 of all ResBlocks in parameter order), copied to
+ * whichever outputs are not NULL.  A sampler re-derives its FiLM table on its next run. */
+int rs_plan_embedding(rs_plan* p, const float* tsteps, int rows, float* sin_out, float* mid_out, float* vec_out,
+                      float* film_out, void* stream);
+/* host only: dst[5 T + 1] = the sampler's fp32 tables coef1, coef2, std, in_scale, timesteps (T each), then the prior
+ * coefficient kappa * sqrt_eta[T - 1] */
+int rs_sampler_tables(const rs_sampler* s, float* dst);
+/* host only: the same tables for a schedule without a plan (rs_sampler_create's arguments); what the per-step generic
+ * path of gaussian_diffusion.p_sample takes its coefficients from */
+int rs_schedule_tables(int steps, const double* sqrt_etas_host, double kappa, const int32_t* timestep_map_host, float* dst);
+/* quant_conv of the VQ-GAN encoder: y[n, co, hw] = b[co] + sum_ci w[co * w_ld + ci] x[n, ci, hw] (fp32 NCHW, fp16 w,
+ * fp32 accumulation); Cin <= 8 */
+int rs_op_pointwise_conv(const float* x, const void* w_f16, int w_ld, const float* b, int Cin, int Cout, int N, int HW,
+                         float* y, void* stream);
+/* quant_conv + posterior sample of the KL first stage (rs_kl_encode's last launch) on h [N, Cin, HW]: moments
+ * [N, 2E, HW], z [N, E, HW] = mean + exp(0.5 clamp(logvar, -30, 20)) * noise, or mean without noise.  Cin <= 16 and
+ * 2E <= 16. */
+int rs_op_kl_posterior(const float* h, const void* w_f16, int w_ld, const float* b, int Cin, int E, const float* noise,
+                       float* z, float* moments, int N, int HW, void* stream);
 
 /* conv / linear on NHWC fp16 views (reference nn.Conv2d / nn.Linear call sites, see csrc/conv_gemm.cuh).
  * x [N,H,W,C] with row stride ld; w_packed fp16 [Cout][k*k][Ipad] from rs_op_pack_conv_weight; optional

@@ -95,6 +95,26 @@ class GnArgsC(C.Structure):
     ]
 
 
+class PSampleArgsC(C.Structure):
+    """Mirror of ``rs_p_sample_args``."""
+    _fields_ = [
+        ("x_t", C.c_void_p), ("x0", C.c_void_p), ("noise", C.c_void_p), ("x_next", C.c_void_p),
+        ("coef1", C.c_void_p), ("coef2", C.c_void_p), ("stdv", C.c_void_p), ("in_scale", C.c_void_p),
+        ("T", C.c_int32), ("t", C.c_int32), ("N", C.c_int32), ("C", C.c_int32), ("HW", C.c_int32),
+        ("next_in", C.c_void_p), ("next_cpad", C.c_int32), ("counters", C.c_void_p), ("n_counters", C.c_int32),
+    ]
+
+
+class PackInputArgsC(C.Structure):
+    """Mirror of ``rs_pack_input_args``."""
+    _fields_ = [
+        ("x", C.c_void_p), ("Cx", C.c_int32), ("scale_tab", C.c_void_p), ("scale_n", C.c_int32), ("scale_idx", C.c_int32),
+        ("lq_nchw", C.c_void_p), ("Cl", C.c_int32), ("mask_nchw", C.c_void_p), ("lq_nhwc", C.c_void_p), ("lq_ld", C.c_int32),
+        ("out", C.c_void_p), ("Cpad", C.c_int32), ("N", C.c_int32), ("HW", C.c_int32), ("lq_unshuffle", C.c_int32),
+        ("W", C.c_int32), ("counters", C.c_void_p), ("n_counters", C.c_int32),
+    ]
+
+
 # every symbol include/resshift_b200.h declares: (restype, argtypes)
 _P = C.c_void_p
 _SIGNATURES = {
@@ -127,6 +147,14 @@ _SIGNATURES = {
     "rs_sampler_staging_bytes": (C.c_size_t, [_P]),
     "rs_sampler_set_taps": (C.c_int, [_P, _P, _P]),
     "rs_p_sample": (C.c_int, [_P, _P, _P, _P, C.c_float, C.c_float, C.c_float, C.c_int, C.c_longlong, _P]),
+    "rs_op_p_sample_ex": (C.c_int, [C.POINTER(PSampleArgsC), _P]),
+    "rs_op_pack_input": (C.c_int, [C.POINTER(PackInputArgsC), _P]),
+    "rs_op_pack_image": (C.c_int, [_P, C.c_int, _P, C.c_int, _P, C.c_int, C.c_int, C.c_int, _P]),
+    "rs_plan_embedding": (C.c_int, [_P, _P, C.c_int, _P, _P, _P, _P, _P]),
+    "rs_sampler_tables": (C.c_int, [_P, C.POINTER(C.c_float)]),
+    "rs_schedule_tables": (C.c_int, [C.c_int, C.POINTER(C.c_double), C.c_double, C.POINTER(C.c_int32), C.POINTER(C.c_float)]),
+    "rs_op_pointwise_conv": (C.c_int, [_P, _P, C.c_int, _P, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P]),
+    "rs_op_kl_posterior": (C.c_int, [_P, _P, C.c_int, _P, C.c_int, C.c_int, _P, _P, _P, C.c_int, C.c_int, _P]),
     "rs_op_pack_conv_weight": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P]),
     "rs_op_conv2d": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, C.c_int, _P, C.c_int, C.c_int,
                                C.c_int, _P, C.c_int, _P, C.c_int, _P, C.c_int, C.c_int, _P]),

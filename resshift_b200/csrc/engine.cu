@@ -1734,29 +1734,73 @@ int sampler_prepare(rs_sampler& S, cudaStream_t st) {
 
 extern "C" {
 
+// posterior tables in float64, cast to fp32 like _extract_into_tensor (reference models/gaussian_diffusion.py:92-105,143-161)
+static void schedule_tables(rs_sampler& s, int steps, const double* sqrt_etas, double kappa, const int32_t* tmap) {
+  std::vector<double> etas(steps), prev(steps), alpha(steps), pv(steps);
+  for (int i = 0; i < steps; ++i) etas[i] = sqrt_etas[i] * sqrt_etas[i];
+  for (int i = 0; i < steps; ++i) { prev[i] = i ? etas[i - 1] : 0.0; alpha[i] = etas[i] - prev[i]; pv[i] = kappa * kappa * prev[i] / etas[i] * alpha[i]; }
+  s.T = steps; s.kappa = kappa;
+  s.coef1.resize(steps); s.coef2.resize(steps); s.stdv.resize(steps); s.in_scale.resize(steps); s.tsteps.resize(steps);
+  for (int i = 0; i < steps; ++i) {
+    const double pvc = pv[i == 0 ? 1 : i];
+    s.coef1[i] = (float)(prev[i] / etas[i]);
+    s.coef2[i] = (float)(alpha[i] / etas[i]);
+    const float logv = (float)std::log(pvc);
+    s.stdv[i] = std::exp(0.5f * logv);
+    const float e32 = (float)etas[i];
+    s.in_scale[i] = 1.0f / std::sqrt(e32 * (float)(kappa * kappa) + 1.0f);
+    s.tsteps[i] = (float)(tmap ? tmap[i] : i);
+  }
+  s.prior_coef = (float)(kappa * sqrt_etas[steps - 1]);
+}
+
+static void copy_tables(const rs_sampler& s, float* dst) {
+  for (const std::vector<float>* v : {&s.coef1, &s.coef2, &s.stdv, &s.in_scale, &s.tsteps}) {
+    std::memcpy(dst, v->data(), (size_t)s.T * sizeof(float));
+    dst += s.T;
+  }
+  *dst = s.prior_coef;
+}
+
 int rs_sampler_create(rs_plan* p, int steps, const double* sqrt_etas, double kappa, const int32_t* tmap, rs_sampler** out) {
   RS_CHECK(p && p->bound && sqrt_etas && out, "bad argument (plan must be bound)");
   RS_CHECK(p->pass == Pass::Denoiser, std::string("samplers are built on denoiser plans: this plan belongs to ") + kind_name(p->e->kind));
   RS_CHECK(steps >= 2 && steps <= p->max_rows && steps <= 1024, "steps out of range for this plan");
   auto s = std::make_unique<rs_sampler>();
-  s->p = p; s->T = steps; s->kappa = kappa;
-  // posterior tables in float64, cast to fp32 like _extract_into_tensor (reference models/gaussian_diffusion.py:92-105,143-161)
-  std::vector<double> etas(steps), prev(steps), alpha(steps), pv(steps);
-  for (int i = 0; i < steps; ++i) etas[i] = sqrt_etas[i] * sqrt_etas[i];
-  for (int i = 0; i < steps; ++i) { prev[i] = i ? etas[i - 1] : 0.0; alpha[i] = etas[i] - prev[i]; pv[i] = kappa * kappa * prev[i] / etas[i] * alpha[i]; }
-  s->coef1.resize(steps); s->coef2.resize(steps); s->stdv.resize(steps); s->in_scale.resize(steps); s->tsteps.resize(steps);
-  for (int i = 0; i < steps; ++i) {
-    const double pvc = pv[i == 0 ? 1 : i];
-    s->coef1[i] = (float)(prev[i] / etas[i]);
-    s->coef2[i] = (float)(alpha[i] / etas[i]);
-    const float logv = (float)std::log(pvc);
-    s->stdv[i] = std::exp(0.5f * logv);
-    const float e32 = (float)etas[i];
-    s->in_scale[i] = 1.0f / std::sqrt(e32 * (float)(kappa * kappa) + 1.0f);
-    s->tsteps[i] = (float)(tmap ? tmap[i] : i);
-  }
-  s->prior_coef = (float)(kappa * sqrt_etas[steps - 1]);
+  s->p = p;
+  schedule_tables(*s, steps, sqrt_etas, kappa, tmap);
   *out = s.release();
+  return 0;
+}
+int rs_sampler_tables(const rs_sampler* s, float* dst) {
+  RS_CHECK(s && dst, "null argument");
+  copy_tables(*s, dst);
+  return 0;
+}
+int rs_plan_embedding(rs_plan* p, const float* tsteps, int rows, float* sin_out, float* mid_out, float* vec_out,
+                      float* film_out, void* stream) {
+  RS_CHECK(p && p->bound && tsteps, "bad argument (plan must be bound)");
+  RS_CHECK(p->pass == Pass::Denoiser, std::string("not a denoiser plan: this plan belongs to ") + kind_name(p->e->kind));
+  RS_CHECK(rows >= 1 && rows <= p->max_rows, "rows must be in [1, " + std::to_string(p->max_rows) + "], got " + std::to_string(rows));
+  int rc = check_plan_device(*p); if (rc) return rc;
+  rs_plan& P = *p;
+  const rs_engine& E = *P.e;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  P.table_owner = nullptr;                       // the FiLM rows a sampler keeps are overwritten
+  rc = run_embedding(P, tsteps, rows, st); if (rc) return rc;
+  const size_t K = (size_t)E.time_dim();
+  const struct { float* dst; size_t off, width; } outs[4] = {
+      {sin_out, P.off_emb_sin, (size_t)E.cfg.model_channels}, {mid_out, P.off_emb_mid, K}, {vec_out, P.off_emb_vec, K},
+      {film_out, P.off_film, (size_t)E.film_rows}};
+  for (const auto& o : outs)
+    if (o.dst) RS_CUDA_OK(cudaMemcpyAsync(o.dst, P.ws + o.off, (size_t)rows * o.width * sizeof(float), cudaMemcpyDeviceToDevice, st));
+  return 0;
+}
+int rs_schedule_tables(int steps, const double* sqrt_etas, double kappa, const int32_t* tmap, float* dst) {
+  RS_CHECK(sqrt_etas && dst && steps >= 1, "bad argument");
+  rs_sampler s;
+  schedule_tables(s, steps, sqrt_etas, kappa, tmap);
+  copy_tables(s, dst);
   return 0;
 }
 void rs_sampler_destroy(rs_sampler* s) {

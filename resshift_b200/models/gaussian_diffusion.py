@@ -154,6 +154,20 @@ class ResShiftDiffusion:
         return out.type(data_dtype) if model_dtype != data_dtype else out
 
     # ------------------------------------------------------------------ one step (generic model callable)
+    def step_tables(self):
+        """The fp32 tables of every step (coef1, coef2, std, in_scale, timesteps) and the prior coefficient, computed by
+        the library exactly as its sampler computes them (rs_schedule_tables), so that both paths step with the same
+        bits."""
+        if getattr(self, "_step_tables", None) is None:
+            T = self.num_timesteps
+            dst = (C.c_float * (5 * T + 1))()
+            _lib.check(_lib.lib.rs_schedule_tables(T, (C.c_double * T)(*self.sqrt_etas.tolist()), float(self.kappa),
+                                                   (C.c_int32 * T)(*self.timestep_map), dst))
+            a = np.frombuffer(dst, dtype=np.float32).copy()
+            self._step_tables = {k: a[j * T:(j + 1) * T] for j, k in enumerate(("coef1", "coef2", "std", "in_scale", "tsteps"))}
+            self._step_tables["prior_coef"] = a[5 * T]
+        return self._step_tables
+
     def _model_t(self, t):
         m = torch.tensor(self.timestep_map, device=t.device, dtype=t.dtype)   # reference models/respace.py:60-63
         return m[t]
@@ -196,9 +210,8 @@ class ResShiftDiffusion:
         pred = out["pred_xstart"].float().contiguous()
         nz = noise.float().contiguous()
         sample = torch.empty_like(xf)
-        c1 = float(np.float32(self.posterior_mean_coef1[i]))
-        c2 = float(np.float32(self.posterior_mean_coef2[i]))
-        sd = float(np.exp(np.float32(0.5) * np.float32(self.posterior_log_variance_clipped[i])))
+        tabs = self.step_tables()
+        c1, c2, sd = (float(tabs[k][i]) for k in ("coef1", "coef2", "std"))
         _lib.check(_lib.lib.rs_p_sample(xf.data_ptr(), pred.data_ptr(), nz.data_ptr(), sample.data_ptr(), c1, c2, sd,
                                         int(i == 0), xf.numel(), _lib.current_stream()))
         return {"sample": sample, "pred_xstart": out["pred_xstart"], "mean": out["mean"]}
