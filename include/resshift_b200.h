@@ -180,6 +180,22 @@ int rs_plan_probe(rs_plan* p, const char* block, float* dst, int32_t* channels, 
  *      p_sample :332-365, _scale_input :598-603, prior_sample :517-529; models/respace.py:43-63) ------ */
 int rs_sampler_create(rs_plan* p, int steps, const double* sqrt_etas_host, double kappa,
                       const int32_t* timestep_map_host, rs_sampler** out);
+/* What the denoiser predicts (create_gaussian_diffusion's predict_type, reference models/script_util.py:35-44) and
+ * how its input is scaled (_scale_input, models/gaussian_diffusion.py:598-609).  The step turns the model output into
+ * x0 (p_mean_variance :277-292): xstart x0 = out; residual x0 = z_y - out; epsilon x0 = (x_t - sqrt_eta kappa out -
+ * eta z_y) / (1 - eta); epsilon_scale x0 = (x_t - out - eta z_y) / (1 - eta). */
+typedef enum rs_mean_type {
+  RS_MEAN_XSTART = 0, RS_MEAN_EPSILON = 1, RS_MEAN_EPSILON_SCALE = 2, RS_MEAN_RESIDUAL = 3
+} rs_mean_type;
+typedef struct rs_sampler_options {
+  int32_t mean_type;          /* rs_mean_type */
+  int32_t normalize_input;    /* 0: the denoiser sees x_t unscaled */
+  int32_t latent_flag;        /* 1: x_t / sqrt(eta kappa^2 + 1); 0: x_t / (sqrt_eta kappa 3 + 1) */
+} rs_sampler_options;
+/* rs_sampler_create is rs_sampler_create_ex with {RS_MEAN_XSTART, 1, 1}.  Unknown mean types and flags other than 0 / 1
+ * are refused. */
+int rs_sampler_create_ex(rs_plan* p, int steps, const double* sqrt_etas_host, double kappa,
+                         const int32_t* timestep_map_host, const rs_sampler_options* options, rs_sampler** out);
 void rs_sampler_destroy(rs_sampler* s);
 /* z_y [B, C, H, W] fp32; noises [(T+1), B, C, H, W] fp32 in the reference's draw order (prior first);
  * lq/mask as in rs_plan_forward; out_latent [B, C, H, W] fp32 (the loop's final `sample`).
@@ -192,7 +208,8 @@ int rs_sampler_run_host(rs_sampler* s, const float* z_y_host, const float* noise
                         const float* mask_host, float* out_latent_host, void* staging_dev, size_t staging_bytes,
                         int use_graph, void* stream);
 size_t rs_sampler_staging_bytes(const rs_sampler* s);
-/* optional taps for parity tests: per-step pred_xstart / sample, [T, B, C, H, W] fp32 device buffers or NULL */
+/* optional taps for parity tests: per-step pred_xstart (the converted x0 whatever the mean type) / sample,
+ * [T, B, C, H, W] fp32 device buffers or NULL */
 int rs_sampler_set_taps(rs_sampler* s, float* pred_xstart_steps, float* sample_steps);
 
 /* ---- VQ-GAN first stage: ldm.models.autoencoder.VQModelTorch (reference ldm/models/autoencoder.py:12-47) -------
@@ -289,6 +306,21 @@ typedef struct rs_p_sample_args {
   uint32_t* counters; int32_t n_counters;       /* optional                                                             */
 } rs_p_sample_args;
 int rs_op_p_sample_ex(const rs_p_sample_args* a, void* stream);
+/* The same step from the raw model output of a mean type (rs_sampler_options): x0 is converted in registers in the
+ * reference's operation order, every operation rounded in fp32 (eps_coef = fp32(sqrt_eta) * kappa, eta, one_minus_eta
+ * = fp32(1 - eta): rs_schedule_tables_ex's rows), then stepped as rs_op_p_sample_ex does (no counters).  x0_out
+ * (optional) receives x0.  Refused: an unknown mean type, y or a conversion table missing for a type that reads it, t
+ * outside [0, T), next_cpad < C. */
+typedef struct rs_p_sample_pred_args {
+  const float* out; const float* x_t; const float* y; const float* noise; float* x_next;   /* [N, C, HW] fp32       */
+  const float* coef1; const float* coef2; const float* stdv; const float* in_scale;          /* [T] fp32 device tables */
+  const float* eps_coef; const float* eta; const float* one_minus_eta;                       /* [T] fp32 device tables */
+  int32_t T, t, N, C, HW;
+  int32_t mean_type;
+  void* next_in; int32_t next_cpad;             /* optional fp16 [N*HW][next_cpad]                                     */
+  float* x0_out;                                /* optional [N, C, HW] fp32                                            */
+} rs_p_sample_pred_args;
+int rs_op_p_sample_pred(const rs_p_sample_pred_args* a, void* stream);
 /* The denoiser's input packing: out[N*HW][Cpad] fp16 = cat([fp16(x * scale_tab[scale_idx]), lq, mask], channels) + zero
  * padding (scale 1 without scale_tab).  lq is one of: lq_nchw [N, Cl, HW] fp32 (optionally followed by mask_nchw
  * [N, 1, HW]); lq_nchw [N, Cl / 4, 2H, 2W] packed as pixel_unshuffle(lq, 2) (lq_unshuffle, W = the latent width); the
@@ -322,6 +354,10 @@ int rs_sampler_tables(const rs_sampler* s, float* dst);
 /* host only: the same tables for a schedule without a plan (rs_sampler_create's arguments); what the per-step generic
  * path of gaussian_diffusion.p_sample takes its coefficients from */
 int rs_schedule_tables(int steps, const double* sqrt_etas_host, double kappa, const int32_t* timestep_map_host, float* dst);
+/* host only: dst[8 T + 1] = rs_schedule_tables' 5 T + 1 values for a sampler built with `options` (in_scale follows its
+ * input scaling), then the conversion rows eps_coef, eta, one_minus_eta (T each) */
+int rs_schedule_tables_ex(int steps, const double* sqrt_etas_host, double kappa, const int32_t* timestep_map_host,
+                          const rs_sampler_options* options, float* dst);
 /* quant_conv of the VQ-GAN encoder: y[n, co, hw] = b[co] + sum_ci w[co * w_ld + ci] x[n, ci, hw] (fp32 NCHW, fp16 w,
  * fp32 accumulation); Cin <= 8 */
 int rs_op_pointwise_conv(const float* x, const void* w_f16, int w_ld, const float* b, int Cin, int Cout, int N, int HW,

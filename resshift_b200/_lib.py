@@ -105,6 +105,26 @@ class PSampleArgsC(C.Structure):
     ]
 
 
+class PSamplePredArgsC(C.Structure):
+    """Mirror of ``rs_p_sample_pred_args``."""
+    _fields_ = [
+        ("out", C.c_void_p), ("x_t", C.c_void_p), ("y", C.c_void_p), ("noise", C.c_void_p), ("x_next", C.c_void_p),
+        ("coef1", C.c_void_p), ("coef2", C.c_void_p), ("stdv", C.c_void_p), ("in_scale", C.c_void_p),
+        ("eps_coef", C.c_void_p), ("eta", C.c_void_p), ("one_minus_eta", C.c_void_p),
+        ("T", C.c_int32), ("t", C.c_int32), ("N", C.c_int32), ("C", C.c_int32), ("HW", C.c_int32),
+        ("mean_type", C.c_int32), ("next_in", C.c_void_p), ("next_cpad", C.c_int32), ("x0_out", C.c_void_p),
+    ]
+
+
+class SamplerOptionsC(C.Structure):
+    """Mirror of ``rs_sampler_options``."""
+    _fields_ = [("mean_type", C.c_int32), ("normalize_input", C.c_int32), ("latent_flag", C.c_int32)]
+
+
+# rs_mean_type, by the reference's predict_type names (models/script_util.py:35-44)
+MEAN_TYPES = {"xstart": 0, "epsilon": 1, "epsilon_scale": 2, "residual": 3}
+
+
 class PackInputArgsC(C.Structure):
     """Mirror of ``rs_pack_input_args``."""
     _fields_ = [
@@ -141,6 +161,8 @@ _SIGNATURES = {
     "rs_plan_profile_ops": (C.c_int, [_P, _P, _P, _P, _P, C.POINTER(C.c_double), C.c_char_p, C.c_int, C.c_int, C.POINTER(C.c_int32), _P]),
     "rs_plan_probe": (C.c_int, [_P, C.c_char_p, _P, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(C.c_int32), _P]),
     "rs_sampler_create": (C.c_int, [_P, C.c_int, C.POINTER(C.c_double), C.c_double, C.POINTER(C.c_int32), C.POINTER(_P)]),
+    "rs_sampler_create_ex": (C.c_int, [_P, C.c_int, C.POINTER(C.c_double), C.c_double, C.POINTER(C.c_int32),
+                                       C.POINTER(SamplerOptionsC), C.POINTER(_P)]),
     "rs_sampler_destroy": (None, [_P]),
     "rs_sampler_run": (C.c_int, [_P, _P, _P, _P, _P, _P, C.c_int, _P]),
     "rs_sampler_run_host": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, C.c_size_t, C.c_int, _P]),
@@ -148,11 +170,14 @@ _SIGNATURES = {
     "rs_sampler_set_taps": (C.c_int, [_P, _P, _P]),
     "rs_p_sample": (C.c_int, [_P, _P, _P, _P, C.c_float, C.c_float, C.c_float, C.c_int, C.c_longlong, _P]),
     "rs_op_p_sample_ex": (C.c_int, [C.POINTER(PSampleArgsC), _P]),
+    "rs_op_p_sample_pred": (C.c_int, [C.POINTER(PSamplePredArgsC), _P]),
     "rs_op_pack_input": (C.c_int, [C.POINTER(PackInputArgsC), _P]),
     "rs_op_pack_image": (C.c_int, [_P, C.c_int, _P, C.c_int, _P, C.c_int, C.c_int, C.c_int, _P]),
     "rs_plan_embedding": (C.c_int, [_P, _P, C.c_int, _P, _P, _P, _P, _P]),
     "rs_sampler_tables": (C.c_int, [_P, C.POINTER(C.c_float)]),
     "rs_schedule_tables": (C.c_int, [C.c_int, C.POINTER(C.c_double), C.c_double, C.POINTER(C.c_int32), C.POINTER(C.c_float)]),
+    "rs_schedule_tables_ex": (C.c_int, [C.c_int, C.POINTER(C.c_double), C.c_double, C.POINTER(C.c_int32),
+                                        C.POINTER(SamplerOptionsC), C.POINTER(C.c_float)]),
     "rs_op_pointwise_conv": (C.c_int, [_P, _P, C.c_int, _P, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P]),
     "rs_op_kl_posterior": (C.c_int, [_P, _P, C.c_int, _P, C.c_int, C.c_int, _P, _P, _P, C.c_int, C.c_int, _P]),
     "rs_op_pack_conv_weight": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P]),

@@ -2,6 +2,8 @@
 // embedding MLP, the residual-shift sampling update, and weight repacking.
 #pragma once
 
+#include <type_traits>
+
 #include "common.cuh"
 #include "gn_stats.cuh"
 
@@ -198,10 +200,20 @@ __global__ void linear_small_kernel(const float* __restrict__ x, const __half* _
 //     x_{t-1} = coef1[t] * x_t + coef2[t] * x0_pred + [t != 0] * std[t] * noise
 // fp32 NCHW in/out.  When `next_in` is set it also emits the NEXT denoiser input
 // cat([x_{t-1} * in_scale[t-1], lq]) as NHWC fp16 (fusing _scale_input + th.cat + layout change).
+// x0_pred comes from the model output by the parameterisation MT (reference p_mean_variance :277-292 and
+// _predict_xstart_from_* :308-324), in registers, op by op in the reference's order with no FMA contraction:
+//     xstart        x0 = out
+//     residual      x0 = y - out
+//     epsilon       x0 = ((x_t - eps_coef[t] * out) - eta[t] * y) / one_minus_eta[t]
+//     epsilon_scale x0 = ((x_t - out) - eta[t] * y) / one_minus_eta[t]
+// with eps_coef = fp32(fp32(sqrt_eta) * kappa), eta = fp32(eta), one_minus_eta = fp32(1 - eta) (_extract_into_tensor
+// tables), so x0 is bit for bit the reference's fp32 expression.
 // ------------------------------------------------------------------------------------------------
+enum MeanType : int { kMeanXstart = 0, kMeanEpsilon = 1, kMeanEpsilonScale = 2, kMeanResidual = 3 };
+
 struct PSampleParams {
   const float* x_t;       // [N, C, HW]
-  const float* x0;        // [N, C, HW]
+  const float* x0;        // [N, C, HW]: the model output (x0 itself for xstart)
   const float* noise;     // [N, C, HW]
   float* x_next;          // [N, C, HW]
   const float* coef1; const float* coef2; const float* stdv; const float* in_scale;   // [T] fp32 tables
@@ -210,7 +222,31 @@ struct PSampleParams {
   __half* next_in; int next_cpad;     // optional: [N*HW, next_cpad]; channels [0, C) are written here
   unsigned int* zero_ptr; int zero_n; // GroupNorm arrival counters of the NEXT denoiser forward: reset here
 };
-__global__ void p_sample_kernel(const PSampleParams p) {
+// what the converting instances read besides (the xstart instance keeps the plain struct, and with it its code)
+struct PSamplePredParams : PSampleParams {
+  const float* y;                     // [N, C, HW] z_y
+  const float* eps_coef; const float* eta; const float* one_minus_eta;   // [T] fp32 tables of the conversions
+  float* x0_out;                      // optional [N, C, HW]: the converted x0
+};
+template <int MT>
+using PSampleParamsOf = std::conditional_t<MT == kMeanXstart, PSampleParams, PSamplePredParams>;
+
+template <int MT>
+__device__ __forceinline__ float predict_xstart(const PSamplePredParams& p, long long i, float xt) {
+  if constexpr (MT == kMeanResidual) {
+    return __fsub_rn(p.y[i], p.x0[i]);
+  } else if constexpr (MT == kMeanEpsilon) {
+    const float num = __fsub_rn(__fsub_rn(xt, __fmul_rn(p.eps_coef[p.t], p.x0[i])), __fmul_rn(p.eta[p.t], p.y[i]));
+    return __fdiv_rn(num, p.one_minus_eta[p.t]);
+  } else {
+    static_assert(MT == kMeanEpsilonScale, "unknown mean type");
+    const float num = __fsub_rn(__fsub_rn(xt, p.x0[i]), __fmul_rn(p.eta[p.t], p.y[i]));
+    return __fdiv_rn(num, p.one_minus_eta[p.t]);
+  }
+}
+
+template <int MT>
+__global__ void p_sample_kernel(const PSampleParamsOf<MT> p) {
   pdl_trigger();
   pdl_wait();
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -219,7 +255,15 @@ __global__ void p_sample_kernel(const PSampleParams p) {
   if (i >= total) return;
   const float c1 = p.coef1[p.t], c2 = p.coef2[p.t];
   const float sd = p.t != 0 ? p.stdv[p.t] : 0.f;
-  float v = c1 * p.x_t[i] + c2 * p.x0[i];
+  float v;
+  if constexpr (MT == kMeanXstart) {
+    v = c1 * p.x_t[i] + c2 * p.x0[i];
+  } else {
+    const float xt = p.x_t[i];
+    const float x0 = predict_xstart<MT>(p, i, xt);
+    if (p.x0_out) p.x0_out[i] = x0;
+    v = c1 * xt + c2 * x0;
+  }
   if (p.t != 0) v += sd * p.noise[i];
   p.x_next[i] = v;
   if (p.next_in && p.t > 0) {

@@ -812,7 +812,7 @@ int finish_layout(rs_plan& P, Builder& b, size_t state_bytes, bool unet) {
   size_t off = 0;
   auto region = [&](size_t bytes) { size_t o = off; off = align_up(off + bytes, 256); return o; };
   if (unet) {
-    P.off_tables = region(4 * 1024 * sizeof(float));                   // coef1, coef2, std, in_scale (<= 1024 steps)
+    P.off_tables = region(7 * 1024 * sizeof(float));   // coef1, coef2, std, in_scale, eps_coef, eta, 1 - eta (<= 1024 steps)
     P.off_tsteps = region((size_t)P.max_rows * sizeof(float));
     P.off_emb_sin = region((size_t)P.max_rows * c.model_channels * sizeof(float));
     P.off_emb_mid = region((size_t)P.max_rows * E.time_dim() * sizeof(float));
@@ -1668,7 +1668,9 @@ struct rs_sampler {
   int T = 0;
   double kappa = 0;
   std::vector<float> coef1, coef2, stdv, in_scale, tsteps;
+  std::vector<float> eps_coef, eta, one_minus_eta;     // x0 conversions of the epsilon parameterisations
   float prior_coef = 0;
+  rs_sampler_options opt{RS_MEAN_XSTART, 1, 1};
   float* tap_pred = nullptr; float* tap_sample = nullptr;
   cudaGraphExec_t graph = nullptr;
   cudaStream_t cap_stream = nullptr;     // capture happens on a private stream (the legacy default stream cannot capture)
@@ -1678,16 +1680,34 @@ struct rs_sampler {
 
 namespace {
 
+static_assert((int)kMeanXstart == (int)RS_MEAN_XSTART && (int)kMeanEpsilon == (int)RS_MEAN_EPSILON &&
+              (int)kMeanEpsilonScale == (int)RS_MEAN_EPSILON_SCALE && (int)kMeanResidual == (int)RS_MEAN_RESIDUAL,
+              "MeanType mirrors rs_mean_type");
+
+// p_sample_kernel instance of a mean type (rs_sampler_options::mean_type); unknown types are refused
+int launch_p_sample(int mean_type, const PSamplePredParams& pp, long long numel, cudaStream_t st) {
+  const dim3 grid((unsigned)((numel + 255) / 256)), block(256);
+  switch (mean_type) {
+    case RS_MEAN_XSTART: (void)launch_k(p_sample_kernel<kMeanXstart>, grid, block, (size_t)(0), st, PSampleParams(pp)); break;
+    case RS_MEAN_EPSILON: (void)launch_k(p_sample_kernel<kMeanEpsilon>, grid, block, (size_t)(0), st, pp); break;
+    case RS_MEAN_EPSILON_SCALE: (void)launch_k(p_sample_kernel<kMeanEpsilonScale>, grid, block, (size_t)(0), st, pp); break;
+    case RS_MEAN_RESIDUAL: (void)launch_k(p_sample_kernel<kMeanResidual>, grid, block, (size_t)(0), st, pp); break;
+    default: RS_CHECK(false, "unknown mean type " + std::to_string(mean_type) + " (RS_MEAN_XSTART .. RS_MEAN_RESIDUAL)");
+  }
+  return 0;
+}
+
 int sampler_enqueue(rs_sampler& S, const float* z_y, const float* noises, const float* lq, const float* mask,
                     float* out_latent, cudaStream_t st) {
   rs_plan& P = *S.p;
   const rs_unet_config& c = P.e->cfg;
-  RS_CHECK(c.in_channels == c.out_channels, "predict_type xstart needs out_channels == in_channels");
+  RS_CHECK(c.in_channels == c.out_channels, "the sampler needs out_channels == in_channels (x0, x_t and z_y share a shape)");
   const long long numel = (long long)P.B * c.in_channels * P.H * P.W;
   const size_t lat = align_up((size_t)numel * 4, 256);
   float* x_t = reinterpret_cast<float*>(P.ws + P.off_state);
   float* tab = reinterpret_cast<float*>(P.ws + P.off_tables);
   const float* coef1 = tab, *coef2 = tab + 1024, *stdv = tab + 2048, *in_scale = tab + 3072;
+  const bool xstart = S.opt.mean_type == RS_MEAN_XSTART;
   (void)lat;
   // x_T = z_y + kappa * sqrt_eta_T * noise_0   (prior_sample)
   (void)launch_k(prior_sample_kernel, dim3((unsigned)((numel + 255) / 256)), dim3(256), (size_t)(0), st, z_y, noises, x_t, S.prior_coef, numel);
@@ -1697,15 +1717,18 @@ int sampler_enqueue(rs_sampler& S, const float* z_y, const float* noises, const 
   for (int k = 0; k < S.T; ++k) {
     const int t = S.T - 1 - k;
     rc = run_ops(P, P.ops, film_all + (long long)t * P.e->film_rows, 0, st); if (rc) return rc;
-    PSampleParams pp{};
+    PSamplePredParams pp{};
     pp.x_t = x_t; pp.x0 = P.out_f32; pp.noise = noises + (long long)(k + 1) * numel;
     pp.x_next = (t == 0) ? out_latent : x_t;
     pp.coef1 = coef1; pp.coef2 = coef2; pp.stdv = stdv; pp.in_scale = in_scale; pp.t = t;
     pp.N = P.B; pp.C = c.in_channels; pp.HW = P.H * P.W;
     pp.next_in = P.xin.ptr; pp.next_cpad = P.cin_pad;
     pp.zero_ptr = reinterpret_cast<unsigned int*>(P.ws + P.off_counters); pp.zero_n = P.n_gn * P.B;
-    if (S.tap_pred) RS_CUDA_OK(cudaMemcpyAsync(S.tap_pred + (long long)k * numel, P.out_f32, numel * 4, cudaMemcpyDeviceToDevice, st));
-    (void)launch_k(p_sample_kernel, dim3((unsigned)((numel + 255) / 256)), dim3(256), (size_t)(0), st, pp);
+    pp.y = z_y; pp.eps_coef = tab + 4096; pp.eta = tab + 5120; pp.one_minus_eta = tab + 6144;
+    // the pred_xstart tap: the head output itself for xstart, the step kernel's converted x0 otherwise
+    if (S.tap_pred && xstart) RS_CUDA_OK(cudaMemcpyAsync(S.tap_pred + (long long)k * numel, P.out_f32, numel * 4, cudaMemcpyDeviceToDevice, st));
+    if (S.tap_pred && !xstart) pp.x0_out = S.tap_pred + (long long)k * numel;
+    rc = launch_p_sample(S.opt.mean_type, pp, numel, st); if (rc) return rc;
     if (S.tap_sample) RS_CUDA_OK(cudaMemcpyAsync(S.tap_sample + (long long)k * numel, pp.x_next, numel * 4, cudaMemcpyDeviceToDevice, st));
   }
   RS_CUDA_OK(cudaGetLastError());
@@ -1722,6 +1745,11 @@ int sampler_prepare(rs_sampler& S, cudaStream_t st) {
   RS_CUDA_OK(cudaMemcpyAsync(tab + 1024, S.coef2.data(), S.T * 4, cudaMemcpyHostToDevice, st));
   RS_CUDA_OK(cudaMemcpyAsync(tab + 2048, S.stdv.data(), S.T * 4, cudaMemcpyHostToDevice, st));
   RS_CUDA_OK(cudaMemcpyAsync(tab + 3072, S.in_scale.data(), S.T * 4, cudaMemcpyHostToDevice, st));
+  if (S.opt.mean_type != RS_MEAN_XSTART) {
+    RS_CUDA_OK(cudaMemcpyAsync(tab + 4096, S.eps_coef.data(), S.T * 4, cudaMemcpyHostToDevice, st));
+    RS_CUDA_OK(cudaMemcpyAsync(tab + 5120, S.eta.data(), S.T * 4, cudaMemcpyHostToDevice, st));
+    RS_CUDA_OK(cudaMemcpyAsync(tab + 6144, S.one_minus_eta.data(), S.T * 4, cudaMemcpyHostToDevice, st));
+  }
   float* ts = reinterpret_cast<float*>(P.ws + P.off_tsteps);
   RS_CUDA_OK(cudaMemcpyAsync(ts, S.tsteps.data(), S.T * 4, cudaMemcpyHostToDevice, st));
   int rc = run_embedding(P, ts, S.T, st); if (rc) return rc;
@@ -1735,12 +1763,17 @@ int sampler_prepare(rs_sampler& S, cudaStream_t st) {
 extern "C" {
 
 // posterior tables in float64, cast to fp32 like _extract_into_tensor (reference models/gaussian_diffusion.py:92-105,143-161)
-static void schedule_tables(rs_sampler& s, int steps, const double* sqrt_etas, double kappa, const int32_t* tmap) {
+// in_scale follows _scale_input (:598-609): 1 / sqrt(eta kappa^2 + 1) with latent_flag, 1 / (sqrt_eta kappa 3 + 1)
+// without, 1 without normalize_input; every operation of the reference's fp32 expression rounded in fp32 on its fp32
+// table value.  eps_coef, eta and one_minus_eta are the fp32 factors of _predict_xstart_from_eps / _eps_scale (:308-318).
+static void schedule_tables(rs_sampler& s, int steps, const double* sqrt_etas, double kappa, const int32_t* tmap,
+                            const rs_sampler_options& opt = rs_sampler_options{RS_MEAN_XSTART, 1, 1}) {
   std::vector<double> etas(steps), prev(steps), alpha(steps), pv(steps);
   for (int i = 0; i < steps; ++i) etas[i] = sqrt_etas[i] * sqrt_etas[i];
   for (int i = 0; i < steps; ++i) { prev[i] = i ? etas[i - 1] : 0.0; alpha[i] = etas[i] - prev[i]; pv[i] = kappa * kappa * prev[i] / etas[i] * alpha[i]; }
-  s.T = steps; s.kappa = kappa;
+  s.T = steps; s.kappa = kappa; s.opt = opt;
   s.coef1.resize(steps); s.coef2.resize(steps); s.stdv.resize(steps); s.in_scale.resize(steps); s.tsteps.resize(steps);
+  s.eps_coef.resize(steps); s.eta.resize(steps); s.one_minus_eta.resize(steps);
   for (int i = 0; i < steps; ++i) {
     const double pvc = pv[i == 0 ? 1 : i];
     s.coef1[i] = (float)(prev[i] / etas[i]);
@@ -1748,10 +1781,27 @@ static void schedule_tables(rs_sampler& s, int steps, const double* sqrt_etas, d
     const float logv = (float)std::log(pvc);
     s.stdv[i] = std::exp(0.5f * logv);
     const float e32 = (float)etas[i];
-    s.in_scale[i] = 1.0f / std::sqrt(e32 * (float)(kappa * kappa) + 1.0f);
+    if (!opt.normalize_input) {
+      s.in_scale[i] = 1.0f;
+    } else if (opt.latent_flag) {
+      s.in_scale[i] = 1.0f / std::sqrt(e32 * (float)(kappa * kappa) + 1.0f);
+    } else {
+      s.in_scale[i] = 1.0f / ((float)sqrt_etas[i] * (float)kappa * 3.0f + 1.0f);
+    }
     s.tsteps[i] = (float)(tmap ? tmap[i] : i);
+    s.eps_coef[i] = (float)sqrt_etas[i] * (float)kappa;
+    s.eta[i] = e32;
+    s.one_minus_eta[i] = (float)(1.0 - etas[i]);
   }
   s.prior_coef = (float)(kappa * sqrt_etas[steps - 1]);
+}
+
+static int check_sampler_options(const rs_sampler_options& o) {
+  RS_CHECK(o.mean_type >= RS_MEAN_XSTART && o.mean_type <= RS_MEAN_RESIDUAL,
+           "unknown mean type " + std::to_string(o.mean_type) + " (RS_MEAN_XSTART .. RS_MEAN_RESIDUAL)");
+  RS_CHECK((o.normalize_input == 0 || o.normalize_input == 1) && (o.latent_flag == 0 || o.latent_flag == 1),
+           "normalize_input and latent_flag must be 0 or 1");
+  return 0;
 }
 
 static void copy_tables(const rs_sampler& s, float* dst) {
@@ -1762,15 +1812,21 @@ static void copy_tables(const rs_sampler& s, float* dst) {
   *dst = s.prior_coef;
 }
 
-int rs_sampler_create(rs_plan* p, int steps, const double* sqrt_etas, double kappa, const int32_t* tmap, rs_sampler** out) {
-  RS_CHECK(p && p->bound && sqrt_etas && out, "bad argument (plan must be bound)");
+int rs_sampler_create_ex(rs_plan* p, int steps, const double* sqrt_etas, double kappa, const int32_t* tmap,
+                         const rs_sampler_options* opt, rs_sampler** out) {
+  RS_CHECK(p && p->bound && sqrt_etas && opt && out, "bad argument (plan must be bound)");
   RS_CHECK(p->pass == Pass::Denoiser, std::string("samplers are built on denoiser plans: this plan belongs to ") + kind_name(p->e->kind));
   RS_CHECK(steps >= 2 && steps <= p->max_rows && steps <= 1024, "steps out of range for this plan");
+  int rc = check_sampler_options(*opt); if (rc) return rc;
   auto s = std::make_unique<rs_sampler>();
   s->p = p;
-  schedule_tables(*s, steps, sqrt_etas, kappa, tmap);
+  schedule_tables(*s, steps, sqrt_etas, kappa, tmap, *opt);
   *out = s.release();
   return 0;
+}
+int rs_sampler_create(rs_plan* p, int steps, const double* sqrt_etas, double kappa, const int32_t* tmap, rs_sampler** out) {
+  const rs_sampler_options opt{RS_MEAN_XSTART, 1, 1};
+  return rs_sampler_create_ex(p, steps, sqrt_etas, kappa, tmap, &opt, out);
 }
 int rs_sampler_tables(const rs_sampler* s, float* dst) {
   RS_CHECK(s && dst, "null argument");
@@ -1801,6 +1857,20 @@ int rs_schedule_tables(int steps, const double* sqrt_etas, double kappa, const i
   rs_sampler s;
   schedule_tables(s, steps, sqrt_etas, kappa, tmap);
   copy_tables(s, dst);
+  return 0;
+}
+int rs_schedule_tables_ex(int steps, const double* sqrt_etas, double kappa, const int32_t* tmap,
+                          const rs_sampler_options* opt, float* dst) {
+  RS_CHECK(sqrt_etas && opt && dst && steps >= 1, "bad argument");
+  int rc = check_sampler_options(*opt); if (rc) return rc;
+  rs_sampler s;
+  schedule_tables(s, steps, sqrt_etas, kappa, tmap, *opt);
+  copy_tables(s, dst);
+  dst += 5 * steps + 1;
+  for (const std::vector<float>* v : {&s.eps_coef, &s.eta, &s.one_minus_eta}) {
+    std::memcpy(dst, v->data(), (size_t)steps * sizeof(float));
+    dst += steps;
+  }
   return 0;
 }
 void rs_sampler_destroy(rs_sampler* s) {

@@ -5,9 +5,10 @@ Mirrors the call surface of the reference's ``GaussianDiffusion`` / ``SpacedDiff
 ``p_sample_loop``, ``p_sample_loop_progressive``, ``p_sample``, ``p_mean_variance``, ``prior_sample``,
 ``encode_first_stage``, ``decode_first_stage``, ``_scale_input``, ``q_sample``, ``num_timesteps``.
 
-When the model is this package's ``UNetModelSwin`` the whole T-step loop (input scaling, denoiser,
-posterior mean, noise injection, next-input packing) runs inside ``librs_b200.so`` as one CUDA graph;
-for any other callable the per-step update still runs through the library's ``rs_p_sample`` kernel.
+When the model is one of this package's UNets the whole T-step loop (input scaling, denoiser, the model output's
+conversion to x0 for every predict_type, posterior mean, noise injection, next-input packing) runs inside
+``librs_b200.so`` as one CUDA graph; for any other callable, with clipping or with a ``denoised_fn`` the per-step update
+still runs through the library's ``rs_p_sample`` kernel.
 The VQ-GAN bookends (``encode_first_stage`` / ``decode_first_stage``) stay in PyTorch.
 Training (``training_losses``) is out of scope.
 """
@@ -217,11 +218,20 @@ class ResShiftDiffusion:
         return {"sample": sample, "pred_xstart": out["pred_xstart"], "mean": out["mean"]}
 
     # ------------------------------------------------------------------ the loop
+    _NATIVE_MEAN_TYPES = {ModelMeanType.START_X: "xstart", ModelMeanType.EPSILON: "epsilon",
+                          ModelMeanType.EPSILON_SCALE: "epsilon_scale", ModelMeanType.RESIDUAL: "residual"}
+
     def _native_ok(self, model, clip_denoised, denoised_fn, model_kwargs) -> bool:
-        return (isinstance(model, (UNetModelSwin, UNetModel, UNetModelConv)) and self.model_mean_type == ModelMeanType.START_X
-                and not clip_denoised and denoised_fn is None and self.normalize_input and self.latent_flag
+        return (isinstance(model, (UNetModelSwin, UNetModel, UNetModelConv))
+                and self.model_mean_type in self._NATIVE_MEAN_TYPES
+                and not clip_denoised and denoised_fn is None
                 and model_kwargs is not None and "lq" in model_kwargs
-                and 2 <= self.num_timesteps <= 64)       # rs_sampler_create: 2 <= T <= FiLM-table rows of a plan
+                and 2 <= self.num_timesteps <= 64)       # rs_sampler_create_ex: 2 <= T <= FiLM-table rows of a plan
+
+    def sampler_options(self) -> "_lib.SamplerOptionsC":
+        """rs_sampler_options of this process: the step's x0 conversion and the denoiser's input scaling."""
+        return _lib.SamplerOptionsC(_lib.MEAN_TYPES[self._NATIVE_MEAN_TYPES[self.model_mean_type]],
+                                    int(bool(self.normalize_input)), int(bool(self.latent_flag)))
 
     @staticmethod
     def _check_native_inputs(model: UNetModelSwin, z_y, lq, mask):
@@ -251,12 +261,15 @@ class ResShiftDiffusion:
 
     def native_sampler(self, model: UNetModelSwin, batch, height, width):
         plan = model.plan(batch, height, width)
-        key = (self.num_timesteps, self.kappa, tuple(self.sqrt_etas.tolist()), tuple(self.timestep_map))
+        opt = self.sampler_options()
+        key = (self.num_timesteps, self.kappa, tuple(self.sqrt_etas.tolist()), tuple(self.timestep_map),
+               (opt.mean_type, opt.normalize_input, opt.latent_flag))
         if key not in plan.samplers:
             h = C.c_void_p()
             se = (C.c_double * self.num_timesteps)(*self.sqrt_etas.tolist())
             tm = (C.c_int32 * self.num_timesteps)(*self.timestep_map)
-            _lib.check(_lib.lib.rs_sampler_create(plan.handle, self.num_timesteps, se, float(self.kappa), tm, C.byref(h)))
+            _lib.check(_lib.lib.rs_sampler_create_ex(plan.handle, self.num_timesteps, se, float(self.kappa), tm,
+                                                     C.byref(opt), C.byref(h)))
             plan.samplers[key] = h
         return plan.samplers[key]
 
@@ -296,6 +309,7 @@ class ResShiftDiffusion:
                                                    final.data_ptr(), 0, _lib.current_stream()))
             finally:
                 _lib.check(_lib.lib.rs_sampler_set_taps(s, None, None))
+            # preds holds the step kernel's converted x0 (pred_xstart); the mean follows from it
             c1 = self.posterior_mean_coef1.astype(np.float32)
             c2 = self.posterior_mean_coef2.astype(np.float32)
             x_prev = self.prior_sample(zf, noises[0])

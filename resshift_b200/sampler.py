@@ -440,8 +440,8 @@ class ResShiftSampler(BaseSampler):
                                               model_kwargs={"lq": None}):
             raise RuntimeError(
                 f"{mode} needs the fused sampling loop, whose noise can be drawn ahead of the encoder; this "
-                "configuration takes the generic per-step route (no autoencoder, a model other than this package's "
-                "UNetModelSwin, predict_type other than xstart, or T outside 2..64)")
+                "configuration takes the generic per-step route (no autoencoder, so x0 is clipped; a model other than "
+                "this package's UNetModelSwin, UNetModel or UNetModelConv; or T outside 2..64)")
 
     def _sample_unit(self, y0, mask, noises, spec, replica):
         """sample_func with its noise given (a UnitNoise): reflect-pad, encode_first_stage(up_sample=True) with the
