@@ -109,7 +109,8 @@ typedef struct rs_unetconv_config {
 
 /* ``autoencoder.params`` of the shipped yaml files: VQModelTorch(ddconfig, n_embed, embed_dim)
  * (reference ldm/models/autoencoder.py:12-26; ddconfig -> ldm/modules/diffusionmodules/model.py:452-470,563-581).
- * Covered: double_z = False, attn_resolutions = [], dropout = 0 (every shipped config). */
+ * The ddconfig keys that place attention blocks or change the resampling and the output are in rs_vq_options;
+ * dropout is identity at inference. */
 typedef struct rs_vq_config {
   int32_t embed_dim;
   int32_t n_embed;
@@ -121,6 +122,21 @@ typedef struct rs_vq_config {
   int32_t ch_mult[RS_MAX_LEVELS];
   int32_t num_res_blocks[RS_MAX_LEVELS];
 } rs_vq_config;
+
+/* The remaining Encoder / Decoder options of ddconfig (reference ldm/modules/diffusionmodules/model.py:452-660), each
+ * 0 or 1.  rs_vq_create / rs_kl_create use the values of every shipped config: no level attention, the mid-block
+ * attention, conv resampling, no tanh.  Every attention block is AttnBlock (model.py:152-203; attn_type "vanilla" or
+ * "vanilla-xformers", the same math and parameters) and runs in the GEMM + row-softmax form up to 8192 positions, in
+ * the fused form above (128, 256 or 512 channels, H and W multiples of 8; rs_vq_plan_create refuses other levels). */
+typedef struct rs_vq_options {
+  int32_t enc_attn[RS_MAX_LEVELS];   /* 1: an AttnBlock after every ResnetBlock of encoder level i: the level's curr_res
+                                        (resolution halved i times) is in attn_resolutions (model.py:491-498,543-546) */
+  int32_t dec_attn[RS_MAX_LEVELS];   /* 1: the same after every ResnetBlock of decoder level i: curr_res =
+                                        (resolution // 2^(L-1)) * 2^(L-1-i) is in attn_resolutions (model.py:596-616,643-646) */
+  int32_t mid_attn;                  /* 0: attn_type "none", mid.attn_1 is nn.Identity (model.py:280-298)             */
+  int32_t resamp_with_conv;          /* 0: Downsample = 2x2 average pool, Upsample = nearest 2x, no conv (model.py:51-88) */
+  int32_t tanh_out;                  /* 1: the decoder's image is tanh(conv_out(h)) (model.py:658-659)                 */
+} rs_vq_options;
 
 typedef struct rs_engine rs_engine;     /* architecture + packed weights      */
 typedef struct rs_plan rs_plan;         /* engine bound to (batch, H, W)      */
@@ -217,6 +233,9 @@ int rs_sampler_set_taps(rs_sampler* s, float* pred_xstart_steps, float* sample_s
  * _set_arena / _load_param work on it unchanged (state_dict names and shapes of the reference's VQModelTorch, so
  * autoencoder_vq_f4.pth / ffhq512_vq_f8_dim8_face.pth load as they are). */
 int rs_vq_create(const rs_vq_config* cfg, rs_engine** out);
+/* rs_vq_create is rs_vq_create_ex with the shipped options {0..., 0..., 1, 1, 0}.  Option flags other than 0 / 1 and an
+ * attention level whose channels are not a multiple of 64 are refused. */
+int rs_vq_create_ex(const rs_vq_config* cfg, const rs_vq_options* opts, rs_engine** out);
 /* plan for a fixed (batch, image H, image W); which = 0: encode (image -> latent), 1: decode (latent -> image).
  * Uses rs_plan_workspace_bytes / rs_plan_bind / rs_plan_destroy like a denoiser plan. */
 int rs_vq_plan_create(rs_engine* e, int batch, int image_h, int image_w, int which, rs_plan** out);
@@ -226,22 +245,32 @@ int rs_vq_encode(rs_plan* p, const float* x, float* h_out, void* stream);
  * ldm/modules/vqvae/quantize.py:271-284; skipped when force_not_quantize) -> post_quant_conv -> Decoder -> [B, 3, H, W] fp32.
  * idx_out: optional [B, H/f, W/f] int32 code indices. */
 int rs_vq_decode(rs_plan* p, const float* h, float* out, int32_t* idx_out, int force_not_quantize, void* stream);
-/* Each pass split at its mid-block attention, so that the query rows of that attention can be computed by several
- * devices and exchanged in between.  rs_vq_encode = rs_vq_encode_begin + rs_vq_encode_end and rs_vq_decode =
- * rs_vq_decode_begin + rs_vq_decode_end, the same launches in the same order.  _begin runs the input stage and every op
- * up to and including the fused attention (the whole op list on plans without one: bottlenecks of <= 8192 positions);
- * _end runs the rest and the output stage (quant_conv / the copy of the image). */
+/* Each pass split at its fused attentions (attention blocks over more than 8192 positions, in pass order 0 .. n-1), so
+ * that the query rows of each can be computed by several devices and exchanged in between.  _begin runs the input stage
+ * and every op up to and including fused attention 0 (the whole op list on plans without one); rs_vq_run_between(p, a)
+ * runs the ops after fused attention a-1 up to and including fused attention a, 1 <= a < n; _end runs the rest and the
+ * output stage (quant_conv / the copy of the image).  rs_vq_encode = rs_vq_encode_begin + rs_vq_run_between(1 .. n-1) +
+ * rs_vq_encode_end, and so for the decode and KL passes: the same launches in the same order.  On a plan with two or
+ * more fused attentions, rs_vq_run_between and _end refuse calls out of that order. */
 int rs_vq_encode_begin(rs_plan* p, const float* x, void* stream);
 int rs_vq_encode_end(rs_plan* p, float* h_out, void* stream);
 int rs_vq_decode_begin(rs_plan* p, const float* h, int32_t* idx_out, int force_not_quantize, void* stream);
 int rs_vq_decode_end(rs_plan* p, float* out, void* stream);
-/* Query rows [row_begin, row_end) of every image that the plan's fused attention computes (default [0, T), T = the
- * bottleneck's H*W); multiples of 64 inside [0, T].  An empty range skips the attention launch.  Rows outside the
- * range keep whatever the attention output view held (the caller writes them between _begin and _end). */
-int rs_vq_set_attention_rows(rs_plan* p, int row_begin, int row_end);
-/* The fused attention's output as proj_out reads it (bound plans): fp16, element (n, t, c) at
+int rs_vq_run_between(rs_plan* p, int a, void* stream);       /* VQ-GAN and KL plans */
+/* n = the number of fused attentions of the plan's pass (0 when every attention has 8192 positions or fewer) */
+int rs_vq_attention_count(rs_plan* p, int32_t* n);
+/* Query rows [row_begin, row_end) of every image that fused attention a computes (default [0, T), T = its H*W);
+ * multiples of 64 inside [0, T].  An empty range skips the attention launch.  Rows outside the range keep whatever the
+ * attention output view held (the caller writes them before the next segment of the pass runs). */
+int rs_vq_set_attention_rows_at(rs_plan* p, int a, int row_begin, int row_end);
+/* fused attention a's output as its proj_out reads it (bound plans): fp16, element (n, t, c) at
  * ptr + n * image_stride + t * row_stride + c (strides in elements), n < batch, t < T, c < C.  It holds the attention
- * result from the end of _begin until _end reads it; nothing else in the plan writes it in between. */
+ * result from the end of the segment that computes it until the next segment reads it; nothing else in the plan writes
+ * it in between. */
+int rs_vq_attention_output_at(rs_plan* p, int a, void** ptr, long long* row_stride, long long* image_stride, int32_t* T,
+                              int32_t* C);
+/* rs_vq_set_attention_rows_at / rs_vq_attention_output_at with a = 0 */
+int rs_vq_set_attention_rows(rs_plan* p, int row_begin, int row_end);
 int rs_vq_attention_output(rs_plan* p, void** ptr, long long* row_stride, long long* image_stride, int32_t* T, int32_t* C);
 /* diagnostics: per-launch times (ms) and descriptions of the plan's op list on the inputs of the last encode/decode
  * call (counterpart of rs_plan_profile_ops for the first-stage plans); VQ-GAN and KL plans */
@@ -259,6 +288,8 @@ int rs_vq_decode_code(rs_plan* p, const int32_t* idx, float* out, void* stream);
  * rs_vq_attention_output and rs_vq_profile_ops work as for the VQ-GAN; the rs_vq_encode / _decode calls refuse KL
  * plans and the rs_kl_* calls refuse VQ-GAN plans. */
 int rs_kl_create(const rs_vq_config* cfg, rs_engine** out);
+/* rs_kl_create with rs_vq_options, as rs_vq_create_ex */
+int rs_kl_create_ex(const rs_vq_config* cfg, const rs_vq_options* opts, rs_engine** out);
 /* AutoencoderKLTorch.encode (autoencoder.py:65-76) with DiagonalGaussianDistribution
  * (ldm/modules/distributions/distributions.py:24-37,61-62): x [B, 3, H, W] fp32 -> moments = quant_conv(Encoder(x))
  * [B, 2 embed_dim, H/f, W/f]; mean, logvar = moments[:, :e], clamp(moments[:, e:], -30, 20);
@@ -269,7 +300,7 @@ int rs_kl_encode(rs_plan* p, const float* x, const float* noise_or_null, float* 
 /* AutoencoderKLTorch.decode (autoencoder.py:78-81): z [B, embed_dim, H/f, W/f] -> post_quant_conv -> Decoder ->
  * out [B, 3, H, W] fp32 */
 int rs_kl_decode(rs_plan* p, const float* z, float* out, void* stream);
-/* the two halves of each pass, split at the mid-block attention as the rs_vq_*_begin / _end calls are */
+/* each pass split at its fused attentions as the rs_vq_*_begin / rs_vq_run_between / _end calls are */
 int rs_kl_encode_begin(rs_plan* p, const float* x, void* stream);
 int rs_kl_encode_end(rs_plan* p, const float* noise_or_null, float* z_out, float* moments_out_or_null, void* stream);
 int rs_kl_decode_begin(rs_plan* p, const float* z, void* stream);

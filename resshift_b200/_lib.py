@@ -66,6 +66,14 @@ class VQConfigC(C.Structure):
     ]
 
 
+class VQOptionsC(C.Structure):
+    """Mirror of ``rs_vq_options``."""
+    _fields_ = [
+        ("enc_attn", C.c_int32 * RS_MAX_LEVELS), ("dec_attn", C.c_int32 * RS_MAX_LEVELS), ("mid_attn", C.c_int32),
+        ("resamp_with_conv", C.c_int32), ("tanh_out", C.c_int32),
+    ]
+
+
 class ConvArgsC(C.Structure):
     """Mirror of ``rs_conv_args``."""
     _fields_ = [
@@ -223,6 +231,13 @@ _SIGNATURES = {
     "rs_op_upsample2x_ex": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P, _P]),
     "rs_op_avgpool2x2": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P, _P]),
     "rs_vq_create": (C.c_int, [C.POINTER(VQConfigC), C.POINTER(_P)]),
+    "rs_vq_create_ex": (C.c_int, [C.POINTER(VQConfigC), C.POINTER(VQOptionsC), C.POINTER(_P)]),
+    "rs_kl_create_ex": (C.c_int, [C.POINTER(VQConfigC), C.POINTER(VQOptionsC), C.POINTER(_P)]),
+    "rs_vq_run_between": (C.c_int, [_P, C.c_int, _P]),
+    "rs_vq_attention_count": (C.c_int, [_P, C.POINTER(C.c_int32)]),
+    "rs_vq_set_attention_rows_at": (C.c_int, [_P, C.c_int, C.c_int, C.c_int]),
+    "rs_vq_attention_output_at": (C.c_int, [_P, C.c_int, C.POINTER(_P), C.POINTER(C.c_longlong), C.POINTER(C.c_longlong),
+                                            C.POINTER(C.c_int32), C.POINTER(C.c_int32)]),
     "rs_vq_plan_create": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(_P)]),
     "rs_vq_encode": (C.c_int, [_P, _P, _P, _P]),
     "rs_vq_decode": (C.c_int, [_P, _P, _P, _P, C.c_int, _P]),
@@ -347,3 +362,12 @@ def make_vq_config(cfg) -> VQConfigC:
     for i, v in enumerate(cfg.num_res_blocks):
         c.num_res_blocks[i] = int(v)
     return c
+
+
+def make_vq_options(cfg) -> VQOptionsC:
+    """``rs_vq_options`` of a VQConfig: its attention levels (encoder and decoder apart), mid attention, resampling, tanh."""
+    o = VQOptionsC()
+    for i, (e, d) in enumerate(zip(cfg.enc_attn, cfg.dec_attn)):
+        o.enc_attn[i], o.dec_attn[i] = int(e), int(d)
+    o.mid_attn, o.resamp_with_conv, o.tanh_out = int(cfg.has_attn), int(cfg.resamp_with_conv), int(cfg.tanh_out)
+    return o

@@ -467,5 +467,13 @@ __global__ void copy_f32_kernel(const float* __restrict__ src, float* __restrict
   if (i < n) dst[i] = src[i];
 }
 
+// the decoder's fp32 output stage with tanh_out (reference model.py:658-659)
+__global__ void copy_tanh_f32_kernel(const float* __restrict__ src, float* __restrict__ dst, long long n) {
+  pdl_trigger();
+  pdl_wait();
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) dst[i] = tanhf(src[i]);
+}
+
 #endif
 }  // namespace rs

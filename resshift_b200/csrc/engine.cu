@@ -63,6 +63,7 @@ constexpr int kDenoiserOuterLaunches = 6, kEncodeOuterLaunches = 3, kDecodeOuter
 struct rs_engine {
   EngineKind kind = EngineKind::Denoiser;   // the parameter store is shared by all kinds
   rs_vq_config vq{};
+  rs_vq_options vqopt{};                    // first stages: attention levels, mid attention, resampling, tanh (rs_vq_create_ex)
   rs_unet_config cfg;
   rs_unet_options opt{1, 0, 1, 0};
   // UNetModel (rs_unetmodel_create): global-attention blocks instead of Swin layers, no feature extractor; cfg then holds
@@ -432,7 +433,8 @@ struct rs_plan {
   int launches = 0;
   Pass pass = Pass::Denoiser;
   int imgH = 0, imgW = 0;    // VQ plans: image size (H, W above are the latent size)
-  int vq_attn_op = -1;       // VQ plans: index in ops of the fused bottleneck attention (-1: none, T <= 8192)
+  std::vector<int> vq_attn_ops;  // VQ plans: indices in ops of the fused attentions (T > 8192), in pass order
+  int vq_next = 0;           // VQ plans: the fused attention whose segment runs next (1 after _begin; 0 after _end)
   // The schedule tables and the FiLM table live in this plan's workspace and are shared by rs_plan_forward (FiLM rows
   // 0..B-1 for the caller's timesteps) and by every sampler of the plan (rows 0..T-1 for its schedule): whoever wrote them
   // last owns them.  A sampler re-derives them when it is not the owner or when the weights changed since (weights_epoch).

@@ -35,19 +35,29 @@ class _Node(nn.Module):
 
 
 def _config(ddconfig, embed_dim, n_embed=0, kl=False) -> VQConfig:
+    """The VQConfig of a reference ``ddconfig`` (the keyword arguments of Encoder / Decoder, model.py:452-470,563-581);
+    ValueError names what the native kernels do not run."""
     dd = dict(ddconfig)
+    if dd.get("give_pre_end", False):
+        raise ValueError("give_pre_end=True: the decoder would return its pre-norm features instead of an image "
+                         "(ldm/modules/diffusionmodules/model.py:651-652); only image decoders are supported")
+    attn_type = dd.get("attn_type", "vanilla")
+    if dd.get("use_linear_attn", False):
+        raise ValueError("use_linear_attn=True selects attn_type 'linear', for which the reference's make_attn raises "
+                         "NotImplementedError (ldm/modules/diffusionmodules/model.py:280-298)")
     return VQConfig(embed_dim=embed_dim, n_embed=n_embed, z_channels=dd["z_channels"], resolution=dd.get("resolution", 256),
                     in_channels=dd.get("in_channels", 3), out_ch=dd.get("out_ch", 3), ch=dd["ch"],
                     ch_mult=tuple(dd["ch_mult"]), num_res_blocks=dd["num_res_blocks"],
                     attn_resolutions=tuple(dd.get("attn_resolutions", ())), dropout=dd.get("dropout", 0.0),
-                    double_z=dd.get("double_z", kl), kl=kl)
+                    double_z=dd.get("double_z", kl), kl=kl, attn_type=attn_type,
+                    resamp_with_conv=dd.get("resamp_with_conv", True), tanh_out=dd.get("tanh_out", False))
 
 
 class _FirstStage(nn.Module):
     """What the first stages share: reference-named parameters, the native engine and its weight arena, one plan per
     (pass, batch, image size), and attention teams.  ``_create`` is the engine constructor of the C ABI."""
 
-    _create = "rs_vq_create"
+    _create = "rs_vq_create_ex"
     _name = "VQModelTorch"
     _encoder_only = False          # the module holds the encoder's parameters only (the engine lists the decoder's too)
 
@@ -77,8 +87,8 @@ class _FirstStage(nn.Module):
             raise RuntimeError(f"resshift_b200.{self._name} runs on CUDA only (no CPU fallback); call .cuda() first")
         if self._engine is None:
             h = C.c_void_p()
-            cfgc = _lib.make_vq_config(self.cfg)
-            _lib.check(getattr(_lib.lib, self._create)(C.byref(cfgc), C.byref(h)))
+            cfgc, optc = _lib.make_vq_config(self.cfg), _lib.make_vq_options(self.cfg)
+            _lib.check(getattr(_lib.lib, self._create)(C.byref(cfgc), C.byref(optc), C.byref(h)))
             self._engine = h
             n = _lib.lib.rs_unet_param_count(h)
             theirs = []
@@ -161,8 +171,8 @@ class _FirstStage(nn.Module):
         return torch.empty(b, self.cfg.out_ch, lh * f, lw * f, dtype=torch.float32, device=h.device)
 
     def _run(self, plan: "_VQPlan", which: int, begin: Callable[[], None], end: Callable[[], None], whole: Callable[[], None]):
-        """One pass: split at the fused attention inside an attention team, else the single call ``whole``."""
-        if self._team is not None and plan.attention is not None:
+        """One pass: split at every fused attention inside an attention team, else the single call ``whole``."""
+        if self._team is not None and plan.attentions:
             self._run_team_split(plan, which, begin, end)
         else:
             whole()
@@ -170,13 +180,14 @@ class _FirstStage(nn.Module):
     # ------------------------------------------------------------------ attention teams
     @contextmanager
     def attention_team(self, member: int, size: int, exchange: Callable[[torch.Tensor, int, int], None]):
-        """Inside this context, ``encode`` / ``decode`` on a plan with the fused bottleneck attention (more than 8192
-        positions) compute only this member's query rows of it: 64-row blocks ``parallel.shard_range(T / 64, size,
-        member)``.  After the first half of the pass, ``exchange(view, row_begin, row_end)`` is called with the attention
-        output ``view`` ([N, T, C] fp16, on the current stream) and this member's rows; it must write every other
-        member's rows into ``view``.  Then the pass finishes.  Every member must run the same calls on the same inputs.
-        The attention rows are independent, so the result is bit-identical to a call outside the context.  Rows computed
-        are recorded in ``attention_rows``.  Plans without the fused attention run as usual."""
+        """Inside this context, ``encode`` / ``decode`` on a plan with fused attentions (attention blocks over more than
+        8192 positions) compute only this member's query rows of each: 64-row blocks ``parallel.shard_range(T / 64,
+        size, member)``.  After the part of the pass up to each such attention, ``exchange(view, row_begin, row_end)`` is
+        called with that attention's output ``view`` ([N, T, C] fp16, on the current stream) and this member's rows; it
+        must write every other member's rows into ``view``.  Then the pass goes on to the next one, and finishes.  Every
+        member must run the same calls on the same inputs.  The attention rows are independent, so the result is
+        bit-identical to a call outside the context.  Rows computed are recorded in ``attention_rows``, one entry per
+        fused attention in pass order.  Plans without a fused attention run as usual."""
         if not (0 <= member < size):
             raise ValueError(f"team member {member} of {size}")
         if self._team is not None:
@@ -189,19 +200,26 @@ class _FirstStage(nn.Module):
             self._team = None
 
     def _run_team_split(self, plan: "_VQPlan", which: int, begin: Callable[[], None], end: Callable[[], None]):
+        """_begin, then rs_vq_run_between for every further fused attention, then _end: each segment computes this
+        member's rows of the attention it ends with, and ``exchange`` fills in the others' before the next one reads
+        them."""
         member, size, exchange = self._team
-        view = plan.attention
-        t = view.shape[1]
-        b0, e0 = shard_range(t // 64, size, member)
-        rb, re = 64 * b0, 64 * e0
-        _lib.check(_lib.lib.rs_vq_set_attention_rows(plan.handle, rb, re))
-        try:
-            begin()
-        finally:
-            _lib.check(_lib.lib.rs_vq_set_attention_rows(plan.handle, 0, t))
-        exchange(view, rb, re)
+        stream = _lib.current_stream()
+        for a, view in enumerate(plan.attentions):
+            t = view.shape[1]
+            b0, e0 = shard_range(t // 64, size, member)
+            rb, re = 64 * b0, 64 * e0
+            _lib.check(_lib.lib.rs_vq_set_attention_rows_at(plan.handle, a, rb, re))
+            try:
+                if a == 0:
+                    begin()
+                else:
+                    _lib.check(_lib.lib.rs_vq_run_between(plan.handle, a, stream))
+            finally:
+                _lib.check(_lib.lib.rs_vq_set_attention_rows_at(plan.handle, a, 0, t))
+            exchange(view, rb, re)
+            self.attention_rows.append((which, rb, re))
         end()
-        self.attention_rows.append((which, rb, re))
 
     def __del__(self):
         try:
@@ -273,7 +291,7 @@ class EncoderKLTorch(_FirstStage):
     """The encoder half of the KL first stage (reference autoencoder.py:88-112): ``encode`` / ``forward`` as in
     AutoencoderKLTorch; its ``state_dict`` holds only ``encoder.*`` and ``quant_conv.*``."""
 
-    _create = "rs_kl_create"
+    _create = "rs_kl_create_ex"
     _name = "EncoderKLTorch"
     _encoder_only = True
     # encode() samples the posterior by default: ResShiftSampler draws that noise ahead of the unit (posterior_noise=)
@@ -352,14 +370,20 @@ class _VQPlan:
         self.workspace_ptr = (self.workspace.data_ptr() + 255) // 256 * 256
         _lib.check(_lib.lib.rs_plan_bind(h, self.workspace_ptr))
         self.launches = _lib.lib.rs_plan_num_launches(h)
-        # the fused attention's output [N, T, C] fp16 as a view of the workspace (None: the plan has no fused attention)
-        self.attention: Optional[torch.Tensor] = None
+        # each fused attention's output [N, T, C] fp16 as a view of the workspace, in pass order
+        self.attentions: List[torch.Tensor] = []
+        n = C.c_int32()
+        _lib.check(_lib.lib.rs_vq_attention_count(h, C.byref(n)))
         ptr, rstride, istride, t, cc = C.c_void_p(), C.c_longlong(), C.c_longlong(), C.c_int32(), C.c_int32()
-        if _lib.lib.rs_vq_attention_output(h, C.byref(ptr), C.byref(rstride), C.byref(istride), C.byref(t), C.byref(cc)) == 0:
+        for a in range(n.value):
+            _lib.check(_lib.lib.rs_vq_attention_output_at(h, a, C.byref(ptr), C.byref(rstride), C.byref(istride), C.byref(t),
+                                                          C.byref(cc)))
             off = ptr.value - self.workspace.data_ptr()
             assert off % 2 == 0 and self.workspace.numel() % 2 == 0
-            self.attention = torch.as_strided(self.workspace.view(torch.float16), (batch, t.value, cc.value),
-                                              (istride.value, rstride.value, 1), off // 2)
+            self.attentions.append(torch.as_strided(self.workspace.view(torch.float16), (batch, t.value, cc.value),
+                                                    (istride.value, rstride.value, 1), off // 2))
+        # the first fused attention's output (None: the plan has none)
+        self.attention: Optional[torch.Tensor] = self.attentions[0] if self.attentions else None
 
     def __del__(self):
         try:

@@ -29,9 +29,12 @@ class VQConfig:
     ch_mult: Sequence[int] = (1, 2, 4)
     num_res_blocks: Sequence[int] = (2, 2, 2)
     attn_resolutions: Sequence[int] = ()
-    dropout: float = 0.0
+    dropout: float = 0.0        # identity at inference
     double_z: bool = False
     kl: bool = False            # AutoencoderKLTorch: double_z encoder, posterior moments, no codebook (n_embed unused)
+    attn_type: str = "vanilla"  # "vanilla" / "vanilla-xformers" (AttnBlock, the same math and keys) or "none"
+    resamp_with_conv: bool = True   # False: Downsample = avg_pool2d(2, 2), Upsample = nearest x2, no conv
+    tanh_out: bool = False      # the decoder's image is tanh(conv_out(h))
 
     def __post_init__(self):
         self.ch_mult = tuple(int(v) for v in self.ch_mult)
@@ -39,9 +42,41 @@ class VQConfig:
             self.num_res_blocks = (self.num_res_blocks,) * len(self.ch_mult)
         self.num_res_blocks = tuple(int(v) for v in self.num_res_blocks)
         self.attn_resolutions = tuple(int(v) for v in self.attn_resolutions)
-        # what this implementation covers (every shipped yaml satisfies these)
-        assert self.double_z == self.kl and self.dropout == 0 and len(self.attn_resolutions) == 0
+        self.resamp_with_conv, self.tanh_out = bool(self.resamp_with_conv), bool(self.tanh_out)
+        assert self.double_z == self.kl
         assert len(self.num_res_blocks) == len(self.ch_mult)
+        if self.attn_type in ("linear", "memory-efficient-cross-attn"):
+            raise ValueError(f"attn_type {self.attn_type!r}: the reference's make_attn raises NotImplementedError for it "
+                             "(ldm/modules/diffusionmodules/model.py:280-298), so no checkpoint of it exists")
+        if self.attn_type not in ("vanilla", "vanilla-xformers", "none"):
+            raise ValueError(f"attn_type {self.attn_type!r} unknown (vanilla, vanilla-xformers or none)")
+        for i, c in enumerate(self.ch_mult):
+            if (self.enc_attn[i] or self.dec_attn[i]) and (self.ch * c) % 64:
+                raise ValueError(f"attention at level {i} ({self.ch * c} channels): the attention GEMMs need channels that "
+                                 "are a multiple of 64")
+
+    @property
+    def has_attn(self) -> bool:
+        """AttnBlocks are built (attn_type "none" makes every one of them nn.Identity)."""
+        return self.attn_type != "none"
+
+    @property
+    def enc_attn(self) -> Tuple[bool, ...]:
+        """Per encoder level: an AttnBlock after each ResnetBlock.  Encoder.__init__ tests curr_res = resolution halved
+        (floor) once per level below (model.py:483-503)."""
+        out, r = [], self.resolution
+        for _ in range(self.levels):
+            out.append(self.has_attn and r in self.attn_resolutions)
+            r //= 2
+        return tuple(out)
+
+    @property
+    def dec_attn(self) -> Tuple[bool, ...]:
+        """Per decoder level (indexed by level, not by execution order): Decoder.__init__ tests curr_res =
+        (resolution // 2^(L-1)) * 2^(L-1-i) (model.py:576-616), which differs from the encoder's when resolution is
+        not a multiple of 2^(L-1)."""
+        base = self.resolution // 2 ** (self.levels - 1)
+        return tuple(self.has_attn and base * 2 ** (self.levels - 1 - i) in self.attn_resolutions for i in range(self.levels))
 
     @property
     def levels(self) -> int:
@@ -52,10 +87,18 @@ class VQConfig:
         return 2 ** (self.levels - 1)
 
     def ddconfig(self) -> dict:
-        return {"double_z": self.double_z, "z_channels": self.z_channels, "resolution": self.resolution,
-                "in_channels": self.in_channels, "out_ch": self.out_ch, "ch": self.ch, "ch_mult": list(self.ch_mult),
-                "num_res_blocks": list(self.num_res_blocks), "attn_resolutions": list(self.attn_resolutions),
-                "dropout": 0.0, "padding_mode": "zeros"}
+        dd = {"double_z": self.double_z, "z_channels": self.z_channels, "resolution": self.resolution,
+              "in_channels": self.in_channels, "out_ch": self.out_ch, "ch": self.ch, "ch_mult": list(self.ch_mult),
+              "num_res_blocks": list(self.num_res_blocks), "attn_resolutions": list(self.attn_resolutions),
+              "dropout": self.dropout, "padding_mode": "zeros"}
+        # the options the shipped configs leave at their defaults are written only when they differ from them
+        if self.attn_type != "vanilla":
+            dd["attn_type"] = self.attn_type
+        if not self.resamp_with_conv:
+            dd["resamp_with_conv"] = False
+        if self.tanh_out:
+            dd["tanh_out"] = True
+        return dd
 
     def to_kwargs(self) -> dict:
         if self.kl:
@@ -82,6 +125,24 @@ def kl_preset(name: str) -> VQConfig:
     if name == "tiny":                                  # the VQ "tiny" topology with a KL bottleneck
         return VQConfig(embed_dim=4, z_channels=4, resolution=64, ch=32, ch_mult=(1, 2, 4), num_res_blocks=(1, 2, 2),
                         double_z=True, kl=True)
+    raise KeyError(name)
+
+
+def ldm_vq_preset(name: str) -> VQConfig:
+    """LDM's VQ first stages with level attention or none, the ones a user would train ResShift's latent space in (not
+    shipped with ResShift: test and measurement configurations with synthetic weights)."""
+    if name == "vq-f8":
+        return VQConfig(embed_dim=4, n_embed=16384, z_channels=4, resolution=256, ch=128, ch_mult=(1, 2, 2, 4),
+                        num_res_blocks=2, attn_resolutions=(32,))
+    if name == "vq-f8-n256":
+        return VQConfig(embed_dim=4, n_embed=256, z_channels=4, resolution=256, ch=128, ch_mult=(1, 2, 2, 4),
+                        num_res_blocks=2, attn_resolutions=(32,))
+    if name == "vq-f16":
+        return VQConfig(embed_dim=8, n_embed=16384, z_channels=8, resolution=256, ch=128, ch_mult=(1, 1, 2, 2, 4),
+                        num_res_blocks=2, attn_resolutions=(16,))
+    if name == "vq-f4-noattn":
+        return VQConfig(embed_dim=3, n_embed=8192, z_channels=3, resolution=256, ch=128, ch_mult=(1, 2, 4),
+                        num_res_blocks=2, attn_type="none")
     raise KeyError(name)
 
 
@@ -158,20 +219,27 @@ def _first_stage_spec(cfg: VQConfig) -> Spec:
     for i, blocks, down in encoder_blocks(cfg):
         for j, (a, b) in enumerate(blocks):
             s += _resblock(f"encoder.down.{i}.block.{j}", a, b)
-        if down:
+        if cfg.enc_attn[i]:
+            for j, (_, b) in enumerate(blocks):
+                s += _attn(f"encoder.down.{i}.attn.{j}", b)
+        if down and cfg.resamp_with_conv:
             s += _conv(f"encoder.down.{i}.downsample.conv", blocks[-1][1], blocks[-1][1], 3)
     top = cfg.ch * cfg.ch_mult[-1]
-    s += _resblock("encoder.mid.block_1", top, top) + _attn("encoder.mid.attn_1", top) + _resblock("encoder.mid.block_2", top, top)
+    mid_attn = (lambda p: _attn(p, top)) if cfg.has_attn else (lambda p: [])
+    s += _resblock("encoder.mid.block_1", top, top) + mid_attn("encoder.mid.attn_1") + _resblock("encoder.mid.block_2", top, top)
     s += _gn("encoder.norm_out", top) + _conv("encoder.conv_out", top, z_out, 3)
     # decoder (state_dict order follows module registration: conv_in, mid, up.0 .. up.L-1, norm_out, conv_out)
     s += _conv("decoder.conv_in", cfg.z_channels, top, 3)
-    s += _resblock("decoder.mid.block_1", top, top) + _attn("decoder.mid.attn_1", top) + _resblock("decoder.mid.block_2", top, top)
+    s += _resblock("decoder.mid.block_1", top, top) + mid_attn("decoder.mid.attn_1") + _resblock("decoder.mid.block_2", top, top)
     by_level = {i: (blocks, up) for i, blocks, up in decoder_blocks(cfg)}
     for i in range(cfg.levels):
         blocks, up = by_level[i]
         for j, (a, b) in enumerate(blocks):
             s += _resblock(f"decoder.up.{i}.block.{j}", a, b)
-        if up:
+        if cfg.dec_attn[i]:
+            for j, (_, b) in enumerate(blocks):
+                s += _attn(f"decoder.up.{i}.attn.{j}", b)
+        if up and cfg.resamp_with_conv:
             s += _conv(f"decoder.up.{i}.upsample.conv", blocks[-1][1], blocks[-1][1], 3)
     s += _gn("decoder.norm_out", cfg.ch * cfg.ch_mult[0]) + _conv("decoder.conv_out", cfg.ch * cfg.ch_mult[0], cfg.out_ch, 3)
     # quantiser (VQ) and the two 1x1 convs around it / around the posterior (KL)
