@@ -186,9 +186,11 @@ int rs_plan_profile(rs_plan* p, const float* x, const float* timesteps, const fl
 /* per-operator variant: ms[i] and desc[i*desc_stride] for the first `cap` operators of the forward program */
 int rs_plan_profile_ops(rs_plan* p, const float* x, const float* timesteps, const float* lq, const float* mask,
                         double* ms, char* desc, int desc_stride, int cap, int32_t* n_ops, void* stream);
-/* debugging aid: copy an intermediate block output ("input_blocks.3", "middle_block", "output_blocks.11")
- * as fp32 NCHW into dst (device); returns channel count through *channels.  Valid right after a forward
- * only for blocks whose buffer is still live; used by the parity tests. */
+/* debugging aid: copy an intermediate block output ("input_blocks.3", "middle_block", "output_blocks.11"; in
+ * first-stage plans each attention block's "<prefix>.in", ".norm", ".q", ".k", ".attn" and "<prefix>" itself, e.g.
+ * "encoder.mid.attn_1.q", and the decoder's "quantize") as fp32 NCHW into dst (device); returns channel count through
+ * *channels.  Valid right after a forward or pass only for blocks whose buffer is still live (all of them under
+ * RS_NO_REUSE=1); used by the parity tests. */
 int rs_plan_probe(rs_plan* p, const char* block, float* dst, int32_t* channels, int32_t* h, int32_t* w,
                   void* stream);
 

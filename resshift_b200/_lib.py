@@ -300,6 +300,16 @@ def current_stream() -> int:
     return torch.cuda.current_stream().cuda_stream
 
 
+def probe(plan_handle, batch: int, block: str, device):
+    """rs_plan_probe: the named tensor of a bound plan's last run as a new fp32 NCHW tensor [batch, C, H, W]."""
+    import torch
+    c, hh, ww = C.c_int32(), C.c_int32(), C.c_int32()
+    check(lib.rs_plan_probe(plan_handle, block.encode(), None, C.byref(c), C.byref(hh), C.byref(ww), None))
+    out = torch.empty(batch, c.value, hh.value, ww.value, dtype=torch.float32, device=device)
+    check(lib.rs_plan_probe(plan_handle, block.encode(), out.data_ptr(), C.byref(c), C.byref(hh), C.byref(ww), current_stream()))
+    return out
+
+
 def make_config(cfg) -> UNetConfigC:
     c = UNetConfigC()
     c.image_size, c.in_channels, c.model_channels, c.out_channels = cfg.image_size, cfg.in_channels, cfg.model_channels, cfg.out_channels

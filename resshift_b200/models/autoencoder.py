@@ -141,6 +141,14 @@ class _FirstStage(nn.Module):
             self._plans[key] = _VQPlan(self, which, batch, image_h, image_w, device)
         return self._plans[key]
 
+    def probe(self, which: int, batch: int, image_h: int, image_w: int, block: str) -> torch.Tensor:
+        """A tensor of the LAST pass of plan (which, batch, image_h, image_w) as fp32 NCHW: an attention block's
+        ``<prefix>.in``, ``.norm``, ``.q``, ``.k``, ``.attn`` (before proj_out) or ``<prefix>`` (its output), or the
+        decoder's ``quantize`` (post_quant_conv's output).  Needs RS_NO_REUSE=1 when the plan is created to be valid for
+        every tensor."""
+        plan = self.plan(which, batch, image_h, image_w)
+        return _lib.probe(plan.handle, batch, block, plan.workspace.device)
+
     def _encode_plan(self, x, what):
         """The encode plan of image batch ``x`` and ``x`` as contiguous fp32."""
         if x.device.type != "cuda":

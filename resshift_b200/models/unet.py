@@ -142,12 +142,7 @@ class _NativeDenoiser(nn.Module):
     def probe(self, batch, height, width, block: str) -> torch.Tensor:
         """Block output of the LAST forward as fp32 NCHW (needs RS_NO_REUSE=1 to be valid for every block)."""
         plan = self.plan(batch, height, width)
-        c, hh, ww = C.c_int32(), C.c_int32(), C.c_int32()
-        _lib.check(_lib.lib.rs_plan_probe(plan.handle, block.encode(), None, C.byref(c), C.byref(hh), C.byref(ww), None))
-        out = torch.empty(batch, c.value, hh.value, ww.value, dtype=torch.float32, device=plan.workspace.device)
-        _lib.check(_lib.lib.rs_plan_probe(plan.handle, block.encode(), out.data_ptr(), C.byref(c), C.byref(hh),
-                                          C.byref(ww), _lib.current_stream()))
-        return out
+        return _lib.probe(plan.handle, batch, block, plan.workspace.device)
 
     def convert_to_fp16(self):   # reference API; precision is fixed by the kernels (fp16 storage, fp32 accumulate)
         return self

@@ -1,9 +1,12 @@
-"""Every attention kernel instance, and each attention the shipped plans run, against float64 references on the fp16
-operands, with a bound per output element.
+"""Every attention kernel instance, and each attention the shipped plans run on one of them, against float64 references
+on the fp16 operands, with a bound per output element.
 
 Kernels: window_attn_kernel<WS, HD> (WS 8 / 16, HD 32 / 64) and the SIMT cross-check (rs_op_window_attention_cfg, with
 forced heads per CTA), swin_attn_fused_kernel<E> (rs_op_swin_attn_ex, with forced persistent grids), unet_attn_sm90_kernel
-<D> (rs_op_unet_attention) and vq_attn_sm90_kernel<C> (rs_op_vq_attention / _rows).
+<D> (rs_op_unet_attention) and vq_attn_sm90_kernel<C> (rs_op_vq_attention / _rows).  The first stage's attention over
+8192 positions or fewer runs in GEMM form instead (three GEMMs on the conv kernel with softmax_rows_kernel between them,
+csrc/vq.inc attn_block); test_gpu_first_stage_kernels.py holds every such block of the first-stage plans and the row
+softmax to float64.
 
 Bound.  For query row i and output channel c, with p_ij the exact (float64) softmax weights, o_ic the exact output and
 u16 = 2^-11, u32 = 2^-23 (one fp32 operation; tensor-core accumulation may truncate, so a full ulp):
