@@ -188,7 +188,8 @@ int rs_plan_profile_ops(rs_plan* p, const float* x, const float* timesteps, cons
                         double* ms, char* desc, int desc_stride, int cap, int32_t* n_ops, void* stream);
 /* debugging aid: copy an intermediate block output ("input_blocks.3", "middle_block", "output_blocks.11"; in
  * first-stage plans each attention block's "<prefix>.in", ".norm", ".q", ".k", ".attn" and "<prefix>" itself, e.g.
- * "encoder.mid.attn_1.q", and the decoder's "quantize") as fp32 NCHW into dst (device); returns channel count through
+ * "encoder.mid.attn_1.q", the decoder's "quantize" and "quantize.padded", the same with the zero channels that pad it to
+ * a multiple of 8) as fp32 NCHW into dst (device); returns channel count through
  * *channels.  Valid right after a forward or pass only for blocks whose buffer is still live (all of them under
  * RS_NO_REUSE=1); used by the parity tests. */
 int rs_plan_probe(rs_plan* p, const char* block, float* dst, int32_t* channels, int32_t* h, int32_t* w,
@@ -392,12 +393,15 @@ int rs_schedule_tables(int steps, const double* sqrt_etas_host, double kappa, co
 int rs_schedule_tables_ex(int steps, const double* sqrt_etas_host, double kappa, const int32_t* timestep_map_host,
                           const rs_sampler_options* options, float* dst);
 /* quant_conv of the VQ-GAN encoder: y[n, co, hw] = b[co] + sum_ci w[co * w_ld + ci] x[n, ci, hw] (fp32 NCHW, fp16 w,
- * fp32 accumulation); Cin <= 8 */
+ * fp32 accumulation); Cin <= 8 (pointwise_conv_f32_kernel), or Cin a multiple of 8 from 16 to 64 with Cout <= 64
+ * (pointwise_conv_wide_kernel: w 16-byte aligned, w_ld a multiple of 8) */
 int rs_op_pointwise_conv(const float* x, const void* w_f16, int w_ld, const float* b, int Cin, int Cout, int N, int HW,
                          float* y, void* stream);
 /* quant_conv + posterior sample of the KL first stage (rs_kl_encode's last launch) on h [N, Cin, HW]: moments
  * [N, 2E, HW], z [N, E, HW] = mean + exp(0.5 clamp(logvar, -30, 20)) * noise, or mean without noise.  Cin <= 16 and
- * 2E <= 16. */
+ * 2E <= 16 (kl_posterior_kernel); otherwise Cin <= 16 or a multiple of 8 up to 128, and E <= 8 or a multiple of 8 from
+ * 16 to 64 (kl_posterior_wide_kernel: w 16-byte aligned, w_ld a multiple of 8).  Both compute the same: fmaf from the
+ * bias in ascending input order, mean + std * noise rounded as two operations. */
 int rs_op_kl_posterior(const float* h, const void* w_f16, int w_ld, const float* b, int Cin, int E, const float* noise,
                        float* z, float* moments, int N, int HW, void* stream);
 

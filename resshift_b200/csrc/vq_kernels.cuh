@@ -157,6 +157,93 @@ __global__ void kl_posterior_kernel(const KlPosteriorParams p) {
 }
 
 // ------------------------------------------------------------------------------------------------
+// Wide forms of the two kernels above, for latents of 16 to 64 channels (LDM's kl-f16 / kl-f32, 16-channel f8 KL
+// autoencoders): a CTA stages a tile of kWideTile positions of one image (NCHW fp32, read coalesced along HW) and the
+// whole fp16 weight matrix in shared memory, so nothing is held in per-thread arrays.  Warp w computes output rows
+// w, w + 8, ... of the tile, lane = position.  Same arithmetic as the narrow kernels: fp32 input times fp16 weight,
+// fmaf from the bias in ascending input-channel order; the KL form computes the mean and logvar rows of channel c in
+// the same pass, clamps logvar to [-30, 20] and rounds mean + std * noise as two operations.
+// The weight rows are moved as 16-byte vectors: w 16-byte aligned, w_ld a multiple of 8 (the arena's packed rows are).
+// ------------------------------------------------------------------------------------------------
+constexpr int kWideTile = 32;                      // positions per CTA (one per lane)
+constexpr int kWidePointwiseMaxCin = 64, kWidePointwiseMaxCout = 64;
+constexpr int kWideKlMaxCin = 128, kWideKlMaxE = 64;
+__host__ __device__ constexpr int wide_ldw(int cin) { return (cin + 7) / 8 * 8; }
+// dynamic shared memory of a wide launch: the weight rows [rows][ldw] fp16, then the tile [Cin][kWideTile] fp32
+__host__ __device__ constexpr size_t wide_1x1_smem(int cin, int rows) {
+  return (size_t)rows * wide_ldw(cin) * 2 + (size_t)cin * kWideTile * 4;
+}
+
+// stage weight rows [0, rows) and positions [hw0, hw0 + kWideTile) of x (one image, [Cin][HW]); positions past HW read 0
+__device__ __forceinline__ void wide_1x1_stage(const float* x, int Cin, int HW, int hw0, const __half* w, int w_ld, int rows,
+                                               __half* s_w, float* s_x) {
+  const int ldw = wide_ldw(Cin), vrow = ldw / 8;
+  for (int v = threadIdx.x; v < rows * vrow; v += blockDim.x) {
+    const int r = v / vrow, k = v % vrow;
+    reinterpret_cast<uint4*>(s_w)[v] = *reinterpret_cast<const uint4*>(w + (long long)r * w_ld + 8 * k);
+  }
+  for (int v = threadIdx.x; v < Cin * kWideTile; v += blockDim.x) {
+    const int c = v / kWideTile, t = v % kWideTile;
+    s_x[v] = hw0 + t < HW ? x[(long long)c * HW + hw0 + t] : 0.f;
+  }
+  __syncthreads();
+}
+
+// pointwise_conv_f32_kernel for 9 <= Cin <= 64 (Cout <= 64); grid (ceil(HW / kWideTile), N), 256 threads
+__global__ void __launch_bounds__(256) pointwise_conv_wide_kernel(const PointwiseParams p) {
+  pdl_trigger();
+  pdl_wait();
+  extern __shared__ __align__(16) unsigned char s_raw[];
+  __half* s_w = reinterpret_cast<__half*>(s_raw);
+  float* s_x = reinterpret_cast<float*>(s_raw + (size_t)p.Cout * wide_ldw(p.Cin) * 2);
+  const int n = blockIdx.y, hw0 = blockIdx.x * kWideTile;
+  wide_1x1_stage(p.x + (long long)n * p.Cin * p.HW, p.Cin, p.HW, hw0, p.w, p.w_ld, p.Cout, s_w, s_x);
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, ldw = wide_ldw(p.Cin);
+  if (hw0 + lane >= p.HW) return;
+  for (int co = warp; co < p.Cout; co += blockDim.x / 32) {
+    const __half* wr = s_w + co * ldw;                         // broadcast reads
+    float acc = p.b[co];
+    for (int c = 0; c < p.Cin; ++c) acc = fmaf(__half2float(wr[c]), s_x[c * kWideTile + lane], acc);
+    p.y[((long long)n * p.Cout + co) * p.HW + hw0 + lane] = acc;
+  }
+}
+
+// kl_posterior_kernel for Cin > 16 or 2E > 16 (Cin <= 128, E <= 64); grid (ceil(HW / kWideTile), N), 256 threads
+__global__ void __launch_bounds__(256) kl_posterior_wide_kernel(const KlPosteriorParams p) {
+  pdl_trigger();
+  pdl_wait();
+  extern __shared__ __align__(16) unsigned char s_raw[];
+  __half* s_w = reinterpret_cast<__half*>(s_raw);
+  float* s_x = reinterpret_cast<float*>(s_raw + (size_t)2 * p.E * wide_ldw(p.Cin) * 2);
+  const int n = blockIdx.y, hw0 = blockIdx.x * kWideTile;
+  wide_1x1_stage(p.h + (long long)n * p.Cin * p.HW, p.Cin, p.HW, hw0, p.w, p.w_ld, 2 * p.E, s_w, s_x);
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, ldw = wide_ldw(p.Cin);
+  const int hw = hw0 + lane;
+  if (hw >= p.HW) return;
+  for (int c = warp; c < p.E; c += blockDim.x / 32) {
+    const __half* wm = s_w + c * ldw;                          // mean row c and logvar row E + c, broadcast reads
+    const __half* wl = s_w + (p.E + c) * ldw;
+    float am = p.b[c], al = p.b[p.E + c];
+    for (int k = 0; k < p.Cin; ++k) {
+      const float xv = s_x[k * kWideTile + lane];
+      am = fmaf(__half2float(wm[k]), xv, am);
+      al = fmaf(__half2float(wl[k]), xv, al);
+    }
+    if (p.moments) {
+      p.moments[((long long)n * 2 * p.E + c) * p.HW + hw] = am;
+      p.moments[((long long)n * 2 * p.E + p.E + c) * p.HW + hw] = al;
+    }
+    const long long o = ((long long)n * p.E + c) * p.HW + hw;
+    float zc = am;
+    if (p.noise) {
+      const float logvar = fminf(fmaxf(al, -30.0f), 20.0f);
+      zc = __fadd_rn(zc, __fmul_rn(expf(0.5f * logvar), p.noise[o]));
+    }
+    p.z[o] = zc;
+  }
+}
+
+// ------------------------------------------------------------------------------------------------
 // VectorQuantizer2.forward (reference ldm/modules/vqvae/quantize.py:271-284) fused with post_quant_conv
 // (ldm/models/autoencoder.py:33-38) and the layout change the decoder's first conv wants:
 //   idx = argmin_j ( |z|^2 + |e_j|^2 - 2 z.e_j )   (first minimum, fp32)
@@ -226,6 +313,106 @@ __global__ void __launch_bounds__(256) vq_quantize_kernel(const QuantizeParams p
     o[co] = __float2half_rn(acc);
   }
   for (; co < p.Cpad; ++co) o[co] = __float2half_rn(0.f);
+}
+
+// ------------------------------------------------------------------------------------------------
+// vq_quantize_kernel for E = 16, 24, .., 64 (compile-time, so z stays in registers), Cz <= 64, Cpad = round_up(Cz, 8):
+// the same nearest code ((|z|^2 + |e|^2) - 2 z.e in fp32, the first minimum wins), the same decode_code gather (NaN for
+// an index outside [0, n_e)), the same post_quant_conv arithmetic (fmaf from the bias in ascending e order), the output
+// row written as 16-byte stores.  The codebook streams through shared memory in chunks of kQuantWideChunk<E> codes
+// (rows padded to E + 4 floats, |e|^2 beside them: 32 KB), post_quant_conv's rows [Cz][E] fp16 are staged once.
+// One thread per latent position, 256 per CTA.  codebook, pw and out must be 16-byte aligned, pw_ld a multiple of 8.
+// ------------------------------------------------------------------------------------------------
+constexpr int kQuantWideMaxCz = 64;
+template <int E>
+constexpr int kQuantWideChunk = (32 * 1024 / (4 * (E + 5))) / 32 * 32;
+template <int E>
+__global__ void __launch_bounds__(256) vq_quantize_wide_kernel(const QuantizeParams p) {
+  static_assert(E % 8 == 0 && E >= 16 && E <= 64, "wide quantiser: E a multiple of 8 in [16, 64]");
+  constexpr int kChunk = kQuantWideChunk<E>, kLd = E + 4, kV = E / 4;
+  __shared__ __align__(16) float s_code[kChunk * kLd];
+  __shared__ float s_ee[kChunk];
+  __shared__ __align__(16) __half s_w[kQuantWideMaxCz * E];
+  __shared__ float s_b[kQuantWideMaxCz];
+  pdl_trigger();
+  pdl_wait();
+  const int cpad = p.Cpad;
+  for (int v = threadIdx.x; v < cpad * (E / 8); v += blockDim.x) {      // rows past Cz are zero
+    const int r = v / (E / 8), k = v % (E / 8);
+    reinterpret_cast<uint4*>(s_w)[v] = r < p.Cz ? *reinterpret_cast<const uint4*>(p.pw + (long long)r * p.pw_ld + 8 * k)
+                                                : make_uint4(0u, 0u, 0u, 0u);
+  }
+  for (int r = threadIdx.x; r < cpad; r += blockDim.x) s_b[r] = r < p.Cz ? p.pb[r] : 0.f;
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  const bool live = i < (long long)p.N * p.HW;
+  const int n = live ? (int)(i / p.HW) : 0, hw = live ? (int)(i % p.HW) : 0;
+  float zv[E];
+  float zz = 0.f;
+#pragma unroll
+  for (int c = 0; c < E; ++c) zv[c] = live && !p.idx_in ? p.z[((long long)n * E + c) * p.HW + hw] : 0.f;
+#pragma unroll
+  for (int c = 0; c < E; ++c) zz += zv[c] * zv[c];           // torch.sum(z ** 2, dim=1): sequential over E
+  int best = 0;
+  if (p.quantize) {
+    float bestd = 3.0e38f;
+    for (int j0 = 0; j0 < p.n_e; j0 += kChunk) {
+      const int cnt = min(kChunk, p.n_e - j0);
+      __syncthreads();
+      const float4* src = reinterpret_cast<const float4*>(p.codebook + (long long)j0 * E);
+      for (int v = threadIdx.x; v < cnt * kV; v += blockDim.x)                 // coalesced 16-byte reads
+        *reinterpret_cast<float4*>(s_code + (v / kV) * kLd + 4 * (v % kV)) = src[v];
+      __syncthreads();
+      for (int t = threadIdx.x; t < cnt; t += blockDim.x) {
+        const float* e = s_code + t * kLd;
+        float ee = 0.f;
+#pragma unroll
+        for (int c = 0; c < E; ++c) ee += e[c] * e[c];
+        s_ee[t] = ee;
+      }
+      __syncthreads();
+      for (int t = 0; t < cnt; ++t) {
+        const float4* e4 = reinterpret_cast<const float4*>(s_code + t * kLd);   // broadcast reads
+        float dot = 0.f;
+#pragma unroll
+        for (int v = 0; v < kV; ++v) {
+          const float4 e = e4[v];
+          dot = fmaf(zv[4 * v], e.x, dot); dot = fmaf(zv[4 * v + 1], e.y, dot);
+          dot = fmaf(zv[4 * v + 2], e.z, dot); dot = fmaf(zv[4 * v + 3], e.w, dot);
+        }
+        const float d = (zz + s_ee[t]) - 2.0f * dot;
+        if (d < bestd) { bestd = d; best = j0 + t; }           // strict <: the first minimum wins, like torch.argmin
+      }
+    }
+  }
+  __syncthreads();                                             // s_w / s_b staged (no chunk loop without quantize)
+  if (!live) return;
+  // q overwrites z in registers: the code row, the given code's row (NaN when out of range) or z itself
+  if (p.idx_in) {
+    const int code = p.idx_in[i];
+    const bool ok = code >= 0 && code < p.n_e;
+#pragma unroll
+    for (int c = 0; c < E; ++c) zv[c] = ok ? p.codebook[(long long)code * E + c] : __int_as_float(0x7fc00000);
+  } else if (p.quantize) {
+#pragma unroll
+    for (int c = 0; c < E; ++c) zv[c] = p.codebook[(long long)best * E + c];
+  }
+  if (p.idx_out) p.idx_out[i] = p.quantize ? best : -1;
+  uint4* o = reinterpret_cast<uint4*>(p.out + i * cpad);
+  for (int co0 = 0; co0 < cpad; co0 += 8) {
+    float acc[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) acc[j] = s_b[co0 + j];
+#pragma unroll
+    for (int c = 0; c < E; ++c) {
+#pragma unroll
+      for (int j = 0; j < 8; ++j) acc[j] = fmaf(__half2float(s_w[(co0 + j) * E + c]), zv[c], acc[j]);
+    }
+    uint4 u;
+    __half* h = reinterpret_cast<__half*>(&u);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) h[j] = __float2half_rn(co0 + j < p.Cz ? acc[j] : 0.f);
+    o[co0 / 8] = u;
+  }
 }
 
 // ------------------------------------------------------------------------------------------------

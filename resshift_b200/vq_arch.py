@@ -16,6 +16,11 @@ from typing import Dict, List, Sequence, Tuple
 import torch
 
 
+def latent_channels_ok(c: int) -> bool:
+    """Latent widths (z_channels, embed_dim) the first stage runs: 1..8, or a multiple of 8 from 16 to 64."""
+    return 1 <= c <= 8 or (c % 8 == 0 and 16 <= c <= 64)
+
+
 @dataclass
 class VQConfig:
     """``autoencoder.params`` of the shipped yaml files (embed_dim, n_embed, ddconfig.*)."""
@@ -45,6 +50,10 @@ class VQConfig:
         self.resamp_with_conv, self.tanh_out = bool(self.resamp_with_conv), bool(self.tanh_out)
         assert self.double_z == self.kl
         assert len(self.num_res_blocks) == len(self.ch_mult)
+        for what, c in (("z_channels", self.z_channels), ("embed_dim", self.embed_dim)):
+            if not latent_channels_ok(c):
+                raise ValueError(f"{what} must be 1..8 or a multiple of 8 from 16 to 64, got {c}: the first-stage kernels "
+                                 "run latents of up to 8 channels, and wider ones as whole 16-byte fp16 rows up to 64")
         if self.attn_type in ("linear", "memory-efficient-cross-attn"):
             raise ValueError(f"attn_type {self.attn_type!r}: the reference's make_attn raises NotImplementedError for it "
                              "(ldm/modules/diffusionmodules/model.py:280-298), so no checkpoint of it exists")
@@ -125,6 +134,25 @@ def kl_preset(name: str) -> VQConfig:
     if name == "tiny":                                  # the VQ "tiny" topology with a KL bottleneck
         return VQConfig(embed_dim=4, z_channels=4, resolution=64, ch=32, ch_mult=(1, 2, 4), num_res_blocks=(1, 2, 2),
                         double_z=True, kl=True)
+    if name == "f16":                                   # LDM's kl-f16 (16-channel latent)
+        return VQConfig(embed_dim=16, z_channels=16, resolution=256, ch=128, ch_mult=(1, 1, 2, 2, 4), num_res_blocks=2,
+                        attn_resolutions=(16,), double_z=True, kl=True)
+    if name == "f32":                                   # LDM's kl-f32 (64-channel latent)
+        return VQConfig(embed_dim=64, z_channels=64, resolution=256, ch=128, ch_mult=(1, 1, 2, 2, 4, 4), num_res_blocks=2,
+                        attn_resolutions=(16, 8), double_z=True, kl=True)
+    if name in ("tiny16", "tiny64"):                    # the "tiny" topology with a 16- / 64-channel latent
+        c = int(name[4:])
+        return VQConfig(embed_dim=c, z_channels=c, resolution=64, ch=32, ch_mult=(1, 2, 4), num_res_blocks=(1, 2, 2),
+                        double_z=True, kl=True)
+    raise KeyError(name)
+
+
+def wide_vq_preset(name: str) -> VQConfig:
+    """VQ first stages with 16- or 64-channel latents on the "tiny" topology (test configurations)."""
+    if name in ("tiny16", "tiny64"):
+        c = int(name[4:])
+        return VQConfig(embed_dim=c, n_embed=512, z_channels=c, resolution=64, ch=32, ch_mult=(1, 2, 4),
+                        num_res_blocks=(1, 2, 2))
     raise KeyError(name)
 
 
