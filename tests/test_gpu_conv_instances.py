@@ -130,34 +130,52 @@ class Conv:
                                            ("reduce" if info["splitk"] > 1 else "staged"))))
         return (o32 if out_f32 else out[..., oc0:oc0 + self.Cout]), info
 
-    def ref(self):
-        """float64 (output NHWC, mag NHWC) of the layer."""
-        if self._ref is None:
+    def ref(self, rows=None):
+        """float64 (output NHWC, mag NHWC) of the layer; with rows (a 1-D index tensor), of those output rows of every
+        image only, each computed from the k input rows it reads (zero rows outside the map)."""
+        if rows is None and self._ref is not None:
+            return self._ref
+        wq = self.w.half().double()
+        pt = 0 if (self.stride == 2 and self.pad_lo == 0) else self.k // 2     # input rows / columns before the first
+        if rows is None:
             x = self.x[..., :self.Cin].permute(0, 3, 1, 2).double()
-            wq = self.w.half().double()
+        else:                                           # [N * R, Cin, k, W]: one k-row slab per output row
+            idx = rows.to(self.x.device)[:, None] * self.stride - pt + torch.arange(self.k, device=self.x.device)
+            keep = ((idx >= 0) & (idx < self.H)).double()
+            x = self.x[:, idx.clamp(0, self.H - 1), :, :self.Cin].double() * keep[None, :, :, None, None]
+            x = x.permute(0, 1, 4, 2, 3).reshape(-1, self.Cin, self.k, self.W)
 
-            def conv(a, b):
-                if self.stride == 2 and self.pad_lo == 0:          # the VQ-GAN Downsample: pad (0, 1, 0, 1), no conv padding
-                    return F.conv2d(F.pad(a, (0, 1, 0, 1)), b, stride=2)
-                return F.conv2d(a, b, stride=self.stride, padding=self.k // 2)
-            y, mag = conv(x, wq), conv(x.abs(), wq.abs())
-            if self.brows is not None:
-                y = y + self.brows.double()[:, :, None, None]
-                mag = mag + self.brows.double().abs()[:, :, None, None]
-            if self.act == 1:
-                y, mag = F.gelu(y), mag * ACT_GAIN
-            elif self.act == 2:
-                y, mag = F.silu(y), mag * ACT_GAIN
-            if self.res is not None:
-                r = self.res.permute(0, 3, 1, 2).double()
-                y, mag = y + r, mag + r.abs()
-            self._ref = (y.permute(0, 2, 3, 1), mag.permute(0, 2, 3, 1))
-        return self._ref
+        def conv(a, b):
+            if self.stride == 2 and self.pad_lo == 0:          # the VQ-GAN Downsample: pad (0, 1, 0, 1), no conv padding
+                return F.conv2d(F.pad(a, (0, 1, 0, 0 if rows is not None else 1)), b, stride=2)
+            if rows is not None:
+                return F.conv2d(F.pad(a, (pt, pt)), b, stride=self.stride)
+            return F.conv2d(a, b, stride=self.stride, padding=self.k // 2)
+        y, mag = conv(x, wq), conv(x.abs(), wq.abs())
+        if rows is not None:                            # [N * R, Cout, 1, Wo] -> [N, Cout, R, Wo]
+            y, mag = (t.reshape(self.N, -1, self.Cout, self.Wo).permute(0, 2, 1, 3) for t in (y, mag))
+        if self.brows is not None:
+            y = y + self.brows.double()[:, :, None, None]
+            mag = mag + self.brows.double().abs()[:, :, None, None]
+        if self.act == 1:
+            y, mag = F.gelu(y), mag * ACT_GAIN
+        elif self.act == 2:
+            y, mag = F.silu(y), mag * ACT_GAIN
+        if self.res is not None:
+            r = (self.res if rows is None else self.res[:, rows.to(self.res.device)]).permute(0, 3, 1, 2).double()
+            y, mag = y + r, mag + r.abs()
+        out = (y.permute(0, 2, 3, 1), mag.permute(0, 2, 3, 1))
+        if rows is None:
+            self._ref = out
+        return out
 
-    def check(self, tag, got, f32=False):
-        ref, mag = self.ref()
+    def check(self, tag, got, f32=False, rows=None):
+        """got against the float64 bound, on every element or on the output rows `rows` of every image."""
+        ref, mag = self.ref(rows)
         if f32:
             got = got.permute(0, 2, 3, 1)
+        if rows is not None:
+            got = got[:, rows.to(got.device)]
         return G.assert_within(tag, got, ref, mag, KAPPA, fp16=not f32)
 
 
@@ -182,9 +200,10 @@ def _box(Ho, Wo):
     return bw, bh, 128 // (bw * bh), (Wo // bw) * (Ho // bh)
 
 
-def _run(tag, L, want=None, stats=True, **kw):
-    """Two launches of layer L: bit-identical outputs and statistics, info as wanted, output within the bound, the
-    statistics of each sink against the stored output.  Returns (output, sink buffers, info)."""
+def _run(tag, L, want=None, stats=True, rows=None, **kw):
+    """Two launches of layer L: bit-identical outputs and statistics, info as wanted, output within the bound (on the
+    output rows `rows` only, if given), the statistics of each sink against the stored output.  Returns (output, sink
+    buffers, info)."""
     bw, bh, box_n, slots = _box(L.Ho, L.Wo)
     stats = stats and box_n <= 2 and not kw.get("out_f32")
     runs = []
@@ -200,7 +219,7 @@ def _run(tag, L, want=None, stats=True, **kw):
     assert (info["bw"], info["bh"], info["box_n"], info["gn_slots"]) == (bw, bh, box_n, slots), info
     for k, v in (want or {}).items():
         assert info[k] == v, f"{tag}: launched {k} = {info[k]}, wanted {v} ({info})"
-    L.check(f"{tag} {info}", out, f32=bool(kw.get("out_f32")))
+    L.check(f"{tag} {info}", out, f32=bool(kw.get("out_f32")), rows=rows)
     for i, (part, cstride, coff) in enumerate(sinks):
         G.check_slot_pairs(f"{tag} sink {i}", part, out, bw, bh, slots, cstride, coff)
     return out, parts, info

@@ -80,16 +80,16 @@ def _boxes(x, bh, bw):
 
 
 def _data(kind, N, H, W, Cc, g):
-    """float64 [N, H, W, C] of fp16-representable values."""
-    x = torch.randn(N, H, W, Cc, generator=g, dtype=torch.float64)
-    grp = torch.arange(Cc) // (Cc // 32)
+    """float64 [N, H, W, C] of fp16-representable values, on the generator's device."""
+    x = torch.randn(N, H, W, Cc, generator=g, dtype=torch.float64, device=g.device)
+    grp = torch.arange(Cc, device=g.device) // (Cc // 32)
     if kind == "randn":
         x = x * 2 + 0.5
     elif kind == "large_mean":            # per-group mean +-30, std 0.5
         x = x * 0.5 + torch.where(grp % 2 == 0, 30.0, -30.0).double()
     elif kind == "constant":              # groups exactly constant (rstd set by eps), near-constant, and ordinary
         base = torch.where(grp % 2 == 0, 30.0, -0.75).double().expand(N, H, W, Cc).clone()
-        near = base + torch.randint(-1, 2, (N, H, W, Cc), generator=g).double() * 2.0 ** -6
+        near = base + torch.randint(-1, 2, (N, H, W, Cc), generator=g, device=g.device).double() * 2.0 ** -6
         x = torch.where((grp % 3 == 0), base, torch.where(grp % 3 == 1, near, x))
     elif kind == "outlier":               # one value 300 in every group of every image
         x = x.clone()
@@ -107,44 +107,51 @@ def _data(kind, N, H, W, Cc, g):
 
 class Case:
     """One GroupNorm launch: fp16 input view (channel slice of a wider row when padded), gamma, beta, optional FiLM
-    rows inside a wider embedding row (per image, or one shared row), and the float64 reference."""
+    rows inside a wider embedding row (per image, or one shared row), and the float64 reference.  The data and the
+    reference live on `device` (the CPU unless given; "cuda" for maps whose float64 reference is too slow there)."""
 
-    def __init__(self, N, H, W, Cc, eps=1e-5, silu=0, film=None, pad=False, kind="randn", seed=0):
-        g = torch.Generator().manual_seed(seed)
+    def __init__(self, N, H, W, Cc, eps=1e-5, silu=0, film=None, pad=False, kind="randn", seed=0, device="cpu"):
+        g = torch.Generator(device=device).manual_seed(seed)
+        self.dev = g.device
         self.N, self.H, self.W, self.C, self.eps, self.silu, self.film_kind = N, H, W, Cc, eps, silu, film
         self.x64 = _data(kind, N, H, W, Cc, g)
         self.xc0, self.x_ld = (8, Cc + 24) if pad else (0, Cc)
         self.yc0, self.y_ld = (16, Cc + 40) if pad else (0, Cc)
-        xbuf = (torch.randn(N, H, W, self.x_ld, generator=g) * 1e4).half()       # what lies outside the view
+        xbuf = (torch.randn(N, H, W, self.x_ld, generator=g, device=g.device) * 1e4).half()   # what lies outside the view
         xbuf[..., self.xc0:self.xc0 + Cc] = self.x64.half()
         self.xbuf = xbuf.cuda()
-        self.gamma = (1 + 0.2 * torch.randn(Cc, generator=g)).float()
-        self.beta = (0.2 * torch.randn(Cc, generator=g)).float()
+        self.gamma = (1 + 0.2 * torch.randn(Cc, generator=g, device=g.device)).float()
+        self.beta = (0.2 * torch.randn(Cc, generator=g, device=g.device)).float()
         self.film_off, self.film_sN, self.fbuf = 0, 0, None
         if film is not None:              # this layer's [2C] slice at offset film_off of rows film_sN apart
             self.film_off = 24
             self.film_sN = self.film_off + 2 * Cc + 40 if film == "image" else 0
             rows = N if film == "image" else 1
-            self.fbuf = (0.3 * torch.randn(rows * max(self.film_sN, self.film_off + 2 * Cc), generator=g)).float()
-        self._ref = None
+            self.fbuf = (0.3 * torch.randn(rows * max(self.film_sN, self.film_off + 2 * Cc), generator=g,
+                                           device=g.device)).float()
+        self._ref = self._stats = None
 
     def film_rows(self):
         """float64 (scale, shift) [N, C] or None."""
         if self.fbuf is None:
             return None
         f = self.fbuf.double()
-        idx = self.film_off + torch.arange(self.N)[:, None] * self.film_sN + torch.arange(self.C)[None]
+        idx = self.film_off + torch.arange(self.N, device=self.dev)[:, None] * self.film_sN + torch.arange(self.C, device=self.dev)[None]
         return f[idx], f[idx + self.C]
 
     def group_stats(self):
         """float64 group mean, biased variance, std [N, 32]."""
-        t = self.x64.reshape(self.N, -1, 32, self.C // 32).permute(0, 2, 1, 3).reshape(self.N, 32, -1)
-        mu, var = t.mean(-1), t.var(-1, unbiased=False)
-        return mu, var, var.sqrt()
+        if self._stats is None:
+            t = self.x64.reshape(self.N, -1, 32, self.C // 32)          # (a view: no copy of a large map)
+            mu = t.mean((1, 3))
+            var = ((t - mu[:, None, :, None]) ** 2).mean((1, 3))
+            self._stats = (mu, var, var.sqrt())
+        return self._stats
 
-    def ref(self):
-        """float64 (y, y before SiLU, a, b) as [N, H, W, C], [N, C], [N, C]."""
-        if self._ref is None:
+    def ref(self, rows=None):
+        """float64 (y, y before SiLU, a, b) as [N, H, W, C], [N, C], [N, C]; with rows (a 1-D index tensor), y of those
+        rows of every image only, [N, R, W, C]."""
+        if self._ref is None or rows is not None:
             mu, var, _ = self.group_stats()
             r = 1.0 / (var + self.eps).sqrt()
             cpg = self.C // 32
@@ -155,14 +162,17 @@ class Case:
             fr = self.film_rows()
             if fr is not None:
                 a, b = a * (1 + fr[0]), b * (1 + fr[0]) + fr[1]
-            x = self.x64
-            # the module's own reference op on the same values, as a cross-check of the affine form above
-            yg = F.group_norm(x.permute(0, 3, 1, 2), 32, gm[0], bt[0], eps=self.eps).permute(0, 2, 3, 1)
-            if fr is not None:
-                yg = yg * (1 + fr[0][:, None, None]) + fr[1][:, None, None]
+            x = self.x64 if rows is None else self.x64[:, rows.to(self.dev)]
             lin = x * a[:, None, None] + b[:, None, None]
-            assert (yg - lin).abs().max().item() <= 1e-9 * (1 + lin.abs().max().item())
+            if rows is None:
+                # the module's own reference op on the same values, as a cross-check of the affine form above
+                yg = F.group_norm(x.permute(0, 3, 1, 2), 32, gm[0], bt[0], eps=self.eps).permute(0, 2, 3, 1)
+                if fr is not None:
+                    yg = yg * (1 + fr[0][:, None, None]) + fr[1][:, None, None]
+                assert (yg - lin).abs().max().item() <= 1e-9 * (1 + lin.abs().max().item())
             y = F.silu(lin) if self.silu else lin
+            if rows is not None:
+                return (y, lin, a, b)
             self._ref = (y, lin, a, b)
         return self._ref
 
@@ -237,7 +247,7 @@ class Case:
     def check_gstat(self, tag, route, gs):
         mu, var, sd = self.group_stats()
         r = 1.0 / (var + self.eps).sqrt()
-        gs = gs.double().cpu()
+        gs = gs.double().to(self.dev)
         assert torch.isfinite(gs).all(), f"{tag}: gstat not written"
         e_mu = ((gs[..., 0] - mu).abs() / (U * (mu.abs() + sd)).clamp(min=1e-300)).max().item()
         e_r = ((gs[..., 1] / r - 1).abs() / U).max().item()
@@ -251,7 +261,7 @@ class Case:
         dev = t - m[:, :, None]
         m2 = (dev ** 2).sum(2)
         maxdev = dev.abs().amax(2)
-        p = part.double().cpu()
+        p = part.double().to(self.dev)
         assert torch.isfinite(p).all(), f"{tag}: pairs not written"
         e_m = ((p[..., 0] - m).abs() / (U * (m.abs() + maxdev)).clamp(min=1e-300)).max().item()
         e_q = ((p[..., 1] - m2).abs() / (U * (m2 + t.shape[2] * maxdev ** 2)).clamp(min=1e-300)).max().item()
@@ -259,41 +269,45 @@ class Case:
         _note(route, "pair_m2", e_q / K_Q)
         assert e_m <= K_MU and e_q <= K_Q, f"{tag}: pair mean error {e_m:.1f} U, M2 error {e_q:.1f} U"
 
-    def check_y(self, tag, route, y):
-        ref, lin, a, b = self.ref()
+    def check_y(self, tag, route, y, rows=None):
+        """y against the float64 bound, on every element or on the rows `rows` of every image (the apply is local)."""
+        ref, lin, a, b = self.ref(rows)
         mu, _, sd = self.group_stats()
         cpg = self.C // 32
         mu_c, sd_c = mu.repeat_interleave(cpg, 1)[:, None, None], sd.repeat_interleave(cpg, 1)[:, None, None]
         x = self.x64
+        if rows is not None:
+            x, y = x[:, rows.to(self.dev)], y[:, rows.to(y.device)]
         A, B = a[:, None, None], b[:, None, None]
         gain = 1.1 if self.silu else 1.0
         allow = gain * (K_FOLD * U * ((x * A).abs() + B.abs()) + A.abs() * K_MU * U * (mu_c.abs() + sd_c)
                         + (A * (x - mu_c)).abs() * K_R * U)
         tol = G.ulp16(ref.abs() + allow) + allow
-        err = (y.double().cpu() - ref).abs()
+        err = (y.double().to(self.dev) - ref).abs()
         ratio = (err / tol).max().item()
         _note(route, "y", ratio)
         bad = ~(err <= tol)
         assert not bad.any(), f"{tag}: {int(bad.sum())} of {bad.numel()} outside the bound (worst {ratio:.2f} of it)"
         if not self.silu:
-            self.check_implied(tag, route, y, (K_FOLD * U * ((x * A).abs() + B.abs())))
+            self.check_implied(tag, route, y, (K_FOLD * U * ((x * A).abs() + B.abs())), x)
 
-    def check_implied(self, tag, route, y, fold):
+    def check_implied(self, tag, route, y, fold, x=None):
         """Group mean and rstd implied by the output: with A = gamma (1 + scale), B = beta (1 + scale) + shift,
-        y' = (y - B) / A = rstd (x - mean); least squares per group."""
+        y' = (y - B) / A = rstd (x - mean); least squares per group, over the elements of x (all of them unless given)
+        and y."""
         N, cpg = self.N, self.C // 32
         A, B = self.gamma.double()[None].expand(N, -1), self.beta.double()[None].expand(N, -1)
         fr = self.film_rows()
         if fr is not None:
             A, B = A * (1 + fr[0]), B * (1 + fr[0]) + fr[1]
         A, B = A[:, None, None], B[:, None, None]
-        yd = y.double().cpu()
+        yd = y.double().to(self.dev)
         u = (0.5 * G.ulp16(yd) + fold) / A.abs()
         yp = (yd - B) / A
 
         def grp(t):
             return t.reshape(N, -1, 32, cpg).permute(0, 2, 1, 3).reshape(N, 32, -1)
-        x, yp, u = grp(self.x64), grp(yp), grp(u)
+        x, yp, u = grp(self.x64 if x is None else x), grp(yp), grp(u)
         n = x.shape[-1]
         xm = x.mean(-1, keepdim=True)
         dx = x - xm
@@ -313,13 +327,13 @@ class Case:
             assert e_r.max().item() <= 1 and e_mu.max().item() <= 1, \
                 f"{tag}: implied statistics off (rstd {e_r.max().item():.2f}, mean {e_mu.max().item():.2f} of the bound)"
 
-    def check(self, tag, route, out):
+    def check(self, tag, route, out, rows=None):
         y, info, gs, part = out
         if gs is not None:
             self.check_gstat(tag, route, gs)
         if route.startswith("stats"):
             self.check_stats_pairs(tag, route, part, info)
-        self.check_y(tag, route, y)
+        self.check_y(tag, route, y, rows)
 
 
 # ---------------------------------------------------------------------------------------------- a. route matrix

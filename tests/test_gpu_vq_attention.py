@@ -5,7 +5,8 @@ x4 pipeline on a 128x128 LQ tile (a 512x512 image, a 128x128 bottleneck).
 The operator tests hold it per element to float64 (the bound of tests/test_gpu_attention.py); the plan references run
 in fp32 with TF32 off.  The oracle's attention is evaluated in chunks of query rows here (rows are
 independent: the same math without the T x T temporaries, which are 17 GB each in fp32 at T = 65536).
-Tolerances are the repository's: max|d| <= 1e-2, mean|d| <= 2e-3.
+Tolerances are the repository's: max|d| <= 1e-2, mean|d| <= 2e-3.  The default CLI tile (T = 262144, the 2048x2048
+encode and decode) is held to float64 and to the oracle by test_gpu_cli_tile.py.
 """
 import ctypes as C
 
