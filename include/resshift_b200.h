@@ -231,6 +231,38 @@ size_t rs_sampler_staging_bytes(const rs_sampler* s);
  * [T, B, C, H, W] fp32 device buffers or NULL */
 int rs_sampler_set_taps(rs_sampler* s, float* pred_xstart_steps, float* sample_steps);
 
+/* ---- DDPM / DDIM sampler: SpacedDiffusionDDPM.p_sample_loop / ddim_sample_loop (reference
+ *      models/gaussian_diffusion.py:742-1147, models/respace.py:65-99) on the same plan and entry points -------------
+ * x_T = noises[0] (no shift), then T x (denoiser forward on x_t unscaled + one step kernel).  The schedule comes in as
+ * the process's float64 tables, rows of `steps` values in the order of rs_ddpm_table_row; the library rounds each to
+ * fp32 (_extract_into_tensor) and keeps the log variance of options->var_type.  rs_sampler_run / _run_host / _set_taps /
+ * _destroy work unchanged; z_y is not read and may be NULL.  rs_sampler_tables refuses these samplers. */
+typedef enum rs_ddpm_kind { RS_DDPM_ANCESTRAL = 0, RS_DDPM_DDIM = 1 } rs_ddpm_kind;
+typedef enum rs_ddpm_var_type { RS_VAR_FIXED_LARGE = 0, RS_VAR_FIXED_SMALL = 1 } rs_ddpm_var_type;
+typedef enum rs_ddpm_table_row {
+  RS_DDPM_SQRT_RECIP_ACP = 0,       /* sqrt(1 / alphas_cumprod)                                               */
+  RS_DDPM_SQRT_RECIPM1_ACP = 1,     /* sqrt(1 / alphas_cumprod - 1)                                           */
+  RS_DDPM_COEF1 = 2,                /* posterior_mean_coef1 (multiplies x0)                                   */
+  RS_DDPM_COEF2 = 3,                /* posterior_mean_coef2 (multiplies x_t)                                  */
+  RS_DDPM_LOGVAR_LARGE = 4,         /* log(append(posterior_variance[1], betas[1:]))  (FIXED_LARGE)           */
+  RS_DDPM_LOGVAR_SMALL = 5,         /* posterior_log_variance_clipped                  (FIXED_SMALL)          */
+  RS_DDPM_ACP = 6,                  /* alphas_cumprod                                                         */
+  RS_DDPM_ACP_PREV = 7,             /* alphas_cumprod_prev                                                    */
+  RS_DDPM_TABLE_ROWS = 8
+} rs_ddpm_table_row;
+typedef struct rs_ddpm_options {
+  int32_t kind;               /* RS_DDPM_ANCESTRAL or RS_DDPM_DDIM                                         */
+  int32_t mean_type;          /* RS_MEAN_EPSILON or RS_MEAN_XSTART                                         */
+  int32_t var_type;           /* RS_VAR_FIXED_LARGE / _SMALL: the ancestral step's noise; DDIM ignores it */
+  int32_t clip;               /* 1: clamp x0 to [-1, 1] (clip_denoised)                                    */
+  double eta;                 /* DDIM's eta >= 0 (the ancestral step ignores it)                           */
+} rs_ddpm_options;
+/* tables_host [RS_DDPM_TABLE_ROWS][steps] float64; timestep_map_host [steps] (the model's timesteps; NULL = 0 .. T-1).
+ * Refused, each with its reason: NULL tables or options, an unknown kind / var_type, a mean type other than eps or x0,
+ * clip other than 0 / 1, a negative or non-finite eta, steps outside [2, the plan's FiLM rows]. */
+int rs_ddpm_sampler_create(rs_plan* p, int steps, const double* tables_host, const int32_t* timestep_map_host,
+                           const rs_ddpm_options* options, rs_sampler** out);
+
 /* ---- VQ-GAN first stage: ldm.models.autoencoder.VQModelTorch (reference ldm/models/autoencoder.py:12-47) -------
  * The engine handle is the same opaque type as the denoiser's: rs_unet_param_count / _param_info / _arena_bytes /
  * _set_arena / _load_param work on it unchanged (state_dict names and shapes of the reference's VQModelTorch, so
@@ -355,6 +387,24 @@ typedef struct rs_p_sample_pred_args {
   float* x0_out;                                /* optional [N, C, HW] fp32                                            */
 } rs_p_sample_pred_args;
 int rs_op_p_sample_pred(const rs_p_sample_pred_args* a, void* stream);
+/* The DDPM sampler's step kernel (rs_ddpm_sampler_create) on its own: x0 from the model output (eps or x0, clamped
+ * with clip), then the ancestral or DDIM update, with the grid the loop launches.  Tables are [T] fp32 device arrays:
+ * the ancestral step reads coef1, coef2 and log_var, DDIM acp and acp_prev, eps prediction (and DDIM) sqrt_recip_acp
+ * and sqrt_recipm1_acp.  next_in (t > 0 only) receives fp16(x_next) in channels [0, C); counters as in
+ * rs_op_p_sample_ex; x0_out (optional) receives x0.  Refused: a table the step reads missing, an unknown kind or mean
+ * type, clip other than 0 / 1, a negative eta, t outside [0, T), next_cpad < C, more counters than launched threads. */
+typedef struct rs_ddpm_step_args {
+  const float* out; const float* x_t; const float* noise; float* x_next;                     /* [N, C, HW] fp32       */
+  const float* sqrt_recip_acp; const float* sqrt_recipm1_acp;                                /* [T] fp32 device tables */
+  const float* coef1; const float* coef2; const float* log_var; const float* acp; const float* acp_prev;
+  int32_t T, t, N, C, HW;
+  int32_t kind, mean_type, clip;
+  float eta;
+  void* next_in; int32_t next_cpad;
+  uint32_t* counters; int32_t n_counters;
+  float* x0_out;
+} rs_ddpm_step_args;
+int rs_op_ddpm_step(const rs_ddpm_step_args* a, void* stream);
 /* The denoiser's input packing: out[N*HW][Cpad] fp16 = cat([fp16(x * scale_tab[scale_idx]), lq, mask], channels) + zero
  * padding (scale 1 without scale_tab).  lq is one of: lq_nchw [N, Cl, HW] fp32 (optionally followed by mask_nchw
  * [N, 1, HW]); lq_nchw [N, Cl / 4, 2H, 2W] packed as pixel_unshuffle(lq, 2) (lq_unshuffle, W = the latent width); the

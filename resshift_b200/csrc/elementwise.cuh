@@ -284,6 +284,83 @@ __global__ void prior_sample_kernel(const float* __restrict__ zy, const float* _
 }
 
 // ------------------------------------------------------------------------------------------------
+// DDPM / DDIM steps of GaussianDiffusionDDPM (reference models/gaussian_diffusion.py:742-1028), fp32 NCHW in/out:
+//   x0       = sqrt_recip_acp[t] x_t - sqrt_recipm1_acp[t] eps (_predict_xstart_from_eps :838-843), or the model
+//              output itself for x0 prediction; clamped to [-1, 1] with clip (process_xstart :803-808)
+//   ancestral  mean = coef1[t] x0 + coef2[t] x_t (q_posterior_mean_variance :726-729);
+//              x_{t-1} = mean + [t != 0] exp(0.5 log_variance[t]) noise (p_sample :887-891)
+//   DDIM       eps' = (sqrt_recip_acp[t] x_t - x0) / sqrt_recipm1_acp[t] (_predict_eps_from_xstart :855-859);
+//              sigma = eta sqrt((1 - acp_prev) / (1 - acp)) sqrt(1 - acp / acp_prev);
+//              x_{t-1} = x0 sqrt(acp_prev) + sqrt(1 - acp_prev - sigma^2) eps' + [t != 0] sigma noise (ddim_sample
+//              :1010-1027)
+// Every operation is the reference's fp32 tensor operation on the fp32 table values (_extract_into_tensor), in its
+// order and rounded on its own (no FMA contraction); the [t != 0] factor multiplies as the reference's nonzero_mask does.
+// The denoiser sees x_t unscaled (_scale_input is the identity, :1213-1214): next_in receives fp16(x_{t-1}).
+// ------------------------------------------------------------------------------------------------
+enum DdpmKind : int { kDdpmAncestral = 0, kDdpmDdim = 1 };
+
+struct DdpmStepParams {
+  const float* x_t;       // [N, C, HW]
+  const float* out;       // [N, C, HW]: the model output (eps or x0)
+  const float* noise;     // [N, C, HW]
+  float* x_next;          // [N, C, HW]
+  const float* sqrt_recip_acp; const float* sqrt_recipm1_acp;     // [T] fp32 tables
+  const float* coef1; const float* coef2; const float* log_var;    // [T] (ancestral)
+  const float* acp; const float* acp_prev;                         // [T] (DDIM)
+  float eta;              // DDIM
+  int clip;
+  int t;                  // schedule index of THIS step (T-1 .. 0)
+  int N, C, HW;
+  __half* next_in; int next_cpad;     // optional: [N*HW, next_cpad]; channels [0, C) are written here
+  unsigned int* zero_ptr; int zero_n; // GroupNorm arrival counters of the NEXT denoiser forward: reset here
+  float* x0_out;                      // optional [N, C, HW]: pred_xstart
+};
+
+template <int KIND, int MT>
+__global__ void ddpm_step_kernel(const DdpmStepParams p) {
+  pdl_trigger();
+  pdl_wait();
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < p.zero_n) p.zero_ptr[i] = 0u;
+  const long long total = (long long)p.N * p.C * p.HW;
+  if (i >= total) return;
+  const int t = p.t;
+  const float xt = p.x_t[i];
+  const float nonzero = t != 0 ? 1.0f : 0.0f;
+  float x0;
+  if constexpr (MT == kMeanEpsilon) {
+    x0 = __fsub_rn(__fmul_rn(p.sqrt_recip_acp[t], xt), __fmul_rn(p.sqrt_recipm1_acp[t], p.out[i]));
+  } else {
+    static_assert(MT == kMeanXstart, "DDPM steps predict eps or x0");
+    x0 = p.out[i];
+  }
+  if (p.clip) x0 = x0 < -1.0f ? -1.0f : (x0 > 1.0f ? 1.0f : x0);     // clamp(-1, 1): NaN stays NaN
+  if (p.x0_out) p.x0_out[i] = x0;
+  float v;
+  if constexpr (KIND == kDdpmAncestral) {
+    const float mean = __fadd_rn(__fmul_rn(p.coef1[t], x0), __fmul_rn(p.coef2[t], xt));
+    const float sd = expf(__fmul_rn(0.5f, p.log_var[t]));
+    v = __fadd_rn(mean, __fmul_rn(__fmul_rn(nonzero, sd), p.noise[i]));
+  } else {
+    static_assert(KIND == kDdpmDdim, "unknown DDPM step");
+    const float ab = p.acp[t], abp = p.acp_prev[t];
+    const float eps = __fdiv_rn(__fsub_rn(__fmul_rn(p.sqrt_recip_acp[t], xt), x0), p.sqrt_recipm1_acp[t]);
+    const float sigma = __fmul_rn(__fmul_rn(p.eta, __fsqrt_rn(__fdiv_rn(__fsub_rn(1.0f, abp), __fsub_rn(1.0f, ab)))),
+                                  __fsqrt_rn(__fsub_rn(1.0f, __fdiv_rn(ab, abp))));
+    const float mean = __fadd_rn(__fmul_rn(x0, __fsqrt_rn(abp)),
+                                 __fmul_rn(__fsqrt_rn(__fsub_rn(__fsub_rn(1.0f, abp), __fmul_rn(sigma, sigma))), eps));
+    v = __fadd_rn(mean, __fmul_rn(__fmul_rn(nonzero, sigma), p.noise[i]));
+  }
+  p.x_next[i] = v;
+  if (p.next_in && t > 0) {
+    const int hw = (int)(i % p.HW);
+    const int c = (int)((i / p.HW) % p.C);
+    const int n = (int)(i / ((long long)p.HW * p.C));
+    p.next_in[((long long)n * p.HW + hw) * p.next_cpad + c] = __float2half_rn(v);
+  }
+}
+
+// ------------------------------------------------------------------------------------------------
 // Split-K finish: out = act(sum_s partial[s] + bias) + residual, fp16 NHWC view (or fp32 NCHW), plus the
 // GroupNorm partial statistics of the result.  One CTA per (128-pixel slot, image) — the same slots the
 // conv epilogue would have produced; splits are summed in a fixed order, statistics reduced in a fixed tree.

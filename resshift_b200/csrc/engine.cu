@@ -1,5 +1,5 @@
 // Engine: the Swin-UNet denoiser of ResShift as a static program of sm_90a kernel launches, plus the
-// residual-shift sampling loop, behind the C ABI declared in include/resshift_b200.h.
+// residual-shift and DDPM / DDIM sampling loops, behind the C ABI declared in include/resshift_b200.h.
 //
 // Topology restates UNetModelSwin.__init__/forward (reference models/unet.py:659-895), ResBlock
 // (:110-206), BasicLayer / SwinTransformerBlock (models/swin_transformer.py:163-281,348-442).
@@ -9,6 +9,8 @@
 //   * every tensor lives in one caller-owned workspace; lifetimes are resolved at plan time;
 //   * timestep embeddings (time_embed + all 22 emb_layers) are one small table computed by two tiny
 //     kernels; in the sampling loop the table for all T steps is computed once.
+#include <algorithm>
+#include <cmath>
 #include <map>
 #include <memory>
 #include <numeric>
@@ -1673,6 +1675,10 @@ struct rs_sampler {
   std::vector<float> eps_coef, eta, one_minus_eta;     // x0 conversions of the epsilon parameterisations
   float prior_coef = 0;
   rs_sampler_options opt{RS_MEAN_XSTART, 1, 1};
+  // DDPM / DDIM sampler (rs_ddpm_sampler_create): its options and fp32 tables, kDdpmDevRows rows of T
+  bool ddpm = false;
+  rs_ddpm_options dopt{};
+  std::vector<float> dtab;
   float* tap_pred = nullptr; float* tap_sample = nullptr;
   cudaGraphExec_t graph = nullptr;
   cudaStream_t cap_stream = nullptr;     // capture happens on a private stream (the legacy default stream cannot capture)
@@ -1699,8 +1705,65 @@ int launch_p_sample(int mean_type, const PSamplePredParams& pp, long long numel,
   return 0;
 }
 
+// the DDPM sampler's fp32 tables in the plan's table region, one 1024-entry row each: sqrt_recip_acp,
+// sqrt_recipm1_acp, coef1, coef2, the log variance of its var_type, acp, acp_prev
+constexpr int kDdpmDevRows = 7;
+
+void ddpm_tables(DdpmStepParams& dp, const float* tab, int ld) {
+  dp.sqrt_recip_acp = tab; dp.sqrt_recipm1_acp = tab + ld; dp.coef1 = tab + 2 * ld; dp.coef2 = tab + 3 * ld;
+  dp.log_var = tab + 4 * ld; dp.acp = tab + 5 * ld; dp.acp_prev = tab + 6 * ld;
+}
+
+// ddpm_step_kernel instance of (kind, mean type); unknown values are refused
+int launch_ddpm_step(int kind, int mean_type, const DdpmStepParams& dp, long long numel, cudaStream_t st) {
+  const dim3 grid((unsigned)((numel + 255) / 256)), block(256);
+  RS_CHECK(kind == RS_DDPM_ANCESTRAL || kind == RS_DDPM_DDIM,
+           "unknown DDPM sampler kind " + std::to_string(kind) + " (RS_DDPM_ANCESTRAL or RS_DDPM_DDIM)");
+  RS_CHECK(mean_type == RS_MEAN_EPSILON || mean_type == RS_MEAN_XSTART,
+           "DDPM steps predict eps or x0 (RS_MEAN_EPSILON or RS_MEAN_XSTART), got mean type " + std::to_string(mean_type));
+  const bool eps = mean_type == RS_MEAN_EPSILON;
+  if (kind == RS_DDPM_ANCESTRAL) {
+    if (eps) (void)launch_k(ddpm_step_kernel<kDdpmAncestral, kMeanEpsilon>, grid, block, (size_t)(0), st, dp);
+    else (void)launch_k(ddpm_step_kernel<kDdpmAncestral, kMeanXstart>, grid, block, (size_t)(0), st, dp);
+  } else {
+    if (eps) (void)launch_k(ddpm_step_kernel<kDdpmDdim, kMeanEpsilon>, grid, block, (size_t)(0), st, dp);
+    else (void)launch_k(ddpm_step_kernel<kDdpmDdim, kMeanXstart>, grid, block, (size_t)(0), st, dp);
+  }
+  return 0;
+}
+
+// x_T = noises[0]; then per step the denoiser on x_t (unscaled) and the DDPM / DDIM step
+int ddpm_enqueue(rs_sampler& S, const float* noises, const float* lq, const float* mask, float* out_latent,
+                 cudaStream_t st) {
+  rs_plan& P = *S.p;
+  const rs_unet_config& c = P.e->cfg;
+  RS_CHECK(c.in_channels == c.out_channels, "the sampler needs out_channels == in_channels (x0 and x_t share a shape)");
+  const long long numel = (long long)P.B * c.in_channels * P.H * P.W;
+  float* state = reinterpret_cast<float*>(P.ws + P.off_state);
+  int rc = pack_lq_and_input(P, noises, lq, mask, nullptr, 0, st); if (rc) return rc;
+  const float* film_all = reinterpret_cast<const float*>(P.ws + P.off_film);
+  for (int k = 0; k < S.T; ++k) {
+    const int t = S.T - 1 - k;
+    rc = run_ops(P, P.ops, film_all + (long long)t * P.e->film_rows, 0, st); if (rc) return rc;
+    DdpmStepParams dp{};
+    dp.x_t = k == 0 ? noises : state; dp.out = P.out_f32; dp.noise = noises + (long long)(k + 1) * numel;
+    dp.x_next = (t == 0) ? out_latent : state;
+    ddpm_tables(dp, reinterpret_cast<const float*>(P.ws + P.off_tables), 1024);
+    dp.eta = (float)S.dopt.eta; dp.clip = S.dopt.clip; dp.t = t;
+    dp.N = P.B; dp.C = c.in_channels; dp.HW = P.H * P.W;
+    dp.next_in = P.xin.ptr; dp.next_cpad = P.cin_pad;
+    dp.zero_ptr = reinterpret_cast<unsigned int*>(P.ws + P.off_counters); dp.zero_n = P.n_gn * P.B;
+    if (S.tap_pred) dp.x0_out = S.tap_pred + (long long)k * numel;
+    rc = launch_ddpm_step(S.dopt.kind, S.dopt.mean_type, dp, numel, st); if (rc) return rc;
+    if (S.tap_sample) RS_CUDA_OK(cudaMemcpyAsync(S.tap_sample + (long long)k * numel, dp.x_next, numel * 4, cudaMemcpyDeviceToDevice, st));
+  }
+  RS_CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
 int sampler_enqueue(rs_sampler& S, const float* z_y, const float* noises, const float* lq, const float* mask,
                     float* out_latent, cudaStream_t st) {
+  if (S.ddpm) return ddpm_enqueue(S, noises, lq, mask, out_latent, st);
   rs_plan& P = *S.p;
   const rs_unet_config& c = P.e->cfg;
   RS_CHECK(c.in_channels == c.out_channels, "the sampler needs out_channels == in_channels (x0, x_t and z_y share a shape)");
@@ -1743,11 +1806,16 @@ int sampler_prepare(rs_sampler& S, cudaStream_t st) {
   rs_plan& P = *S.p;
   if (P.table_owner == &S && P.table_epoch == P.e->weights_epoch) return 0;
   float* tab = reinterpret_cast<float*>(P.ws + P.off_tables);
-  RS_CUDA_OK(cudaMemcpyAsync(tab, S.coef1.data(), S.T * 4, cudaMemcpyHostToDevice, st));
-  RS_CUDA_OK(cudaMemcpyAsync(tab + 1024, S.coef2.data(), S.T * 4, cudaMemcpyHostToDevice, st));
-  RS_CUDA_OK(cudaMemcpyAsync(tab + 2048, S.stdv.data(), S.T * 4, cudaMemcpyHostToDevice, st));
-  RS_CUDA_OK(cudaMemcpyAsync(tab + 3072, S.in_scale.data(), S.T * 4, cudaMemcpyHostToDevice, st));
-  if (S.opt.mean_type != RS_MEAN_XSTART) {
+  if (S.ddpm) {
+    for (int r = 0; r < kDdpmDevRows; ++r)
+      RS_CUDA_OK(cudaMemcpyAsync(tab + r * 1024, S.dtab.data() + (size_t)r * S.T, S.T * 4, cudaMemcpyHostToDevice, st));
+  } else {
+    RS_CUDA_OK(cudaMemcpyAsync(tab, S.coef1.data(), S.T * 4, cudaMemcpyHostToDevice, st));
+    RS_CUDA_OK(cudaMemcpyAsync(tab + 1024, S.coef2.data(), S.T * 4, cudaMemcpyHostToDevice, st));
+    RS_CUDA_OK(cudaMemcpyAsync(tab + 2048, S.stdv.data(), S.T * 4, cudaMemcpyHostToDevice, st));
+    RS_CUDA_OK(cudaMemcpyAsync(tab + 3072, S.in_scale.data(), S.T * 4, cudaMemcpyHostToDevice, st));
+  }
+  if (!S.ddpm && S.opt.mean_type != RS_MEAN_XSTART) {
     RS_CUDA_OK(cudaMemcpyAsync(tab + 4096, S.eps_coef.data(), S.T * 4, cudaMemcpyHostToDevice, st));
     RS_CUDA_OK(cudaMemcpyAsync(tab + 5120, S.eta.data(), S.T * 4, cudaMemcpyHostToDevice, st));
     RS_CUDA_OK(cudaMemcpyAsync(tab + 6144, S.one_minus_eta.data(), S.T * 4, cudaMemcpyHostToDevice, st));
@@ -1830,8 +1898,42 @@ int rs_sampler_create(rs_plan* p, int steps, const double* sqrt_etas, double kap
   const rs_sampler_options opt{RS_MEAN_XSTART, 1, 1};
   return rs_sampler_create_ex(p, steps, sqrt_etas, kappa, tmap, &opt, out);
 }
+// DDPM / DDIM sampler: the process's float64 tables (rs_ddpm_table_row) rounded to fp32 as _extract_into_tensor does
+// (reference models/gaussian_diffusion.py:92-105); the log-variance row of the options' var_type (:788-801)
+int rs_ddpm_sampler_create(rs_plan* p, int steps, const double* tables, const int32_t* tmap, const rs_ddpm_options* o,
+                           rs_sampler** out) {
+  RS_CHECK(p && p->bound && out, "bad argument (plan must be bound)");
+  RS_CHECK(tables, "DDPM sampler: the schedule tables are NULL");
+  RS_CHECK(o, "DDPM sampler: the options are NULL");
+  RS_CHECK(p->pass == Pass::Denoiser, std::string("samplers are built on denoiser plans: this plan belongs to ") + kind_name(p->e->kind));
+  RS_CHECK(o->kind == RS_DDPM_ANCESTRAL || o->kind == RS_DDPM_DDIM,
+           "DDPM sampler: unknown kind " + std::to_string(o->kind) + " (RS_DDPM_ANCESTRAL or RS_DDPM_DDIM)");
+  RS_CHECK(o->mean_type == RS_MEAN_EPSILON || o->mean_type == RS_MEAN_XSTART,
+           "DDPM sampler: the model must predict eps or x0 (RS_MEAN_EPSILON or RS_MEAN_XSTART), got mean type " +
+           std::to_string(o->mean_type));
+  RS_CHECK(o->var_type == RS_VAR_FIXED_LARGE || o->var_type == RS_VAR_FIXED_SMALL,
+           "DDPM sampler: unknown variance type " + std::to_string(o->var_type) + " (RS_VAR_FIXED_LARGE or RS_VAR_FIXED_SMALL)");
+  RS_CHECK(o->clip == 0 || o->clip == 1, "DDPM sampler: clip must be 0 or 1, got " + std::to_string(o->clip));
+  RS_CHECK(std::isfinite(o->eta) && o->eta >= 0.0, "DDPM sampler: eta must be finite and >= 0, got " + std::to_string(o->eta));
+  RS_CHECK(steps >= 2 && steps <= p->max_rows && steps <= 1024,
+           "DDPM sampler: steps must be in [2, " + std::to_string(std::min(p->max_rows, 1024)) +
+           "] (the plan's FiLM-table rows), got " + std::to_string(steps));
+  auto s = std::make_unique<rs_sampler>();
+  s->p = p; s->T = steps; s->ddpm = true; s->dopt = *o;
+  const int rows[kDdpmDevRows] = {RS_DDPM_SQRT_RECIP_ACP, RS_DDPM_SQRT_RECIPM1_ACP, RS_DDPM_COEF1, RS_DDPM_COEF2,
+                                  o->var_type == RS_VAR_FIXED_LARGE ? RS_DDPM_LOGVAR_LARGE : RS_DDPM_LOGVAR_SMALL,
+                                  RS_DDPM_ACP, RS_DDPM_ACP_PREV};
+  s->dtab.resize((size_t)kDdpmDevRows * steps);
+  for (int r = 0; r < kDdpmDevRows; ++r)
+    for (int i = 0; i < steps; ++i) s->dtab[(size_t)r * steps + i] = (float)tables[(size_t)rows[r] * steps + i];
+  s->tsteps.resize(steps);
+  for (int i = 0; i < steps; ++i) s->tsteps[i] = (float)(tmap ? tmap[i] : i);
+  *out = s.release();
+  return 0;
+}
 int rs_sampler_tables(const rs_sampler* s, float* dst) {
   RS_CHECK(s && dst, "null argument");
+  RS_CHECK(!s->ddpm, "rs_sampler_tables: a DDPM sampler has no residual-shift tables");
   copy_tables(*s, dst);
   return 0;
 }
@@ -1890,7 +1992,7 @@ int rs_sampler_set_taps(rs_sampler* s, float* pred, float* sample) {
 
 int rs_sampler_run(rs_sampler* s, const float* z_y, const float* noises, const float* lq, const float* mask,
                    float* out_latent, int use_graph, void* stream) {
-  RS_CHECK(s && z_y && noises && lq && out_latent, "null argument");
+  RS_CHECK(s && (z_y || s->ddpm) && noises && lq && out_latent, "null argument");
   int rc = check_plan_device(*s->p); if (rc) return rc;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   rc = sampler_prepare(*s, st); if (rc) return rc;
@@ -1926,7 +2028,7 @@ size_t rs_sampler_staging_bytes(const rs_sampler* s) {
 
 int rs_sampler_run_host(rs_sampler* s, const float* z_y_h, const float* noises_h, const float* lq_h, const float* mask_h,
                         float* out_h, void* staging, size_t staging_bytes, int use_graph, void* stream) {
-  RS_CHECK(s && z_y_h && noises_h && lq_h && out_h && staging, "null argument");
+  RS_CHECK(s && (z_y_h || s->ddpm) && noises_h && lq_h && out_h && staging, "null argument");
   RS_CHECK(staging_bytes >= rs_sampler_staging_bytes(s), "staging buffer too small");
   { int rc = check_plan_device(*s->p); if (rc) return rc; }
   cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -1941,11 +2043,11 @@ int rs_sampler_run_host(rs_sampler* s, const float* z_y_h, const float* noises_h
   float* d_noise = reinterpret_cast<float*>(base + 2 * lat);
   float* d_lq = reinterpret_cast<float*>(base + lat * (s->T + 3));
   float* d_mask = reinterpret_cast<float*>(base + lat * (s->T + 3) + align_up(n_lq * 4, 256));
-  RS_CUDA_OK(cudaMemcpyAsync(d_zy, z_y_h, n_lat * 4, cudaMemcpyHostToDevice, st));
+  if (z_y_h) RS_CUDA_OK(cudaMemcpyAsync(d_zy, z_y_h, n_lat * 4, cudaMemcpyHostToDevice, st));
   RS_CUDA_OK(cudaMemcpyAsync(d_noise, noises_h, n_lat * 4 * (s->T + 1), cudaMemcpyHostToDevice, st));
   RS_CUDA_OK(cudaMemcpyAsync(d_lq, lq_h, n_lq * 4, cudaMemcpyHostToDevice, st));
   if (mask_h) RS_CUDA_OK(cudaMemcpyAsync(d_mask, mask_h, n_mk * 4, cudaMemcpyHostToDevice, st));
-  int rc = rs_sampler_run(s, d_zy, d_noise, d_lq, mask_h ? d_mask : nullptr, d_out, use_graph, stream);
+  int rc = rs_sampler_run(s, z_y_h ? d_zy : nullptr, d_noise, d_lq, mask_h ? d_mask : nullptr, d_out, use_graph, stream);
   if (rc) return rc;
   RS_CUDA_OK(cudaMemcpyAsync(out_h, d_out, n_lat * 4, cudaMemcpyDeviceToHost, st));
   RS_CUDA_OK(cudaStreamSynchronize(st));

@@ -11,6 +11,13 @@ conversion to x0 for every predict_type, posterior mean, noise injection, next-i
 still runs through the library's ``rs_p_sample`` kernel.
 The VQ-GAN bookends (``encode_first_stage`` / ``decode_first_stage``) stay in PyTorch.
 Training (``training_losses``) is out of scope.
+
+``SpacedDiffusionDDPM`` is the reference's other process, the classic DDPM / DDIM one (``GaussianDiffusionDDPM``,
+reference models/gaussian_diffusion.py:611-1239, models/respace.py:65-99), with its ancestral ``p_sample_loop`` and
+``ddim_sample_loop``.  With one of this package's UNets, eps or x0 prediction, a fixed variance, no ``denoised_fn``, an
+``lq`` in ``model_kwargs`` and 2 <= T <= 64, the whole loop (denoiser, x0 conversion, clamp, ancestral or DDIM update,
+next-input packing) runs inside ``librs_b200.so`` as one CUDA graph; everything else runs this module's torch port of
+the reference on the caller's device.
 """
 from __future__ import annotations
 
@@ -38,6 +45,21 @@ class ModelMeanType(enum.Enum):
 class LossType(enum.Enum):
     MSE = enum.auto()
     WEIGHTED_MSE = enum.auto()
+
+
+class ModelVarTypeDDPM(enum.Enum):
+    """What the DDPM process uses as the model's output variance (reference models/gaussian_diffusion.py:82-90)."""
+    LEARNED = enum.auto()
+    LEARNED_RANGE = enum.auto()
+    FIXED_LARGE = enum.auto()
+    FIXED_SMALL = enum.auto()
+
+
+def get_named_beta_schedule(schedule_name, num_diffusion_timesteps, beta_start, beta_end):
+    """Betas of the DDPM process, float64 (reference models/gaussian_diffusion.py:14-30): "linear" only."""
+    if schedule_name == "linear":
+        return np.linspace(beta_start ** 0.5, beta_end ** 0.5, num_diffusion_timesteps, dtype=np.float64) ** 2
+    raise NotImplementedError(f"unknown beta schedule: {schedule_name}")
 
 
 def get_named_eta_schedule(schedule_name, num_diffusion_timesteps, min_noise_level, etas_end=0.99, kappa=1.0,
@@ -381,6 +403,356 @@ class ResShiftDiffusion:
                                            _lib.ptr(bufs["mask"]), bufs["out"].data_ptr(), int(use_graph),
                                            _lib.current_stream()))
         return bufs["out"].clone()
+
+    def training_losses(self, *a, **k):
+        raise NotImplementedError("training is outside the covered hot path (inference only)")
+
+
+class SpacedDiffusionDDPM:
+    """``SpacedDiffusionDDPM(GaussianDiffusionDDPM)`` of the reference (models/respace.py:65-99,
+    models/gaussian_diffusion.py:611-1239), inference side: the respaced schedule, ``p_mean_variance`` for every
+    variance and mean type, the ancestral and DDIM steps and loops, and the first-stage bookends."""
+
+    def __init__(self, use_timesteps, *, betas, model_mean_type, model_var_type, scale_factor=None, sf=4):
+        # respacing (reference models/respace.py:74-88): the kept steps' betas from the base process's alphas_cumprod
+        self.use_timesteps = set(use_timesteps)
+        base = np.array(betas, dtype=np.float64)
+        self.original_num_steps = len(base)
+        self.timestep_map = []
+        new_betas, last = [], 1.0
+        for i, acp in enumerate(np.cumprod(1.0 - base, axis=0)):
+            if i in self.use_timesteps:
+                new_betas.append(1 - acp / last)
+                last = acp
+                self.timestep_map.append(i)
+        self.model_mean_type, self.model_var_type = model_mean_type, model_var_type
+        self.scale_factor, self.sf = scale_factor, sf
+        # float64 tables (reference models/gaussian_diffusion.py:642-680)
+        betas = np.array(new_betas, dtype=np.float64)
+        self.betas = betas
+        assert len(betas.shape) == 1, "betas must be 1-D"
+        assert (betas > 0).all() and (betas <= 1).all()
+        self.num_timesteps = int(betas.shape[0])
+        alphas = 1.0 - betas
+        self.alphas_cumprod = np.cumprod(alphas, axis=0)
+        self.alphas_cumprod_prev = np.append(1.0, self.alphas_cumprod[:-1])
+        self.alphas_cumprod_next = np.append(self.alphas_cumprod[1:], 0.0)
+        self.sqrt_alphas_cumprod = np.sqrt(self.alphas_cumprod)
+        self.sqrt_one_minus_alphas_cumprod = np.sqrt(1.0 - self.alphas_cumprod)
+        self.log_one_minus_alphas_cumprod = np.log(1.0 - self.alphas_cumprod)
+        self.sqrt_recip_alphas_cumprod = np.sqrt(1.0 / self.alphas_cumprod)
+        self.sqrt_recipm1_alphas_cumprod = np.sqrt(1.0 / self.alphas_cumprod - 1)
+        self.posterior_variance = betas * (1.0 - self.alphas_cumprod_prev) / (1.0 - self.alphas_cumprod)
+        self.posterior_log_variance_clipped = np.log(np.append(self.posterior_variance[1], self.posterior_variance[1:]))
+        self.posterior_mean_coef1 = betas * np.sqrt(self.alphas_cumprod_prev) / (1.0 - self.alphas_cumprod)
+        self.posterior_mean_coef2 = (1.0 - self.alphas_cumprod_prev) * np.sqrt(alphas) / (1.0 - self.alphas_cumprod)
+        # FIXED_LARGE's variance (p_mean_variance :791-794)
+        self.variance_fixed_large = np.append(self.posterior_variance[1], self.betas[1:])
+        self.log_variance_fixed_large = np.log(self.variance_fixed_large)
+
+    # ------------------------------------------------------------------ small pieces (torch)
+    def _scale_input(self, inputs, t):
+        """reference models/gaussian_diffusion.py:1213-1214"""
+        return inputs
+
+    def _model_t(self, t):
+        """_WrappedModel's timestep map (reference models/respace.py:60-63)"""
+        return torch.tensor(self.timestep_map, device=t.device, dtype=t.dtype)[t]
+
+    def q_mean_variance(self, x_start, t):
+        """reference models/gaussian_diffusion.py:681-696"""
+        return (_tab(self.sqrt_alphas_cumprod, t, x_start) * x_start, _tab(1.0 - self.alphas_cumprod, t, x_start),
+                _tab(self.log_one_minus_alphas_cumprod, t, x_start))
+
+    def q_sample(self, x_start, t, noise=None):
+        """reference models/gaussian_diffusion.py:698-716"""
+        if noise is None:
+            noise = torch.randn_like(x_start)
+        assert noise.shape == x_start.shape
+        return (_tab(self.sqrt_alphas_cumprod, t, x_start) * x_start
+                + _tab(self.sqrt_one_minus_alphas_cumprod, t, x_start) * noise)
+
+    def q_posterior_mean_variance(self, x_start, x_t, t):
+        """reference models/gaussian_diffusion.py:718-740"""
+        assert x_start.shape == x_t.shape
+        mean = _tab(self.posterior_mean_coef1, t, x_t) * x_start + _tab(self.posterior_mean_coef2, t, x_t) * x_t
+        return mean, _tab(self.posterior_variance, t, x_t), _tab(self.posterior_log_variance_clipped, t, x_t)
+
+    def _predict_xstart_from_eps(self, x_t, t, eps):
+        """reference models/gaussian_diffusion.py:838-843"""
+        assert x_t.shape == eps.shape
+        return _tab(self.sqrt_recip_alphas_cumprod, t, x_t) * x_t - _tab(self.sqrt_recipm1_alphas_cumprod, t, x_t) * eps
+
+    def _predict_xstart_from_xprev(self, x_t, t, xprev):
+        """reference models/gaussian_diffusion.py:845-853"""
+        assert x_t.shape == xprev.shape
+        return (_tab(1.0 / self.posterior_mean_coef1, t, x_t) * xprev
+                - _tab(self.posterior_mean_coef2 / self.posterior_mean_coef1, t, x_t) * x_t)
+
+    def _predict_eps_from_xstart(self, x_t, t, pred_xstart):
+        """reference models/gaussian_diffusion.py:855-859"""
+        return (_tab(self.sqrt_recip_alphas_cumprod, t, x_t) * x_t - pred_xstart) / _tab(self.sqrt_recipm1_alphas_cumprod, t, x_t)
+
+    def p_mean_variance(self, model, x, t, clip_denoised=True, denoised_fn=None, model_kwargs=None):
+        """reference models/gaussian_diffusion.py:742-836, the model's timesteps mapped as models/respace.py:90-91 does."""
+        if model_kwargs is None:
+            model_kwargs = {}
+        B, Cc = x.shape[:2]
+        assert t.shape == (B,)
+        model_output = model(x, self._model_t(t), **model_kwargs)
+        if self.model_var_type in (ModelVarTypeDDPM.LEARNED, ModelVarTypeDDPM.LEARNED_RANGE):
+            assert model_output.shape == (B, Cc * 2, *x.shape[2:])
+            model_output, model_var_values = torch.split(model_output, Cc, dim=1)
+            if self.model_var_type == ModelVarTypeDDPM.LEARNED:
+                model_log_variance = model_var_values
+                model_variance = torch.exp(model_log_variance)
+            else:
+                min_log = _tab(self.posterior_log_variance_clipped, t, x)
+                max_log = _tab(np.log(self.betas), t, x)
+                frac = (model_var_values + 1) / 2               # [-1, 1] -> [min_var, max_var]
+                model_log_variance = frac * max_log + (1 - frac) * min_log
+                model_variance = torch.exp(model_log_variance)
+        else:
+            var, log_var = {
+                ModelVarTypeDDPM.FIXED_LARGE: (self.variance_fixed_large, self.log_variance_fixed_large),
+                ModelVarTypeDDPM.FIXED_SMALL: (self.posterior_variance, self.posterior_log_variance_clipped),
+            }[self.model_var_type]
+            model_variance, model_log_variance = _tab(var, t, x), _tab(log_var, t, x)
+
+        def process_xstart(v):
+            if denoised_fn is not None:
+                v = denoised_fn(v)
+            return v.clamp(-1, 1) if clip_denoised else v
+
+        if self.model_mean_type == ModelMeanType.PREVIOUS_X:
+            pred_xstart = process_xstart(self._predict_xstart_from_xprev(x_t=x, t=t, xprev=model_output))
+            model_mean = model_output
+        elif self.model_mean_type in (ModelMeanType.START_X, ModelMeanType.EPSILON):
+            if self.model_mean_type == ModelMeanType.START_X:
+                pred_xstart = process_xstart(model_output)
+            else:
+                pred_xstart = process_xstart(self._predict_xstart_from_eps(x_t=x, t=t, eps=model_output))
+            model_mean, _, _ = self.q_posterior_mean_variance(x_start=pred_xstart, x_t=x, t=t)
+        else:
+            raise NotImplementedError(self.model_mean_type)
+        assert model_mean.shape == model_log_variance.shape == pred_xstart.shape == x.shape
+        return {"mean": model_mean, "variance": model_variance, "log_variance": model_log_variance,
+                "pred_xstart": pred_xstart}
+
+    # ------------------------------------------------------------------ one step (torch, any model callable)
+    def _p_finish(self, x, t, out, noise):
+        """the rest of reference p_sample (models/gaussian_diffusion.py:887-892) on p_mean_variance's output"""
+        nonzero_mask = (t != 0).float().view(-1, *([1] * (len(x.shape) - 1)))      # no noise when t == 0
+        sample = out["mean"] + nonzero_mask * torch.exp(0.5 * out["log_variance"]) * noise
+        return {"sample": sample, "pred_xstart": out["pred_xstart"]}
+
+    def _ddim_finish(self, x, t, out, noise, eta):
+        """the rest of reference ddim_sample (models/gaussian_diffusion.py:1010-1028) on p_mean_variance's output"""
+        eps = self._predict_eps_from_xstart(x, t, out["pred_xstart"])
+        alpha_bar = _tab(self.alphas_cumprod, t, x)
+        alpha_bar_prev = _tab(self.alphas_cumprod_prev, t, x)
+        sigma = eta * torch.sqrt((1 - alpha_bar_prev) / (1 - alpha_bar)) * torch.sqrt(1 - alpha_bar / alpha_bar_prev)
+        mean_pred = out["pred_xstart"] * torch.sqrt(alpha_bar_prev) + torch.sqrt(1 - alpha_bar_prev - sigma ** 2) * eps
+        nonzero_mask = (t != 0).float().view(-1, *([1] * (len(x.shape) - 1)))      # no noise when t == 0
+        return {"sample": mean_pred + nonzero_mask * sigma * noise, "pred_xstart": out["pred_xstart"]}
+
+    def p_sample(self, model, x, t, clip_denoised=True, denoised_fn=None, model_kwargs=None):
+        """reference models/gaussian_diffusion.py:861-892"""
+        out = self.p_mean_variance(model, x, t, clip_denoised=clip_denoised, denoised_fn=denoised_fn,
+                                   model_kwargs=model_kwargs)
+        return self._p_finish(x, t, out, torch.randn_like(x))
+
+    def ddim_sample(self, model, x, t, clip_denoised=True, denoised_fn=None, model_kwargs=None, eta=0.0):
+        """reference models/gaussian_diffusion.py:985-1028"""
+        out = self.p_mean_variance(model, x, t, clip_denoised=clip_denoised, denoised_fn=denoised_fn,
+                                   model_kwargs=model_kwargs)
+        return self._ddim_finish(x, t, out, torch.randn_like(x), eta)
+
+    # ------------------------------------------------------------------ the loops
+    def draw_noises(self, shape, noise=None, device=None):
+        """The T + 1 noise tensors of a loop in the reference's draw order: x_T = ``noise`` or randn(*shape)
+        (models/gaussian_diffusion.py:959-962, :1122-1125), then one randn_like(x) per step (:887, :1019; DDIM draws
+        one at eta = 0 too).  Drawn ahead, so that the fused and the torch route see the same values under one seed."""
+        first = torch.randn(*shape, device=device) if noise is None else noise
+        out = torch.empty((self.num_timesteps + 1,) + tuple(first.shape), dtype=first.dtype, device=first.device)
+        out[0] = first
+        for k in range(self.num_timesteps):
+            out[k + 1] = torch.randn_like(first)
+        return out
+
+    _NATIVE_MEAN_TYPES = {ModelMeanType.EPSILON: 1, ModelMeanType.START_X: 0}        # rs_mean_type
+    _NATIVE_VAR_TYPES = {ModelVarTypeDDPM.FIXED_LARGE: 0, ModelVarTypeDDPM.FIXED_SMALL: 1}   # rs_ddpm_var_type
+
+    def _native_ok(self, model, denoised_fn, model_kwargs) -> bool:
+        return (isinstance(model, (UNetModelSwin, UNetModel, UNetModelConv))
+                and self.model_mean_type in self._NATIVE_MEAN_TYPES
+                and self.model_var_type in self._NATIVE_VAR_TYPES
+                and denoised_fn is None
+                and model_kwargs is not None and "lq" in model_kwargs
+                and 2 <= self.num_timesteps <= 64)       # rs_ddpm_sampler_create: 2 <= T <= FiLM-table rows of a plan
+
+    def ddpm_tables(self) -> np.ndarray:
+        """[8, T] float64: the rows of rs_ddpm_sampler_create (rs_ddpm_table_row)"""
+        return np.ascontiguousarray(np.stack([getattr(self, name) for name in _lib.DDPM_TABLE_ROWS]), dtype=np.float64)
+
+    def native_sampler(self, model, batch, height, width, kind: str, clip_denoised: bool, eta: float = 0.0):
+        """The plan's DDPM sampler for this process and these options ("ancestral" or "ddim"), created once."""
+        plan = model.plan(batch, height, width)
+        opt = _lib.DdpmOptionsC(_lib.DDPM_KINDS[kind], self._NATIVE_MEAN_TYPES[self.model_mean_type],
+                                self._NATIVE_VAR_TYPES[self.model_var_type], int(bool(clip_denoised)), float(eta))
+        key = ("ddpm", self.num_timesteps, tuple(self.betas.tolist()), tuple(self.timestep_map),
+               (opt.kind, opt.mean_type, opt.var_type, opt.clip, opt.eta))
+        if key not in plan.samplers:
+            h = C.c_void_p()
+            tabs = self.ddpm_tables()
+            tm = (C.c_int32 * self.num_timesteps)(*self.timestep_map)
+            _lib.check(_lib.lib.rs_ddpm_sampler_create(plan.handle, self.num_timesteps,
+                                                       tabs.ctypes.data_as(C.POINTER(C.c_double)), tm, C.byref(opt),
+                                                       C.byref(h)))
+            plan.samplers[key] = h
+        return plan.samplers[key]
+
+    def sample_latent(self, model, noises, model_kwargs, kind="ancestral", clip_denoised=True, eta=0.0, use_graph=True):
+        """The fused loop: noises [T + 1, B, C, H, W] (draw_noises) -> the final latent, all T steps inside librs_b200
+        (CUDA graph replay)."""
+        T = self.num_timesteps
+        if noises.dim() != 5 or noises.shape[0] != T + 1:
+            raise ValueError(f"noises must have shape (T + 1 = {T + 1}, B, C, H, W), got {tuple(noises.shape)}")
+        B, Cc, H, W = noises.shape[1:]
+        lq_in, mask_in = model_kwargs["lq"], model_kwargs.get("mask", None)
+        ResShiftDiffusion._check_native_inputs(model, noises[0], lq_in, mask_in)
+        s = self.native_sampler(model, B, H, W, kind, clip_denoised, eta)
+        # stable device buffers (shared with the plan's ResShift samplers) so that each captured graph can be replayed
+        plan = model.plan(B, H, W)
+        bufs = getattr(plan, "_io", None)
+        dev = noises.device
+        if (bufs is None or bufs["lq"].shape != lq_in.shape or (mask_in is None) != (bufs["mask"] is None)
+                or bufs["noise"].shape != noises.shape):
+            bufs = {"zy": torch.empty(B, Cc, H, W, dtype=torch.float32, device=dev),
+                    "noise": torch.empty(noises.shape, dtype=torch.float32, device=dev),
+                    "lq": torch.empty(lq_in.shape, dtype=torch.float32, device=dev),
+                    "mask": None if mask_in is None else torch.empty(mask_in.shape, dtype=torch.float32, device=dev),
+                    "out": torch.empty(B, Cc, H, W, dtype=torch.float32, device=dev)}
+            plan._io = bufs
+        bufs["noise"].copy_(noises)
+        bufs["lq"].copy_(lq_in)
+        if mask_in is not None:
+            bufs["mask"].copy_(mask_in)
+        _lib.check(_lib.lib.rs_sampler_run(s, None, bufs["noise"].data_ptr(), bufs["lq"].data_ptr(),
+                                           _lib.ptr(bufs["mask"]), bufs["out"].data_ptr(), int(use_graph),
+                                           _lib.current_stream()))
+        return bufs["out"].clone()
+
+    def _native_progressive(self, model, noises, model_kwargs, kind, clip_denoised, eta):
+        """The fused loop run eagerly with the per-step taps: yields sample / pred_xstart of every step."""
+        T = self.num_timesteps
+        x = noises[0].float().contiguous()
+        B, Cc, H, W = x.shape
+        lq = model_kwargs["lq"].float().contiguous()
+        mask = model_kwargs.get("mask", None)
+        mask = mask.float().contiguous() if mask is not None else None
+        ResShiftDiffusion._check_native_inputs(model, x, lq, mask)
+        s = self.native_sampler(model, B, H, W, kind, clip_denoised, eta)
+        nz = noises.float().contiguous()
+        final = torch.empty_like(x)
+        preds = torch.empty((T,) + tuple(x.shape), dtype=torch.float32, device=x.device)
+        samples = torch.empty_like(preds)
+        _lib.check(_lib.lib.rs_sampler_set_taps(s, preds.data_ptr(), samples.data_ptr()))
+        try:
+            _lib.check(_lib.lib.rs_sampler_run(s, None, nz.data_ptr(), lq.data_ptr(), _lib.ptr(mask), final.data_ptr(),
+                                               0, _lib.current_stream()))
+        finally:
+            _lib.check(_lib.lib.rs_sampler_set_taps(s, None, None))
+        for k in range(T):
+            yield {"sample": samples[k], "pred_xstart": preds[k]}
+
+    def _progressive(self, kind, model, shape, noise, clip_denoised, denoised_fn, model_kwargs, device, progress, eta):
+        if device is None:
+            device = next(model.parameters()).device
+        assert isinstance(shape, (tuple, list))
+        noises = self.draw_noises(shape, noise, device)
+        if self._native_ok(model, denoised_fn, model_kwargs):
+            yield from self._native_progressive(model, noises, model_kwargs, kind, clip_denoised, eta)
+            return
+        img = noises[0]
+        indices = list(range(self.num_timesteps))[::-1]
+        if progress:
+            from tqdm.auto import tqdm      # lazy, as the reference does
+            indices = tqdm(indices)
+        for k, i in enumerate(indices):
+            t = torch.tensor([i] * shape[0], device=device)
+            if kind == "ddim":
+                t = t.long()
+            with torch.no_grad():
+                out = self.p_mean_variance(model, img, t, clip_denoised=clip_denoised, denoised_fn=denoised_fn,
+                                           model_kwargs=model_kwargs)
+                if kind == "ddim":
+                    out = self._ddim_finish(img, t, out, noises[k + 1], eta)
+                else:
+                    out = self._p_finish(img, t, out, noises[k + 1])
+                yield out
+                img = out["sample"]
+
+    def p_sample_loop_progressive(self, model, shape, noise=None, clip_denoised=True, denoised_fn=None,
+                                  model_kwargs=None, device=None, progress=False):
+        """reference models/gaussian_diffusion.py:937-983 — one dict (sample, pred_xstart) per step."""
+        yield from self._progressive("ancestral", model, shape, noise, clip_denoised, denoised_fn, model_kwargs, device,
+                                     progress, 0.0)
+
+    def ddim_sample_loop_progressive(self, model, shape, noise=None, clip_denoised=True, denoised_fn=None,
+                                     model_kwargs=None, device=None, progress=False, eta=0.0):
+        """reference models/gaussian_diffusion.py:1101-1147 — one dict (sample, pred_xstart) per step."""
+        yield from self._progressive("ddim", model, shape, noise, clip_denoised, denoised_fn, model_kwargs, device,
+                                     progress, eta)
+
+    def _loop(self, kind, model, shape, noise, clip_denoised, denoised_fn, first_stage_model, model_kwargs, device,
+              progress, eta):
+        if self._native_ok(model, denoised_fn, model_kwargs):
+            if device is None:
+                device = next(model.parameters()).device
+            assert isinstance(shape, (tuple, list))
+            noises = self.draw_noises(shape, noise, device)
+            final = self.sample_latent(model, noises, model_kwargs, kind, clip_denoised, eta)
+        else:
+            final = None
+            for sample in self._progressive(kind, model, shape, noise, clip_denoised, denoised_fn, model_kwargs, device,
+                                            progress, eta):
+                final = sample["sample"]
+        return self.decode_first_stage(final, first_stage_model)
+
+    def p_sample_loop(self, model, shape, noise=None, clip_denoised=True, denoised_fn=None, first_stage_model=None,
+                      model_kwargs=None, device=None, progress=False):
+        """reference models/gaussian_diffusion.py:894-935 — returns the DECODED sample."""
+        return self._loop("ancestral", model, shape, noise, clip_denoised, denoised_fn, first_stage_model, model_kwargs,
+                          device, progress, 0.0)
+
+    def ddim_sample_loop(self, model, shape, noise=None, first_stage_model=None, clip_denoised=True, denoised_fn=None,
+                         model_kwargs=None, device=None, progress=False, eta=0.0):
+        """reference models/gaussian_diffusion.py:1068-1099 — returns the DECODED sample."""
+        return self._loop("ddim", model, shape, noise, clip_denoised, denoised_fn, first_stage_model, model_kwargs,
+                          device, progress, eta)
+
+    # ------------------------------------------------------------------ first-stage bookends (PyTorch)
+    def decode_first_stage(self, z_sample, first_stage_model=None):
+        """reference models/gaussian_diffusion.py:1216-1225"""
+        ori_dtype = z_sample.dtype
+        if first_stage_model is None:
+            return z_sample
+        with torch.no_grad():
+            z_sample = 1 / self.scale_factor * z_sample
+            z_sample = z_sample.type(next(first_stage_model.parameters()).dtype)
+            return first_stage_model.decode(z_sample).type(ori_dtype)
+
+    def encode_first_stage(self, y, first_stage_model, up_sample=False):
+        """reference models/gaussian_diffusion.py:1227-1239"""
+        ori_dtype = y.dtype
+        if up_sample:
+            y = bicubic_upsample(y, self.sf)
+        if first_stage_model is None:
+            return y
+        with torch.no_grad():
+            y = y.type(dtype=next(first_stage_model.parameters()).dtype)
+            return (first_stage_model.encode(y) * self.scale_factor).type(ori_dtype)
 
     def training_losses(self, *a, **k):
         raise NotImplementedError("training is outside the covered hot path (inference only)")

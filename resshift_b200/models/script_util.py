@@ -1,5 +1,5 @@
-"""``create_gaussian_diffusion`` — the yaml ``diffusion.target`` factory, same keyword-only signature
-as the reference (reference models/script_util.py:7-55)."""
+"""``create_gaussian_diffusion`` and ``create_gaussian_diffusion_ddpm`` — the yaml ``diffusion.target`` factories, same
+keyword-only signatures as the reference (reference models/script_util.py:7-92)."""
 from __future__ import annotations
 
 from . import gaussian_diffusion as gd
@@ -24,3 +24,22 @@ def create_gaussian_diffusion(*, normalize_input, schedule_name, sf=4, min_noise
         use_timesteps=gd.space_timesteps(steps, timestep_respacing), sqrt_etas=sqrt_etas, kappa=kappa,
         model_mean_type=mean_type, loss_type=gd.LossType.WEIGHTED_MSE if weighted_mse else gd.LossType.MSE,
         scale_factor=scale_factor, normalize_input=normalize_input, sf=sf, latent_flag=latent_flag)
+
+
+def create_gaussian_diffusion_ddpm(*, beta_start, beta_end, sf=4, steps=1000, learn_sigma=False, sigma_small=False,
+                                   noise_schedule="linear", predict_xstart=False, timestep_respacing=None,
+                                   scale_factor=1.0):
+    """The DDPM / DDIM process (reference models/script_util.py:57-92)."""
+    betas = gd.get_named_beta_schedule(noise_schedule, steps, beta_start, beta_end)
+    if timestep_respacing is None:
+        timestep_respacing = steps
+    else:
+        assert isinstance(timestep_respacing, int)
+    if learn_sigma:
+        var_type = gd.ModelVarTypeDDPM.LEARNED_RANGE
+    else:
+        var_type = gd.ModelVarTypeDDPM.FIXED_SMALL if sigma_small else gd.ModelVarTypeDDPM.FIXED_LARGE
+    return gd.SpacedDiffusionDDPM(
+        use_timesteps=gd.space_timesteps(steps, timestep_respacing), betas=betas,
+        model_mean_type=gd.ModelMeanType.START_X if predict_xstart else gd.ModelMeanType.EPSILON,
+        model_var_type=var_type, scale_factor=scale_factor, sf=sf)
