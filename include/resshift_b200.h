@@ -216,7 +216,8 @@ typedef struct rs_sampler_options {
 int rs_sampler_create_ex(rs_plan* p, int steps, const double* sqrt_etas_host, double kappa,
                          const int32_t* timestep_map_host, const rs_sampler_options* options, rs_sampler** out);
 void rs_sampler_destroy(rs_sampler* s);
-/* z_y [B, C, H, W] fp32; noises [(T+1), B, C, H, W] fp32 in the reference's draw order (prior first);
+/* z_y [B, C, H, W] fp32 (x_start for a DDIM inversion sampler); noises [(T+1), B, C, H, W] fp32 in the reference's
+ * draw order (prior first; a DDIM inversion sampler does not read it, and it may be NULL there);
  * lq/mask as in rs_plan_forward; out_latent [B, C, H, W] fp32 (the loop's final `sample`).
  * use_graph != 0 replays a CUDA graph captured on first use (same pointers required on later calls). */
 int rs_sampler_run(rs_sampler* s, const float* z_y, const float* noises, const float* lq, const float* mask,
@@ -248,7 +249,8 @@ typedef enum rs_ddpm_table_row {
   RS_DDPM_LOGVAR_SMALL = 5,         /* posterior_log_variance_clipped                  (FIXED_SMALL)          */
   RS_DDPM_ACP = 6,                  /* alphas_cumprod                                                         */
   RS_DDPM_ACP_PREV = 7,             /* alphas_cumprod_prev                                                    */
-  RS_DDPM_TABLE_ROWS = 8
+  RS_DDPM_TABLE_ROWS = 8,
+  RS_DDPM_ACP_NEXT = 8              /* alphas_cumprod_next (0 at T - 1): read by rs_ddim_reverse_sampler_create only */
 } rs_ddpm_table_row;
 typedef struct rs_ddpm_options {
   int32_t kind;               /* RS_DDPM_ANCESTRAL or RS_DDPM_DDIM                                         */
@@ -262,6 +264,22 @@ typedef struct rs_ddpm_options {
  * clip other than 0 / 1, a negative or non-finite eta, steps outside [2, the plan's FiLM rows]. */
 int rs_ddpm_sampler_create(rs_plan* p, int steps, const double* tables_host, const int32_t* timestep_map_host,
                            const rs_ddpm_options* options, rs_sampler** out);
+
+/* ---- DDIM inversion: SpacedDiffusionDDPM.ddim_reverse_sample (reference models/gaussian_diffusion.py:1030-1066) in
+ *      a t = 0 .. T-1 loop, on the same plan and entry points --------------------------------------------------------
+ * x = x_start, then for t = 0 .. T-1: denoiser forward on x (unscaled, FiLM row t) + one reverse step
+ * x <- x0 sqrt(acp_next[t]) + sqrt(1 - acp_next[t]) eps'; out_latent receives x_T.  rs_sampler_run / _run_host read
+ * x_start from z_y (required) and draw nothing: noises is not read and may be NULL.  _set_taps / _destroy work
+ * unchanged; rs_sampler_tables refuses these samplers. */
+typedef struct rs_ddim_reverse_options {
+  int32_t mean_type;          /* RS_MEAN_EPSILON or RS_MEAN_XSTART                                         */
+  int32_t clip;               /* 1: clamp x0 to [-1, 1] (clip_denoised)                                    */
+} rs_ddim_reverse_options;
+/* tables_host [RS_DDPM_TABLE_ROWS + 1][steps] float64: the rows of rs_ddpm_sampler_create, then RS_DDPM_ACP_NEXT;
+ * timestep_map_host as there.  Refused, each with its reason: NULL tables or options, a mean type other than eps or
+ * x0, clip other than 0 / 1, steps outside [2, the plan's FiLM rows]. */
+int rs_ddim_reverse_sampler_create(rs_plan* p, int steps, const double* tables_host, const int32_t* timestep_map_host,
+                                   const rs_ddim_reverse_options* options, rs_sampler** out);
 
 /* ---- VQ-GAN first stage: ldm.models.autoencoder.VQModelTorch (reference ldm/models/autoencoder.py:12-47) -------
  * The engine handle is the same opaque type as the denoiser's: rs_unet_param_count / _param_info / _arena_bytes /
@@ -405,6 +423,22 @@ typedef struct rs_ddpm_step_args {
   float* x0_out;
 } rs_ddpm_step_args;
 int rs_op_ddpm_step(const rs_ddpm_step_args* a, void* stream);
+/* The DDIM inversion step (rs_ddim_reverse_sampler_create) on its own, with the grid the loop launches: x0 from the
+ * model output (eps or x0, clamped with clip), eps' = (sqrt_recip_acp[t] x_t - x0) / sqrt_recipm1_acp[t], then
+ * x_next = x0 sqrt(acp_next[t]) + sqrt(1 - acp_next[t]) eps'.  Tables are [T] fp32 device arrays.  next_in (t < T - 1
+ * only) receives fp16(x_next) in channels [0, C); counters as in rs_op_p_sample_ex; x0_out (optional) receives x0.
+ * Refused: a NULL table, an unknown mean type, clip other than 0 / 1, t outside [0, T), next_cpad < C, more counters
+ * than launched threads. */
+typedef struct rs_ddim_reverse_step_args {
+  const float* out; const float* x_t; float* x_next;                                          /* [N, C, HW] fp32       */
+  const float* sqrt_recip_acp; const float* sqrt_recipm1_acp; const float* acp_next;          /* [T] fp32 device tables */
+  int32_t T, t, N, C, HW;
+  int32_t mean_type, clip;
+  void* next_in; int32_t next_cpad;
+  uint32_t* counters; int32_t n_counters;
+  float* x0_out;
+} rs_ddim_reverse_step_args;
+int rs_op_ddim_reverse_step(const rs_ddim_reverse_step_args* a, void* stream);
 /* The denoiser's input packing: out[N*HW][Cpad] fp16 = cat([fp16(x * scale_tab[scale_idx]), lq, mask], channels) + zero
  * padding (scale 1 without scale_tab).  lq is one of: lq_nchw [N, Cl, HW] fp32 (optionally followed by mask_nchw
  * [N, 1, HW]); lq_nchw [N, Cl / 4, 2H, 2W] packed as pixel_unshuffle(lq, 2) (lq_unshuffle, W = the latent width); the

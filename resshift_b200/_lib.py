@@ -148,12 +148,31 @@ class DdpmStepArgsC(C.Structure):
     ]
 
 
+class DdimReverseOptionsC(C.Structure):
+    """Mirror of ``rs_ddim_reverse_options``."""
+    _fields_ = [("mean_type", C.c_int32), ("clip", C.c_int32)]
+
+
+class DdimReverseStepArgsC(C.Structure):
+    """Mirror of ``rs_ddim_reverse_step_args``."""
+    _fields_ = [
+        ("out", C.c_void_p), ("x_t", C.c_void_p), ("x_next", C.c_void_p),
+        ("sqrt_recip_acp", C.c_void_p), ("sqrt_recipm1_acp", C.c_void_p), ("acp_next", C.c_void_p),
+        ("T", C.c_int32), ("t", C.c_int32), ("N", C.c_int32), ("C", C.c_int32), ("HW", C.c_int32),
+        ("mean_type", C.c_int32), ("clip", C.c_int32),
+        ("next_in", C.c_void_p), ("next_cpad", C.c_int32), ("counters", C.c_void_p), ("n_counters", C.c_int32),
+        ("x0_out", C.c_void_p),
+    ]
+
+
 # rs_ddpm_kind, rs_ddpm_var_type, and the rows of rs_ddpm_sampler_create's float64 tables (rs_ddpm_table_row)
 DDPM_KINDS = {"ancestral": 0, "ddim": 1}
 DDPM_VAR_TYPES = {"fixed_large": 0, "fixed_small": 1}
 DDPM_TABLE_ROWS = ("sqrt_recip_alphas_cumprod", "sqrt_recipm1_alphas_cumprod", "posterior_mean_coef1",
                    "posterior_mean_coef2", "log_variance_fixed_large", "posterior_log_variance_clipped",
                    "alphas_cumprod", "alphas_cumprod_prev")
+# rs_ddim_reverse_sampler_create's rows: the same, then RS_DDPM_ACP_NEXT
+DDIM_REVERSE_TABLE_ROWS = DDPM_TABLE_ROWS + ("alphas_cumprod_next",)
 
 # rs_mean_type, by the reference's predict_type names (models/script_util.py:35-44)
 MEAN_TYPES = {"xstart": 0, "epsilon": 1, "epsilon_scale": 2, "residual": 3}
@@ -205,6 +224,9 @@ _SIGNATURES = {
     "rs_ddpm_sampler_create": (C.c_int, [_P, C.c_int, C.POINTER(C.c_double), C.POINTER(C.c_int32),
                                          C.POINTER(DdpmOptionsC), C.POINTER(_P)]),
     "rs_op_ddpm_step": (C.c_int, [C.POINTER(DdpmStepArgsC), _P]),
+    "rs_ddim_reverse_sampler_create": (C.c_int, [_P, C.c_int, C.POINTER(C.c_double), C.POINTER(C.c_int32),
+                                                 C.POINTER(DdimReverseOptionsC), C.POINTER(_P)]),
+    "rs_op_ddim_reverse_step": (C.c_int, [C.POINTER(DdimReverseStepArgsC), _P]),
     "rs_p_sample": (C.c_int, [_P, _P, _P, _P, C.c_float, C.c_float, C.c_float, C.c_int, C.c_longlong, _P]),
     "rs_op_p_sample_ex": (C.c_int, [C.POINTER(PSampleArgsC), _P]),
     "rs_op_p_sample_pred": (C.c_int, [C.POINTER(PSamplePredArgsC), _P]),

@@ -361,6 +361,61 @@ __global__ void ddpm_step_kernel(const DdpmStepParams p) {
 }
 
 // ------------------------------------------------------------------------------------------------
+// DDIM inversion step of GaussianDiffusionDDPM.ddim_reverse_sample (reference models/gaussian_diffusion.py:1030-1066),
+// fp32 NCHW in/out, t walking 0 .. T-1 upward:
+//   x0       as ddpm_step_kernel (eps or x0 prediction, clamped to [-1, 1] with clip)
+//   eps'     = (sqrt_recip_acp[t] x_t - x0) / sqrt_recipm1_acp[t]                               (:1054-1057)
+//   x_{t+1}  = x0 sqrt(acp_next[t]) + sqrt(1 - acp_next[t]) eps'                                (:1058-1064)
+// acp_next[T-1] is 0, so the last step returns eps'.  Every operation is the reference's fp32 tensor operation on the
+// fp32 table values, in its order and rounded on its own (no FMA contraction); nothing is drawn.
+// next_in receives fp16(x_{t+1}) for t < T - 1 (the denoiser sees x_t unscaled).
+// ------------------------------------------------------------------------------------------------
+struct DdimReverseStepParams {
+  const float* x_t;       // [N, C, HW]
+  const float* out;       // [N, C, HW]: the model output (eps or x0)
+  float* x_next;          // [N, C, HW]
+  const float* sqrt_recip_acp; const float* sqrt_recipm1_acp; const float* acp_next;   // [T] fp32 tables
+  int clip;
+  int T, t;               // t: schedule index of THIS step (0 .. T-1)
+  int N, C, HW;
+  __half* next_in; int next_cpad;     // optional: [N*HW, next_cpad]; channels [0, C) are written here
+  unsigned int* zero_ptr; int zero_n; // GroupNorm arrival counters of the NEXT denoiser forward: reset here
+  float* x0_out;                      // optional [N, C, HW]: pred_xstart
+};
+
+template <int MT>
+__global__ void ddim_reverse_step_kernel(const DdimReverseStepParams p) {
+  pdl_trigger();
+  pdl_wait();
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < p.zero_n) p.zero_ptr[i] = 0u;
+  const long long total = (long long)p.N * p.C * p.HW;
+  if (i >= total) return;
+  const int t = p.t;
+  const float xt = p.x_t[i];
+  const float sra = p.sqrt_recip_acp[t], srm1 = p.sqrt_recipm1_acp[t];
+  float x0;
+  if constexpr (MT == kMeanEpsilon) {
+    x0 = __fsub_rn(__fmul_rn(sra, xt), __fmul_rn(srm1, p.out[i]));
+  } else {
+    static_assert(MT == kMeanXstart, "DDIM inversion predicts eps or x0");
+    x0 = p.out[i];
+  }
+  if (p.clip) x0 = x0 < -1.0f ? -1.0f : (x0 > 1.0f ? 1.0f : x0);     // clamp(-1, 1): NaN stays NaN
+  if (p.x0_out) p.x0_out[i] = x0;
+  const float an = p.acp_next[t];
+  const float eps = __fdiv_rn(__fsub_rn(__fmul_rn(sra, xt), x0), srm1);
+  const float v = __fadd_rn(__fmul_rn(x0, __fsqrt_rn(an)), __fmul_rn(__fsqrt_rn(__fsub_rn(1.0f, an)), eps));
+  p.x_next[i] = v;
+  if (p.next_in && t + 1 < p.T) {
+    const int hw = (int)(i % p.HW);
+    const int c = (int)((i / p.HW) % p.C);
+    const int n = (int)(i / ((long long)p.HW * p.C));
+    p.next_in[((long long)n * p.HW + hw) * p.next_cpad + c] = __float2half_rn(v);
+  }
+}
+
+// ------------------------------------------------------------------------------------------------
 // Split-K finish: out = act(sum_s partial[s] + bias) + residual, fp16 NHWC view (or fp32 NCHW), plus the
 // GroupNorm partial statistics of the result.  One CTA per (128-pixel slot, image) — the same slots the
 // conv epilogue would have produced; splits are summed in a fixed order, statistics reduced in a fixed tree.

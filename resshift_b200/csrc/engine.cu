@@ -1,5 +1,5 @@
 // Engine: the Swin-UNet denoiser of ResShift as a static program of sm_90a kernel launches, plus the
-// residual-shift and DDPM / DDIM sampling loops, behind the C ABI declared in include/resshift_b200.h.
+// residual-shift, DDPM / DDIM and DDIM-inversion sampling loops, behind the C ABI declared in include/resshift_b200.h.
 //
 // Topology restates UNetModelSwin.__init__/forward (reference models/unet.py:659-895), ResBlock
 // (:110-206), BasicLayer / SwinTransformerBlock (models/swin_transformer.py:163-281,348-442).
@@ -1679,6 +1679,10 @@ struct rs_sampler {
   bool ddpm = false;
   rs_ddpm_options dopt{};
   std::vector<float> dtab;
+  // DDIM inversion sampler (rs_ddim_reverse_sampler_create; ddpm is set too): x_start comes in as z_y, nothing is
+  // drawn, and dtab holds kReverseDevRows rows of T
+  bool reverse = false;
+  rs_ddim_reverse_options ropt{};
   float* tap_pred = nullptr; float* tap_sample = nullptr;
   cudaGraphExec_t graph = nullptr;
   cudaStream_t cap_stream = nullptr;     // capture happens on a private stream (the legacy default stream cannot capture)
@@ -1732,6 +1736,49 @@ int launch_ddpm_step(int kind, int mean_type, const DdpmStepParams& dp, long lon
   return 0;
 }
 
+// the DDIM inversion sampler's fp32 tables in the plan's table region, one 1024-entry row each: sqrt_recip_acp,
+// sqrt_recipm1_acp, acp_next
+constexpr int kReverseDevRows = 3;
+
+// ddim_reverse_step_kernel instance of a mean type; unknown values are refused
+int launch_ddim_reverse_step(int mean_type, const DdimReverseStepParams& rp, long long numel, cudaStream_t st) {
+  const dim3 grid((unsigned)((numel + 255) / 256)), block(256);
+  RS_CHECK(mean_type == RS_MEAN_EPSILON || mean_type == RS_MEAN_XSTART,
+           "DDIM inversion predicts eps or x0 (RS_MEAN_EPSILON or RS_MEAN_XSTART), got mean type " + std::to_string(mean_type));
+  if (mean_type == RS_MEAN_EPSILON) (void)launch_k(ddim_reverse_step_kernel<kMeanEpsilon>, grid, block, (size_t)(0), st, rp);
+  else (void)launch_k(ddim_reverse_step_kernel<kMeanXstart>, grid, block, (size_t)(0), st, rp);
+  return 0;
+}
+
+// x = x_start; then for t = 0 .. T-1 the denoiser on x (unscaled) and the reverse step; the last writes out_latent
+int reverse_enqueue(rs_sampler& S, const float* x_start, const float* lq, const float* mask, float* out_latent,
+                    cudaStream_t st) {
+  rs_plan& P = *S.p;
+  const rs_unet_config& c = P.e->cfg;
+  RS_CHECK(c.in_channels == c.out_channels, "the sampler needs out_channels == in_channels (x0 and x_t share a shape)");
+  const long long numel = (long long)P.B * c.in_channels * P.H * P.W;
+  float* state = reinterpret_cast<float*>(P.ws + P.off_state);
+  const float* tab = reinterpret_cast<const float*>(P.ws + P.off_tables);
+  int rc = pack_lq_and_input(P, x_start, lq, mask, nullptr, 0, st); if (rc) return rc;
+  const float* film_all = reinterpret_cast<const float*>(P.ws + P.off_film);
+  for (int t = 0; t < S.T; ++t) {
+    rc = run_ops(P, P.ops, film_all + (long long)t * P.e->film_rows, 0, st); if (rc) return rc;
+    DdimReverseStepParams rp{};
+    rp.x_t = t == 0 ? x_start : state; rp.out = P.out_f32;
+    rp.x_next = (t == S.T - 1) ? out_latent : state;
+    rp.sqrt_recip_acp = tab; rp.sqrt_recipm1_acp = tab + 1024; rp.acp_next = tab + 2048;
+    rp.clip = S.ropt.clip; rp.T = S.T; rp.t = t;
+    rp.N = P.B; rp.C = c.in_channels; rp.HW = P.H * P.W;
+    rp.next_in = P.xin.ptr; rp.next_cpad = P.cin_pad;
+    rp.zero_ptr = reinterpret_cast<unsigned int*>(P.ws + P.off_counters); rp.zero_n = P.n_gn * P.B;
+    if (S.tap_pred) rp.x0_out = S.tap_pred + (long long)t * numel;
+    rc = launch_ddim_reverse_step(S.ropt.mean_type, rp, numel, st); if (rc) return rc;
+    if (S.tap_sample) RS_CUDA_OK(cudaMemcpyAsync(S.tap_sample + (long long)t * numel, rp.x_next, numel * 4, cudaMemcpyDeviceToDevice, st));
+  }
+  RS_CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
 // x_T = noises[0]; then per step the denoiser on x_t (unscaled) and the DDPM / DDIM step
 int ddpm_enqueue(rs_sampler& S, const float* noises, const float* lq, const float* mask, float* out_latent,
                  cudaStream_t st) {
@@ -1763,6 +1810,7 @@ int ddpm_enqueue(rs_sampler& S, const float* noises, const float* lq, const floa
 
 int sampler_enqueue(rs_sampler& S, const float* z_y, const float* noises, const float* lq, const float* mask,
                     float* out_latent, cudaStream_t st) {
+  if (S.reverse) return reverse_enqueue(S, z_y, lq, mask, out_latent, st);
   if (S.ddpm) return ddpm_enqueue(S, noises, lq, mask, out_latent, st);
   rs_plan& P = *S.p;
   const rs_unet_config& c = P.e->cfg;
@@ -1807,7 +1855,8 @@ int sampler_prepare(rs_sampler& S, cudaStream_t st) {
   if (P.table_owner == &S && P.table_epoch == P.e->weights_epoch) return 0;
   float* tab = reinterpret_cast<float*>(P.ws + P.off_tables);
   if (S.ddpm) {
-    for (int r = 0; r < kDdpmDevRows; ++r)
+    const int dev_rows = S.reverse ? kReverseDevRows : kDdpmDevRows;
+    for (int r = 0; r < dev_rows; ++r)
       RS_CUDA_OK(cudaMemcpyAsync(tab + r * 1024, S.dtab.data() + (size_t)r * S.T, S.T * 4, cudaMemcpyHostToDevice, st));
   } else {
     RS_CUDA_OK(cudaMemcpyAsync(tab, S.coef1.data(), S.T * 4, cudaMemcpyHostToDevice, st));
@@ -1931,6 +1980,32 @@ int rs_ddpm_sampler_create(rs_plan* p, int steps, const double* tables, const in
   *out = s.release();
   return 0;
 }
+// DDIM inversion sampler: sqrt_recip_acp, sqrt_recipm1_acp and acp_next of the process's float64 tables, rounded to
+// fp32 as _extract_into_tensor does (reference models/gaussian_diffusion.py:92-105, :1054-1058)
+int rs_ddim_reverse_sampler_create(rs_plan* p, int steps, const double* tables, const int32_t* tmap,
+                                   const rs_ddim_reverse_options* o, rs_sampler** out) {
+  RS_CHECK(p && p->bound && out, "bad argument (plan must be bound)");
+  RS_CHECK(tables, "DDIM reverse sampler: the schedule tables are NULL");
+  RS_CHECK(o, "DDIM reverse sampler: the options are NULL");
+  RS_CHECK(p->pass == Pass::Denoiser, std::string("samplers are built on denoiser plans: this plan belongs to ") + kind_name(p->e->kind));
+  RS_CHECK(o->mean_type == RS_MEAN_EPSILON || o->mean_type == RS_MEAN_XSTART,
+           "DDIM reverse sampler: the model must predict eps or x0 (RS_MEAN_EPSILON or RS_MEAN_XSTART), got mean type " +
+           std::to_string(o->mean_type));
+  RS_CHECK(o->clip == 0 || o->clip == 1, "DDIM reverse sampler: clip must be 0 or 1, got " + std::to_string(o->clip));
+  RS_CHECK(steps >= 2 && steps <= p->max_rows && steps <= 1024,
+           "DDIM reverse sampler: steps must be in [2, " + std::to_string(std::min(p->max_rows, 1024)) +
+           "] (the plan's FiLM-table rows), got " + std::to_string(steps));
+  auto s = std::make_unique<rs_sampler>();
+  s->p = p; s->T = steps; s->ddpm = true; s->reverse = true; s->ropt = *o;
+  const int rows[kReverseDevRows] = {RS_DDPM_SQRT_RECIP_ACP, RS_DDPM_SQRT_RECIPM1_ACP, RS_DDPM_ACP_NEXT};
+  s->dtab.resize((size_t)kReverseDevRows * steps);
+  for (int r = 0; r < kReverseDevRows; ++r)
+    for (int i = 0; i < steps; ++i) s->dtab[(size_t)r * steps + i] = (float)tables[(size_t)rows[r] * steps + i];
+  s->tsteps.resize(steps);
+  for (int i = 0; i < steps; ++i) s->tsteps[i] = (float)(tmap ? tmap[i] : i);
+  *out = s.release();
+  return 0;
+}
 int rs_sampler_tables(const rs_sampler* s, float* dst) {
   RS_CHECK(s && dst, "null argument");
   RS_CHECK(!s->ddpm, "rs_sampler_tables: a DDPM sampler has no residual-shift tables");
@@ -1992,7 +2067,8 @@ int rs_sampler_set_taps(rs_sampler* s, float* pred, float* sample) {
 
 int rs_sampler_run(rs_sampler* s, const float* z_y, const float* noises, const float* lq, const float* mask,
                    float* out_latent, int use_graph, void* stream) {
-  RS_CHECK(s && (z_y || s->ddpm) && noises && lq && out_latent, "null argument");
+  RS_CHECK(!(s && s->reverse) || z_y, "DDIM reverse sampler: x_start (z_y) is NULL");
+  RS_CHECK(s && (z_y || s->ddpm) && (noises || s->reverse) && lq && out_latent, "null argument");
   int rc = check_plan_device(*s->p); if (rc) return rc;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   rc = sampler_prepare(*s, st); if (rc) return rc;
@@ -2023,12 +2099,14 @@ size_t rs_sampler_staging_bytes(const rs_sampler* s) {
   const size_t lat = align_up((size_t)P.B * c.in_channels * P.H * P.W * 4, 256);
   const size_t lq = align_up((size_t)P.B * 3 * P.lqH * P.lqW * 4, 256);
   const size_t mk = align_up((size_t)P.B * 1 * P.lqH * P.lqW * 4, 256);
-  return lat * (s->T + 3) + lq + mk;
+  const size_t n_noise = s->reverse ? 0 : (size_t)s->T + 1;      // a DDIM inversion sampler draws nothing
+  return lat * (n_noise + 2) + lq + mk;
 }
 
 int rs_sampler_run_host(rs_sampler* s, const float* z_y_h, const float* noises_h, const float* lq_h, const float* mask_h,
                         float* out_h, void* staging, size_t staging_bytes, int use_graph, void* stream) {
-  RS_CHECK(s && (z_y_h || s->ddpm) && noises_h && lq_h && out_h && staging, "null argument");
+  RS_CHECK(!(s && s->reverse) || z_y_h, "DDIM reverse sampler: x_start (z_y) is NULL");
+  RS_CHECK(s && (z_y_h || s->ddpm) && (noises_h || s->reverse) && lq_h && out_h && staging, "null argument");
   RS_CHECK(staging_bytes >= rs_sampler_staging_bytes(s), "staging buffer too small");
   { int rc = check_plan_device(*s->p); if (rc) return rc; }
   cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -2040,14 +2118,16 @@ int rs_sampler_run_host(rs_sampler* s, const float* z_y_h, const float* noises_h
   uint8_t* base = static_cast<uint8_t*>(staging);
   float* d_zy = reinterpret_cast<float*>(base);
   float* d_out = reinterpret_cast<float*>(base + lat);
+  const size_t n_noise = s->reverse ? 0 : (size_t)s->T + 1;      // as rs_sampler_staging_bytes
   float* d_noise = reinterpret_cast<float*>(base + 2 * lat);
-  float* d_lq = reinterpret_cast<float*>(base + lat * (s->T + 3));
-  float* d_mask = reinterpret_cast<float*>(base + lat * (s->T + 3) + align_up(n_lq * 4, 256));
+  float* d_lq = reinterpret_cast<float*>(base + lat * (n_noise + 2));
+  float* d_mask = reinterpret_cast<float*>(base + lat * (n_noise + 2) + align_up(n_lq * 4, 256));
   if (z_y_h) RS_CUDA_OK(cudaMemcpyAsync(d_zy, z_y_h, n_lat * 4, cudaMemcpyHostToDevice, st));
-  RS_CUDA_OK(cudaMemcpyAsync(d_noise, noises_h, n_lat * 4 * (s->T + 1), cudaMemcpyHostToDevice, st));
+  if (n_noise) RS_CUDA_OK(cudaMemcpyAsync(d_noise, noises_h, n_lat * 4 * n_noise, cudaMemcpyHostToDevice, st));
   RS_CUDA_OK(cudaMemcpyAsync(d_lq, lq_h, n_lq * 4, cudaMemcpyHostToDevice, st));
   if (mask_h) RS_CUDA_OK(cudaMemcpyAsync(d_mask, mask_h, n_mk * 4, cudaMemcpyHostToDevice, st));
-  int rc = rs_sampler_run(s, z_y_h ? d_zy : nullptr, d_noise, d_lq, mask_h ? d_mask : nullptr, d_out, use_graph, stream);
+  int rc = rs_sampler_run(s, z_y_h ? d_zy : nullptr, n_noise ? d_noise : nullptr, d_lq, mask_h ? d_mask : nullptr, d_out,
+                          use_graph, stream);
   if (rc) return rc;
   RS_CUDA_OK(cudaMemcpyAsync(out_h, d_out, n_lat * 4, cudaMemcpyDeviceToHost, st));
   RS_CUDA_OK(cudaStreamSynchronize(st));

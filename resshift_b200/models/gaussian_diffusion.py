@@ -14,10 +14,11 @@ Training (``training_losses``) is out of scope.
 
 ``SpacedDiffusionDDPM`` is the reference's other process, the classic DDPM / DDIM one (``GaussianDiffusionDDPM``,
 reference models/gaussian_diffusion.py:611-1239, models/respace.py:65-99), with its ancestral ``p_sample_loop`` and
-``ddim_sample_loop``.  With one of this package's UNets, eps or x0 prediction, a fixed variance, no ``denoised_fn``, an
-``lq`` in ``model_kwargs`` and 2 <= T <= 64, the whole loop (denoiser, x0 conversion, clamp, ancestral or DDIM update,
-next-input packing) runs inside ``librs_b200.so`` as one CUDA graph; everything else runs this module's torch port of
-the reference on the caller's device.
+``ddim_sample_loop``, and DDIM inversion (``ddim_reverse_sample``, reference :1030-1066, walked t = 0 .. T-1 by this
+package's ``ddim_reverse_sample_loop``).  With one of this package's UNets, eps or x0 prediction, a fixed variance, no
+``denoised_fn``, an ``lq`` in ``model_kwargs`` and 2 <= T <= 64, the whole loop (denoiser, x0 conversion, clamp,
+ancestral, DDIM or reverse update, next-input packing) runs inside ``librs_b200.so`` as one CUDA graph; everything else
+runs this module's torch port of the reference on the caller's device.
 """
 from __future__ import annotations
 
@@ -411,7 +412,8 @@ class ResShiftDiffusion:
 class SpacedDiffusionDDPM:
     """``SpacedDiffusionDDPM(GaussianDiffusionDDPM)`` of the reference (models/respace.py:65-99,
     models/gaussian_diffusion.py:611-1239), inference side: the respaced schedule, ``p_mean_variance`` for every
-    variance and mean type, the ancestral and DDIM steps and loops, and the first-stage bookends."""
+    variance and mean type, the ancestral and DDIM steps and loops, DDIM inversion (``ddim_reverse_sample`` and this
+    package's loop around it), and the first-stage bookends."""
 
     def __init__(self, use_timesteps, *, betas, model_mean_type, model_var_type, scale_factor=None, sf=4):
         # respacing (reference models/respace.py:74-88): the kept steps' betas from the base process's alphas_cumprod
@@ -568,6 +570,21 @@ class SpacedDiffusionDDPM:
                                    model_kwargs=model_kwargs)
         return self._ddim_finish(x, t, out, torch.randn_like(x), eta)
 
+    def _ddim_reverse_finish(self, x, t, out):
+        """the rest of reference ddim_reverse_sample (models/gaussian_diffusion.py:1052-1066) on p_mean_variance's
+        output: eps re-derived from pred_xstart, then x_{t+1} = x0 sqrt(acp_next) + sqrt(1 - acp_next) eps"""
+        eps = self._predict_eps_from_xstart(x, t, out["pred_xstart"])
+        alpha_bar_next = _tab(self.alphas_cumprod_next, t, x)
+        mean_pred = out["pred_xstart"] * torch.sqrt(alpha_bar_next) + torch.sqrt(1 - alpha_bar_next) * eps
+        return {"sample": mean_pred, "pred_xstart": out["pred_xstart"]}
+
+    def ddim_reverse_sample(self, model, x, t, clip_denoised=True, denoised_fn=None, model_kwargs=None, eta=0.0):
+        """reference models/gaussian_diffusion.py:1030-1066 — x_{t+1} from x_t by the deterministic DDIM ODE."""
+        assert eta == 0.0, "Reverse ODE only for deterministic path"
+        out = self.p_mean_variance(model, x, t, clip_denoised=clip_denoised, denoised_fn=denoised_fn,
+                                   model_kwargs=model_kwargs)
+        return self._ddim_reverse_finish(x, t, out)
+
     # ------------------------------------------------------------------ the loops
     def draw_noises(self, shape, noise=None, device=None):
         """The T + 1 noise tensors of a loop in the reference's draw order: x_T = ``noise`` or randn(*shape)
@@ -595,9 +612,28 @@ class SpacedDiffusionDDPM:
         """[8, T] float64: the rows of rs_ddpm_sampler_create (rs_ddpm_table_row)"""
         return np.ascontiguousarray(np.stack([getattr(self, name) for name in _lib.DDPM_TABLE_ROWS]), dtype=np.float64)
 
+    def ddim_reverse_tables(self) -> np.ndarray:
+        """[9, T] float64: the rows of rs_ddim_reverse_sampler_create (ddpm_tables, then alphas_cumprod_next)"""
+        return np.ascontiguousarray(np.stack([getattr(self, name) for name in _lib.DDIM_REVERSE_TABLE_ROWS]),
+                                    dtype=np.float64)
+
     def native_sampler(self, model, batch, height, width, kind: str, clip_denoised: bool, eta: float = 0.0):
-        """The plan's DDPM sampler for this process and these options ("ancestral" or "ddim"), created once."""
+        """The plan's DDPM sampler for this process and these options ("ancestral", "ddim", or "reverse" for DDIM
+        inversion, which has no eta), created once."""
         plan = model.plan(batch, height, width)
+        if kind == "reverse":
+            ropt = _lib.DdimReverseOptionsC(self._NATIVE_MEAN_TYPES[self.model_mean_type], int(bool(clip_denoised)))
+            key = ("ddim_reverse", self.num_timesteps, tuple(self.betas.tolist()), tuple(self.timestep_map),
+                   (ropt.mean_type, ropt.clip))
+            if key not in plan.samplers:
+                h = C.c_void_p()
+                tabs = self.ddim_reverse_tables()
+                tm = (C.c_int32 * self.num_timesteps)(*self.timestep_map)
+                _lib.check(_lib.lib.rs_ddim_reverse_sampler_create(plan.handle, self.num_timesteps,
+                                                                   tabs.ctypes.data_as(C.POINTER(C.c_double)), tm,
+                                                                   C.byref(ropt), C.byref(h)))
+                plan.samplers[key] = h
+            return plan.samplers[key]
         opt = _lib.DdpmOptionsC(_lib.DDPM_KINDS[kind], self._NATIVE_MEAN_TYPES[self.model_mean_type],
                                 self._NATIVE_VAR_TYPES[self.model_var_type], int(bool(clip_denoised)), float(eta))
         key = ("ddpm", self.num_timesteps, tuple(self.betas.tolist()), tuple(self.timestep_map),
@@ -660,6 +696,56 @@ class SpacedDiffusionDDPM:
         _lib.check(_lib.lib.rs_sampler_set_taps(s, preds.data_ptr(), samples.data_ptr()))
         try:
             _lib.check(_lib.lib.rs_sampler_run(s, None, nz.data_ptr(), lq.data_ptr(), _lib.ptr(mask), final.data_ptr(),
+                                               0, _lib.current_stream()))
+        finally:
+            _lib.check(_lib.lib.rs_sampler_set_taps(s, None, None))
+        for k in range(T):
+            yield {"sample": samples[k], "pred_xstart": preds[k]}
+
+    def reverse_latent(self, model, x_start, model_kwargs, clip_denoised=True, use_graph=True):
+        """The fused DDIM inversion: x_start [B, C, H, W] -> x_T, all T steps inside librs_b200 (CUDA graph replay)."""
+        if x_start.dim() != 4:
+            raise ValueError(f"x_start must have shape (B, C, H, W), got {tuple(x_start.shape)}")
+        B, Cc, H, W = x_start.shape
+        lq_in, mask_in = model_kwargs["lq"], model_kwargs.get("mask", None)
+        ResShiftDiffusion._check_native_inputs(model, x_start, lq_in, mask_in)
+        s = self.native_sampler(model, B, H, W, "reverse", clip_denoised)
+        # stable device buffers (shared with the plan's other samplers) so that the captured graph can be replayed
+        plan = model.plan(B, H, W)
+        bufs = getattr(plan, "_io", None)
+        dev = x_start.device
+        if bufs is None or bufs["lq"].shape != lq_in.shape or (mask_in is None) != (bufs["mask"] is None):
+            bufs = {"zy": torch.empty(B, Cc, H, W, dtype=torch.float32, device=dev),
+                    "noise": torch.empty(0, dtype=torch.float32, device=dev),
+                    "lq": torch.empty(lq_in.shape, dtype=torch.float32, device=dev),
+                    "mask": None if mask_in is None else torch.empty(mask_in.shape, dtype=torch.float32, device=dev),
+                    "out": torch.empty(B, Cc, H, W, dtype=torch.float32, device=dev)}
+            plan._io = bufs
+        bufs["zy"].copy_(x_start)
+        bufs["lq"].copy_(lq_in)
+        if mask_in is not None:
+            bufs["mask"].copy_(mask_in)
+        _lib.check(_lib.lib.rs_sampler_run(s, bufs["zy"].data_ptr(), None, bufs["lq"].data_ptr(),
+                                           _lib.ptr(bufs["mask"]), bufs["out"].data_ptr(), int(use_graph),
+                                           _lib.current_stream()))
+        return bufs["out"].clone()
+
+    def _native_reverse_progressive(self, model, x_start, model_kwargs, clip_denoised):
+        """The fused DDIM inversion run eagerly with the per-step taps: yields sample / pred_xstart of every step."""
+        T = self.num_timesteps
+        x = x_start.float().contiguous()
+        B, Cc, H, W = x.shape
+        lq = model_kwargs["lq"].float().contiguous()
+        mask = model_kwargs.get("mask", None)
+        mask = mask.float().contiguous() if mask is not None else None
+        ResShiftDiffusion._check_native_inputs(model, x, lq, mask)
+        s = self.native_sampler(model, B, H, W, "reverse", clip_denoised)
+        final = torch.empty_like(x)
+        preds = torch.empty((T,) + tuple(x.shape), dtype=torch.float32, device=x.device)
+        samples = torch.empty_like(preds)
+        _lib.check(_lib.lib.rs_sampler_set_taps(s, preds.data_ptr(), samples.data_ptr()))
+        try:
+            _lib.check(_lib.lib.rs_sampler_run(s, x.data_ptr(), None, lq.data_ptr(), _lib.ptr(mask), final.data_ptr(),
                                                0, _lib.current_stream()))
         finally:
             _lib.check(_lib.lib.rs_sampler_set_taps(s, None, None))
@@ -731,6 +817,41 @@ class SpacedDiffusionDDPM:
         """reference models/gaussian_diffusion.py:1068-1099 — returns the DECODED sample."""
         return self._loop("ddim", model, shape, noise, clip_denoised, denoised_fn, first_stage_model, model_kwargs,
                           device, progress, eta)
+
+    def ddim_reverse_sample_loop_progressive(self, model, x_start, clip_denoised=True, denoised_fn=None,
+                                             model_kwargs=None, device=None, progress=False):
+        """DDIM inversion, x_0 -> x_T: ``ddim_reverse_sample`` (reference models/gaussian_diffusion.py:1030-1066) for
+        t = 0 .. T-1, each step fed the previous step's sample; one dict (sample, pred_xstart) per step.  The reference
+        has the step only; this loop is this package's addition.  ``x_start`` is a latent (encode an image with
+        ``encode_first_stage`` first); ``device`` defaults to x_start's."""
+        img = x_start if device is None else x_start.to(device)
+        if self._native_ok(model, denoised_fn, model_kwargs):
+            yield from self._native_reverse_progressive(model, img, model_kwargs, clip_denoised)
+            return
+        indices = list(range(self.num_timesteps))
+        if progress:
+            from tqdm.auto import tqdm      # lazy, as the reference's loops do
+            indices = tqdm(indices)
+        for i in indices:
+            t = torch.tensor([i] * img.shape[0], device=img.device)
+            with torch.no_grad():
+                out = self.ddim_reverse_sample(model, img, t, clip_denoised=clip_denoised, denoised_fn=denoised_fn,
+                                               model_kwargs=model_kwargs)
+                yield out
+                img = out["sample"]
+
+    def ddim_reverse_sample_loop(self, model, x_start, clip_denoised=True, denoised_fn=None, model_kwargs=None,
+                                 device=None, progress=False):
+        """DDIM inversion, x_0 -> x_T (this package's loop around the reference's ``ddim_reverse_sample``, see
+        ``ddim_reverse_sample_loop_progressive``): returns the last step's sample, the latent x_T (not decoded)."""
+        if self._native_ok(model, denoised_fn, model_kwargs):
+            return self.reverse_latent(model, x_start if device is None else x_start.to(device), model_kwargs,
+                                       clip_denoised)
+        final = None
+        for sample in self.ddim_reverse_sample_loop_progressive(model, x_start, clip_denoised, denoised_fn,
+                                                                model_kwargs, device, progress):
+            final = sample["sample"]
+        return final
 
     # ------------------------------------------------------------------ first-stage bookends (PyTorch)
     def decode_first_stage(self, z_sample, first_stage_model=None):
