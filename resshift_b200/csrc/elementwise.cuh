@@ -2,8 +2,6 @@
 // embedding MLP, the residual-shift sampling update, and weight repacking.
 #pragma once
 
-#include <type_traits>
-
 #include "common.cuh"
 #include "gn_stats.cuh"
 
@@ -195,82 +193,137 @@ __global__ void linear_small_kernel(const float* __restrict__ x, const __half* _
 }
 
 // ------------------------------------------------------------------------------------------------
-// Residual-shift sampling update (reference p_sample, models/gaussian_diffusion.py:332-365, with
-// q_posterior_mean_variance :210-232):
-//     x_{t-1} = coef1[t] * x_t + coef2[t] * x0_pred + [t != 0] * std[t] * noise
-// fp32 NCHW in/out.  When `next_in` is set it also emits the NEXT denoiser input
-// cat([x_{t-1} * in_scale[t-1], lq]) as NHWC fp16 (fusing _scale_input + th.cat + layout change).
-// x0_pred comes from the model output by the parameterisation MT (reference p_mean_variance :277-292 and
-// _predict_xstart_from_* :308-324), in registers, op by op in the reference's order with no FMA contraction:
+// The sampler's step: one kernel family for the four processes the loop runs, fp32 NCHW in/out.  Every instance
+// resets the next forward's GroupNorm arrival counters, turns the model output into x0 by its mean type, applies the
+// process's update, writes x_next and, when `next_in` is set (the host leaves it NULL on a process's last step),
+// emits the NEXT denoiser input x_next (times in_scale[t-1] for ResShift) as NHWC fp16 in channels [0, C).
+//
+// ResShift (reference p_sample, models/gaussian_diffusion.py:332-365, with q_posterior_mean_variance :210-232):
+//     x_{t-1} = coef1[t] * x_t + coef2[t] * x0 + [t != 0] * std[t] * noise
+// x0 by the parameterisation MT (reference p_mean_variance :277-292 and _predict_xstart_from_* :308-324), op by op in
+// the reference's order with no FMA contraction:
 //     xstart        x0 = out
 //     residual      x0 = y - out
 //     epsilon       x0 = ((x_t - eps_coef[t] * out) - eta[t] * y) / one_minus_eta[t]
 //     epsilon_scale x0 = ((x_t - out) - eta[t] * y) / one_minus_eta[t]
 // with eps_coef = fp32(fp32(sqrt_eta) * kappa), eta = fp32(eta), one_minus_eta = fp32(1 - eta) (_extract_into_tensor
-// tables), so x0 is bit for bit the reference's fp32 expression.
+// tables), so x0 is bit for bit the reference's fp32 expression.  The xstart instance writes no x0 (it is `out`).
+//
+// GaussianDiffusionDDPM (reference models/gaussian_diffusion.py:742-1066); the denoiser sees x_t unscaled
+// (_scale_input is the identity, :1213-1214):
+//   x0       = sqrt_recip_acp[t] x_t - sqrt_recipm1_acp[t] eps (_predict_xstart_from_eps :838-843), or the model
+//              output itself for x0 prediction; clamped to [-1, 1] with clip (process_xstart :803-808)
+//   ancestral  mean = coef1[t] x0 + coef2[t] x_t (q_posterior_mean_variance :726-729);
+//              x_{t-1} = mean + [t != 0] exp(0.5 log_variance[t]) noise (p_sample :887-891)
+//   DDIM       eps' = (sqrt_recip_acp[t] x_t - x0) / sqrt_recipm1_acp[t] (_predict_eps_from_xstart :855-859);
+//              sigma = eta sqrt((1 - acp_prev) / (1 - acp)) sqrt(1 - acp / acp_prev);
+//              x_{t-1} = x0 sqrt(acp_prev) + sqrt(1 - acp_prev - sigma^2) eps' + [t != 0] sigma noise (ddim_sample
+//              :1010-1027)
+//   inversion  eps' as DDIM; x_{t+1} = x0 sqrt(acp_next[t]) + sqrt(1 - acp_next[t]) eps' (ddim_reverse_sample
+//              :1054-1064), t walking 0 .. T-1 upward; acp_next[T-1] is 0, so the last step returns eps'; nothing is drawn
+// Every operation is the reference's fp32 tensor operation on the fp32 table values (_extract_into_tensor), in its
+// order and rounded on its own (no FMA contraction); the [t != 0] factor multiplies as the reference's nonzero_mask does.
 // ------------------------------------------------------------------------------------------------
 enum MeanType : int { kMeanXstart = 0, kMeanEpsilon = 1, kMeanEpsilonScale = 2, kMeanResidual = 3 };
+enum StepProcess : int { kStepResShift = 0, kStepAncestral = 1, kStepDdim = 2, kStepInversion = 3 };
 
-struct PSampleParams {
+// The step's [T] fp32 tables, by process: row[r] is the table the plan's table region holds at r * 1024.
+enum ResShiftRow : int { kRsCoef1 = 0, kRsCoef2, kRsStd, kRsInScale, kRsEpsCoef, kRsEta, kRsOneMinusEta, kRsRows };
+enum DdpmRow : int { kDdSqrtRecipAcp = 0, kDdSqrtRecipm1Acp, kDdCoef1, kDdCoef2, kDdLogVar, kDdAcp, kDdAcpPrev, kDdRows };
+enum InversionRow : int { kInvSqrtRecipAcp = 0, kInvSqrtRecipm1Acp, kInvAcpNext, kInvRows };
+constexpr int kStepRows = 7;
+
+struct StepParams {
   const float* x_t;       // [N, C, HW]
-  const float* x0;        // [N, C, HW]: the model output (x0 itself for xstart)
-  const float* noise;     // [N, C, HW]
+  const float* out;       // [N, C, HW]: the model output
+  const float* y;         // [N, C, HW] z_y: read by the ResShift residual and epsilon types
+  const float* noise;     // [N, C, HW]: not read by inversion
   float* x_next;          // [N, C, HW]
-  const float* coef1; const float* coef2; const float* stdv; const float* in_scale;   // [T] fp32 tables
-  int t;                  // schedule index of THIS step (T-1 .. 0)
+  float* x0_out;          // optional [N, C, HW]: x0 (not written by the ResShift xstart instance)
+  const float* row[kStepRows];        // [T] fp32 tables, indexed by the process's row enum
+  float eta;              // DDIM
+  int clip;               // DDPM processes: clamp x0 to [-1, 1]
+  int t;                  // schedule index of THIS step
   int N, C, HW;
   __half* next_in; int next_cpad;     // optional: [N*HW, next_cpad]; channels [0, C) are written here
   unsigned int* zero_ptr; int zero_n; // GroupNorm arrival counters of the NEXT denoiser forward: reset here
 };
-// what the converting instances read besides (the xstart instance keeps the plain struct, and with it its code)
-struct PSamplePredParams : PSampleParams {
-  const float* y;                     // [N, C, HW] z_y
-  const float* eps_coef; const float* eta; const float* one_minus_eta;   // [T] fp32 tables of the conversions
-  float* x0_out;                      // optional [N, C, HW]: the converted x0
-};
-template <int MT>
-using PSampleParamsOf = std::conditional_t<MT == kMeanXstart, PSampleParams, PSamplePredParams>;
 
 template <int MT>
-__device__ __forceinline__ float predict_xstart(const PSamplePredParams& p, long long i, float xt) {
+__device__ __forceinline__ float predict_xstart(const StepParams& p, long long i, float xt) {
   if constexpr (MT == kMeanResidual) {
-    return __fsub_rn(p.y[i], p.x0[i]);
+    return __fsub_rn(p.y[i], p.out[i]);
   } else if constexpr (MT == kMeanEpsilon) {
-    const float num = __fsub_rn(__fsub_rn(xt, __fmul_rn(p.eps_coef[p.t], p.x0[i])), __fmul_rn(p.eta[p.t], p.y[i]));
-    return __fdiv_rn(num, p.one_minus_eta[p.t]);
+    const float num = __fsub_rn(__fsub_rn(xt, __fmul_rn(p.row[kRsEpsCoef][p.t], p.out[i])), __fmul_rn(p.row[kRsEta][p.t], p.y[i]));
+    return __fdiv_rn(num, p.row[kRsOneMinusEta][p.t]);
   } else {
     static_assert(MT == kMeanEpsilonScale, "unknown mean type");
-    const float num = __fsub_rn(__fsub_rn(xt, p.x0[i]), __fmul_rn(p.eta[p.t], p.y[i]));
-    return __fdiv_rn(num, p.one_minus_eta[p.t]);
+    const float num = __fsub_rn(__fsub_rn(xt, p.out[i]), __fmul_rn(p.row[kRsEta][p.t], p.y[i]));
+    return __fdiv_rn(num, p.row[kRsOneMinusEta][p.t]);
   }
 }
 
-template <int MT>
-__global__ void p_sample_kernel(const PSampleParamsOf<MT> p) {
+template <int PROCESS, int MT>
+__global__ void step_kernel(const StepParams p) {
   pdl_trigger();
   pdl_wait();
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i < p.zero_n) p.zero_ptr[i] = 0u;
   const long long total = (long long)p.N * p.C * p.HW;
   if (i >= total) return;
-  const float c1 = p.coef1[p.t], c2 = p.coef2[p.t];
-  const float sd = p.t != 0 ? p.stdv[p.t] : 0.f;
-  float v;
-  if constexpr (MT == kMeanXstart) {
-    v = c1 * p.x_t[i] + c2 * p.x0[i];
+  const int t = p.t;
+  const float xt = p.x_t[i];
+  // x0 (eps prediction) and eps' (DDIM, inversion) factors of the DDPM processes, read once ahead of the x0_out store
+  const float sra = p.row[kDdSqrtRecipAcp][t], srm1 = p.row[kDdSqrtRecipm1Acp][t];
+  float x0;
+  if constexpr (PROCESS == kStepResShift) {
+    if constexpr (MT == kMeanXstart) x0 = p.out[i];
+    else x0 = predict_xstart<MT>(p, i, xt);
   } else {
-    const float xt = p.x_t[i];
-    const float x0 = predict_xstart<MT>(p, i, xt);
-    if (p.x0_out) p.x0_out[i] = x0;
-    v = c1 * xt + c2 * x0;
+    static_assert(MT == kMeanEpsilon || MT == kMeanXstart, "DDPM steps predict eps or x0");
+    if constexpr (MT == kMeanEpsilon)
+      x0 = __fsub_rn(__fmul_rn(sra, xt), __fmul_rn(srm1, p.out[i]));
+    else x0 = p.out[i];
+    if (p.clip) x0 = x0 < -1.0f ? -1.0f : (x0 > 1.0f ? 1.0f : x0);     // clamp(-1, 1): NaN stays NaN
   }
-  if (p.t != 0) v += sd * p.noise[i];
+  if constexpr (PROCESS != kStepResShift || MT != kMeanXstart) {
+    if (p.x0_out) p.x0_out[i] = x0;
+  }
+  float v;
+  if constexpr (PROCESS == kStepResShift) {
+    const float c1 = p.row[kRsCoef1][t], c2 = p.row[kRsCoef2][t];
+    v = c1 * xt + c2 * x0;
+    if (t != 0) v += p.row[kRsStd][t] * p.noise[i];
+  } else if constexpr (PROCESS == kStepAncestral) {
+    const float nonzero = t != 0 ? 1.0f : 0.0f;
+    const float mean = __fadd_rn(__fmul_rn(p.row[kDdCoef1][t], x0), __fmul_rn(p.row[kDdCoef2][t], xt));
+    const float sd = expf(__fmul_rn(0.5f, p.row[kDdLogVar][t]));
+    v = __fadd_rn(mean, __fmul_rn(__fmul_rn(nonzero, sd), p.noise[i]));
+  } else {
+    static_assert((int)kDdSqrtRecipAcp == (int)kInvSqrtRecipAcp && (int)kDdSqrtRecipm1Acp == (int)kInvSqrtRecipm1Acp,
+                  "DDIM and inversion keep the eps' rows in the same place");
+    const float eps = __fdiv_rn(__fsub_rn(__fmul_rn(sra, xt), x0), srm1);
+    if constexpr (PROCESS == kStepDdim) {
+      const float nonzero = t != 0 ? 1.0f : 0.0f;
+      const float ab = p.row[kDdAcp][t], abp = p.row[kDdAcpPrev][t];
+      const float sigma = __fmul_rn(__fmul_rn(p.eta, __fsqrt_rn(__fdiv_rn(__fsub_rn(1.0f, abp), __fsub_rn(1.0f, ab)))),
+                                    __fsqrt_rn(__fsub_rn(1.0f, __fdiv_rn(ab, abp))));
+      const float mean = __fadd_rn(__fmul_rn(x0, __fsqrt_rn(abp)),
+                                   __fmul_rn(__fsqrt_rn(__fsub_rn(__fsub_rn(1.0f, abp), __fmul_rn(sigma, sigma))), eps));
+      v = __fadd_rn(mean, __fmul_rn(__fmul_rn(nonzero, sigma), p.noise[i]));
+    } else {
+      static_assert(PROCESS == kStepInversion, "unknown step process");
+      const float an = p.row[kInvAcpNext][t];
+      v = __fadd_rn(__fmul_rn(x0, __fsqrt_rn(an)), __fmul_rn(__fsqrt_rn(__fsub_rn(1.0f, an)), eps));
+    }
+  }
   p.x_next[i] = v;
-  if (p.next_in && p.t > 0) {
+  if (p.next_in) {
+    const float vin = PROCESS == kStepResShift ? v * p.row[kRsInScale][t - 1] : v;
     const int hw = (int)(i % p.HW);
     const int c = (int)((i / p.HW) % p.C);
     const int n = (int)(i / ((long long)p.HW * p.C));
-    p.next_in[((long long)n * p.HW + hw) * p.next_cpad + c] = __float2half_rn(v * p.in_scale[p.t - 1]);
+    p.next_in[((long long)n * p.HW + hw) * p.next_cpad + c] = __float2half_rn(vin);
   }
 }
 
@@ -281,138 +334,6 @@ __global__ void prior_sample_kernel(const float* __restrict__ zy, const float* _
   pdl_wait();
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i < total) out[i] = zy[i] + coef * noise[i];
-}
-
-// ------------------------------------------------------------------------------------------------
-// DDPM / DDIM steps of GaussianDiffusionDDPM (reference models/gaussian_diffusion.py:742-1028), fp32 NCHW in/out:
-//   x0       = sqrt_recip_acp[t] x_t - sqrt_recipm1_acp[t] eps (_predict_xstart_from_eps :838-843), or the model
-//              output itself for x0 prediction; clamped to [-1, 1] with clip (process_xstart :803-808)
-//   ancestral  mean = coef1[t] x0 + coef2[t] x_t (q_posterior_mean_variance :726-729);
-//              x_{t-1} = mean + [t != 0] exp(0.5 log_variance[t]) noise (p_sample :887-891)
-//   DDIM       eps' = (sqrt_recip_acp[t] x_t - x0) / sqrt_recipm1_acp[t] (_predict_eps_from_xstart :855-859);
-//              sigma = eta sqrt((1 - acp_prev) / (1 - acp)) sqrt(1 - acp / acp_prev);
-//              x_{t-1} = x0 sqrt(acp_prev) + sqrt(1 - acp_prev - sigma^2) eps' + [t != 0] sigma noise (ddim_sample
-//              :1010-1027)
-// Every operation is the reference's fp32 tensor operation on the fp32 table values (_extract_into_tensor), in its
-// order and rounded on its own (no FMA contraction); the [t != 0] factor multiplies as the reference's nonzero_mask does.
-// The denoiser sees x_t unscaled (_scale_input is the identity, :1213-1214): next_in receives fp16(x_{t-1}).
-// ------------------------------------------------------------------------------------------------
-enum DdpmKind : int { kDdpmAncestral = 0, kDdpmDdim = 1 };
-
-struct DdpmStepParams {
-  const float* x_t;       // [N, C, HW]
-  const float* out;       // [N, C, HW]: the model output (eps or x0)
-  const float* noise;     // [N, C, HW]
-  float* x_next;          // [N, C, HW]
-  const float* sqrt_recip_acp; const float* sqrt_recipm1_acp;     // [T] fp32 tables
-  const float* coef1; const float* coef2; const float* log_var;    // [T] (ancestral)
-  const float* acp; const float* acp_prev;                         // [T] (DDIM)
-  float eta;              // DDIM
-  int clip;
-  int t;                  // schedule index of THIS step (T-1 .. 0)
-  int N, C, HW;
-  __half* next_in; int next_cpad;     // optional: [N*HW, next_cpad]; channels [0, C) are written here
-  unsigned int* zero_ptr; int zero_n; // GroupNorm arrival counters of the NEXT denoiser forward: reset here
-  float* x0_out;                      // optional [N, C, HW]: pred_xstart
-};
-
-template <int KIND, int MT>
-__global__ void ddpm_step_kernel(const DdpmStepParams p) {
-  pdl_trigger();
-  pdl_wait();
-  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < p.zero_n) p.zero_ptr[i] = 0u;
-  const long long total = (long long)p.N * p.C * p.HW;
-  if (i >= total) return;
-  const int t = p.t;
-  const float xt = p.x_t[i];
-  const float nonzero = t != 0 ? 1.0f : 0.0f;
-  float x0;
-  if constexpr (MT == kMeanEpsilon) {
-    x0 = __fsub_rn(__fmul_rn(p.sqrt_recip_acp[t], xt), __fmul_rn(p.sqrt_recipm1_acp[t], p.out[i]));
-  } else {
-    static_assert(MT == kMeanXstart, "DDPM steps predict eps or x0");
-    x0 = p.out[i];
-  }
-  if (p.clip) x0 = x0 < -1.0f ? -1.0f : (x0 > 1.0f ? 1.0f : x0);     // clamp(-1, 1): NaN stays NaN
-  if (p.x0_out) p.x0_out[i] = x0;
-  float v;
-  if constexpr (KIND == kDdpmAncestral) {
-    const float mean = __fadd_rn(__fmul_rn(p.coef1[t], x0), __fmul_rn(p.coef2[t], xt));
-    const float sd = expf(__fmul_rn(0.5f, p.log_var[t]));
-    v = __fadd_rn(mean, __fmul_rn(__fmul_rn(nonzero, sd), p.noise[i]));
-  } else {
-    static_assert(KIND == kDdpmDdim, "unknown DDPM step");
-    const float ab = p.acp[t], abp = p.acp_prev[t];
-    const float eps = __fdiv_rn(__fsub_rn(__fmul_rn(p.sqrt_recip_acp[t], xt), x0), p.sqrt_recipm1_acp[t]);
-    const float sigma = __fmul_rn(__fmul_rn(p.eta, __fsqrt_rn(__fdiv_rn(__fsub_rn(1.0f, abp), __fsub_rn(1.0f, ab)))),
-                                  __fsqrt_rn(__fsub_rn(1.0f, __fdiv_rn(ab, abp))));
-    const float mean = __fadd_rn(__fmul_rn(x0, __fsqrt_rn(abp)),
-                                 __fmul_rn(__fsqrt_rn(__fsub_rn(__fsub_rn(1.0f, abp), __fmul_rn(sigma, sigma))), eps));
-    v = __fadd_rn(mean, __fmul_rn(__fmul_rn(nonzero, sigma), p.noise[i]));
-  }
-  p.x_next[i] = v;
-  if (p.next_in && t > 0) {
-    const int hw = (int)(i % p.HW);
-    const int c = (int)((i / p.HW) % p.C);
-    const int n = (int)(i / ((long long)p.HW * p.C));
-    p.next_in[((long long)n * p.HW + hw) * p.next_cpad + c] = __float2half_rn(v);
-  }
-}
-
-// ------------------------------------------------------------------------------------------------
-// DDIM inversion step of GaussianDiffusionDDPM.ddim_reverse_sample (reference models/gaussian_diffusion.py:1030-1066),
-// fp32 NCHW in/out, t walking 0 .. T-1 upward:
-//   x0       as ddpm_step_kernel (eps or x0 prediction, clamped to [-1, 1] with clip)
-//   eps'     = (sqrt_recip_acp[t] x_t - x0) / sqrt_recipm1_acp[t]                               (:1054-1057)
-//   x_{t+1}  = x0 sqrt(acp_next[t]) + sqrt(1 - acp_next[t]) eps'                                (:1058-1064)
-// acp_next[T-1] is 0, so the last step returns eps'.  Every operation is the reference's fp32 tensor operation on the
-// fp32 table values, in its order and rounded on its own (no FMA contraction); nothing is drawn.
-// next_in receives fp16(x_{t+1}) for t < T - 1 (the denoiser sees x_t unscaled).
-// ------------------------------------------------------------------------------------------------
-struct DdimReverseStepParams {
-  const float* x_t;       // [N, C, HW]
-  const float* out;       // [N, C, HW]: the model output (eps or x0)
-  float* x_next;          // [N, C, HW]
-  const float* sqrt_recip_acp; const float* sqrt_recipm1_acp; const float* acp_next;   // [T] fp32 tables
-  int clip;
-  int T, t;               // t: schedule index of THIS step (0 .. T-1)
-  int N, C, HW;
-  __half* next_in; int next_cpad;     // optional: [N*HW, next_cpad]; channels [0, C) are written here
-  unsigned int* zero_ptr; int zero_n; // GroupNorm arrival counters of the NEXT denoiser forward: reset here
-  float* x0_out;                      // optional [N, C, HW]: pred_xstart
-};
-
-template <int MT>
-__global__ void ddim_reverse_step_kernel(const DdimReverseStepParams p) {
-  pdl_trigger();
-  pdl_wait();
-  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < p.zero_n) p.zero_ptr[i] = 0u;
-  const long long total = (long long)p.N * p.C * p.HW;
-  if (i >= total) return;
-  const int t = p.t;
-  const float xt = p.x_t[i];
-  const float sra = p.sqrt_recip_acp[t], srm1 = p.sqrt_recipm1_acp[t];
-  float x0;
-  if constexpr (MT == kMeanEpsilon) {
-    x0 = __fsub_rn(__fmul_rn(sra, xt), __fmul_rn(srm1, p.out[i]));
-  } else {
-    static_assert(MT == kMeanXstart, "DDIM inversion predicts eps or x0");
-    x0 = p.out[i];
-  }
-  if (p.clip) x0 = x0 < -1.0f ? -1.0f : (x0 > 1.0f ? 1.0f : x0);     // clamp(-1, 1): NaN stays NaN
-  if (p.x0_out) p.x0_out[i] = x0;
-  const float an = p.acp_next[t];
-  const float eps = __fdiv_rn(__fsub_rn(__fmul_rn(sra, xt), x0), srm1);
-  const float v = __fadd_rn(__fmul_rn(x0, __fsqrt_rn(an)), __fmul_rn(__fsqrt_rn(__fsub_rn(1.0f, an)), eps));
-  p.x_next[i] = v;
-  if (p.next_in && t + 1 < p.T) {
-    const int hw = (int)(i % p.HW);
-    const int c = (int)((i / p.HW) % p.C);
-    const int n = (int)(i / ((long long)p.HW * p.C));
-    p.next_in[((long long)n * p.HW + hw) * p.next_cpad + c] = __float2half_rn(v);
-  }
 }
 
 // ------------------------------------------------------------------------------------------------

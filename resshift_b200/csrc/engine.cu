@@ -816,7 +816,7 @@ int finish_layout(rs_plan& P, Builder& b, size_t state_bytes, bool unet) {
   size_t off = 0;
   auto region = [&](size_t bytes) { size_t o = off; off = align_up(off + bytes, 256); return o; };
   if (unet) {
-    P.off_tables = region(7 * 1024 * sizeof(float));   // coef1, coef2, std, in_scale, eps_coef, eta, 1 - eta (<= 1024 steps)
+    P.off_tables = region(kStepRows * 1024 * sizeof(float));   // the sampler's step tables (StepParams::row), <= 1024 steps each
     P.off_tsteps = region((size_t)P.max_rows * sizeof(float));
     P.off_emb_sin = region((size_t)P.max_rows * c.model_channels * sizeof(float));
     P.off_emb_mid = region((size_t)P.max_rows * E.time_dim() * sizeof(float));
@@ -1670,19 +1670,16 @@ int rs_plan_probe(rs_plan* p, const char* block, float* dst, int32_t* channels, 
 struct rs_sampler {
   rs_plan* p = nullptr;
   int T = 0;
-  double kappa = 0;
-  std::vector<float> coef1, coef2, stdv, in_scale, tsteps;
-  std::vector<float> eps_coef, eta, one_minus_eta;     // x0 conversions of the epsilon parameterisations
-  float prior_coef = 0;
-  rs_sampler_options opt{RS_MEAN_XSTART, 1, 1};
-  // DDPM / DDIM sampler (rs_ddpm_sampler_create): its options and fp32 tables, kDdpmDevRows rows of T
-  bool ddpm = false;
-  rs_ddpm_options dopt{};
-  std::vector<float> dtab;
-  // DDIM inversion sampler (rs_ddim_reverse_sampler_create; ddpm is set too): x_start comes in as z_y, nothing is
-  // drawn, and dtab holds kReverseDevRows rows of T
-  bool reverse = false;
-  rs_ddim_reverse_options ropt{};
+  // the process (StepProcess) and the scalars its step reads
+  int process = kStepResShift;
+  int mean_type = RS_MEAN_XSTART;
+  int clip = 0;                 // DDPM processes: clamp x0 to [-1, 1]
+  float eta = 0;                // DDIM
+  float prior_coef = 0;         // ResShift: kappa * sqrt_eta[T - 1]
+  // rows x T fp32: row r is what the plan's table region holds at r * 1024 (the process's row enum)
+  int rows = 0;
+  std::vector<float> tab;
+  std::vector<float> tsteps;    // [T] the model's timesteps
   float* tap_pred = nullptr; float* tap_sample = nullptr;
   cudaGraphExec_t graph = nullptr;
   cudaStream_t cap_stream = nullptr;     // capture happens on a private stream (the legacy default stream cannot capture)
@@ -1695,154 +1692,88 @@ namespace {
 static_assert((int)kMeanXstart == (int)RS_MEAN_XSTART && (int)kMeanEpsilon == (int)RS_MEAN_EPSILON &&
               (int)kMeanEpsilonScale == (int)RS_MEAN_EPSILON_SCALE && (int)kMeanResidual == (int)RS_MEAN_RESIDUAL,
               "MeanType mirrors rs_mean_type");
+static_assert(kRsRows <= kStepRows && kDdRows <= kStepRows && kInvRows <= kStepRows, "the table region holds every row");
 
-// p_sample_kernel instance of a mean type (rs_sampler_options::mean_type); unknown types are refused
-int launch_p_sample(int mean_type, const PSamplePredParams& pp, long long numel, cudaStream_t st) {
+// what rs_sampler_run reads of a process: z_y (the ResShift conditioning, or the inversion's x_start), and the T + 1
+// noises (the first state, then one per step) of every process but inversion
+bool reads_zy(const rs_sampler& s) { return s.process == kStepResShift || s.process == kStepInversion; }
+size_t noise_count(const rs_sampler& s) { return s.process == kStepInversion ? 0 : (size_t)s.T + 1; }
+// whether the step at t has a next step (whose denoiser input it packs): t walks down to 0, or up to T - 1 in inversion
+bool step_has_next(int process, int t, int T) { return process == kStepInversion ? t + 1 < T : t > 0; }
+
+// the step_kernel instance of (process, mean type), with the grid every caller launches; combinations without an
+// instance are refused.  The ResShift xstart instance writes no x0: x0_out receives a copy of the model output, ahead.
+int launch_step(int process, int mean_type, const StepParams& sp, cudaStream_t st) {
+  const long long numel = (long long)sp.N * sp.C * sp.HW;
   const dim3 grid((unsigned)((numel + 255) / 256)), block(256);
-  switch (mean_type) {
-    case RS_MEAN_XSTART: (void)launch_k(p_sample_kernel<kMeanXstart>, grid, block, (size_t)(0), st, PSampleParams(pp)); break;
-    case RS_MEAN_EPSILON: (void)launch_k(p_sample_kernel<kMeanEpsilon>, grid, block, (size_t)(0), st, pp); break;
-    case RS_MEAN_EPSILON_SCALE: (void)launch_k(p_sample_kernel<kMeanEpsilonScale>, grid, block, (size_t)(0), st, pp); break;
-    case RS_MEAN_RESIDUAL: (void)launch_k(p_sample_kernel<kMeanResidual>, grid, block, (size_t)(0), st, pp); break;
-    default: RS_CHECK(false, "unknown mean type " + std::to_string(mean_type) + " (RS_MEAN_XSTART .. RS_MEAN_RESIDUAL)");
+  auto go = [&](void (*kernel)(const StepParams)) {
+    (void)launch_k(kernel, grid, block, (size_t)(0), st, sp);
+    RS_CUDA_OK(cudaGetLastError());
+    return 0;
+  };
+  const bool eps = mean_type == RS_MEAN_EPSILON, x0 = mean_type == RS_MEAN_XSTART;
+  switch (process) {
+    case kStepResShift:
+      if (x0 && sp.x0_out) RS_CUDA_OK(cudaMemcpyAsync(sp.x0_out, sp.out, (size_t)numel * 4, cudaMemcpyDeviceToDevice, st));
+      if (x0) return go(step_kernel<kStepResShift, kMeanXstart>);
+      if (eps) return go(step_kernel<kStepResShift, kMeanEpsilon>);
+      if (mean_type == RS_MEAN_EPSILON_SCALE) return go(step_kernel<kStepResShift, kMeanEpsilonScale>);
+      if (mean_type == RS_MEAN_RESIDUAL) return go(step_kernel<kStepResShift, kMeanResidual>);
+      break;
+    case kStepAncestral:
+      if (eps) return go(step_kernel<kStepAncestral, kMeanEpsilon>);
+      if (x0) return go(step_kernel<kStepAncestral, kMeanXstart>);
+      break;
+    case kStepDdim:
+      if (eps) return go(step_kernel<kStepDdim, kMeanEpsilon>);
+      if (x0) return go(step_kernel<kStepDdim, kMeanXstart>);
+      break;
+    case kStepInversion:
+      if (eps) return go(step_kernel<kStepInversion, kMeanEpsilon>);
+      if (x0) return go(step_kernel<kStepInversion, kMeanXstart>);
+      break;
   }
-  return 0;
+  return ::rs::fail(-1, "no step kernel for process " + std::to_string(process) + " and mean type " + std::to_string(mean_type));
 }
 
-// the DDPM sampler's fp32 tables in the plan's table region, one 1024-entry row each: sqrt_recip_acp,
-// sqrt_recipm1_acp, coef1, coef2, the log variance of its var_type, acp, acp_prev
-constexpr int kDdpmDevRows = 7;
-
-void ddpm_tables(DdpmStepParams& dp, const float* tab, int ld) {
-  dp.sqrt_recip_acp = tab; dp.sqrt_recipm1_acp = tab + ld; dp.coef1 = tab + 2 * ld; dp.coef2 = tab + 3 * ld;
-  dp.log_var = tab + 4 * ld; dp.acp = tab + 5 * ld; dp.acp_prev = tab + 6 * ld;
-}
-
-// ddpm_step_kernel instance of (kind, mean type); unknown values are refused
-int launch_ddpm_step(int kind, int mean_type, const DdpmStepParams& dp, long long numel, cudaStream_t st) {
-  const dim3 grid((unsigned)((numel + 255) / 256)), block(256);
-  RS_CHECK(kind == RS_DDPM_ANCESTRAL || kind == RS_DDPM_DDIM,
-           "unknown DDPM sampler kind " + std::to_string(kind) + " (RS_DDPM_ANCESTRAL or RS_DDPM_DDIM)");
-  RS_CHECK(mean_type == RS_MEAN_EPSILON || mean_type == RS_MEAN_XSTART,
-           "DDPM steps predict eps or x0 (RS_MEAN_EPSILON or RS_MEAN_XSTART), got mean type " + std::to_string(mean_type));
-  const bool eps = mean_type == RS_MEAN_EPSILON;
-  if (kind == RS_DDPM_ANCESTRAL) {
-    if (eps) (void)launch_k(ddpm_step_kernel<kDdpmAncestral, kMeanEpsilon>, grid, block, (size_t)(0), st, dp);
-    else (void)launch_k(ddpm_step_kernel<kDdpmAncestral, kMeanXstart>, grid, block, (size_t)(0), st, dp);
-  } else {
-    if (eps) (void)launch_k(ddpm_step_kernel<kDdpmDdim, kMeanEpsilon>, grid, block, (size_t)(0), st, dp);
-    else (void)launch_k(ddpm_step_kernel<kDdpmDdim, kMeanXstart>, grid, block, (size_t)(0), st, dp);
-  }
-  return 0;
-}
-
-// the DDIM inversion sampler's fp32 tables in the plan's table region, one 1024-entry row each: sqrt_recip_acp,
-// sqrt_recipm1_acp, acp_next
-constexpr int kReverseDevRows = 3;
-
-// ddim_reverse_step_kernel instance of a mean type; unknown values are refused
-int launch_ddim_reverse_step(int mean_type, const DdimReverseStepParams& rp, long long numel, cudaStream_t st) {
-  const dim3 grid((unsigned)((numel + 255) / 256)), block(256);
-  RS_CHECK(mean_type == RS_MEAN_EPSILON || mean_type == RS_MEAN_XSTART,
-           "DDIM inversion predicts eps or x0 (RS_MEAN_EPSILON or RS_MEAN_XSTART), got mean type " + std::to_string(mean_type));
-  if (mean_type == RS_MEAN_EPSILON) (void)launch_k(ddim_reverse_step_kernel<kMeanEpsilon>, grid, block, (size_t)(0), st, rp);
-  else (void)launch_k(ddim_reverse_step_kernel<kMeanXstart>, grid, block, (size_t)(0), st, rp);
-  return 0;
-}
-
-// x = x_start; then for t = 0 .. T-1 the denoiser on x (unscaled) and the reverse step; the last writes out_latent
-int reverse_enqueue(rs_sampler& S, const float* x_start, const float* lq, const float* mask, float* out_latent,
-                    cudaStream_t st) {
+// The fused loop of every process.  x at the first step is x_T = z_y + kappa sqrt_eta_T noises[0] (ResShift
+// prior_sample), noises[0] (ancestral, DDIM) or z_y (inversion's x_start); then per step the denoiser on x (scaled by
+// in_scale[t] for ResShift) with FiLM row t, and one step launch; the last step writes out_latent.
+int sampler_enqueue(rs_sampler& S, const float* z_y, const float* noises, const float* lq, const float* mask,
+                    float* out_latent, cudaStream_t st) {
   rs_plan& P = *S.p;
   const rs_unet_config& c = P.e->cfg;
   RS_CHECK(c.in_channels == c.out_channels, "the sampler needs out_channels == in_channels (x0 and x_t share a shape)");
   const long long numel = (long long)P.B * c.in_channels * P.H * P.W;
   float* state = reinterpret_cast<float*>(P.ws + P.off_state);
   const float* tab = reinterpret_cast<const float*>(P.ws + P.off_tables);
-  int rc = pack_lq_and_input(P, x_start, lq, mask, nullptr, 0, st); if (rc) return rc;
-  const float* film_all = reinterpret_cast<const float*>(P.ws + P.off_film);
-  for (int t = 0; t < S.T; ++t) {
-    rc = run_ops(P, P.ops, film_all + (long long)t * P.e->film_rows, 0, st); if (rc) return rc;
-    DdimReverseStepParams rp{};
-    rp.x_t = t == 0 ? x_start : state; rp.out = P.out_f32;
-    rp.x_next = (t == S.T - 1) ? out_latent : state;
-    rp.sqrt_recip_acp = tab; rp.sqrt_recipm1_acp = tab + 1024; rp.acp_next = tab + 2048;
-    rp.clip = S.ropt.clip; rp.T = S.T; rp.t = t;
-    rp.N = P.B; rp.C = c.in_channels; rp.HW = P.H * P.W;
-    rp.next_in = P.xin.ptr; rp.next_cpad = P.cin_pad;
-    rp.zero_ptr = reinterpret_cast<unsigned int*>(P.ws + P.off_counters); rp.zero_n = P.n_gn * P.B;
-    if (S.tap_pred) rp.x0_out = S.tap_pred + (long long)t * numel;
-    rc = launch_ddim_reverse_step(S.ropt.mean_type, rp, numel, st); if (rc) return rc;
-    if (S.tap_sample) RS_CUDA_OK(cudaMemcpyAsync(S.tap_sample + (long long)t * numel, rp.x_next, numel * 4, cudaMemcpyDeviceToDevice, st));
+  const bool resshift = S.process == kStepResShift, inversion = S.process == kStepInversion;
+  const float* x = inversion ? z_y : noises;
+  if (resshift) {
+    (void)launch_k(prior_sample_kernel, dim3((unsigned)((numel + 255) / 256)), dim3(256), (size_t)(0), st, z_y, noises, state, S.prior_coef, numel);
+    x = state;
   }
-  RS_CUDA_OK(cudaGetLastError());
-  return 0;
-}
-
-// x_T = noises[0]; then per step the denoiser on x_t (unscaled) and the DDPM / DDIM step
-int ddpm_enqueue(rs_sampler& S, const float* noises, const float* lq, const float* mask, float* out_latent,
-                 cudaStream_t st) {
-  rs_plan& P = *S.p;
-  const rs_unet_config& c = P.e->cfg;
-  RS_CHECK(c.in_channels == c.out_channels, "the sampler needs out_channels == in_channels (x0 and x_t share a shape)");
-  const long long numel = (long long)P.B * c.in_channels * P.H * P.W;
-  float* state = reinterpret_cast<float*>(P.ws + P.off_state);
-  int rc = pack_lq_and_input(P, noises, lq, mask, nullptr, 0, st); if (rc) return rc;
+  // LQ feature (once) + the first packed input
+  int rc = pack_lq_and_input(P, x, lq, mask, resshift ? tab + kRsInScale * 1024 : nullptr, S.T - 1, st); if (rc) return rc;
   const float* film_all = reinterpret_cast<const float*>(P.ws + P.off_film);
+  StepParams sp{};
+  sp.out = P.out_f32; sp.y = z_y;
+  for (int r = 0; r < S.rows; ++r) sp.row[r] = tab + r * 1024;
+  sp.eta = S.eta; sp.clip = S.clip;
+  sp.N = P.B; sp.C = c.in_channels; sp.HW = P.H * P.W;
+  sp.next_cpad = P.cin_pad;
+  sp.zero_ptr = reinterpret_cast<unsigned int*>(P.ws + P.off_counters); sp.zero_n = P.n_gn * P.B;
   for (int k = 0; k < S.T; ++k) {
-    const int t = S.T - 1 - k;
+    const int t = inversion ? k : S.T - 1 - k;
     rc = run_ops(P, P.ops, film_all + (long long)t * P.e->film_rows, 0, st); if (rc) return rc;
-    DdpmStepParams dp{};
-    dp.x_t = k == 0 ? noises : state; dp.out = P.out_f32; dp.noise = noises + (long long)(k + 1) * numel;
-    dp.x_next = (t == 0) ? out_latent : state;
-    ddpm_tables(dp, reinterpret_cast<const float*>(P.ws + P.off_tables), 1024);
-    dp.eta = (float)S.dopt.eta; dp.clip = S.dopt.clip; dp.t = t;
-    dp.N = P.B; dp.C = c.in_channels; dp.HW = P.H * P.W;
-    dp.next_in = P.xin.ptr; dp.next_cpad = P.cin_pad;
-    dp.zero_ptr = reinterpret_cast<unsigned int*>(P.ws + P.off_counters); dp.zero_n = P.n_gn * P.B;
-    if (S.tap_pred) dp.x0_out = S.tap_pred + (long long)k * numel;
-    rc = launch_ddpm_step(S.dopt.kind, S.dopt.mean_type, dp, numel, st); if (rc) return rc;
-    if (S.tap_sample) RS_CUDA_OK(cudaMemcpyAsync(S.tap_sample + (long long)k * numel, dp.x_next, numel * 4, cudaMemcpyDeviceToDevice, st));
-  }
-  RS_CUDA_OK(cudaGetLastError());
-  return 0;
-}
-
-int sampler_enqueue(rs_sampler& S, const float* z_y, const float* noises, const float* lq, const float* mask,
-                    float* out_latent, cudaStream_t st) {
-  if (S.reverse) return reverse_enqueue(S, z_y, lq, mask, out_latent, st);
-  if (S.ddpm) return ddpm_enqueue(S, noises, lq, mask, out_latent, st);
-  rs_plan& P = *S.p;
-  const rs_unet_config& c = P.e->cfg;
-  RS_CHECK(c.in_channels == c.out_channels, "the sampler needs out_channels == in_channels (x0, x_t and z_y share a shape)");
-  const long long numel = (long long)P.B * c.in_channels * P.H * P.W;
-  const size_t lat = align_up((size_t)numel * 4, 256);
-  float* x_t = reinterpret_cast<float*>(P.ws + P.off_state);
-  float* tab = reinterpret_cast<float*>(P.ws + P.off_tables);
-  const float* coef1 = tab, *coef2 = tab + 1024, *stdv = tab + 2048, *in_scale = tab + 3072;
-  const bool xstart = S.opt.mean_type == RS_MEAN_XSTART;
-  (void)lat;
-  // x_T = z_y + kappa * sqrt_eta_T * noise_0   (prior_sample)
-  (void)launch_k(prior_sample_kernel, dim3((unsigned)((numel + 255) / 256)), dim3(256), (size_t)(0), st, z_y, noises, x_t, S.prior_coef, numel);
-  // LQ feature (once) + first packed input, scaled by in_scale[T-1]
-  int rc = pack_lq_and_input(P, x_t, lq, mask, in_scale, S.T - 1, st); if (rc) return rc;
-  const float* film_all = reinterpret_cast<const float*>(P.ws + P.off_film);
-  for (int k = 0; k < S.T; ++k) {
-    const int t = S.T - 1 - k;
-    rc = run_ops(P, P.ops, film_all + (long long)t * P.e->film_rows, 0, st); if (rc) return rc;
-    PSamplePredParams pp{};
-    pp.x_t = x_t; pp.x0 = P.out_f32; pp.noise = noises + (long long)(k + 1) * numel;
-    pp.x_next = (t == 0) ? out_latent : x_t;
-    pp.coef1 = coef1; pp.coef2 = coef2; pp.stdv = stdv; pp.in_scale = in_scale; pp.t = t;
-    pp.N = P.B; pp.C = c.in_channels; pp.HW = P.H * P.W;
-    pp.next_in = P.xin.ptr; pp.next_cpad = P.cin_pad;
-    pp.zero_ptr = reinterpret_cast<unsigned int*>(P.ws + P.off_counters); pp.zero_n = P.n_gn * P.B;
-    pp.y = z_y; pp.eps_coef = tab + 4096; pp.eta = tab + 5120; pp.one_minus_eta = tab + 6144;
-    // the pred_xstart tap: the head output itself for xstart, the step kernel's converted x0 otherwise
-    if (S.tap_pred && xstart) RS_CUDA_OK(cudaMemcpyAsync(S.tap_pred + (long long)k * numel, P.out_f32, numel * 4, cudaMemcpyDeviceToDevice, st));
-    if (S.tap_pred && !xstart) pp.x0_out = S.tap_pred + (long long)k * numel;
-    rc = launch_p_sample(S.opt.mean_type, pp, numel, st); if (rc) return rc;
-    if (S.tap_sample) RS_CUDA_OK(cudaMemcpyAsync(S.tap_sample + (long long)k * numel, pp.x_next, numel * 4, cudaMemcpyDeviceToDevice, st));
+    sp.x_t = k == 0 ? x : state;
+    sp.noise = inversion ? nullptr : noises + (long long)(k + 1) * numel;
+    sp.x_next = k == S.T - 1 ? out_latent : state;
+    sp.t = t;
+    sp.next_in = step_has_next(S.process, t, S.T) ? P.xin.ptr : nullptr;
+    sp.x0_out = S.tap_pred ? S.tap_pred + (long long)k * numel : nullptr;
+    rc = launch_step(S.process, S.mean_type, sp, st); if (rc) return rc;
+    if (S.tap_sample) RS_CUDA_OK(cudaMemcpyAsync(S.tap_sample + (long long)k * numel, sp.x_next, numel * 4, cudaMemcpyDeviceToDevice, st));
   }
   RS_CUDA_OK(cudaGetLastError());
   return 0;
@@ -1854,21 +1785,8 @@ int sampler_prepare(rs_sampler& S, cudaStream_t st) {
   rs_plan& P = *S.p;
   if (P.table_owner == &S && P.table_epoch == P.e->weights_epoch) return 0;
   float* tab = reinterpret_cast<float*>(P.ws + P.off_tables);
-  if (S.ddpm) {
-    const int dev_rows = S.reverse ? kReverseDevRows : kDdpmDevRows;
-    for (int r = 0; r < dev_rows; ++r)
-      RS_CUDA_OK(cudaMemcpyAsync(tab + r * 1024, S.dtab.data() + (size_t)r * S.T, S.T * 4, cudaMemcpyHostToDevice, st));
-  } else {
-    RS_CUDA_OK(cudaMemcpyAsync(tab, S.coef1.data(), S.T * 4, cudaMemcpyHostToDevice, st));
-    RS_CUDA_OK(cudaMemcpyAsync(tab + 1024, S.coef2.data(), S.T * 4, cudaMemcpyHostToDevice, st));
-    RS_CUDA_OK(cudaMemcpyAsync(tab + 2048, S.stdv.data(), S.T * 4, cudaMemcpyHostToDevice, st));
-    RS_CUDA_OK(cudaMemcpyAsync(tab + 3072, S.in_scale.data(), S.T * 4, cudaMemcpyHostToDevice, st));
-  }
-  if (!S.ddpm && S.opt.mean_type != RS_MEAN_XSTART) {
-    RS_CUDA_OK(cudaMemcpyAsync(tab + 4096, S.eps_coef.data(), S.T * 4, cudaMemcpyHostToDevice, st));
-    RS_CUDA_OK(cudaMemcpyAsync(tab + 5120, S.eta.data(), S.T * 4, cudaMemcpyHostToDevice, st));
-    RS_CUDA_OK(cudaMemcpyAsync(tab + 6144, S.one_minus_eta.data(), S.T * 4, cudaMemcpyHostToDevice, st));
-  }
+  for (int r = 0; r < S.rows; ++r)
+    RS_CUDA_OK(cudaMemcpyAsync(tab + r * 1024, S.tab.data() + (size_t)r * S.T, S.T * 4, cudaMemcpyHostToDevice, st));
   float* ts = reinterpret_cast<float*>(P.ws + P.off_tsteps);
   RS_CUDA_OK(cudaMemcpyAsync(ts, S.tsteps.data(), S.T * 4, cudaMemcpyHostToDevice, st));
   int rc = run_embedding(P, ts, S.T, st); if (rc) return rc;
@@ -1890,27 +1808,28 @@ static void schedule_tables(rs_sampler& s, int steps, const double* sqrt_etas, d
   std::vector<double> etas(steps), prev(steps), alpha(steps), pv(steps);
   for (int i = 0; i < steps; ++i) etas[i] = sqrt_etas[i] * sqrt_etas[i];
   for (int i = 0; i < steps; ++i) { prev[i] = i ? etas[i - 1] : 0.0; alpha[i] = etas[i] - prev[i]; pv[i] = kappa * kappa * prev[i] / etas[i] * alpha[i]; }
-  s.T = steps; s.kappa = kappa; s.opt = opt;
-  s.coef1.resize(steps); s.coef2.resize(steps); s.stdv.resize(steps); s.in_scale.resize(steps); s.tsteps.resize(steps);
-  s.eps_coef.resize(steps); s.eta.resize(steps); s.one_minus_eta.resize(steps);
+  s.T = steps; s.rows = kRsRows; s.mean_type = opt.mean_type;
+  s.tab.resize((size_t)kRsRows * steps); s.tsteps.resize(steps);
+  float* row[kRsRows];
+  for (int r = 0; r < kRsRows; ++r) row[r] = s.tab.data() + (size_t)r * steps;
   for (int i = 0; i < steps; ++i) {
     const double pvc = pv[i == 0 ? 1 : i];
-    s.coef1[i] = (float)(prev[i] / etas[i]);
-    s.coef2[i] = (float)(alpha[i] / etas[i]);
+    row[kRsCoef1][i] = (float)(prev[i] / etas[i]);
+    row[kRsCoef2][i] = (float)(alpha[i] / etas[i]);
     const float logv = (float)std::log(pvc);
-    s.stdv[i] = std::exp(0.5f * logv);
+    row[kRsStd][i] = std::exp(0.5f * logv);
     const float e32 = (float)etas[i];
     if (!opt.normalize_input) {
-      s.in_scale[i] = 1.0f;
+      row[kRsInScale][i] = 1.0f;
     } else if (opt.latent_flag) {
-      s.in_scale[i] = 1.0f / std::sqrt(e32 * (float)(kappa * kappa) + 1.0f);
+      row[kRsInScale][i] = 1.0f / std::sqrt(e32 * (float)(kappa * kappa) + 1.0f);
     } else {
-      s.in_scale[i] = 1.0f / ((float)sqrt_etas[i] * (float)kappa * 3.0f + 1.0f);
+      row[kRsInScale][i] = 1.0f / ((float)sqrt_etas[i] * (float)kappa * 3.0f + 1.0f);
     }
     s.tsteps[i] = (float)(tmap ? tmap[i] : i);
-    s.eps_coef[i] = (float)sqrt_etas[i] * (float)kappa;
-    s.eta[i] = e32;
-    s.one_minus_eta[i] = (float)(1.0 - etas[i]);
+    row[kRsEpsCoef][i] = (float)sqrt_etas[i] * (float)kappa;
+    row[kRsEta][i] = e32;
+    row[kRsOneMinusEta][i] = (float)(1.0 - etas[i]);
   }
   s.prior_coef = (float)(kappa * sqrt_etas[steps - 1]);
 }
@@ -1923,22 +1842,41 @@ static int check_sampler_options(const rs_sampler_options& o) {
   return 0;
 }
 
-static void copy_tables(const rs_sampler& s, float* dst) {
-  for (const std::vector<float>* v : {&s.coef1, &s.coef2, &s.stdv, &s.in_scale, &s.tsteps}) {
-    std::memcpy(dst, v->data(), (size_t)s.T * sizeof(float));
-    dst += s.T;
-  }
-  *dst = s.prior_coef;
+// rs_sampler_tables' layout: coef1, coef2, std, in_scale, the timesteps (T each), then the prior coefficient; returns
+// the end of what it wrote
+static float* copy_tables(const rs_sampler& s, float* dst) {
+  std::memcpy(dst, s.tab.data(), (size_t)4 * s.T * sizeof(float));
+  std::memcpy(dst + 4 * s.T, s.tsteps.data(), (size_t)s.T * sizeof(float));
+  dst[5 * s.T] = s.prior_coef;
+  return dst + 5 * s.T + 1;
+}
+
+// A sampler of `process` on plan p (bound): the checks every sampler shares (`who` names it in the steps refusal),
+// the timestep row, and table row r = the float64 row rows[r] of `tables` ([*][steps], rs_ddpm_table_row order)
+// rounded to fp32 as _extract_into_tensor does (reference models/gaussian_diffusion.py:92-105)
+static int sampler_new(rs_plan* p, int process, int steps, const int32_t* tmap, const char* who, const double* tables,
+                       std::initializer_list<int> rows, std::unique_ptr<rs_sampler>& s) {
+  RS_CHECK(p->pass == Pass::Denoiser, std::string("samplers are built on denoiser plans: this plan belongs to ") + kind_name(p->e->kind));
+  RS_CHECK(steps >= 2 && steps <= p->max_rows && steps <= 1024,
+           std::string(who) + ": steps must be in [2, " + std::to_string(std::min(p->max_rows, 1024)) +
+           "] (the plan's FiLM-table rows), got " + std::to_string(steps));
+  s = std::make_unique<rs_sampler>();
+  s->p = p; s->process = process; s->T = steps; s->rows = (int)rows.size();
+  s->tab.resize(rows.size() * steps);
+  float* dst = s->tab.data();
+  for (int r : rows)
+    for (int i = 0; i < steps; ++i) *dst++ = (float)tables[(size_t)r * steps + i];
+  s->tsteps.resize(steps);
+  for (int i = 0; i < steps; ++i) s->tsteps[i] = (float)(tmap ? tmap[i] : i);
+  return 0;
 }
 
 int rs_sampler_create_ex(rs_plan* p, int steps, const double* sqrt_etas, double kappa, const int32_t* tmap,
                          const rs_sampler_options* opt, rs_sampler** out) {
   RS_CHECK(p && p->bound && sqrt_etas && opt && out, "bad argument (plan must be bound)");
-  RS_CHECK(p->pass == Pass::Denoiser, std::string("samplers are built on denoiser plans: this plan belongs to ") + kind_name(p->e->kind));
-  RS_CHECK(steps >= 2 && steps <= p->max_rows && steps <= 1024, "steps out of range for this plan");
   int rc = check_sampler_options(*opt); if (rc) return rc;
-  auto s = std::make_unique<rs_sampler>();
-  s->p = p;
+  std::unique_ptr<rs_sampler> s;
+  rc = sampler_new(p, kStepResShift, steps, tmap, "ResShift sampler", nullptr, {}, s); if (rc) return rc;
   schedule_tables(*s, steps, sqrt_etas, kappa, tmap, *opt);
   *out = s.release();
   return 0;
@@ -1954,7 +1892,6 @@ int rs_ddpm_sampler_create(rs_plan* p, int steps, const double* tables, const in
   RS_CHECK(p && p->bound && out, "bad argument (plan must be bound)");
   RS_CHECK(tables, "DDPM sampler: the schedule tables are NULL");
   RS_CHECK(o, "DDPM sampler: the options are NULL");
-  RS_CHECK(p->pass == Pass::Denoiser, std::string("samplers are built on denoiser plans: this plan belongs to ") + kind_name(p->e->kind));
   RS_CHECK(o->kind == RS_DDPM_ANCESTRAL || o->kind == RS_DDPM_DDIM,
            "DDPM sampler: unknown kind " + std::to_string(o->kind) + " (RS_DDPM_ANCESTRAL or RS_DDPM_DDIM)");
   RS_CHECK(o->mean_type == RS_MEAN_EPSILON || o->mean_type == RS_MEAN_XSTART,
@@ -1964,19 +1901,15 @@ int rs_ddpm_sampler_create(rs_plan* p, int steps, const double* tables, const in
            "DDPM sampler: unknown variance type " + std::to_string(o->var_type) + " (RS_VAR_FIXED_LARGE or RS_VAR_FIXED_SMALL)");
   RS_CHECK(o->clip == 0 || o->clip == 1, "DDPM sampler: clip must be 0 or 1, got " + std::to_string(o->clip));
   RS_CHECK(std::isfinite(o->eta) && o->eta >= 0.0, "DDPM sampler: eta must be finite and >= 0, got " + std::to_string(o->eta));
-  RS_CHECK(steps >= 2 && steps <= p->max_rows && steps <= 1024,
-           "DDPM sampler: steps must be in [2, " + std::to_string(std::min(p->max_rows, 1024)) +
-           "] (the plan's FiLM-table rows), got " + std::to_string(steps));
-  auto s = std::make_unique<rs_sampler>();
-  s->p = p; s->T = steps; s->ddpm = true; s->dopt = *o;
-  const int rows[kDdpmDevRows] = {RS_DDPM_SQRT_RECIP_ACP, RS_DDPM_SQRT_RECIPM1_ACP, RS_DDPM_COEF1, RS_DDPM_COEF2,
-                                  o->var_type == RS_VAR_FIXED_LARGE ? RS_DDPM_LOGVAR_LARGE : RS_DDPM_LOGVAR_SMALL,
-                                  RS_DDPM_ACP, RS_DDPM_ACP_PREV};
-  s->dtab.resize((size_t)kDdpmDevRows * steps);
-  for (int r = 0; r < kDdpmDevRows; ++r)
-    for (int i = 0; i < steps; ++i) s->dtab[(size_t)r * steps + i] = (float)tables[(size_t)rows[r] * steps + i];
-  s->tsteps.resize(steps);
-  for (int i = 0; i < steps; ++i) s->tsteps[i] = (float)(tmap ? tmap[i] : i);
+  std::unique_ptr<rs_sampler> s;
+  static_assert(kDdSqrtRecipAcp == 0 && kDdSqrtRecipm1Acp == 1 && kDdCoef1 == 2 && kDdCoef2 == 3 && kDdLogVar == 4 &&
+                kDdAcp == 5 && kDdAcpPrev == 6, "the rows below are in DdpmRow order");
+  int rc = sampler_new(p, o->kind == RS_DDPM_DDIM ? kStepDdim : kStepAncestral, steps, tmap, "DDPM sampler", tables,
+                       {RS_DDPM_SQRT_RECIP_ACP, RS_DDPM_SQRT_RECIPM1_ACP, RS_DDPM_COEF1, RS_DDPM_COEF2,
+                        o->var_type == RS_VAR_FIXED_LARGE ? RS_DDPM_LOGVAR_LARGE : RS_DDPM_LOGVAR_SMALL, RS_DDPM_ACP,
+                        RS_DDPM_ACP_PREV}, s);
+  if (rc) return rc;
+  s->mean_type = o->mean_type; s->clip = o->clip; s->eta = (float)o->eta;
   *out = s.release();
   return 0;
 }
@@ -1987,28 +1920,22 @@ int rs_ddim_reverse_sampler_create(rs_plan* p, int steps, const double* tables, 
   RS_CHECK(p && p->bound && out, "bad argument (plan must be bound)");
   RS_CHECK(tables, "DDIM reverse sampler: the schedule tables are NULL");
   RS_CHECK(o, "DDIM reverse sampler: the options are NULL");
-  RS_CHECK(p->pass == Pass::Denoiser, std::string("samplers are built on denoiser plans: this plan belongs to ") + kind_name(p->e->kind));
   RS_CHECK(o->mean_type == RS_MEAN_EPSILON || o->mean_type == RS_MEAN_XSTART,
            "DDIM reverse sampler: the model must predict eps or x0 (RS_MEAN_EPSILON or RS_MEAN_XSTART), got mean type " +
            std::to_string(o->mean_type));
   RS_CHECK(o->clip == 0 || o->clip == 1, "DDIM reverse sampler: clip must be 0 or 1, got " + std::to_string(o->clip));
-  RS_CHECK(steps >= 2 && steps <= p->max_rows && steps <= 1024,
-           "DDIM reverse sampler: steps must be in [2, " + std::to_string(std::min(p->max_rows, 1024)) +
-           "] (the plan's FiLM-table rows), got " + std::to_string(steps));
-  auto s = std::make_unique<rs_sampler>();
-  s->p = p; s->T = steps; s->ddpm = true; s->reverse = true; s->ropt = *o;
-  const int rows[kReverseDevRows] = {RS_DDPM_SQRT_RECIP_ACP, RS_DDPM_SQRT_RECIPM1_ACP, RS_DDPM_ACP_NEXT};
-  s->dtab.resize((size_t)kReverseDevRows * steps);
-  for (int r = 0; r < kReverseDevRows; ++r)
-    for (int i = 0; i < steps; ++i) s->dtab[(size_t)r * steps + i] = (float)tables[(size_t)rows[r] * steps + i];
-  s->tsteps.resize(steps);
-  for (int i = 0; i < steps; ++i) s->tsteps[i] = (float)(tmap ? tmap[i] : i);
+  std::unique_ptr<rs_sampler> s;
+  static_assert(kInvSqrtRecipAcp == 0 && kInvSqrtRecipm1Acp == 1 && kInvAcpNext == 2, "the rows below are in InversionRow order");
+  int rc = sampler_new(p, kStepInversion, steps, tmap, "DDIM reverse sampler", tables,
+                       {RS_DDPM_SQRT_RECIP_ACP, RS_DDPM_SQRT_RECIPM1_ACP, RS_DDPM_ACP_NEXT}, s);
+  if (rc) return rc;
+  s->mean_type = o->mean_type; s->clip = o->clip;
   *out = s.release();
   return 0;
 }
 int rs_sampler_tables(const rs_sampler* s, float* dst) {
   RS_CHECK(s && dst, "null argument");
-  RS_CHECK(!s->ddpm, "rs_sampler_tables: a DDPM sampler has no residual-shift tables");
+  RS_CHECK(s->process == kStepResShift, "rs_sampler_tables: a DDPM sampler has no residual-shift tables");
   copy_tables(*s, dst);
   return 0;
 }
@@ -2044,12 +1971,8 @@ int rs_schedule_tables_ex(int steps, const double* sqrt_etas, double kappa, cons
   int rc = check_sampler_options(*opt); if (rc) return rc;
   rs_sampler s;
   schedule_tables(s, steps, sqrt_etas, kappa, tmap, *opt);
-  copy_tables(s, dst);
-  dst += 5 * steps + 1;
-  for (const std::vector<float>* v : {&s.eps_coef, &s.eta, &s.one_minus_eta}) {
-    std::memcpy(dst, v->data(), (size_t)steps * sizeof(float));
-    dst += steps;
-  }
+  dst = copy_tables(s, dst);
+  std::memcpy(dst, s.tab.data() + (size_t)kRsEpsCoef * steps, (size_t)3 * steps * sizeof(float));   // eps_coef, eta, 1 - eta
   return 0;
 }
 void rs_sampler_destroy(rs_sampler* s) {
@@ -2067,8 +1990,8 @@ int rs_sampler_set_taps(rs_sampler* s, float* pred, float* sample) {
 
 int rs_sampler_run(rs_sampler* s, const float* z_y, const float* noises, const float* lq, const float* mask,
                    float* out_latent, int use_graph, void* stream) {
-  RS_CHECK(!(s && s->reverse) || z_y, "DDIM reverse sampler: x_start (z_y) is NULL");
-  RS_CHECK(s && (z_y || s->ddpm) && (noises || s->reverse) && lq && out_latent, "null argument");
+  RS_CHECK(!(s && s->process == kStepInversion) || z_y, "DDIM reverse sampler: x_start (z_y) is NULL");
+  RS_CHECK(s && (z_y || !reads_zy(*s)) && (noises || !noise_count(*s)) && lq && out_latent, "null argument");
   int rc = check_plan_device(*s->p); if (rc) return rc;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   rc = sampler_prepare(*s, st); if (rc) return rc;
@@ -2099,14 +2022,13 @@ size_t rs_sampler_staging_bytes(const rs_sampler* s) {
   const size_t lat = align_up((size_t)P.B * c.in_channels * P.H * P.W * 4, 256);
   const size_t lq = align_up((size_t)P.B * 3 * P.lqH * P.lqW * 4, 256);
   const size_t mk = align_up((size_t)P.B * 1 * P.lqH * P.lqW * 4, 256);
-  const size_t n_noise = s->reverse ? 0 : (size_t)s->T + 1;      // a DDIM inversion sampler draws nothing
-  return lat * (n_noise + 2) + lq + mk;
+  return lat * (noise_count(*s) + 2) + lq + mk;
 }
 
 int rs_sampler_run_host(rs_sampler* s, const float* z_y_h, const float* noises_h, const float* lq_h, const float* mask_h,
                         float* out_h, void* staging, size_t staging_bytes, int use_graph, void* stream) {
-  RS_CHECK(!(s && s->reverse) || z_y_h, "DDIM reverse sampler: x_start (z_y) is NULL");
-  RS_CHECK(s && (z_y_h || s->ddpm) && (noises_h || s->reverse) && lq_h && out_h && staging, "null argument");
+  RS_CHECK(!(s && s->process == kStepInversion) || z_y_h, "DDIM reverse sampler: x_start (z_y) is NULL");
+  RS_CHECK(s && (z_y_h || !reads_zy(*s)) && (noises_h || !noise_count(*s)) && lq_h && out_h && staging, "null argument");
   RS_CHECK(staging_bytes >= rs_sampler_staging_bytes(s), "staging buffer too small");
   { int rc = check_plan_device(*s->p); if (rc) return rc; }
   cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -2118,7 +2040,7 @@ int rs_sampler_run_host(rs_sampler* s, const float* z_y_h, const float* noises_h
   uint8_t* base = static_cast<uint8_t*>(staging);
   float* d_zy = reinterpret_cast<float*>(base);
   float* d_out = reinterpret_cast<float*>(base + lat);
-  const size_t n_noise = s->reverse ? 0 : (size_t)s->T + 1;      // as rs_sampler_staging_bytes
+  const size_t n_noise = noise_count(*s);
   float* d_noise = reinterpret_cast<float*>(base + 2 * lat);
   float* d_lq = reinterpret_cast<float*>(base + lat * (n_noise + 2));
   float* d_mask = reinterpret_cast<float*>(base + lat * (n_noise + 2) + align_up(n_lq * 4, 256));

@@ -101,6 +101,67 @@ def _tab(arr, t, like):
     return res.expand(like.shape)
 
 
+def _cached_sampler(plan, key, create):
+    """The plan's native sampler for `key` (a process and its options), made on first use by create(out_handle)."""
+    if key not in plan.samplers:
+        h = C.c_void_p()
+        _lib.check(create(C.byref(h)))
+        plan.samplers[key] = h
+    return plan.samplers[key]
+
+
+def _native_inputs(model, x, model_kwargs):
+    """lq and mask of model_kwargs as contiguous fp32, checked against the model for the latent x."""
+    lq = model_kwargs["lq"].float().contiguous()
+    mask = model_kwargs.get("mask", None)
+    mask = mask.float().contiguous() if mask is not None else None
+    ResShiftDiffusion._check_native_inputs(model, x, lq, mask)
+    return lq, mask
+
+
+def _run_tapped(s, T, x, lq, mask, z_y=None, noises=None):
+    """Sampler s run eagerly with the per-step taps on inputs shaped like the latent x: returns (final, preds,
+    samples), preds / samples [T, *x.shape] holding every step's pred_xstart / sample."""
+    final = torch.empty_like(x)
+    preds = torch.empty((T,) + tuple(x.shape), dtype=torch.float32, device=x.device)
+    samples = torch.empty_like(preds)
+    _lib.check(_lib.lib.rs_sampler_set_taps(s, preds.data_ptr(), samples.data_ptr()))
+    try:
+        _lib.check(_lib.lib.rs_sampler_run(s, _lib.ptr(z_y), _lib.ptr(noises), lq.data_ptr(), _lib.ptr(mask),
+                                           final.data_ptr(), 0, _lib.current_stream()))
+    finally:
+        _lib.check(_lib.lib.rs_sampler_set_taps(s, None, None))
+    return final, preds, samples
+
+
+def _run_graphed(model, s, shape, model_kwargs, z_y=None, noises=None, use_graph=True):
+    """Sampler s run on the plan's stable device buffers (plan._io), so that its captured CUDA graph replays call after
+    call: z_y and noises (whichever the process reads), lq and mask are copied in, and the final latent of `shape`
+    comes back as a new tensor.  Every sampler of the plan shares the buffers; each is made again when its shape
+    changes."""
+    B, _, H, W = shape
+    plan = model.plan(B, H, W)
+    dev = (z_y if z_y is not None else noises).device
+    io = getattr(plan, "_io", None)
+    if io is None:
+        io = plan._io = {}
+
+    def buf(name, shp):
+        if name not in io or tuple(io[name].shape) != tuple(shp):
+            io[name] = torch.empty(tuple(shp), dtype=torch.float32, device=dev)
+        return io[name]
+
+    def stage(name, src):
+        return None if src is None else buf(name, src.shape).copy_(src)
+
+    zy, nz, lq, mask = (stage(k, v) for k, v in (("zy", z_y), ("noise", noises), ("lq", model_kwargs["lq"]),
+                                                  ("mask", model_kwargs.get("mask", None))))
+    out = buf("out", shape)
+    _lib.check(_lib.lib.rs_sampler_run(s, _lib.ptr(zy), _lib.ptr(nz), lq.data_ptr(), _lib.ptr(mask), out.data_ptr(),
+                                       int(use_graph), _lib.current_stream()))
+    return out.clone()
+
+
 class ResShiftDiffusion:
     """``SpacedDiffusion(GaussianDiffusion)`` of the reference, inference side."""
 
@@ -287,14 +348,10 @@ class ResShiftDiffusion:
         opt = self.sampler_options()
         key = (self.num_timesteps, self.kappa, tuple(self.sqrt_etas.tolist()), tuple(self.timestep_map),
                (opt.mean_type, opt.normalize_input, opt.latent_flag))
-        if key not in plan.samplers:
-            h = C.c_void_p()
-            se = (C.c_double * self.num_timesteps)(*self.sqrt_etas.tolist())
-            tm = (C.c_int32 * self.num_timesteps)(*self.timestep_map)
-            _lib.check(_lib.lib.rs_sampler_create_ex(plan.handle, self.num_timesteps, se, float(self.kappa), tm,
-                                                     C.byref(opt), C.byref(h)))
-            plan.samplers[key] = h
-        return plan.samplers[key]
+        T = self.num_timesteps
+        return _cached_sampler(plan, key, lambda out: _lib.lib.rs_sampler_create_ex(
+            plan.handle, T, (C.c_double * T)(*self.sqrt_etas.tolist()), float(self.kappa),
+            (C.c_int32 * T)(*self.timestep_map), C.byref(opt), out))
 
     def draw_noises(self, z_y, noise=None, noise_repeat=False):
         """T+1 noise tensors in the reference's draw order and dtypes (prior: randn_like(z_y),
@@ -319,19 +376,8 @@ class ResShiftDiffusion:
             noises = self.draw_noises(z_y, noise, noise_repeat)
             s = self.native_sampler(model, B, H, W)
             zf = z_y.float().contiguous()
-            lq = model_kwargs["lq"].float().contiguous()
-            mask = model_kwargs.get("mask", None)
-            mask = mask.float().contiguous() if mask is not None else None
-            self._check_native_inputs(model, zf, lq, mask)
-            final = torch.empty_like(zf)
-            preds = torch.empty((T,) + tuple(zf.shape), dtype=torch.float32, device=zf.device)
-            samples = torch.empty_like(preds)
-            _lib.check(_lib.lib.rs_sampler_set_taps(s, preds.data_ptr(), samples.data_ptr()))
-            try:
-                _lib.check(_lib.lib.rs_sampler_run(s, zf.data_ptr(), noises.data_ptr(), lq.data_ptr(), _lib.ptr(mask),
-                                                   final.data_ptr(), 0, _lib.current_stream()))
-            finally:
-                _lib.check(_lib.lib.rs_sampler_set_taps(s, None, None))
+            lq, mask = _native_inputs(model, zf, model_kwargs)
+            _, preds, samples = _run_tapped(s, T, zf, lq, mask, z_y=zf, noises=noises)
             # preds holds the step kernel's converted x0 (pred_xstart); the mean follows from it
             c1 = self.posterior_mean_coef1.astype(np.float32)
             c2 = self.posterior_mean_coef2.astype(np.float32)
@@ -379,31 +425,10 @@ class ResShiftDiffusion:
         if noises is None:
             noises = self.draw_noises(z_y, noise, noise_repeat)
         s = self.native_sampler(model, B, H, W)
-        # stable device buffers so that the captured graph can be replayed call after call
-        plan = model.plan(B, H, W)
-        bufs = getattr(plan, "_io", None)
-        lq_in = model_kwargs["lq"]
-        mask_in = model_kwargs.get("mask", None)
-        self._check_native_inputs(model, z_y, lq_in, mask_in)
+        self._check_native_inputs(model, z_y, model_kwargs["lq"], model_kwargs.get("mask", None))
         if tuple(noises.shape) != (self.num_timesteps + 1,) + tuple(z_y.shape):
             raise ValueError(f"noises must have shape {(self.num_timesteps + 1,) + tuple(z_y.shape)}, got {tuple(noises.shape)}")
-        if (bufs is None or bufs["lq"].shape != lq_in.shape or (mask_in is None) != (bufs["mask"] is None)
-                or bufs["noise"].shape != noises.shape):
-            bufs = {"zy": torch.empty(B, Cc, H, W, dtype=torch.float32, device=z_y.device),
-                    "noise": torch.empty_like(noises),
-                    "lq": torch.empty(lq_in.shape, dtype=torch.float32, device=z_y.device),
-                    "mask": None if mask_in is None else torch.empty(mask_in.shape, dtype=torch.float32, device=z_y.device),
-                    "out": torch.empty(B, Cc, H, W, dtype=torch.float32, device=z_y.device)}
-            plan._io = bufs
-        bufs["zy"].copy_(z_y)
-        bufs["noise"].copy_(noises)
-        bufs["lq"].copy_(lq_in)
-        if mask_in is not None:
-            bufs["mask"].copy_(mask_in)
-        _lib.check(_lib.lib.rs_sampler_run(s, bufs["zy"].data_ptr(), bufs["noise"].data_ptr(), bufs["lq"].data_ptr(),
-                                           _lib.ptr(bufs["mask"]), bufs["out"].data_ptr(), int(use_graph),
-                                           _lib.current_stream()))
-        return bufs["out"].clone()
+        return _run_graphed(model, s, z_y.shape, model_kwargs, z_y=z_y, noises=noises, use_graph=use_graph)
 
     def training_losses(self, *a, **k):
         raise NotImplementedError("training is outside the covered hot path (inference only)")
@@ -621,32 +646,22 @@ class SpacedDiffusionDDPM:
         """The plan's DDPM sampler for this process and these options ("ancestral", "ddim", or "reverse" for DDIM
         inversion, which has no eta), created once."""
         plan = model.plan(batch, height, width)
+        T = self.num_timesteps
+        process = (T, tuple(self.betas.tolist()), tuple(self.timestep_map))
         if kind == "reverse":
             ropt = _lib.DdimReverseOptionsC(self._NATIVE_MEAN_TYPES[self.model_mean_type], int(bool(clip_denoised)))
-            key = ("ddim_reverse", self.num_timesteps, tuple(self.betas.tolist()), tuple(self.timestep_map),
-                   (ropt.mean_type, ropt.clip))
-            if key not in plan.samplers:
-                h = C.c_void_p()
-                tabs = self.ddim_reverse_tables()
-                tm = (C.c_int32 * self.num_timesteps)(*self.timestep_map)
-                _lib.check(_lib.lib.rs_ddim_reverse_sampler_create(plan.handle, self.num_timesteps,
-                                                                   tabs.ctypes.data_as(C.POINTER(C.c_double)), tm,
-                                                                   C.byref(ropt), C.byref(h)))
-                plan.samplers[key] = h
-            return plan.samplers[key]
+            tabs = self.ddim_reverse_tables()
+            return _cached_sampler(plan, ("ddim_reverse",) + process + ((ropt.mean_type, ropt.clip),),
+                                   lambda out: _lib.lib.rs_ddim_reverse_sampler_create(
+                                       plan.handle, T, tabs.ctypes.data_as(C.POINTER(C.c_double)),
+                                       (C.c_int32 * T)(*self.timestep_map), C.byref(ropt), out))
         opt = _lib.DdpmOptionsC(_lib.DDPM_KINDS[kind], self._NATIVE_MEAN_TYPES[self.model_mean_type],
                                 self._NATIVE_VAR_TYPES[self.model_var_type], int(bool(clip_denoised)), float(eta))
-        key = ("ddpm", self.num_timesteps, tuple(self.betas.tolist()), tuple(self.timestep_map),
-               (opt.kind, opt.mean_type, opt.var_type, opt.clip, opt.eta))
-        if key not in plan.samplers:
-            h = C.c_void_p()
-            tabs = self.ddpm_tables()
-            tm = (C.c_int32 * self.num_timesteps)(*self.timestep_map)
-            _lib.check(_lib.lib.rs_ddpm_sampler_create(plan.handle, self.num_timesteps,
-                                                       tabs.ctypes.data_as(C.POINTER(C.c_double)), tm, C.byref(opt),
-                                                       C.byref(h)))
-            plan.samplers[key] = h
-        return plan.samplers[key]
+        tabs = self.ddpm_tables()
+        return _cached_sampler(plan, ("ddpm",) + process + ((opt.kind, opt.mean_type, opt.var_type, opt.clip, opt.eta),),
+                               lambda out: _lib.lib.rs_ddpm_sampler_create(
+                                   plan.handle, T, tabs.ctypes.data_as(C.POINTER(C.c_double)),
+                                   (C.c_int32 * T)(*self.timestep_map), C.byref(opt), out))
 
     def sample_latent(self, model, noises, model_kwargs, kind="ancestral", clip_denoised=True, eta=0.0, use_graph=True):
         """The fused loop: noises [T + 1, B, C, H, W] (draw_noises) -> the final latent, all T steps inside librs_b200
@@ -658,47 +673,16 @@ class SpacedDiffusionDDPM:
         lq_in, mask_in = model_kwargs["lq"], model_kwargs.get("mask", None)
         ResShiftDiffusion._check_native_inputs(model, noises[0], lq_in, mask_in)
         s = self.native_sampler(model, B, H, W, kind, clip_denoised, eta)
-        # stable device buffers (shared with the plan's ResShift samplers) so that each captured graph can be replayed
-        plan = model.plan(B, H, W)
-        bufs = getattr(plan, "_io", None)
-        dev = noises.device
-        if (bufs is None or bufs["lq"].shape != lq_in.shape or (mask_in is None) != (bufs["mask"] is None)
-                or bufs["noise"].shape != noises.shape):
-            bufs = {"zy": torch.empty(B, Cc, H, W, dtype=torch.float32, device=dev),
-                    "noise": torch.empty(noises.shape, dtype=torch.float32, device=dev),
-                    "lq": torch.empty(lq_in.shape, dtype=torch.float32, device=dev),
-                    "mask": None if mask_in is None else torch.empty(mask_in.shape, dtype=torch.float32, device=dev),
-                    "out": torch.empty(B, Cc, H, W, dtype=torch.float32, device=dev)}
-            plan._io = bufs
-        bufs["noise"].copy_(noises)
-        bufs["lq"].copy_(lq_in)
-        if mask_in is not None:
-            bufs["mask"].copy_(mask_in)
-        _lib.check(_lib.lib.rs_sampler_run(s, None, bufs["noise"].data_ptr(), bufs["lq"].data_ptr(),
-                                           _lib.ptr(bufs["mask"]), bufs["out"].data_ptr(), int(use_graph),
-                                           _lib.current_stream()))
-        return bufs["out"].clone()
+        return _run_graphed(model, s, noises.shape[1:], model_kwargs, noises=noises, use_graph=use_graph)
 
     def _native_progressive(self, model, noises, model_kwargs, kind, clip_denoised, eta):
         """The fused loop run eagerly with the per-step taps: yields sample / pred_xstart of every step."""
         T = self.num_timesteps
         x = noises[0].float().contiguous()
         B, Cc, H, W = x.shape
-        lq = model_kwargs["lq"].float().contiguous()
-        mask = model_kwargs.get("mask", None)
-        mask = mask.float().contiguous() if mask is not None else None
-        ResShiftDiffusion._check_native_inputs(model, x, lq, mask)
+        lq, mask = _native_inputs(model, x, model_kwargs)
         s = self.native_sampler(model, B, H, W, kind, clip_denoised, eta)
-        nz = noises.float().contiguous()
-        final = torch.empty_like(x)
-        preds = torch.empty((T,) + tuple(x.shape), dtype=torch.float32, device=x.device)
-        samples = torch.empty_like(preds)
-        _lib.check(_lib.lib.rs_sampler_set_taps(s, preds.data_ptr(), samples.data_ptr()))
-        try:
-            _lib.check(_lib.lib.rs_sampler_run(s, None, nz.data_ptr(), lq.data_ptr(), _lib.ptr(mask), final.data_ptr(),
-                                               0, _lib.current_stream()))
-        finally:
-            _lib.check(_lib.lib.rs_sampler_set_taps(s, None, None))
+        _, preds, samples = _run_tapped(s, T, x, lq, mask, noises=noises.float().contiguous())
         for k in range(T):
             yield {"sample": samples[k], "pred_xstart": preds[k]}
 
@@ -710,45 +694,16 @@ class SpacedDiffusionDDPM:
         lq_in, mask_in = model_kwargs["lq"], model_kwargs.get("mask", None)
         ResShiftDiffusion._check_native_inputs(model, x_start, lq_in, mask_in)
         s = self.native_sampler(model, B, H, W, "reverse", clip_denoised)
-        # stable device buffers (shared with the plan's other samplers) so that the captured graph can be replayed
-        plan = model.plan(B, H, W)
-        bufs = getattr(plan, "_io", None)
-        dev = x_start.device
-        if bufs is None or bufs["lq"].shape != lq_in.shape or (mask_in is None) != (bufs["mask"] is None):
-            bufs = {"zy": torch.empty(B, Cc, H, W, dtype=torch.float32, device=dev),
-                    "noise": torch.empty(0, dtype=torch.float32, device=dev),
-                    "lq": torch.empty(lq_in.shape, dtype=torch.float32, device=dev),
-                    "mask": None if mask_in is None else torch.empty(mask_in.shape, dtype=torch.float32, device=dev),
-                    "out": torch.empty(B, Cc, H, W, dtype=torch.float32, device=dev)}
-            plan._io = bufs
-        bufs["zy"].copy_(x_start)
-        bufs["lq"].copy_(lq_in)
-        if mask_in is not None:
-            bufs["mask"].copy_(mask_in)
-        _lib.check(_lib.lib.rs_sampler_run(s, bufs["zy"].data_ptr(), None, bufs["lq"].data_ptr(),
-                                           _lib.ptr(bufs["mask"]), bufs["out"].data_ptr(), int(use_graph),
-                                           _lib.current_stream()))
-        return bufs["out"].clone()
+        return _run_graphed(model, s, x_start.shape, model_kwargs, z_y=x_start, use_graph=use_graph)
 
     def _native_reverse_progressive(self, model, x_start, model_kwargs, clip_denoised):
         """The fused DDIM inversion run eagerly with the per-step taps: yields sample / pred_xstart of every step."""
         T = self.num_timesteps
         x = x_start.float().contiguous()
         B, Cc, H, W = x.shape
-        lq = model_kwargs["lq"].float().contiguous()
-        mask = model_kwargs.get("mask", None)
-        mask = mask.float().contiguous() if mask is not None else None
-        ResShiftDiffusion._check_native_inputs(model, x, lq, mask)
+        lq, mask = _native_inputs(model, x, model_kwargs)
         s = self.native_sampler(model, B, H, W, "reverse", clip_denoised)
-        final = torch.empty_like(x)
-        preds = torch.empty((T,) + tuple(x.shape), dtype=torch.float32, device=x.device)
-        samples = torch.empty_like(preds)
-        _lib.check(_lib.lib.rs_sampler_set_taps(s, preds.data_ptr(), samples.data_ptr()))
-        try:
-            _lib.check(_lib.lib.rs_sampler_run(s, x.data_ptr(), None, lq.data_ptr(), _lib.ptr(mask), final.data_ptr(),
-                                               0, _lib.current_stream()))
-        finally:
-            _lib.check(_lib.lib.rs_sampler_set_taps(s, None, None))
+        _, preds, samples = _run_tapped(s, T, x, lq, mask, z_y=x)
         for k in range(T):
             yield {"sample": samples[k], "pred_xstart": preds[k]}
 
