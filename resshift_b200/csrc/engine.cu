@@ -1563,18 +1563,23 @@ static void collect_profile(const rs_plan& P, const Prof& prof, double* ms, char
     const Op& op = P.ops[i];
     char* d = desc + (size_t)i * desc_stride;
     switch (kind_of(op)) {
-      case OP_CONV: {
-        const ConvDesc& cd = payload<ConvOp>(op).d;
+      case OP_CONV: {   // everything rs_op_conv2d_ex needs to replay it with the plan's epilogue, and the launch it reports
+        const ConvOp& co = payload<ConvOp>(op);
+        const ConvDesc& cd = co.d;
         const ConvParams& c = cd.prm;
+        // the statistics sinks the kernel (or, under split-K, the reduce kernel) writes; gstat bit i: the GroupNorm that
+        // reads sink i reduces its pairs with gn_finalize_kernel (many tile slots); bsN: the per-image bias row stride
+        const GnSink* sk = c.splitk > 1 ? cd.red.sink : c.sink;
+        const int sinks = (sk[0].part != nullptr) + (sk[1].part != nullptr);
+        int gstat = 0;
+        for (int k = 0; k < sinks && k < (int)co.stat_dst.size(); ++k) gstat |= gn_finalizes(co.stat_dst[k].to) ? 1 << k : 0;
+        const long long bsN = co.bias_film_off >= 0 ? film_sN : 0;
         snprintf(d, desc_stride, "conv%dx%d s%d %dx%d Cin=%d Cout=%d grid=%d BN=%d st=%d %s cg=%d ms=%d sk=%d box=%dx%dx%d "
-                 "N=%d persist=%d pad=%d act=%d res=%d f32=%d",
+                 "N=%d persist=%d pad=%d act=%d res=%d f32=%d silu=%d film=%d bsN=%lld sinks=%d cs=%d,%d co=%d,%d gstat=%d",
                  cd.ksize, cd.ksize, cd.stride, c.Hout, c.Wout, cd.in.C, c.Cout, cd.grid, c.BN, c.stages,
-                 payload<ConvOp>(op).w_name.c_str(), c.cg, c.msub, c.splitk, c.bw, c.bh, c.bn, c.Nimg, c.persist, cd.pad_lo,
-                 cd.act, (int)cd.has_res, (int)(cd.out_f32 != nullptr));
-        if (cd.has_silu || cd.film) {       // (UNetModelConv only: the other plans' rows keep their form)
-          const size_t len = std::strlen(d);
-          snprintf(d + len, desc_stride - len, " silu=%d film=%d", (int)cd.has_silu, (int)cd.film);
-        }
+                 co.w_name.c_str(), c.cg, c.msub, c.splitk, c.bw, c.bh, c.bn, c.Nimg, c.persist, cd.pad_lo,
+                 cd.act, (int)cd.has_res, (int)(cd.out_f32 != nullptr), (int)cd.has_silu, (int)cd.film, bsN, sinks,
+                 sk[0].cstride, sk[1].cstride, sk[0].coff, sk[1].coff, gstat);
         break;
       }
       case OP_GN: {   // everything rs_op_groupnorm_ex needs to replay it, and the launch geometry it should report

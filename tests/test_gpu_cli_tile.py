@@ -21,8 +21,9 @@ each 132-CTA wave boundary: 8128 rows.  The float64 reference of all 262144 rows
 a. Plan replays (vq_f4_encode_2048, vq_f4_decode_2048, realsr_denoiser_b1_512x512, random weights): every distinct conv,
    GroupNorm, window attention, fused Swin attention and fused MLP through its _ex entry point, unforced: the entry
    reports the plan's configuration, two launches are bit-identical, every checked element is within its module's
-   float64 bound.  Every op row of each plan is claimed by a replay here or by a check below (vq_attn: b; upsample:
-   the end-to-end decode in d), so an op kind a plan gains later fails test_plan_replay until something checks it.
+   float64 bound; the decoder's nearest upsamples through rs_op_upsample2x_ex with the SiLU output
+   (test_gpu_unetconv.resample_case).  Every op row of each plan is claimed by a replay here or by b (vq_attn), so an
+   op kind a plan gains later fails test_plan_replay until something checks it.
 
 b. vq_attn_sm90_kernel<512> at N = 1, T = 262144 against float64 in the classes of test_gpu_attention.py (randn, peaked,
    equal, large) and "needle": q and k rows are +-2 sign codes (a matching scaled logit is 90.5, others have standard
@@ -277,9 +278,20 @@ def _replay_mlps(plan, rows, N=1):
     return len(mlps)
 
 
-# op kinds checked elsewhere in this module: the T = 262144 attention by b, the decoder's nearest upsample by the
-# end-to-end decode of d (it has no single-operator entry)
-CHECKED_BY = {"vq_attn": "test_vq_attention_* (b)", "upsample": "test_decode_512_latent (d)"}
+_UPSAMPLE = re.compile(r"upsample (\d+)x(\d+) C=(\d+)$")
+
+
+def _replay_upsamples(plan, rows, N=1):
+    from tests.test_gpu_unetconv import resample_case
+    ups = _distinct(rows, _UPSAMPLE)
+    for H, W, Cc in ups:
+        resample_case(N, int(H), int(W), int(Cc), False)
+        _free()
+    return len(ups)
+
+
+# op kinds checked elsewhere in this module: the T = 262144 attention by b
+CHECKED_BY = {"vq_attn": "test_vq_attention_* (b)"}
 
 
 @pytest.mark.parametrize("plan", list(PLANS))
@@ -287,7 +299,7 @@ def test_plan_replay(plan):
     rows = plan_rows(plan)
     assert rows
     kinds = {"conv": _replay_convs, "gn": _replay_gns, "attn": _replay_windows, "swin_attn": _replay_swins,
-             "mlp": _replay_mlps}
+             "mlp": _replay_mlps, "upsample": _replay_upsamples}
     done = {}
     for kind, fn in kinds.items():
         done[kind] = fn(plan, rows)
@@ -295,7 +307,7 @@ def test_plan_replay(plan):
         assert tuple(map(int, r)) == (T_CLI, C_CLI, 1), r          # the shape b holds to float64
     REPLAYED[plan] = done
     print(f"[plan] {plan}: " + ", ".join(f"{n} distinct {k}" for k, n in done.items()))
-    claimed = [k + " " for k in done if k not in ("conv",)] + ["conv", "vq_attn ", "upsample "]
+    claimed = [k + " " for k in done if k not in ("conv",)] + ["conv", "vq_attn "]
     unclaimed = [r for r in rows if not any(r.startswith(c) for c in claimed)]
     assert not unclaimed, f"{plan}: op rows no check claims: {sorted(set(unclaimed))}"
     assert not any(_UNET.match(r) for r in rows)

@@ -179,13 +179,12 @@ class Conv:
         return G.assert_within(tag, got, ref, mag, KAPPA, fp16=not f32)
 
 
-def _sinks(N, Cout, slots):
-    """Two statistics sinks at different channel offsets of wider buffers, NaN-filled."""
-    out = []
-    for extra, coff in ((16, 8), (72, 40)):
-        cstride = Cout + extra
-        out.append((torch.full((N * slots * cstride * 2 + 64,), float("nan"), device="cuda"), cstride, coff))
-    return out
+def _sinks(N, Cout, slots, spec=None):
+    """Statistics sinks (cstride, coff) of NaN-filled buffers: by default two at different channel offsets of wider
+    buffers."""
+    spec = ((Cout + 16, 8), (Cout + 72, 40)) if spec is None else spec
+    return [(torch.full((N * slots * cstride * 2 + 64,), float("nan"), device="cuda"), cstride, coff)
+            for cstride, coff in spec]
 
 
 def _box(Ho, Wo):
@@ -200,15 +199,17 @@ def _box(Ho, Wo):
     return bw, bh, 128 // (bw * bh), (Wo // bw) * (Ho // bh)
 
 
-def _run(tag, L, want=None, stats=True, rows=None, **kw):
+def _run(tag, L, want=None, stats=True, rows=None, sink_spec=None, **kw):
     """Two launches of layer L: bit-identical outputs and statistics, info as wanted, output within the bound (on the
-    output rows `rows` only, if given), the statistics of each sink against the stored output.  Returns (output, sink
-    buffers, info)."""
+    output rows `rows` only, if given), the statistics of each sink against the stored output (in full).  Sinks: the
+    (cstride, coff) of sink_spec, or two default ones where the launcher takes statistics (boxes of at most two images,
+    fp16 output).  Returns (output, sink buffers, info)."""
     bw, bh, box_n, slots = _box(L.Ho, L.Wo)
-    stats = stats and box_n <= 2 and not kw.get("out_f32")
+    if sink_spec is None:
+        sink_spec = None if stats and box_n <= 2 and not kw.get("out_f32") else ()
     runs = []
     for _ in range(2):
-        sinks = _sinks(L.N, L.Cout, slots) if stats else ()
+        sinks = _sinks(L.N, L.Cout, slots, sink_spec)
         out, info = L.run(sinks=sinks, **kw)
         runs.append((out.clone(), [(s[0].clone(), s[1], s[2]) for s in sinks], info))
     (out, sinks, info), (out2, sinks2, info2) = runs
@@ -358,19 +359,24 @@ def test_channel_slices(mode):
 # ---------------------------------------------------------------------------------------------- d. the shipped plans
 
 _DESC = re.compile(r"conv(\d)x\d s(\d) (\d+)x(\d+) Cin=(\d+) Cout=(\d+) grid=(\d+) BN=(\d+) st=(\d+) \S* cg=(\d+) ms=(\d+) "
-                   r"sk=(\d+) box=(\d+)x(\d+)x(\d+) N=(\d+) persist=(\d+) pad=(\d+) act=(\d+) res=(\d+) f32=(\d+)")
+                   r"sk=(\d+) box=(\d+)x(\d+)x(\d+) N=(\d+) persist=(\d+) pad=(\d+) act=(\d+) res=(\d+) f32=(\d+)"
+                   r"(?: silu=(\d) film=(\d) bsN=(\d+) sinks=(\d) cs=(\d+),(\d+) co=(\d+),(\d+) gstat=(\d)$)?")
+_EPI_KEYS = ("silu", "film", "bsN", "sinks", "cs0", "cs1", "co0", "co1", "gstat")
 
 
-def _conv_rows(rows):
-    """Distinct conv launches of an op list, as dicts of the description's fields."""
+def _conv_rows(rows, epilogue=False):
+    """Distinct conv launches of an op list, as dicts of the description's fields; with epilogue, also of the fields
+    that describe the epilogue (SiLU output, FiLM, per-image bias row stride, statistics sinks, gstat bits)."""
     keys = ("k", "s", "Ho", "Wo", "Cin", "Cout", "grid", "BN", "stages", "cg", "msub", "splitk", "bw", "bh", "box_n", "N",
-            "persist", "pad", "act", "res", "f32")
+            "persist", "pad", "act", "res", "f32") + _EPI_KEYS
     seen = {}
     for r in rows:
         if r.startswith("conv"):
             m = _DESC.match(r)
-            assert m, r
-            d = dict(zip(keys, (int(v) for v in m.groups())))
+            assert m and (m.group(len(keys)) is not None or not epilogue), r
+            d = dict(zip(keys, (None if v is None else int(v) for v in m.groups())))
+            if not epilogue:
+                d = {k: d[k] for k in keys if k not in _EPI_KEYS}
             seen.setdefault(tuple(d.values()), d)
     return list(seen.values())
 

@@ -157,7 +157,11 @@ SOFTMAX_ROWS = {"1": (lambda c: 1, 0), "300": (lambda c: 300, 24), "T": (lambda 
 @pytest.mark.parametrize("cols", SOFTMAX_COLS)
 def test_softmax_rows(cols, rows_key):
     nrows, pad = SOFTMAX_ROWS[rows_key]
-    rows, ld = nrows(cols), cols + pad
+    softmax_case(nrows(cols), cols, cols + pad)
+
+
+def softmax_case(rows, cols, ld):
+    """rs_op_softmax_rows on rows x cols scores of every class in an fp16 [rows][ld] buffer, against float64."""
     scale = _f32((64, 128, 512)[cols % 3] ** -0.5)
     s, classes = score_rows(rows, cols, scale, seed=cols * 7 + rows)
     sentinel = 1234.0

@@ -153,7 +153,11 @@ def test_silu_output_refusals():
 @pytest.mark.parametrize("pool", [False, True])
 @pytest.mark.parametrize("shape", [(2, 8, 12, 64), (3, 16, 16, 8), (1, 40, 24, 96)])
 def test_resample_with_silu_output(shape, pool):
-    N, H, W, Cc = shape
+    resample_case(*shape, pool)
+
+
+def resample_case(N, H, W, Cc, pool):
+    """rs_op_avgpool2x2 / rs_op_upsample2x_ex with the SiLU output against float64; without it, the same first output."""
     g = torch.Generator(device="cuda").manual_seed(H * W + Cc)
     x = (torch.randn(N, H, W, Cc, device="cuda", generator=g) * 3).half()
     Ho, Wo = (H // 2, W // 2) if pool else (2 * H, 2 * W)
