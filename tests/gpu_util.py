@@ -1,6 +1,9 @@
 """Helpers shared by the GPU parity tests (thin wrappers over the C ABI single-operator entry points)."""
-import ctypes as C
+import gc
+import time
+from contextlib import contextmanager
 
+import pytest
 import torch
 import torch.nn.functional as F
 
@@ -8,9 +11,61 @@ from resshift_b200 import _lib
 
 L = _lib.lib
 
+# a denoiser forward against the fp32 oracle (test_gpu_unet.py's module docstring)
+FWD_MAX, FWD_MEAN = 1e-2, 2.5e-3
+
 
 def stream():
     return _lib.current_stream()
+
+
+def gen(seed):
+    return torch.Generator(device="cuda").manual_seed(seed)
+
+
+def free():
+    gc.collect()
+    torch.cuda.empty_cache()
+
+
+def note(obs, key, ratio):
+    """obs[key] = the worst ratio seen so far."""
+    obs[key] = max(obs.get(key, 0.0), float(ratio))
+
+
+@pytest.fixture(scope="module", autouse=True)
+def module_clock():
+    """In a module that imports it: the time its first test started, the peak memory statistics reset then."""
+    torch.cuda.reset_peak_memory_stats()
+    return time.time()
+
+
+def nan16(*shape):
+    return torch.full(shape, float("nan"), dtype=torch.float16, device="cuda")
+
+
+@contextmanager
+def fp32_matmuls():
+    """Exact fp32 matmuls / convolutions (TF32 off) for reference computations; restored afterwards."""
+    old = (torch.backends.cuda.matmul.allow_tf32, torch.backends.cudnn.allow_tf32)
+    torch.backends.cuda.matmul.allow_tf32 = False
+    torch.backends.cudnn.allow_tf32 = False
+    try:
+        yield
+    finally:
+        torch.backends.cuda.matmul.allow_tf32, torch.backends.cudnn.allow_tf32 = old
+
+
+def box128(H, W):
+    """The conv launcher's 128-pixel box over an H x W output map: (bw, bh, images per box, tile slots per image)."""
+    def p2(x, cap):
+        p = 1
+        while p * 2 <= cap and x % (p * 2) == 0:
+            p *= 2
+        return p
+    bw = p2(W, 128)
+    bh = p2(H, 128 // bw)
+    return bw, bh, 128 // (bw * bh), (W // bw) * (H // bh)
 
 
 def nhwc16(x_nchw: torch.Tensor) -> torch.Tensor:
@@ -108,11 +163,12 @@ def assert_within(tag, got, ref, mag, kappa, slack=None, fp16=True):
     return ratio
 
 
-def check_slot_pairs(tag, part, out16, bw, bh, slots, cstride, coff):
-    """(mean, M2) pairs part[N][slots][cstride][2] of the stored fp16 output out16 [N, H, W, C] (slot = (bw x bh) box of
-    one image, row-major over the map) at channel offset coff, against float64 statistics of the same values; the bounds
-    of test_gpu_ops.py's combined statistics.  Channels outside [coff, coff + C) must still hold their NaN fill."""
+def check_slot_pairs(tag, part, out16, cstride, coff):
+    """(mean, M2) pairs part[N][slots][cstride][2] of the stored fp16 output out16 [N, H, W, C] (slot = (bw x bh) box128
+    of one image, row-major over the map) at channel offset coff, against float64 statistics of the same values; the
+    bounds of test_gpu_ops.py's combined statistics.  Channels outside [coff, coff + C) must still hold their NaN fill."""
     N, H, W, Co = out16.shape
+    bw, bh, _, slots = box128(H, W)
     o = out16.double()
     t = o.reshape(N, H // bh, bh, W // bw, bw, Co).permute(0, 1, 3, 2, 4, 5).reshape(N, slots, bh * bw, Co)
     mean = t.mean(dim=2)

@@ -1,9 +1,9 @@
 """The default CLI tile: one 512x512 LQ tile at x4 (inference_resshift.py --chop_size 512), i.e. a bicubic x4 to
 2048x2048, an f4 VQ-GAN encode at 2048x2048 (bottleneck attention over T = 262144 positions at C = 512), the realsr
 denoiser on a 512x512 latent at batch 1, an f4 decode back to 2048x2048 and the overlap-average of such tiles, held to
-float64 references and to the fp32 oracle at that size.  The smaller sizes are held by the modules whose helpers this
-one imports (test_gpu_conv_instances.py, test_gpu_groupnorm.py, test_gpu_attention.py, test_gpu_mlp_instances.py,
-test_gpu_vq_attention.py); their bounds apply unchanged.
+float64 references and to the fp32 oracle at that size.  The smaller sizes are held by test_gpu_conv_instances.py,
+test_gpu_groupnorm.py, test_gpu_attention.py, test_gpu_mlp_instances.py and test_gpu_vq_attention.py, whose references
+this one runs from the support modules (conv_ref, gn_ref, attn_ref, mlp_ref, plan_ops); their bounds apply unchanged.
 
 Row bands.  Where a float64 reference of a whole 2048x2048 map costs too much (convs, GroupNorm applies, the fused MLP),
 it is computed on the output rows BAND_ROWS(H) of every image of an H-row map, H > 256:
@@ -22,7 +22,7 @@ a. Plan replays (vq_f4_encode_2048, vq_f4_decode_2048, realsr_denoiser_b1_512x51
    GroupNorm, window attention, fused Swin attention and fused MLP through its _ex entry point, unforced: the entry
    reports the plan's configuration, two launches are bit-identical, every checked element is within its module's
    float64 bound; the decoder's nearest upsamples through rs_op_upsample2x_ex with the SiLU output
-   (test_gpu_unetconv.resample_case).  Every op row of each plan is claimed by a replay here or by b (vq_attn), so an
+   (conv_ref.resample_case).  Every op row of each plan is claimed by a replay here or by b (vq_attn), so an
    op kind a plan gains later fails test_plan_replay until something checks it.
 
 b. vq_attn_sm90_kernel<512> at N = 1, T = 262144 against float64 in the classes of test_gpu_attention.py (randn, peaked,
@@ -41,7 +41,8 @@ c. GroupNorm at 32768 slots per image: each plan GroupNorm on the finalisation r
    in the first placement); a second placement moves every group's box.  A skipped or double-counted slot moves that
    group's mean by about 50 * 128 / (H W) = 1.5e-3, some 600 times the bound.  The statistics bound adds the
    count-dependent term of the kernel's per-thread fp32 sum of K / 256 items to test_gpu_groupnorm.py's constants
-   (check_finalize_gstat): at K = 262144 the decoder's rstd error (843 U in one H100 run) exceeds K_R = 512 U alone.
+   (gn_ref.check_finalize_gstat): at K = 262144 the decoder's rstd error (843 U in one H100 run) exceeds K_R = 512 U
+   alone.
 
 d. End to end against the fp32 oracle on the GPU, TF32 off (max|d| <= 1e-2, mean <= 2e-3; the denoiser forward
    test_gpu_unet.py's 1e-2 / 2.5e-3): f4 encode of the bicubic x4 of a 512x512 LQ, f4 decode of a 512x512 latent
@@ -53,8 +54,6 @@ d. End to end against the fp32 oracle on the GPU, TF32 off (max|d| <= 1e-2, mean
 test_report prints the worst ratio of error to bound per check, the ops replayed per plan, the wall time and the peak
 torch.cuda.max_memory_allocated.
 """
-import gc
-import re
 import time
 
 import pytest
@@ -64,52 +63,22 @@ pytestmark = pytest.mark.gpu
 
 if torch.cuda.is_available():
     from tests import gpu_util as G
+    from tests import plan_ops
+    from tests.gpu_util import module_clock  # noqa: F401  (the module's wall-time fixture)
     from resshift_b200 import _lib
-    from tests.test_gpu_attention import (_ATTN, _SWIN, _UNET, _VQ, SwinCase, WindowCase, allowance, kappas, run_window,
-                                          vq_check)
-    from tests.test_gpu_conv_instances import Conv, _conv_rows, _desc_rows, _first_stage_rows, _run, conv_env
-    from tests.test_gpu_groupnorm import Case, _gn_rows
-    from tests.test_gpu_mlp_instances import KAPPA as MLP_KAPPA
-    from tests.test_gpu_mlp_instances import _mlp
-    from tests.test_gpu_mlp_instances import _reference as mlp_reference
+    from tests.attn_ref import kappas, online_qkv, vq_check
+    from tests.conv_ref import KAPPA, conv_env, run_conv
+    from tests.first_stage_ref import no_reuse, tokens, w16
+    from tests.gn_ref import Case, check_finalize_gstat
 
 TOL_MAX, TOL_MEAN = 1e-2, 2e-3
 T_CLI, C_CLI = 262144, 512
 OBS = {}              # check -> worst ratio of error to bound
 REPLAYED = {}         # plan -> {op kind: distinct ops replayed}
-_T0 = []
 
 
 def _note(check, ratio):
-    OBS[check] = max(OBS.get(check, 0.0), float(ratio))
-
-
-def _gen(seed):
-    return torch.Generator(device="cuda").manual_seed(seed)
-
-
-def _free():
-    gc.collect()
-    torch.cuda.empty_cache()
-
-
-@pytest.fixture(scope="module", autouse=True)
-def _clock():
-    torch.cuda.reset_peak_memory_stats()
-    _T0.append(time.time())
-    yield
-
-
-def band_rows(H):
-    """BAND_ROWS(H) of the module docstring (None: every row)."""
-    if H <= 256:
-        return None
-    r = {0, 1, H - 2, H - 1}
-    for j in range(1, 8):
-        r |= {j * H // 8 - 1, j * H // 8}
-    s = H // 32
-    r |= {j * s + (5 * j) % s for j in range(32)}
-    return torch.tensor(sorted(r), device="cuda")
+    G.note(OBS, check, ratio)
 
 
 def attn_rows(T=T_CLI):
@@ -123,171 +92,35 @@ def attn_rows(T=T_CLI):
 
 # ---------------------------------------------------------------------------------------------- plans and their op rows
 
-def _denoiser_rows(name="realsr", B=1, H=512, W=512):
-    from resshift_b200.config import preset
-    from resshift_b200.models.unet import UNetModelSwin
-    from resshift_b200.weights import random_state_dict
-    ucfg, _ = preset(name)
-    m = UNetModelSwin(**ucfg.to_kwargs())
-    m.load_state_dict(random_state_dict(ucfg, 0))
-    m = m.cuda().eval()
-    g = _gen(1)
-    x = torch.randn(B, 3, H, W, device="cuda", generator=g)
-    lq = torch.rand(B, 3, H, W, device="cuda", generator=g) * 2 - 1
-    t = torch.full((B,), 7.0, device="cuda")
-    m(x, t, lq=lq)
-    plan = m.plan(B, H, W)
-    return _desc_rows(_lib.lib.rs_plan_profile_ops, plan.handle, x.data_ptr(), t.data_ptr(), lq.data_ptr(), None)
-
-
 PLANS = {
-    "vq_f4_encode_2048": lambda: _first_stage_rows("vq", "f4", 0, 1, 2048, 2048),
-    "vq_f4_decode_2048": lambda: _first_stage_rows("vq", "f4", 1, 1, 2048, 2048),
-    "realsr_denoiser_b1_512x512": _denoiser_rows,
+    "vq_f4_encode_2048": lambda: plan_ops.first_stage_rows("vq", "f4", 0, 1, 2048, 2048),
+    "vq_f4_decode_2048": lambda: plan_ops.first_stage_rows("vq", "f4", 1, 1, 2048, 2048),
+    "realsr_denoiser_b1_512x512": lambda: plan_ops.swin_rows("realsr", 1, 512, 512),
 }
 _ROWS = {}
 
 
 def plan_rows(plan):
     if plan not in _ROWS:
-        with conv_env():
-            _ROWS[plan] = PLANS[plan]()
-        _free()
+        _ROWS[plan] = plan_ops.unforced(PLANS[plan])
     return _ROWS[plan]
-
-
-_MLP = re.compile(r"mlp (\d+)x(\d+) E=(\d+) Hd=(\d+) grid=(\d+)")
-
-
-def _distinct(rows, rx):
-    return sorted({tuple(rx.match(r).groups()) for r in rows if rx.match(r)})
 
 
 # ---------------------------------------------------------------------------------------------- a. plan replays
 
 def _replay_convs(plan, rows):
-    convs = _conv_rows(rows)
+    """Each distinct conv without statistics sinks, on the row bands."""
+    convs = plan_ops.conv_rows(rows)
     for i, d in enumerate(convs):
-        L = Conv(d["N"], d["Ho"] * d["s"], d["Wo"] * d["s"], d["Cin"], d["Cout"], d["k"], stride=d["s"], pad_lo=d["pad"],
-                 act=d["act"], res=bool(d["res"]), seed=i)
-        want = {k: d[k] for k in ("grid", "BN", "stages", "cg", "msub", "splitk", "persist", "bw", "bh", "box_n")}
+        L = plan_ops.conv_of(d, seed=i)
+        want = {k: d[k] for k in plan_ops.CONV_WANT}
         with conv_env():
-            out, _, _ = _run(f"{plan} {d}", L, stats=False, want=want, out_f32=bool(d["f32"]), splitk=d["splitk"] > 1,
-                             rows=band_rows(d["Ho"]))
-        _note("conv", G.accumulation_ratio(*_conv_sel(L, out, d)) / 2.0 ** -18)
+            out, _, _, ratio = run_conv(f"{plan} {d}", L, stats=False, want=want, out_f32=bool(d["f32"]),
+                                        splitk=d["splitk"] > 1, rows=plan_ops.band_rows(d["Ho"]))
+        _note("conv", ratio / KAPPA)
         del L, out
-        _free()
-    return len(convs)
-
-
-def _conv_sel(L, out, d):
-    rows = band_rows(d["Ho"])
-    ref, mag = L.ref(rows)
-    got = out.permute(0, 2, 3, 1) if d["f32"] else out
-    if rows is not None:
-        got = got[:, rows]
-    return got, ref, mag, not d["f32"]
-
-
-def _replay_gns(plan, rows):
-    gns = _gn_rows(rows)
-    for i, d in enumerate(gns):
-        films = [None] if d["film"] == "none" else ["image", "shared"]
-        print(f"[gn route] {plan} {d['H']}x{d['W']} C={d['C']}: route={d['route']} slots={d['slots']} "
-              f"K={d['slots'] * d['C'] // 32} items per group")
-        for film in films:
-            L = Case(d["N"], d["H"], d["W"], d["C"], eps=d["eps"], silu=d["silu"], film=film, seed=i, device="cuda")
-            slots = d["slots"] if d["route"].startswith("stats") else None
-            out = L.run(d["route"], slots=slots)
-            again = L.run(d["route"], slots=slots)
-            assert torch.equal(G.bits(out[0]), G.bits(again[0])), f"{plan} {d}: two launches differ"
-            if out[2] is not None:
-                assert torch.equal(G.bits(out[2]), G.bits(again[2])), f"{plan} {d}: gstat of two launches differ"
-            del again
-            info = out[1]
-            assert (info["slots"], info["apply_ctas"], info["apply_rows"], info["csplit"]) == \
-                (d["slots"], d["apply"], d["rows"], d["csplit"]), f"{plan} {d}: launched {info}"
-            L.check(f"{plan} {d} film={film}", d["route"], out, rows=band_rows(d["H"]))
-            del L, out
-            _free()
-    return len(gns)
-
-
-def _replay_windows(plan, rows):
-    attn = _distinct(rows, _ATTN)
-    for i, d in enumerate(attn):
-        H, W, ws, shift, N, heads, hd, hpc, simt = map(int, d)
-        assert not simt
-        L = WindowCase("randn", N, H // ws, W // ws, heads, ws, hd, shift, seed=i)
-        out, info = L.check(f"{plan} attn {d}", hpc=0)
-        assert info["hpc"] == hpc, (d, info)
-        again, _ = run_window(L.qkv, L.dense, heads, ws, hd, shift, 0, False)
-        assert torch.equal(G.bits(out), G.bits(again)), f"{plan} attn {d}: two launches differ"
-        kp, ks, s16 = kappas("window", ws * ws, hd)
-        _note("window attention", _worst_window(L, out, kp, ks, s16))
-        del L
-        _free()
-    return len(attn)
-
-
-def _worst_window(L, out, kp, ks, s16):
-    from tests.test_gpu_attention import from_windows
-    B, T = L.r["o"].shape[0], L.ws * L.ws
-    a = from_windows(allowance(L.r, kp, ks, s16).permute(0, 2, 1, 3).reshape(B, T, -1), L.N, L.H, L.W, L.ws, L.shift)
-    err = (out.double() - L.ref).abs()
-    return ((err - 0.5 * G.ulp16(L.ref)).clamp(min=0) / a).max().item()
-
-
-def _replay_swins(plan, rows):
-    swin = _distinct(rows, _SWIN)
-    for i, d in enumerate(swin):
-        H, W, shift, grid, N, E, heads, slots = map(int, d)
-        L = SwinCase("randn", N, H, W, E, shift, slots, seed=i)
-        y, pout, info = L.run(0)
-        assert info["grid"] == grid, (d, info)
-        y2, pout2 = L.check(f"{plan} swin_attn {d}")
-        assert torch.equal(G.bits(y), G.bits(y2)) and torch.equal(G.bits(pout), G.bits(pout2)), f"{plan} swin {d}: differ"
-        err = (y.double() - L.ref).abs()
-        _note("fused Swin attention", ((err - 0.5 * G.ulp16(L.ref)).clamp(min=0) / L.allow).max().item())
-        del L, y, y2
-        _free()
-    return len(swin)
-
-
-def _replay_mlps(plan, rows, N=1):
-    mlps = _distinct(rows, _MLP)
-    for i, d in enumerate(mlps):
-        H, W, E, Hd, _grid = map(int, d)
-        g = _gen(100 + i)
-        x = (torch.randn(N, H, W, E, device="cuda", generator=g) * 1.5 + 0.3).half()
-        res = torch.randn(N, H, W, E, device="cuda", generator=g).half()
-        w1 = torch.randn(Hd, E, device="cuda", generator=g) / E ** 0.5
-        b1 = torch.randn(Hd, device="cuda", generator=g) * 0.5
-        w2 = torch.randn(E, Hd, device="cuda", generator=g) / Hd ** 0.5
-        b2 = torch.randn(E, device="cuda", generator=g) * 0.5
-        w1p, _ = G.pack_weight(w1)
-        w2p, _ = G.pack_weight(w2)
-        out, _ = _mlp(x, res, w1p, b1, w2p, b2, E, Hd)
-        out2, _ = _mlp(x, res, w1p, b1, w2p, b2, E, Hd)
-        assert torch.equal(G.bits(out), G.bits(out2)), f"{plan} mlp {d}: two launches differ"
-        sel = band_rows(H)
-        xs, rs, os_ = (t if sel is None else t[:, sel] for t in (x, res, out))
-        ref, mag, slack = mlp_reference(xs.reshape(-1, E), rs.reshape(-1, E), w1, b1, w2, b2)
-        _note("fused MLP", G.assert_within(f"{plan} mlp {d}", os_.reshape(-1, E), ref, mag, MLP_KAPPA, slack=slack) / MLP_KAPPA)
-        _free()
-    return len(mlps)
-
-
-_UPSAMPLE = re.compile(r"upsample (\d+)x(\d+) C=(\d+)$")
-
-
-def _replay_upsamples(plan, rows, N=1):
-    from tests.test_gpu_unetconv import resample_case
-    ups = _distinct(rows, _UPSAMPLE)
-    for H, W, Cc in ups:
-        resample_case(N, int(H), int(W), int(Cc), False)
-        _free()
-    return len(ups)
+        G.free()
+    return len(convs), {}
 
 
 # op kinds checked elsewhere in this module: the T = 262144 attention by b
@@ -298,26 +131,29 @@ CHECKED_BY = {"vq_attn": "test_vq_attention_* (b)"}
 def test_plan_replay(plan):
     rows = plan_rows(plan)
     assert rows
-    kinds = {"conv": _replay_convs, "gn": _replay_gns, "attn": _replay_windows, "swin_attn": _replay_swins,
-             "mlp": _replay_mlps, "upsample": _replay_upsamples}
+    replays = {"conv": lambda: _replay_convs(plan, rows), "gn": lambda: plan_ops.replay_gns(plan, rows),
+               "attn": lambda: plan_ops.replay_windows(plan, rows),
+               "swin_attn": lambda: plan_ops.replay_swins(plan, rows), "mlp": lambda: plan_ops.replay_mlps(plan, rows),
+               "upsample": lambda: plan_ops.replay_resamples(rows, 1)}
     done = {}
-    for kind, fn in kinds.items():
-        done[kind] = fn(plan, rows)
-    for r in _distinct(rows, _VQ):
+    for kind, replay in replays.items():
+        done[kind], obs = replay()
+        for k, r in obs.items():
+            _note(f"gn {k}" if kind == "gn" else k, r)
+    for r in plan_ops.distinct(rows, "vq_attn"):
         assert tuple(map(int, r)) == (T_CLI, C_CLI, 1), r          # the shape b holds to float64
     REPLAYED[plan] = done
     print(f"[plan] {plan}: " + ", ".join(f"{n} distinct {k}" for k, n in done.items()))
-    claimed = [k + " " for k in done if k not in ("conv",)] + ["conv", "vq_attn "]
-    unclaimed = [r for r in rows if not any(r.startswith(c) for c in claimed)]
+    unclaimed = [r for r in rows if not plan_ops.claimed(r)]
     assert not unclaimed, f"{plan}: op rows no check claims: {sorted(set(unclaimed))}"
-    assert not any(_UNET.match(r) for r in rows)
+    assert not plan_ops.distinct(rows, "unet_attn")
 
 
 # ---------------------------------------------------------------------------------------------- b. T = 262144 attention
 
 def needle_qkv(T=T_CLI, Cc=C_CLI, seed=0):
     """fp16 q, k, v [1, T, C] of the needle class and j(r)."""
-    g = _gen(seed)
+    g = G.gen(seed)
     k = torch.where(torch.rand(1, T, Cc, device="cuda", generator=g) < 0.5, -2.0, 2.0).half()
     r = torch.arange(T, device="cuda")
     j = 16 * (r % 16384) + (r // 16384) % 16
@@ -339,7 +175,6 @@ def _vq_op(q, k, v, rows=None, out=None):
 
 @pytest.mark.parametrize("cls", ["needle", "randn", "peaked", "equal", "large"])
 def test_vq_attention_262144(cls):
-    from tests.test_gpu_attention import _online_qkv
     rows = attn_rows()
     if cls == "needle":
         q, k, v, j = needle_qkv(seed=3)
@@ -351,7 +186,7 @@ def test_vq_attention_262144(cls):
             s[torch.arange(r.numel(), device="cuda"), j[r]] = -1e9
             assert (top - s.amax(1)).min().item() >= 40
     else:
-        q, k, v = (t[:, 0].half().contiguous() for t in _online_qkv(cls, 1, 1, T_CLI, C_CLI, _gen(7 + len(cls))))
+        q, k, v = (t[:, 0].half().contiguous() for t in online_qkv(cls, 1, 1, T_CLI, C_CLI, G.gen(7 + len(cls))))
     out = _vq_op(q, k, v)
     assert torch.isfinite(out).all()
     _note(f"vq<512> T=262144 {cls}", vq_check(cls, q, k, v, out, rows=rows))
@@ -387,11 +222,10 @@ def _vq_model(seed=0):
 @pytest.mark.parametrize("which", [0, 1])
 def test_vq_attention_plan_mid_blocks(which):
     """encoder.mid.attn_1 (which 0) / decoder.mid.attn_1 (which 1) of the 2048 plans, probed under RS_NO_REUSE=1."""
-    from tests.test_gpu_first_stage_kernels import _tokens, _w16, no_reuse
     p = ("encoder", "decoder")[which] + ".mid.attn_1"
     with no_reuse():
         cfg, sd, m = _vq_model()
-        g = _gen(40 + which)
+        g = G.gen(40 + which)
         if which == 0:
             m.encode(torch.rand(1, 3, 2048, 2048, device="cuda", generator=g) * 2 - 1)
         else:
@@ -399,21 +233,21 @@ def test_vq_attention_plan_mid_blocks(which):
         torch.cuda.synchronize()
         pr = {s: m.probe(which, 1, 2048, 2048, p + s) for s in (".in", ".q", ".k", ".v", ".attn", "")}
     del m
-    _free()
+    G.free()
     q, k, v, a = (pr[s].flatten(2).transpose(1, 2).half().contiguous() for s in (".q", ".k", ".v", ".attn"))
     assert q.shape == (1, T_CLI, C_CLI)
     assert torch.equal(pr[".v"].half().float(), pr[".v"]), "the .v probe is not the fp16 tensor the kernel read"
     rows = attn_rows()
     _note(f"plan {p}.attn", vq_check("plan", q, k, v, a, rows=rows))
-    x, out, at = (_tokens(pr[s])[0] for s in (".in", "", ".attn"))
-    wp, bp = _w16(sd, f"{p}.proj_out.weight", C_CLI), sd[f"{p}.proj_out.bias"].cuda().double()
+    x, out, at = (tokens(pr[s])[0] for s in (".in", "", ".attn"))
+    wp, bp = w16(sd, f"{p}.proj_out.weight", C_CLI), sd[f"{p}.proj_out.bias"].cuda().double()
     x, out, at = x[rows], out[rows], at[rows]
     ref = x + at @ wp.t() + bp
     mag = at.abs() @ wp.abs().t() + bp.abs() + x.abs()
     U32 = 2.0 ** -23
     _note(f"plan {p} output", G.assert_within(f"{p} block output", out, ref, (C_CLI + 2) * U32 * mag, 1.0))
     del pr
-    _free()
+    G.free()
 
 
 # ---------------------------------------------------------------------------------------------- c. GroupNorm, 32768 slots
@@ -437,44 +271,15 @@ def outlier_slots(slots, cpg, seed):
     return out
 
 
-def check_finalize_gstat(tag, L, gs, slots):
-    """gstat of gn_finalize_kernel against float64.  Besides test_gpu_groupnorm.py's fixed K_MU / K_R allowances, each of
-    the K = slots * cpg items passes through at most n + 16 fp32 roundings (n = K / 256 in one thread's sequential sum,
-    5 shuffle levels, 8 warp partials, the pivot subtraction and the scaling), so with d_i = mean_i - pivot:
-        |mean - mean64| <= K_MU U (|mean64| + std64) + (n + 16) U mean|d_i|
-        |rstd / rstd64 - 1| <= K_R U + (n + 16) U (1/2 (var + dm^2) + |dm| mean|d_i|) / (var + eps),  dm = mean(d_i),
-    the first-order bound of a recursive fp32 sum (relative to the sum of |terms|) pushed through the mean and through
-    rsqrt(m2 / (ns K) + eps).  At K = 262144 the count-dependent term is what the rstd needs (n = 1024)."""
-    from tests.test_gpu_groupnorm import K_MU, K_R, U
-    N, Cc = L.N, L.C
-    cpg = Cc // 32
-    items = L.conv_pairs()[0].double()[..., 0].reshape(N, slots, 32, cpg).permute(0, 2, 1, 3).reshape(N, 32, -1)
-    n = items.shape[-1] // 256
-    dd = items - items[..., :1]
-    md, dm = dd.abs().mean(-1), dd.mean(-1)
-    mu, var, sd = L.group_stats()
-    gs = gs.double()
-    assert torch.isfinite(gs).all(), f"{tag}: gstat not written"
-    a_mu = K_MU * U * (mu.abs() + sd) + (n + 16) * U * md
-    a_r = K_R * U + (n + 16) * U * (0.5 * (var + dm * dm) + dm.abs() * md) / (var + L.eps)
-    e_mu = ((gs[..., 0] - mu).abs() / a_mu).max().item()
-    e_r = ((gs[..., 1] * (var + L.eps).sqrt() - 1).abs() / a_r).max().item()
-    _note("gn finalize outlier: mean", e_mu)
-    _note("gn finalize outlier: rstd", e_r)
-    print(f"[gn outlier] {tag}: mean {e_mu:.3g}, rstd {e_r:.3g} of the bound (n = {n})")
-    assert e_mu <= 1 and e_r <= 1, f"{tag}: gstat mean {e_mu:.2f}, rstd {e_r:.2f} of the bound"
-
-
 @pytest.mark.parametrize("plan", ["vq_f4_encode_2048", "vq_f4_decode_2048"])
 def test_groupnorm_outlier_slots(plan):
-    from tests.test_gpu_groupnorm import _box
-    rows = [d for d in _gn_rows(plan_rows(plan)) if d["H"] == 2048]
+    rows = [d for d in plan_ops.gn_rows(plan_rows(plan)) if d["H"] == 2048]
     assert rows, "no GroupNorm at 2048x2048"
     fin = [d for d in rows if d["route"] == "finalize"]
     print(f"[gn route] {plan} 2048x2048: " + ", ".join(f"C={d['C']} route={d['route']} slots={d['slots']}" for d in rows))
     assert fin, "no 2048x2048 GroupNorm takes the finalisation route"
     for i, d in enumerate(fin):
-        bw, bh, box_n, slots = _box(d["H"], d["W"])
+        bw, bh, box_n, slots = G.box128(d["H"], d["W"])
         assert slots == d["slots"] == 32768 and box_n == 1
         cpg = d["C"] // 32
         print(f"[gn outlier] {plan} C={d['C']}: K = {slots * cpg} items per group, remainder {slots * cpg % 1024}")
@@ -489,21 +294,20 @@ def test_groupnorm_outlier_slots(plan):
             out = L.run("finalize")
             assert out[1]["finalize"], out[1]
             tag = f"{plan} C={d['C']} outlier slots placement {placement}"
-            check_finalize_gstat(tag, L, out[2], slots)
-            L.check_y(tag, "finalize", out[0], rows=band_rows(d["H"]))
+            e_mu, e_r = check_finalize_gstat(tag, L.x64, L.eps, out[2], slots)
+            _note("gn finalize outlier: mean", e_mu)
+            _note("gn finalize outlier: rstd", e_r)
+            L.check_y(tag, out[0], rows=plan_ops.band_rows(d["H"]))
             del L, out
-            _free()
+            G.free()
 
 
 # ---------------------------------------------------------------------------------------------- d. end to end
 
 @pytest.fixture
 def fp32_reference():
-    old = (torch.backends.cuda.matmul.allow_tf32, torch.backends.cudnn.allow_tf32)
-    torch.backends.cuda.matmul.allow_tf32 = False
-    torch.backends.cudnn.allow_tf32 = False
-    yield
-    torch.backends.cuda.matmul.allow_tf32, torch.backends.cudnn.allow_tf32 = old
+    with G.fp32_matmuls():
+        yield
 
 
 def _report(tag, got, ref, tol_max=TOL_MAX, tol_mean=TOL_MEAN):
@@ -519,7 +323,7 @@ _ORACLE = {}
 
 
 def _lq(seed=61):
-    return torch.rand(1, 3, 512, 512, device="cuda", generator=_gen(seed)) * 2 - 1
+    return torch.rand(1, 3, 512, 512, device="cuda", generator=G.gen(seed)) * 2 - 1
 
 
 def _oracle_z_y():
@@ -549,7 +353,7 @@ def test_decode_512_latent(fp32_reference):
     from oracle import vq_options_oracle as vx
     cfg, sd, m = _vq_model()
     sd = {n: t.cuda() for n, t in sd.items()}
-    z = torch.randn(1, 3, 512, 512, device="cuda", generator=_gen(62)) * 0.6
+    z = torch.randn(1, 3, 512, 512, device="cuda", generator=G.gen(62)) * 0.6
     got = m.decode(z, force_not_quantize=True)
     with torch.no_grad():
         ref = vx.vq_decode(z, sd, cfg, force_not_quantize=True, chunk=2048)
@@ -572,7 +376,7 @@ def test_decode_batch2(fp32_reference):
     """chop_bs = 2: 2^31-byte 128-channel and 2^32-byte 256-channel activations."""
     from oracle import vq_options_oracle as vx
     cfg, sd, m = _vq_model()
-    g = _gen(63)
+    g = G.gen(63)
     z = torch.randn(2, 3, 512, 512, device="cuda", generator=g) * 0.6
     a = m.decode(z, force_not_quantize=True)[1].clone()
     z2 = z.clone()
@@ -580,7 +384,7 @@ def test_decode_batch2(fp32_reference):
     b = m.decode(z2, force_not_quantize=True)[1].clone()
     assert torch.equal(G.bits(a), G.bits(b)), "image 1 changed with image 0"
     del m
-    _free()
+    G.free()
     sd = {n: t.cuda() for n, t in sd.items()}
     with torch.no_grad():
         ref = vx.vq_decode(z[1:], sd, cfg, force_not_quantize=True, chunk=2048)[0]
@@ -593,14 +397,13 @@ def test_denoiser_512(fp32_reference):
     from resshift_b200.config import preset
     from resshift_b200.models.unet import UNetModelSwin
     from resshift_b200.weights import random_state_dict
-    from tests.test_gpu_unet import FWD_MAX, FWD_MEAN
     ucfg, _ = preset("realsr")
     sd = random_state_dict(ucfg, 0)
     m = UNetModelSwin(**ucfg.to_kwargs())
     m.load_state_dict(sd)
     m = m.cuda().eval()
     sdc = {n: t.cuda() for n, t in sd.items()}
-    g = _gen(64)
+    g = G.gen(64)
     x = torch.randn(1, 3, 512, 512, device="cuda", generator=g)
     lq = torch.rand(1, 3, 512, 512, device="cuda", generator=g) * 2 - 1
     for tt in (14, 2):
@@ -608,8 +411,8 @@ def test_denoiser_512(fp32_reference):
         got = m(x, t, lq=lq)
         with torch.no_grad():
             ref = uo.unet_forward(sdc, ucfg, x, t, lq=lq)
-        mx, mn = _report(f"realsr denoiser 512x512 b1 t={tt}", got, ref, FWD_MAX, FWD_MEAN)
-        assert mx <= FWD_MAX and mn <= FWD_MEAN
+        mx, mn = _report(f"realsr denoiser 512x512 b1 t={tt}", got, ref, G.FWD_MAX, G.FWD_MEAN)
+        assert mx <= G.FWD_MAX and mn <= G.FWD_MEAN
 
 
 def test_cli_unit_sampler(fp32_reference):
@@ -621,7 +424,6 @@ def test_cli_unit_sampler(fp32_reference):
     from resshift_b200.sampler import ResShiftSampler, make_configs
     from resshift_b200.vq_arch import random_vq_state_dict, vq_preset
     from resshift_b200.weights import random_state_dict
-    from tests.test_gpu_unet import FWD_MEAN
     ucfg, dcfg = preset("realsr_journal")
     dcfg.sf = 4
     vcfg = vq_preset("f4")
@@ -632,7 +434,7 @@ def test_cli_unit_sampler(fp32_reference):
     T = diff.num_timesteps
     assert T == 4
     y0 = _lq()
-    g = _gen(65)
+    g = G.gen(65)
     noises = torch.stack([torch.randn(1, 3, 512, 512, device="cuda", generator=g) for _ in range(T + 1)])
     sd_u = {n: t.cuda() for n, t in random_state_dict(ucfg, 0).items()}
     sd_v = {n: t.cuda() for n, t in random_vq_state_dict(vcfg, 0).items()}
@@ -647,8 +449,8 @@ def test_cli_unit_sampler(fp32_reference):
     mx, mn = _report("CLI unit: z_y", z_y, z_y_ref)
     assert mx <= TOL_MAX and mn <= TOL_MEAN
     z = diff.sample_latent(z_y, model, {"lq": y0}, noises=noises)
-    mx, mn = _report("CLI unit: final latent", z, z_ref, TOL_MAX, FWD_MEAN)
-    assert mx <= TOL_MAX and mn <= FWD_MEAN
+    mx, mn = _report("CLI unit: final latent", z, z_ref, TOL_MAX, G.FWD_MEAN)
+    assert mx <= TOL_MAX and mn <= G.FWD_MEAN
     img_same = aem.decode(z_ref)
     flips = (aem.last_indices.to(idx_ref.device) != idx_ref).float().mean().item()
     mx, mn = _report(f"CLI unit: decode(quantise(z_ref)), code flips {flips * 100:.4f} %", img_same, img_ref)
@@ -669,7 +471,7 @@ def test_cli_unit_sampler(fp32_reference):
 
 def test_tile_gather_cli_geometry():
     """Two 2048x2048 tiles at output columns 0 and 1792 (stride 448 x 4) against float64."""
-    g = _gen(66)
+    g = G.gen(66)
     N, Cc, th, tw = 1, 3, 2048, 2048
     ys, xs = [0], [0, 1792]
     H, W = th, xs[-1] + tw
@@ -696,7 +498,7 @@ def test_tile_gather_cli_geometry():
 
 # ---------------------------------------------------------------------------------------------- report
 
-def test_report():
+def test_report(module_clock):
     """Run with the rest of the module: the worst ratio of error to bound per check, ops per plan, wall time, memory."""
     if not OBS:
         pytest.skip("run with the rest of the module")
@@ -705,5 +507,5 @@ def test_report():
     for plan, d in REPLAYED.items():
         print(f"[replayed] {plan}: " + ", ".join(f"{n} {k}" for k, n in d.items()))
     props = torch.cuda.get_device_properties(0)
-    print(f"[cli tile] wall time {time.time() - _T0[0]:.1f} s, peak max_memory_allocated "
+    print(f"[cli tile] wall time {time.time() - module_clock:.1f} s, peak max_memory_allocated "
           f"{torch.cuda.max_memory_allocated() / 2 ** 30:.1f} GiB on {props.name}")

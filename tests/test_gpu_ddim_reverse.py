@@ -24,7 +24,7 @@ from oracle.make_golden_ddpm import learned_range_model
 from resshift_b200 import _lib
 from resshift_b200.models import gaussian_diffusion as gd
 from resshift_b200.models.script_util import create_gaussian_diffusion, create_gaussian_diffusion_ddpm
-from tests.test_gpu_ddpm import _bound, _cached_model, _compare, _dev32, _ulps
+from tests.sampler_ref import bound, cached_model, compare, dev32, ulps
 
 pytestmark = pytest.mark.gpu
 
@@ -37,8 +37,8 @@ def gold(golden_dir):
 
 
 def _step_args(diff, mean_eps, clip, t, x, out, x_next, x0_out, next_in=None, counters=None, n_counters=0):
-    tabs = [_dev32(diff.sqrt_recip_alphas_cumprod), _dev32(diff.sqrt_recipm1_alphas_cumprod),
-            _dev32(diff.alphas_cumprod_next)]
+    tabs = [dev32(diff.sqrt_recip_alphas_cumprod), dev32(diff.sqrt_recipm1_alphas_cumprod),
+            dev32(diff.alphas_cumprod_next)]
     N, Cc, H, W = x.shape
     a = _lib.DdimReverseStepArgsC(out.data_ptr(), x.data_ptr(), x_next.data_ptr(),
                                   tabs[0].data_ptr(), tabs[1].data_ptr(), tabs[2].data_ptr(),
@@ -77,8 +77,8 @@ def test_step_kernel_is_reference_expression(mean, clip):
         torch.cuda.synchronize()
         ref = _torch_step(diff, bool(clip), t, x, out)
         tag = f"{mean} clip={clip} t={t}"
-        assert torch.equal(G.bits(x0), G.bits(ref["pred_xstart"])), f"{tag}: pred_xstart, {_ulps(x0, ref['pred_xstart'])} ulp"
-        assert torch.equal(G.bits(x_next), G.bits(ref["sample"])), f"{tag}: sample, {_ulps(x_next, ref['sample'])} ulp"
+        assert torch.equal(G.bits(x0), G.bits(ref["pred_xstart"])), f"{tag}: pred_xstart, {ulps(x0, ref['pred_xstart'])} ulp"
+        assert torch.equal(G.bits(x_next), G.bits(ref["sample"])), f"{tag}: sample, {ulps(x_next, ref['sample'])} ulp"
         if clip:
             assert x0.abs().max() <= 1.0
         exp_next = torch.full_like(next_in, 7.0)
@@ -126,7 +126,7 @@ TEACHER = [
 @pytest.mark.parametrize("family,name,kw,clip", TEACHER,
                          ids=[f"{t[0]}-{'x0' if t[2] else 'eps'}-clip{int(t[3])}" for t in TEACHER])
 def test_loop_is_forwards_and_steps(family, name, kw, clip):
-    m, (H, W) = _cached_model(family, name)
+    m, (H, W) = cached_model(family, name)
     diff = create_gaussian_diffusion_ddpm(**KW8, **kw)
     assert diff.timestep_map != list(range(diff.num_timesteps))
     T, B = diff.num_timesteps, 2
@@ -157,7 +157,7 @@ def test_loop_is_forwards_and_steps(family, name, kw, clip):
 @pytest.mark.parametrize("case", FUSED)
 def test_fused_case_matches_reference(gold, case):
     family, name, kw, clip, _ = CASES[case]
-    m, hw = _cached_model(family, name)
+    m, hw = cached_model(family, name)
     assert hw == model_config(case)[1]
     diff = create_gaussian_diffusion_ddpm(**diffusion_kwargs(case))
     lq, x_start = (v.cuda() for v in case_inputs(case))
@@ -177,14 +177,14 @@ def test_fused_case_matches_reference(gold, case):
         # position, plus the model-output bound.  x0 carries sqrt(1 / acp_t) |d x_t| for eps prediction (the clamp only
         # shrinks errors); the sample sqrt(acp_next) |d x0| + sqrt(1 - acp_next) |d eps'| with
         # |d eps'| <= (sqrt(1 / acp_t) |d x_t| + |d x0|) / sqrt(1 / acp_t - 1).
-        mx, mn = _bound(ref_x, f)
+        mx, mn = bound(ref_x, f)
         carried = A * d_prev if eps else 0.0 * d_prev
         d_x = np.abs(got_x - ref_x)
         print(f"{case} pred_xstart {t}: max|d| {d_x.max():.3e} mean|d| {d_x.mean():.3e} (carried from x_t: max "
               f"{np.max(carried):.3e}; model bounds {mx:.3e} / {mn:.3e})")
         assert (d_x < carried + mx).all() and d_x.mean() < np.mean(carried) + mn, f"{case} pred_xstart {t}"
         carried = np.sqrt(an) * d_x + np.sqrt(1 - an) * (A * d_prev + d_x) / B
-        mx, mn = _bound(ref_s, f)
+        mx, mn = bound(ref_s, f)
         d_s = np.abs(got_s - ref_s)
         print(f"{case} sample {t}: max|d| {d_s.max():.3e} mean|d| {d_s.mean():.3e} (carried: max "
               f"{np.max(carried):.3e}; model bounds {mx:.3e} / {mn:.3e})")
@@ -193,7 +193,7 @@ def test_fused_case_matches_reference(gold, case):
         last = (float(np.max(carried)) + mx, float(np.mean(carried)) + mn)
     final = diff.reverse_latent(m, x_start, {"lq": lq}, clip)
     assert torch.equal(G.bits(final), G.bits(rec[-1]["sample"]))
-    _compare(f"{case} final", final.cpu(), gold[f"{case}/final"], last)     # every position, the last step's bounds
+    compare(f"{case} final", final.cpu(), gold[f"{case}/final"], last)     # every position, the last step's bounds
 
 
 def test_torch_route_learned_range(gold):
@@ -204,7 +204,7 @@ def test_torch_route_learned_range(gold):
     out = diff.ddim_reverse_sample_loop(learned_range_model, x_start, clip_denoised=False, model_kwargs={"lq": lq})
     assert out.is_cuda
     ref = gold["e/final"]
-    _compare("e final", out.cpu(), ref, bounds=(1e-4 * np.abs(ref).max(), 1e-5 * np.abs(ref).max()))
+    compare("e final", out.cpu(), ref, bounds=(1e-4 * np.abs(ref).max(), 1e-5 * np.abs(ref).max()))
 
 
 # ------------------------------------------------------------------------------------------------ loop properties
@@ -217,7 +217,7 @@ def _inputs(H, W, seed, B=2):
 
 
 def test_graph_replay_equals_eager():
-    m, (H, W) = _cached_model("unetmodel", "legacy")
+    m, (H, W) = cached_model("unetmodel", "legacy")
     lq, x, _ = _inputs(H, W, 15)
     for kw, clip in ((dict(), True), (dict(predict_xstart=True), False)):
         diff = create_gaussian_diffusion_ddpm(**KW8, **kw)
@@ -228,7 +228,7 @@ def test_graph_replay_equals_eager():
 
 
 def test_image_independent_of_batch():
-    m, (H, W) = _cached_model("unetconv", "defaults")
+    m, (H, W) = cached_model("unetconv", "defaults")
     diff = create_gaussian_diffusion_ddpm(**KW8)
     lq, x, g = _inputs(H, W, 16)
     a = diff.reverse_latent(m, x, {"lq": lq}, True)
@@ -242,7 +242,7 @@ def test_image_independent_of_batch():
 
 def test_reverse_ddpm_and_resshift_samplers_alternate_on_one_plan():
     from resshift_b200.config import DiffusionConfig
-    m, (H, W) = _cached_model("unetmodel", "legacy")
+    m, (H, W) = cached_model("unetmodel", "legacy")
     rs = create_gaussian_diffusion(**DiffusionConfig(steps=4, min_noise_level=0.2, sf=1).to_kwargs())
     dd = create_gaussian_diffusion_ddpm(**KW8)
     lq, x, g = _inputs(H, W, 18)
@@ -268,7 +268,7 @@ def test_reverse_ddpm_and_resshift_samplers_alternate_on_one_plan():
 def test_invert_then_ddim_fused_equals_torch_route():
     """x_0 -> x_T by inversion, then x_T -> x_0 by ddim_sample_loop(eta=0): the fused route for both against the torch
     route for both (the same native UNet called step by step through a wrapper the fused gate does not take)"""
-    m, (H, W) = _cached_model("unetmodel", "legacy")
+    m, (H, W) = cached_model("unetmodel", "legacy")
     diff = create_gaussian_diffusion_ddpm(**KW8)
     lq, x, _ = _inputs(H, W, 19)
     kw = {"lq": lq}
@@ -277,15 +277,15 @@ def test_invert_then_ddim_fused_equals_torch_route():
     xt_fused = diff.ddim_reverse_sample_loop(m, x, clip_denoised=False, model_kwargs=kw)
     xt_torch = diff.ddim_reverse_sample_loop(wrapped, x, clip_denoised=False, model_kwargs=kw)
     f = float(np.max(diff.sqrt_recipm1_alphas_cumprod))
-    _compare("x_T fused vs torch route", xt_fused.cpu(), xt_torch.cpu().double().numpy(),
-             _bound(xt_torch.cpu().numpy(), f))
+    compare("x_T fused vs torch route", xt_fused.cpu(), xt_torch.cpu().double().numpy(),
+             bound(xt_torch.cpu().numpy(), f))
     torch.manual_seed(0)
     back_fused = diff.ddim_sample_loop(m, tuple(x.shape), noise=xt_fused, clip_denoised=False, model_kwargs=kw, eta=0.0)
     torch.manual_seed(0)
     back_torch = diff.ddim_sample_loop(wrapped, tuple(x.shape), noise=xt_torch, clip_denoised=False, model_kwargs=kw,
                                        device="cuda", eta=0.0)
-    _compare("x_0 round trip fused vs torch route", back_fused.cpu(), back_torch.cpu().double().numpy(),
-             _bound(back_torch.cpu().numpy(), f))
+    compare("x_0 round trip fused vs torch route", back_fused.cpu(), back_torch.cpu().double().numpy(),
+             bound(back_torch.cpu().numpy(), f))
     d = (back_fused - x).abs()
     print(f"round trip vs x_start: max|d| {d.max():.3e} mean|d| {d.mean():.3e}; fused == torch route: "
           f"x_T {torch.equal(xt_fused, xt_torch)}, x_0 {torch.equal(back_fused, back_torch)}")
@@ -293,7 +293,7 @@ def test_invert_then_ddim_fused_equals_torch_route():
 
 def test_host_entry_point():
     """rs_sampler_run_host sizes its staging for a sampler that reads no noises, and returns the device run's latent"""
-    m, (H, W) = _cached_model("unetmodel", "legacy")
+    m, (H, W) = cached_model("unetmodel", "legacy")
     diff = create_gaussian_diffusion_ddpm(**KW8)
     lq, x, _ = _inputs(H, W, 20)
     ref = diff.reverse_latent(m, x, {"lq": lq}, True)
@@ -315,7 +315,7 @@ def test_host_entry_point():
 
 
 def test_c_abi_refusals():
-    m, (H, W) = _cached_model("unetmodel", "legacy")
+    m, (H, W) = cached_model("unetmodel", "legacy")
     plan = m.plan(2, H, W)
     diff = create_gaussian_diffusion_ddpm(**KW8)
     tabs = diff.ddim_reverse_tables()

@@ -23,7 +23,7 @@ from oracle.make_golden_ddpm import CASES, E_STEPS, FUSED, OUT_STRIDE, case_inpu
 from resshift_b200 import _lib
 from resshift_b200.models import gaussian_diffusion as gd
 from resshift_b200.models.script_util import create_gaussian_diffusion, create_gaussian_diffusion_ddpm
-from resshift_b200.weights import random_state_dict
+from tests.sampler_ref import bound, cached_model, compare, dev32, ulps
 
 pytestmark = pytest.mark.gpu
 
@@ -36,16 +36,11 @@ def gold(golden_dir):
     return np.load(golden_dir / "ddpm.npz")
 
 
-def _dev32(a):
-    """_extract_into_tensor's fp32 rounding of a float64 table, on the device"""
-    return torch.from_numpy(np.asarray(a, dtype=np.float64)).float().cuda()
-
-
 def _step_args(diff, kind, mean_eps, clip, eta, t, x, out, noise, x_next, x0_out, next_in=None, counters=None, n_counters=0):
-    tabs = {n: _dev32(getattr(diff, n)) for n in ROWS}
+    tabs = {n: dev32(getattr(diff, n)) for n in ROWS}
     small = diff.model_var_type == gd.ModelVarTypeDDPM.FIXED_SMALL
-    tabs["log_var"] = _dev32(diff.posterior_log_variance_clipped if small else diff.log_variance_fixed_large)
-    tabs["acp"], tabs["acp_prev"] = _dev32(diff.alphas_cumprod), _dev32(diff.alphas_cumprod_prev)
+    tabs["log_var"] = dev32(diff.posterior_log_variance_clipped if small else diff.log_variance_fixed_large)
+    tabs["acp"], tabs["acp_prev"] = dev32(diff.alphas_cumprod), dev32(diff.alphas_cumprod_prev)
     N, Cc, H, W = x.shape
     a = _lib.DdpmStepArgsC(out.data_ptr(), x.data_ptr(), noise.data_ptr(), x_next.data_ptr(),
                            tabs[ROWS[0]].data_ptr(), tabs[ROWS[1]].data_ptr(), tabs[ROWS[2]].data_ptr(),
@@ -62,13 +57,6 @@ def _torch_step(diff, kind, clip, eta, t, x, out, noise):
     tt = torch.full((x.shape[0],), t, device="cuda", dtype=torch.long)
     pmv = diff.p_mean_variance(lambda xx, ts, **k: out, x, tt, clip_denoised=clip)
     return diff._ddim_finish(x, tt, pmv, noise, eta) if kind == "ddim" else diff._p_finish(x, tt, pmv, noise)
-
-
-def _ulps(a, b):
-    ia, ib = G.bits(a).long(), G.bits(b).long()
-    ia = torch.where(ia < 0, -(ia & 0x7FFFFFFF), ia)
-    ib = torch.where(ib < 0, -(ib & 0x7FFFFFFF), ib)
-    return int((ia - ib).abs().max())
 
 
 # ------------------------------------------------------------------------------------------------ step kernel
@@ -98,8 +86,8 @@ def test_step_kernel_is_reference_expression(kind, mean, clip, var):
             torch.cuda.synchronize()
             ref = _torch_step(diff, kind, bool(clip), eta, t, x, out, noise)
             tag = f"{kind} {mean} clip={clip} {var} eta={eta} t={t}"
-            assert torch.equal(G.bits(x0), G.bits(ref["pred_xstart"])), f"{tag}: pred_xstart, {_ulps(x0, ref['pred_xstart'])} ulp"
-            assert torch.equal(G.bits(x_next), G.bits(ref["sample"])), f"{tag}: sample, {_ulps(x_next, ref['sample'])} ulp"
+            assert torch.equal(G.bits(x0), G.bits(ref["pred_xstart"])), f"{tag}: pred_xstart, {ulps(x0, ref['pred_xstart'])} ulp"
+            assert torch.equal(G.bits(x_next), G.bits(ref["sample"])), f"{tag}: sample, {ulps(x_next, ref['sample'])} ulp"
             if clip:
                 assert x0.abs().max() <= 1.0
             exp_next = torch.full_like(next_in, 7.0)
@@ -136,34 +124,6 @@ def test_step_kernel_refusals():
 
 # ------------------------------------------------------------------------------------------------ models
 
-def _model(family, name):
-    from resshift_b200.config import preset
-    from resshift_b200.models.unet import UNetModel, UNetModelConv, UNetModelSwin
-    if family == "unetmodel":
-        from oracle.make_golden_unetmodel import case_config
-        ucfg, _, hw = case_config(name)
-        cls = UNetModel
-    elif family == "unetconv":
-        from oracle.make_golden_unetconv import case_config
-        ucfg, _, hw = case_config(name)
-        cls = UNetModelConv
-    else:
-        ucfg, _ = preset(name)
-        hw, cls = (64, 64), UNetModelSwin
-    m = cls(**ucfg.to_kwargs())
-    m.load_state_dict(random_state_dict(ucfg, 0), strict=True)
-    return m.cuda().eval(), hw
-
-
-_MODELS = {}
-
-
-def _cached_model(family, name):
-    if (family, name) not in _MODELS:
-        _MODELS[(family, name)] = _model(family, name)
-    return _MODELS[(family, name)]
-
-
 # (family, model case, loop, diffusion kwargs, clip, eta)
 TEACHER = [
     ("swin", "tiny", "ancestral", dict(predict_xstart=True, sigma_small=True), True, 0.0),
@@ -175,7 +135,7 @@ TEACHER = [
 
 @pytest.mark.parametrize("family,name,loop,kw,clip,eta", TEACHER, ids=[f"{t[0]}-{t[2]}" for t in TEACHER])
 def test_loop_is_forwards_and_steps(family, name, loop, kw, clip, eta):
-    m, (H, W) = _cached_model(family, name)
+    m, (H, W) = cached_model(family, name)
     diff = create_gaussian_diffusion_ddpm(**KW8, **kw)
     assert diff.timestep_map != list(range(diff.num_timesteps))
     T, B = diff.num_timesteps, 2
@@ -200,26 +160,9 @@ def test_loop_is_forwards_and_steps(family, name, loop, kw, clip, eta):
 
 def _case_model(case):
     family, name = CASES[case][:2]
-    m, hw = _cached_model(family, name)
+    m, hw = cached_model(family, name)
     assert hw == model_config(case)[1]
     return m, hw
-
-
-def _bound(ref, factor=1.0):
-    """test_gpu_unetmodel's bounds on a denoiser output (1e-2 max, 3e-3 mean), scaled by what carries that error into the
-    step's results: the trajectory's magnitude (unclipped eps trajectories reach |x| ~ 85, and the denoiser's error is
-    relative), and for eps prediction the x0 conversion's factor sqrt(1 / acp_t - 1) (``factor``, at most 15.9 on the
-    1000 -> 8 schedule), which multiplies the model output's error in pred_xstart and in the step built on it"""
-    s = max(1.0, float(np.abs(ref).max())) * max(1.0, factor)
-    return 1e-2 * s, 3e-3 * s
-
-
-def _compare(tag, got, ref, bounds=None):
-    got = np.asarray(got, dtype=np.float64)
-    d = np.abs(got - ref)
-    mx, mn = bounds or _bound(ref)
-    print(f"{tag}: max|d| {d.max():.3e} (bound {mx:.3e}) mean|d| {d.mean():.3e} (bound {mn:.3e}) max|ref| {np.abs(ref).max():.3e}")
-    assert d.max() < mx and d.mean() < mn, tag
 
 
 def _progressive(diff, loop, m, noises, lq, clip, eta, monkeypatch):
@@ -257,7 +200,7 @@ def test_fused_case_matches_reference(gold, case, monkeypatch):
         # model-output bound: x0 carries sqrt(1 / acp_t) |d x_t| for eps prediction (the clamp only shrinks errors);
         # the ancestral sample coef1 |d x0| + coef2 |d x_t|; the DDIM sample sqrt(acp_prev) |d x0| + sqrt(1 - acp_prev -
         # sigma^2) |d eps'| with |d eps'| <= (sqrt(1 / acp_t) |d x_t| + |d x0|) / sqrt(1 / acp_t - 1).
-        mx, mn = _bound(ref_x, f)
+        mx, mn = bound(ref_x, f)
         carried = A * d_prev if eps else 0.0 * d_prev
         d_x = np.abs(got_x - ref_x)
         print(f"{case} pred_xstart {k}: max|d| {d_x.max():.3e} mean|d| {d_x.mean():.3e} (carried from x_t: max "
@@ -269,7 +212,7 @@ def test_fused_case_matches_reference(gold, case, monkeypatch):
             carried = np.sqrt(abp) * d_x + np.sqrt(max(1 - abp - sig ** 2, 0.0)) * (A * d_prev + d_x) / B
         else:
             carried = float(diff.posterior_mean_coef1[t]) * d_x + float(diff.posterior_mean_coef2[t]) * d_prev
-        mx, mn = _bound(ref_s, f)
+        mx, mn = bound(ref_s, f)
         d_s = np.abs(got_s - ref_s)
         print(f"{case} sample {k}: max|d| {d_s.max():.3e} mean|d| {d_s.mean():.3e} (carried: max "
               f"{np.max(carried):.3e}; model bounds {mx:.3e} / {mn:.3e})")
@@ -278,7 +221,7 @@ def test_fused_case_matches_reference(gold, case, monkeypatch):
         last = (float(np.max(carried)) + mx, float(np.mean(carried)) + mn)
     final = diff.sample_latent(m, noises, {"lq": lq}, loop, clip, eta)
     assert torch.equal(G.bits(final), G.bits(rec[-1]["sample"]))
-    _compare(f"{case} final", final.cpu(), gold[f"{case}/final"], last)     # every position, the last step's bounds
+    compare(f"{case} final", final.cpu(), gold[f"{case}/final"], last)     # every position, the last step's bounds
     if case == "a":
         from resshift_b200.models.autoencoder import VQModelTorch
         from resshift_b200.vq_arch import random_vq_state_dict, vq_preset
@@ -288,12 +231,12 @@ def test_fused_case_matches_reference(gold, case, monkeypatch):
         vq = vq.cuda().eval()
         # the bookend on the reference's own final latent: the decode alone
         ref_dec = diff.decode_first_stage(torch.from_numpy(gold["a/final"]).cuda(), vq)
-        _compare("a decoded (reference latent)", ref_dec.reshape(-1)[::OUT_STRIDE].cpu(), gold["a/decoded"])
+        compare("a decoded (reference latent)", ref_dec.reshape(-1)[::OUT_STRIDE].cpu(), gold["a/decoded"])
         # end to end: the nearest-code quantiser turns the loop's latent error into a whole code wherever it crosses a
         # boundary between codes, so the decoded image is held to the mean bound only
         dec = diff.decode_first_stage(final, vq)
         ref = gold["a/decoded"]
-        _compare("a decoded", dec.reshape(-1)[::OUT_STRIDE].cpu(), ref, bounds=(float("inf"), _bound(ref)[1]))
+        compare("a decoded", dec.reshape(-1)[::OUT_STRIDE].cpu(), ref, bounds=(float("inf"), bound(ref)[1]))
         # p_sample_loop returns the same decoded image
         queue = list(noises[1:])
         monkeypatch.setattr(torch, "randn_like", lambda ref: queue.pop(0))
@@ -312,8 +255,8 @@ def test_generic_route_80_steps(gold, monkeypatch):
     assert diff.num_timesteps == 80 and not diff._native_ok(m, None, {"lq": lq})
     rec = _progressive(diff, loop, m, noises, lq, clip, eta, monkeypatch)
     for k in E_STEPS:
-        _compare(f"e sample {k}", rec[k]["sample"].reshape(-1)[::OUT_STRIDE].cpu(), gold[f"e/sample/{k}"])
-    _compare("e final", rec[-1]["sample"].cpu(), gold["e/final"])
+        compare(f"e sample {k}", rec[k]["sample"].reshape(-1)[::OUT_STRIDE].cpu(), gold[f"e/sample/{k}"])
+    compare("e final", rec[-1]["sample"].cpu(), gold["e/final"])
 
 
 def test_generic_route_learned_range(gold, monkeypatch):
@@ -327,13 +270,13 @@ def test_generic_route_learned_range(gold, monkeypatch):
                              model_kwargs={"lq": lq}, device="cuda")
     monkeypatch.undo()
     ref = gold["f/final"]
-    _compare("f final", out.cpu(), ref, bounds=(1e-4 * np.abs(ref).max(), 1e-5 * np.abs(ref).max()))
+    compare("f final", out.cpu(), ref, bounds=(1e-4 * np.abs(ref).max(), 1e-5 * np.abs(ref).max()))
 
 
 # ------------------------------------------------------------------------------------------------ loop properties
 
 def test_graph_replay_equals_eager():
-    m, (H, W) = _cached_model("unetmodel", "legacy")
+    m, (H, W) = cached_model("unetmodel", "legacy")
     diff = create_gaussian_diffusion_ddpm(**KW8)
     g = torch.Generator(device="cuda").manual_seed(5)
     lq = torch.rand(2, 3, H, W, device="cuda", generator=g) * 2 - 1
@@ -346,7 +289,7 @@ def test_graph_replay_equals_eager():
 
 
 def test_image_independent_of_batch():
-    m, (H, W) = _cached_model("unetconv", "defaults")
+    m, (H, W) = cached_model("unetconv", "defaults")
     diff = create_gaussian_diffusion_ddpm(**KW8)
     g = torch.Generator(device="cuda").manual_seed(6)
     lq = torch.rand(2, 3, H, W, device="cuda", generator=g) * 2 - 1
@@ -362,7 +305,7 @@ def test_image_independent_of_batch():
 
 def test_ddpm_and_resshift_samplers_alternate_on_one_plan():
     from resshift_b200.config import DiffusionConfig
-    m, (H, W) = _cached_model("unetmodel", "legacy")
+    m, (H, W) = cached_model("unetmodel", "legacy")
     rs = create_gaussian_diffusion(**DiffusionConfig(steps=4, min_noise_level=0.2, sf=1).to_kwargs())
     dd = create_gaussian_diffusion_ddpm(**KW8)
     g = torch.Generator(device="cuda").manual_seed(8)
@@ -383,7 +326,7 @@ def test_ddpm_and_resshift_samplers_alternate_on_one_plan():
 
 
 def test_c_abi_refusals():
-    m, (H, W) = _cached_model("unetmodel", "legacy")
+    m, (H, W) = cached_model("unetmodel", "legacy")
     plan = m.plan(2, H, W)
     diff = create_gaussian_diffusion_ddpm(**KW8)
     tabs = diff.ddpm_tables()

@@ -54,8 +54,6 @@ c. The quantiser's output (`quantize`, the decoder's first conv input) against f
 test_coverage prints the worst ratio of each check to its allowance.
 """
 import math
-import os
-from contextlib import contextmanager
 from dataclasses import replace
 
 import pytest
@@ -65,88 +63,17 @@ pytestmark = pytest.mark.gpu
 
 if torch.cuda.is_available():
     from tests import gpu_util as G
-    from resshift_b200 import _lib
+    from tests import plan_ops
+    from tests.first_stage_ref import (FTZ, R32, S16, SM_CLASSES, U16, U32, f32, no_reuse, softmax_allowance, softmax_case,
+                                       tokens, w16)
 
-U16, U32, R32, S16 = 2.0 ** -11, 2.0 ** -23, 2.0 ** -24, 2.0 ** -25
-FTZ = 2.0 ** -126
-SM_CLASSES = ("randn", "uniform", "equal", "peaked", "gap")
 W_CLASSES = ("drawn", "peaked", "uniform", "bias")
 
 RAN = set()          # what ran
 OBS = {}             # worst ratio per check
 
 
-def _note(check, ratio):
-    OBS[check] = max(OBS.get(check, 0.0), ratio)
-
-
-def _gen(seed):
-    return torch.Generator(device="cuda").manual_seed(seed)
-
-
-def _f32(x):
-    """x rounded to fp32, as a Python float."""
-    return torch.tensor(x, dtype=torch.float32).item()
-
-
 # ------------------------------------------------------------------------------------------------ a. row softmax
-
-def softmax_allowance(z, cols):
-    """float64 softmax of the logits z [rows, cols] and its per-element allowance (module docstring, a)."""
-    m = z.amax(-1, keepdim=True)
-    d = z - m
-    e = torch.exp(d)
-    p = e / e.sum(-1, keepdim=True)
-    rho = (z.abs() + d.abs()) * R32 + (2 + 1.173 * d.abs()) * U32
-    n_l = 8 * -(-cols // 2048) + 12
-    rel = torch.expm1(rho + (p * rho).sum(-1, keepdim=True) + (n_l + 2) * R32)
-    return p, rel
-
-
-def peak_columns(cols):
-    """The first and last column, and one column in the range of every warp of every 16-byte vector a thread holds."""
-    out = [0, cols - 1]
-    for i in range(4):
-        for w in range(8):
-            start = 2048 * i + 256 * w
-            if start < cols:
-                out.append(min(start + (37 * (8 * i + w)) % 256, cols - 1))
-    return out
-
-
-def score_rows(rows, cols, scale, seed):
-    """fp16 S [rows][cols] and the input class of each row (module docstring, a)."""
-    g = _gen(seed)
-    z = torch.empty(rows, cols, device="cuda")
-    peaks = peak_columns(cols)
-    classes = ["peaked"] if rows == 1 else [SM_CLASSES[r % len(SM_CLASSES)] for r in range(rows)]
-    counts = {"peaked": 0, "gap": 0}
-    for cls in SM_CLASSES:
-        idx = [r for r in range(rows) if classes[r] == cls]
-        if not idx:
-            continue
-        sel = torch.tensor(idx, device="cuda")
-        n = len(idx)
-        if cls == "randn":
-            z[sel] = 3 * torch.randn(n, cols, device="cuda", generator=g)
-        elif cls == "uniform":
-            z[sel] = 1e-3 * torch.randn(n, cols, device="cuda", generator=g)
-        elif cls == "equal":
-            z[sel] = 0.7
-        else:
-            lo, hi, top = (-40.0, 30.0, 40.0) if cls == "peaked" else (-55.0, -45.0, 50.0)
-            z[sel] = lo + (hi - lo) * torch.rand(n, cols, device="cuda", generator=g)
-            pos = torch.tensor([peaks[(counts[cls] + k) % len(peaks)] for k in range(n)], device="cuda")
-            z[sel, pos] = top
-            counts[cls] += n
-    return (z / scale).half(), classes
-
-
-def run_softmax(s, rows, cols, ld, scale):
-    """rs_op_softmax_rows in place on the fp16 [rows][ld] buffer s."""
-    _lib.check(_lib.lib.rs_op_softmax_rows(s.data_ptr(), rows, cols, ld, scale, G.stream()))
-    torch.cuda.synchronize()
-
 
 SOFTMAX_COLS = sorted({8, 16, 56, 64, 1792, 1800, 2048, 2056, 4096, 6144, 6152, 8184, 8192} |
                       {256, 384, 1024, 2880})          # the last four: the T of plans in b not among the first
@@ -157,54 +84,13 @@ SOFTMAX_ROWS = {"1": (lambda c: 1, 0), "300": (lambda c: 300, 24), "T": (lambda 
 @pytest.mark.parametrize("cols", SOFTMAX_COLS)
 def test_softmax_rows(cols, rows_key):
     nrows, pad = SOFTMAX_ROWS[rows_key]
-    softmax_case(nrows(cols), cols, cols + pad)
-
-
-def softmax_case(rows, cols, ld):
-    """rs_op_softmax_rows on rows x cols scores of every class in an fp16 [rows][ld] buffer, against float64."""
-    scale = _f32((64, 128, 512)[cols % 3] ** -0.5)
-    s, classes = score_rows(rows, cols, scale, seed=cols * 7 + rows)
-    sentinel = 1234.0
-    buf = torch.full((rows, ld), sentinel, dtype=torch.float16, device="cuda")
-    buf[:, :cols] = s
-    run_softmax(buf, rows, cols, ld, scale)
-    assert (buf[:, cols:] == sentinel).all(), "columns beyond cols were written"
-    again = torch.full_like(buf, sentinel)
-    again[:, :cols] = s
-    run_softmax(again, rows, cols, ld, scale)
-    assert torch.equal(G.bits(again), G.bits(buf)), "not bit-reproducible"
-    step = max(1, (1 << 23) // cols)
-    cls_t = torch.tensor([SM_CLASSES.index(c) for c in classes], device="cuda")
-    for r0 in range(0, rows, step):
-        r1 = min(rows, r0 + step)
-        p, rel = softmax_allowance(s[r0:r1].double() * scale, cols)
-        got = buf[r0:r1, :cols]
-        allow = p * rel + FTZ
-        tag = f"softmax cols={cols} rows={rows} ld={ld} rows {r0}:{r1}"
-        G.assert_within(tag, got, p, allow, 1.0)
-        for ci, cls in enumerate(SM_CLASSES):
-            sel = cls_t[r0:r1] == ci
-            if sel.any():
-                _note(f"softmax {cls}", G.accumulation_ratio(got[sel], p[sel], allow[sel]))
-                RAN.add(("softmax class", cls))
+    for cls, r in softmax_case(nrows(cols), cols, cols + pad)[1].items():
+        G.note(OBS, f"softmax {cls}", r)
+        RAN.add(("softmax class", cls))
     RAN.add(("softmax cols", cols))
 
 
 # ------------------------------------------------------------------------------------------------ b. plan attention
-
-@contextmanager
-def no_reuse():
-    """Plans created inside keep every tensor alive for rs_plan_probe."""
-    old = os.environ.get("RS_NO_REUSE")
-    os.environ["RS_NO_REUSE"] = "1"
-    try:
-        yield
-    finally:
-        if old is None:
-            os.environ.pop("RS_NO_REUSE", None)
-        else:
-            os.environ["RS_NO_REUSE"] = old
-
 
 def options_config():
     """Attention at every level at C = 64, 192, 384 (a partial W_v tile at 64 and 192, channels not a power of two)."""
@@ -250,15 +136,6 @@ def attention_blocks(cfg, which):
     return out + [f"decoder.up.{i}.attn.{j}" for i in reversed(range(L)) if cfg.dec_attn[i] for j in range(cfg.num_res_blocks[i] + 1)]
 
 
-def _tokens(t):
-    """[N, C, H, W] -> [N, T, C] float64."""
-    return t.flatten(2).transpose(1, 2).double()
-
-
-def _w16(sd, name, cc):
-    return sd[name].reshape(cc, -1).cuda().half().double()
-
-
 def check_block(tag, m, sd, key, p):
     """The block's attention output and block output against float64 (module docstring, b).  Returns C, T, the span of
     the scaled logits and the worst ratio to the bound of each check."""
@@ -266,10 +143,10 @@ def check_block(tag, m, sd, key, p):
     pr = {s: m.probe(which, B, H, W, p + s) for s in (".in", ".norm", ".q", ".k", ".attn", "")}
     cc = pr[".q"].shape[1]
     T = pr[".q"].shape[2] * pr[".q"].shape[3]
-    x, n, q, k, a, out = (_tokens(pr[s]) for s in (".in", ".norm", ".q", ".k", ".attn", ""))
-    wv, bv = _w16(sd, f"{p}.v.weight", cc), sd[f"{p}.v.bias"].cuda().double()
-    wp, bp = _w16(sd, f"{p}.proj_out.weight", cc), sd[f"{p}.proj_out.bias"].cuda().double()
-    scale = _f32(cc ** -0.5)
+    x, n, q, k, a, out = (tokens(pr[s]) for s in (".in", ".norm", ".q", ".k", ".attn", ""))
+    wv, bv = w16(sd, f"{p}.v.weight", cc), sd[f"{p}.v.bias"].cuda().double()
+    wp, bp = w16(sd, f"{p}.proj_out.weight", cc), sd[f"{p}.proj_out.bias"].cuda().double()
+    scale = f32(cc ** -0.5)
     worst_a = worst_o = span = 0.0
     step = max(1, (1 << 23) // T)
     for b in range(B):
@@ -306,7 +183,7 @@ def _model(kind, cfg, sd):
 
 
 def _run_pass(m, kind, cfg, which, B, H, W, seed):
-    g = _gen(seed)
+    g = G.gen(seed)
     if which == 0:
         x = torch.rand(B, 3, H, W, device="cuda", generator=g) * 2 - 1
         m.encode(x, sample_posterior=False) if kind == "kl" else m.encode(x)
@@ -339,7 +216,6 @@ def test_plan_attention(plan):
     """Every GEMM-form attention block of the plan, in every weight class: `<p>.attn` and `<p>` within their float64
     bounds; the op list runs one row softmax of T columns per block and image, and no fused attention."""
     from resshift_b200.vq_arch import random_kl_state_dict, random_vq_state_dict
-    from tests.test_gpu_conv_instances import _desc_rows
     kind, name, which, B, H, W = PLANS[plan]
     cfg = _config(kind, name)
     sd = (random_kl_state_dict if kind == "kl" else random_vq_state_dict)(cfg, 0)
@@ -362,12 +238,12 @@ def test_plan_attention(plan):
             print(f"[plan] {plan} {cls} {p}: C={cc} T={T} scaled logits within +-{span:.1f}")
             if cls == "peaked":
                 assert span >= 15, (p, span)
-            _note(f"attn {cls}", wa)
-            _note("block output", wo)
+            G.note(OBS, f"attn {cls}", wa)
+            G.note(OBS, "block output", wo)
             RAN.add(("ct", cc, T))
             RAN.add(("weight class", cls))
         if cls == "drawn":
-            rows = _desc_rows(_lib.lib.rs_vq_profile_ops, m.plan(which, B, H, W).handle)
+            rows = plan_ops.vq_rows(m.plan(which, B, H, W))
             softmax = [r for r in rows if r.startswith("softmax")]
             want = sorted(f"softmax {ts[p]}" for p in blocks for _ in range(B))
             assert sorted(softmax) == want and not [r for r in rows if r.startswith("vq_attn")], (softmax, want)
@@ -402,7 +278,7 @@ def test_quantize_output(name, B, H, W):
     sd["post_quant_conv.bias"] = 0.5 * torch.randn(sd["post_quant_conv.bias"].shape, generator=torch.Generator().manual_seed(3))
     m = _model("vq", cfg, sd)
     f = cfg.downscale
-    g = _gen(17)
+    g = G.gen(17)
     z = torch.randn(B, cfg.embed_dim, H // f, W // f, device="cuda", generator=g) * 0.6
     book = sd["quantize.embedding.weight"].cuda().double()
     m.decode(z)
@@ -410,12 +286,12 @@ def test_quantize_output(name, B, H, W):
     assert ((idx >= 0) & (idx < cfg.n_embed)).all()
     ref, mag, E = _post_quant_ref(book[idx], sd)
     got = m.probe(1, B, H, W, "quantize")
-    _note("quantize codes", G.assert_within(f"{name} quantize (codes)", got, ref, E * R32 * mag, 1.0))
+    G.note(OBS, "quantize codes", G.assert_within(f"{name} quantize (codes)", got, ref, E * R32 * mag, 1.0))
     m.decode(z, force_not_quantize=True)
     assert (m.last_indices == -1).all()
     ref_z, mag_z, _ = _post_quant_ref(z.double().permute(0, 2, 3, 1), sd)
-    _note("quantize z", G.assert_within(f"{name} quantize (force_not_quantize)", m.probe(1, B, H, W, "quantize"), ref_z,
-                                        E * R32 * mag_z, 1.0))
+    G.note(OBS, "quantize z", G.assert_within(f"{name} quantize (force_not_quantize)", m.probe(1, B, H, W, "quantize"),
+                                              ref_z, E * R32 * mag_z, 1.0))
     bad = idx.clone()
     hits = [(0, 3, 5, cfg.n_embed), (B - 1, H // f - 2, 1, -1)]
     for n_, y_, x_, v_ in hits:

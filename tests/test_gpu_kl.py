@@ -16,6 +16,7 @@ import pytest
 import torch
 
 from oracle import kl_oracle as ko
+from tests.gpu_util import fp32_matmuls
 
 pytestmark = pytest.mark.gpu
 
@@ -24,11 +25,8 @@ MAX_ABS, MEAN_ABS = 1e-2, 2e-3
 
 @pytest.fixture(scope="module")
 def fp32_reference():
-    old = (torch.backends.cuda.matmul.allow_tf32, torch.backends.cudnn.allow_tf32)
-    torch.backends.cuda.matmul.allow_tf32 = False
-    torch.backends.cudnn.allow_tf32 = False
-    yield
-    torch.backends.cuda.matmul.allow_tf32, torch.backends.cudnn.allow_tf32 = old
+    with fp32_matmuls():
+        yield
 
 
 _MODELS = {}

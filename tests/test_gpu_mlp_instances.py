@@ -7,53 +7,23 @@ H = fp16(GELU(X W1^T + b1)), and of the output fp16(res + b2 + H W2^T).  Per ele
 |got - ref| <= 1/2 ulp16(ref) + KAPPA * mag2 + slack, with mag2 = |H| |W2|^T + |b2| + |res| and slack = sum_j |W2_ij| e_j
 over the hidden values whose float64 value lies so close to an fp16 rounding boundary (closer than the first GEMM's
 allowance KAPPA * (|X| |W1|^T + |b1|) x 1.13) that the kernel may have rounded it to the neighbour (e_j = that spacing)."""
-import ctypes as C
-
 import pytest
 import torch
-import torch.nn.functional as F
 
 pytestmark = pytest.mark.gpu
 
 if torch.cuda.is_available():
     from tests import gpu_util as G
+    from tests import plan_ops
+    from tests.mlp_ref import KAPPA, mlp, reference
     from resshift_b200 import _lib
 
-# the conv tests' allowance (test_gpu_conv_instances.py: 6.6 times the largest ratio observed there).  On an H100 80GB HBM3
-# (700 W) no MLP output exceeded 1/2 ulp16 + slack at all: every deviation from the float64 reference was explained by
-# hidden values rounded to the neighbouring fp16 number, so the slack term dominates this bound
-KAPPA = 2.0 ** -18
-ACT_GAIN = 1.13
 # (N, H, W): 8x8 with an odd batch (two images per 128-pixel tile, the second tile half padding), 16x16, 64x64, 32x64
 MAPS = {"8x8_n3": (3, 8, 8), "16x16_n2": (2, 16, 16), "64x64_n1": (1, 64, 64), "32x64_n2": (2, 32, 64)}
 # input: "none" = the random tensor as is; "gstat" / "pairs" = that tensor normalised by the separate GroupNorm apply the
 # Swin block runs in front of the MLP (norm2), from finalised group statistics or from the producers' per-slot pairs
 CASES = [(E, r, m, src) for E in (64, 128, 192, 256) for r in (4, 2) for m in MAPS
          for src in (("none", "gstat", "pairs") if r == 4 else ("none",))]
-
-
-def _box(H, W):
-    def p2(x, cap):
-        p = 1
-        while p * 2 <= cap and x % (p * 2) == 0:
-            p *= 2
-        return p
-    bw = p2(W, 128)
-    bh = p2(H, 128 // bw)
-    return bw, bh, (W // bw) * (H // bh)
-
-
-def _mlp(x, res, w1p, b1, w2p, b2, E, Hd, sinks=()):
-    N, H, W, _ = x.shape
-    out = torch.full_like(x, float("nan"))
-    parts = (C.c_void_p * 2)(*[s[0].data_ptr() for s in sinks] + [None] * (2 - len(sinks)))
-    cst = (C.c_int32 * 2)(*[s[1] for s in sinks] + [0] * (2 - len(sinks)))
-    cof = (C.c_int32 * 2)(*[s[2] for s in sinks] + [0] * (2 - len(sinks)))
-    slots_out = C.c_int32()
-    _lib.check(_lib.lib.rs_op_mlp_ex(x.data_ptr(), N, H, W, E, Hd, w1p.data_ptr(), b1.data_ptr(), w2p.data_ptr(), b2.data_ptr(),
-                                     _lib.ptr(res), out.data_ptr(), parts, cst, cof, C.byref(slots_out), G.stream()))
-    torch.cuda.synchronize()
-    return out, slots_out.value
 
 
 def _group_stats(x, N):
@@ -69,25 +39,6 @@ def _slot_pairs(x, bw, bh, slots):
     t = x.float().reshape(N, H // bh, bh, W // bw, bw, E).permute(0, 1, 3, 2, 4, 5).reshape(N, slots, bh * bw, E)
     m = t.mean(dim=2)
     return torch.stack([m, ((t - m[:, :, None]) ** 2).sum(dim=2)], dim=-1).contiguous()
-
-
-def _reference(xin, res, w1, b1, w2, b2):
-    """float64 output, mag2 and slack (module docstring) of the MLP on the fp16 input xin [M, E]."""
-    x = xin.double()
-    w1q, w2q = w1.half().double(), w2.half().double()
-    pre = x @ w1q.T + b1.double()
-    dh = KAPPA * ACT_GAIN * (x.abs() @ w1q.abs().T + b1.double().abs()) + 2.0 ** -21 * pre.abs()
-    h64 = F.gelu(pre)
-    h16 = h64.half()
-    hc = h16.cpu()                                          # (fp16 nextafter on the CPU)
-    inf = torch.full_like(hc, float("inf"))
-    up, dn = (torch.nextafter(hc, s * inf).to(h16.device).double() for s in (1, -1))
-    hq = h16.double()
-    near = (h64 + dh >= 0.5 * (hq + up)) | (h64 - dh <= 0.5 * (hq + dn))
-    e = torch.where(near, torch.maximum(up - hq, hq - dn), torch.zeros_like(hq))
-    out = hq @ w2q.T + b2.double() + res.double()
-    mag = hq.abs() @ w2q.abs().T + b2.double().abs() + res.double().abs()
-    return out, mag, e @ w2q.abs().T
 
 
 @pytest.mark.parametrize("E,ratio,map_,src", CASES, ids=[f"E{e}-Hd{r}E-{m}-{n}" for e, r, m, n in CASES])
@@ -108,7 +59,7 @@ def test_fused_mlp_vs_float64(E, ratio, map_, src):
     beta = 0.2 * torch.randn(E, device="cuda", generator=g)
     w1p, _ = G.pack_weight(w1)
     w2p, _ = G.pack_weight(w2)
-    bw, bh, slots = _box(H, W)
+    bw, bh, _, slots = G.box128(H, W)
     n_sinks = CASES.index((E, ratio, map_, src)) % 3
     xin = x
     if src != "none":
@@ -135,16 +86,16 @@ def test_fused_mlp_vs_float64(E, ratio, map_, src):
     runs = []
     for _ in range(2):
         sk = sinks()
-        out, nslots = _mlp(xin, res, w1p, b1, w2p, b2, E, Hd, sinks=sk)
+        out, nslots = mlp(xin, res, w1p, b1, w2p, b2, E, Hd, sinks=sk)
         runs.append((out, sk))
     assert nslots == slots
     (out, sk), (out2, sk2) = runs
     assert torch.equal(G.bits(out), G.bits(out2))
     assert all(torch.equal(G.bits(a[0]), G.bits(b[0])) for a, b in zip(sk, sk2))
-    ref, mag, slack = _reference(xin.reshape(-1, E), res.reshape(-1, E), w1, b1, w2, b2)
+    ref, mag, slack = reference(xin.reshape(-1, E), res.reshape(-1, E), w1, b1, w2, b2)
     G.assert_within(f"mlp E={E} Hd={Hd} {map_} {src}", out.reshape(-1, E), ref, mag, KAPPA, slack=slack)
     for i, (part, cstride, coff) in enumerate(sk):
-        G.check_slot_pairs(f"mlp sink {i}", part, out, bw, bh, slots, cstride, coff)
+        G.check_slot_pairs(f"mlp sink {i}", part, out, cstride, coff)
 
 
 def test_mlp_refusals():
@@ -157,7 +108,7 @@ def test_mlp_refusals():
         w2p, _ = G.pack_weight(torch.randn(E, Hd, device="cuda", generator=g))
         b1, b2 = torch.zeros(Hd, device="cuda"), torch.zeros(E, device="cuda")
         with pytest.raises(_lib.RsError, match="fused MLP"):
-            _mlp(x, None, w1p, b1, w2p, b2, E, Hd)
+            mlp(x, None, w1p, b1, w2p, b2, E, Hd)
     attempt(96, 384)
     attempt(64, 4 * 64 + 32)
 
@@ -182,15 +133,7 @@ def _unet_vs_oracle(ucfg, expect_mlp_e):
     print(f"[unet] swin_embed_dim={ucfg.swin_embed_dim} mlp_ratio={ucfg.mlp_ratio}: max|d|={d.max():.3e} mean|d|={d.mean():.3e}")
     assert not torch.isnan(out).any()
     assert d.max().item() <= 1e-2 and d.mean().item() <= 2.5e-3          # test_gpu_unet_variants.py's forward bounds
-    plan = m.plan(2, 64, 64)
-    cap, stride = 2048, 256
-    ms = (C.c_double * cap)()
-    desc = C.create_string_buffer(cap * stride)
-    n = C.c_int32()
-    xc, tc, lqc = x.cuda(), t.float().cuda(), lq.cuda()
-    _lib.check(_lib.lib.rs_plan_profile_ops(plan.handle, xc.data_ptr(), tc.data_ptr(), lqc.data_ptr(), None, ms, desc, stride, cap,
-                                            C.byref(n), _lib.current_stream()))
-    rows = [desc.raw[i * stride:(i + 1) * stride].split(b"\0")[0].decode() for i in range(n.value)]
+    rows = plan_ops.plan_rows(m.plan(2, 64, 64), x.cuda(), t.float().cuda(), lq.cuda())
     mlps = [r for r in rows if r.startswith("mlp")]
     if expect_mlp_e:
         assert mlps and all(f"E={expect_mlp_e} " in r for r in mlps), mlps

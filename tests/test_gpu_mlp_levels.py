@@ -11,7 +11,7 @@ pytestmark = pytest.mark.gpu
 
 if torch.cuda.is_available():
     from tests import gpu_util as G
-    from tests.test_gpu_mlp_instances import KAPPA, _box, _reference
+    from tests.mlp_ref import KAPPA, reference
     from resshift_b200 import _lib
 
 LEVELS = (64, 32, 16, 8)
@@ -29,7 +29,7 @@ def test_fused_mlp_benchmark_levels(hw):
     b2 = torch.randn(E, device="cuda", generator=g) * 0.5
     w1p, _ = G.pack_weight(w1)
     w2p, _ = G.pack_weight(w2)
-    bw, bh, slots = _box(hw, hw)
+    slots = G.box128(hw, hw)[3]
     # two sinks with different channel strides and offsets, as test_fused_mlp_vs_float64 gives them
     specs = [(E + 8, 0), (E + 40, 8)]
 
@@ -51,7 +51,7 @@ def test_fused_mlp_benchmark_levels(hw):
     out2, sk2 = launch()
     assert torch.equal(G.bits(out), G.bits(out2))
     assert all(torch.equal(G.bits(a), G.bits(b)) for a, b in zip(sk, sk2))
-    ref, mag, slack = _reference(x.reshape(-1, E), res.reshape(-1, E), w1, b1, w2, b2)
+    ref, mag, slack = reference(x.reshape(-1, E), res.reshape(-1, E), w1, b1, w2, b2)
     G.assert_within(f"mlp b16 {hw}x{hw}", out.reshape(-1, E), ref, mag, KAPPA, slack=slack)
     for i, (part, (cs, co)) in enumerate(zip(sk, specs)):
-        G.check_slot_pairs(f"mlp b16 {hw}x{hw} sink {i}", part, out, bw, bh, slots, cs, co)
+        G.check_slot_pairs(f"mlp b16 {hw}x{hw} sink {i}", part, out, cs, co)

@@ -394,12 +394,12 @@ def test_window_attention(hw, shift, impl):
     """The 8x8-window, 32-wide-head core (tensor-core instance or SIMT cross-check) per element against float64
     (tests/test_gpu_attention.py), through rs_op_window_attention_cfg; the RS_ATTN_IMPL-selected rs_op_window_attention
     must give the same bits."""
-    from tests.test_gpu_attention import WindowCase
+    from tests.attn_ref import WindowCase
     H, W = hw
     if H == 8 and shift:
         pytest.skip("no shifted windows at a single-window resolution")
     L = WindowCase("randn", 2, H // 8, W // 8, 6, 8, 32, shift, seed=H * 7 + shift)
-    out, _ = L.check(f"window attention {hw} shift={shift} {impl}", simt=impl == "simt")
+    out, _, _ = L.check(f"window attention {hw} shift={shift} {impl}", simt=impl == "simt")
     old = torch.empty_like(out)
     os.environ["RS_ATTN_IMPL"] = impl
     try:
@@ -422,13 +422,13 @@ def test_swin_attention_half_fused(case, E, impl):
     per 8x8 window; a second run is bit-identical.  reference: models/swin_transformer.py:246-275,114-145.  (16, 64x64)
     is the benchmark shape: 512 window pairs on the persistent CTAs, several per CTA with the image changing inside a
     CTA's range; 24x40, 136x8, 7 x 8x8 and 7 x 16x24 have odd window counts per image, so pairs straddle images."""
-    from tests.test_gpu_attention import SwinCase
+    from tests.attn_ref import SwinCase
     if case[0] == 16 and E == 64:
         pytest.skip("the multi-tile case is covered at the model's width")
     N, H, W, shift = case
     slots = H * W // (128 if H * W % 128 == 0 else 64)
     L = SwinCase("randn", N, H, W, E, shift, slots, seed=E + H * 3 + shift + N)
-    y, pout = L.check(f"swin attn fused E={E} {case}")
+    y, pout, _, _ = L.check(f"swin attn fused E={E} {case}")
     y2, pout2, _ = L.run()
     assert torch.equal(G.bits(y), G.bits(y2)) and torch.equal(G.bits(pout), G.bits(pout2))
 

@@ -32,7 +32,7 @@ from resshift_b200.weights import random_state_dict
 if torch.cuda.is_available():
     from resshift_b200 import _lib
     from tests import gpu_util as G
-    from tests.test_gpu_sampler_kernels import step_bound, step_ref
+    from tests.sampler_ref import step_bound, step_ref
 
 FWD_MAX, FWD_MEAN = 1e-2, 2.5e-3
 KAPPA = 2.0

@@ -59,6 +59,7 @@ from resshift_b200.weights import random_state_dict
 if torch.cuda.is_available():
     from resshift_b200 import _lib
     from tests import gpu_util as G
+    from tests.sampler_ref import step_bound, step_ref
 
 U = 2.0 ** -24
 COVERED = {"pack": set(), "t": set(), "family": set()}
@@ -167,21 +168,6 @@ def _p_sample_args(x, x0, nz, out, tabs, T, t, N, Cc, HW, next_in=None, cpad=0, 
     a.next_in, a.next_cpad = _lib.ptr(next_in), cpad
     a.counters, a.n_counters = _lib.ptr(counters), n_counters
     return a
-
-
-def step_bound(x, x0, nz, t, ref64):
-    """The step bound of the module docstring for step t (x, x0, nz fp32 tensors)."""
-    c1, c2 = float(ref64["coef1"][t]), float(ref64["coef2"][t])
-    a, b = (c1 * x.double()).abs(), (c2 * x0.double()).abs()
-    if t == 0:
-        return 4 * U * (a + b)
-    sn = (float(ref64["std"][t]) * nz.double()).abs()
-    return 4 * U * (a + b) + 3 * U * sn + (2 + 0.5 * abs(float(ref64["log_var"][t]))) * U * sn
-
-
-def step_ref(x, x0, nz, t, ref64):
-    v = float(ref64["coef1"][t]) * x.double() + float(ref64["coef2"][t]) * x0.double()
-    return v + float(ref64["std"][t]) * nz.double() if t != 0 else v
 
 
 @pytest.mark.parametrize("N,Cc,H,W", [(2, 3, 64, 64), (1, 4, 37, 5), (3, 3, 7, 9)])

@@ -60,13 +60,13 @@ def _core(qkv, table, heads, ws, hd, shift, impl):
 def test_core_instances_vs_fp32_and_simt(ws, hd, heads, grid, shifted):
     """Each instance and the SIMT cross-check per element against float64 (tests/test_gpu_attention.py); the
     RS_ATTN_IMPL-selected rs_op_window_attention_ex gives the same bits as the explicit launch."""
-    from tests.test_gpu_attention import WindowCase
+    from tests.attn_ref import WindowCase
     if shifted and grid == (1, 1):
         pytest.skip("no shifted windows at a single-window resolution")
     shift = ws // 2 if shifted else 0
     L = WindowCase("randn", 3, grid[0], grid[1], heads, ws, hd, shift, seed=ws * 100 + hd + heads + grid[0] * ws + shift)
     for impl in ("mma", "simt"):
-        out, _ = L.check(f"core {impl} ws={ws} hd={hd} heads={heads} grid={grid} shift={shift}", simt=impl == "simt")
+        out, _, _ = L.check(f"core {impl} ws={ws} hd={hd} heads={heads} grid={grid} shift={shift}", simt=impl == "simt")
         assert torch.equal(out, _core(L.qkv, L.table, heads, ws, hd, shift, impl)), impl
 
 

@@ -3,18 +3,16 @@
 Epilogue: the conv's second, SiLU output (``rs_conv_args.silu_out``, a channel slice of a wider buffer) and its FiLM
 after the activation (``film``, one row per image or one shared row), on every route the launcher can take — one tile,
 CTA pair, persistent, persistent pair, split-K with the reduce kernel, the SIMT cross-check kernel, and RS_CONV_MSUB=2 /
-RS_CONV_EPI=direct, which the launcher steers to one sub-tile / the staged epilogue for such convs — against float64 with
-the error model
-of test_gpu_conv_instances.py.  silu_out must be within one fp16 ulp of SiLU of the stored output, repeated launches
-bit-identical, the reported route the forced one, and nothing outside the views written.  Resampling: pool / upsample
-with the SiLU output against torch.  Models: every fixture of tests/golden/unetconv.npz against the reference and the fp32
-oracle, a 64x128 latent, an image alone equal to the same image in a batch, the fused 4-step loop (graph replay equal to
-eager enqueue) against the reference's trajectory, ResShiftSampler end to end from a ``models.unet.UNetModelConv`` yaml,
-one GPU and a device pool."""
+RS_CONV_EPI=direct, which the launcher steers to one sub-tile / the staged epilogue for such convs — against float64
+with the error model of test_gpu_conv_instances.py (tests/conv_ref.py).  silu_out must be within one fp16 ulp of SiLU of
+the stored output, repeated launches bit-identical, the reported route the forced one, and nothing outside the views
+written.  Resampling: pool / upsample with the SiLU output against torch.  Models: every fixture of
+tests/golden/unetconv.npz against the reference and the fp32 oracle, a 64x128 latent, an image alone equal to the same
+image in a batch, the fused 4-step loop (graph replay equal to eager enqueue) against the reference's trajectory,
+ResShiftSampler end to end from a ``models.unet.UNetModelConv`` yaml, one GPU and a device pool."""
 import numpy as np
 import pytest
 import torch
-import torch.nn.functional as F
 
 pytestmark = pytest.mark.gpu
 
@@ -23,79 +21,13 @@ from oracle.make_golden_unetconv import CASES, OUT_STRIDE, case_config, case_inp
 from resshift_b200.weights import random_state_dict
 
 if torch.cuda.is_available():
-    import ctypes as C
     from resshift_b200 import _lib
     from tests import gpu_util as G
-    from tests.test_gpu_conv_instances import INFO_KEYS, KAPPA, MODES, Conv, _epi_bc, conv_env
+    from tests import plan_ops
+    from tests.conv_ref import MODES, Conv, check_silu_film, conv_env, epi_bc, film_rows, launch_silu, resample_case
 
 FWD_MAX, FWD_MEAN = 1e-2, 2.5e-3
 LOOP_MAX, LOOP_MEAN = 1e-2, 3e-3
-SILU_C0 = 16            # the SiLU output is the channel slice [16, 16 + Cout) of a buffer 40 channels wider
-
-
-def _nan16(*shape):
-    return torch.full(shape, float("nan"), dtype=torch.float16, device="cuda")
-
-
-def _launch(L, film, film_sN, bn=0, msub=0, splitk=False):
-    """One rs_op_conv2d_ex launch of Conv L with the SiLU output (and FiLM rows); returns (out buffer, silu buffer, info)."""
-    cw = (L.Cout + 7) // 8 * 8
-    out, silu = _nan16(L.N, L.Ho, L.Wo, cw + 8), _nan16(L.N, L.Ho, L.Wo, cw + 40)
-    a = _lib.ConvArgsC()
-    a.x, a.N, a.H, a.W, a.C, a.ld = L.xbuf.data_ptr() + 2 * L.xc0, L.N, L.H, L.W, L.cin_x, L.x_ld
-    a.w_packed, a.ipad = L.wp.data_ptr(), L.ipad
-    a.bias, a.bias_sN = _lib.ptr(L.bbuf), L.bias_sN
-    a.cout, a.ksize, a.stride, a.pad_lo = L.Cout, L.k, L.stride, L.pad_lo
-    if L.rbuf is not None:
-        a.residual, a.res_ld = L.rbuf.data_ptr(), L.rbuf.shape[-1]
-    a.out, a.out_ld = out.data_ptr(), out.shape[-1]
-    a.act, a.bn, a.msub = L.act, bn, msub
-    scratch = torch.empty(8 * L.N * L.Ho * L.Wo * L.Cout, device="cuda") if splitk else None
-    a.splitk_scratch = _lib.ptr(scratch)
-    a.silu_out, a.silu_ld = silu.data_ptr() + 2 * SILU_C0, silu.shape[-1]
-    a.film, a.film_sN = _lib.ptr(film), film_sN
-    info = (C.c_int32 * 12)()
-    _lib.check(_lib.lib.rs_op_conv2d_ex(C.byref(a), info, G.stream()))
-    torch.cuda.synchronize()
-    return out, silu, dict(zip(INFO_KEYS, list(info)))
-
-
-def _film_rows(L, form, seed):
-    """None, one row per image ([N, 2 Cout + 8], rows 2 Cout + 8 apart) or one shared row (film_sN = 0)."""
-    if form == "none":
-        return None, 0, None
-    g = torch.Generator(device="cuda").manual_seed(seed)
-    sN = 2 * L.Cout + 8
-    buf = torch.randn(L.N if form == "image" else 1, sN, device="cuda", generator=g) * 0.4
-    rows = buf[:, :2 * L.Cout].expand(L.N, 2 * L.Cout).double()
-    return buf, sN if form == "image" else 0, rows
-
-
-def _check(tag, L, form, seed, want, **kw):
-    """Two launches: bit-identical, the route wanted, out within the bound (FiLM: one more fp16 rounding before it), the
-    SiLU output within one fp16 ulp of SiLU(out), NaN fills outside both views intact."""
-    film, sN, rows = _film_rows(L, form, seed)
-    runs = [_launch(L, film, sN, **kw) for _ in range(2)]
-    (out, silu, info), (out2, silu2, info2) = runs
-    assert info == info2 and torch.equal(G.bits(out), G.bits(out2)) and torch.equal(G.bits(silu), G.bits(silu2)), \
-        f"{tag}: two launches differ"
-    for k, v in want.items():
-        assert (info[k] != 0 if v == "nonzero" else info[k] == v), f"{tag}: launched {k} = {info[k]}, wanted {v} ({info})"
-    Co = L.Cout
-    got, s = out[..., :Co], silu[..., SILU_C0:SILU_C0 + Co]
-    ref, mag = L.ref()
-    slack = None
-    if rows is not None:
-        one, sh = 1 + rows[:, None, None, :Co], rows[:, None, None, Co:]
-        slack = 0.5 * G.ulp16(ref.abs() + KAPPA * mag) * one.abs()        # the fp16 rounding before the FiLM
-        ref, mag = ref * one + sh, mag * one.abs() + sh.abs()
-    G.assert_within(tag, got, ref, mag, KAPPA, slack=slack)
-    sref = F.silu(got.double())
-    assert ((s.double() - sref).abs() <= G.ulp16(sref)).all(), f"{tag}: SiLU output beyond one fp16 ulp of SiLU(out)"
-    assert torch.isnan(out[..., Co:]).all(), f"{tag}: written beyond the output view"
-    assert torch.isnan(silu[..., :SILU_C0]).all() and torch.isnan(silu[..., SILU_C0 + Co:]).all(), \
-        f"{tag}: written outside the SiLU view"
-    return got, s
 
 
 # ---------------------------------------------------------------------------------------------- epilogue
@@ -111,11 +43,11 @@ def test_silu_output_and_film(mode, bn, form):
     L = Conv(3, 16, 16, 72, 2 * bn + 8, 3, act=2, bias="row" if msub == 2 else "image", res=form == "none", seed=bn + len(form))
     if msub == 2:
         with conv_env(**env), pytest.raises(_lib.RsError, match="sub-tiles"):
-            _launch(L, *_film_rows(L, form, bn)[:2], bn=bn, msub=2)
+            launch_silu(L, *film_rows(L, form, bn)[:2], bn=bn, msub=2)
         env = dict(env, RS_CONV_MSUB=2)
     with conv_env(**env):
-        _check(f"silu BN={bn} {mode} film={form}", L, form, bn, bn=bn,
-               want={"BN": bn, "cg": cg, "msub": 1, "persist": persist, "splitk": 1, "epi_bc": _epi_bc(bn)})
+        check_silu_film(f"silu BN={bn} {mode} film={form}", L, form, bn, bn=bn,
+                        want={"BN": bn, "cg": cg, "msub": 1, "persist": persist, "splitk": 1, "epi_bc": epi_bc(bn)})
 
 
 @pytest.mark.parametrize("form", ["none", "image", "shared"])
@@ -127,16 +59,16 @@ def test_silu_output_and_film_other_routes(route, form):
     if route == "split_k":
         L = Conv(3, 8, 8, 392, 104, 3, act=2, bias="image", res=res, seed=7 + len(form))
         with conv_env(RS_CONV_SPLITK=2, RS_CONV_PERSIST=0):
-            _check(f"split-K film={form}", L, form, 11, splitk=True, want={"splitk": 2, "epi_bc": 0, "persist": 0})
+            check_silu_film(f"split-K film={form}", L, form, 11, splitk=True, want={"splitk": 2, "epi_bc": 0, "persist": 0})
     else:
         L = Conv(3, 16, 16, 72, 88, 3, act=2, bias="image", res=res, seed=9 + len(form))
         env = {"RS_CONV_EPI": "direct"} if route == "direct" else {"RS_CONV_IMPL": "simt"}
         want = {"epi_bc": "nonzero"} if route == "direct" else {"epi_bc": 0, "splitk": 1}
         with conv_env(**env):
-            got, s = _check(f"{route} film={form}", L, form, 13, want=want)
+            got, s, _ = check_silu_film(f"{route} film={form}", L, form, 13, want=want)
         if route == "direct":     # the staged epilogue it was steered to: the same launch as without the override
             with conv_env():
-                got2, s2 = _check(f"staged film={form}", L, form, 13, want={"epi_bc": "nonzero"})
+                got2, s2, _ = check_silu_film(f"staged film={form}", L, form, 13, want={"epi_bc": "nonzero"})
             assert torch.equal(G.bits(got), G.bits(got2)) and torch.equal(G.bits(s), G.bits(s2))
 
 
@@ -145,7 +77,7 @@ def test_silu_output_refusals():
     film = torch.zeros(1, 128, device="cuda")
     with conv_env():
         with pytest.raises(_lib.RsError, match="no residual"):
-            _launch(L, film, 0)
+            launch_silu(L, film, 0)
 
 
 # ---------------------------------------------------------------------------------------------- resampling
@@ -154,29 +86,6 @@ def test_silu_output_refusals():
 @pytest.mark.parametrize("shape", [(2, 8, 12, 64), (3, 16, 16, 8), (1, 40, 24, 96)])
 def test_resample_with_silu_output(shape, pool):
     resample_case(*shape, pool)
-
-
-def resample_case(N, H, W, Cc, pool):
-    """rs_op_avgpool2x2 / rs_op_upsample2x_ex with the SiLU output against float64; without it, the same first output."""
-    g = torch.Generator(device="cuda").manual_seed(H * W + Cc)
-    x = (torch.randn(N, H, W, Cc, device="cuda", generator=g) * 3).half()
-    Ho, Wo = (H // 2, W // 2) if pool else (2 * H, 2 * W)
-    y, s = _nan16(N, Ho, Wo, Cc), _nan16(N, Ho, Wo, Cc)
-    fn = _lib.lib.rs_op_avgpool2x2 if pool else _lib.lib.rs_op_upsample2x_ex
-    _lib.check(fn(x.data_ptr(), N, H, W, Cc, y.data_ptr(), s.data_ptr(), G.stream()))
-    torch.cuda.synchronize()
-    xd = x.permute(0, 3, 1, 2).double()
-    ref = (F.avg_pool2d(xd, 2) if pool else F.interpolate(xd, scale_factor=2, mode="nearest")).permute(0, 2, 3, 1)
-    if pool:
-        assert ((y.double() - ref).abs() <= 0.5 * G.ulp16(ref) + 2.0 ** -22 * ref.abs()).all()
-    else:
-        assert torch.equal(y.double(), ref)
-    sref = F.silu(y.double())
-    assert ((s.double() - sref).abs() <= G.ulp16(sref)).all()
-    y2 = _nan16(N, Ho, Wo, Cc)
-    fn(x.data_ptr(), N, H, W, Cc, y2.data_ptr(), None, G.stream())     # without the second output: the same first one
-    torch.cuda.synchronize()
-    assert torch.equal(G.bits(y), G.bits(y2))
 
 
 # ---------------------------------------------------------------------------------------------- models
@@ -255,19 +164,11 @@ def test_native_inputs_are_checked():
 def test_plan_profile_names_the_silu_outputs():
     """Every conv / resample whose output a ResBlockConv or the head reads writes its SiLU twin; the in_layers convs of the
     scale-shift model apply FiLM rows."""
-    import ctypes
     ucfg, _, (h, w) = case_config("ss_updown")
     m = _model(ucfg)
     x, lq = case_inputs(ucfg, 2, h, w, 1)
     m(x.cuda(), torch.tensor([1, 2]).cuda(), lq=lq.cuda())
-    plan = m.plan(2, h, w)
-    cap, stride = 512, 256
-    ms, desc, n = (ctypes.c_double * cap)(), ctypes.create_string_buffer(cap * stride), ctypes.c_int32()
-    xf, lf = x.cuda().contiguous(), lq.cuda().contiguous()
-    t = torch.tensor([1.0, 2.0], device="cuda")
-    _lib.check(_lib.lib.rs_plan_profile_ops(plan.handle, xf.data_ptr(), t.data_ptr(), lf.data_ptr(), None, ms, desc, stride,
-                                            cap, ctypes.byref(n), _lib.current_stream()))
-    rows = [desc.raw[i * stride:(i + 1) * stride].split(b"\0")[0].decode() for i in range(n.value)]
+    rows = plan_ops.plan_rows(m.plan(2, h, w), x.cuda(), torch.tensor([1.0, 2.0], device="cuda"), lq.cuda())
     assert not any(r.startswith("gn ") for r in rows)
     in_convs = [r for r in rows if ".in_layers.1." in r]
     out_convs = [r for r in rows if ".out_layers.1." in r]

@@ -37,7 +37,7 @@ def _attn(qkv, N, T, heads, D, new_order):
 @pytest.mark.parametrize("D", [32, 64, 128])
 def test_unet_attention_vs_fp32(D, heads, T, new_order):
     """Per element against float64 on the fp16 operands (the bound of tests/test_gpu_attention.py)."""
-    from tests.test_gpu_attention import unet_case
+    from tests.attn_ref import unet_case
     unet_case("randn", 3, T, heads, D, new_order, seed=1000 * D + 10 * heads + T % 97)
 
 

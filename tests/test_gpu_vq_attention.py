@@ -16,6 +16,7 @@ import torch.nn.functional as F
 
 from oracle import vq_oracle as vo
 from resshift_b200.vq_arch import random_vq_state_dict, vq_preset
+from tests.gpu_util import fp32_matmuls
 
 TOL_MAX, TOL_MEAN = 1e-2, 2e-3
 
@@ -64,12 +65,8 @@ def test_chunked_oracle_attention_matches_unchunked():
 
 @pytest.fixture
 def fp32_reference():
-    """Exact fp32 matmuls / convolutions for the reference computations; restored afterwards."""
-    old = (torch.backends.cuda.matmul.allow_tf32, torch.backends.cudnn.allow_tf32)
-    torch.backends.cuda.matmul.allow_tf32 = False
-    torch.backends.cudnn.allow_tf32 = False
-    yield
-    torch.backends.cuda.matmul.allow_tf32, torch.backends.cudnn.allow_tf32 = old
+    with fp32_matmuls():
+        yield
 
 
 @pytest.fixture
@@ -120,7 +117,7 @@ OP_CASES = [(c, t) for c in (128, 256, 512) for t in (64, 384, 4096, 16384)] + [
 @pytest.mark.parametrize("C,T", OP_CASES, ids=[f"C{c}-T{t}" for c, t in OP_CASES])
 def test_op_vs_fp32(fp32_reference, C, T):
     """Per element against float64 on the fp16 operands (the bound of tests/test_gpu_attention.py)."""
-    from tests.test_gpu_attention import vq_check
+    from tests.attn_ref import vq_check
     q, k, v = (t.contiguous() for t in _qkv(2, T, C, seed=C + T))
     vq_check("randn", q, k, v, _op(q, k, v))
 
@@ -128,7 +125,7 @@ def test_op_vs_fp32(fp32_reference, C, T):
 @pytest.mark.gpu
 def test_op_strided_rows(fp32_reference):
     """q, k, v as column slices of wider rows (row stride ld > C), as a plan view may be."""
-    from tests.test_gpu_attention import vq_check
+    from tests.attn_ref import vq_check
     q, k, v = _qkv(2, 384, 256, seed=9, ld=384)
     vq_check("randn", q, k, v, _op(q, k, v, ld=384))
 
@@ -150,7 +147,7 @@ def test_op_peaked_softmax_max_in_last_block(fp32_reference):
     print(f"[vq attention] peaked: scores {s.min().item():.1f} .. {s.max().item():.1f}")
     assert (s.argmax(-1) >= T - 16).all() and (s.argmin(-1) < 16).all()
     assert s.max().item() >= 40 and s.min().item() <= -40
-    from tests.test_gpu_attention import vq_check
+    from tests.attn_ref import vq_check
     vq_check("peaked", q, k, v, _op(q, k, v))
 
 

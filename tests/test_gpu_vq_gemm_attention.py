@@ -7,14 +7,14 @@ References run in fp32 with TF32 off.  Operators are compared with fp32 torch on
 oracle on the GPU.  Tolerances are the repository's: max|d| <= 1e-2, mean|d| <= 2e-3 for plans, `_tol` of
 test_gpu_ops.py for the GEMMs, fp16 rounding of the result for the softmax.
 """
-import ctypes as C
-
 import pytest
 import torch
 import torch.nn.functional as F
 
 from oracle import vq_oracle as vo
 from resshift_b200.vq_arch import random_vq_state_dict, vq_preset
+from tests import plan_ops
+from tests.gpu_util import fp32_matmuls
 
 pytestmark = pytest.mark.gpu
 
@@ -23,12 +23,8 @@ TOL_MAX, TOL_MEAN = 1e-2, 2e-3
 
 @pytest.fixture
 def fp32_reference():
-    """Exact fp32 matmuls / convolutions for the reference computations; restored afterwards."""
-    old = (torch.backends.cuda.matmul.allow_tf32, torch.backends.cudnn.allow_tf32)
-    torch.backends.cuda.matmul.allow_tf32 = False
-    torch.backends.cudnn.allow_tf32 = False
-    yield
-    torch.backends.cuda.matmul.allow_tf32, torch.backends.cudnn.allow_tf32 = old
+    with fp32_matmuls():
+        yield
 
 
 def _report(tag, got, ref):
@@ -177,17 +173,6 @@ def _sd_cuda(cfg, seed=0):
     return {n: t.cuda() for n, t in random_vq_state_dict(cfg, seed).items()}
 
 
-def _op_rows(plan):
-    """Descriptions of the ops of a plan (rs_vq_profile_ops re-runs them on the inputs the last call left)."""
-    from resshift_b200 import _lib
-    cap, stride = 1024, 160
-    ms = (C.c_double * cap)()
-    desc = C.create_string_buffer(cap * stride)
-    n = C.c_int32()
-    _lib.check(_lib.lib.rs_vq_profile_ops(plan.handle, ms, desc, stride, cap, C.byref(n), _lib.current_stream()))
-    return [desc.raw[i * stride:(i + 1) * stride].split(b"\0")[0].decode() for i in range(n.value)]
-
-
 def _inputs(batch, h, w, seed):
     g = torch.Generator(device="cuda").manual_seed(seed)
     x = torch.rand(batch, 3, h, w, device="cuda", generator=g) * 2 - 1
@@ -219,7 +204,7 @@ def test_f8_face_512_encode_decode(fp32_reference):
     _check_encode("f8_face encode 512x512 b2 (T=4096 C=512)", m, sd, cfg, x)
     z = torch.randn(2, cfg.embed_dim, 64, 64, device="cuda", generator=g) * 0.6
     _check_decode("f8_face decode 64x64 latent b2 (not quantised)", m, sd, cfg, z)
-    assert _op_rows(m.plan(1, 2, 512, 512)).count("softmax 4096") == 2
+    assert plan_ops.vq_rows(m.plan(1, 2, 512, 512)).count("softmax 4096") == 2
 
 
 def test_f4_256_batch3(fp32_reference):
@@ -266,10 +251,10 @@ def test_f4_both_sides_of_the_8192_threshold(fp32_reference, width, batch, T):
     m = _vq("f4", sd)
     x, g = _inputs(batch, 256, width, seed=T)
     _check_encode(f"f4 encode 256x{width} b{batch} (T={T})", m, sd, cfg, x)
-    enc_rows = _op_rows(m.plan(0, batch, 256, width))
+    enc_rows = plan_ops.vq_rows(m.plan(0, batch, 256, width))
     z = torch.randn(batch, cfg.embed_dim, 64, width // 4, device="cuda", generator=g) * 0.6
     _check_decode(f"f4 decode 64x{width // 4} latent b{batch} (not quantised)", m, sd, cfg, z)
-    dec_rows = _op_rows(m.plan(1, batch, 256, width))
+    dec_rows = plan_ops.vq_rows(m.plan(1, batch, 256, width))
     for rows in (enc_rows, dec_rows):
         softmax = [r for r in rows if r.startswith("softmax")]
         fused = [r for r in rows if r.startswith("vq_attn")]

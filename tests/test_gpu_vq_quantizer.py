@@ -11,6 +11,7 @@ import torch
 
 from oracle import vq_oracle as vo
 from resshift_b200.vq_arch import random_vq_state_dict, vq_preset
+from tests.gpu_util import fp32_matmuls
 
 pytestmark = pytest.mark.gpu
 
@@ -19,12 +20,8 @@ TOL_MAX, TOL_MEAN = 1e-2, 2e-3
 
 @pytest.fixture
 def fp32_reference():
-    """Exact fp32 matmuls / convolutions for the reference computations; restored afterwards."""
-    old = (torch.backends.cuda.matmul.allow_tf32, torch.backends.cudnn.allow_tf32)
-    torch.backends.cuda.matmul.allow_tf32 = False
-    torch.backends.cudnn.allow_tf32 = False
-    yield
-    torch.backends.cuda.matmul.allow_tf32, torch.backends.cudnn.allow_tf32 = old
+    with fp32_matmuls():
+        yield
 
 
 def _report(tag, got, ref):

@@ -30,6 +30,7 @@ from oracle import kl_oracle as ko
 from oracle import vq_oracle as vo
 from oracle import vq_options_oracle as voo
 from resshift_b200.vq_arch import VQConfig, kl_preset, random_kl_state_dict, random_vq_state_dict, wide_vq_preset
+from tests.gpu_util import fp32_matmuls
 
 pytestmark = pytest.mark.gpu
 
@@ -43,11 +44,8 @@ MAX_ABS, MEAN_ABS = 1e-2, 2e-3
 
 @pytest.fixture(scope="module")
 def fp32_reference():
-    old = (torch.backends.cuda.matmul.allow_tf32, torch.backends.cudnn.allow_tf32)
-    torch.backends.cuda.matmul.allow_tf32 = False
-    torch.backends.cudnn.allow_tf32 = False
-    yield
-    torch.backends.cuda.matmul.allow_tf32, torch.backends.cudnn.allow_tf32 = old
+    with fp32_matmuls():
+        yield
 
 
 def _check(tag, got, ref, bound):
