@@ -239,7 +239,13 @@ int rs_sampler_set_taps(rs_sampler* s, float* pred_xstart_steps, float* sample_s
  * fp32 (_extract_into_tensor) and keeps the log variance of options->var_type.  rs_sampler_run / _run_host / _set_taps /
  * _destroy work unchanged; z_y is not read and may be NULL.  rs_sampler_tables refuses these samplers. */
 typedef enum rs_ddpm_kind { RS_DDPM_ANCESTRAL = 0, RS_DDPM_DDIM = 1 } rs_ddpm_kind;
-typedef enum rs_ddpm_var_type { RS_VAR_FIXED_LARGE = 0, RS_VAR_FIXED_SMALL = 1 } rs_ddpm_var_type;
+/* The learned types (learn_sigma=True, reference models/script_util.py:87-88) take the log variance from the model's
+ * second C output channels: LEARNED log_var = v; LEARNED_RANGE log_var = frac log(betas)[t] + (1 - frac)
+ * posterior_log_variance_clipped[t] with frac = (v + 1) / 2 (models/gaussian_diffusion.py:772-786).  Value 2 is left
+ * unassigned: it was refused as unknown before the learned types existed, and stays so. */
+typedef enum rs_ddpm_var_type {
+  RS_VAR_FIXED_LARGE = 0, RS_VAR_FIXED_SMALL = 1, RS_VAR_LEARNED_RANGE = 3, RS_VAR_LEARNED = 4
+} rs_ddpm_var_type;
 typedef enum rs_ddpm_table_row {
   RS_DDPM_SQRT_RECIP_ACP = 0,       /* sqrt(1 / alphas_cumprod)                                               */
   RS_DDPM_SQRT_RECIPM1_ACP = 1,     /* sqrt(1 / alphas_cumprod - 1)                                           */
@@ -250,18 +256,24 @@ typedef enum rs_ddpm_table_row {
   RS_DDPM_ACP = 6,                  /* alphas_cumprod                                                         */
   RS_DDPM_ACP_PREV = 7,             /* alphas_cumprod_prev                                                    */
   RS_DDPM_TABLE_ROWS = 8,
-  RS_DDPM_ACP_NEXT = 8              /* alphas_cumprod_next (0 at T - 1): read by rs_ddim_reverse_sampler_create only */
+  RS_DDPM_ACP_NEXT = 8,             /* alphas_cumprod_next (0 at T - 1): read by rs_ddim_reverse_sampler_create only */
+  RS_DDPM_LOG_BETAS = 8             /* log(betas): LEARNED_RANGE's max_log, read by rs_ddpm_sampler_create with that
+                                       var_type only (its min_log is RS_DDPM_LOGVAR_SMALL)                         */
 } rs_ddpm_table_row;
 typedef struct rs_ddpm_options {
   int32_t kind;               /* RS_DDPM_ANCESTRAL or RS_DDPM_DDIM                                         */
   int32_t mean_type;          /* RS_MEAN_EPSILON or RS_MEAN_XSTART                                         */
-  int32_t var_type;           /* RS_VAR_FIXED_LARGE / _SMALL: the ancestral step's noise; DDIM ignores it */
+  int32_t var_type;           /* rs_ddpm_var_type: the ancestral step's noise; DDIM ignores it but for the
+                                 model output's width                                                      */
   int32_t clip;               /* 1: clamp x0 to [-1, 1] (clip_denoised)                                    */
   double eta;                 /* DDIM's eta >= 0 (the ancestral step ignores it)                           */
 } rs_ddpm_options;
-/* tables_host [RS_DDPM_TABLE_ROWS][steps] float64; timestep_map_host [steps] (the model's timesteps; NULL = 0 .. T-1).
- * Refused, each with its reason: NULL tables or options, an unknown kind / var_type, a mean type other than eps or x0,
- * clip other than 0 / 1, a negative or non-finite eta, steps outside [2, the plan's FiLM rows]. */
+/* tables_host [RS_DDPM_TABLE_ROWS][steps] float64 ([RS_DDPM_TABLE_ROWS + 1][steps], the last row RS_DDPM_LOG_BETAS,
+ * with RS_VAR_LEARNED_RANGE); timestep_map_host [steps] (the model's timesteps; NULL = 0 .. T-1).  A fixed var_type
+ * needs a plan whose model outputs as many channels as x has, a learned one twice as many (the mean half, then the
+ * variance half).  Refused, each with its reason: NULL tables or options, an unknown kind / var_type, a mean type other
+ * than eps or x0, clip other than 0 / 1, a negative or non-finite eta, steps outside [2, the plan's FiLM rows], a model
+ * output width that does not match var_type. */
 int rs_ddpm_sampler_create(rs_plan* p, int steps, const double* tables_host, const int32_t* timestep_map_host,
                            const rs_ddpm_options* options, rs_sampler** out);
 
@@ -276,8 +288,9 @@ typedef struct rs_ddim_reverse_options {
   int32_t clip;               /* 1: clamp x0 to [-1, 1] (clip_denoised)                                    */
 } rs_ddim_reverse_options;
 /* tables_host [RS_DDPM_TABLE_ROWS + 1][steps] float64: the rows of rs_ddpm_sampler_create, then RS_DDPM_ACP_NEXT;
- * timestep_map_host as there.  Refused, each with its reason: NULL tables or options, a mean type other than eps or
- * x0, clip other than 0 / 1, steps outside [2, the plan's FiLM rows]. */
+ * timestep_map_host as there.  The plan's model may output C or 2C channels (a learned variance): the step reads the
+ * first C only.  Refused, each with its reason: NULL tables or options, a mean type other than eps or x0, clip other
+ * than 0 / 1, steps outside [2, the plan's FiLM rows], any other model output width. */
 int rs_ddim_reverse_sampler_create(rs_plan* p, int steps, const double* tables_host, const int32_t* timestep_map_host,
                                    const rs_ddim_reverse_options* options, rs_sampler** out);
 
@@ -410,7 +423,13 @@ int rs_op_p_sample_pred(const rs_p_sample_pred_args* a, void* stream);
  * the ancestral step reads coef1, coef2 and log_var, DDIM acp and acp_prev, eps prediction (and DDIM) sqrt_recip_acp
  * and sqrt_recipm1_acp.  next_in (t > 0 only) receives fp16(x_next) in channels [0, C); counters as in
  * rs_op_p_sample_ex; x0_out (optional) receives x0.  Refused: a table the step reads missing, an unknown kind or mean
- * type, clip other than 0 / 1, a negative eta, t outside [0, T), next_cpad < C, more counters than launched threads. */
+ * type, clip other than 0 / 1, a negative eta, t outside [0, T), next_cpad < C, more counters than launched threads.
+ * The trailing fields describe a learned-variance output; zero / NULL is a [N, C, HW] output with log_var's variance.
+ * out_sN (> 0) is out's image stride in elements: C * HW, or at least 2C * HW for a learned var_type, whose variance
+ * half starts C * HW after the mean half.  var_type (ancestral only; DDIM reads the stride alone) is an
+ * rs_ddpm_var_type: 0 / 1 read log_var, RS_VAR_LEARNED the variance half, RS_VAR_LEARNED_RANGE the variance half with
+ * log_var as min_log and log_betas as max_log.  Refused as well: an unknown var_type, a learned one with a stride below
+ * 2C * HW or a missing table, a fixed ancestral step at a stride other than C * HW, a DDIM stride below C * HW. */
 typedef struct rs_ddpm_step_args {
   const float* out; const float* x_t; const float* noise; float* x_next;                     /* [N, C, HW] fp32       */
   const float* sqrt_recip_acp; const float* sqrt_recipm1_acp;                                /* [T] fp32 device tables */
@@ -421,6 +440,9 @@ typedef struct rs_ddpm_step_args {
   void* next_in; int32_t next_cpad;
   uint32_t* counters; int32_t n_counters;
   float* x0_out;
+  int64_t out_sN;               /* 0: C * HW                                                                     */
+  int32_t var_type;             /* rs_ddpm_var_type; 0 (FIXED_LARGE) and 1 both read log_var                      */
+  const float* log_betas;       /* [T] fp32 device table: RS_VAR_LEARNED_RANGE only                              */
 } rs_ddpm_step_args;
 int rs_op_ddpm_step(const rs_ddpm_step_args* a, void* stream);
 /* The DDIM inversion step (rs_ddim_reverse_sampler_create) on its own, with the grid the loop launches: x0 from the
@@ -428,7 +450,8 @@ int rs_op_ddpm_step(const rs_ddpm_step_args* a, void* stream);
  * x_next = x0 sqrt(acp_next[t]) + sqrt(1 - acp_next[t]) eps'.  Tables are [T] fp32 device arrays.  next_in (t < T - 1
  * only) receives fp16(x_next) in channels [0, C); counters as in rs_op_p_sample_ex; x0_out (optional) receives x0.
  * Refused: a NULL table, an unknown mean type, clip other than 0 / 1, t outside [0, T), next_cpad < C, more counters
- * than launched threads. */
+ * than launched threads.  out_sN (trailing; 0 = C * HW) is out's image stride in elements, at least C * HW: a
+ * learned-variance model's [N, 2C, HW] output is read at 2C * HW, its variance half never. */
 typedef struct rs_ddim_reverse_step_args {
   const float* out; const float* x_t; float* x_next;                                          /* [N, C, HW] fp32       */
   const float* sqrt_recip_acp; const float* sqrt_recipm1_acp; const float* acp_next;          /* [T] fp32 device tables */
@@ -437,6 +460,7 @@ typedef struct rs_ddim_reverse_step_args {
   void* next_in; int32_t next_cpad;
   uint32_t* counters; int32_t n_counters;
   float* x0_out;
+  int64_t out_sN;
 } rs_ddim_reverse_step_args;
 int rs_op_ddim_reverse_step(const rs_ddim_reverse_step_args* a, void* stream);
 /* The denoiser's input packing: out[N*HW][Cpad] fp16 = cat([fp16(x * scale_tab[scale_idx]), lq, mask], channels) + zero

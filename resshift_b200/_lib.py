@@ -144,7 +144,7 @@ class DdpmStepArgsC(C.Structure):
         ("T", C.c_int32), ("t", C.c_int32), ("N", C.c_int32), ("C", C.c_int32), ("HW", C.c_int32),
         ("kind", C.c_int32), ("mean_type", C.c_int32), ("clip", C.c_int32), ("eta", C.c_float),
         ("next_in", C.c_void_p), ("next_cpad", C.c_int32), ("counters", C.c_void_p), ("n_counters", C.c_int32),
-        ("x0_out", C.c_void_p),
+        ("x0_out", C.c_void_p), ("out_sN", C.c_int64), ("var_type", C.c_int32), ("log_betas", C.c_void_p),
     ]
 
 
@@ -161,18 +161,20 @@ class DdimReverseStepArgsC(C.Structure):
         ("T", C.c_int32), ("t", C.c_int32), ("N", C.c_int32), ("C", C.c_int32), ("HW", C.c_int32),
         ("mean_type", C.c_int32), ("clip", C.c_int32),
         ("next_in", C.c_void_p), ("next_cpad", C.c_int32), ("counters", C.c_void_p), ("n_counters", C.c_int32),
-        ("x0_out", C.c_void_p),
+        ("x0_out", C.c_void_p), ("out_sN", C.c_int64),
     ]
 
 
 # rs_ddpm_kind, rs_ddpm_var_type, and the rows of rs_ddpm_sampler_create's float64 tables (rs_ddpm_table_row)
 DDPM_KINDS = {"ancestral": 0, "ddim": 1}
-DDPM_VAR_TYPES = {"fixed_large": 0, "fixed_small": 1}
+DDPM_VAR_TYPES = {"fixed_large": 0, "fixed_small": 1, "learned_range": 3, "learned": 4}     # 2 is unassigned
 DDPM_TABLE_ROWS = ("sqrt_recip_alphas_cumprod", "sqrt_recipm1_alphas_cumprod", "posterior_mean_coef1",
                    "posterior_mean_coef2", "log_variance_fixed_large", "posterior_log_variance_clipped",
                    "alphas_cumprod", "alphas_cumprod_prev")
 # rs_ddim_reverse_sampler_create's rows: the same, then RS_DDPM_ACP_NEXT
 DDIM_REVERSE_TABLE_ROWS = DDPM_TABLE_ROWS + ("alphas_cumprod_next",)
+# rs_ddpm_sampler_create's rows with RS_VAR_LEARNED_RANGE: the same, then RS_DDPM_LOG_BETAS (its max_log)
+DDPM_LEARNED_RANGE_TABLE_ROWS = DDPM_TABLE_ROWS + ("log_betas",)
 
 # rs_mean_type, by the reference's predict_type names (models/script_util.py:35-44)
 MEAN_TYPES = {"xstart": 0, "epsilon": 1, "epsilon_scale": 2, "residual": 3}

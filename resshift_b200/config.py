@@ -13,6 +13,16 @@ from dataclasses import dataclass, field, asdict
 from typing import Optional, Sequence, Tuple
 
 
+def _x_channels(in_channels: int, out_channels: int) -> Optional[int]:
+    """Channels of x in a UNetModel / UNetModelConv, whose input is x and lq (3 channels at the latent size, or 12 at
+    twice it through pixel_unshuffle) concatenated: out_channels, else out_channels / 2 (a learned-variance head outputs
+    the mean, then as many variance values).  None when neither reading fits."""
+    for x in (out_channels, out_channels // 2 if out_channels % 2 == 0 else None):
+        if x is not None and x > 0 and in_channels - x in (3, 12):
+            return x
+    return None
+
+
 @dataclass
 class UNetConfig:
     image_size: int = 64
@@ -89,6 +99,11 @@ class UNetConfig:
             return self.lq_in_channels
         return 16 * (2 ** self.fe_stages)
 
+    @property
+    def x_channels(self) -> int:
+        """Channels of x (the latent): in_channels; lq enters through its own path"""
+        return self.in_channels
+
     def to_kwargs(self) -> dict:
         d = asdict(self)
         d["num_res_blocks"] = list(self.num_res_blocks)
@@ -135,10 +150,12 @@ class UNetModelConfig:
                              "labels, so the reference's own `y is not None` assert would fire)")
         if not self.cond_lq:
             raise ValueError("cond_lq=False: the ResShift sampler always passes lq, and the reference asserts cond_lq then")
-        if self.in_channels - self.out_channels not in (3, 12):
+        if _x_channels(self.in_channels, self.out_channels) is None:
             raise ValueError(f"in_channels={self.in_channels}, out_channels={self.out_channels}: x has out_channels "
                              f"channels and lq is a 3-channel image, so in_channels must be out_channels + 3 (lq at the "
-                             f"latent size) or out_channels + 12 (lq at twice it, through pixel_unshuffle)")
+                             f"latent size) or out_channels + 12 (lq at twice it, through pixel_unshuffle); with a "
+                             f"learned variance (even out_channels) x has out_channels / 2 channels, and in_channels "
+                             f"is out_channels / 2 + 3 or + 12")
         if self.model_channels % 32:
             raise ValueError(f"model_channels={self.model_channels}: GroupNorm32 needs channel counts divisible by 32")
         for ch, output_block in self.attention_layers():
@@ -165,7 +182,13 @@ class UNetModelConfig:
     @property
     def lq_factor(self) -> int:
         """1: lq enters at the latent size; 2: at twice it, through F.pixel_unshuffle(lq, 2) (reference :569-573)."""
-        return 2 if self.in_channels - self.out_channels == 12 else 1
+        return 2 if self.in_channels - self.x_channels == 12 else 1
+
+    @property
+    def x_channels(self) -> int:
+        """Channels of x (the latent): out_channels, or out_channels / 2 when the model also outputs a learned variance
+        (learn_sigma).  Where both readings fit (e.g. in 21, out 18) the fixed-variance one wins."""
+        return _x_channels(self.in_channels, self.out_channels)
 
     @property
     def time_embed_dim(self) -> int:
@@ -209,10 +232,12 @@ class UNetModelConvConfig:
             raise ValueError(f"dims={self.dims}: only 2-D UNets are covered (every ResShift config uses dims=2)")
         if not self.cond_lq:
             raise ValueError("cond_lq=False: the ResShift sampler always passes lq, and the reference asserts cond_lq then")
-        if self.in_channels - self.out_channels not in (3, 12):
+        if _x_channels(self.in_channels, self.out_channels) is None:
             raise ValueError(f"in_channels={self.in_channels}, out_channels={self.out_channels}: x has out_channels "
                              f"channels and lq is a 3-channel image, so in_channels must be out_channels + 3 (lq at the "
-                             f"latent size) or out_channels + 12 (lq at twice it, through pixel_unshuffle)")
+                             f"latent size) or out_channels + 12 (lq at twice it, through pixel_unshuffle); with a "
+                             f"learned variance (even out_channels) x has out_channels / 2 channels, and in_channels "
+                             f"is out_channels / 2 + 3 or + 12")
         for level, mult in enumerate(self.channel_mult):
             if mult <= 0 or self.model_channels <= 0 or (self.model_channels * mult) % 8:
                 raise ValueError(f"level {level} has {self.model_channels * mult} channels: the conv kernels read and "
@@ -222,7 +247,13 @@ class UNetModelConvConfig:
     @property
     def lq_factor(self) -> int:
         """1: lq enters at the latent size; 2: at twice it, through F.pixel_unshuffle(lq, 2) (reference :1166-1167)."""
-        return 2 if self.in_channels - self.out_channels == 12 else 1
+        return 2 if self.in_channels - self.x_channels == 12 else 1
+
+    @property
+    def x_channels(self) -> int:
+        """Channels of x (the latent): out_channels, or out_channels / 2 when the model also outputs a learned variance
+        (learn_sigma).  Where both readings fit (e.g. in 21, out 18) the fixed-variance one wins."""
+        return _x_channels(self.in_channels, self.out_channels)
 
     @property
     def time_embed_dim(self) -> int:

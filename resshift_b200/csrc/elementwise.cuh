@@ -223,19 +223,33 @@ __global__ void linear_small_kernel(const float* __restrict__ x, const __half* _
 //              :1054-1064), t walking 0 .. T-1 upward; acp_next[T-1] is 0, so the last step returns eps'; nothing is drawn
 // Every operation is the reference's fp32 tensor operation on the fp32 table values (_extract_into_tensor), in its
 // order and rounded on its own (no FMA contraction); the [t != 0] factor multiplies as the reference's nonzero_mask does.
+//
+// A learned-variance model (learn_sigma: LEARNED / LEARNED_RANGE, p_mean_variance :772-786) outputs 2C channels: the
+// mean half [0, C) is read as above, at the image stride out_sN, and the ancestral step takes its log variance from the
+// variance half v = out[C + c] instead of the kDdLogVar row:
+//   LEARNED        log_var = v
+//   LEARNED_RANGE  frac = (v + 1) / 2;  log_var = frac * log(betas)[t] + (1 - frac) * posterior_log_variance_clipped[t]
+// DDIM and inversion never read the variance half.  The fixed instances (VAR = kVarFixed) read a [N, C, HW] output at i.
 // ------------------------------------------------------------------------------------------------
 enum MeanType : int { kMeanXstart = 0, kMeanEpsilon = 1, kMeanEpsilonScale = 2, kMeanResidual = 3 };
 enum StepProcess : int { kStepResShift = 0, kStepAncestral = 1, kStepDdim = 2, kStepInversion = 3 };
+// the model output's layout and, for the ancestral step, where its log variance comes from; DDIM and inversion run
+// every 2C-output model as kVarLearned (they read the mean half only)
+enum StepVar : int { kVarFixed = 0, kVarLearned = 1, kVarLearnedRange = 2 };
 
-// The step's [T] fp32 tables, by process: row[r] is the table the plan's table region holds at r * 1024.
+// The step's [T] fp32 tables, by process: row[r] is the table the plan's table region holds at r * 1024.  kDdLogVar
+// holds the fixed log variance, or LEARNED_RANGE's min_log (posterior_log_variance_clipped); kDdLogBetas (its max_log)
+// is read by LEARNED_RANGE only.
 enum ResShiftRow : int { kRsCoef1 = 0, kRsCoef2, kRsStd, kRsInScale, kRsEpsCoef, kRsEta, kRsOneMinusEta, kRsRows };
-enum DdpmRow : int { kDdSqrtRecipAcp = 0, kDdSqrtRecipm1Acp, kDdCoef1, kDdCoef2, kDdLogVar, kDdAcp, kDdAcpPrev, kDdRows };
+enum DdpmRow : int {
+  kDdSqrtRecipAcp = 0, kDdSqrtRecipm1Acp, kDdCoef1, kDdCoef2, kDdLogVar, kDdAcp, kDdAcpPrev, kDdLogBetas, kDdRows
+};
 enum InversionRow : int { kInvSqrtRecipAcp = 0, kInvSqrtRecipm1Acp, kInvAcpNext, kInvRows };
-constexpr int kStepRows = 7;
+constexpr int kStepRows = 8;
 
 struct StepParams {
   const float* x_t;       // [N, C, HW]
-  const float* out;       // [N, C, HW]: the model output
+  const float* out;       // [N, C, HW] (kVarFixed), or [N, >= 2C, HW] at image stride out_sN: the model output
   const float* y;         // [N, C, HW] z_y: read by the ResShift residual and epsilon types
   const float* noise;     // [N, C, HW]: not read by inversion
   float* x_next;          // [N, C, HW]
@@ -247,6 +261,8 @@ struct StepParams {
   int N, C, HW;
   __half* next_in; int next_cpad;     // optional: [N*HW, next_cpad]; channels [0, C) are written here
   unsigned int* zero_ptr; int zero_n; // GroupNorm arrival counters of the NEXT denoiser forward: reset here
+  long long out_sN;       // the model output's image stride in elements: C * HW, or 2C * HW for a learned variance
+  int var_mode;           // StepVar of the ancestral step (launch_step picks the instance by it and out_sN)
 };
 
 template <int MT>
@@ -263,8 +279,10 @@ __device__ __forceinline__ float predict_xstart(const StepParams& p, long long i
   }
 }
 
-template <int PROCESS, int MT>
+template <int PROCESS, int MT, int VAR = kVarFixed>
 __global__ void step_kernel(const StepParams p) {
+  static_assert(VAR == kVarFixed || PROCESS != kStepResShift, "the ResShift process has no learned variance");
+  static_assert(VAR != kVarLearnedRange || PROCESS == kStepAncestral, "only the ancestral step reads the variance half");
   pdl_trigger();
   pdl_wait();
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -273,6 +291,12 @@ __global__ void step_kernel(const StepParams p) {
   if (i >= total) return;
   const int t = p.t;
   const float xt = p.x_t[i];
+  // where element i's mean value sits in the model output: i itself, or the same (c, hw) of image n at stride out_sN
+  long long io = i;
+  if constexpr (VAR != kVarFixed) {
+    const long long img = (long long)p.C * p.HW;
+    io = i + (i / img) * (p.out_sN - img);
+  }
   // x0 (eps prediction) and eps' (DDIM, inversion) factors of the DDPM processes, read once ahead of the x0_out store
   const float sra = p.row[kDdSqrtRecipAcp][t], srm1 = p.row[kDdSqrtRecipm1Acp][t];
   float x0;
@@ -282,8 +306,8 @@ __global__ void step_kernel(const StepParams p) {
   } else {
     static_assert(MT == kMeanEpsilon || MT == kMeanXstart, "DDPM steps predict eps or x0");
     if constexpr (MT == kMeanEpsilon)
-      x0 = __fsub_rn(__fmul_rn(sra, xt), __fmul_rn(srm1, p.out[i]));
-    else x0 = p.out[i];
+      x0 = __fsub_rn(__fmul_rn(sra, xt), __fmul_rn(srm1, p.out[io]));
+    else x0 = p.out[io];
     if (p.clip) x0 = x0 < -1.0f ? -1.0f : (x0 > 1.0f ? 1.0f : x0);     // clamp(-1, 1): NaN stays NaN
   }
   if constexpr (PROCESS != kStepResShift || MT != kMeanXstart) {
@@ -297,7 +321,20 @@ __global__ void step_kernel(const StepParams p) {
   } else if constexpr (PROCESS == kStepAncestral) {
     const float nonzero = t != 0 ? 1.0f : 0.0f;
     const float mean = __fadd_rn(__fmul_rn(p.row[kDdCoef1][t], x0), __fmul_rn(p.row[kDdCoef2][t], xt));
-    const float sd = expf(__fmul_rn(0.5f, p.row[kDdLogVar][t]));
+    float log_var;
+    if constexpr (VAR == kVarFixed) {
+      log_var = p.row[kDdLogVar][t];
+    } else {
+      const float v = p.out[io + (long long)p.C * p.HW];          // the variance half
+      if constexpr (VAR == kVarLearned) {
+        log_var = v;
+      } else {
+        // (v + 1) / 2: halving is exact, so the product by 0.5 is the reference's division bit for bit
+        const float frac = __fmul_rn(__fadd_rn(v, 1.0f), 0.5f);
+        log_var = __fadd_rn(__fmul_rn(frac, p.row[kDdLogBetas][t]), __fmul_rn(__fsub_rn(1.0f, frac), p.row[kDdLogVar][t]));
+      }
+    }
+    const float sd = expf(__fmul_rn(0.5f, log_var));
     v = __fadd_rn(mean, __fmul_rn(__fmul_rn(nonzero, sd), p.noise[i]));
   } else {
     static_assert((int)kDdSqrtRecipAcp == (int)kInvSqrtRecipAcp && (int)kDdSqrtRecipm1Acp == (int)kInvSqrtRecipm1Acp,

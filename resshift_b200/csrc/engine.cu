@@ -69,7 +69,8 @@ struct rs_engine {
   rs_unet_config cfg;
   rs_unet_options opt{1, 0, 1, 0};
   // UNetModel (rs_unetmodel_create): global-attention blocks instead of Swin layers, no feature extractor; cfg then holds
-  // its levels with in_channels = out_channels (the channels of x) and lq_size = image_size
+  // its levels with in_channels = the channels of x (out_channels, or half of it with a learned variance) and
+  // lq_size = image_size
   bool unetmodel = false;
   rs_unetmodel_config um{};
   // UNetModelConv (rs_unetconv_create): a UNetModel-style engine (unetmodel set, no attention levels) whose ResBlocks are
@@ -95,7 +96,7 @@ struct rs_engine {
   }
   int lq_in_ch() const { return cfg.cond_mask ? 4 : 3; }
   int lq_feat_ch() const {
-    if (unetmodel) return um.in_channels - um.out_channels;
+    if (unetmodel) return um.in_channels - cfg.in_channels;     // cfg.in_channels: the channels of x
     return fe_stages() == 0 ? lq_in_ch() : 16 << fe_stages();
   }
   // UNetModel: the LQ image enters at the latent size (1) or at twice it through pixel_unshuffle (2)
@@ -1289,6 +1290,18 @@ int rs_unet_create(const rs_unet_config* cfg, rs_engine** out) {
   const rs_unet_options shipped{1, 0, 1, 0};
   return rs_unet_create_ex(cfg, &shipped, out);
 }
+// The channels of x of a UNetModel / UNetModelConv (x and lq concatenated): out_channels, or with a learned variance
+// (learn_sigma: the model outputs the mean, then as many variance values) out_channels / 2; lq adds 3 channels at the
+// latent size or 12 at twice it.  Where both readings fit (in 21, out 18) the fixed-variance one wins.  0: neither fits.
+static int unet_x_channels(int in, int out) {
+  if (out > 0 && (in - out == 3 || in - out == 12)) return out;
+  if (out > 0 && out % 2 == 0 && (in - out / 2 == 3 || in - out / 2 == 12)) return out / 2;
+  return 0;
+}
+static const char* const kUnetChannelRule =
+    "in_channels must be out_channels + 3 (lq at the latent size) or out_channels + 12 (lq at twice the latent size, "
+    "pixel_unshuffle): x has out_channels channels and lq is a 3-channel image; or, with a learned variance (even "
+    "out_channels), out_channels / 2 + 3 or out_channels / 2 + 12: x has out_channels / 2 channels";
 int rs_unetmodel_create(const rs_unetmodel_config* cfg, const rs_unet_options* opts, rs_engine** out) {
   RS_CHECK(cfg && opts && out, "null argument");
   RS_CHECK(cfg->n_levels >= 1 && cfg->n_levels <= RS_MAX_LEVELS && cfg->n_attn >= 0 && cfg->n_attn <= RS_MAX_LEVELS, "n_levels / n_attn");
@@ -1296,9 +1309,8 @@ int rs_unetmodel_create(const rs_unetmodel_config* cfg, const rs_unet_options* o
   for (int v : {opts->use_scale_shift_norm, opts->resblock_updown, opts->conv_resample})
     RS_CHECK(v == 0 || v == 1, "rs_unet_options fields are 0 or 1");
   RS_CHECK(cfg->use_new_attention_order == 0 || cfg->use_new_attention_order == 1, "use_new_attention_order is 0 or 1");
-  RS_CHECK(cfg->out_channels > 0 && (cfg->in_channels - cfg->out_channels == 3 || cfg->in_channels - cfg->out_channels == 12),
-           "in_channels must be out_channels + 3 (lq at the latent size) or out_channels + 12 (lq at twice the latent size, "
-           "pixel_unshuffle): x has out_channels channels and lq is a 3-channel image");
+  const int x_ch = unet_x_channels(cfg->in_channels, cfg->out_channels);
+  RS_CHECK(x_ch > 0, kUnetChannelRule);
   RS_CHECK(cfg->num_head_channels == -1 || cfg->num_head_channels > 0, "num_head_channels is -1 or positive");
   RS_CHECK(cfg->num_head_channels != -1 || cfg->num_heads > 0, "num_heads must be positive");
   RS_CHECK(cfg->model_channels > 0 && cfg->model_channels % 32 == 0, "GroupNorm32 needs model_channels % 32 == 0");
@@ -1310,7 +1322,7 @@ int rs_unetmodel_create(const rs_unetmodel_config* cfg, const rs_unet_options* o
   e->opt = *opts;
   rs_unet_config& c = e->cfg;
   std::memset(&c, 0, sizeof(c));
-  c.image_size = cfg->image_size; c.in_channels = cfg->out_channels; c.model_channels = cfg->model_channels;
+  c.image_size = cfg->image_size; c.in_channels = x_ch; c.model_channels = cfg->model_channels;
   c.out_channels = cfg->out_channels; c.n_levels = cfg->n_levels; c.n_attn = cfg->n_attn; c.lq_size = cfg->image_size;
   for (int l = 0; l < RS_MAX_LEVELS; ++l) {
     c.channel_mult[l] = cfg->channel_mult[l]; c.num_res_blocks[l] = cfg->num_res_blocks[l];
@@ -1338,9 +1350,8 @@ int rs_unetconv_create(const rs_unetconv_config* cfg, const rs_unet_options* opt
     RS_CHECK(v == 0 || v == 1, "rs_unet_options fields are 0 or 1");
   RS_CHECK(cfg->dims == 2, "dims=" + std::to_string(cfg->dims) + ": only 2-D UNets are covered (set dims=2)");
   RS_CHECK(cfg->cond_lq == 1, "cond_lq must be 1: the ResShift sampler always passes lq, and the reference asserts cond_lq then");
-  RS_CHECK(cfg->out_channels > 0 && (cfg->in_channels - cfg->out_channels == 3 || cfg->in_channels - cfg->out_channels == 12),
-           "in_channels must be out_channels + 3 (lq at the latent size) or out_channels + 12 (lq at twice the latent size, "
-           "pixel_unshuffle): x has out_channels channels and lq is a 3-channel image");
+  const int x_ch = unet_x_channels(cfg->in_channels, cfg->out_channels);
+  RS_CHECK(x_ch > 0, kUnetChannelRule);
   RS_CHECK(cfg->model_channels > 0, "model_channels must be positive");
   for (int l = 0; l < cfg->n_levels; ++l) {
     RS_CHECK(cfg->channel_mult[l] > 0 && cfg->num_res_blocks[l] >= 0, "channel_mult / num_res_blocks");
@@ -1359,7 +1370,7 @@ int rs_unetconv_create(const rs_unetconv_config* cfg, const rs_unet_options* opt
   rs_unet_config& c = e->cfg;
   std::memset(&c, 0, sizeof(c));
   c.image_size = 64; c.lq_size = 64;            // (no image_size: unused without attention levels and feature extractor)
-  c.in_channels = cfg->out_channels; c.model_channels = cfg->model_channels; c.out_channels = cfg->out_channels;
+  c.in_channels = x_ch; c.model_channels = cfg->model_channels; c.out_channels = cfg->out_channels;
   c.n_levels = cfg->n_levels; c.n_attn = 0;
   for (int l = 0; l < RS_MAX_LEVELS; ++l) {
     c.channel_mult[l] = u.channel_mult[l] = cfg->channel_mult[l];
@@ -1681,6 +1692,7 @@ struct rs_sampler {
   int clip = 0;                 // DDPM processes: clamp x0 to [-1, 1]
   float eta = 0;                // DDIM
   float prior_coef = 0;         // ResShift: kappa * sqrt_eta[T - 1]
+  int var_mode = 0;             // StepVar of the ancestral step (kVarFixed for every other process)
   // rows x T fp32: row r is what the plan's table region holds at r * 1024 (the process's row enum)
   int rows = 0;
   std::vector<float> tab;
@@ -1706,8 +1718,10 @@ size_t noise_count(const rs_sampler& s) { return s.process == kStepInversion ? 0
 // whether the step at t has a next step (whose denoiser input it packs): t walks down to 0, or up to T - 1 in inversion
 bool step_has_next(int process, int t, int T) { return process == kStepInversion ? t + 1 < T : t > 0; }
 
-// the step_kernel instance of (process, mean type), with the grid every caller launches; combinations without an
-// instance are refused.  The ResShift xstart instance writes no x0: x0_out receives a copy of the model output, ahead.
+// the step_kernel instance of (process, mean type, output layout), with the grid every caller launches; combinations
+// without an instance are refused.  A packed output (out_sN = C * HW) runs the fixed instances; the ancestral step's
+// learned modes, and DDIM / inversion on a wider stride, run the strided ones.  The ResShift xstart instance writes no
+// x0: x0_out receives a copy of the model output, ahead.
 int launch_step(int process, int mean_type, const StepParams& sp, cudaStream_t st) {
   const long long numel = (long long)sp.N * sp.C * sp.HW;
   const dim3 grid((unsigned)((numel + 255) / 256)), block(256);
@@ -1717,6 +1731,10 @@ int launch_step(int process, int mean_type, const StepParams& sp, cudaStream_t s
     return 0;
   };
   const bool eps = mean_type == RS_MEAN_EPSILON, x0 = mean_type == RS_MEAN_XSTART;
+  const bool packed = sp.out_sN == (long long)sp.C * sp.HW, learned = sp.var_mode != kVarFixed;
+  RS_CHECK(sp.out_sN >= (long long)sp.C * sp.HW * (learned ? 2 : 1) && (process == kStepAncestral || !learned) &&
+           (packed || learned || process == kStepDdim || process == kStepInversion),
+           "step: no layout for var mode " + std::to_string(sp.var_mode) + " at image stride " + std::to_string(sp.out_sN));
   switch (process) {
     case kStepResShift:
       if (x0 && sp.x0_out) RS_CUDA_OK(cudaMemcpyAsync(sp.x0_out, sp.out, (size_t)numel * 4, cudaMemcpyDeviceToDevice, st));
@@ -1726,16 +1744,24 @@ int launch_step(int process, int mean_type, const StepParams& sp, cudaStream_t s
       if (mean_type == RS_MEAN_RESIDUAL) return go(step_kernel<kStepResShift, kMeanResidual>);
       break;
     case kStepAncestral:
-      if (eps) return go(step_kernel<kStepAncestral, kMeanEpsilon>);
-      if (x0) return go(step_kernel<kStepAncestral, kMeanXstart>);
+      if (sp.var_mode == kVarLearned) {
+        if (eps) return go(step_kernel<kStepAncestral, kMeanEpsilon, kVarLearned>);
+        if (x0) return go(step_kernel<kStepAncestral, kMeanXstart, kVarLearned>);
+      } else if (sp.var_mode == kVarLearnedRange) {
+        if (eps) return go(step_kernel<kStepAncestral, kMeanEpsilon, kVarLearnedRange>);
+        if (x0) return go(step_kernel<kStepAncestral, kMeanXstart, kVarLearnedRange>);
+      } else {
+        if (eps) return go(step_kernel<kStepAncestral, kMeanEpsilon>);
+        if (x0) return go(step_kernel<kStepAncestral, kMeanXstart>);
+      }
       break;
     case kStepDdim:
-      if (eps) return go(step_kernel<kStepDdim, kMeanEpsilon>);
-      if (x0) return go(step_kernel<kStepDdim, kMeanXstart>);
+      if (eps) return go(packed ? step_kernel<kStepDdim, kMeanEpsilon> : step_kernel<kStepDdim, kMeanEpsilon, kVarLearned>);
+      if (x0) return go(packed ? step_kernel<kStepDdim, kMeanXstart> : step_kernel<kStepDdim, kMeanXstart, kVarLearned>);
       break;
     case kStepInversion:
-      if (eps) return go(step_kernel<kStepInversion, kMeanEpsilon>);
-      if (x0) return go(step_kernel<kStepInversion, kMeanXstart>);
+      if (eps) return go(packed ? step_kernel<kStepInversion, kMeanEpsilon> : step_kernel<kStepInversion, kMeanEpsilon, kVarLearned>);
+      if (x0) return go(packed ? step_kernel<kStepInversion, kMeanXstart> : step_kernel<kStepInversion, kMeanXstart, kVarLearned>);
       break;
   }
   return ::rs::fail(-1, "no step kernel for process " + std::to_string(process) + " and mean type " + std::to_string(mean_type));
@@ -1748,7 +1774,9 @@ int sampler_enqueue(rs_sampler& S, const float* z_y, const float* noises, const 
                     float* out_latent, cudaStream_t st) {
   rs_plan& P = *S.p;
   const rs_unet_config& c = P.e->cfg;
-  RS_CHECK(c.in_channels == c.out_channels, "the sampler needs out_channels == in_channels (x0 and x_t share a shape)");
+  // the DDPM processes' output width was checked against the variance type when the sampler was made
+  RS_CHECK(S.process != kStepResShift || c.in_channels == c.out_channels,
+           "the sampler needs out_channels == in_channels (x0 and x_t share a shape)");
   const long long numel = (long long)P.B * c.in_channels * P.H * P.W;
   float* state = reinterpret_cast<float*>(P.ws + P.off_state);
   const float* tab = reinterpret_cast<const float*>(P.ws + P.off_tables);
@@ -1766,6 +1794,7 @@ int sampler_enqueue(rs_sampler& S, const float* z_y, const float* noises, const 
   for (int r = 0; r < S.rows; ++r) sp.row[r] = tab + r * 1024;
   sp.eta = S.eta; sp.clip = S.clip;
   sp.N = P.B; sp.C = c.in_channels; sp.HW = P.H * P.W;
+  sp.out_sN = (long long)c.out_channels * sp.HW; sp.var_mode = S.var_mode;
   sp.next_cpad = P.cin_pad;
   sp.zero_ptr = reinterpret_cast<unsigned int*>(P.ws + P.off_counters); sp.zero_n = P.n_gn * P.B;
   for (int k = 0; k < S.T; ++k) {
@@ -1902,19 +1931,34 @@ int rs_ddpm_sampler_create(rs_plan* p, int steps, const double* tables, const in
   RS_CHECK(o->mean_type == RS_MEAN_EPSILON || o->mean_type == RS_MEAN_XSTART,
            "DDPM sampler: the model must predict eps or x0 (RS_MEAN_EPSILON or RS_MEAN_XSTART), got mean type " +
            std::to_string(o->mean_type));
-  RS_CHECK(o->var_type == RS_VAR_FIXED_LARGE || o->var_type == RS_VAR_FIXED_SMALL,
-           "DDPM sampler: unknown variance type " + std::to_string(o->var_type) + " (RS_VAR_FIXED_LARGE or RS_VAR_FIXED_SMALL)");
+  const bool learned = o->var_type == RS_VAR_LEARNED || o->var_type == RS_VAR_LEARNED_RANGE;
+  RS_CHECK(o->var_type == RS_VAR_FIXED_LARGE || o->var_type == RS_VAR_FIXED_SMALL || learned,
+           "DDPM sampler: unknown variance type " + std::to_string(o->var_type) +
+           " (RS_VAR_FIXED_LARGE, RS_VAR_FIXED_SMALL, RS_VAR_LEARNED_RANGE or RS_VAR_LEARNED)");
   RS_CHECK(o->clip == 0 || o->clip == 1, "DDPM sampler: clip must be 0 or 1, got " + std::to_string(o->clip));
   RS_CHECK(std::isfinite(o->eta) && o->eta >= 0.0, "DDPM sampler: eta must be finite and >= 0, got " + std::to_string(o->eta));
+  // the model output: the mean (C channels, as x), then with a learned variance the variance values (C more)
+  const rs_unet_config& c = p->e->cfg;
+  RS_CHECK(c.out_channels == c.in_channels * (learned ? 2 : 1),
+           std::string("DDPM sampler: ") + (learned ? "a learned" : "a fixed") + " variance type (" +
+           std::to_string(o->var_type) + ") needs a model with " + std::to_string(c.in_channels * (learned ? 2 : 1)) +
+           " output channels (" + (learned ? "twice" : "as many as") + " the " + std::to_string(c.in_channels) +
+           " channels of x), this plan's model has " + std::to_string(c.out_channels));
   std::unique_ptr<rs_sampler> s;
   static_assert(kDdSqrtRecipAcp == 0 && kDdSqrtRecipm1Acp == 1 && kDdCoef1 == 2 && kDdCoef2 == 3 && kDdLogVar == 4 &&
-                kDdAcp == 5 && kDdAcpPrev == 6, "the rows below are in DdpmRow order");
-  int rc = sampler_new(p, o->kind == RS_DDPM_DDIM ? kStepDdim : kStepAncestral, steps, tmap, "DDPM sampler", tables,
-                       {RS_DDPM_SQRT_RECIP_ACP, RS_DDPM_SQRT_RECIPM1_ACP, RS_DDPM_COEF1, RS_DDPM_COEF2,
-                        o->var_type == RS_VAR_FIXED_LARGE ? RS_DDPM_LOGVAR_LARGE : RS_DDPM_LOGVAR_SMALL, RS_DDPM_ACP,
-                        RS_DDPM_ACP_PREV}, s);
+                kDdAcp == 5 && kDdAcpPrev == 6 && kDdLogBetas == 7, "the rows below are in DdpmRow order");
+  const int logvar_row = o->var_type == RS_VAR_FIXED_LARGE ? RS_DDPM_LOGVAR_LARGE : RS_DDPM_LOGVAR_SMALL;
+  const int process = o->kind == RS_DDPM_DDIM ? kStepDdim : kStepAncestral;
+  int rc = o->var_type == RS_VAR_LEARNED_RANGE
+               ? sampler_new(p, process, steps, tmap, "DDPM sampler", tables,
+                             {RS_DDPM_SQRT_RECIP_ACP, RS_DDPM_SQRT_RECIPM1_ACP, RS_DDPM_COEF1, RS_DDPM_COEF2, logvar_row,
+                              RS_DDPM_ACP, RS_DDPM_ACP_PREV, RS_DDPM_LOG_BETAS}, s)
+               : sampler_new(p, process, steps, tmap, "DDPM sampler", tables,
+                             {RS_DDPM_SQRT_RECIP_ACP, RS_DDPM_SQRT_RECIPM1_ACP, RS_DDPM_COEF1, RS_DDPM_COEF2, logvar_row,
+                              RS_DDPM_ACP, RS_DDPM_ACP_PREV}, s);
   if (rc) return rc;
   s->mean_type = o->mean_type; s->clip = o->clip; s->eta = (float)o->eta;
+  if (process == kStepAncestral && learned) s->var_mode = o->var_type == RS_VAR_LEARNED ? kVarLearned : kVarLearnedRange;
   *out = s.release();
   return 0;
 }
@@ -1929,6 +1973,10 @@ int rs_ddim_reverse_sampler_create(rs_plan* p, int steps, const double* tables, 
            "DDIM reverse sampler: the model must predict eps or x0 (RS_MEAN_EPSILON or RS_MEAN_XSTART), got mean type " +
            std::to_string(o->mean_type));
   RS_CHECK(o->clip == 0 || o->clip == 1, "DDIM reverse sampler: clip must be 0 or 1, got " + std::to_string(o->clip));
+  const rs_unet_config& c = p->e->cfg;
+  RS_CHECK(c.out_channels == c.in_channels || c.out_channels == 2 * c.in_channels,
+           "DDIM reverse sampler: the model must output as many channels as x has (" + std::to_string(c.in_channels) +
+           ") or twice as many (a learned variance), this plan's model has " + std::to_string(c.out_channels));
   std::unique_ptr<rs_sampler> s;
   static_assert(kInvSqrtRecipAcp == 0 && kInvSqrtRecipm1Acp == 1 && kInvAcpNext == 2, "the rows below are in InversionRow order");
   int rc = sampler_new(p, kStepInversion, steps, tmap, "DDIM reverse sampler", tables,

@@ -325,7 +325,7 @@ class ResShiftDiffusion:
         cfg = model.cfg
         B, Cc, H, W = z_y.shape
         plain_lq = isinstance(model, (UNetModel, UNetModelConv))     # x + lq concatenated, no feature extractor or mask
-        latent_ch = cfg.out_channels if plain_lq else cfg.in_channels
+        latent_ch = model.x_channels
         if Cc != latent_ch:
             raise ValueError(f"latent has {Cc} channels, the model expects {latent_ch}")
         exp_lq = model.lq_shape(B, H, W)
@@ -476,6 +476,8 @@ class SpacedDiffusionDDPM:
         # FIXED_LARGE's variance (p_mean_variance :791-794)
         self.variance_fixed_large = np.append(self.posterior_variance[1], self.betas[1:])
         self.log_variance_fixed_large = np.log(self.variance_fixed_large)
+        # LEARNED_RANGE's max_log (p_mean_variance :781)
+        self.log_betas = np.log(self.betas)
 
     # ------------------------------------------------------------------ small pieces (torch)
     def _scale_input(self, inputs, t):
@@ -535,7 +537,7 @@ class SpacedDiffusionDDPM:
                 model_variance = torch.exp(model_log_variance)
             else:
                 min_log = _tab(self.posterior_log_variance_clipped, t, x)
-                max_log = _tab(np.log(self.betas), t, x)
+                max_log = _tab(self.log_betas, t, x)
                 frac = (model_var_values + 1) / 2               # [-1, 1] -> [min_var, max_var]
                 model_log_variance = frac * max_log + (1 - frac) * min_log
                 model_variance = torch.exp(model_log_variance)
@@ -623,19 +625,31 @@ class SpacedDiffusionDDPM:
         return out
 
     _NATIVE_MEAN_TYPES = {ModelMeanType.EPSILON: 1, ModelMeanType.START_X: 0}        # rs_mean_type
-    _NATIVE_VAR_TYPES = {ModelVarTypeDDPM.FIXED_LARGE: 0, ModelVarTypeDDPM.FIXED_SMALL: 1}   # rs_ddpm_var_type
+    _NATIVE_VAR_TYPES = {ModelVarTypeDDPM.FIXED_LARGE: 0, ModelVarTypeDDPM.FIXED_SMALL: 1,   # rs_ddpm_var_type
+                         ModelVarTypeDDPM.LEARNED_RANGE: 3, ModelVarTypeDDPM.LEARNED: 4}
+    _LEARNED = (ModelVarTypeDDPM.LEARNED, ModelVarTypeDDPM.LEARNED_RANGE)
 
     def _native_ok(self, model, denoised_fn, model_kwargs) -> bool:
-        return (isinstance(model, (UNetModelSwin, UNetModel, UNetModelConv))
+        """Whether the fused loop runs this call.  A learned variance needs a model whose output has twice the latent's
+        channels (mean, then variance values), a fixed one the same count; any other model goes to the torch route,
+        where the reference's own shape assertion speaks."""
+        if not (isinstance(model, (UNetModelSwin, UNetModel, UNetModelConv))
                 and self.model_mean_type in self._NATIVE_MEAN_TYPES
                 and self.model_var_type in self._NATIVE_VAR_TYPES
                 and denoised_fn is None
                 and model_kwargs is not None and "lq" in model_kwargs
-                and 2 <= self.num_timesteps <= 64)       # rs_ddpm_sampler_create: 2 <= T <= FiLM-table rows of a plan
+                and 2 <= self.num_timesteps <= 64):      # rs_ddpm_sampler_create: 2 <= T <= FiLM-table rows of a plan
+            return False
+        return model.cfg.out_channels == model.x_channels * (2 if self.model_var_type in self._LEARNED else 1)
 
     def ddpm_tables(self) -> np.ndarray:
         """[8, T] float64: the rows of rs_ddpm_sampler_create (rs_ddpm_table_row)"""
         return np.ascontiguousarray(np.stack([getattr(self, name) for name in _lib.DDPM_TABLE_ROWS]), dtype=np.float64)
+
+    def ddpm_learned_range_tables(self) -> np.ndarray:
+        """[9, T] float64: the rows of rs_ddpm_sampler_create with RS_VAR_LEARNED_RANGE (ddpm_tables, then log(betas))"""
+        return np.ascontiguousarray(np.stack([getattr(self, name) for name in _lib.DDPM_LEARNED_RANGE_TABLE_ROWS]),
+                                    dtype=np.float64)
 
     def ddim_reverse_tables(self) -> np.ndarray:
         """[9, T] float64: the rows of rs_ddim_reverse_sampler_create (ddpm_tables, then alphas_cumprod_next)"""
@@ -657,7 +671,8 @@ class SpacedDiffusionDDPM:
                                        (C.c_int32 * T)(*self.timestep_map), C.byref(ropt), out))
         opt = _lib.DdpmOptionsC(_lib.DDPM_KINDS[kind], self._NATIVE_MEAN_TYPES[self.model_mean_type],
                                 self._NATIVE_VAR_TYPES[self.model_var_type], int(bool(clip_denoised)), float(eta))
-        tabs = self.ddpm_tables()
+        tabs = (self.ddpm_learned_range_tables() if self.model_var_type == ModelVarTypeDDPM.LEARNED_RANGE
+                else self.ddpm_tables())
         return _cached_sampler(plan, ("ddpm",) + process + ((opt.kind, opt.mean_type, opt.var_type, opt.clip, opt.eta),),
                                lambda out: _lib.lib.rs_ddpm_sampler_create(
                                    plan.handle, T, tabs.ctypes.data_as(C.POINTER(C.c_double)),

@@ -119,6 +119,19 @@ class _NativeDenoiser(nn.Module):
             self._plans[key] = _Plan(self, batch, height, width, device)
         return self._plans[key]
 
+    @property
+    def x_channels(self) -> int:
+        """Channels of x, the latent the model denoises: in_channels for UNetModelSwin; out_channels for UNetModel and
+        UNetModelConv, or out_channels / 2 when their head also outputs a learned variance (learn_sigma)."""
+        return self.cfg.x_channels
+
+    def _check_x(self, x):
+        if x.shape[1] != self.x_channels:
+            if self.x_channels == self.cfg.out_channels:
+                raise ValueError(f"x must have out_channels={self.cfg.out_channels} channels, got {x.shape[1]}")
+            raise ValueError(f"x must have out_channels / 2 = {self.x_channels} channels (out_channels="
+                             f"{self.cfg.out_channels} holds the mean and the learned variance), got {x.shape[1]}")
+
     def num_launches(self, batch, height, width) -> int:
         return _lib.lib.rs_plan_num_launches(self.plan(batch, height, width).handle)
 
@@ -240,14 +253,13 @@ class UNetModel(_NativeDenoiser):
 
     @torch.no_grad()
     def forward(self, x, timesteps, y=None, lq=None):
-        """x [N, out_channels, H, W]; timesteps [N]; lq [N, 3, H, W] or [N, 3, 2H, 2W] as in_channels says
+        """x [N, x_channels, H, W]; timesteps [N]; lq [N, 3, H, W] or [N, 3, 2H, 2W] as in_channels says
         -> [N, out_channels, H, W] fp32 (reference models/unet.py:549-585)."""
         if y is not None:
             raise ValueError("y: class-conditional UNetModel is not covered (num_classes must be None)")
         if lq is None:
             raise ValueError("UNetModel is LQ-conditioned (cond_lq=True): pass lq=")
-        if x.shape[1] != self.cfg.out_channels:
-            raise ValueError(f"x must have out_channels={self.cfg.out_channels} channels, got {x.shape[1]}")
+        self._check_x(x)
         return self._run_forward(x, timesteps, lq, None)
 
 
@@ -284,12 +296,11 @@ class UNetModelConv(_NativeDenoiser):
 
     @torch.no_grad()
     def forward(self, x, timesteps, lq=None):
-        """x [N, out_channels, H, W]; timesteps [N]; lq [N, 3, H, W] or [N, 3, 2H, 2W] as in_channels says
+        """x [N, x_channels, H, W]; timesteps [N]; lq [N, 3, H, W] or [N, 3, 2H, 2W] as in_channels says
         -> [N, out_channels, H, W] fp32 (reference models/unet.py:1153-1181)."""
         if lq is None:
             raise ValueError("UNetModelConv is LQ-conditioned (cond_lq=True): pass lq=")
-        if x.shape[1] != self.cfg.out_channels:
-            raise ValueError(f"x must have out_channels={self.cfg.out_channels} channels, got {x.shape[1]}")
+        self._check_x(x)
         return self._run_forward(x, timesteps, lq, None)
 
 
